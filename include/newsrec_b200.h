@@ -1,4 +1,4 @@
-/* newsrec_b200 -- C ABI of the Blackwell-native (sm_100a) NRMS / NAML / LSTUR / TANR hot path.
+/* newsrec_b200 -- C ABI of the Hopper-native (sm_90a) NRMS / NAML / LSTUR / TANR hot path.
  *
  * Drop-in boundary for the reference's Python modules (yusanshi/news-recommendation @ 8323a4f).  The
  * reference has no FFI of its own (pure PyTorch); these are the entry points a maintainer binds with
@@ -33,20 +33,15 @@ int nr_device_error(int out4[4]);           /* watchdog record {code, block, thr
 long long nr_launch_count(void);            /* kernels this library has launched so far */
 int nr_num_sms(void);
 /* TRIAGE ONLY (tests): route the GEMMs through a plain SIMT accumulate + the same epilogue functors, to
- * tell a tcgen05/TMA pipeline bug from an epilogue bug.  Never enabled by the product path. */
+ * tell a wgmma/TMA pipeline bug from an epilogue bug.  Never enabled by the product path. */
 void nr_debug_set_simt_gemm(int on);
 /* 1 in a triage build (`make TRIAGE=1`), 0 in the release library, where nr_debug_set_simt_gemm is a no-op, the SIMT
  * kernels are not compiled and no environment switch is consulted on a launch path */
 int nr_has_triage_backends(void);
 /* TUNING ONLY (tools/kbench.py): dev_buf holds slots x 148 x 16 int64; the k-th gemm_nt planned after this call
- * writes, per CTA, cycle counters into slot k: [0] TMA producer waiting for a free A stage, [1] MMA issuer waiting
- * for A data, [2] MMA issuer waiting for a free TMEM accumulator, [3] epilogue waiting for a finished accumulator,
- * [4] epilogue body, [5] kernel, [6] tiles, [7] MMA issue loops, [8] tcgen05.commit.  Null (default) switches the counters off. */
+ * writes, per CTA, cycle counters into slot k: [0] TMA producer waiting for a free A stage, [1] consumer warpgroups
+ * waiting for A data, [4] epilogue body, [5] kernel, [6] tiles.  Null (default) switches the counters off. */
 void nr_debug_set_gemm_timing(void* dev_buf, int slots);
-/* TUNING ONLY (tools/fused_timing.py): dev_buf holds 148 x 32 int64; every fused front-end launch after this call writes,
- * per CTA, cycle counters of its warp roles (epilogue groups [0..6], [8..14]; gather [16,17]; weight producer [20];
- * tcgen05 issuer [24..29]).  Null (default) switches the counters off. */
-void nr_debug_set_fused_timing(void* dev_buf);
 /* Data parallel: the weight-gradient GEMMs (nr_gemm_tn and the composites' internal calls) leave n SMs free, so that the
  * channel CTAs of a gradient all-reduce running on a side stream have somewhere to run (0 = use every SM, the default). */
 void nr_reserve_sms_for_comm(int n);
@@ -73,7 +68,7 @@ int nr_rows_to_bf16(const float* src, long long n, int D, long long s_row, long 
 int nr_gather_rows(const long long* ids, long long n_tok, int T, const void* table_bf16, int V, int D, int ld,
                    void* X_bf16, int padded, float p_drop, unsigned long long seed, int* bad_id_flag, void* stream);
 
-/* ---- reference: nn.Linear / nn.Conv2d(1,F,(3,d)) as a tcgen05 GEMM with fused bias/ReLU/dropout --- */
+/* ---- reference: nn.Linear / nn.Conv2d(1,F,(3,d)) as a wgmma GEMM with fused bias/ReLU/dropout --- */
 /* out[M][N] = act(A . W^T + bias); taps==3: window-3 conv over the padded layout (rows_per_tile = k*(T+2)) */
 int nr_linear(const void* A_bf16, int M, int lda, const void* W_bf16, int N, int ldw, int K, int taps, int w_tap_rows,
               int rows_per_tile, const float* bias, int relu, void* out, int ld_out, int out_is_bf16, void* stream);
@@ -161,13 +156,7 @@ typedef struct {
     float* w;                 /* [n_seq*T] additive-attention weights                               */
     float* out;               /* [n_seq][d] fp32                                                    */
     int* bad_id_flag;         /* device int, set if an id is out of range                           */
-    /* fused front end (ids variant, shapes nr_mhsa_fused_supported() accepts; all three NULL = unfused kernel sequence):
-     * gather -> Q|K|V -> attention run as ONE kernel; the gathered rows are written to X_bf16 only when that pointer is
-     * non-NULL (a backward pass will read them), Q|K|V never leaves the chip (QKV_bf16 must be NULL; the backward
-     * recomputes it from X), and the context leaves as a bf16 hi plane (C_bf16) plus a bf16 lo plane (C_lo_bf16): the
-     * pooled sum uses hi + lo. */
-    const void* wqkv_heads_bf16; /* [heads*64][ldx]: per head the rows W_Q[h] | W_K[h] | W_V[h] | zero rows up to 64 */
-    const float* bqkv_heads;     /* [heads*64] biases in the same order                                */
+    /* low plane of the context (precise variants below): the pooled sum uses C_bf16 + C_lo_bf16 */
     void* C_lo_bf16;             /* [n_seq*T][ldx]                                                      */
     /* precise DENSE variant (user encoder of the precise mode; selected by dense != NULL and C_lo_bf16 != NULL): the fp32
      * input enters the projection as a hi/lo bf16 pair against K-concatenated weights, Q|K|V stays fp32, the attention runs
@@ -182,8 +171,6 @@ typedef struct {
 } nr_mhsa_encoder_fwd_args;
 int nr_mhsa_accurate_supported(int T, int d, int heads); /* 1: the accurate news variant exists for this shape */
 int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream);
-/* 1 if the fused front end handles (tokens per title, model width, heads): the reference's news level, T = 20, d_k = 20 */
-int nr_mhsa_fused_supported(int T, int d, int heads);
 
 typedef struct {
     long long n_seq;
@@ -210,7 +197,7 @@ typedef struct {
     float* ddense;                       /* [n_seq*T][d] (=) input gradient (dense variant)              */
     void* workspace;
     long long workspace_bytes;
-    /* QKV_bf16 == NULL (the fused forward keeps Q|K|V on chip): recomputed here from X_bf16 with these operands */
+    /* QKV_bf16 == NULL (the precise dense forward keeps no bf16 Q|K|V): recomputed here from X_bf16 with these operands */
     const void* wqkv_bf16;               /* [3d][ldx]                                                    */
     const float* bqkv;                   /* [3d]                                                         */
     /* optional cudaEvent_t recorded on `stream` as soon as demb is complete (before the weight-gradient GEMM): a data-
@@ -225,7 +212,7 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream);
  *   LSTUR title branch     src/model/LSTUR/news_encoder.py:56-72
  *   TANR  NewsEncoder      src/model/TANR/news_encoder.py:40-52
  * embedding -> dropout -> Conv2d(1, F, (3, d), padding (1, 0)) -> ReLU -> dropout -> additive pooling.
- * The conv is three row-shifted tcgen05 GEMM taps over a zero-padded layout (T+2 rows per segment). */
+ * The conv is three row-shifted wgmma GEMM taps over a zero-padded layout (T+2 rows per segment). */
 typedef struct {
     long long n_seq;
     int T, d, F, q, ldx, ldf;       /* ldx = round_up(d+1, 8), ldf = round_up(F+1, 8)                       */

@@ -11,7 +11,6 @@ int read_device_error(int* out4);
 void set_debug_simt_gemm(int on);
 int has_triage_backends();
 void set_debug_gemm_timing(void* dev_buf, int slots);
-void set_debug_fused_timing(void* dev_buf);
 void set_comm_reserved_sms(int n);
 extern int g_launches;
 }  // namespace nr
@@ -33,7 +32,6 @@ void nr_debug_set_simt_gemm(int on) { set_debug_simt_gemm(on); }
 int nr_has_triage_backends(void) { return has_triage_backends(); }
 void nr_reserve_sms_for_comm(int n) { set_comm_reserved_sms(n); }
 void nr_debug_set_gemm_timing(void* dev_buf, int slots) { set_debug_gemm_timing(dev_buf, slots); }
-void nr_debug_set_fused_timing(void* dev_buf) { set_debug_fused_timing(dev_buf); }
 void nr_profile_enable(int on) { prof_enable(on); }
 void nr_profile_context(const char* ctx) { prof_context(ctx ? ctx : ""); }
 int nr_profile_report(char* buf, int cap) { return prof_report(buf, cap); }
@@ -128,7 +126,6 @@ int nr_dot_score_bwd(const float* cand, const float* user, const float* dlogits,
     return dot_score_bwd(cand, user, dlogits, B, C, D, dcand, duser, S(stream));
 }
 
-int nr_mhsa_fused_supported(int T, int d, int heads) { return mhsa_fused_supported(T, d, heads); }
 
 int nr_segment_dot(const float* news, long long n_news, int D, const long long* cand, long long n_cand, const long long* seg_offsets,
                    long long n_seg, const float* user, float* scores, int* bad_id_flag, void* stream) {
@@ -178,28 +175,14 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_mhsa_encoder_fwd: null args");
     NR_PROPAGATE(check_mhsa_shape(a->n_seq, a->T, a->d, a->heads, a->q, a->ldx, a->ld3));
     NR_REQUIRE((a->ids != nullptr) != (a->dense != nullptr), "nr_mhsa_encoder_fwd: exactly one of ids / dense");
-    const bool fused = a->ids != nullptr && a->wqkv_heads_bf16 != nullptr && a->bqkv_heads != nullptr && a->C_lo_bf16 != nullptr &&
-                       mhsa_fused_supported(a->T, a->d, a->heads);
     NR_REQUIRE(a->wa_bf16 && a->ba && a->qv && a->C_bf16 && a->w && a->out, "nr_mhsa_encoder_fwd: null operand");
     const bool precise_dense = a->dense != nullptr && a->C_lo_bf16 != nullptr;
-    NR_REQUIRE(fused || precise_dense || (a->wqkv_bf16 && a->bqkv && a->X_bf16 && a->QKV_bf16), "nr_mhsa_encoder_fwd: null operand");
-    NR_REQUIRE(!fused || a->QKV_bf16 == nullptr, "nr_mhsa_encoder_fwd: the fused front end never writes Q|K|V (pass QKV_bf16 = NULL)");
+    NR_REQUIRE(precise_dense || (a->wqkv_bf16 && a->bqkv && a->X_bf16 && a->QKV_bf16), "nr_mhsa_encoder_fwd: null operand");
     NR_REQUIRE(a->p_drop >= 0.f && a->p_drop < 1.f, "nr_mhsa_encoder_fwd: dropout p=%f", a->p_drop);
     if (a->n_seq == 0) return 0;
     const int M = static_cast<int>(a->n_seq * a->T);
     const cudaStream_t st = S(stream);
     prof_context(a->ids != nullptr ? "news.fwd" : "user.fwd");
-    if (fused) {
-        // one kernel: gather -> Q|K|V -> attention (news_encoder.py:38-43); then the pooling GEMM on the hi plane with
-        // the pooled sum over hi + lo (additive.py:35-53)
-        NR_REQUIRE(a->table_bf16 && a->bad_id_flag && a->V >= 1, "nr_mhsa_encoder_fwd: table / bad_id_flag missing");
-        NR_PROPAGATE(mhsa_fused_fwd(a->ids, a->n_seq, a->T, a->table_bf16, a->V, a->d, a->heads, a->ldx, a->wqkv_heads_bf16,
-                                    a->bqkv_heads, DropoutCfg{a->p_drop, a->seed}, DropoutCfg{a->p_drop, a->seed ^ 0x5bd1e995u},
-                                    a->X_bf16, a->C_bf16, a->C_lo_bf16, a->bad_id_flag, st));
-        NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
-                                        a->w, st, a->C_lo_bf16));
-        return 0;
-    }
     if (a->dense != nullptr && a->C_lo_bf16 != nullptr) {
         // precise user encoder (user_encoder.py:15-26 at fp32 accuracy): the input enters as a hi/lo pair against the
         // K-concatenated weights [W | W], Q|K|V stays fp32, the attention runs in fp32, the context leaves as hi/lo planes
@@ -275,7 +258,7 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
                    a->w && a->dout && a->dWqkv_ext && a->dWa_ext && a->dqv && a->workspace,
                "nr_mhsa_encoder_bwd: null operand");
     NR_REQUIRE(a->QKV_bf16 != nullptr || (a->wqkv_bf16 != nullptr && a->bqkv != nullptr),
-               "nr_mhsa_encoder_bwd: Q|K|V was not saved (fused forward): pass wqkv_bf16 / bqkv so that it can be recomputed from X");
+               "nr_mhsa_encoder_bwd: Q|K|V was not saved (precise dense forward): pass wqkv_bf16 / bqkv so that it can be recomputed from X");
     NR_REQUIRE((a->ids != nullptr) ? (a->demb != nullptr) : (a->ddense != nullptr),
                "nr_mhsa_encoder_bwd: missing input-gradient buffer");
     NR_REQUIRE(a->workspace_bytes >= nr_mhsa_encoder_bwd_workspace(a->n_seq, a->T, a->d, a->q),
@@ -297,7 +280,7 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
 
     prof_context(a->ids != nullptr ? "news.bwd" : "user.bwd");
     const void* QKV = a->QKV_bf16;
-    if (QKV == nullptr) {  // the fused forward keeps Q|K|V on chip: recompute it from the saved rows (multihead_self.py:53-58)
+    if (QKV == nullptr) {  // the precise dense forward keeps no bf16 Q|K|V: recompute it from the saved rows (multihead_self.py:53-58)
         NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, 128, a->bqkv, 0, ws, a->ld3, 1,
                                 kIdentity, 0, kNoDrop, -1, 0, st));
         QKV = ws;

@@ -1,6 +1,6 @@
 // Multi-head self-attention core (reference src/model/general/attention/multihead_self.py:15-23) on the
 // legacy tensor path (mma.sync m16n8k16 bf16 + ldmatrix): the per-(sequence, head) products are 20x20x20 /
-// 50x50x20 -- 3 % of the model's FLOPs and far too small for a 128-row tcgen05 tile -- so one WARP owns one
+// 50x50x20 -- 3 % of the model's FLOPs and far too small for a 128-row wgmma tile -- so one WARP owns one
 // head, all operands live in shared-memory tiles and nothing but Q|K|V (+dCtx) is read from HBM.
 //
 //   forward : S = QK^T/sqrt(dk);  A = exp(S)/(sum exp(S) + 1e-8)  [stable form];  ctx = A V
@@ -27,7 +27,7 @@ constexpr int kPitch = 40;   // bf16 elements per tile row (80 B: 16-byte aligne
 constexpr int kPitch24 = 24; // fixed-shape d_k = 20 kernels: 48-byte rows (also conflict-free: 8 rows x 16 B hit 8 distinct bank
                              // quads); the second k-step over d_k is then an m16n8k8 MMA over columns 16..23 (20..23 stay zero).
                              // 40 % less shared memory per tile -> 4 instead of 3 resident CTAs (backward), 6 instead of 5 (forward):
-                             // the kernels are latency bound (25-36 % issue-active, ncu profiles/), residency is what they lack.
+                             // the kernels are latency bound (25-36 % issue-active under ncu), residency is what they lack.
 
 // A fragment (16 x 16) of a row-major [row][k] tile:           rows row0.., k columns k0..
 __device__ __forceinline__ void load_a(uint32_t* a, const __nv_bfloat16* tile, int pitch, int row0, int k0, int lane) {

@@ -5,7 +5,7 @@
 //
 // Why a second kernel next to attn.cu: the head-level kernel there moves every 20 x 20 head tile with 8-byte cp.async
 // pieces (a 40-byte head row has no 16-byte phase) and is bound by the LSU data pipe -- 418 shared-memory wavefronts per
-// head, a third of them the asynchronous copies themselves (ncu, profiles/ncu_r01_attention_final.csv).  Here a CTA owns
+// head, a third of them the asynchronous copies themselves.  Here a CTA owns
 // WHOLE TITLES: one TMA box brings the 20 full Q|K|V rows of a title (all heads, contiguous, sector aligned), a second one
 // the 20 dCtx rows, and one TMA store writes the 20 dQ|dK|dV rows back.  Warp h owns head h.  No copy instruction touches
 // the LSU pipe; what is left are the ldmatrix fragment loads and a 2.3 KB per-warp scratch for A / dS (126 wavefronts).
@@ -569,7 +569,7 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
         if (drop) {
             // dropout acts on the context (multihead_self.py:23 -> news_encoder.py:43): second pass over the head's 20 x 20 block in
             // 8-byte pieces, ONE counter hash per 4 aligned columns (hashing per fragment pair in the loop above costs 3x the
-            // hashes and made the kernel issue bound: 0.41 ms against 0.26 ms without dropout, ncu profiles/)
+            // hashes and made the kernel issue bound)
             __syncwarp();
             const uint64_t gbase = (static_cast<uint64_t>(row_base) * p.ld_ctx + 20u * h) >> 2;
 #pragma unroll

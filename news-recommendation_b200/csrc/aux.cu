@@ -1,4 +1,4 @@
-// Memory-bound companions of the tcgen05 GEMMs: operand preparation, the embedding-row gather,
+// Memory-bound companions of the wgmma GEMMs: operand preparation, the embedding-row gather,
 // the per-(sequence, head) self-attention core (fwd/bwd), pooling-backward row dots, the dot-product
 // click scorer.  All HBM-bound integer/byte or small-reduction work: coalesced 16-byte accesses,
 // warp-shuffle reductions, no tensor cores.

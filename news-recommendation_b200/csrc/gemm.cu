@@ -1,4 +1,4 @@
-// tcgen05 GEMM building blocks + their fused-epilogue instantiations.  See nr_gemm.cuh for the design.
+// wgmma GEMM building blocks + their fused-epilogue instantiations.  See nr_gemm.cuh for the design.
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
@@ -15,6 +15,7 @@
 
 namespace nr {
 
+int read_gru_device_error(int* out4);
 int g_launches = 0;
 
 // ------------------------------------------------------------------------------------------------
@@ -31,7 +32,7 @@ const char* last_error() { return t_err; }
 int read_device_error(int* out4) {
     const int rc = (int)cudaMemcpyFromSymbol(out4, g_dev_error, sizeof(int) * 4);
     if (rc != 0 || out4[0] != 0) return rc;
-    return read_fused_device_error(out4);  // the fused encoder kernels keep their own record (fused_fwd.cu)
+    return read_gru_device_error(out4);  // the persistent GRU kernel keeps its own record (gru_persist.cu)
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -245,30 +246,40 @@ int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B,
         fprintf(stderr, "[nr] gemm timing slot %d: M=%d N=%d K=%d taps=%d\n", g_gemm_timing_next, M, N, K, taps);
         ++g_gemm_timing_next;
     }
-    const int fixed = 1024 + round_up(scratch_bytes, 16) + 512;
+    const int fixed = 1024 + kXposeBytes + round_up(scratch_bytes, 16) + 512;
     int slices = 1;
+    long bbytes = 0;
     for (;; ++slices) {
         NR_REQUIRE(slices <= 64, "plan_gemm_nt: cannot fit weight slice (N=%d K=%d taps=%d)", N, K, taps);
         p.n_stride = round_up(ceil_div(N, slices), 16);  // 32-byte aligned slice starts (STG.256 epilogues)
-        p.n_box = round_up(std::min(p.n_stride, N), 16);
+        // whole 32-column chunks of resident weight rows: a warpgroup's wgmma covers its chunks entirely (rows past the
+        // slice are the next slice's weights or TMA zero fill, never uninitialised shared memory)
+        p.n_box = round_up(std::min(p.n_stride, N), 32);
         if (p.n_box > 256 || (max_n_stride > 0 && p.n_stride > max_n_stride)) continue;
-        const long bbytes = static_cast<long>(taps) * p.k_chunks * (p.n_box / 2) * 128;  // per CTA: half the slice
-        if (bbytes + 4L * kAStageBytes + fixed <= kSmemLimit) break;
-        // epilogues that reduce over the whole output row need ONE slice: accept a shallower A ring instead
-        if (slices == max_slices && bbytes + 2L * kAStageBytes + fixed <= kSmemLimit) break;
+        bbytes = static_cast<long>(taps) * p.k_chunks * p.n_box * 128;
+        if (bbytes + 3L * kAStageBytes + fixed <= kSmemLimit) break;
+        // epilogues that reduce over the whole output row need ONE slice, and slices of <= 64 columns re-read A too often:
+        // accept a shallower A ring, or else stream the weight boxes with the A tiles instead of keeping them resident
+        if (slices == max_slices || p.n_box <= 64) {
+            if (bbytes + 2L * kAStageBytes + fixed > kSmemLimit) {
+                p.b_stream = 1;
+                bbytes = 0;
+            }
+            break;
+        }
     }
     p.n_slices = ceil_div(N, p.n_stride);
-    const long bbytes = static_cast<long>(taps) * p.k_chunks * (p.n_box / 2) * 128;
-    p.stages = static_cast<int>(std::min<long>(kMaxStages, (kSmemLimit - fixed - bbytes) / kAStageBytes));
+    p.stage_bytes = kAStageBytes + (p.b_stream ? p.n_box * 128 : 0);
+    p.stages = static_cast<int>(std::min<long>(kMaxStages, (kSmemLimit - fixed - bbytes) / p.stage_bytes));
     NR_REQUIRE(p.stages >= 2, "plan_gemm_nt: only %d pipeline stages fit", p.stages);
-    plan->smem = static_cast<size_t>(bbytes) + static_cast<size_t>(p.stages) * kAStageBytes + fixed;
-    // CTA pairs: a group = n_slices pairs working on the same 256-row blocks
-    const int groups = std::max(1, std::min((sms / 2) / p.n_slices, ceil_div(p.num_m_tiles, 2)));
-    plan->grid = 2 * groups * p.n_slices;
+    plan->smem = static_cast<size_t>(bbytes) + static_cast<size_t>(p.stages) * p.stage_bytes + fixed;
+    // a group = n_slices CTAs working on the same 128-row tiles
+    const int groups = std::max(1, std::min(sms / p.n_slices, p.num_m_tiles));
+    plan->grid = groups * p.n_slices;
     if (p.num_m_tiles == 0) return 0;
     NR_PROPAGATE(make_tmap_bf16_2d(&plan->tmA, A, M, K, lda, kChunkK, kTileM));
     const int64_t brows = (taps > 1) ? static_cast<int64_t>(taps) * b_tap_rows : N;
-    NR_PROPAGATE(make_tmap_bf16_2d(&plan->tmB, B, brows, K, ldb, kChunkK, p.n_box / 2));
+    NR_PROPAGATE(make_tmap_bf16_2d(&plan->tmB, B, brows, K, ldb, kChunkK, p.n_box));
     return 0;
 }
 
@@ -298,130 +309,115 @@ __global__ void gemm_nt_simt_acc_kernel(const __nv_bfloat16* A, int lda, const _
 #endif  // NEWSREC_TRIAGE
 
 // ------------------------------------------------------------------------------------------------
-// gemm_tn kernel
+// gemm_tn kernel: CTA = (128 output rows, <= 256 output columns, a range of 64-row k-chunks).  Warpgroup h owns output rows
+// [64h, 64h + 64) and accumulates all NT columns in registers (MN-major operands straight from the TMA boxes); the result
+// is added to D with vector reductions.
 // ------------------------------------------------------------------------------------------------
+template <int NT>
 __global__ void __launch_bounds__(kTnThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmTNParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    constexpr int kBoxes = NT / 64;
+    constexpr int stage_bytes = (2 + kBoxes) * 8192;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int stage_bytes = (2 + p.n_boxes) * 8192;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
     uint64_t* full = bars;
     uint64_t* empty = bars + kMaxStages;
-    uint64_t* tfull = bars + 2 * kMaxStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 1);
 
     const int mt = blockIdx.x % p.m_tiles;
-    const int ks = blockIdx.x / p.m_tiles;
+    const int rest = blockIdx.x / p.m_tiles;
+    const int nt = rest % p.n_tiles;
+    const int ks = rest / p.n_tiles;
     const int total_chunks = (p.Kr + 63) >> 6;
     const int chunk0 = ks * p.chunks_per_slice;
     const int n_my = max(0, min(p.chunks_per_slice, total_chunks - chunk0));
-    const int nb_pad = (p.Nb + 15) & ~15;
-    // more than 256 columns take two MMAs per k-step: split them near the middle, on a 64-column box boundary -- a single-CTA
-    // tcgen05.mma costs >= 86 cycles whatever its N (tools/mmabench_small.cu), so 256 + 48 is 128 + 86 cycles where 192 + 112
-    // is 96 + 86
-    const int n0 = nb_pad <= 256 ? nb_pad : (((nb_pad >> 1) + 63) & ~63);
-    const int n1 = nb_pad - n0;
-    const uint32_t tmem_cols = nb_pad > 256 ? 512u : (nb_pad > 128 ? 256u : (nb_pad > 64 ? 128u : (nb_pad > 32 ? 64u : 32u)));
+    const int n0 = nt * NT;                       // first output column of this CTA
+    const int ncol = min(NT, p.Nb - n0);
 
-    if (warp == 4 && lane == 0) {
+    if (warp == kEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
+            mbar_init(&empty[i], 8);
         }
-        mbar_init(tfull, 1);
         fence_barrier_init();
-    } else if (warp == 5) {
-        tmem_alloc(tmem_slot, tmem_cols);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (n_my == 0) return;
 
-    if (n_my > 0) {
-        // producer and issuer loops are warp-uniform, one elected lane issues (see gemm_nt)
-        if (warp == 4) {
-            int st = 0;
-            uint32_t ph = 0;
-            for (int c = 0; c < n_my; ++c) {
-                const int k0 = (chunk0 + c) * 64;
-                mbar_wait(&empty[st], ph ^ 1, 201);
-                if (elect_one()) {
-                    mbar_arrive_expect_tx(&full[st], static_cast<uint32_t>(stage_bytes));
-                    uint8_t* sa = smem + st * stage_bytes;
-                    uint8_t* sb = sa + 2 * 8192;
-                    tma_load_2d(sa, &tmA, &full[st], mt * 128, k0);
-                    tma_load_2d(sa + 8192, &tmA, &full[st], mt * 128 + 64, k0);
-                    for (int j = 0; j < p.n_boxes; ++j)
-                        tma_load_2d(sb + j * 8192, &tmB, &full[st], p.b_col0 + j * 64, k0 + p.b_row_shift);
-                }
-                __syncwarp();
-                if (++st == p.stages) { st = 0; ph ^= 1; }
-            }
-        } else if (warp == 5) {
-            const uint32_t idesc0 = make_idesc_bf16(kTileM, n0, 1, 1);
-            const uint32_t idesc1 = make_idesc_bf16(kTileM, n1 > 0 ? n1 : 16, 1, 1);
-            int st = 0;
-            uint32_t ph = 0;
-            uint32_t acc = 0;
-            for (int c = 0; c < n_my; ++c) {
-                mbar_wait(&full[st], ph, 202);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t sa = smem_u32(smem + st * stage_bytes);
-                    const uint32_t sb = sa + 2 * 8192;
-                    const uint64_t da = make_sw128_desc(sa, 8192, 1024);
-                    const uint64_t db0 = make_sw128_desc(sb, 8192, 1024);
-                    const uint64_t db1 = make_sw128_desc(sb + (n0 >> 6) * 8192, 8192, 1024);
+    if (warp >= kEpiWarps) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        if (warp != kEpiWarps) return;
+        // producer loop is warp-uniform, one elected lane issues
+        int st = 0;
+        uint32_t ph = 0;
+        for (int c = 0; c < n_my; ++c) {
+            const int k0 = (chunk0 + c) * 64;
+            mbar_wait(&empty[st], ph ^ 1, 201);
+            if (elect_one()) {
+                mbar_arrive_expect_tx(&full[st], static_cast<uint32_t>(stage_bytes));
+                uint8_t* sa = smem + st * stage_bytes;
+                uint8_t* sb = sa + 2 * 8192;
+                tma_load_2d(sa, &tmA, &full[st], mt * 128, k0);
+                tma_load_2d(sa + 8192, &tmA, &full[st], mt * 128 + 64, k0);
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {  // +2048 bytes per k-step = +128 in the descriptor's >>4 address field
-                        umma_bf16(tmem_base, da + 128 * k, db0 + 128 * k, idesc0, (k == 0) ? acc : 1u);
-                        if (n1 > 0) umma_bf16(tmem_base + n0, da + 128 * k, db1 + 128 * k, idesc1, (k == 0) ? acc : 1u);
-                    }
-                    umma_commit(&empty[st]);
-                }
-                __syncwarp();
-                acc = 1;
-                if (++st == p.stages) { st = 0; ph ^= 1; }
+                for (int j = 0; j < kBoxes; ++j)
+                    tma_load_2d(sb + j * 8192, &tmB, &full[st], p.b_col0 + n0 + j * 64, k0 + p.b_row_shift);
             }
-            if (elect_one()) umma_commit(tfull);
             __syncwarp();
-        } else {
-            mbar_wait(tfull, 0, 203);
-            tc_fence_after();
-            const int grow = mt * 128 + warp * 32 + lane;
-            const bool valid = grow < p.Ma;
-            float* drow = p.D + static_cast<size_t>(valid ? grow : 0) * p.ldd;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-            const int nch = (p.Nb + 31) >> 5;
-            const bool vec4 = (p.ldd & 3) == 0 && (reinterpret_cast<uintptr_t>(p.D) & 15) == 0;
-            for (int ch = 0; ch < nch; ++ch) {
-                float x[32];
-                tmem_ld32(taddr + ch * 32, x);
-                tmem_ld_wait();
-                if (!valid) continue;
+            if (++st == p.stages) { st = 0; ph ^= 1; }
+        }
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+        const int h = warp >> 2;
+        float acc[NT / 2];
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {  // 16-byte vector reductions: 4x fewer L2 atomic operations
-                    const int col = ch * 32 + j;
-                    if (vec4 && col + 4 <= p.Nb) {
-                        red_add_v4_f32(drow + col, x[j], x[j + 1], x[j + 2], x[j + 3]);
-                    } else {
+        for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+        int st = 0;
+        uint32_t ph = 0;
+        for (int c = 0; c < n_my; ++c) {
+            mbar_wait(&full[st], ph, 202);
+            const uint32_t sa = smem_u32(smem + st * stage_bytes) + h * 8192;
+            const uint32_t sb = smem_u32(smem + st * stage_bytes) + 2 * 8192;
+            const uint64_t da = make_sw128_desc(sa, 8192, 1024);
+            const uint64_t db = make_sw128_desc(sb, 8192, 1024);
 #pragma unroll
-                        for (int i = 0; i < 4; ++i)
-                            if (col + i < p.Nb) red_add_f32(drow + col + i, x[j + i]);
-                    }
+            for (int i = 0; i < NT / 2; ++i) wgmma_reg_fence(acc[i]);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)  // +2048 bytes per k-step = +128 in the descriptor's >>4 address field
+                Wgmma<NT, 1, 1>::mma(acc, da + 128 * k, db + 128 * k, (c | k) ? 1 : 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < NT / 2; ++i) wgmma_reg_fence(acc[i]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[st]);
+            if (++st == p.stages) { st = 0; ph ^= 1; }
+        }
+        // fragment: acc[4j + 2e + i] = row 16 * (warp % 4) + lane / 4 + 8e, column 8j + 2 * (lane % 4) + i
+        const bool vec2 = (p.ldd & 1) == 0 && (reinterpret_cast<uintptr_t>(p.D) & 7) == 0;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int grow = mt * 128 + 64 * h + 16 * (warp & 3) + (lane >> 2) + 8 * e;
+            if (grow >= p.Ma) continue;
+            float* drow = p.D + static_cast<size_t>(grow) * p.ldd + n0;
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j) {
+                const int col = 8 * j + 2 * (lane & 3);
+                const float v0 = acc[4 * j + 2 * e], v1 = acc[4 * j + 2 * e + 1];
+                if (vec2 && col + 2 <= ncol) {
+                    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(drow + col), "f"(v0), "f"(v1) : "memory");
+                } else {
+                    if (col < ncol) red_add_f32(drow + col, v0);
+                    if (col + 1 < ncol) red_add_f32(drow + col + 1, v1);
                 }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 5) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 #ifdef NEWSREC_TRIAGE
@@ -446,6 +442,19 @@ __global__ void gemm_tn_simt_kernel(const __nv_bfloat16* A, int lda, const __nv_
 // 200 KB gemm_tn CTA the "overlapped" reduction simply waited for the GEMM to finish (2 GPUs: +0.27 ms per step, unchanged).
 static int g_comm_reserved_sms = 0;
 void set_comm_reserved_sms(int n) { g_comm_reserved_sms = n < 0 ? 0 : n; }
+
+template <int NT>
+static int launch_gemm_tn_kernel(dim3 grid, size_t smem, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmTNParams& p,
+                                 cudaStream_t stream) {
+    static bool attr_set = false;  // per instantiation
+    if (!attr_set) {
+        NR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tn_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+        attr_set = true;
+    }
+    gemm_tn_kernel<NT><<<grid, kTnThreads, smem, stream>>>(tmA, tmB, p);
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
 
 int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, int b_rows, int b_cols, int ldb,
                        int b_col0, int Nb, int b_row_shift, float* D, int ldd, cudaStream_t stream) {
@@ -474,12 +483,15 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     NR_REQUIRE(num_sms() > 0, "no CUDA device");
     const int sms = std::max(num_sms() / 2, num_sms() - g_comm_reserved_sms);
     p.m_tiles = ceil_div(Ma, 128);
+    // output columns per CTA: <= 256 (the accumulators of one warpgroup), in whole 64-column boxes
+    p.n_tiles = ceil_div(Nb, 256);
+    const int nt_cols = round_up(ceil_div(Nb, p.n_tiles), 64);
     const int total_chunks = ceil_div(Kr, 64);
-    int k_slices = std::max(1, std::min(sms / p.m_tiles, total_chunks));
+    int k_slices = std::max(1, std::min(sms / (p.m_tiles * p.n_tiles), total_chunks));
     p.chunks_per_slice = ceil_div(total_chunks, k_slices);
     k_slices = ceil_div(total_chunks, p.chunks_per_slice);
     p.k_slices = k_slices;
-    p.n_boxes = ceil_div(Nb, 64);
+    p.n_boxes = nt_cols / 64;
     const int stage_bytes = (2 + p.n_boxes) * 8192;
     p.stages = std::min(kMaxStages, (kSmemLimit - 1024 - 512) / stage_bytes);
     NR_REQUIRE(p.stages >= 2, "gemm_tn: stage of %d bytes does not double-buffer", stage_bytes);
@@ -487,15 +499,15 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     CUtensorMap tmA, tmB;
     NR_PROPAGATE(make_tmap_bf16_2d(&tmA, A, Kr, Ma, lda, 64, 64));
     NR_PROPAGATE(make_tmap_bf16_2d(&tmB, B, b_rows, b_cols, ldb, 64, 64));
-    static bool attr_set = false;
-    if (!attr_set) {
-        NR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-        attr_set = true;
-    }
     const size_t smem = static_cast<size_t>(p.stages) * stage_bytes + 1024 + 512;
-    gemm_tn_kernel<<<p.m_tiles * k_slices, kTnThreads, smem, stream>>>(tmA, tmB, p);
+    const dim3 grid(p.m_tiles * p.n_tiles * k_slices);
+    switch (p.n_boxes) {
+        case 1: NR_PROPAGATE(launch_gemm_tn_kernel<64>(grid, smem, tmA, tmB, p, stream)); break;
+        case 2: NR_PROPAGATE(launch_gemm_tn_kernel<128>(grid, smem, tmA, tmB, p, stream)); break;
+        case 3: NR_PROPAGATE(launch_gemm_tn_kernel<192>(grid, smem, tmA, tmB, p, stream)); break;
+        default: NR_PROPAGATE(launch_gemm_tn_kernel<256>(grid, smem, tmA, tmB, p, stream)); break;
+    }
     ++g_launches;
-    NR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 

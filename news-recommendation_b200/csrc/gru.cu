@@ -1,8 +1,8 @@
 // LSTUR user encoder: nn.GRU over the (left-padded) history, packed-sequence semantics, last hidden state.
 // reference: src/model/LSTUR/user_encoder.py:16-45  (pack_padded_sequence(first len[b] steps) -> nn.GRU).
 //
-// The input projection is ONE tcgen05 GEMM over all (user, step) rows; the recurrent projection is a chain of
-// S sequentially dependent [B x Hd] x [Hd x 3Hd] tcgen05 GEMMs (weight slices stay resident per launch, rows of
+// The input projection is ONE wgmma GEMM over all (user, step) rows; the recurrent projection is a chain of
+// S sequentially dependent [B x Hd] x [Hd x 3Hd] wgmma GEMMs (weight slices stay resident per launch, rows of
 // one step are one or a few M tiles), each followed by a fused gate kernel.  Gate order r, z, n (torch):
 //   r = sig(gi_r + gh_r), z = sig(gi_z + gh_z), n = tanh(gi_n + r * gh_n), h' = (1 - z) n + z h ;
 // user b stops updating after len[b] steps.

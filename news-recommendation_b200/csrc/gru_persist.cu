@@ -1,15 +1,15 @@
 // Persistent recurrence of the LSTUR user encoder's GRU (reference src/model/LSTUR/user_encoder.py:27-45), forward:
 // ONE cooperative launch runs all S time steps instead of 3 launches per step.
 //
-//   gh_t = h_{t-1} . W_hh^T + b_hh            [B x Hd] x [Hd x 3Hd]   (tcgen05, bf16 operands, fp32 accumulate)
+//   gh_t = h_{t-1} . W_hh^T + b_hh            [B x Hd] x [Hd x 3Hd]   (wgmma, bf16 operands, fp32 accumulate)
 //   r = sig(gi_r + gh_r), z = sig(gi_z + gh_z), n = tanh(gi_n + r * gh_n), h_t = (1 - z) n + z h_{t-1}   for t < len[b]
 //
 // Decomposition: users in 128-row tiles (m) x hidden units in slices of 32 (s); CTA (m, s) keeps its 96 weight rows
-// (32 units x gates r, z, n; 180 KB, SWIZZLE_128B K-major) resident in shared memory for the whole launch and the fp32
-// hidden state of its 128 x 32 block in REGISTERS.  Per step it streams the bf16 h_{t-1} rows of its tile (all Hd columns,
-// written by the 29 slice CTAs of the same row tile) through a 2-stage TMA ring, issues ceil(Hd/16) MMAs of N = 96 into
-// TMEM, and runs the gates in the epilogue (gi of the step is prefetched into registers while the previous step's barrier
-// is pending).  Steps are separated by a release/acquire counter barrier per ROW TILE (only the slices of one tile exchange
+// (32 units x gates r, z, n; 12 KB per 64 columns of Hd, SWIZZLE_128B K-major) resident in shared memory for the whole launch
+// and the fp32 hidden state of its 128 x 32 block in REGISTERS.  Per step it streams the bf16 h_{t-1} rows of its tile (all
+// Hd columns, written by the slice CTAs of the same row tile) through a 2-stage TMA ring; the four gate warps (one
+// warpgroup) issue two m64n96 wgmmas per k-step and run the gates straight on the accumulator fragments (the r, z and n
+// columns of a unit sit in the same thread).  Up to Hd = 1024 (16 k-chunks of resident weights).  Steps are separated by a release/acquire counter barrier per ROW TILE (only the slices of one tile exchange
 // data).  The launch is cooperative (all CTAs resident) -- row_tiles * slices <= SM count is checked by the host.
 // Saved for the (per-step) backward: gh (fp32), hs (fp32), hb (bf16 operand rows with the ones column), as before.
 #include <algorithm>
@@ -34,7 +34,7 @@ namespace gru {
 
 using namespace fused;
 
-constexpr int kThreads = 6 * 32;   // 4 epilogue warps + TMA producer + tcgen05 issuer
+constexpr int kThreads = 5 * 32;   // 4 gate warps (one warpgroup: wgmma + gates) + TMA producer
 constexpr int kU = 32;             // hidden units per slice
 constexpr int kN = 3 * kU;         // MMA N: gates r | z | n of the slice
 constexpr int kWChunk = kN * 128;  // one 64-column k-chunk of the resident weight slice
@@ -43,7 +43,7 @@ constexpr int kAStages = 2;
 
 struct Params {
     int B, S, Hd, ldh, ldg;
-    int slices, k_chunks, ksteps_last;
+    int slices, k_chunks;
     const float* gi;         // [B*S][ldg]  rows b*S + t
     const float* bhh;        // [3Hd]
     const float* h0;         // [B][Hd]
@@ -74,9 +74,6 @@ __global__ void __launch_bounds__(kThreads, 1) gru_fwd_persistent_kernel(const _
     uint64_t* wfull = bars;            // resident weights landed
     uint64_t* afull = bars + 1;        // [kAStages]
     uint64_t* aempty = bars + 1 + kAStages;
-    uint64_t* tfull = bars + 1 + 2 * kAStages;
-    uint64_t* tempty = tfull + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
     float* sBias = reinterpret_cast<float*>(bars + 16);      // [3][kU] b_hh of this slice (zero for units that do not exist); 16-byte aligned
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m = blockIdx.x / p.slices, s = blockIdx.x - m * p.slices;
@@ -88,22 +85,15 @@ __global__ void __launch_bounds__(kThreads, 1) gru_fwd_persistent_kernel(const _
         mbar_init(wfull, 1);
         for (int i = 0; i < kAStages; ++i) {
             mbar_init(&afull[i], 1);
-            mbar_init(&aempty[i], 1);
+            mbar_init(&aempty[i], 4);  // one arrival per gate warp
         }
-        mbar_init(tfull, 1);
-        mbar_init(tempty, 4);
         fence_barrier_init();
-    } else if (warp == 5) {
-        tmem_alloc(tmem_slot, 128);
     }
     if (threadIdx.x < kN) {
         const int g = threadIdx.x / kU, u = threadIdx.x - g * kU;
         sBias[threadIdx.x] = (j0 + u < p.Hd) ? p.bhh[g * p.Hd + j0 + u] : 0.f;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 4) {
         // ===================== TMA producer: the weight slice once, then h_{t-1} tiles step by step =====================
@@ -140,158 +130,142 @@ __global__ void __launch_bounds__(kThreads, 1) gru_fwd_persistent_kernel(const _
                 if (++st == kAStages) { st = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == 5) {
-        // ===================== tcgen05 issuer =====================
-        const uint32_t idesc = make_idesc_bf16(128, kN, 0, 0);
+    } else {
+        // ===================== gate warps: wgmma, then the gates in the accumulator fragment layout =====================
+        // Fragment of m64n96 block bb: acc[bb][4j + 2e + i] = row 64bb + 16 * warp + lane / 4 + 8e, column 8j + 2 * (lane % 4) + i.
+        // Gate g of unit u is column 32g + u, so the r, z and n pre-activations of (row, u) sit in the same thread:
+        // j = jj (r), jj + 4 (z), jj + 8 (n) with u = 8jj + 2 * (lane % 4) + i.  Each thread owns 4 rows x 8 units.
         const uint32_t a_s = smem_u32(sA), w_s = smem_u32(sW);
-        f_wait(wfull, 0, 403);
-        tc_fence_after();
+        const int nvalid = min(kU, p.Hd - j0);  // units of this slice that exist (multiple of 4)
+        const int uq = 2 * (lane & 3);
+        int brow[2][2];
+        bool valid[2][2];
+        long long L[2][2];
+        float h[2][2][4][2];
+#pragma unroll
+        for (int bb = 0; bb < 2; ++bb)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                brow[bb][e] = m * 128 + 64 * bb + 16 * warp + (lane >> 2) + 8 * e;
+                valid[bb][e] = brow[bb][e] < p.B;
+                L[bb][e] = valid[bb][e] ? p.len[brow[bb][e]] : 1;
+                if (L[bb][e] < 1) L[bb][e] = 1;  // reference clamps 0 -> 1 (user_encoder.py:27)
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int u = 8 * jj + uq;
+                    float2 v = make_float2(0.f, 0.f);
+                    if (valid[bb][e] && u < nvalid) v = *reinterpret_cast<const float2*>(p.h0 + static_cast<size_t>(brow[bb][e]) * p.Hd + j0 + u);
+                    h[bb][e][jj][0] = v.x;
+                    h[bb][e][jj][1] = v.y;
+                }
+            }
         int st = 0;
         uint32_t ph = 0;
         for (int t = 0; t < p.S; ++t) {
-            f_wait(tempty, static_cast<uint32_t>(t & 1) ^ 1u, 404);  // the epilogue has read the accumulator of step t - 1
-            tc_fence_after();
+            float acc[2][kN / 2];
             for (int c = 0; c < p.k_chunks; ++c) {
                 f_wait(&afull[st], ph, 405);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint64_t da = make_sw128_desc(a_s + st * kAStage, 0, 1024);
-                    const uint64_t db = make_sw128_desc(w_s + c * kWChunk, 0, 1024);
-                    const int nk = (c == p.k_chunks - 1) ? p.ksteps_last : 4;
+                const uint64_t db = make_sw128_desc(w_s + c * kWChunk, 16, 1024);
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        if (k < nk) umma_bf16(tmem_base, da + 2 * k, db + 2 * k, idesc, (c | k) ? 1u : 0u);
-                    umma_commit(&aempty[st]);
-                }
+                for (int bb = 0; bb < 2; ++bb)
+#pragma unroll
+                    for (int i = 0; i < kN / 2; ++i) wgmma_reg_fence(acc[bb][i]);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k)  // columns past Hd are zero filled by TMA in both operands
+#pragma unroll
+                    for (int bb = 0; bb < 2; ++bb)
+                        Wgmma<kN, 0, 0>::mma(acc[bb], make_sw128_desc(a_s + st * kAStage + bb * 8192, 16, 1024) + 2 * k, db + 2 * k,
+                                             (c | k) ? 1 : 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+#pragma unroll
+                for (int bb = 0; bb < 2; ++bb)
+#pragma unroll
+                    for (int i = 0; i < kN / 2; ++i) wgmma_reg_fence(acc[bb][i]);
                 __syncwarp();
+                if (lane == 0) mbar_arrive(&aempty[st]);
                 if (++st == kAStages) { st = 0; ph ^= 1u; }
             }
-            if (elect_one()) umma_commit(tfull);
-            __syncwarp();
-        }
-    } else {
-        // ===================== epilogue: gates, hidden state in registers =====================
-        const int r = warp * 32 + lane;
-        const int b = m * 128 + r;
-        const bool valid = b < p.B;
-        const int nvalid = min(kU, p.Hd - j0);  // units of this slice that exist (multiple of 4)
-        const uint32_t acc_t = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-        long long L = valid ? p.len[b] : 1;
-        if (L < 1) L = 1;  // reference clamps 0 -> 1 (user_encoder.py:27)
-        float h[kU];
 #pragma unroll
-        for (int u = 0; u < kU; u += 4) {
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (valid && u < nvalid) v = *reinterpret_cast<const float4*>(p.h0 + static_cast<size_t>(b) * p.Hd + j0 + u);
-            h[u] = v.x; h[u + 1] = v.y; h[u + 2] = v.z; h[u + 3] = v.w;
-        }
-        auto add_bias = [&](float* x, int g) {
+            for (int bb = 0; bb < 2; ++bb)
 #pragma unroll
-            for (int u = 0; u < kU; u += 4) {
-                const float4 b4 = lds_f4(sBias + g * kU + u);
-                x[u] += b4.x; x[u + 1] += b4.y; x[u + 2] += b4.z; x[u + 3] += b4.w;
-            }
-        };
-        float gi[3][kU];
-        auto load_gi = [&](int t) {  // input projections of step t for this row's units (prefetched under the barrier / the MMAs)
-            const float* row = p.gi + (static_cast<size_t>(valid ? b : 0) * p.S + t) * p.ldg + j0;
+                for (int e = 0; e < 2; ++e) {
+                    const int b = valid[bb][e] ? brow[bb][e] : 0;
+                    const float* girow = p.gi + (static_cast<size_t>(b) * p.S + t) * p.ldg + j0;
+                    float* ghrow = p.gh + (static_cast<size_t>(t) * p.B + b) * p.ldg + j0;
+                    float* hsrow = p.hs + (static_cast<size_t>(t + 1) * p.B + b) * p.Hd + j0;
+                    __nv_bfloat16* hbrow = p.hb + (static_cast<size_t>(t + 1) * p.B + b) * p.ldh + j0;
 #pragma unroll
-            for (int g = 0; g < 3; ++g)
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int u = 8 * jj + uq;
+                        if (u >= nvalid) continue;
+                        float x[3][2], gv[3][2];
 #pragma unroll
-                for (int u = 0; u < kU; u += 4) {
-                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (u < nvalid) v = __ldg(reinterpret_cast<const float4*>(row + g * p.Hd + u));
-                    gi[g][u] = v.x; gi[g][u + 1] = v.y; gi[g][u + 2] = v.z; gi[g][u + 3] = v.w;
-                }
-        };
-        load_gi(0);
-        for (int t = 0; t < p.S; ++t) {
-            f_wait(tfull, static_cast<uint32_t>(t & 1), 406);
-            tc_fence_after();
-            float rg[kU], zg[kU], x[kU];
-            float* ghrow = p.gh + (static_cast<size_t>(t) * p.B + (valid ? b : 0)) * p.ldg + j0;
-            // gate r
-            tmem_ld32(acc_t, x);
-            tmem_ld_wait();
+                        for (int g = 0; g < 3; ++g) {
+                            const float2 bv = *reinterpret_cast<const float2*>(sBias + g * kU + u);
+                            x[g][0] = acc[bb][4 * (jj + 4 * g) + 2 * e] + bv.x;
+                            x[g][1] = acc[bb][4 * (jj + 4 * g) + 2 * e + 1] + bv.y;
+                            const float2 gg = __ldg(reinterpret_cast<const float2*>(girow + g * p.Hd + u));
+                            gv[g][0] = gg.x;
+                            gv[g][1] = gg.y;
+                        }
+                        if (valid[bb][e]) {
 #pragma unroll
-            add_bias(x, 0);
+                            for (int g = 0; g < 3; ++g) *reinterpret_cast<float2*>(ghrow + g * p.Hd + u) = make_float2(x[g][0], x[g][1]);
+                        }
+                        if (t < L[bb][e]) {
 #pragma unroll
-            for (int u = 0; u < kU; ++u) rg[u] = fast_sigmoid(gi[0][u] + x[u]);
-            if (valid) {
-#pragma unroll
-                for (int u = 0; u < kU; u += 4)
-                    if (u < nvalid) *reinterpret_cast<float4*>(ghrow + u) = make_float4(x[u], x[u + 1], x[u + 2], x[u + 3]);
-            }
-            // gate z
-            tmem_ld32(acc_t + kU, x);
-            tmem_ld_wait();
-#pragma unroll
-            add_bias(x, 1);
-#pragma unroll
-            for (int u = 0; u < kU; ++u) zg[u] = fast_sigmoid(gi[1][u] + x[u]);
-            if (valid) {
-#pragma unroll
-                for (int u = 0; u < kU; u += 4)
-                    if (u < nvalid) *reinterpret_cast<float4*>(ghrow + p.Hd + u) = make_float4(x[u], x[u + 1], x[u + 2], x[u + 3]);
-            }
-            // gate n and the state update
-            tmem_ld32(acc_t + 2 * kU, x);
-            tmem_ld_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty);  // the issuer may overwrite the accumulator (after the next step's barrier)
-            add_bias(x, 2);
-            if (valid) {
-#pragma unroll
-                for (int u = 0; u < kU; u += 4)
-                    if (u < nvalid) *reinterpret_cast<float4*>(ghrow + 2 * p.Hd + u) = make_float4(x[u], x[u + 1], x[u + 2], x[u + 3]);
-            }
-            if (t < L) {
-#pragma unroll
-                for (int u = 0; u < kU; ++u) {
-                    const float n = fast_tanh(gi[2][u] + rg[u] * x[u]);
-                    h[u] = (1.f - zg[u]) * n + zg[u] * h[u];
-                }
-            }
-            if (valid) {
-                float* hsrow = p.hs + (static_cast<size_t>(t + 1) * p.B + b) * p.Hd + j0;
-                __nv_bfloat16* hbrow = p.hb + (static_cast<size_t>(t + 1) * p.B + b) * p.ldh + j0;
-#pragma unroll
-                for (int u = 0; u < kU; u += 4) {
-                    if (u < nvalid) {
-                        *reinterpret_cast<float4*>(hsrow + u) = make_float4(h[u], h[u + 1], h[u + 2], h[u + 3]);
-                        *reinterpret_cast<uint2*>(hbrow + u) = make_uint2(pack_bf16x2(h[u], h[u + 1]), pack_bf16x2(h[u + 2], h[u + 3]));
+                            for (int i = 0; i < 2; ++i) {
+                                const float rg = fast_sigmoid(gv[0][i] + x[0][i]);
+                                const float zg = fast_sigmoid(gv[1][i] + x[1][i]);
+                                const float n = fast_tanh(gv[2][i] + rg * x[2][i]);
+                                h[bb][e][jj][i] = (1.f - zg) * n + zg * h[bb][e][jj][i];
+                            }
+                        }
+                        if (valid[bb][e]) {
+                            *reinterpret_cast<float2*>(hsrow + u) = make_float2(h[bb][e][jj][0], h[bb][e][jj][1]);
+                            *reinterpret_cast<uint32_t*>(hbrow + u) = pack_bf16x2(h[bb][e][jj][0], h[bb][e][jj][1]);
+                        }
+                    }
+                    // the slice that ends at Hd also owns the ones column and the zero pad of the bf16 rows
+                    if (valid[bb][e] && (lane & 3) == 0 && (nvalid < kU || j0 + kU == p.Hd)) {
+                        for (int c = p.Hd; c < p.ldh; ++c)
+                            p.hb[(static_cast<size_t>(t + 1) * p.B + b) * p.ldh + c] = __float2bfloat16_rn(c == p.Hd ? 1.0f : 0.f);
                     }
                 }
-                if (nvalid < kU || j0 + kU == p.Hd) {  // the slice that ends at Hd also owns the ones column and the zero pad
-                    for (int c = p.Hd; c < p.ldh; ++c) p.hb[(static_cast<size_t>(t + 1) * p.B + b) * p.ldh + c] = __float2bfloat16_rn(c == p.Hd ? 1.0f : 0.f);
-                }
-            }
             if (t + 1 < p.S) {
-                load_gi(t + 1);
                 __threadfence();                                   // this thread's h_{t+1} rows are visible GPU-wide ...
-                asm volatile("bar.sync 1, 128;" ::: "memory");     // ... for all four epilogue warps ...
+                asm volatile("bar.sync 1, 128;" ::: "memory");     // ... for all four gate warps ...
                 if (threadIdx.x == 0) red_release(p.bar + m);      // ... before the slice counts as arrived
             }
         }
-        if (valid) {
-            float* o = p.out + static_cast<size_t>(b) * p.Hd + j0;
 #pragma unroll
-            for (int u = 0; u < kU; u += 4)
-                if (u < nvalid) *reinterpret_cast<float4*>(o + u) = make_float4(h[u], h[u + 1], h[u + 2], h[u + 3]);
-        }
+        for (int bb = 0; bb < 2; ++bb)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (!valid[bb][e]) continue;
+                float* o = p.out + static_cast<size_t>(brow[bb][e]) * p.Hd + j0;
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int u = 8 * jj + uq;
+                    if (u < nvalid) *reinterpret_cast<float2*>(o + u) = make_float2(h[bb][e][jj][0], h[bb][e][jj][1]);
+                }
+            }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 5) tmem_dealloc(tmem_base, 128);
 }
 
 }  // namespace gru
 
 // 1 if the persistent recurrence covers this shape on this device (else the caller runs the per-step sequence)
+// dynamic shared memory of one CTA: alignment slack + resident weight slice + A ring + barriers / bias
+static size_t gru_smem_bytes(int Hd) {
+    return 1024 + static_cast<size_t>(ceil_div(Hd, 64)) * gru::kWChunk + gru::kAStages * gru::kAStage + 1024;
+}
+
 int gru_persistent_supported(int B, int Hd) {
     using namespace gru;
-    if (B < 1 || Hd < 32 || Hd % 4 != 0 || Hd > 960) return 0;
+    if (B < 1 || Hd < 32 || Hd % 4 != 0 || gru_smem_bytes(Hd) > 232448) return 0;
     const int row_tiles = ceil_div(B, 128), slices = ceil_div(Hd, kU);
     return row_tiles * slices <= num_sms() ? 1 : 0;
 }
@@ -306,7 +280,6 @@ int gru_fwd_persistent(int B, int S, int Hd, int ldh, int ldg, const float* gi, 
     p.B = B; p.S = S; p.Hd = Hd; p.ldh = ldh; p.ldg = ldg;
     p.slices = ceil_div(Hd, kU);
     p.k_chunks = ceil_div(Hd, 64);
-    p.ksteps_last = ceil_div(Hd - (p.k_chunks - 1) * 64, 16);
     p.gi = gi; p.bhh = bhh; p.h0 = h0; p.len = len; p.gh = gh; p.hs = hs;
     p.hb = static_cast<__nv_bfloat16*>(hb);
     p.out = out;
@@ -318,7 +291,7 @@ int gru_fwd_persistent(int B, int S, int Hd, int ldh, int ldg, const float* gi, 
     CUtensorMap tmH, tmW;
     NR_PROPAGATE(make_tmap_bf16_2d(&tmH, hb, static_cast<int64_t>(S + 1) * B, Hd, ldh, 64, 128));
     NR_PROPAGATE(make_tmap_bf16_2d(&tmW, whh, 3 * static_cast<int64_t>(Hd), Hd, ldh, 64, kU));
-    const size_t smem = 1024 + static_cast<size_t>(p.k_chunks) * kWChunk + kAStages * kAStage + 1024;
+    const size_t smem = gru_smem_bytes(Hd);
     NR_REQUIRE(smem <= 232448, "gru_fwd_persistent: %zu bytes of shared memory", smem);
     static bool attr_set = false;
     if (!attr_set) {

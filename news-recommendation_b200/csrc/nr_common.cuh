@@ -1,11 +1,13 @@
-// Common device/host helpers for the sm_100a news-recommendation hot path.
-// Raw PTX wrappers for mbarrier / TMA / tcgen05 (TMEM) -- no CUTLASS dependency.
+// Common device/host helpers for the sm_90a news-recommendation hot path.
+// Raw PTX wrappers for mbarrier / TMA / wgmma -- no CUTLASS dependency.
 #pragma once
 
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "nr_wgmma.cuh"
 
 namespace nr {
 
@@ -94,7 +96,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // try_wait with a suspend-time hint: the warp sleeps in hardware until the phase completes or `ns` nanoseconds pass.  Without
 // the hint the instruction gives up after ~30 cycles and a waiting warp turns into a busy loop that competes for issue
 // slots with the warps it is waiting for (ncu on the fused front end: 8 waiting warps per SM took most of the issue slots,
-// tensor pipe 8 % active; profiles/).
+// tensor pipe 8 % active).
 __device__ __forceinline__ bool mbar_try_wait_sleep(uint64_t* bar, uint32_t parity, uint32_t ns) {
     uint32_t ok;
     asm volatile(
@@ -164,120 +166,8 @@ __device__ __forceinline__ void bulk_wait_read() {  // at most N groups of this 
 }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- CTA pairs (cluster of 2, tcgen05 cta_group::2) ----------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-// shared::cluster address of the same shared-memory location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(const void* local, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(local)), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    // default (.release.cta) form, as CUTLASS's umma_arrive_2x1SM_sm0: the .release.cluster form compiles to
-    // MEMBAR.ALL.CTA + ERRBAR in front of the arrive and cost the epilogue warps a third of their time (ncu, profiles/);
-    // the TMEM reads this arrival publishes are ordered by tcgen05.wait::ld + tcgen05.fence::before_thread_sync.
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load of a CTA pair: the data lands in THIS CTA's shared memory, the bytes are counted on the mbarrier at
-// bar_cluster_addr, which may live in the peer (leader) CTA.
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-
-// ---- tcgen05 / TMEM ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// cta_group::2 variants: executed by the same warp of BOTH CTAs of the pair (alloc/dealloc) ...
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// ... and by one thread of the leader CTA only (mma/commit).  D rows 0-127 land in the leader's TMEM, rows 128-255 in
-// the peer's; A comes from both CTAs' shared memory (128 rows each), B rows [0,N/2) from the leader, [N/2,N) from the peer.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on the mbarrier at this shared-memory offset in BOTH CTAs when all earlier MMAs of this thread retire
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 in, fp32 accumulate.  One thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05.mma of this thread complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets TMEM lane (lane_base + i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Wait for an earlier tmem_ld32 into v: the registers are in/out operands, so no use of v can be scheduled before
-// the wait and the 32 registers stay reserved between the (asynchronous) load and this point.
-__device__ __forceinline__ void tmem_ld_wait32(float* v) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                   "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                   "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :
-                 : "memory");
-}
 // Explicit shared-space loads (the epilogue scratch is reached through a generic pointer; LD.E through the generic
-// path is slower than LDS).  volatile keeps them ordered against the TMEM asm statements, where they are placed by hand.
+// path is slower than LDS).  volatile keeps them ordered against the other asm statements, where they are placed by hand.
 __device__ __forceinline__ float4 lds_f4(const float* p) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_u32(p)));
@@ -296,22 +186,18 @@ __device__ __forceinline__ void cp_async_f32(float* smem_dst, const float* gsrc,
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-// Shared-memory matrix descriptor, SWIZZLE_128B (sm_100 "version 1" encoding):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2
+// wgmma shared-memory matrix descriptor, SWIZZLE_128B:
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 1 (128-byte swizzle)
+// K-major operand: rows of 128 bytes (64 bf16 of K), SBO = 1024 between 8-row groups.  MN-major operand: LBO = bytes between
+// 64-element blocks along M / N, SBO = 1024 between 8-row groups along K.  A k-step of 16 elements adds 32 bytes (K-major)
+// or 2048 bytes (MN-major) to the start address.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
-}
-// Instruction descriptor for kind::f16 with bf16 A/B, fp32 D.  major: 0 = K-major, 1 = MN-major.
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-           (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-           (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 // ---- small math / packing ---------------------------------------------------------------------

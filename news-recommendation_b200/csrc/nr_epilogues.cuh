@@ -1,12 +1,12 @@
 // Fused epilogue functors for gemm_nt.  256 epilogue threads: thread (quarter, lane) owns accumulator row
-// r = 32*quarter + lane (= TMEM lane) and the two warps of a quarter ("halves") split the row's 32-column chunks
+// r = 32*quarter + lane and the two warps of a quarter ("halves", one per warpgroup) split the row's 32-column chunks
 // [ch0, ch1).  Contract for every functor:
-//   * the accumulator is read through epi_chunks() (nr_gemm.cuh): one tcgen05.ld per chunk of the thread's range
-//     (warp-collective, the range is warp-uniform), software pipelined, acc.release() exactly once per tile
+//   * the accumulator is read through epi_chunks() (nr_gemm.cuh): one load per chunk of the thread's range (collective
+//     over the thread's warpgroup, the range is warpgroup-uniform), acc.release() exactly once per tile
 //   * init()/finish() bracket the CTA's whole tile loop (all 256 epilogue threads call them)
 //   * kScratchBytes of shared memory belong to the functor (the planner sizes the A ring around it)
 //   * per-slice vectors (bias, query vector, dOut rows) are staged in shared memory: with ~220 KB of smem carved out
-//     the L1 holds next to nothing and per-element global loads made the epilogue 10x the MMA time (ncu, profiles/).
+//     the L1 holds next to nothing and per-element global loads made the epilogue 10x the MMA time.
 //     Anything that must come from global memory per tile is fetched with many loads in flight or prefetched one
 //     tile ahead with cp.async -- a dependent L2 round trip (~600 cycles) per chunk was the whole epilogue time.
 #pragma once
@@ -47,7 +47,7 @@ struct Dropout {
     }
     // the same for a precomputed group index ((row * ld + col) >> 2; callers that walk a row keep row * ld / 4 in a register);
     // 32-bit field tests: the 64-bit shifts / compares of the straightforward form were a quarter of the instructions of the
-    // dropout-carrying epilogues (ncu source page, profiles/)
+    // dropout-carrying epilogues (ncu source page)
     __device__ __forceinline__ void mask4_group(uint64_t group, float* m) const {
         const uint64_t bits = dropout_bits4(seed, group);
         const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
@@ -58,14 +58,11 @@ struct Dropout {
     }
 };
 
-// 16 bf16 = one full 32-byte sector per thread (STG.256, sm_100): halves the L2 write requests of the row-per-thread
-// epilogues compared with two half-sector 16-byte stores.  Needs a 32-byte aligned destination.
+// 16 bf16 = one full 32-byte sector per thread, as two 16-byte stores (sm_90 has no 32-byte store).
 __device__ __forceinline__ void store_bf16x16(__nv_bfloat16* o, const float* y) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(o), "r"(pack_bf16x2(y[0], y[1])),
-                 "r"(pack_bf16x2(y[2], y[3])), "r"(pack_bf16x2(y[4], y[5])), "r"(pack_bf16x2(y[6], y[7])),
-                 "r"(pack_bf16x2(y[8], y[9])), "r"(pack_bf16x2(y[10], y[11])), "r"(pack_bf16x2(y[12], y[13])),
-                 "r"(pack_bf16x2(y[14], y[15]))
-                 : "memory");
+    uint4* q = reinterpret_cast<uint4*>(o);
+    q[0] = make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7]));
+    q[1] = make_uint4(pack_bf16x2(y[8], y[9]), pack_bf16x2(y[10], y[11]), pack_bf16x2(y[12], y[13]), pack_bf16x2(y[14], y[15]));
 }
 __device__ __forceinline__ bool aligned32(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 31) == 0; }
 
@@ -115,7 +112,7 @@ struct EpiStore {
     }
 
     template <class Acc>
-    __device__ void operator()(const Acc& acc, const EpiCtx& c) const {
+    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
         long long orow;
         int t;
         const bool v = rm.map(c.grow, orow, t) && c.valid;
@@ -301,7 +298,7 @@ struct EpiPool {
     }
 
     template <class Acc>
-    __device__ void operator()(const Acc& acc, const EpiCtx& c) const {
+    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
         float score = 0.f;
         epi_chunks(
             acc, c, [](int) {},
@@ -410,7 +407,7 @@ struct EpiDPre {
         if (use_tma) WarpTileStore::drain(e.tid & 31);
     }
     template <class Acc>
-    __device__ void operator()(const Acc& acc, const EpiCtx& c) const {
+    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
         const float ds = c.valid ? __ldg(dscore + c.grow) : 0.f;
         const int lane = c.tid & 31;
         WarpTileStore ts;
@@ -507,7 +504,7 @@ struct EpiDPoolIn {
     }
 
     template <class Acc>
-    __device__ void operator()(const Acc& acc, const EpiCtx& c) const {
+    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
         long long orow;
         int t;
         const bool v = rm.map(c.grow, orow, t) && c.valid;
@@ -702,7 +699,7 @@ struct EpiScatter {
     __device__ void finish(const EpiInit&) const {}
 
     template <class Acc>
-    __device__ void operator()(const Acc& acc, const EpiCtx& c) const {
+    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
         long long trow;
         int t;
         const bool v = rm.map(c.grow, trow, t) && c.valid;

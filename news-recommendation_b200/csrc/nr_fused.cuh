@@ -1,36 +1,10 @@
-// Shared pieces of the fused NRMS news-encoder kernels (fused_fwd.cu, fused_bwd.cu): PTX wrappers that nr_common.cuh does
-// not have (A operand in TMEM, tcgen05.st, x16 loads), the bounded mbarrier wait of this translation-unit family, and the
-// tile geometry both kernels share.
+// Device error record and bounded mbarrier wait of the translation units that keep their own watchdog record
+// (gru_persist.cu, attn_title.cu).
 #pragma once
 #include "nr_common.cuh"
 
 namespace nr {
 namespace fused {
-
-// ---- tile geometry (news level of the reference: num_words_title = 20, 15 heads x d_k 20; config.py:14-33) -------------
-// A tile is 128 accumulator rows = kTPT whole titles (kRows used rows, the rest dead): titles never straddle tiles, so the
-// per-title attention is block diagonal inside one 128 x 128 score tile.
-template <int T>
-struct Geo {
-    static constexpr int kTPT = 128 / T;        // titles per tile
-    static constexpr int kRows = kTPT * T;      // used rows per tile
-    static_assert(T % 4 == 0 && T >= 16 && T <= 20, "title length: multiple of 4 in [16, 20] (three titles of a lane quarter fit one 64-column window)");
-};
-
-// Score-window geometry of one TMEM lane quarter (32 accumulator rows): the rows of quarter QD belong to titles
-// [tlo, thi]; their keys are the score columns [tlo*T, (thi+1)*T), loaded as ONE 64-column window starting at `start`.
-template <int T, int QD>
-struct Win {
-    static constexpr int kTPT = 128 / T;
-    static constexpr int tlo = (32 * QD) / T;
-    static constexpr int thi_raw = (32 * QD + 31) / T;
-    static constexpr int thi = thi_raw < kTPT ? thi_raw : kTPT - 1;
-    static constexpr int ncand = thi - tlo + 1;                      // 1..3 candidate titles
-    static constexpr int start = (tlo * T < 64) ? tlo * T : 64;     // window = score columns [start, start + 64)
-    static_assert(ncand >= 1 && ncand <= 3, "a lane quarter spans at most three titles");
-    static_assert((thi + 1) * T - start <= 64, "score window of a lane quarter exceeds 64 columns");
-    static_assert(start % 4 == 0, "window start must stay 4-column aligned");
-};
 
 // ---- device error record + bounded waits of the fused kernels -------------------------------------------------------------
 // every translation unit of this family names its own record (no relocatable device code): #define NR_WATCHDOG_SYMBOL first
@@ -54,69 +28,6 @@ __device__ __forceinline__ void f_wait(uint64_t* bar, uint32_t parity, int code)
     }
 }
 #endif
-
-// ---- tcgen05 pieces ------------------------------------------------------------------------------------------------------------
-// D[tmem] (+)= A[tmem, bf16 packed two per 32-bit column] * B[smem desc]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp writes TMEM lane (lane_base + i)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-          "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-          "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- shared-memory operand tiles written by hand -----------------------------------------------------------------------------
-// SWIZZLE_128B tile of 128-byte rows: 16-byte piece j of row r lives at r*128 + ((j ^ (r & 7)) << 4).  The same bytes serve as
-// a K-major operand ([row][k]) and as an MN-major operand ([k][n]) -- only the descriptor differs.
-__device__ __forceinline__ uint32_t sw128_off(int r, int piece) { return static_cast<uint32_t>(r) * 128u + (static_cast<uint32_t>(piece ^ (r & 7)) << 4); }
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void sts64(uint32_t saddr, uint32_t a, uint32_t b) {
-    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(saddr), "r"(a), "r"(b) : "memory");
-}
-// 20 bf16 values (10 packed words) of row r into elements [e0, e0 + 20) of a SW128 tile; e0 % 8 == 0
-__device__ __forceinline__ void sts_row20(uint32_t tile, int r, int e0, const uint32_t* w) {
-    const int p0 = e0 >> 3;
-    sts128(tile + sw128_off(r, p0), w[0], w[1], w[2], w[3]);
-    sts128(tile + sw128_off(r, p0 + 1), w[4], w[5], w[6], w[7]);
-    sts64(tile + sw128_off(r, p0 + 2), w[8], w[9]);
-}
-__device__ __forceinline__ void stg64(void* p, uint32_t a, uint32_t b) {
-    asm volatile("st.global.v2.b32 [%0], {%1, %2};" ::"l"(p), "r"(a), "r"(b) : "memory");
-}
-
-// keep-multipliers of the four elements of one aligned dropout group (see Dropout::mask4 in nr_epilogues.cuh: same counter
-// hash, same (row * ld + col) >> 2 group index, so forward and backward kernels of either path agree on every mask)
-__device__ __forceinline__ void drop4(uint64_t seed, uint32_t thresh, float scale, long long row, int ld, int col4, float* m) {
-    const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(row) * ld + col4) >> 2);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) m[i] = (((bits >> (16 * i)) & 0xffffu) >= thresh) ? scale : 0.f;
-}
 
 }  // namespace fused
 }  // namespace nr

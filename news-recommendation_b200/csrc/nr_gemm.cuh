@@ -1,35 +1,38 @@
-// Weight-stationary persistent tcgen05 GEMMs for the news-recommendation hot path (sm_100a).
+// Weight-stationary persistent wgmma GEMMs for the news-recommendation hot path (sm_90a).
 //
 //  gemm_nt : D[M x N] = A[M x K] . B[N x K]^T      (both K-major; "activation x weight^T")
-//            * a CTA pair's weight slice (<=256 output columns, all K, all conv taps; half the rows in
-//              each CTA) is loaded ONCE by TMA and stays resident in shared memory; 128-row activation
-//              tiles stream through a TMA/mbarrier ring; accumulators are double buffered in TMEM
-//              (2 x 256 fp32 columns); 8 epilogue warps run a fused epilogue functor on tcgen05.ld'ed rows.
+//            * a CTA's weight slice (<=256 output columns, all K, all conv taps) is loaded ONCE by TMA and stays
+//              resident in shared memory; 128-row activation tiles stream through a TMA/mbarrier ring; two consumer
+//              warpgroups issue wgmma into registers and then run a fused epilogue functor on the accumulator rows.
 //            * conv taps: tap s re-loads the A tile shifted by (s - taps/2) rows (zero rows separate
-//              the segments in the padded layout), accumulating into the same TMEM tile.
+//              the segments in the padded layout), accumulating into the same registers.
 //  gemm_tn : D[Ma x Nb] += A[Kr x Ma]^T . B[Kr x Nb]  (both MN-major; weight gradients, Kr = all tokens)
-//            split over Kr across CTAs, fp32 red.global.add epilogue.
+//            split over Kr (and over Nb past 256 columns) across CTAs, fp32 red.global.add epilogue.
 //
-// Warp roles of gemm_nt (kGemmThreads per CTA, CTAs launched as pairs): warps 0..kEpiWarps-1 epilogue (TMEM lane
-// quarter = warp & 3; the kEpiParts warps of a quarter split the accumulator columns -- with 4 warps the row-per-thread
-// epilogue was latency bound at ~20 % issue utilisation, ncu profiles/), then the TMA producer warp and the warp that
-// allocates TMEM and, in the leader CTA, issues the MMAs.
-// gemm_tn keeps 192 threads (4 epilogue warps, one-shot epilogue).
+// Warp roles of gemm_nt (kGemmThreads per CTA): warps 0..kEpiWarps-1 form two warpgroups.  Warpgroup h computes ALL 128
+// rows of the tile for its share of the slice's 32-column chunks (the "half" of the epilogue contract) with two m64 wgmmas
+// per k-step, so each epilogue thread finds its row and its columns inside its own warpgroup: the row-per-thread view the
+// epilogues read is made by passing one 32-column chunk at a time through a small shared-memory transpose buffer.  The
+// first warp of the last warpgroup is the TMA producer.
 #pragma once
 #include "nr_common.cuh"
 
 namespace nr {
 
-constexpr int kTnThreads = 192;     // gemm_tn
-constexpr int kEpiWarps = 8;  // gemm_nt epilogue warps: 4 TMEM lane quarters x kEpiParts column parts
+constexpr int kEpiWarps = 8;  // gemm_nt epilogue warps: 2 warpgroups (= column parts) x 4 warps (32 rows each)
 constexpr int kEpiParts = kEpiWarps / 4;
 constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kGemmThreads = kEpiThreads + 64;  // + TMA producer warp + MMA warp
+// + a producer warpgroup (one warp issues TMA): registers are allocated per warpgroup, and setmaxnreg moves the producer's
+// share to the consumers, whose accumulators and epilogue registers need more than the even split of 168
+constexpr int kGemmThreads = kEpiThreads + 128;
+constexpr int kTnThreads = kGemmThreads;        // gemm_tn: the same two consumer warpgroups + producer
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr int kTileM = 128;
 constexpr int kChunkK = 64;                     // bf16 elements per 128-byte swizzle row
 constexpr int kAStageBytes = kTileM * 128;      // 16 KB
 constexpr int kMaxStages = 12;
 constexpr int kSmemLimit = 232448;              // 227 KB
+constexpr int kXposeBytes = kEpiParts * 128 * 16 * 4;  // per warpgroup: 128 rows x 16 fp32 columns (half a chunk)
 
 struct GemmNTParams {
     int M;              // rows of A that exist
@@ -44,25 +47,27 @@ struct GemmNTParams {
     int taps;           // 1, or 3 for the window-3 title CNN
     int b_tap_rows;     // row offset between taps inside the weight operand
     int stages;
+    int b_stream;       // 1: the weight slice does not fit beside the ring; its (tap, k-chunk) box travels with every A stage
+    int stage_bytes;    // kAStageBytes (+ one weight box when b_stream)
     float* dbg_acc;     // debug backend only: fp32 accumulators [num_m_tiles*128][dbg_ld]
     int dbg_ld;
-    int dbg_flags;      // tuning only (NEWSREC_GEMM_DBG): bit 1 = the producers skip the A loads (MMA on stale data)
+    int dbg_flags;      // tuning only (NEWSREC_GEMM_DBG): bit 1 = the producer skips the A loads (MMA on stale data)
     long long* timing;  // tuning only (nr_debug_set_gemm_timing): per CTA 16 cycle counters, see the kernel
 };
 
 // What an epilogue functor sees for one (tile,row).
 struct EpiCtx {
     int tile;
-    int r;        // row inside the tile (0..127) == TMEM lane
+    int r;        // row inside the tile (0..127)
     int grow;     // global A row
     bool valid;   // r < rows_per_tile && grow < M
     int col0;     // first output column of this CTA's slice
     int ncols;    // valid output columns in the slice
     int tid;      // 0..255 within the epilogue group
-    int half;     // 0 .. kEpiParts-1: which of the warps of this TMEM lane quarter (column part)
+    int half;     // 0 .. kEpiParts-1: column part (= warpgroup)
     int ch0, ch1; // this thread's range of 32-column chunks
     float* scratch;  // Epi::kScratchBytes of shared memory private to the epilogue group
-    int it;          // how many tiles this CTA has finished before this one (double-buffer parity)
+    int it;          // how many tiles this CTA has finished before this one (double-buffer parity of the epilogue staging)
     int next_tile;   // the tile this CTA processes next, or -1
 };
 // What init()/finish() see.
@@ -82,21 +87,54 @@ __device__ __forceinline__ void epi_chunk_range(int ncols, int part, int& ch0, i
     ch1 = ch0 + base + (part < rem ? 1 : 0);
 }
 
-struct TmemAcc {
-    uint32_t taddr;
-    uint32_t release_bar;  // shared::cluster address of the leader CTA's "accumulator free" barrier
+// Accumulators of one warpgroup: acc[b] is the m64 wgmma fragment of rows [64b, 64b + 64) for the warpgroup's chunks
+// [ch0, ch1) (at most 4).  load32(ch) hands every thread the 32 columns of chunk ch of its own row (row = thread of the
+// warpgroup), through the warpgroup's transpose buffer, 16 columns at a time; every thread of the warpgroup calls it with the
+// same chunk sequence (the chunk range is per warpgroup).  Buffer layout: row r, column c at r*16 + ((c/4) ^ ((r/2)&3))*4 + c%4
+// (conflict-free row reads).
+struct RegAcc {
+    float (*acc)[64];
+    float* xpose;   // this warpgroup's 8 KB
+    int ch0;
+    int bar_id;     // named barrier of the warpgroup
+    __device__ __forceinline__ void sync() const { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); }
+    template <int Q>
+    __device__ __forceinline__ void put_half(int hf) const {  // columns [32Q + 16hf, +16) of the fragment into the buffer
+        const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj) {
+                const int j = 4 * Q + 2 * hf + jj;  // 8-column group of the fragment
+                const int c = 8 * jj + 2 * (lane & 3);
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int r = 64 * b + 16 * wq + (lane >> 2) + 8 * e;
+                    *reinterpret_cast<float2*>(xpose + r * 16 + (((c >> 2) ^ ((r >> 1) & 3)) << 2) + (c & 3)) =
+                        make_float2(acc[b][4 * j + 2 * e], acc[b][4 * j + 2 * e + 1]);
+                }
+            }
+    }
     __device__ __forceinline__ void load32(int chunk, float* v) const {
-        tmem_ld32(taddr + chunk * 32, v);
-        tmem_ld_wait();
+        const int q = chunk - ch0, r = threadIdx.x & 127;
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            sync();  // every thread has read the previous half out of the buffer
+            switch (q) {
+                case 0: put_half<0>(hf); break;
+                case 1: put_half<1>(hf); break;
+                case 2: put_half<2>(hf); break;
+                default: put_half<3>(hf); break;
+            }
+            sync();
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+                const float4 f = lds_f4(xpose + r * 16 + ((g ^ ((r >> 1) & 3)) << 2));
+                v[16 * hf + 4 * g] = f.x; v[16 * hf + 4 * g + 1] = f.y; v[16 * hf + 4 * g + 2] = f.z; v[16 * hf + 4 * g + 3] = f.w;
+            }
+        }
     }
-    __device__ __forceinline__ void issue32(int chunk, float* v) const { tmem_ld32(taddr + chunk * 32, v); }
-    __device__ __forceinline__ void wait32(float* v) const { tmem_ld_wait32(v); }
-    // All TMEM reads of this tile by this WARP are done (every call site is warp-uniform): one arrival per warp.
-    __device__ __forceinline__ void release() const {
-        tc_fence_before();
-        __syncwarp();
-        if ((threadIdx.x & 31) == 0) mbar_arrive_cluster(release_bar);
-    }
+    __device__ __forceinline__ void release() const {}
 };
 struct GlobalAcc {  // debug backend: accumulators computed by a plain SIMT kernel
     const float* row;
@@ -104,42 +142,27 @@ struct GlobalAcc {  // debug backend: accumulators computed by a plain SIMT kern
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = row[chunk * 32 + j];
     }
-    __device__ __forceinline__ void issue32(int chunk, float* v) const { load32(chunk, v); }
-    __device__ __forceinline__ void wait32(float*) const {}
     __device__ __forceinline__ void release() const {}
 };
 
-// The chunk loop every epilogue shares, software pipelined over two register buffers: the tcgen05.ld of chunk i+1 is
-// in flight while body(i) runs (a single-buffered loop exposed the TMEM round trip once per chunk).  pre(ch) runs
-// before the wait of chunk ch (shared-memory operand loads go there).  Calls acc.release() exactly once, right after
-// the last chunk has landed in registers.
+// The chunk loop every epilogue shares.  pre(ch) runs before the load of chunk ch (shared-memory operand loads go there).
+// Calls acc.release() exactly once, after the last chunk has landed in registers.
 template <class Acc, class Pre, class Body>
 __device__ __forceinline__ void epi_chunks(const Acc& acc, const EpiCtx& c, Pre&& pre, Body&& body) {
-    if (c.ch0 >= c.ch1) {
-        acc.release();
-        return;
-    }
-    float xa[32], xb[32];
-    acc.issue32(c.ch0, xa);
-    for (int ch = c.ch0; ch < c.ch1; ch += 2) {
+    for (int ch = c.ch0; ch < c.ch1; ++ch) {
+        float x[32];
         pre(ch);
-        acc.wait32(xa);
-        if (ch + 1 < c.ch1) acc.issue32(ch + 1, xb); else acc.release();
-        body(ch, xa);
-        if (ch + 1 < c.ch1) {
-            pre(ch + 1);
-            acc.wait32(xb);
-            if (ch + 2 < c.ch1) acc.issue32(ch + 2, xa); else acc.release();
-            body(ch + 1, xb);
-        }
+        acc.load32(ch, x);
+        if (ch + 1 == c.ch1) acc.release();
+        body(ch, x);
     }
+    if (c.ch0 >= c.ch1) acc.release();
 }
 
 // bf16 output tiles leave through TMA instead of 32 scattered rows per store instruction: a warp packs its 32 rows x 32
 // columns into a private staging buffer (SWIZZLE_64B layout: 16-byte chunk q of row r at r*64 + ((q ^ (r>>1)) & 3)*16,
 // conflict-free for row-per-lane 16-byte writes) and one lane issues cp.async.bulk.tensor.  Two buffers per warp.
-// Measured alone (tools/stbench.cu): 5.7 TB/s vs 2.6 (2 x STG.128) / 5.0 (STG.256); inside the GEMM the row-per-thread
-// stores sat in the LSU queue and stalled the warps on their source registers (ncu, profiles/).
+// Row-per-thread stores of 32 rows sit in the LSU queue and stall the warps on their source registers.
 constexpr int kTileStoreBufs = 2;                                  // staging tiles per warp (2 KB each)
 constexpr int kTileStoreBytes = kEpiWarps * kTileStoreBufs * 2048 + 1024;  // + alignment slack
 struct WarpTileStore {
@@ -197,57 +220,91 @@ struct WarpTileStore {
 };
 
 // ---------------------------------------------------------------------------------------------
-// gemm_nt kernel: one CTA PAIR (cluster of 2, tcgen05 cta_group::2) per (256-row block, weight slice)
+// gemm_nt kernel: one CTA per (tile sequence, weight slice)
 // ---------------------------------------------------------------------------------------------
-// Both CTAs stream their own 128-row activation tiles and hold HALF of the slice's weight rows; the leader (cluster rank
-// 0) issues M=256 MMAs that read A and B from both CTAs' shared memory and leave rows 0-127 of D in its own TMEM, rows
-// 128-255 in the peer's.  Halving the resident weight bytes is what buys the A ring its depth: with 4 stages the ring
-// was latency bound (a stage is refilled only after its MMAs retire; (TMA latency + MMA time) / stages > MMA time).
-// mbarrier protocol (every barrier exists in both CTAs at the same offset; "L" = only the leader's copy is used):
-//   bfull  L  count 1 + tx of both weight halves        -> MMA issuer may start
-//   full[s] L count 1 + tx of both CTAs' A boxes         (leader's producer arrives with expect_tx of 2 boxes; the
-//                                                         peer's TMA signals the leader's barrier, cta_group::2)
-//   empty[s]  count 1, multicast tcgen05.commit          -> each CTA's producer refills its own stage s
-//   tfull[a]  count 1, multicast tcgen05.commit          -> each CTA's epilogue reads its own TMEM rows
-//   tempty[a] L count 16 (8 epilogue warps x 2 CTAs, the peer arrives through shared::cluster)
+// mbarrier protocol:
+//   bfull     count 1 + tx of the resident weight slice    -> the consumers may start (not used when b_stream)
+//   full[s]   count 1 + tx of one A box (+ its weight box when b_stream; the producer's expect_tx)
+//   empty[s]  count kEpiWarps: every consumer warp arrives once its wgmmas on stage s have completed
+// Warpgroup h multiplies the 128-row A tile by the weight rows of its chunks [ch0, ch1): two m64 x (32 * nch) wgmmas per
+// k-step, nch <= 4 (a slice is <= 256 columns, split into two parts).
+// The MMAs of one tile for a warpgroup with NCH chunks (a compile-time N keeps the wgmmas asynchronous): one wgmma group
+// per ring stage, one group left in flight while the next stage is awaited; a stage is released once its group completed.
+template <int NCH>
+__device__ __forceinline__ void gemm_nt_mma_tile(float (*acc)[64], const GemmNTParams& p, uint64_t* full, uint64_t* empty,
+                                                 int& st, uint32_t& ph, uint32_t a_s, uint32_t b_s, uint32_t b_off, int b_region,
+                                                 int lane) {
+    int prev = -1;
+    for (int s = 0; s < p.taps; ++s)
+        for (int kc = 0; kc < p.k_chunks; ++kc) {
+            mbar_wait(&full[st], ph, 104);
+            if constexpr (NCH > 0) {
+                const uint32_t a_st = a_s + st * p.stage_bytes;
+                const uint32_t b_box = p.b_stream ? a_st + kAStageBytes + b_off : b_s + (s * p.k_chunks + kc) * b_region;
+                const uint64_t db = make_sw128_desc(b_box, 16, 1024);
+                const int first = (s | kc) == 0;
+#pragma unroll
+                for (int b = 0; b < 2; ++b)
+#pragma unroll
+                    for (int i = 0; i < 16 * NCH; ++i) wgmma_reg_fence(acc[b][i]);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k)  // +32 bytes per k-step = +2 in the descriptor's >>4 address field
+#pragma unroll
+                    for (int b = 0; b < 2; ++b)
+                        Wgmma<32 * NCH, 0, 0>::mma(acc[b], make_sw128_desc(a_st + b * 8192, 16, 1024) + 2 * k, db + 2 * k,
+                                                   (first && k == 0) ? 0 : 1);
+                wgmma_commit();
+                wgmma_wait<1>();  // the group of the previous stage has completed
+            }
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev]);  // this warp's reads of stage prev are complete
+            }
+            prev = st;
+            if (++st == p.stages) { st = 0; ph ^= 1; }
+        }
+    if constexpr (NCH > 0) {
+        wgmma_wait<0>();
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int i = 0; i < 16 * NCH; ++i) wgmma_reg_fence(acc[b][i]);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+}
+
 template <class Epi>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmNTParams p,
                const __grid_constant__ Epi epi) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
 
-    const int b_region = (p.n_box >> 1) * 128;  // bytes of one (tap, k-chunk) box of this CTA's weight half
+    const int b_region = p.n_box * 128;  // bytes of one (tap, k-chunk) box of the weight slice
     uint8_t* sB = smem;
-    uint8_t* sA = sB + p.taps * p.k_chunks * b_region;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sA + p.stages * kAStageBytes);
+    uint8_t* sA = sB + (p.b_stream ? 0 : p.taps * p.k_chunks * b_region);
+    float* xpose = reinterpret_cast<float*>(sA + p.stages * p.stage_bytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(xpose) + kXposeBytes);
     uint64_t* full = bars;
     uint64_t* empty = bars + kMaxStages;
     uint64_t* bfull = bars + 2 * kMaxStages;
-    uint64_t* tfull = bars + 2 * kMaxStages + 1;
-    uint64_t* tempty = bars + 2 * kMaxStages + 3;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 5);
     float* scratch = reinterpret_cast<float*>(bars + 2 * kMaxStages + 8);
 
-    const int pair = blockIdx.x >> 1;
-    const int slice = pair % p.n_slices;
-    const int ptile0 = pair / p.n_slices;                // pair tile = 256 rows_per_tile-rows: tiles 2*pt and 2*pt + 1
-    const int ptile_step = (gridDim.x >> 1) / p.n_slices;
-    const int num_ptiles = (p.num_m_tiles + 1) >> 1;
+    const int slice = blockIdx.x % p.n_slices;
+    const int tile0 = blockIdx.x / p.n_slices;
+    const int tile_step = gridDim.x / p.n_slices;
     const int col0 = slice * p.n_stride;
     const int ncols = min(p.n_stride, p.N - col0);
-    const int n_mma = (ncols + 15) & ~15;                // MMA N of this slice; each CTA supplies n_mma/2 weight rows
     const int tap_shift = p.taps / 2;
-    // tuning counters: [0] producer waits for a free A stage, [1] MMA waits for A data, [2] MMA waits for a free
-    // accumulator, [3] epilogue waits for a finished accumulator, [4] epilogue body, [5] kernel, [6] tiles,
-    // [7] MMA issue loops, [8] tcgen05.commit
+    // tuning counters: [0] producer waits for a free A stage, [1] MMA loops incl. waits for A data, [4] epilogue body, [5] kernel,
+    // [6] tiles
     long long* tmr = p.timing != nullptr ? p.timing + blockIdx.x * 16 : nullptr;
     const long long t_begin = tmr != nullptr ? clock64() : 0;
-    long long tw_a = 0, tw_b = 0, tw_c = 0, tw_d = 0;
+    long long tw_a = 0, tw_b = 0;
     auto timed_wait = [&](uint64_t* bar, uint32_t parity, int code, long long& acc_t) {
         if (tmr != nullptr) {
             const long long t = clock64();
@@ -263,51 +320,42 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
+            mbar_init(&empty[i], kEpiWarps);
         }
         mbar_init(bfull, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], 2 * (kEpiThreads / 32));
-        }
         fence_barrier_init();
-    } else if (warp == kEpiWarps + 1) {
-        tmem_alloc_pair(tmem_slot, 512);
     }
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();  // the peer's barriers are initialised before anything is multicast to them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == kEpiWarps) {
-        // ===================== TMA producer (both CTAs; uniform loops, one elected lane issues) =====================
-        const uint32_t bfull_l = mapa_shared(bfull, 0);
-        if (elect_one()) {
-            if (leader) mbar_arrive_expect_tx(bfull, static_cast<uint32_t>(2 * p.taps * p.k_chunks * b_region));
+    if (warp >= kEpiWarps) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        if (warp != kEpiWarps) return;
+        // ===================== TMA producer (uniform loops, one elected lane issues) =====================
+        if (!p.b_stream && elect_one()) {
+            mbar_arrive_expect_tx(bfull, static_cast<uint32_t>(p.taps * p.k_chunks * b_region));
             for (int s = 0; s < p.taps; ++s)
                 for (int kc = 0; kc < p.k_chunks; ++kc)
-                    tma_load_2d_pair(sB + (s * p.k_chunks + kc) * b_region, &tmB, bfull_l, kc * kChunkK,
-                                     s * p.b_tap_rows + col0 + static_cast<int>(rank) * (n_mma >> 1));
+                    tma_load_2d(sB + (s * p.k_chunks + kc) * b_region, &tmB, bfull, kc * kChunkK, s * p.b_tap_rows + col0);
         }
         __syncwarp();
         int st = 0;
         uint32_t ph = 0;
-        for (int pt = ptile0; pt < num_ptiles; pt += ptile_step) {
-            const int row0 = (2 * pt + static_cast<int>(rank)) * p.rows_per_tile;  // past M: zero filled
+        for (int tile = tile0; tile < p.num_m_tiles; tile += tile_step) {
+            const int row0 = tile * p.rows_per_tile;
             for (int s = 0; s < p.taps; ++s)
                 for (int kc = 0; kc < p.k_chunks; ++kc) {
                     timed_wait(&empty[st], ph ^ 1, 101, tw_a);
                     if (elect_one()) {
 #ifdef NEWSREC_TRIAGE
                         if (p.dbg_flags & 2) {
-                            if (leader) mbar_arrive(&full[st]);
+                            mbar_arrive(&full[st]);
                         } else
 #endif
                         {
-                            if (leader) mbar_arrive_expect_tx(&full[st], 2 * kAStageBytes);
-                            tma_load_2d_pair(sA + st * kAStageBytes, &tmA, mapa_shared(&full[st], 0), kc * kChunkK,
-                                             row0 + s - tap_shift);
+                            mbar_arrive_expect_tx(&full[st], p.stage_bytes);
+                            tma_load_2d(sA + st * p.stage_bytes, &tmA, &full[st], kc * kChunkK, row0 + s - tap_shift);  // rows past M / before 0: zero filled
+                            if (p.b_stream)
+                                tma_load_2d(sA + st * p.stage_bytes + kAStageBytes, &tmB, &full[st], kc * kChunkK, s * p.b_tap_rows + col0);
                         }
                     }
                     __syncwarp();
@@ -315,62 +363,38 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
         }
         if (tmr != nullptr && lane == 0) tmr[0] = tw_a;
-    } else if (warp == kEpiWarps + 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        // The whole warp runs the loops (uniform control flow) and one elected lane issues: under an `if (lane == 0)`
-        // the compiler wraps every tcgen05 instruction in a uniform-register waterfall loop, and together with the
-        // run-time k-step count that made the issuing thread -- not the tensor pipe -- the limiter (~240 cycles per MMA
-        // against the pipe's 120 even with loads and epilogue switched off).  Columns past K are zero filled by TMA in
-        // both operands, so every k-chunk issues all four k-steps.
-        if (leader) {
-            const uint32_t idesc = make_idesc_bf16(2 * kTileM, n_mma, 0, 0);
-            mbar_wait(bfull, 0, 102);
-            tc_fence_after();
-            int st = 0;
-            uint32_t ph = 0;
-            int it = 0;
-            for (int pt = ptile0; pt < num_ptiles; pt += ptile_step, ++it) {
-                const int as = it & 1;
-                timed_wait(&tempty[as], ((it >> 1) & 1) ^ 1, 103, tw_b);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * 256;
-                uint32_t acc = 0;
-                for (int s = 0; s < p.taps; ++s)
-                    for (int kc = 0; kc < p.k_chunks; ++kc) {
-                        timed_wait(&full[st], ph, 104, tw_a);
-                        tc_fence_after();
-                        const long long t_i0 = tmr != nullptr ? clock64() : 0;
-                        if (elect_one()) {
-                            const uint64_t da = make_sw128_desc(smem_u32(sA + st * kAStageBytes), 0, 1024);
-                            const uint64_t db = make_sw128_desc(smem_u32(sB + (s * p.k_chunks + kc) * b_region), 0, 1024);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k)  // +32 bytes per k-step = +2 in the descriptor's >>4 address field
-                                umma_bf16_pair(d_tmem, da + 2 * k, db + 2 * k, idesc, (k == 0) ? acc : 1u);
-                            umma_commit_pair(&empty[st]);  // frees stage st in both CTAs when these MMAs retire
-                        }
-                        __syncwarp();
-                        acc = 1;
-                        if (tmr != nullptr) tw_c += clock64() - t_i0;
-                        if (++st == p.stages) { st = 0; ph ^= 1; }
-                    }
-                if (elect_one()) umma_commit_pair(&tfull[as]);
-                __syncwarp();
-            }
-            if (tmr != nullptr && lane == 0) { tmr[1] = tw_a; tmr[2] = tw_b; tmr[7] = tw_c; tmr[8] = tw_d; }
-        }
     } else {
-        // ===================== epilogue warps 0..kEpiWarps-1 (both CTAs, own TMEM rows) =====================
-        const int tile_step = 2 * ptile_step;
-        const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, 2 * ptile0 + static_cast<int>(rank), p.num_m_tiles};
-        epi.init(ei, tile_step);
+        // ===================== consumer warpgroups: wgmma, then the epilogue on the same registers =====================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+        const int half = warp >> 2;
         const int quarter = warp & 3;
-        const uint32_t tempty_l0 = mapa_shared(&tempty[0], 0), tempty_l1 = mapa_shared(&tempty[1], 0);
+        int ch0, ch1;
+        epi_chunk_range(ncols, half, ch0, ch1);
+        const int nch = ch1 - ch0;
+        const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, p.num_m_tiles};
+        epi.init(ei, tile_step);
+        const uint32_t a_s = smem_u32(sA), b_s = smem_u32(sB) + ch0 * 32 * 128;
+        const uint32_t b_off = ch0 * 32 * 128;
+        float acc[2][64];
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[b][i] = 0.f;
+        const RegAcc racc{acc, xpose + half * (kXposeBytes / 4 / kEpiParts), ch0, 2 + half};
+        if (!p.b_stream) mbar_wait(bfull, 0, 102);
+        int st = 0;
+        uint32_t ph = 0;
         int it = 0;
-        for (int pt = ptile0; pt < num_ptiles; pt += ptile_step, ++it) {
-            const int tile = 2 * pt + static_cast<int>(rank);  // may be one past the last tile: every row invalid
-            const int as = it & 1;
-            timed_wait(&tfull[as], (it >> 1) & 1, 105, tw_a);
-            tc_fence_after();
+        for (int tile = tile0; tile < p.num_m_tiles; tile += tile_step, ++it) {
+            const long long t_mma = tmr != nullptr ? clock64() : 0;
+            switch (nch) {
+                case 0: gemm_nt_mma_tile<0>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
+                case 1: gemm_nt_mma_tile<1>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
+                case 2: gemm_nt_mma_tile<2>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
+                case 3: gemm_nt_mma_tile<3>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
+                default: gemm_nt_mma_tile<4>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
+            }
+            if (tmr != nullptr) tw_b += clock64() - t_mma;
             const long long t_epi = tmr != nullptr ? clock64() : 0;
             EpiCtx c;
             c.tile = tile;
@@ -380,23 +404,18 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             c.col0 = col0;
             c.ncols = ncols;
             c.tid = threadIdx.x;
-            c.half = warp >> 2;
-            epi_chunk_range(ncols, c.half, c.ch0, c.ch1);
+            c.half = half;
+            c.ch0 = ch0;
+            c.ch1 = ch1;
             c.scratch = scratch;
             c.it = it;
             c.next_tile = tile + tile_step < p.num_m_tiles ? tile + tile_step : -1;
-            TmemAcc acc{tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * 256, as ? tempty_l1 : tempty_l0};
-            epi(acc, c);
-            if (tmr != nullptr) tw_b += clock64() - t_epi;
+            epi(racc, c);
+            if (tmr != nullptr) tw_a += clock64() - t_epi;
         }
         epi.finish(ei);
-        if (tmr != nullptr && threadIdx.x == 0) { tmr[3] = tw_a; tmr[4] = tw_b; tmr[5] = clock64() - t_begin; tmr[6] = it; }
+        if (tmr != nullptr && threadIdx.x == 0) { tmr[1] = tw_b; tmr[4] = tw_a; tmr[5] = clock64() - t_begin; tmr[6] = it; }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();  // nobody leaves (or frees TMEM) while the partner may still read its shared memory / signal it
-    if (warp == kEpiWarps + 1) tmem_dealloc_pair(tmem_base, 512);
 }
 
 // Debug backend (TRIAGE builds only -- `make TRIAGE=1`, -DNEWSREC_TRIAGE; the release library has no second backend and
@@ -448,6 +467,7 @@ struct GemmTNParams {
     int b_col0;      // first B column
     int b_row_shift; // B row = A row + shift (conv taps)
     int m_tiles;
+    int n_tiles;     // CTAs along Nb (<= 256 columns each)
     int k_slices;
     int chunks_per_slice;  // 64-row chunks per CTA
     int n_boxes;     // ceil(Nb/64)
@@ -456,8 +476,6 @@ struct GemmTNParams {
     int ldd;
 };
 
-__global__ void __launch_bounds__(kTnThreads, 1)
-gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmTNParams p);
 
 // ---------------------------------------------------------------------------------------------
 // host-side launch helpers (gemm.cu)

@@ -15,7 +15,7 @@ struct RowMapCfg {  // see RowMap in nr_epilogues.cuh; seg_in == 0 => identity
     int seg_in, in_off, seg_len, seg_out, out_off;
 };
 
-// ---- tcgen05 GEMMs with fused epilogues (gemm.cu) ------------------------------------------------
+// ---- wgmma GEMMs with fused epilogues (gemm.cu) ------------------------------------------------
 // out[rows x N] = act(A . W^T + bias) (bf16 or fp32).  A bf16 [M x K] pitch lda (taps>1: padded CNN layout),
 // W bf16 [taps*w_tap_rows x K] pitch ldw.
 int gemm_store(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,
@@ -92,14 +92,6 @@ int embedding_f32_fwd(const long long* ids, long long n, const float* table, int
                       cudaStream_t stream);
 int embedding_f32_bwd(const long long* ids, long long n, const float* dout, int V, int D, float* dtable, cudaStream_t stream);
 
-// ---- fused NRMS news-encoder front end (fused_fwd.cu): ids -> gather -> Q|K|V -> attention -> context hi/lo planes -----
-// w_heads bf16 [heads*64][ldx]: per head the rows W_Q[h] | W_K[h] | W_V[h] | zero rows up to 64; b_heads fp32 [heads*64].
-// X may be null (inference): it is only written for the backward kernels.  Q|K|V never reaches HBM.
-int mhsa_fused_supported(int T, int d, int heads);
-int mhsa_fused_fwd(const long long* ids, long long n_seq, int T, const void* table, int V, int d, int heads, int ldx,
-                   const void* w_heads, const float* b_heads, DropoutCfg drop_x, DropoutCfg drop_c, void* X, void* C_hi, void* C_lo,
-                   int* bad_id_flag, cudaStream_t stream);
-int read_fused_device_error(int* out4);
 
 // ---- persistent GRU recurrence (gru_persist.cu): all S steps of h_t = GRU(gi_t, h_{t-1}) in one cooperative launch --------
 int gru_persistent_supported(int B, int Hd);

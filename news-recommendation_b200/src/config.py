@@ -31,14 +31,12 @@ BaseConfig = type("BaseConfig", (), dict(_COMMON, __doc__="General configuration
 
 _CNN = {"num_filters": 300, "window_size": 3}
 _PER_MODEL = {
-    # precision / fused_news_encoder are extension knobs of this build (not in the reference; DESIGN.md section 4):
+    # precision is an extension knob of this build (not in the reference; DESIGN.md section 4):
     #   precision "accurate" (default): V / attention probabilities / context as hi/lo bf16 pairs and an fp32-accurate user
     #   encoder -- logits within 1e-3 of the fp32 oracle on bf16-rounded weights (the blueprint's tolerance); "fast": every
-    #   activation stored bf16 (~6e-3, 18 % less time per step); fused_news_encoder=True selects the one-kernel news front end
-    #   instead (same numerics as "accurate", slower).  Shapes the title-level attention kernel does not cover fall back to "fast".
+    #   activation stored bf16 (~6e-3).  Shapes the title-level attention kernel does not cover fall back to "fast".
     "NRMS": dict(dataset_attributes={"news": ["title"], "record": []}, num_attention_heads=15,
-                 precision=os.environ.get("NEWSREC_PRECISION", "accurate"),
-                 fused_news_encoder=os.environ.get("NEWSREC_FUSED") == "1"),
+                 precision=os.environ.get("NEWSREC_PRECISION", "accurate")),
     "NAML": dict(dataset_attributes={"news": ["category", "subcategory", "title", "abstract"], "record": []}, **_CNN),
     "LSTUR": dict(dataset_attributes={"news": ["category", "subcategory", "title"],
                                       "record": ["user", "clicked_news_length"]},

@@ -1,4 +1,4 @@
-"""NRMS NewsEncoder: embedding gather -> dropout -> MHSA -> dropout -> additive pooling, fused on sm_100a
+"""NRMS NewsEncoder: embedding gather -> dropout -> MHSA -> dropout -> additive pooling, fused on sm_90a
 (replaces reference src/model/NRMS/news_encoder.py:10-48; same submodule / parameter names)."""
 import torch
 import torch.nn as nn

@@ -1,4 +1,4 @@
-"""NRMS UserEncoder: MHSA over the browsed-news vectors -> additive pooling, fused on sm_100a
+"""NRMS UserEncoder: MHSA over the browsed-news vectors -> additive pooling, fused on sm_90a
 (replaces reference src/model/NRMS/user_encoder.py:6-26)."""
 import torch.nn as nn
 

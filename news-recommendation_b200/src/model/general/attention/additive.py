@@ -1,4 +1,4 @@
-"""AdditiveAttention on the fused tcgen05 pooling kernel (replaces reference
+"""AdditiveAttention on the fused wgmma pooling kernel (replaces reference
 src/model/general/attention/additive.py:6-53; same constructor, parameter names and shapes)."""
 import torch
 import torch.nn as nn

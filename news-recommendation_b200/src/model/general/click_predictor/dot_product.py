@@ -1,4 +1,4 @@
-"""DotProductClickPredictor on the sm_100a dot-score kernel (replaces reference
+"""DotProductClickPredictor on the sm_90a dot-score kernel (replaces reference
 src/model/general/click_predictor/dot_product.py:4-19; same class name and call signature)."""
 import torch
 

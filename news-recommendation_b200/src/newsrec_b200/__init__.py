@@ -1,7 +1,7 @@
 """ctypes binding of the newsrec_b200 C ABI (include/newsrec_b200.h).
 
 Host glue only: PyTorch supplies device memory, streams and autograd bookkeeping; every arithmetic
-step of the hot path runs in the sm_100a kernels behind ``libnewsrec_b200.so``.  There is NO CPU or
+step of the hot path runs in the sm_90a kernels behind ``libnewsrec_b200.so``.  There is NO CPU or
 PyTorch fallback: if the library is missing or no CUDA device is present the ops raise.
 """
 from __future__ import annotations
@@ -24,7 +24,7 @@ class MhsaEncoderFwdArgs(C.Structure):
         ("wqkv_bf16", _vp), ("bqkv", _vp), ("wa_bf16", _vp), ("ba", _vp), ("qv", _vp),
         ("p_drop", _f), ("seed", _ull),
         ("X_bf16", _vp), ("QKV_bf16", _vp), ("C_bf16", _vp), ("w", _vp), ("out", _vp), ("bad_id_flag", _vp),
-        ("wqkv_heads_bf16", _vp), ("bqkv_heads", _vp), ("C_lo_bf16", _vp),
+        ("C_lo_bf16", _vp),
         ("wqkv_kcat_bf16", _vp), ("X_kcat_bf16", _vp), ("QKV_f32", _vp),
         ("V_lo_bf16", _vp),
     ]
@@ -103,7 +103,6 @@ SIGNATURES = {
     "nr_has_triage_backends": (_i, []),
     "nr_reserve_sms_for_comm": (None, [_i]),
     "nr_debug_set_gemm_timing": (None, [_vp, _i]),
-    "nr_debug_set_fused_timing": (None, [_vp]),
     "nr_profile_enable": (None, [_i]),
     "nr_profile_context": (None, [C.c_char_p]),
     "nr_profile_report": (_i, [C.c_char_p, _i]),
@@ -127,7 +126,6 @@ SIGNATURES = {
     "nr_dot_score_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "nr_mhsa_accurate_supported": (_i, [_i, _i, _i]),
     "nr_mhsa_encoder_fwd": (_i, [C.POINTER(MhsaEncoderFwdArgs), _vp]),
-    "nr_mhsa_fused_supported": (_i, [_i, _i, _i]),
     "nr_mhsa_encoder_bwd_workspace": (_ll, [_ll, _i, _i, _i]),
     "nr_mhsa_encoder_bwd": (_i, [C.POINTER(MhsaEncoderBwdArgs), _vp]),
     "nr_cnn_encoder_fwd": (_i, [C.POINTER(CnnEncoderFwdArgs), _vp]),
@@ -183,7 +181,7 @@ def check(rc: int, what: str = ""):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise NewsrecError("newsrec_b200 needs a CUDA (sm_100a) device: the hot path has no CPU fallback")
+        raise NewsrecError("newsrec_b200 needs a CUDA (sm_90a) device: the hot path has no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 

@@ -115,12 +115,13 @@ def cast_pad(src: torch.Tensor, ld: int, transpose: bool = False) -> torch.Tenso
 
 
 def precision_mode(config):
-    """"fast" | "accurate" | "fused" from a model config (config.py: precision, fused_news_encoder)."""
+    """"fast" | "accurate" from a model config (config.py: precision)."""
     if bool(getattr(config, "fused_news_encoder", False)):
-        return "fused"
+        raise NewsrecError("config.fused_news_encoder: the one-kernel news front end no longer exists; precision='accurate' "
+                           "has the same storage contract")
     mode = str(getattr(config, "precision", "fast"))
-    if mode not in ("fast", "accurate", "fused"):
-        raise NewsrecError(f"config.precision must be 'fast', 'accurate' or 'fused' (got {mode!r})")
+    if mode not in ("fast", "accurate"):
+        raise NewsrecError(f"config.precision must be 'fast' or 'accurate' (got {mode!r})")
     return mode
 
 
@@ -172,19 +173,6 @@ def mhsa_operands(cache: OperandCache, prefix, Wq, bq, Wk, bk, Wv, bv, Wa, ba, q
     return cache.get(prefix, (Wq, bq, Wk, bk, Wv, bv, Wa, ba, qv), build)
 
 
-def pack_head_blocks(Wq, bq, Wk, bk, Wv, bv, heads, ldx, rows_per_head=64):
-    """Per-head weight blocks of the fused front end: rows W_Q[h] | W_K[h] | W_V[h] | zero rows up to `rows_per_head`
-    (head h owns output features [h*d_k, (h+1)*d_k) of each projection, multihead_self.py:53-58).  Layout plumbing only."""
-    d = Wq.shape[0]
-    dk = d // heads
-    W = torch.zeros((heads, rows_per_head, d), dtype=torch.float32, device=Wq.device)
-    b = torch.zeros((heads, rows_per_head), dtype=torch.float32, device=Wq.device)
-    for i, (Wm, bm) in enumerate(((Wq, bq), (Wk, bk), (Wv, bv))):
-        W[:, i * dk:(i + 1) * dk] = Wm.float().view(heads, dk, d)
-        b[:, i * dk:(i + 1) * dk] = bm.float().view(heads, dk)
-    return cast_pad(W.view(heads * rows_per_head, d), ldx), b.view(-1).contiguous()
-
-
 def table_operand(cache: OperandCache, name, weight):
     ldx = ru8(weight.shape[1] + 1)
     return cache.get(name, (weight,), lambda w: cast_pad(w, ldx))
@@ -226,24 +214,16 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
             table = None
         n_tok = n_seq * T
         need_bwd = any(ctx.needs_input_grad)
-        # the fused front end (gather -> Q|K|V -> attention in ONE kernel, V / context as hi/lo bf16 pairs) is the PRECISE
-        # mode of the news level: 2.6e-3 instead of 7e-3 against the reference's fp32 logits, at ~3.6x the time of the
-        # unfused gather | GEMM | attention sequence (DESIGN.md section 8) -- opt-in (config.fused_news_encoder / NEWSREC_FUSED=1)
         # precision modes (config.precision, DESIGN.md section 4):
         #   "fast"      bf16 storage of every activation (Q|K|V, probabilities, context): fastest, ~6e-3 from the fp32 result
         #   "accurate"  V / probabilities / context as hi/lo bf16 pairs on the same unfused kernels + fp32-accurate user
         #               encoder: within the blueprint's 1e-3 of the fp32 oracle on bf16-rounded weights
-        #   "fused"     the one-kernel news front end (same numerics as "accurate", kept for reference; slower)
-        mode = precise if isinstance(precise, str) else ("fused" if precise else "fast")
-        if os.environ.get("NEWSREC_FUSED") == "1":
-            mode = "fused"
-        fused = ids is not None and mode == "fused" and bool(lib.nr_mhsa_fused_supported(T, d, heads))
-        accurate = ids is not None and not fused and mode in ("accurate", "fused") and bool(lib.nr_mhsa_accurate_supported(T, d, heads))
-        precise_dense = ids is None and mode in ("accurate", "fused")  # user encoder: fp32-accurate forward (abi.cu)
+        mode = precise if isinstance(precise, str) else ("accurate" if precise else "fast")
+        accurate = ids is not None and mode == "accurate" and bool(lib.nr_mhsa_accurate_supported(T, d, heads))
+        precise_dense = ids is None and mode == "accurate"  # user encoder: fp32-accurate forward (abi.cu)
         X = QKV = C_lo = V_lo = None
-        if need_bwd or not fused:  # X only exists in HBM when a backward pass (or the unfused sequence) reads it
-            X = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=dev)
-        if not fused and not precise_dense:  # the precise paths keep no bf16 Q|K|V; their backward recomputes it from X
+        X = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=dev)
+        if not precise_dense:  # the precise dense path keeps no bf16 Q|K|V; its backward recomputes it from X
             QKV = torch.empty((n_tok, ld3), dtype=torch.bfloat16, device=dev)
         Cx = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=dev)
         w = torch.empty((n_tok,), dtype=torch.float32, device=dev)
@@ -252,11 +232,6 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
         a.n_seq, a.T, a.d, a.heads, a.q, a.ldx, a.ld3 = n_seq, T, d, heads, q, ldx, ld3
         a.wqkv_bf16, a.bqkv, a.wa_bf16, a.ba, a.qv = _p(ops["wqkv"]), _p(ops["bqkv"]), _p(ops["wa"]), _p(ops["ba"]), _p(ops["qv"])
         a.p_drop, a.seed = float(p_drop), seed
-        if fused:
-            hb = cache.get(prefix + ".heads", (Wq, bq, Wk, bk, Wv, bv),
-                           lambda Wq, bq, Wk, bk, Wv, bv: pack_head_blocks(Wq, bq, Wk, bk, Wv, bv, heads, ldx))
-            C_lo = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=dev)
-            a.wqkv_heads_bf16, a.bqkv_heads, a.C_lo_bf16 = _p(hb[0]), _p(hb[1]), _p(C_lo)
         if accurate:
             C_lo = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=dev)
             V_lo = torch.empty((n_tok, sec), dtype=torch.bfloat16, device=dev)

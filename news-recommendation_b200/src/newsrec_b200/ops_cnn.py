@@ -21,7 +21,7 @@ class CnnPoolEncoderFn(torch.autograd.Function):
         dev = require_cuda()
         Fn, _, win, d = Wc.shape
         if win != 3:
-            raise NewsrecError(f"window_size={win}: the tcgen05 conv path implements the reference default window_size=3")
+            raise NewsrecError(f"window_size={win}: the wgmma conv path implements the reference default window_size=3")
         q = Wa.shape[0]
         ldx, ldf, ldq = ru8(d + 1), ru8(Fn + 1), ru16(q)
         n_seq, T = ids.shape

@@ -94,7 +94,7 @@ class _RoundHiLo(torch.autograd.Function):
 @dataclass(frozen=True)
 class Contract:
     bf16: bool = False
-    hilo: bool = False     # fused news front end (csrc/fused_fwd.cu): V and the context are hi/lo bf16 pairs
+    hilo: bool = False     # precise storage: V and the context are hi/lo bf16 pairs
     acts: bool = True      # False: ONLY parameters / embeddings are rounded to bf16, every activation and gradient stays fp32
                            # (the tolerance definition of SURVEY.md 7.3-5: "the fp32 oracle on bf16-rounded weights/embeddings")
 

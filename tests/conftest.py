@@ -1,4 +1,4 @@
-"""pytest configuration: `-m gpu` tests need a B200; everything else runs on CPU."""
+"""pytest configuration: `-m gpu` tests need an H100 (sm_90a); everything else runs on CPU."""
 import os
 import sys
 
@@ -12,7 +12,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), PKG_SRC):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_100a); run on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

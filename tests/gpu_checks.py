@@ -84,7 +84,7 @@ def _rand_bf16(shape, seed, scale=1.0):
 
 
 def check_linear(M=300, N=900, K=300, taps=1, seg=0, relu=0, out_bf16=1):
-    """nr_linear (tcgen05 gemm_nt + store epilogue) against an fp64 matmul of the same bf16 operands."""
+    """nr_linear (wgmma gemm_nt + store epilogue) against an fp64 matmul of the same bf16 operands."""
     lib = load_library()
     lda, ldw = ru8(K + 1), ru8(K + 1)
     if taps == 1:
@@ -261,9 +261,9 @@ def check_gru(B=37, S=50, D=900, Hd=900, seed=3):
 def nrms_model_and_params(V, seed, heads=15, dropout=0.2, fused=False):
     import config as cfgmod
     from model.NRMS import NRMS
-    # fused: False = fast mode, True = the one-kernel front end, "accurate" = hi/lo pairs on the unfused kernels
+    # fused: False = fast mode, "accurate" = hi/lo pairs (V / probabilities / context) on the unfused kernels
     cfg = type("Cfg", (cfgmod.NRMSConfig,), dict(num_words=V, num_attention_heads=heads, dropout_probability=dropout,
-                                                 fused_news_encoder=fused is True, precision="accurate" if fused == "accurate" else "fast"))
+                                                 precision="accurate" if fused == "accurate" else "fast"))
     sd = O.det_state_dict(O.nrms_shapes(V), seed)
     model = NRMS(cfg)
     model.load_state_dict(sd)
@@ -495,7 +495,7 @@ def check_nrms_full_size_properties(B=512):
 
 # ------------------------------------------------------------------------------------------------
 def check_backend_agreement(M=8800, N=900, K=300):
-    """tcgen05 accumulators vs the SIMT triage backend on identical operands (fp32 output): locates
+    """wgmma accumulators vs the SIMT triage backend on identical operands (fp32 output): locates
     pipeline bugs (which tile / row / column disagrees) that bf16 output rounding would hide."""
     lib = load_library()
     lda = ldw = ru8(K + 1)
@@ -530,11 +530,10 @@ def check_backend_agreement(M=8800, N=900, K=300):
     return res
 
 
-def _encoder_fwd_raw(ids, dense, sd, prefix, heads, V, fused=False, p_drop=0.0, seed=0):
-    """Direct nr_mhsa_encoder_fwd call returning every intermediate buffer (for differential triage).
-    fused=True passes the head-packed operands + the lo plane, i.e. selects the one-kernel front end."""
+def _encoder_fwd_raw(ids, dense, sd, prefix, heads, V, p_drop=0.0, seed=0):
+    """Direct nr_mhsa_encoder_fwd call returning every intermediate buffer (for differential triage)."""
     from newsrec_b200 import MhsaEncoderFwdArgs
-    from newsrec_b200.ops import pack_head_blocks, qkv_pitches, stack_qkv
+    from newsrec_b200.ops import qkv_pitches, stack_qkv
     lib = load_library()
     d, q = 300, 200
     ldx, ld3 = ru8(d + 1), qkv_pitches(d)[1]
@@ -555,7 +554,7 @@ def _encoder_fwd_raw(ids, dense, sd, prefix, heads, V, fused=False, p_drop=0.0, 
         a.dense_s_seq, a.dense_s_tok, a.dense_s_col = dense.stride()
     n_tok = n_seq * T
     bufs = dict(X=torch.zeros((n_tok, ldx), dtype=torch.bfloat16, device=DEV),
-                QKV=None if fused else torch.zeros((n_tok, ld3), dtype=torch.bfloat16, device=DEV),
+                QKV=torch.zeros((n_tok, ld3), dtype=torch.bfloat16, device=DEV),
                 C=torch.zeros((n_tok, ldx), dtype=torch.bfloat16, device=DEV), w=torch.zeros((n_tok,), device=DEV),
                 out=torch.zeros((n_seq, d), device=DEV))
     a.n_seq, a.T, a.d, a.heads, a.q, a.ldx, a.ld3 = n_seq, T, d, heads, q, ldx, ld3
@@ -563,10 +562,6 @@ def _encoder_fwd_raw(ids, dense, sd, prefix, heads, V, fused=False, p_drop=0.0, 
     a.p_drop, a.seed = float(p_drop), int(seed)
     a.X_bf16, a.QKV_bf16, a.C_bf16, a.w, a.out = _p(bufs["X"]), _p(bufs["QKV"]), _p(bufs["C"]), _p(bufs["w"]), _p(bufs["out"])
     a.bad_id_flag = _p(flag)
-    if fused:
-        hw, hb = pack_head_blocks(*[g(f"multihead_self_attention.W_{n}.{k}") for n in "QKV" for k in ("weight", "bias")], heads, ldx)
-        bufs["C_lo"] = torch.zeros((n_tok, ldx), dtype=torch.bfloat16, device=DEV)
-        a.wqkv_heads_bf16, a.bqkv_heads, a.C_lo_bf16 = _p(hw), _p(hb), _p(bufs["C_lo"])
     check(lib.nr_mhsa_encoder_fwd(C.byref(a), _stream()), "nr_mhsa_encoder_fwd")
     torch.cuda.synchronize()
     out = {k: v.float().cpu() for k, v in bufs.items() if v is not None}
@@ -574,42 +569,8 @@ def _encoder_fwd_raw(ids, dense, sd, prefix, heads, V, fused=False, p_drop=0.0, 
     return out
 
 
-def check_fused_front(n_seq=13, V=97, p_drop=0.0, seed=0x1234567, heads=15):
-    """The fused front end (csrc/fused_fwd.cu) against (1) the unfused kernel sequence on identical inputs: the gathered
-    rows X bit for bit (same table rows, same dropout masks), Q|K|V to bf16 rounding flips; (2) the oracle: the context
-    hi + lo planes against an fp64 attention over the kernel's own X with the fused storage contract (Q, K, P bf16; V and the
-    context hi/lo pairs), and the pooled news vector."""
-    T, d = 20, 300
-    sd = O.det_state_dict(O.nrms_shapes(V), 17)
-    ids = O.synth_titles(n_seq, T, V, 91).to(DEV)
-    un = _encoder_fwd_raw(ids, None, sd, "news_encoder", heads, V, fused=False, p_drop=p_drop, seed=seed)
-    fu = _encoder_fwd_raw(ids, None, sd, "news_encoder", heads, V, fused=True, p_drop=p_drop, seed=seed)
-    res = {"x_bit_exact": bool(torch.equal(un["X"], fu["X"])), "bad_flag": fu["bad_flag"]}
-    # oracle context from the kernel's own gathered rows (dropout already applied there); context mask injected
-    p = {k: v.double() for k, v in sd.items()}
-    x = fu["X"][:, :d].double().view(n_seq, T, d)
-    cmask = None
-    if p_drop > 0:
-        cmask = O.dropout_mask(seed ^ 0x5bd1e995, p_drop, n_seq * T, d, ru8(d + 1)).double().view(n_seq, T, d)
-        xmask = O.dropout_mask(seed, p_drop, n_seq * T, d, ru8(d + 1))
-        tab = bf16r(sd["news_encoder.word_embedding.weight"])[ids.cpu().reshape(-1)]
-        res["x_vs_masked_oracle_exact"] = bool(torch.equal(fu["X"][:, :d], bf16r(tab * xmask)))
-    with torch.no_grad():
-        ctx = O.multihead_self_attention(x, p, "news_encoder.multihead_self_attention", heads, O.BF16_FUSED, cmask).view(n_seq * T, d)
-        ctx_exact = O.multihead_self_attention(x, p, "news_encoder.multihead_self_attention", heads, O.EXACT, cmask).view(n_seq * T, d)
-        pooled = O.additive_attention(ctx.view(n_seq, T, d), p, "news_encoder.additive_attention", O.BF16_FUSED)
-    c = fu["C"][:, :d].double() + fu["C_lo"][:, :d].double()
-    res["ctx_vs_oracle_fused_contract"] = relerr(c, ctx)
-    res["ctx_vs_fp64_attention"] = relerr(c, ctx_exact)
-    res["ctx_hi_ones_col"] = bool((fu["C"][:, d] == 1).all() and (fu["C"][:, d + 1:] == 0).all())
-    res["out_vs_oracle"] = relerr(fu["out"], pooled)
-    res["out_fused_vs_unfused"] = relerr(fu["out"], un["out"])
-    res["w_sums_to_one"] = float((fu["w"].view(n_seq, T).sum(1) - 1).abs().max())
-    return res
-
-
 def check_encoder_backend_diff(B=8, V=500, seed=5):
-    """Every intermediate of the news and user encoders, tcgen05 vs SIMT triage backend, same inputs."""
+    """Every intermediate of the news and user encoders, wgmma vs SIMT triage backend, same inputs."""
     lib = load_library()
     cand_t, clicked_t, _ = O.synth_batch(B, 5, 50, 20, V, seed * 100)
     sd = O.det_state_dict(O.nrms_shapes(V), seed)
@@ -655,7 +616,6 @@ def build_model(case, V=120, ncat=15, nusers=40, H=6, dropout=0.2, fused=False):
     name = {"nrms": "NRMS", "naml": "NAML", "naml_f400": "NAML", "tanr": "TANR", "lstur_ini": "LSTUR", "lstur_con": "LSTUR"}[case]
     over = dict(num_words=V, num_categories=ncat, num_users=nusers, num_clicked_news_a_user=H, dropout_probability=dropout)
     if name == "NRMS":
-        over["fused_news_encoder"] = fused is True
         over["precision"] = "accurate" if fused == "accurate" else "fast"
     if name == "LSTUR":
         over["precision"] = "accurate" if fused else "fast"

@@ -3,7 +3,7 @@ independent single-GPU backward passes give when averaged.
 
 The overlapped path is easy to get wrong silently: the backward records a CUDA event behind the embedding-gradient scatter
 GEMM, `FlatGradients.all_reduce_mean` sends that slice from a side stream as soon as the event fires -- while the
-weight-gradient GEMMs still run on 116 of the 148 SMs -- and reduces the rest afterwards (src/newsrec_b200/ddp.py,
+weight-gradient GEMMs still run on 100 of the 132 SMs -- and reduces the rest afterwards (src/newsrec_b200/ddp.py,
 csrc/abi.cu nr_mhsa_encoder_bwd).  An all-reduce that started before the scatter had finished, or a weight-gradient GEMM
 that raced with it, would corrupt gradients without any error.  Needs two GPUs (skipped otherwise)."""
 import os

@@ -1,4 +1,4 @@
-"""Integration on the B200: every drop-in model driven through the call sequence of the reference's trainer and evaluator.
+"""Integration on the H100: every drop-in model driven through the call sequence of the reference's trainer and evaluator.
 
 The reference's drivers cannot travel to the GPU box (and must not be copied), so this test restates ONLY their call
 sequence -- each step cites the line it mirrors -- around the drop-in packages:

@@ -1,4 +1,4 @@
-"""Kernel-level parity on the B200 (every call goes through the C ABI).  Tolerances are written here:
+"""Kernel-level parity on the H100 (every call goes through the C ABI).  Tolerances are written here:
   * integer / byte work (gather, padding layout, operand packing): bit exact;
   * a kernel fed bf16 operands, compared with an fp64 evaluation of the SAME bf16 operands:
       fp32 outputs <= 1e-5 norm-wise, bf16 outputs <= 3e-3 (one bf16 rounding of the result);
@@ -92,24 +92,14 @@ def test_dot_product_click_predictor():
     assert r["fwd_rel"] < 1e-6 and r["dc_rel"] < 1e-6 and r["du_rel"] < 1e-6, r
 
 
-@pytest.mark.parametrize("kw", [dict(n_seq=13), dict(n_seq=6), dict(n_seq=1), dict(n_seq=1000, V=5000),
-                                dict(n_seq=13, p_drop=0.2), dict(n_seq=777, V=3000, p_drop=0.2, seed=0xDEADBEEFCAFE)])
-def test_fused_news_front_end(kw):
-    """One-kernel gather -> Q|K|V -> attention: X bit exact against the unfused gather (same masks), context against the
-    oracle under the fused storage contract <= 1e-3 (measured ~1e-4: bf16 rounding flips of Q / K / P), pooled vector too."""
-    r = G.check_fused_front(**kw)
-    assert r["x_bit_exact"] and r["bad_flag"] == 0 and r["ctx_hi_ones_col"], r
-    assert r.get("x_vs_masked_oracle_exact", True), r
-    assert r["ctx_vs_oracle_fused_contract"] < 1e-3, r
-    assert r["out_vs_oracle"] < 1e-3 and r["w_sums_to_one"] < 1e-5, r
-
-
 @pytest.mark.parametrize("kw", [dict(B=37, S=50), dict(B=300, S=50), dict(B=5, S=7, D=600, Hd=900), dict(B=9, S=12, D=900, Hd=450),
                                 dict(B=700, S=6)])
 def test_gru_last_hidden_history_50_mixed_lengths(kw):
     """BASELINE.json configs[3] shapes (history 50, D = Hd = 900): the persistent recurrence kernel (one cooperative launch
     for all steps) and, for shapes it does not cover (B = 700: more CTAs than SMs), the per-step sequence."""
     r = G.check_gru(**kw)
+    # the persistent kernel covers Hd = 900 at B <= 512; B = 700 needs more CTAs than SMs, Hd = 450 is not a multiple of 4
+    assert r["persistent"] == (kw.get("B", 37) <= 512 and kw.get("Hd", 900) % 4 == 0), r
     assert r["fwd_rel"] < 1e-3, r
     assert r["dx_rel"] < 5e-3 and r["dh0_rel"] < 5e-3 and r["dweight_ih_l0"] < 5e-3 and r["dweight_hh_l0"] < 5e-3, r
 

@@ -129,14 +129,15 @@ def test_qkv_sections_pad_to_a_16_byte_phase():
 
 def test_precision_knob_defaults_and_validation():
     """config.precision: "accurate" by default for NRMS and LSTUR (the blueprint's 1e-3 tolerance), "fast" on request;
-    fused_news_encoder selects the one-kernel front end; anything else is rejected."""
+    the removed fused_news_encoder knob and anything else are rejected."""
     import config as cfgmod
     from newsrec_b200 import NewsrecError
     from newsrec_b200.ops import precision_mode
     assert precision_mode(cfgmod.NRMSConfig) == os.environ.get("NEWSREC_PRECISION", "accurate")
     assert getattr(cfgmod.LSTURConfig, "precision") == os.environ.get("NEWSREC_PRECISION", "accurate")
     assert precision_mode(type("C", (), {"precision": "fast"})) == "fast"
-    assert precision_mode(type("C", (), {"precision": "fast", "fused_news_encoder": True})) == "fused"
+    with pytest.raises(NewsrecError):
+        precision_mode(type("C", (), {"precision": "fast", "fused_news_encoder": True}))
     assert precision_mode(type("C", (), {})) == "fast"  # a config without the knob (NAML / TANR): plain bf16 storage
     with pytest.raises(NewsrecError):
         precision_mode(type("C", (), {"precision": "exact"}))

@@ -1,5 +1,5 @@
 """GPU triage ladder: runs every kernel-vs-oracle check in its own subprocess (a device trap in one
-check cannot poison the next), first on the tcgen05 product path and -- for triage only -- on the debug
+check cannot poison the next), first on the wgmma product path and -- for triage only -- on the debug
 SIMT GEMM backend (NEWSREC_DEBUG_SIMT_GEMM=1, same epilogue functors).  Writes gpurun_out/ladder.json.
 
     python tools/gpu_ladder.py            # everything
@@ -87,7 +87,7 @@ def main():
     names = [n for n in CHECKS if not a.only or n in a.only.split(",")]
     results = {}
     os.makedirs(os.path.dirname(a.out), exist_ok=True)
-    for backend in (["tcgen05"] if a.skip_simt else ["tcgen05", "simt_debug"]):
+    for backend in (["wgmma"] if a.skip_simt else ["wgmma", "simt_debug"]):
         for n in names:
             if backend == "simt_debug" and n in ("linear_big", "nrms_full_size", "gemm_tn_long"):
                 continue
