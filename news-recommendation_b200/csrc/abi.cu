@@ -192,7 +192,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_bf16, a->ldx, st));
         NR_PROPAGATE(rows_to_bf16_hilo(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_kcat_bf16,
                                        a->ldx, st));
-        NR_PROPAGATE(gemm_store(a->X_kcat_bf16, M, 2 * a->ldx, a->wqkv_kcat_bf16, 3 * qkv_section(a->d), 2 * a->ldx, 2 * a->ldx, 1, 0, 128,
+        NR_PROPAGATE(gemm_store(a->X_kcat_bf16, M, 2 * a->ldx, a->wqkv_kcat_bf16, 3 * qkv_section(a->d), 2 * a->ldx, 2 * a->ldx, 1, 0, kGemmTileRows,
                                 a->bqkv, 0, a->QKV_f32, 3 * qkv_section(a->d), 0, kIdentity, 0, kNoDrop, -1, 0, st));
         NR_PROPAGATE(mhsa_f32_fwd(a->QKV_f32, 3 * qkv_section(a->d), qkv_section(a->d), a->n_seq, a->T, a->heads, a->d / a->heads, a->C_bf16, a->C_lo_bf16, a->ldx, st));
         NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
@@ -210,7 +210,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
                    "nr_mhsa_encoder_fwd: the accurate variant needs the title-level attention kernel (T=20, d_k=20, <=15 heads); see nr_mhsa_accurate_supported");
         NR_PROPAGATE(gather_rows(a->ids, M, a->T, a->table_bf16, a->V, a->d, a->ldx, a->X_bf16, a->ldx, 0,
                                  DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
-        NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, 128, a->bqkv, 0, a->QKV_bf16, a->ld3, 1,
+        NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, kGemmTileRows, a->bqkv, 0, a->QKV_bf16, a->ld3, 1,
                                 kIdentity, 0, kNoDrop, -1, 0, st, a->V_lo_bf16, sec, 2 * sec));
         const DropoutCfg cd = {a->p_drop, a->seed ^ 0x5bd1e995u};
         {
@@ -230,7 +230,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
                                   a->X_bf16, a->ldx, st));
     }
     // Q|K|V = X . Wqkv^T + b   (multihead_self.py:53-58)
-    NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * qkv_section(a->d), a->ldx, a->d, 1, 0, 128, a->bqkv, 0,
+    NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * qkv_section(a->d), a->ldx, a->d, 1, 0, kGemmTileRows, a->bqkv, 0,
                             a->QKV_bf16, a->ld3, 1, kIdentity, 0, kNoDrop, -1, 0, st));
     // per-head attention (multihead_self.py:15-23), dropout on the context only in the news encoder
     const DropoutCfg cdrop = {a->ids != nullptr ? a->p_drop : 0.f, a->seed ^ 0x5bd1e995u};
@@ -281,7 +281,7 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     prof_context(a->ids != nullptr ? "news.bwd" : "user.bwd");
     const void* QKV = a->QKV_bf16;
     if (QKV == nullptr) {  // the precise dense forward keeps no bf16 Q|K|V: recompute it from the saved rows (multihead_self.py:53-58)
-        NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, 128, a->bqkv, 0, ws, a->ld3, 1,
+        NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, kGemmTileRows, a->bqkv, 0, ws, a->ld3, 1,
                                 kIdentity, 0, kNoDrop, -1, 0, st));
         QKV = ws;
     }
@@ -299,11 +299,11 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     //     ones column of X) ---
     if (a->ids != nullptr) {
         NR_REQUIRE(a->V >= 1, "nr_mhsa_encoder_bwd: V=%d", a->V);
-        NR_PROPAGATE(gemm_scatter_emb(dQKV, M, a->ld3, a->wqkvT_bf16, a->d, a->ld3, 3 * sec, 1, 0, 128, a->ids, a->demb, a->V, a->d,
+        NR_PROPAGATE(gemm_scatter_emb(dQKV, M, a->ld3, a->wqkvT_bf16, a->d, a->ld3, 3 * sec, 1, 0, kGemmTileRows, a->ids, a->demb, a->V, a->d,
                                       kIdentity, DropoutCfg{a->p_drop, a->seed}, a->ldx, st));
         if (a->emb_grad_ready_event != nullptr) NR_CHECK_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(a->emb_grad_ready_event), st));
     } else {
-        NR_PROPAGATE(gemm_store(dQKV, M, a->ld3, a->wqkvT_bf16, a->d, a->ld3, 3 * sec, 1, 0, 128, nullptr, 0, a->ddense, a->d,
+        NR_PROPAGATE(gemm_store(dQKV, M, a->ld3, a->wqkvT_bf16, a->d, a->ld3, 3 * sec, 1, 0, kGemmTileRows, nullptr, 0, a->ddense, a->d,
                                 0, kIdentity, 0, kNoDrop, -1, 0, st));
     }
     // both weight-gradient GEMMs run AFTER the embedding gradient is complete: together they are the window (~0.4 ms) under which

@@ -45,7 +45,7 @@ int nr_cnn_encoder_fwd(const nr_cnn_encoder_fwd_args* a, void* stream) {
     NR_PROPAGATE(gather_rows(a->ids, n_tok, T, a->table_bf16, a->V, a->d, a->ldx, a->Xp_bf16, a->ldx, 1,
                              DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
     const RowMapCfg to_compact = {Tp, 1, T, T, 0};
-    NR_PROPAGATE(gemm_store(a->Xp_bf16, Mp, a->ldx, a->wconv_bf16, a->F, a->ldx, a->d, 3, a->F, (128 / Tp) * Tp, a->bconv, 1,
+    NR_PROPAGATE(gemm_store(a->Xp_bf16, Mp, a->ldx, a->wconv_bf16, a->F, a->ldx, a->d, 3, a->F, kGemmTileRows, a->bconv, 1,
                             a->Y_bf16, a->ldf, 1, to_compact, 0, DropoutCfg{a->p_drop, a->seed ^ 0x5bd1e995u}, a->F, a->ldf, st,
                             a->Y_lo_bf16, a->ldf, 0));
     NR_PROPAGATE(gemm_additive_pool(a->Y_bf16, static_cast<int>(n_tok), a->ldf, a->F, a->wa_bf16, a->q, a->ldf, a->ba, a->qv, T,
@@ -93,7 +93,7 @@ int nr_cnn_encoder_bwd(const nr_cnn_encoder_bwd_args* a, void* stream) {
                                         a->dWconv_ext + static_cast<size_t>(s) * a->F * a->ldx, a->ldx, st));
     // embedding gradient: dX[r] = sum_s' W_(2-s')^T dY[r + s' - 1], scattered to the token ids
     const RowMapCfg to_compact = {Tp, 1, T, T, 0};
-    NR_PROPAGATE(gemm_scatter_emb(dYp, Mp, a->ldf, a->wconvT_bf16, a->d, a->ldf, a->F, 3, a->d, (128 / Tp) * Tp, a->ids, a->demb,
+    NR_PROPAGATE(gemm_scatter_emb(dYp, Mp, a->ldf, a->wconvT_bf16, a->d, a->ldf, a->F, 3, a->d, kGemmTileRows, a->ids, a->demb,
                                   a->V, a->d, to_compact, DropoutCfg{a->p_drop, a->seed}, a->ldx, st));
     return 0;
 }
@@ -106,7 +106,7 @@ int nr_linear_rows_fwd(const float* x, long long n, int K, long long s_row, long
     if (n == 0) return 0;
     prof_context("linear.fwd");
     NR_PROPAGATE(rows_to_bf16(x, n, 1, K, s_row, 0, s_col, X_bf16, ldx, S(stream)));
-    return gemm_store(X_bf16, static_cast<int>(n), ldx, W_bf16, N, ldw, K, 1, 0, 128, bias, relu, out, ld_out, 0, kIdentity, 0, kNoDrop,
+    return gemm_store(X_bf16, static_cast<int>(n), ldx, W_bf16, N, ldw, K, 1, 0, kGemmTileRows, bias, relu, out, ld_out, 0, kIdentity, 0, kNoDrop,
                       -1, 0, S(stream));
 }
 
@@ -126,7 +126,7 @@ int nr_linear_rows_bwd(const float* dy, const float* relu_out, long long n, int 
     }
     if (dx != nullptr) {
         NR_REQUIRE(WT_bf16 && ld_dx % 4 == 0, "nr_linear_rows_bwd: transposed weight / dx pitch");
-        NR_PROPAGATE(gemm_store(dY_bf16, static_cast<int>(n), ldn, WT_bf16, K, ldwT, N, 1, 0, 128, nullptr, 0, dx, ld_dx, 0, kIdentity, 0,
+        NR_PROPAGATE(gemm_store(dY_bf16, static_cast<int>(n), ldn, WT_bf16, K, ldwT, N, 1, 0, kGemmTileRows, nullptr, 0, dx, ld_dx, 0, kIdentity, 0,
                                 kNoDrop, -1, 0, S(stream)));
     }
     return 0;
@@ -151,7 +151,7 @@ int nr_element_encoder_fwd(const long long* ids, long long n, const void* table_
     if (n == 0) return 0;
     prof_context("element.fwd");
     NR_PROPAGATE(gather_rows(ids, n, 1, table_bf16, V, E, lde, E_bf16, lde, 0, kNoDrop, bad_id_flag, S(stream)));
-    return gemm_store(E_bf16, static_cast<int>(n), lde, W_bf16, F, lde, E, 1, 0, 128, bias, 1, out, F, 0, kIdentity, 0, kNoDrop, -1, 0,
+    return gemm_store(E_bf16, static_cast<int>(n), lde, W_bf16, F, lde, E, 1, 0, kGemmTileRows, bias, 1, out, F, 0, kIdentity, 0, kNoDrop, -1, 0,
                       S(stream));
 }
 int nr_element_encoder_bwd(const long long* ids, long long n, const float* dout, const float* out, int F, void* dY_bf16, int ldf,
@@ -163,7 +163,7 @@ int nr_element_encoder_bwd(const long long* ids, long long n, const float* dout,
     NR_PROPAGATE(relu_bwd_to_bf16(dout, out, n, F, F, dY_bf16, ldf, S(stream)));
     NR_PROPAGATE(gemm_tn_accumulate(dY_bf16, static_cast<int>(n), F, ldf, E_bf16, static_cast<int>(n), E + 1, lde, 0, E + 1, 0, dW_ext,
                                     lde, S(stream)));
-    return gemm_scatter_emb(dY_bf16, static_cast<int>(n), ldf, WT_bf16, E, ldf, F, 1, 0, 128, ids, dtable, V, E, kIdentity, kNoDrop, lde,
+    return gemm_scatter_emb(dY_bf16, static_cast<int>(n), ldf, WT_bf16, E, ldf, F, 1, 0, kGemmTileRows, ids, dtable, V, E, kIdentity, kNoDrop, lde,
                             S(stream));
 }
 

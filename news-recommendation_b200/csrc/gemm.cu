@@ -15,6 +15,7 @@
 
 namespace nr {
 
+static_assert(kGemmTileRows == kTileM, "nr_ops.h and nr_gemm.cuh disagree on the gemm_nt tile height");
 int read_gru_device_error(int* out4);
 int g_launches = 0;
 
@@ -257,11 +258,12 @@ int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B,
         p.n_box = round_up(std::min(p.n_stride, N), 32);
         if (p.n_box > 256 || (max_n_stride > 0 && p.n_stride > max_n_stride)) continue;
         bbytes = static_cast<long>(taps) * p.k_chunks * p.n_box * 128;
-        if (bbytes + 3L * kAStageBytes + fixed <= kSmemLimit) break;
+        // a ring of 6 stages (48 KB) holds more than one tile of K <= 320 ahead of the MMAs
+        if (bbytes + 6L * kAStageBytes + fixed <= kSmemLimit) break;
         // epilogues that reduce over the whole output row need ONE slice, and slices of <= 64 columns re-read A too often:
         // accept a shallower A ring, or else stream the weight boxes with the A tiles instead of keeping them resident
         if (slices == max_slices || p.n_box <= 64) {
-            if (bbytes + 2L * kAStageBytes + fixed > kSmemLimit) {
+            if (bbytes + 4L * kAStageBytes + fixed > kSmemLimit) {
                 p.b_stream = 1;
                 bbytes = 0;
             }
@@ -273,7 +275,7 @@ int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B,
     p.stages = static_cast<int>(std::min<long>(kMaxStages, (kSmemLimit - fixed - bbytes) / p.stage_bytes));
     NR_REQUIRE(p.stages >= 2, "plan_gemm_nt: only %d pipeline stages fit", p.stages);
     plan->smem = static_cast<size_t>(bbytes) + static_cast<size_t>(p.stages) * p.stage_bytes + fixed;
-    // a group = n_slices CTAs working on the same 128-row tiles
+    // a group = n_slices CTAs working on the same 64-row tiles
     const int groups = std::max(1, std::min(sms / p.n_slices, p.num_m_tiles));
     plan->grid = groups * p.n_slices;
     if (p.num_m_tiles == 0) return 0;
@@ -291,7 +293,7 @@ __global__ void gemm_nt_simt_acc_kernel(const __nv_bfloat16* A, int lda, const _
     const int tile = blockIdx.y;
     if (n >= p.dbg_ld) return;
     const int shift = p.taps / 2;
-    for (int r = 0; r < 128; ++r) {
+    for (int r = 0; r < kTileM; ++r) {
         float acc = 0.f;
         if (n < p.N) {
             for (int s = 0; s < p.taps; ++s) {
@@ -302,7 +304,7 @@ __global__ void gemm_nt_simt_acc_kernel(const __nv_bfloat16* A, int lda, const _
                 for (int k = 0; k < p.K; ++k) acc = fmaf(__bfloat162float(a[k]), __bfloat162float(b[k]), acc);
             }
         }
-        p.dbg_acc[(static_cast<size_t>(tile) * 128 + r) * p.dbg_ld + n] = acc;
+        p.dbg_acc[(static_cast<size_t>(tile) * kTileM + r) * p.dbg_ld + n] = acc;
     }
 }
 
@@ -529,6 +531,7 @@ int gemm_store(const void* A, int M, int lda, const void* W, int N, int ldw, int
                int zero_pad_rows, DropoutCfg drop, int ones_col, int ones_zero_upto, cudaStream_t stream, void* lo_out, int ld_lo,
                int lo_col0, int accumulate) {
     if (M == 0) return 0;
+    rows_per_tile = std::min(rows_per_tile, kTileM);  // every row is owned by exactly one tile: whole tiles are fine
     GemmNTPlan plan;
     NR_PROPAGATE(plan_gemm_nt(&plan, A, M, lda, W, N, ldw, K, taps, w_tap_rows, rows_per_tile, num_sms(), 0, EpiStore::kScratchBytes, 0));
     NR_REQUIRE(out_bf16 ? (ld_out % 8 == 0) : (ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", ld_out);
@@ -663,6 +666,7 @@ int gemm_scatter_emb(const void* A, int M, int lda, const void* W, int N, int ld
                      int drop_ld, cudaStream_t stream) {
     if (M == 0) return 0;
     NR_REQUIRE(N == D && D % 4 == 0 && V >= 1, "scatter_emb: N=%d D=%d V=%d", N, D, V);
+    rows_per_tile = std::min(rows_per_tile, kTileM);
     GemmNTPlan plan;
     NR_PROPAGATE(plan_gemm_nt(&plan, A, M, lda, W, N, ldw, K, taps, w_tap_rows, rows_per_tile, num_sms(), 0,
                               EpiScatter::kScratchBytes, 0));

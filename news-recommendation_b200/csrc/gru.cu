@@ -131,13 +131,13 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
     prof_context("gru.fwd");
     // gi = X Wih^T + bih over all (user, step) rows
     NR_PROPAGATE(rows_to_bf16(a->x, B, S, D, a->x_s_b, a->x_s_t, a->x_s_c, a->xb, ldd, st));
-    NR_PROPAGATE(gemm_store(a->xb, B * S, ldd, a->wih_bf16, 3 * Hd, ldd, D, 1, 0, 128, a->bih, 0, a->gi, ldg, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+    NR_PROPAGATE(gemm_store(a->xb, B * S, ldd, a->wih_bf16, 3 * Hd, ldd, D, 1, 0, kGemmTileRows, a->bih, 0, a->gi, ldg, 0, kIdentity, 0, kNoDrop, -1, 0, st));
     if (a->x_lo_bf16 != nullptr) {
         // accurate mode: the news vectors enter as a hi/lo bf16 pair, gi = x_hi . W_ih^T + b + x_lo . W_ih^T.  Two passes over the
         // SAME resident weights with fp32 accumulation into gi: a K-concatenated single pass doubles K, which shrinks the weight-
         // stationary slices to N = 80 and costs 0.86 ms instead of 2 x 0.23
         NR_PROPAGATE(rows_to_bf16_lo(a->x, B, S, D, a->x_s_b, a->x_s_t, a->x_s_c, a->x_lo_bf16, ldd, st));
-        NR_PROPAGATE(gemm_store(a->x_lo_bf16, B * S, ldd, a->wih_bf16, 3 * Hd, ldd, D, 1, 0, 128, nullptr, 0, a->gi, ldg, 0, kIdentity, 0, kNoDrop,
+        NR_PROPAGATE(gemm_store(a->x_lo_bf16, B * S, ldd, a->wih_bf16, 3 * Hd, ldd, D, 1, 0, kGemmTileRows, nullptr, 0, a->gi, ldg, 0, kIdentity, 0, kNoDrop,
                                 -1, 0, st, nullptr, 0, 0, 1));
     }
     // h_0
@@ -153,7 +153,7 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
         const void* hb_t = static_cast<const __nv_bfloat16*>(a->hb) + static_cast<size_t>(t) * B * ldh;
         __nv_bfloat16* hb_n = static_cast<__nv_bfloat16*>(a->hb) + static_cast<size_t>(t + 1) * B * ldh;
         float* h_n = a->hs + static_cast<size_t>(t + 1) * BH;
-        NR_PROPAGATE(gemm_store(hb_t, B, ldh, a->whh_bf16, 3 * Hd, ldh, Hd, 1, 0, 128, a->bhh, 0, gh_t, ldg, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+        NR_PROPAGATE(gemm_store(hb_t, B, ldh, a->whh_bf16, 3 * Hd, ldh, Hd, 1, 0, kGemmTileRows, a->bhh, 0, gh_t, ldg, 0, kIdentity, 0, kNoDrop, -1, 0, st));
         NR_CHECK_CUDA(cudaMemcpyAsync(h_n, a->hs + static_cast<size_t>(t) * BH, sizeof(float) * BH, cudaMemcpyDeviceToDevice, st));
         {
             ProfScope ps("gru_gate_fwd", B, Hd, t, st);
@@ -213,7 +213,7 @@ int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream) {
         }
         NR_CHECK_CUDA(cudaGetLastError());
         // recurrent path: dh_{t-1} += dgh_t . Whh
-        NR_PROPAGATE(gemm_store(dgh_t, B, ldb, a->whhT_bf16, Hd, ldb, 3 * Hd, 1, 0, 128, nullptr, 0, dh_rec, P, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+        NR_PROPAGATE(gemm_store(dgh_t, B, ldb, a->whhT_bf16, Hd, ldb, 3 * Hd, 1, 0, kGemmTileRows, nullptr, 0, dh_rec, P, 0, kIdentity, 0, kNoDrop, -1, 0, st));
         dha = dh_direct;
         dhb = dh_rec;
         pa = P;
@@ -230,7 +230,7 @@ int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream) {
         NR_PROPAGATE(gemm_tn_accumulate(dgi, B * S, 3 * Hd, ldb, a->xb, B * S, D + 1, ldd, c0, nb, 0, a->dWih_ext + c0, ldd, st));
     }
     // input gradient
-    NR_PROPAGATE(gemm_store(dgi, B * S, ldb, a->wihT_bf16, D, ldb, 3 * Hd, 1, 0, 128, nullptr, 0, a->dx, D, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+    NR_PROPAGATE(gemm_store(dgi, B * S, ldb, a->wihT_bf16, D, ldb, 3 * Hd, 1, 0, kGemmTileRows, nullptr, 0, a->dx, D, 0, kIdentity, 0, kNoDrop, -1, 0, st));
     return 0;
 }
 

@@ -1,10 +1,12 @@
-// Fused epilogue functors for gemm_nt.  256 epilogue threads: thread (quarter, lane) owns accumulator row
-// r = 32*quarter + lane and the two warps of a quarter ("halves", one per warpgroup) split the row's 32-column chunks
-// [ch0, ch1).  Contract for every functor:
-//   * the accumulator is read through epi_chunks() (nr_gemm.cuh): one load per chunk of the thread's range (collective
-//     over the thread's warpgroup, the range is warpgroup-uniform), acc.release() exactly once per tile
-//   * init()/finish() bracket the CTA's whole tile loop (all 256 epilogue threads call them)
-//   * kScratchBytes of shared memory belong to the functor (the planner sizes the A ring around it)
+// Fused epilogue functors for gemm_nt.  A tile (64 rows) belongs to one consumer warpgroup, 128 threads: thread t of the
+// warpgroup owns accumulator row r = 32*((t>>5)&1) + lane and column half t>>6; the two halves split the slice's 32-column
+// chunks as epi_chunk_range does ([ch0, ch1), warp-uniform).  Contract for every functor:
+//   * the accumulator is read through epi_chunks() (nr_gemm.cuh): c.rounds loads per tile, collective over the warpgroup,
+//     acc.release() exactly once per tile
+//   * operator() synchronises only its own warpgroup (epi_bar_sync(c.wg)); the other warpgroup is issuing wgmmas meanwhile
+//   * init()/finish() bracket the CTA's whole tile loop (all 256 consumer threads call them; consumers_bar_sync())
+//   * kScratchBytes of shared memory belong to the functor (the planner sizes the A ring around it); per-tile state is
+//     kept per warpgroup
 //   * per-slice vectors (bias, query vector, dOut rows) are staged in shared memory: with ~220 KB of smem carved out
 //     the L1 holds next to nothing and per-element global loads made the epilogue 10x the MMA time.
 //     Anything that must come from global memory per tile is fetched with many loads in flight or prefetched one
@@ -105,7 +107,7 @@ struct EpiStore {
 
     __device__ void init(const EpiInit& e, int) const {
         for (int i = e.tid; i < 256; i += kEpiThreads) e.scratch[i] = (bias != nullptr && i < e.ncols) ? bias[e.col0 + i] : 0.f;
-        epi_bar_sync();
+        consumers_bar_sync();
     }
     __device__ void finish(const EpiInit& e) const {
         if (use_tma) WarpTileStore::drain(e.tid & 31);
@@ -126,16 +128,8 @@ struct EpiStore {
         WarpTileStore ts;
         ts.attach(c.scratch + 256, c.tid >> 5);
         if (use_tma) ts.begin_tile(lane);
-        float b[32];
         epi_chunks(
-            acc, c,
-            [&](int ch) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 b4 = lds_f4(c.scratch + ch * 32 + j);
-                    b[j] = b4.x; b[j + 1] = b4.y; b[j + 2] = b4.z; b[j + 3] = b4.w;
-                }
-            },
+            acc, c, [](int) {},
             [&](int ch, float* x) {
                 const int lc0 = ch * 32;
                 const bool whole = use_tma && lc0 + 32 <= c.ncols;  // warp-uniform
@@ -145,7 +139,10 @@ struct EpiStore {
                                   ((c.col0 + lc0) & 7) == 0;  // warp-uniform
                 if (!whole && !coop && !v) return;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) x[j] += b[j];
+                for (int j = 0; j < 32; j += 4) {  // bias from shared memory (zero past ncols)
+                    const float4 b4 = lds_f4(c.scratch + lc0 + j);
+                    x[j] += b4.x; x[j + 1] += b4.y; x[j + 2] += b4.z; x[j + 3] += b4.w;
+                }
                 if (relu) {
 #pragma unroll
                     for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.f);
@@ -249,8 +246,9 @@ struct EpiStore {
 // ------------------------------------------------------------------------------------------------
 // Additive-attention pooling (reference additive.py:35-53) fused behind  pre = X.Wa^T:
 //   score_r = sum_c tanh(pre_rc + ba_c) * qv_c ; w = softmax over the segment ; out_s = sum_r w_r X_r
-// Requires n_slices == 1 and rows_per_tile = (segments per tile) * seg_len.
-// scratch floats: [0,384) partial scores (part*128 + row) | [384,512) weights | [512,768) bias | [768,1024) query
+// Requires n_slices == 1 and rows_per_tile = (segments per tile) * seg_len, seg_len <= 64.
+// scratch floats: [0,256) bias | [256,512) query | per warpgroup w at 512 + 192w: [0,128) partial scores (half*64 + row),
+// [128,192) softmax weights
 // ------------------------------------------------------------------------------------------------
 struct EpiPool {
     static constexpr int kScratchBytes = 4096;
@@ -269,10 +267,10 @@ struct EpiPool {
 
     __device__ void init(const EpiInit& e, int) const {
         for (int i = e.tid; i < 256; i += kEpiThreads) {
-            e.scratch[512 + i] = i < e.ncols ? bias[e.col0 + i] : 0.f;
-            e.scratch[768 + i] = i < e.ncols ? qv[e.col0 + i] : 0.f;
+            e.scratch[i] = i < e.ncols ? bias[e.col0 + i] : 0.f;
+            e.scratch[256 + i] = i < e.ncols ? qv[e.col0 + i] : 0.f;
         }
-        epi_bar_sync();
+        consumers_bar_sync();
     }
     __device__ void finish(const EpiInit&) const {}
 
@@ -303,8 +301,8 @@ struct EpiPool {
         epi_chunks(
             acc, c, [](int) {},
             [&](int ch, float* x) {
-                const float* sb = c.scratch + 512 + ch * 32;
-                const float* sq = c.scratch + 768 + ch * 32;
+                const float* sb = c.scratch + ch * 32;
+                const float* sq = c.scratch + 256 + ch * 32;
 #pragma unroll
                 for (int j = 0; j < 32; j += 4) {
                     const float4 b4 = lds_f4(sb + j);
@@ -315,17 +313,12 @@ struct EpiPool {
                     score = fmaf(fast_tanh(x[j + 3] + b4.w), q4.w, score);
                 }
             });
-        float* s_part = c.scratch;
-        float* s_w = c.scratch + 384;
-        static_assert(kEpiParts <= 3, "EpiPool scratch layout");
-        auto row_score = [&](int r) {
-            float t = s_part[r];
-#pragma unroll
-            for (int pp = 1; pp < kEpiParts; ++pp) t += s_part[pp * 128 + r];
-            return t;
-        };
-        s_part[c.half * 128 + c.r] = score;
-        epi_bar_sync();
+        float* s_part = c.scratch + 512 + 192 * c.wg;
+        float* s_w = s_part + 128;
+        static_assert(kEpiHalves == 2 && (512 + 2 * 192) * 4 <= kScratchBytes, "EpiPool scratch layout");
+        auto row_score = [&](int r) { return s_part[r] + s_part[kTileM + r]; };
+        s_part[c.half * kTileM + c.r] = score;
+        epi_bar_sync(c.wg);
         if (c.half == 0) {
             float w = 0.f;
             if (c.valid) {
@@ -340,14 +333,14 @@ struct EpiPool {
             }
             s_w[c.r] = w;
         }
-        epi_bar_sync();
+        epi_bar_sync(c.wg);
         // out[segment] = sum_t w_t X_t: work item = (segment, 16-byte column chunk); the rows come back from L2 and
         // the loop keeps 10 (then 4, then 1) independent loads in flight per thread.
         const int row0 = c.tile * rows_per_tile;
         const int nseg = rows_per_tile / seg_len;
         const int nck = (D + 7) >> 3;  // the A pitch is a multiple of 8 elements: the last chunk stays in bounds
         const size_t pitch16 = static_cast<size_t>(lda) >> 3;
-        for (int item = c.tid; item < nseg * nck; item += kEpiThreads) {
+        for (int item = c.wtid; item < nseg * nck; item += kWgThreads) {
             const int s = item / nck, ck = item - s * nck;
             const int r0 = row0 + s * seg_len;
             if (r0 >= M) continue;
@@ -373,7 +366,7 @@ struct EpiPool {
                 for (int j = 0; j < 8 && ck * 8 + j < D; ++j) o[j] = a[j];
             }
         }
-        epi_bar_sync();
+        epi_bar_sync(c.wg);  // s_w is rewritten by this warpgroup's next tile
     }
 };
 
@@ -399,10 +392,10 @@ struct EpiDPre {
             e.scratch[256 + i] = i < e.ncols ? bias[e.col0 + i] : 0.f;
             e.scratch[512 + i] = i < e.ncols ? qv[e.col0 + i] : 0.f;
         }
-        epi_bar_sync();
+        consumers_bar_sync();
     }
     __device__ void finish(const EpiInit& e) const {
-        epi_bar_sync();
+        consumers_bar_sync();  // both warpgroups' column sums are in; one add per column and CTA
         for (int i = e.tid; i < e.ncols; i += kEpiThreads) atomicAdd(dqv + e.col0 + i, e.scratch[i]);
         if (use_tma) WarpTileStore::drain(e.tid & 31);
     }
@@ -419,37 +412,35 @@ struct EpiDPre {
             acc, c, [](int) {},
             [&](int ch, float* x) {
                 // bias and query vector are zero past ncols in shared memory: dp = 0 there without a column test, and
-                // the column sums of those columns are never added to dqv
-                float dp[32];
+                // the column sums of those columns are never added to dqv.  dp leaves packed (bf16 pairs) as soon as a pair is
+                // done: x (reused for ds * tanh) and the packed pairs are all the chunk keeps in registers.
+                uint32_t w[16];
 #pragma unroll
                 for (int j = 0; j < 32; j += 4) {
                     const float4 b4 = lds_f4(c.scratch + 256 + ch * 32 + j);
                     const float4 q4 = lds_f4(c.scratch + 512 + ch * 32 + j);
                     const float bb[4] = {b4.x, b4.y, b4.z, b4.w}, qq[4] = {q4.x, q4.y, q4.z, q4.w};
+                    float dp[4];
 #pragma unroll
                     for (int i = 0; i < 4; ++i) {
                         const float tt = tanh_approx(x[j + i] + bb[i]);
-                        dp[j + i] = (ds * qq[i]) * fmaf(-tt, tt, 1.f);
+                        dp[i] = (ds * qq[i]) * fmaf(-tt, tt, 1.f);
                         x[j + i] = ds * tt;
                     }
+                    w[j / 2] = pack_bf16x2(dp[0], dp[1]);
+                    w[j / 2 + 1] = pack_bf16x2(dp[2], dp[3]);
                 }
                 if (use_tma && ch * 32 + 32 <= c.ncols) {  // invalid rows carry ds = 0 and are clipped at M anyway
-                    uint32_t w[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) w[j] = pack_bf16x2(dp[2 * j], dp[2 * j + 1]);
                     ts.put(&tm_out, w, c.col0 + ch * 32, c.grow - lane, lane);
                 } else if (c.valid) {
-                    __nv_bfloat16* o = dpre + static_cast<size_t>(c.grow) * ld + c.col0 + ch * 32;
+                    uint4* o = reinterpret_cast<uint4*>(dpre + static_cast<size_t>(c.grow) * ld + c.col0 + ch * 32);
 #pragma unroll
-                    for (int g = 0; g < 2; ++g) {
+                    for (int g = 0; g < 2; ++g) {  // 16-byte groups of 8 columns (ld and col0 are multiples of 8)
                         const int lc = ch * 32 + g * 16;
                         if (lc >= c.ncols) break;  // ld is padded to a multiple of 8: whole 8-groups are in bounds
-                        if (lc + 16 <= ld - c.col0 && aligned32(o + g * 16)) {
-                            store_bf16x16(o + g * 16, dp + g * 16);
-                        } else {
-                            store_bf16x8(o + g * 16, dp + g * 16, 8);
-                            if (lc + 8 < c.ncols) store_bf16x8(o + g * 16 + 8, dp + g * 16 + 8, 8);
-                        }
+                        o[2 * g] = make_uint4(w[8 * g], w[8 * g + 1], w[8 * g + 2], w[8 * g + 3]);
+                        if ((lc + 16 <= ld - c.col0 && aligned32(o + 2 * g)) || lc + 8 < c.ncols)
+                            o[2 * g + 1] = make_uint4(w[8 * g + 4], w[8 * g + 5], w[8 * g + 6], w[8 * g + 7]);
                     }
                 }
                 const float colsum = warp_transpose_sum32(x);
@@ -460,12 +451,13 @@ struct EpiDPre {
 
 // ------------------------------------------------------------------------------------------------
 // dX_rc = acc_rc + w_r * dOut[seg(r)][c]  (pool backward, both paths into X) [* relu mask] [* dropout] -> bf16
-// scratch floats: two staging buffers of kStageFloats: the dOut rows (slice columns only) of every segment the tile
-// touches, [segment][pitch = slice width]; the buffer of the NEXT tile is filled by cp.async while this one is used.
+// scratch floats: two staging buffers of kStageFloats per warpgroup: the dOut rows (slice columns only) of every segment
+// the tile touches (<= 64/seg_len + 2), [segment][pitch = slice width]; the buffer of the warpgroup's NEXT tile is filled by
+// cp.async while this one is used.
 // ------------------------------------------------------------------------------------------------
 struct EpiDPoolIn {
-    static constexpr int kStageFloats = 2560;
-    static constexpr int kScratchBytes = 2 * kStageFloats * 4 + kTileStoreBytes;
+    static constexpr int kStageFloats = 1536;
+    static constexpr int kScratchBytes = 4 * kStageFloats * 4 + kTileStoreBytes;
     CUtensorMap tm_out;  // dx as a TMA tensor (32 x 32 boxes); valid when use_tma (identity row map, no ReLU mask)
     int use_tma;
     const float* w;      // [rows]
@@ -483,21 +475,22 @@ struct EpiDPoolIn {
     int M;
     int rows_per_tile;
 
-    // all 256 threads: queue the dOut rows of `tile` (columns [col0, col0 + ncols)) into buf
-    __device__ __forceinline__ void stage_tile(int tile, int col0, int ncols, int tid, float* buf) const {
+    // the 128 threads of a warpgroup (wtid): queue the dOut rows of `tile` (columns [col0, col0 + ncols)) into buf
+    __device__ __forceinline__ void stage_tile(int tile, int col0, int ncols, int wtid, float* buf) const {
         const int row0 = tile * rows_per_tile;
         const int seg_first = row0 / seg_len;
-        const int seg_last = min(row0 + 127, M - 1) / seg_len;
+        const int seg_last = min(row0 + kTileM - 1, M - 1) / seg_len;
         const int total = (seg_last - seg_first + 1) * ncols;
-        for (int i = tid; i < total; i += kEpiThreads) {
+        for (int i = wtid; i < total; i += kWgThreads) {
             const int sgi = i / ncols, j = i - sgi * ncols;
             const bool ok = col0 + j < N;
             cp_async_f32(buf + i, dout + static_cast<size_t>(seg_first + sgi) * ldo + (ok ? col0 + j : 0), ok);
         }
         cp_async_commit();
     }
-    __device__ void init(const EpiInit& e, int) const {
-        if (e.first_tile < e.num_tiles) stage_tile(e.first_tile, e.col0, e.ncols, e.tid, e.scratch);
+    __device__ void init(const EpiInit& e, int tile_step) const {  // each warpgroup queues its own first tile
+        const int wg = e.tid >> 7, first = e.first_tile + wg * tile_step;
+        if (first < e.num_tiles) stage_tile(first, e.col0, e.ncols, e.tid & 127, e.scratch + 2 * wg * kStageFloats);
     }
     __device__ void finish(const EpiInit& e) const {
         if (use_tma) WarpTileStore::drain(e.tid & 31);
@@ -511,15 +504,16 @@ struct EpiDPoolIn {
         const float wr = c.valid ? __ldg(w + c.grow) : 0.f;
         const int seg_first = (c.tile * rows_per_tile) / seg_len;
         const int myseg = (c.valid ? c.grow / seg_len : seg_first) - seg_first;
-        float* cur = c.scratch + (c.it & 1) * kStageFloats;
+        float* mine = c.scratch + 2 * c.wg * kStageFloats;
+        float* cur = mine + (c.it & 1) * kStageFloats;
         cp_async_wait_all();
-        epi_bar_sync();  // this tile's dOut rows are visible; everybody is done with the other buffer
-        if (c.next_tile >= 0) stage_tile(c.next_tile, c.col0, c.ncols, c.tid, c.scratch + ((c.it + 1) & 1) * kStageFloats);
+        epi_bar_sync(c.wg);  // this tile's dOut rows are visible; the warpgroup is done with its other buffer
+        if (c.next_tile >= 0) stage_tile(c.next_tile, c.col0, c.ncols, c.wtid, mine + ((c.it + 1) & 1) * kStageFloats);
         const float* sd = cur + myseg * c.ncols;
         const int lane = c.tid & 31;
         WarpTileStore ts;
         if (use_tma) {
-            ts.attach(c.scratch + 2 * kStageFloats, c.tid >> 5);
+            ts.attach(c.scratch + 4 * kStageFloats, c.tid >> 5);
             ts.begin_tile(lane);
         }
         epi_chunks(
@@ -557,7 +551,7 @@ struct EpiDPoolIn {
                 const bool coop = !use_tma && ch * 32 + 32 <= c.ncols && col + 32 <= N && (col & 7) == 0 && (ld & 7) == 0 &&
                                   (relu_src == nullptr || (relu_ld & 7) == 0);  // warp-uniform
                 if (coop) {
-                    uint8_t* stage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(c.scratch + 2 * kStageFloats) + 1023) & ~uintptr_t(1023)) +
+                    uint8_t* stage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(c.scratch + 4 * kStageFloats) + 1023) & ~uintptr_t(1023)) +
                                      (c.tid >> 5) * (kTileStoreBufs * 2048);
                     uint8_t* rb = stage;          // mask tile  (32 rows x 64 bytes, SWIZZLE_64B like WarpTileStore)
                     uint8_t* ob = stage + 2048;   // result tile

@@ -2,46 +2,52 @@
 //
 //  gemm_nt : D[M x N] = A[M x K] . B[N x K]^T      (both K-major; "activation x weight^T")
 //            * a CTA's weight slice (<=256 output columns, all K, all conv taps) is loaded ONCE by TMA and stays
-//              resident in shared memory; 128-row activation tiles stream through a TMA/mbarrier ring; two consumer
-//              warpgroups issue wgmma into registers and then run a fused epilogue functor on the accumulator rows.
+//              resident in shared memory; 64-row activation tiles stream through a TMA/mbarrier ring; two consumer
+//              warpgroups take the CTA's tiles in turn and run a fused epilogue functor on the accumulator rows.
 //            * conv taps: tap s re-loads the A tile shifted by (s - taps/2) rows (zero rows separate
 //              the segments in the padded layout), accumulating into the same registers.
 //  gemm_tn : D[Ma x Nb] += A[Kr x Ma]^T . B[Kr x Nb]  (both MN-major; weight gradients, Kr = all tokens)
 //            split over Kr (and over Nb past 256 columns) across CTAs, fp32 red.global.add epilogue.
 //
-// Warp roles of gemm_nt (kGemmThreads per CTA): warps 0..kEpiWarps-1 form two warpgroups.  Warpgroup h computes ALL 128
-// rows of the tile for its share of the slice's 32-column chunks (the "half" of the epilogue contract) with two m64 wgmmas
-// per k-step, so each epilogue thread finds its row and its columns inside its own warpgroup: the row-per-thread view the
-// epilogues read is made by passing one 32-column chunk at a time through a small shared-memory transpose buffer.  The
-// first warp of the last warpgroup is the TMA producer.
+// Warp roles of gemm_nt (kGemmThreads per CTA): warps 0..kEpiWarps-1 form two consumer warpgroups, the first warp of the
+// last warpgroup is the TMA producer.  Ping-pong schedule: warpgroup w owns the CTA's tiles w, w + 2, w + 4, ... and computes
+// a whole tile (64 rows x the whole slice) with one m64nN wgmma per k-step, N = 32 * (chunks of the slice).  The two
+// warpgroups issue their MMAs in strict alternation (a pair of named barriers passes the tensor pipe from one to the other),
+// so one warpgroup's epilogue runs while the other's wgmmas execute.  Inside a warpgroup the epilogue view is row-per-thread:
+// the m64 fragment passes through a small shared-memory transpose buffer one 32-column chunk per column half at a time.
 #pragma once
 #include "nr_common.cuh"
 
 namespace nr {
 
-constexpr int kEpiWarps = 8;  // gemm_nt epilogue warps: 2 warpgroups (= column parts) x 4 warps (32 rows each)
-constexpr int kEpiParts = kEpiWarps / 4;
+constexpr int kEpiWarps = 8;    // gemm_nt consumer / epilogue warps: 2 warpgroups, each owning whole tiles
 constexpr int kEpiThreads = kEpiWarps * 32;
+constexpr int kWgThreads = 128;
+constexpr int kEpiHalves = 2;   // column halves of a warpgroup's epilogue: warps 0-1 and 2-3 of the warpgroup
 // + a producer warpgroup (one warp issues TMA): registers are allocated per warpgroup, and setmaxnreg moves the producer's
 // share to the consumers, whose accumulators and epilogue registers need more than the even split of 168
 constexpr int kGemmThreads = kEpiThreads + 128;
 constexpr int kTnThreads = kGemmThreads;        // gemm_tn: the same two consumer warpgroups + producer
-constexpr int kProducerRegs = 40, kConsumerRegs = 232;
-constexpr int kTileM = 128;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;  // gemm_tn
+// gemm_nt: a consumer holds a whole m64n256 fragment (128 registers) next to its epilogue's; the TMA producer needs few
+constexpr int kNtProducerRegs = 24, kNtConsumerRegs = 240;
+constexpr int kTileM = 64;                      // gemm_nt rows per tile: one m64 wgmma
 constexpr int kChunkK = 64;                     // bf16 elements per 128-byte swizzle row
-constexpr int kAStageBytes = kTileM * 128;      // 16 KB
+constexpr int kAStageBytes = kTileM * 128;      // 8 KB
 constexpr int kMaxStages = 12;
 constexpr int kSmemLimit = 232448;              // 227 KB
-constexpr int kXposeBytes = kEpiParts * 128 * 16 * 4;  // per warpgroup: 128 rows x 16 fp32 columns (half a chunk)
+constexpr int kXposeBytes = 2 * kEpiHalves * kTileM * 16 * 4;  // per warpgroup and column half: 64 rows x 16 fp32 columns
+// named barriers of gemm_nt (0 is __syncthreads): all consumer threads, each warpgroup's own, each warpgroup's MMA turn
+constexpr int kBarConsumers = 1, kBarWg = 2, kBarTurn = 4;
 
 struct GemmNTParams {
     int M;              // rows of A that exist
-    int rows_per_tile;  // rows OWNED by one M tile (<=128); tile t loads rows [t*rpt, t*rpt+128)
+    int rows_per_tile;  // rows OWNED by one M tile (<=64); tile t loads rows [t*rpt, t*rpt+64)
     int num_m_tiles;
     int N;              // output columns
     int n_stride;       // columns per weight slice (multiple of 16)
     int n_slices;
-    int n_box;          // rows of one resident weight box (multiple of 16, <=256)
+    int n_box;          // rows of one resident weight box (multiple of 32, <=256)
     int K;              // reduction length per tap (elements)
     int k_chunks;       // ceil(K/64)
     int taps;           // 1, or 3 for the window-3 title CNN
@@ -49,7 +55,7 @@ struct GemmNTParams {
     int stages;
     int b_stream;       // 1: the weight slice does not fit beside the ring; its (tap, k-chunk) box travels with every A stage
     int stage_bytes;    // kAStageBytes (+ one weight box when b_stream)
-    float* dbg_acc;     // debug backend only: fp32 accumulators [num_m_tiles*128][dbg_ld]
+    float* dbg_acc;     // debug backend only: fp32 accumulators [num_m_tiles*kTileM][dbg_ld]
     int dbg_ld;
     int dbg_flags;      // tuning only (NEWSREC_GEMM_DBG): bit 1 = the producer skips the A loads (MMA on stale data)
     long long* timing;  // tuning only (nr_debug_set_gemm_timing): per CTA 16 cycle counters, see the kernel
@@ -58,78 +64,95 @@ struct GemmNTParams {
 // What an epilogue functor sees for one (tile,row).
 struct EpiCtx {
     int tile;
-    int r;        // row inside the tile (0..127)
+    int r;        // row inside the tile (0..63)
     int grow;     // global A row
     bool valid;   // r < rows_per_tile && grow < M
     int col0;     // first output column of this CTA's slice
     int ncols;    // valid output columns in the slice
-    int tid;      // 0..255 within the epilogue group
-    int half;     // 0 .. kEpiParts-1: column part (= warpgroup)
+    int tid;      // 0..255 over both consumer warpgroups (warp tid/32 owns 32 rows of its warpgroup's tile)
+    int wg;       // consumer warpgroup (0, 1) that owns this tile
+    int wtid;     // 0..127 within the warpgroup
+    int half;     // 0 .. kEpiHalves-1: column half inside the warpgroup
     int ch0, ch1; // this thread's range of 32-column chunks
-    float* scratch;  // Epi::kScratchBytes of shared memory private to the epilogue group
-    int it;          // how many tiles this CTA has finished before this one (double-buffer parity of the epilogue staging)
-    int next_tile;   // the tile this CTA processes next, or -1
+    int rounds;   // collective chunk loads per tile (the larger half's chunk count)
+    float* scratch;  // Epi::kScratchBytes of shared memory private to the epilogue (both warpgroups)
+    int it;          // how many tiles this warpgroup has finished before this one (double-buffer parity of the staging)
+    int next_tile;   // the tile this warpgroup processes next, or -1
 };
-// What init()/finish() see.
+// What init()/finish() see (all kEpiThreads consumer threads call them).
 struct EpiInit {
     int col0, ncols, tid;
     float* scratch;
-    int first_tile;  // first tile of this CTA (>= num_tiles: the CTA has no work)
+    int first_tile;  // first tile of this CTA (warpgroup w starts at first_tile + w * tile_step)
     int num_tiles;
 };
 
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); }
-// the two column halves run different chunk counts: barriers inside a chunk loop are per half
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// init()/finish(): every consumer thread of the CTA
+__device__ __forceinline__ void consumers_bar_sync() { named_bar_sync(kBarConsumers, kEpiThreads); }
+// per tile: the threads of the warpgroup that owns it (the two column halves run different chunk counts: barriers inside a
+// chunk loop are per half)
+__device__ __forceinline__ void epi_bar_sync(int wg) { named_bar_sync(kBarWg + wg, kWgThreads); }
 
 __device__ __forceinline__ void epi_chunk_range(int ncols, int part, int& ch0, int& ch1) {
-    const int nch = (ncols + 31) >> 5, base = nch / kEpiParts, rem = nch - base * kEpiParts;
+    const int nch = (ncols + 31) >> 5, base = nch / kEpiHalves, rem = nch - base * kEpiHalves;
     ch0 = part * base + min(part, rem);
     ch1 = ch0 + base + (part < rem ? 1 : 0);
 }
 
-// Accumulators of one warpgroup: acc[b] is the m64 wgmma fragment of rows [64b, 64b + 64) for the warpgroup's chunks
-// [ch0, ch1) (at most 4).  load32(ch) hands every thread the 32 columns of chunk ch of its own row (row = thread of the
-// warpgroup), through the warpgroup's transpose buffer, 16 columns at a time; every thread of the warpgroup calls it with the
-// same chunk sequence (the chunk range is per warpgroup).  Buffer layout: row r, column c at r*16 + ((c/4) ^ ((r/2)&3))*4 + c%4
-// (conflict-free row reads).
+// Accumulators of one warpgroup: the m64nN wgmma fragment of its tile (acc[4j + 2e + i] = row 16 * (warp % 4) + lane / 4 + 8e,
+// column 8j + 2 * (lane % 4) + i).  Thread t of the warpgroup reads row 32 * ((t / 32) % 2) + t % 32 of column half t / 64:
+// half 0 owns chunks [0, second), half 1 chunks [second, nch).  load32(i) is collective over the warpgroup: round i hands
+// every thread the 32 columns of its half's i-th chunk, through the warpgroup's transpose buffers (one per half, 64 rows x
+// 16 columns), 16 columns at a time; when nch is odd, half 1 has no chunk in the last round and only reads.  Buffer layout:
+// row r, column c at r*16 + ((c/4) ^ ((r/2)&3))*4 + c%4 (conflict-free row reads).
 struct RegAcc {
-    float (*acc)[64];
+    float* acc;
     float* xpose;   // this warpgroup's 8 KB
-    int ch0;
+    int second;     // first chunk of column half 1 (= the number of rounds)
+    int nch;
     int bar_id;     // named barrier of the warpgroup
-    __device__ __forceinline__ void sync() const { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); }
+    __device__ __forceinline__ void sync() const { named_bar_sync(bar_id, kWgThreads); }
     template <int Q>
-    __device__ __forceinline__ void put_half(int hf) const {  // columns [32Q + 16hf, +16) of the fragment into the buffer
+    __device__ __forceinline__ void put_half(int hf, float* buf) const {  // columns [32Q + 16hf, +16) of the fragment
         const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
 #pragma unroll
-        for (int b = 0; b < 2; ++b)
+        for (int jj = 0; jj < 2; ++jj) {
+            const int j = 4 * Q + 2 * hf + jj;  // 8-column group of the fragment
+            const int c = 8 * jj + 2 * (lane & 3);
 #pragma unroll
-            for (int jj = 0; jj < 2; ++jj) {
-                const int j = 4 * Q + 2 * hf + jj;  // 8-column group of the fragment
-                const int c = 8 * jj + 2 * (lane & 3);
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int r = 64 * b + 16 * wq + (lane >> 2) + 8 * e;
-                    *reinterpret_cast<float2*>(xpose + r * 16 + (((c >> 2) ^ ((r >> 1) & 3)) << 2) + (c & 3)) =
-                        make_float2(acc[b][4 * j + 2 * e], acc[b][4 * j + 2 * e + 1]);
-                }
+            for (int e = 0; e < 2; ++e) {
+                const int r = 16 * wq + (lane >> 2) + 8 * e;
+                *reinterpret_cast<float2*>(buf + r * 16 + (((c >> 2) ^ ((r >> 1) & 3)) << 2) + (c & 3)) =
+                    make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]);
             }
+        }
     }
-    __device__ __forceinline__ void load32(int chunk, float* v) const {
-        const int q = chunk - ch0, r = threadIdx.x & 127;
+    __device__ __forceinline__ void put_chunk(int q, int hf, float* buf) const {
+        switch (q) {
+            case 0: put_half<0>(hf, buf); break;
+            case 1: put_half<1>(hf, buf); break;
+            case 2: put_half<2>(hf, buf); break;
+            case 3: put_half<3>(hf, buf); break;
+            case 4: put_half<4>(hf, buf); break;
+            case 5: put_half<5>(hf, buf); break;
+            case 6: put_half<6>(hf, buf); break;
+            default: put_half<7>(hf, buf); break;
+        }
+    }
+    __device__ __forceinline__ void load32(int i, float* v) const {
+        const int t = threadIdx.x & 127, r = 32 * ((t >> 5) & 1) + (t & 31);
+        const float* mine = xpose + (t >> 6) * (kTileM * 16);
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
-            sync();  // every thread has read the previous half out of the buffer
-            switch (q) {
-                case 0: put_half<0>(hf); break;
-                case 1: put_half<1>(hf); break;
-                case 2: put_half<2>(hf); break;
-                default: put_half<3>(hf); break;
-            }
+            sync();  // every thread has read the previous half out of the buffers
+            put_chunk(i, hf, xpose);
+            if (second + i < nch) put_chunk(second + i, hf, xpose + kTileM * 16);
             sync();
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
-                const float4 f = lds_f4(xpose + r * 16 + ((g ^ ((r >> 1) & 3)) << 2));
+                const float4 f = lds_f4(mine + r * 16 + ((g ^ ((r >> 1) & 3)) << 2));
                 v[16 * hf + 4 * g] = f.x; v[16 * hf + 4 * g + 1] = f.y; v[16 * hf + 4 * g + 2] = f.z; v[16 * hf + 4 * g + 3] = f.w;
             }
         }
@@ -138,25 +161,30 @@ struct RegAcc {
 };
 struct GlobalAcc {  // debug backend: accumulators computed by a plain SIMT kernel
     const float* row;
-    __device__ __forceinline__ void load32(int chunk, float* v) const {
+    int ch0, ch1;
+    __device__ __forceinline__ void load32(int i, float* v) const {
+        const int chunk = ch0 + i;
+        if (chunk >= ch1) return;
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = row[chunk * 32 + j];
     }
     __device__ __forceinline__ void release() const {}
 };
 
-// The chunk loop every epilogue shares.  pre(ch) runs before the load of chunk ch (shared-memory operand loads go there).
-// Calls acc.release() exactly once, after the last chunk has landed in registers.
+// The chunk loop every epilogue shares: c.rounds collective loads, the thread's chunk of round i is ch0 + i (when it has one).
+// pre(ch) runs before the load of chunk ch (shared-memory operand loads go there).  Calls acc.release() exactly once, after
+// the last chunk has landed in registers.
 template <class Acc, class Pre, class Body>
 __device__ __forceinline__ void epi_chunks(const Acc& acc, const EpiCtx& c, Pre&& pre, Body&& body) {
-    for (int ch = c.ch0; ch < c.ch1; ++ch) {
+    for (int i = 0; i < c.rounds; ++i) {
+        const int ch = c.ch0 + i;
+        const bool mine = ch < c.ch1;  // warp-uniform
         float x[32];
-        pre(ch);
-        acc.load32(ch, x);
-        if (ch + 1 == c.ch1) acc.release();
-        body(ch, x);
+        if (mine) pre(ch);
+        acc.load32(i, x);
+        if (mine) body(ch, x);
     }
-    if (c.ch0 >= c.ch1) acc.release();
+    acc.release();
 }
 
 // bf16 output tiles leave through TMA instead of 32 scattered rows per store instruction: a warp packs its 32 rows x 32
@@ -225,38 +253,37 @@ struct WarpTileStore {
 // mbarrier protocol:
 //   bfull     count 1 + tx of the resident weight slice    -> the consumers may start (not used when b_stream)
 //   full[s]   count 1 + tx of one A box (+ its weight box when b_stream; the producer's expect_tx)
-//   empty[s]  count kEpiWarps: every consumer warp arrives once its wgmmas on stage s have completed
-// Warpgroup h multiplies the 128-row A tile by the weight rows of its chunks [ch0, ch1): two m64 x (32 * nch) wgmmas per
-// k-step, nch <= 4 (a slice is <= 256 columns, split into two parts).
-// The MMAs of one tile for a warpgroup with NCH chunks (a compile-time N keeps the wgmmas asynchronous): one wgmma group
-// per ring stage, one group left in flight while the next stage is awaited; a stage is released once its group completed.
+//   empty[s]  count 4: every warp of the warpgroup that consumes stage s arrives once its wgmmas on it have completed
+// The producer fills the ring in the CTA's tile order (taps * k_chunks stages per tile); each warpgroup walks the ring past
+// the other warpgroup's tiles.
+// MMA turn (named barriers kBarTurn + w, 256 threads): warpgroup w waits on its barrier before issuing a tile (except the
+// CTA's first tile) and, once all its wgmmas are issued, arrives on the other warpgroup's barrier if the CTA has a next tile.
+// Every arrive therefore meets exactly one wait, and the tiles' MMAs run in the CTA's tile order.
+// The MMAs of one tile with NCH chunks (a compile-time N keeps the wgmmas asynchronous): one wgmma group per ring stage, one
+// group left in flight while the next stage is awaited; a stage is released once its group completed.
 template <int NCH>
-__device__ __forceinline__ void gemm_nt_mma_tile(float (*acc)[64], const GemmNTParams& p, uint64_t* full, uint64_t* empty,
-                                                 int& st, uint32_t& ph, uint32_t a_s, uint32_t b_s, uint32_t b_off, int b_region,
-                                                 int lane) {
+__device__ __forceinline__ void gemm_nt_mma_tile(float* acc, const GemmNTParams& p, uint64_t* full, uint64_t* empty, int& st,
+                                                 uint32_t& ph, uint32_t a_s, uint32_t b_s, int b_region, int lane, int pass_bar) {
+    // the first k-step overwrites the accumulators (scale_d = 0): start a fresh value here, so that the previous tile's
+    // accumulators are dead once the epilogue has read them instead of occupying registers through the whole epilogue
+#pragma unroll
+    for (int i = 0; i < 16 * NCH; ++i) asm volatile("" : "=f"(acc[i]));
     int prev = -1;
     for (int s = 0; s < p.taps; ++s)
         for (int kc = 0; kc < p.k_chunks; ++kc) {
             mbar_wait(&full[st], ph, 104);
-            if constexpr (NCH > 0) {
-                const uint32_t a_st = a_s + st * p.stage_bytes;
-                const uint32_t b_box = p.b_stream ? a_st + kAStageBytes + b_off : b_s + (s * p.k_chunks + kc) * b_region;
-                const uint64_t db = make_sw128_desc(b_box, 16, 1024);
-                const int first = (s | kc) == 0;
+            const uint32_t a_st = a_s + st * p.stage_bytes;
+            const uint32_t b_box = p.b_stream ? a_st + kAStageBytes : b_s + (s * p.k_chunks + kc) * b_region;
+            const uint64_t da = make_sw128_desc(a_st, 16, 1024), db = make_sw128_desc(b_box, 16, 1024);
+            const int first = (s | kc) == 0;
 #pragma unroll
-                for (int b = 0; b < 2; ++b)
+            for (int i = 0; i < 16 * NCH; ++i) wgmma_reg_fence(acc[i]);
+            wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 16 * NCH; ++i) wgmma_reg_fence(acc[b][i]);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < 4; ++k)  // +32 bytes per k-step = +2 in the descriptor's >>4 address field
-#pragma unroll
-                    for (int b = 0; b < 2; ++b)
-                        Wgmma<32 * NCH, 0, 0>::mma(acc[b], make_sw128_desc(a_st + b * 8192, 16, 1024) + 2 * k, db + 2 * k,
-                                                   (first && k == 0) ? 0 : 1);
-                wgmma_commit();
-                wgmma_wait<1>();  // the group of the previous stage has completed
-            }
+            for (int k = 0; k < 4; ++k)  // +32 bytes per k-step = +2 in the descriptor's >>4 address field
+                Wgmma<32 * NCH, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, (first && k == 0) ? 0 : 1);
+            wgmma_commit();
+            wgmma_wait<1>();  // the group of the previous stage has completed
             if (prev >= 0) {
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[prev]);  // this warp's reads of stage prev are complete
@@ -264,13 +291,10 @@ __device__ __forceinline__ void gemm_nt_mma_tile(float (*acc)[64], const GemmNTP
             prev = st;
             if (++st == p.stages) { st = 0; ph ^= 1; }
         }
-    if constexpr (NCH > 0) {
-        wgmma_wait<0>();
+    if (pass_bar >= 0) named_bar_arrive(pass_bar, 2 * kWgThreads);  // the other warpgroup may issue its tile
+    wgmma_wait<0>();
 #pragma unroll
-        for (int b = 0; b < 2; ++b)
-#pragma unroll
-            for (int i = 0; i < 16 * NCH; ++i) wgmma_reg_fence(acc[b][i]);
-    }
+    for (int i = 0; i < 16 * NCH; ++i) wgmma_reg_fence(acc[i]);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
 }
@@ -300,27 +324,17 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int col0 = slice * p.n_stride;
     const int ncols = min(p.n_stride, p.N - col0);
     const int tap_shift = p.taps / 2;
-    // tuning counters: [0] producer waits for a free A stage, [1] MMA loops incl. waits for A data, [4] epilogue body, [5] kernel,
-    // [6] tiles
+    // tuning counters: [0] producer waits for a free A stage, [5] kernel; per consumer warpgroup w at [8 + 4w]: +0 waits for
+    // its MMA turn, +1 MMA loops incl. waits for A data (turn waits excluded), +2 epilogue, +3 tiles
     long long* tmr = p.timing != nullptr ? p.timing + blockIdx.x * 16 : nullptr;
     const long long t_begin = tmr != nullptr ? clock64() : 0;
-    long long tw_a = 0, tw_b = 0;
-    auto timed_wait = [&](uint64_t* bar, uint32_t parity, int code, long long& acc_t) {
-        if (tmr != nullptr) {
-            const long long t = clock64();
-            mbar_wait(bar, parity, code);
-            acc_t += clock64() - t;
-        } else {
-            mbar_wait(bar, parity, code);
-        }
-    };
 
     if (warp == kEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], kEpiWarps);
+            mbar_init(&empty[i], 4);
         }
         mbar_init(bfull, 1);
         fence_barrier_init();
@@ -328,7 +342,7 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     __syncthreads();
 
     if (warp >= kEpiWarps) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kNtProducerRegs));
         if (warp != kEpiWarps) return;
         // ===================== TMA producer (uniform loops, one elected lane issues) =====================
         if (!p.b_stream && elect_one()) {
@@ -340,11 +354,14 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         __syncwarp();
         int st = 0;
         uint32_t ph = 0;
+        long long tw_empty = 0;
         for (int tile = tile0; tile < p.num_m_tiles; tile += tile_step) {
             const int row0 = tile * p.rows_per_tile;
             for (int s = 0; s < p.taps; ++s)
                 for (int kc = 0; kc < p.k_chunks; ++kc) {
-                    timed_wait(&empty[st], ph ^ 1, 101, tw_a);
+                    const long long t = tmr != nullptr ? clock64() : 0;
+                    mbar_wait(&empty[st], ph ^ 1, 101);
+                    if (tmr != nullptr) tw_empty += clock64() - t;
                     if (elect_one()) {
 #ifdef NEWSREC_TRIAGE
                         if (p.dbg_flags & 2) {
@@ -362,64 +379,81 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     if (++st == p.stages) { st = 0; ph ^= 1; }
                 }
         }
-        if (tmr != nullptr && lane == 0) tmr[0] = tw_a;
+        if (tmr != nullptr && lane == 0) tmr[0] = tw_empty;
     } else {
-        // ===================== consumer warpgroups: wgmma, then the epilogue on the same registers =====================
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
-        const int half = warp >> 2;
-        const int quarter = warp & 3;
+        // ===================== consumer warpgroups: whole tiles in turn, wgmma then the epilogue =====================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kNtConsumerRegs));
+        const int wg = warp >> 2;
+        const int half = (warp >> 1) & 1;
         int ch0, ch1;
         epi_chunk_range(ncols, half, ch0, ch1);
-        const int nch = ch1 - ch0;
+        const int nch = (ncols + 31) >> 5;
+        const int rounds = (nch + 1) >> 1;
         const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, p.num_m_tiles};
         epi.init(ei, tile_step);
-        const uint32_t a_s = smem_u32(sA), b_s = smem_u32(sB) + ch0 * 32 * 128;
-        const uint32_t b_off = ch0 * 32 * 128;
-        float acc[2][64];
-#pragma unroll
-        for (int b = 0; b < 2; ++b)
-#pragma unroll
-            for (int i = 0; i < 64; ++i) acc[b][i] = 0.f;
-        const RegAcc racc{acc, xpose + half * (kXposeBytes / 4 / kEpiParts), ch0, 2 + half};
+        const uint32_t a_s = smem_u32(sA), b_s = smem_u32(sB);
+        float acc[128];
+        const RegAcc racc{acc, xpose + wg * (kXposeBytes / 4 / 2), rounds, nch, kBarWg + wg};
         if (!p.b_stream) mbar_wait(bfull, 0, 102);
         int st = 0;
         uint32_t ph = 0;
+        const int tile_stages = p.taps * p.k_chunks;
+        auto skip_tile = [&]() {  // the ring stages of the other warpgroup's tile
+            st += tile_stages;
+            while (st >= p.stages) { st -= p.stages; ph ^= 1; }
+        };
+        if (wg == 1) skip_tile();
+        long long tw_turn = 0, tw_mma = 0, tw_epi = 0;
         int it = 0;
-        for (int tile = tile0; tile < p.num_m_tiles; tile += tile_step, ++it) {
-            const long long t_mma = tmr != nullptr ? clock64() : 0;
+        for (int tile = tile0 + wg * tile_step; tile < p.num_m_tiles; tile += 2 * tile_step, ++it) {
+            long long t = tmr != nullptr ? clock64() : 0;
+            if (tile != tile0) named_bar_sync(kBarTurn + wg, 2 * kWgThreads);  // the other warpgroup has issued its tile
+            if (tmr != nullptr) { const long long u = clock64(); tw_turn += u - t; t = u; }
+            const int pass_bar = tile + tile_step < p.num_m_tiles ? kBarTurn + (wg ^ 1) : -1;
             switch (nch) {
-                case 0: gemm_nt_mma_tile<0>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
-                case 1: gemm_nt_mma_tile<1>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
-                case 2: gemm_nt_mma_tile<2>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
-                case 3: gemm_nt_mma_tile<3>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
-                default: gemm_nt_mma_tile<4>(acc, p, full, empty, st, ph, a_s, b_s, b_off, b_region, lane); break;
+                case 1: gemm_nt_mma_tile<1>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                case 2: gemm_nt_mma_tile<2>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                case 3: gemm_nt_mma_tile<3>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                case 4: gemm_nt_mma_tile<4>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                case 5: gemm_nt_mma_tile<5>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                case 6: gemm_nt_mma_tile<6>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                case 7: gemm_nt_mma_tile<7>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
+                default: gemm_nt_mma_tile<8>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
             }
-            if (tmr != nullptr) tw_b += clock64() - t_mma;
-            const long long t_epi = tmr != nullptr ? clock64() : 0;
+            skip_tile();
+            if (tmr != nullptr) { const long long u = clock64(); tw_mma += u - t; t = u; }
             EpiCtx c;
             c.tile = tile;
-            c.r = quarter * 32 + lane;
+            c.r = 32 * (warp & 1) + lane;
             c.grow = tile * p.rows_per_tile + c.r;
             c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
             c.col0 = col0;
             c.ncols = ncols;
             c.tid = threadIdx.x;
+            c.wg = wg;
+            c.wtid = threadIdx.x & 127;
             c.half = half;
             c.ch0 = ch0;
             c.ch1 = ch1;
+            c.rounds = rounds;
             c.scratch = scratch;
             c.it = it;
-            c.next_tile = tile + tile_step < p.num_m_tiles ? tile + tile_step : -1;
+            c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
             epi(racc, c);
-            if (tmr != nullptr) tw_a += clock64() - t_epi;
+            if (tmr != nullptr) tw_epi += clock64() - t;
         }
         epi.finish(ei);
-        if (tmr != nullptr && threadIdx.x == 0) { tmr[1] = tw_b; tmr[4] = tw_a; tmr[5] = clock64() - t_begin; tmr[6] = it; }
+        if (tmr != nullptr && (threadIdx.x & 127) == 0) {
+            long long* w = tmr + 8 + 4 * wg;
+            w[0] = tw_turn; w[1] = tw_mma; w[2] = tw_epi; w[3] = it;
+            if (wg == 0) tmr[5] = clock64() - t_begin;
+        }
     }
 }
 
 // Debug backend (TRIAGE builds only -- `make TRIAGE=1`, -DNEWSREC_TRIAGE; the release library has no second backend and
-// consults no environment switch on the launch path): plain SIMT accumulate + the SAME epilogue functors.
+// consults no environment switch on the launch path): plain SIMT accumulate + the SAME epilogue functors, with the same two
+// warpgroups taking the CTA's tiles in turn.
 #ifdef NEWSREC_TRIAGE
 __global__ void gemm_nt_simt_acc_kernel(const __nv_bfloat16* A, int lda, const __nv_bfloat16* B, int ldb,
                                         GemmNTParams p);
@@ -431,26 +465,30 @@ __global__ void __launch_bounds__(kEpiThreads, 1) gemm_nt_simt_epi_kernel(const 
     const int tile_step = gridDim.x / p.n_slices;
     const int col0 = slice * p.n_stride;
     const int ncols = min(p.n_stride, p.N - col0);
+    const int wg = threadIdx.x >> 7;
     for (int i = threadIdx.x; i < Epi::kScratchBytes / 4; i += kEpiThreads) scratch[i] = 0.f;
     __syncthreads();
     const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, p.num_m_tiles};
     epi.init(ei, tile_step);
     int it = 0;
-    for (int tile = tile0; tile < p.num_m_tiles; tile += tile_step, ++it) {
+    for (int tile = tile0 + wg * tile_step; tile < p.num_m_tiles; tile += 2 * tile_step, ++it) {
         EpiCtx c;
         c.tile = tile;
-        c.r = threadIdx.x & 127;
+        c.r = 32 * ((threadIdx.x >> 5) & 1) + (threadIdx.x & 31);
         c.grow = tile * p.rows_per_tile + c.r;
         c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
         c.col0 = col0;
         c.ncols = ncols;
         c.tid = threadIdx.x;
-        c.half = threadIdx.x >> 7;
+        c.wg = wg;
+        c.wtid = threadIdx.x & 127;
+        c.half = (threadIdx.x >> 6) & 1;
         epi_chunk_range(ncols, c.half, c.ch0, c.ch1);
+        c.rounds = (((ncols + 31) >> 5) + 1) >> 1;
         c.scratch = scratch;
         c.it = it;
-        c.next_tile = tile + tile_step < p.num_m_tiles ? tile + tile_step : -1;
-        GlobalAcc acc{p.dbg_acc + (static_cast<size_t>(tile) * 128 + c.r) * p.dbg_ld + col0};
+        c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
+        GlobalAcc acc{p.dbg_acc + (static_cast<size_t>(tile) * kTileM + c.r) * p.dbg_ld + col0, c.ch0, c.ch1};
         epi(acc, c);
     }
     epi.finish(ei);
@@ -502,7 +540,7 @@ int launch_gemm_nt(const GemmNTPlan& plan, const Epi& epi, const void* A, int ld
         GemmNTParams p = plan.p;
         const size_t ld = static_cast<size_t>(round_up(p.N, 32) + 32);
         float* acc = nullptr;
-        NR_CHECK_CUDA(cudaMallocAsync(&acc, sizeof(float) * ld * p.num_m_tiles * 128, stream));
+        NR_CHECK_CUDA(cudaMallocAsync(&acc, sizeof(float) * ld * p.num_m_tiles * kTileM, stream));
         p.dbg_acc = acc;
         p.dbg_ld = static_cast<int>(ld);
         dim3 g(ceil_div(static_cast<int>(ld), 128), p.num_m_tiles);

@@ -16,6 +16,10 @@ struct RowMapCfg {  // see RowMap in nr_epilogues.cuh; seg_in == 0 => identity
 };
 
 // ---- wgmma GEMMs with fused epilogues (gemm.cu) ------------------------------------------------
+// rows_per_tile: rows of A owned by one 64-row tile (kGemmTileRows).  gemm_store / gemm_scatter_emb compute every row
+// independently (conv taps read their neighbour rows through shifted loads), so they take whole tiles; larger values are
+// clamped to the tile.
+constexpr int kGemmTileRows = 64;
 // out[rows x N] = act(A . W^T + bias) (bf16 or fp32).  A bf16 [M x K] pitch lda (taps>1: padded CNN layout),
 // W bf16 [taps*w_tap_rows x K] pitch ldw.
 int gemm_store(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,

@@ -1,5 +1,6 @@
-"""Where do the gemm_nt CTAs wait?  One NRMS training step at the bench size with the per-role cycle counters of
-nr_debug_set_gemm_timing switched on; prints, per GEMM launch, the share of the kernel each role spent waiting.
+"""Where do the gemm_nt CTAs spend their time?  One NRMS training step at the bench size with the per-role cycle counters
+of nr_debug_set_gemm_timing switched on; prints, per GEMM launch, the share of the kernel each role (producer, each
+consumer warpgroup's MMA turn wait, MMA loop and epilogue) took.
 
     python tools/gemm_timing.py [NRMS|NAML|LSTUR|TANR] [batch]
 """
@@ -47,14 +48,17 @@ lib.nr_debug_set_gemm_timing(buf.data_ptr(), SLOTS)
 step()
 lib.nr_debug_set_gemm_timing(None, 0)
 t = buf.cpu().double()
-names = ["prod:empty", "mma:full", "mma:tempty", "epi:tfull", "epi:body", "kernel", "tiles"]
+# per CTA (gemm_nt_kernel): [0] producer waits for a free stage, [5] kernel; consumer warpgroup w at [8 + 4w]: +0 waits for
+# its MMA turn, +1 MMA loops (waits for A data included), +2 epilogue, +3 tiles.  With the epilogue overlapped, mma0 + mma1
+# approaches 100% of the kernel while each warpgroup's epilogue share stays large.
 for s in range(SLOTS):
     used = t[s, :, 5] > 0
     if used.sum() == 0:
         continue
     m = t[s][used].mean(0)
     k = m[5].item()
-    print(f"slot {s:2d} ctas={int(used.sum())} kernel={k / 1e3:8.1f} kcyc tiles/cta={m[6].item():6.1f}  " +
-          "  ".join(f"{names[i]}={100 * m[i].item() / k:5.1f}%" for i in range(5)) +
-          f"  epi/tile={m[4].item() / max(m[6].item(), 1):7.0f} cyc  mma:issue={100 * m[7].item() / k:5.1f}% mma:commit={100 * m[8].item() / k:5.1f}% mma:fence={100 * m[9].item() / k:5.1f}%",
-          flush=True)
+    pct = lambda i: 100 * m[i].item() / k
+    wgs = "  ".join(f"wg{w}: turn={pct(8 + 4 * w):5.1f}% mma={pct(9 + 4 * w):5.1f}% epi={pct(10 + 4 * w):5.1f}% "
+                    f"tiles={m[11 + 4 * w].item():6.1f} epi/tile={m[10 + 4 * w].item() / max(m[11 + 4 * w].item(), 1):6.0f} cyc"
+                    for w in range(2))
+    print(f"slot {s:2d} ctas={int(used.sum())} kernel={k / 1e3:8.1f} kcyc prod:empty={pct(0):5.1f}%  {wgs}", flush=True)

@@ -1,7 +1,7 @@
 """Micro-benchmarks of single C-ABI operators at BASELINE sizes (CUDA events on the launching stream, L2 flushed
 between repetitions by a 256 MB memset).  A tuning tool; bench.py is the contract benchmark.
 
-    python tools/kbench.py [op ...]      ops: mhsa_fwd mhsa_fwd_drop mhsa_bwd qkv pool scatter dinput tn900 tn200 gather
+    python tools/kbench.py [op ...]      ops: mhsa_fwd mhsa_fwd_drop mhsa_bwd qkv pool tn900 tn200 gather dx_fp32 lin:N:K
 """
 import ctypes as C
 import os
