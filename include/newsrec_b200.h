@@ -212,7 +212,9 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream);
  *   LSTUR title branch     src/model/LSTUR/news_encoder.py:56-72
  *   TANR  NewsEncoder      src/model/TANR/news_encoder.py:40-52
  * embedding -> dropout -> Conv2d(1, F, (3, d), padding (1, 0)) -> ReLU -> dropout -> additive pooling.
- * The conv is three row-shifted wgmma GEMM taps over a zero-padded layout (T+2 rows per segment). */
+ * The conv is three row-shifted wgmma GEMM taps over a zero-padded layout (T+2 rows per segment).
+ * Shapes: 1 <= T <= 64 (the pooling tile holds whole segments), d and F multiples of 4, d, F >= 8, 1 <= q <= 256;
+ * both entry points reject any other shape with -1 before the first launch. */
 typedef struct {
     long long n_seq;
     int T, d, F, q, ldx, ldf;       /* ldx = round_up(d+1, 8), ldf = round_up(F+1, 8)                       */

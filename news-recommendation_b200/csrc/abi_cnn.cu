@@ -15,11 +15,13 @@ static inline long long align256(long long x) { return (x + 255) & ~255ll; }
 static inline int ru8(int x) { return (x + 7) & ~7; }
 static inline int ru16(int x) { return (x + 15) & ~15; }
 
+// Every shape limit of the kernels the encoder chains is checked here, before the first launch: T <= kGemmTileRows because
+// a pooling tile holds whole segments (gemm_additive_pool), F % 4 == 0 for the float4 dOut rows of pool_dscore.
 static int check_cnn_shape(long long n_seq, int T, int d, int F, int q, int ldx, int ldf) {
-    NR_REQUIRE(n_seq >= 0 && T >= 1 && T <= 126 && d >= 8 && F >= 8 && q >= 1 && q <= 256,
-               "cnn encoder: bad shape n_seq=%lld T=%d d=%d F=%d q=%d", n_seq, T, d, F, q);
+    NR_REQUIRE(n_seq >= 0 && T >= 1 && T <= kGemmTileRows && d >= 8 && F >= 8 && q >= 1 && q <= 256,
+               "cnn encoder: bad shape n_seq=%lld T=%d (at most %d) d=%d F=%d q=%d", n_seq, T, kGemmTileRows, d, F, q);
     NR_REQUIRE(ldx == ru8(d + 1) && ldf == ru8(F + 1), "cnn encoder: pitches must be round_up(width+1, 8) (ldx=%d ldf=%d)", ldx, ldf);
-    NR_REQUIRE(d % 4 == 0 && F % 2 == 0, "cnn encoder: d must be a multiple of 4 and F even (d=%d F=%d)", d, F);
+    NR_REQUIRE(d % 4 == 0 && F % 4 == 0, "cnn encoder: d and F must be multiples of 4 (d=%d F=%d)", d, F);
     NR_REQUIRE(n_seq * (T + 2) < (1ll << 31), "cnn encoder: too many rows");
     return 0;
 }

@@ -816,3 +816,508 @@ def check_pack_slots(B=37, H=50, Cn=5, tail=(20,), where="pinned"):
                      torch.stack([x["f"].cpu() for x in cand], 1).reshape(B * Cn, *tail)), 0)
     return {"equal": bool(torch.equal(ids.cpu(), ref)), "B": Bo, "direct": direct is not None,
             "direct_equal": direct is None or bool(torch.equal(direct[0].cpu(), ref))}
+
+
+# ------------------------------------------------------------------------------------------------
+# The CNN text encoder (nr_cnn_encoder_fwd / _bwd) and its companion operators, called through the C ABI with every output
+# pre-filled (NaN where the ABI writes "=", a known pattern where it accumulates "+=") and followed by a guard of sentinel
+# values, then compared ROW BY ROW with fp64 evaluations on the device built from the kernels' own stored inputs.  A norm
+# over a whole tensor of 600k rows cannot see one wrong row; a per-row or per-segment measure can.
+# ------------------------------------------------------------------------------------------------
+_GUARD = 2048
+_M32 = 0xFFFFFFFF
+_INT_VIEW = {torch.bfloat16: torch.int16, torch.float32: torch.int32, torch.int32: torch.int32, torch.uint8: torch.uint8,
+             torch.int64: torch.int64}
+
+
+class _Guarded:
+    """Flat device buffer of n elements pre-filled with `fill` (a scalar, or a tensor of n elements kept as `prefill` for the
+    "+=" outputs), followed by _GUARD sentinel elements.  Only the guard is copied: the bodies can be hundreds of MB."""
+
+    def __init__(self, n, dtype, fill, sentinel=-1234.5):
+        self.n = int(n)
+        self.all = torch.empty(self.n + _GUARD, dtype=dtype, device=DEV)
+        self.prefill = None
+        if isinstance(fill, torch.Tensor):
+            self.prefill = fill.reshape(-1).to(dtype)
+            self.all[:self.n] = self.prefill
+        else:
+            self.all[:self.n].fill_(fill)
+        self.all[self.n:].fill_(sentinel)
+        self.guard = self.all[self.n:].clone()
+
+    @property
+    def body(self):
+        return self.all[:self.n]
+
+    def guard_ok(self):
+        iv = _INT_VIEW[self.all.dtype]
+        return bool(torch.equal(self.all[self.n:].view(iv), self.guard.view(iv)))
+
+    def unchanged(self, mask):
+        """Elements selected by the boolean mask over the body still hold their pre-fill, bit for bit."""
+        iv = _INT_VIEW[self.all.dtype]
+        return bool(torch.equal(self.body.view(iv)[mask.reshape(-1)], self.prefill.view(iv)[mask.reshape(-1)]))
+
+
+def _bits_equal(a, b):
+    iv = _INT_VIEW[a.dtype]
+    return bool(torch.equal(a.contiguous().view(iv), b.contiguous().view(iv)))
+
+
+def _mul32(a, b):
+    """(a * b) mod 2^32 for an int64 tensor a < 2^32 and a constant b < 2^32, without int64 overflow."""
+    return (a * (b & 0xFFFF) + (((a * (b >> 16)) & 0xFFFF) << 16)) & _M32
+
+
+def dropout_mask_dev(seed, p, rows, n_cols, ld):
+    """Device restatement of oracle.dropout_mask (the kernels' counter hash): fp32 multipliers of the given rows (int64
+    device tensor) and columns [0, n_cols) of a matrix with pitch ld."""
+    import numpy as np
+    if p <= 0.0:
+        return torch.ones(rows.numel(), n_cols, device=rows.device)
+    thresh = int(np.float32(p) * np.float32(65536.0) + np.float32(0.5))
+    scale = float(np.float32(1.0) / (np.float32(1.0) - np.float32(p)))
+    flat = rows.reshape(-1, 1).long() * ld + torch.arange(n_cols, device=rows.device).view(1, -1)
+    group = flat >> 2
+    s_lo, s_hi = seed & _M32, (seed >> 32) & _M32
+    x = ((group & _M32) ^ s_lo) + _mul32(group >> 32, 0x85EBCA6B) + ((s_hi * 0x165667B1) & _M32)
+    x = _mul32(x & _M32, 0x9E3779B1)
+    x ^= x >> 15
+    x = _mul32(x, 0x85EBCA77)
+    x ^= x >> 13
+    y = (_mul32(x, 0xC2B2AE3D) + s_hi) & _M32
+    y ^= y >> 16
+    y = _mul32(y, 0x27D4EB2F)
+    y ^= y >> 15
+    lane = flat & 3
+    half = torch.where(lane < 2, x, y)
+    bits = torch.where((lane & 1) == 0, half & 0xFFFF, half >> 16)
+    return torch.where(bits >= thresh, torch.tensor(scale, device=rows.device), torch.tensor(0.0, device=rows.device))
+
+
+def _bf16_ulp(v):
+    """One bf16 ulp at |v| (fp64 tensor); 0 where v == 0."""
+    _, e = torch.frexp(v.abs())
+    return torch.where(v == 0, torch.zeros_like(v), torch.ldexp(torch.ones_like(v), e - 8))
+
+
+def _safe_div(num, den):
+    return torch.where(num == 0, torch.zeros_like(num), num / den.clamp_min(1e-300))
+
+
+def _worst(t):
+    """Largest element of a metric tensor, +inf if any element is NaN (an output the kernels never wrote keeps its NaN
+    pre-fill: it must fail every bound, never drop out of a max)."""
+    return float(torch.nan_to_num(t, nan=float("inf")).max()) if t.numel() else 0.0
+
+
+def _row_ratio(kern, exact, contract, floor=2e-3):
+    """The project's gradient rule applied to each row of 2-D tensors: (|kernel - exact| / |exact|) divided by
+    max(|contract - exact| / |exact|, floor), which must stay <= 1.5.  Returns (worst ratio, relative kernel and contract
+    error of that row); a NaN anywhere makes the ratio +inf."""
+    nx = exact.norm(dim=1)
+    ek = _safe_div((kern - exact).norm(dim=1), nx)
+    ec = _safe_div((contract - exact).norm(dim=1), nx)
+    r = torch.nan_to_num(ek / ec.clamp_min(floor), nan=float("inf"))
+    i = int(r.argmax())
+    return float(r[i]), float(ek[i]), float(ec[i])
+
+
+def _cnn_ids(n_seq, T, V, seed, bad_ids):
+    """MIND-like right-padded titles with ids 0 and V-1 present; bad_ids plants two out-of-range ids (V + 5 and -1)."""
+    ids = O.synth_titles(n_seq, T, V, seed, min_len=1).reshape(-1)
+    n = ids.numel()
+    if n == 0:  # a one-element buffer, so that the ABI sees a valid pointer
+        return torch.zeros(1, dtype=torch.int64, device=DEV)
+    ids[0] = V - 1
+    if n > 2:
+        ids[n - 1] = V - 1
+        ids[n // 2] = 0
+    if bad_ids and n >= 8:
+        ids[n // 3] = V + 5
+        ids[(2 * n) // 3 + 1] = -1
+    return ids.view(n_seq, T).to(DEV)
+
+
+def check_cnn_encoder(n_seq=37, T=20, d=300, F=400, q=200, V=500, p_drop=0.2, accurate=False, seed=1, bad_ids=True, grad_floor=2e-3):
+    """nr_cnn_encoder_fwd / _bwd stage by stage against fp64 references built from the kernels' own stored Xp, Y, w:
+    exact gather, per-element conv output within one bf16 ulp plus an fp32-accumulation allowance, per-segment pooling,
+    per-row gradients under the project's gradient rule (kernel error <= 1.5 x the bf16 contract's, floor grad_floor), every
+    "=" output finite (nothing left at its NaN pre-fill), the pre-fill of every "+=" output outside the rows / columns the
+    kernels own, and the guard behind every buffer."""
+    from newsrec_b200 import CnnEncoderBwdArgs, CnnEncoderFwdArgs
+    lib = load_library()
+    T_p = T + 2
+    ldx, ldf, ldq = ru8(d + 1), ru8(F + 1), ru16(q)
+    n_tok, Mp = n_seq * T, n_seq * T_p
+    # ---- operands, built the way CnnPoolEncoderFn.build does (tap-major conv weight rows, transposed taps for dX)
+    a_w = 0.5 * math.sqrt(3.0 / d)  # pre-activation std ~0.5: with a small centred bias about half of it is positive
+    Wc = _rand_bf16((F, 3, d), seed + 1, a_w).to(DEV)
+    bc = O.det_uniform((F,), seed + 2, -0.05, 0.05).to(DEV)
+    Wa = _rand_bf16((q, F), seed + 3, math.sqrt(3.0 / F)).to(DEV)
+    ba = O.det_uniform((q,), seed + 4, -0.1, 0.1).to(DEV)
+    qv = O.det_uniform((q,), seed + 5, -1.0, 1.0).to(DEV)
+    table_f = _rand_bf16((V, d), seed + 6).to(DEV)
+    wconv = cast_pad(Wc.permute(1, 0, 2).reshape(3 * F, d), ldx)
+    wconvT = cast_pad(torch.cat([Wc[:, 2 - s, :].t() for s in range(3)], 0), ldf)
+    wa, waT, table = cast_pad(Wa, ldf), cast_pad(Wa, ldq, transpose=True), cast_pad(table_f, ldx)
+    ids = _cnn_ids(n_seq, T, V, seed + 7, bad_ids)
+    kseed = (0x9E3779B97F4A7C15 * (seed + 11)) & 0xFFFFFFFFFFFFFFFF
+
+    def forward():
+        bufs = dict(Xp=_Guarded(Mp * ldx, torch.bfloat16, float("nan")), Y=_Guarded(n_tok * ldf, torch.bfloat16, float("nan")),
+                    w=_Guarded(n_tok, torch.float32, float("nan")), out=_Guarded(n_seq * F, torch.float32, float("nan")),
+                    flag=_Guarded(1, torch.int32, 0, sentinel=-7))
+        if accurate:
+            bufs["Ylo"] = _Guarded(n_tok * ldf, torch.bfloat16, float("nan"))
+        a = CnnEncoderFwdArgs()
+        a.n_seq, a.T, a.d, a.F, a.q, a.ldx, a.ldf = n_seq, T, d, F, q, ldx, ldf
+        a.ids, a.table_bf16, a.V = _p(ids), _p(table), V
+        a.wconv_bf16, a.bconv, a.wa_bf16, a.ba, a.qv = _p(wconv), _p(bc), _p(wa), _p(ba), _p(qv)
+        a.p_drop, a.seed = float(p_drop), kseed
+        a.Xp_bf16, a.Y_bf16, a.w, a.out = _p(bufs["Xp"].all), _p(bufs["Y"].all), _p(bufs["w"].all), _p(bufs["out"].all)
+        a.bad_id_flag = _p(bufs["flag"].all)
+        if accurate:
+            a.Y_lo_bf16 = _p(bufs["Ylo"].all)
+        n0 = int(lib.nr_launch_count())
+        check(lib.nr_cnn_encoder_fwd(C.byref(a), _stream()), "nr_cnn_encoder_fwd")
+        return bufs, int(lib.nr_launch_count()) - n0
+
+    fb, fwd_launches = forward()
+    dout = O.det_uniform((max(n_seq, 1), F), seed + 8).to(DEV)
+    pat = lambda n, s: O.det_uniform((n,), s, 0.5, 1.0).to(DEV) * 2.0 ** -16  # small non-zero "+=" pre-fill
+    bb = dict(dWc=_Guarded(3 * F * ldx, torch.float32, pat(3 * F * ldx, seed + 20)),
+              dWa=_Guarded(q * ldf, torch.float32, pat(q * ldf, seed + 21)),
+              dqv=_Guarded(q, torch.float32, pat(q, seed + 22)), demb=_Guarded(V * d, torch.float32, pat(V * d, seed + 23)))
+    ws_bytes = int(lib.nr_cnn_encoder_bwd_workspace(n_seq, T, F, q))
+    ws = _Guarded(ws_bytes, torch.uint8, 0xFF, sentinel=0xA5)  # 0xFFFF.. = NaN in bf16 and fp32: unwritten rows poison results
+    b = CnnEncoderBwdArgs()
+    b.n_seq, b.T, b.d, b.F, b.q, b.ldx, b.ldf, b.ldq = n_seq, T, d, F, q, ldx, ldf, ldq
+    b.ids, b.V = _p(ids), V
+    b.wconvT_bf16, b.wa_bf16, b.waT_bf16, b.ba, b.qv = _p(wconvT), _p(wa), _p(waT), _p(ba), _p(qv)
+    b.p_drop, b.seed = float(p_drop), kseed
+    b.Xp_bf16, b.Y_bf16, b.w, b.dout = _p(fb["Xp"].all), _p(fb["Y"].all), _p(fb["w"].all), _p(dout)
+    b.dWconv_ext, b.dWa_ext, b.dqv, b.demb = _p(bb["dWc"].all), _p(bb["dWa"].all), _p(bb["dqv"].all), _p(bb["demb"].all)
+    b.workspace, b.workspace_bytes = _p(ws.all), ws_bytes
+    n0 = int(lib.nr_launch_count())
+    check(lib.nr_cnn_encoder_bwd(C.byref(b), _stream()), "nr_cnn_encoder_bwd")
+    bwd_launches = int(lib.nr_launch_count()) - n0
+    torch.cuda.synchronize()
+    res = {"fwd_launches": fwd_launches, "bwd_launches": bwd_launches,
+           "guards_intact": all(g.guard_ok() for g in list(fb.values()) + list(bb.values()) + [ws])}
+    del ws
+    if n_seq == 0:
+        return res
+    res["bad_id_flag"] = int(fb["flag"].body.item())
+    ids_flat = ids.reshape(-1)
+    bad = (ids_flat < 0) | (ids_flat >= V)
+    res["bad_ids_planted"] = int(bad.sum())
+    # every "=" output is written where the ABI says it is (Y_lo: columns [0, F))
+    res["fwd_outputs_finite"] = all(bool(torch.isfinite(fb[k].body.float()).all()) for k in ("Xp", "Y", "w", "out")) and \
+        (not accurate or bool(torch.isfinite(fb["Ylo"].body.view(n_tok, ldf)[:, :F].float()).all()))
+
+    # ---- fp64 references, a chunk of about 8k padded rows at a time (a few hundred MB of fp64 temporaries at any n_seq)
+    Xp3 = fb["Xp"].body.view(n_seq, T_p, ldx)
+    Y2 = fb["Y"].body.view(n_tok, ldf)
+    Ylo2 = fb["Ylo"].body.view(n_tok, ldf) if accurate else None
+    w1, out2 = fb["w"].body, fb["out"].body.view(n_seq, F)
+    W64 = Wc.double().permute(1, 0, 2).contiguous()  # (3, F, d)
+    Wa64, ba64, qv64, bc64 = Wa.double(), ba.double(), qv.double(), bc.double()
+    scale = float(1.0 / (1.0 - torch.tensor(p_drop, dtype=torch.float32))) if p_drop > 0 else 1.0  # the kernels' fp32 1/(1-p)
+    ids_safe = torch.where(bad, torch.zeros_like(ids_flat), ids_flat)
+    scat = (ids_flat >= 1) & (ids_flat < V)
+    acc = {k: 0.0 for k in ("y_ratio", "ylo_ratio", "w_err", "w_sum_err", "out_ratio", "t1_w_err", "t1_out_ratio")}
+    worst = lambda k, t: acc.__setitem__(k, max(acc[k], _worst(t)))
+    cnt = dict(xp_mismatch_rows=0, y_dropped_nonzero=0, y_pos=0, y_n=0)
+    ones_ok = True
+    grads = {v: dict(dWc=torch.zeros(3, F, d + 1, dtype=torch.float64, device=DEV),
+                     dWa=torch.zeros(q, F + 1, dtype=torch.float64, device=DEV),
+                     dqv=torch.zeros(q, dtype=torch.float64, device=DEV),
+                     demb=torch.zeros(V, d, dtype=torch.float64, device=DEV)) for v in ("exact", "contract")}
+    cs = max(1, 8192 // T_p)
+    for s0 in range(0, n_seq, cs):
+        s1 = min(n_seq, s0 + cs)
+        ns = s1 - s0
+        r0, r1 = s0 * T, s1 * T
+        seg = torch.arange(s0, s1, device=DEV)
+        tok_rows = (seg.view(-1, 1) * T_p + 1 + torch.arange(T, device=DEV).view(1, -1)).reshape(-1)  # padded rows of tokens
+        # Xp: masked gather of the bf16 table rows, ones column at d, zeros behind it, zero pad rows -- bit exact
+        mx = dropout_mask_dev(kseed, p_drop, tok_rows, d, ldx)
+        exp_x = torch.zeros(ns, T_p, ldx, dtype=torch.float32, device=DEV)
+        exp_x[:, 1:T + 1, :d] = ((table_f[ids_safe[r0:r1]] * mx).to(torch.bfloat16).float()).view(ns, T, d)
+        exp_x[:, 1:T + 1, d] = 1.0
+        got_x = Xp3[s0:s1]
+        cnt["xp_mismatch_rows"] += int((got_x.view(torch.int16) != exp_x.to(torch.bfloat16).view(torch.int16)).any(dim=2).sum())
+        X64 = got_x.double()
+        # conv: pre[s, t] = sum_k Xp[s, t + k] . W_k + b, and the sum of |products| for the accumulation allowance
+        pre = torch.zeros(ns * T, F, dtype=torch.float64, device=DEV) + bc64
+        absum = torch.zeros(ns * T, F, dtype=torch.float64, device=DEV) + bc64.abs()
+        for k in range(3):
+            xk = X64[:, k:k + T, :d].reshape(-1, d)
+            pre += xk @ W64[k].t()
+            absum += xk.abs() @ W64[k].abs().t()
+        my = dropout_mask_dev(kseed ^ 0x5BD1E995, p_drop, torch.arange(r0, r1, device=DEV), F, ldf).double()
+        ref_y = pre.clamp_min(0) * my
+        y = Y2[r0:r1]
+        y64 = y[:, :F].double()
+        bound = _bf16_ulp(torch.maximum(ref_y.abs(), y64.abs())) + 1e-6 * absum * my.clamp_min(1.0)
+        worst("y_ratio", _safe_div((y64 - ref_y).abs(), bound))
+        cnt["y_dropped_nonzero"] += int(((my == 0) & (y64 != 0)).sum())
+        cnt["y_pos"] += int((pre > 0).sum())
+        cnt["y_n"] += pre.numel()
+        ones_ok &= bool((y[:, F] == 1).all()) and bool((y[:, F + 1:] == 0).all())
+        yy = y64
+        if accurate:
+            yy = y64 + Ylo2[r0:r1, :F].double()
+            rb = 2.0 ** -16 * ref_y.norm(dim=1) + 1e-6 * (absum * my).norm(dim=1)
+            worst("ylo_ratio", _safe_div((yy - ref_y).norm(dim=1), rb))
+        # pooling from the kernel's own Y: fp64 tanh scores, softmax per segment, weighted sum of Y (+ Y_lo)
+        score = torch.tanh(y64 @ Wa64.t() + ba64) @ qv64
+        w_ref = torch.softmax(score.view(ns, T), dim=1)
+        wk = w1[r0:r1].double().view(ns, T)
+        worst("w_err", (wk - w_ref).abs())
+        worst("w_sum_err", (wk.sum(1) - 1).abs())
+        yy3 = yy.view(ns, T, F)
+        o_ref = (wk.unsqueeze(2) * yy3).sum(1)
+        o_abs = (wk.unsqueeze(2) * yy3.abs()).sum(1)
+        o_got = out2[s0:s1].double()
+        worst("out_ratio", _safe_div((o_got - o_ref).norm(dim=1), o_abs.norm(dim=1)))
+        if T == 1:
+            worst("t1_w_err", (wk - 1).abs())
+            worst("t1_out_ratio", _safe_div((o_got - yy).abs(), yy.abs() * 2.0 ** -23))
+        # ---- backward, exact and under the bf16 contract (dPre and dY stored in bf16)
+        do = dout[s0:s1].double()
+        dw = (y64.view(ns, T, F) * do.unsqueeze(1)).sum(2)
+        dscore = wk * (dw - (wk * dw).sum(1, keepdim=True))
+        th = torch.tanh(y64 @ Wa64.t() + ba64)
+        dpre = dscore.reshape(-1, 1) * qv64 * (1 - th * th)
+        dqv_c = (dscore.reshape(-1, 1) * th).sum(0)
+        relu_keep = (y64 > 0).double() * scale
+        xs = X64[:, :, :d + 1].reshape(-1, d + 1)
+        y1 = torch.cat([y64, torch.ones(ns * T, 1, dtype=torch.float64, device=DEV)], 1)
+        sc_ids = ids_flat[r0:r1][scat[r0:r1]]
+        for v in ("exact", "contract"):
+            dp = dpre if v == "exact" else bf16r(dpre.float()).double()
+            dyc = (dp @ Wa64 + wk.reshape(-1, 1) * do.repeat_interleave(T, 0)) * relu_keep
+            if v == "contract":
+                dyc = bf16r(dyc.float()).double()
+            g = grads[v]
+            g["dqv"] += dqv_c
+            g["dWa"] += dp.t() @ y1
+            dyp = torch.zeros(ns, T_p, F, dtype=torch.float64, device=DEV)
+            dyp[:, 1:T + 1] = dyc.view(ns, T, F)
+            dyp = dyp.view(-1, F)
+            n_p = dyp.shape[0]
+            for k in range(3):  # dW_k += dY^T . X[rows + k - 1]; dX[r] += dY[r - k + 1] . W_k
+                sh = k - 1
+                xsh = torch.zeros_like(xs)
+                dys = torch.zeros_like(dyp)
+                if sh >= 0:
+                    xsh[:n_p - sh] = xs[sh:]
+                    dys[sh:] = dyp[:n_p - sh]
+                else:
+                    xsh[-sh:] = xs[:n_p + sh]
+                    dys[:n_p + sh] = dyp[-sh:]
+                g["dWc"][k] += dyp.t() @ xsh
+                dX = dys @ W64[k] if k == 0 else dX + dys @ W64[k]
+            dXt = dX.view(ns, T_p, d)[:, 1:T + 1].reshape(-1, d) * mx.double()
+            g["demb"].index_add_(0, sc_ids, dXt[scat[r0:r1]])
+    res.update({k: v for k, v in acc.items()})
+    res.update(cnt)
+    res["y_pos_fraction"] = cnt["y_pos"] / max(1, cnt["y_n"])
+    res["y_ones_col_and_pad_exact"] = ones_ok
+    # ---- gradients: per row, kernel vs exact against contract vs exact
+    ex, co = grads["exact"], grads["contract"]
+    dWc_k = (bb["dWc"].body.double() - bb["dWc"].prefill.double()).view(3, F, ldx)[:, :, :d + 1]
+    dWa_k = (bb["dWa"].body.double() - bb["dWa"].prefill.double()).view(q, ldf)[:, :F + 1]
+    dqv_k = bb["dqv"].body.double() - bb["dqv"].prefill.double()
+    demb_k = (bb["demb"].body.double() - bb["demb"].prefill.double()).view(V, d)
+    res["dWconv_row_ratio"], res["dWconv_ek"], res["dWconv_ec"] = _row_ratio(*[t.reshape(3 * F, -1) for t in (dWc_k, ex["dWc"], co["dWc"])],
+                                                                            floor=grad_floor)
+    res["dWa_row_ratio"], res["dWa_ek"], res["dWa_ec"] = _row_ratio(dWa_k, ex["dWa"], co["dWa"], floor=grad_floor)
+    res["dqv_ratio"], res["dqv_ek"], res["dqv_ec"] = _row_ratio(*[t.view(1, -1) for t in (dqv_k, ex["dqv"], co["dqv"])], floor=grad_floor)
+    touched = torch.zeros(V, dtype=torch.bool, device=DEV)
+    touched[ids_flat[scat]] = True
+    res["demb_rows_touched"] = int(touched.sum())
+    res["demb_row_ratio"], res["demb_ek"], res["demb_ec"] = _row_ratio(demb_k[touched], ex["demb"][touched], co["demb"][touched],
+                                                                       floor=grad_floor)
+    # what a whole-tensor norm would have said about the same outputs (for comparison only)
+    res["dWconv_tensor_relerr"] = relerr(dWc_k, ex["dWc"])
+    res["demb_tensor_relerr"] = relerr(demb_k, ex["demb"])
+    # ---- the pre-fill outside what the kernels own: pitch columns, untouched embedding rows (row 0, unused ids)
+    colmask = torch.zeros(3, F, ldx, dtype=torch.bool, device=DEV)
+    colmask[:, :, d + 1:] = True
+    res["dWconv_pitch_cols_untouched"] = bb["dWc"].unchanged(colmask)
+    colmask = torch.zeros(q, ldf, dtype=torch.bool, device=DEV)
+    colmask[:, F + 1:] = True
+    res["dWa_pitch_cols_untouched"] = bb["dWa"].unchanged(colmask)
+    res["demb_untouched_rows_exact"] = bb["demb"].unchanged((~touched).view(V, 1).expand(V, d))
+    if T == 1:  # dscore = w (dw - w dw) vanishes: dqv and dWa_ext keep their pre-fill
+        res["t1_dqv_rel"] = _worst(dqv_k.abs() / bb["dqv"].prefill.double())
+        res["t1_dWa_rel"] = _worst(dWa_k.abs() / bb["dWa"].prefill.double().view(q, ldf)[:, :F + 1])
+    del grads, ex, co, dWc_k, dWa_k, dqv_k, demb_k, bb
+
+    # ---- determinism: a second forward is bit-identical (run last, when the references are freed)
+    fb2, _ = forward()
+    torch.cuda.synchronize()
+    res["fwd_deterministic"] = all(_bits_equal(fb[k].body, fb2[k].body) for k in fb if k != "flag")
+    return res
+
+
+# ------------------------------------------------------------------------------------------------
+def _abs_allow_rows(got, ref, absref):
+    """max over rows of |got - ref| / |absref| (row norms): fp32 accumulation error against the sum of |products|."""
+    return _worst(_safe_div((got - ref).norm(dim=1), absref.norm(dim=1)))
+
+
+def check_element_encoder(n=512 * 55, E=100, F=400, V=300, seed=3):
+    """NAML category / subcategory encoder relu(Linear(embedding(id))) through nr_element_encoder_fwd / _bwd: exact gather,
+    fp32 output per element, the ReLU mask the backward takes from the fp32 output (bit-exact dY), the bias column of dW_ext
+    and the dtable scatter (row 0 and out-of-range ids skipped, repeated ids summed) per row."""
+    lib = load_library()
+    lde, ldf = ru8(E + 1), ru8(F + 1)
+    table_f = _rand_bf16((V, E), seed).to(DEV)
+    W = _rand_bf16((F, E), seed + 1, math.sqrt(3.0 / E)).to(DEV)
+    bias = O.det_uniform((F,), seed + 2, -0.3, 0.3).to(DEV)
+    ids = O.det_randint((n,), seed + 3, 0, V)
+    ids[0], ids[-1] = 0, V - 1
+    if n >= 8:
+        ids[n // 3], ids[n // 2] = V + 5, -1
+    ids = ids.to(DEV)
+    table, w, wT = cast_pad(table_f, lde), cast_pad(W, lde), cast_pad(W, ldf, transpose=True)
+    Eb = _Guarded(n * lde, torch.bfloat16, float("nan"))
+    out = _Guarded(n * F, torch.float32, float("nan"))
+    flag = _Guarded(1, torch.int32, 0, sentinel=-7)
+    check(lib.nr_element_encoder_fwd(_p(ids), n, _p(table), V, E, lde, _p(Eb.all), _p(w), F, _p(bias), _p(out.all), _p(flag.all),
+                                     _stream()), "nr_element_encoder_fwd")
+    bad = (ids < 0) | (ids >= V)
+    safe = torch.where(bad, torch.zeros_like(ids), ids)
+    exp_e = torch.zeros(n, lde, device=DEV)
+    exp_e[:, :E] = table_f[safe]
+    exp_e[:, E] = 1.0
+    e64 = Eb.body.view(n, lde)[:, :E].double()
+    pre = e64 @ W.double().t() + bias.double()
+    ref = pre.clamp_min(0)
+    absum = e64.abs() @ W.double().abs().t() + bias.double().abs()
+    o = out.body.view(n, F)
+    res = {"gather_exact": _bits_equal(Eb.body.view(n, lde), exp_e.to(torch.bfloat16)), "bad_id_flag": int(flag.body.item()),
+           "out_elem_ratio": _worst(_safe_div((o.double() - ref).abs(), 1e-6 * absum)),
+           "relu_zero_exact": bool((o[pre < -1e-5 * absum] == 0).all())}
+    dout = O.det_uniform((n, F), seed + 4).to(DEV)
+    dY = _Guarded(n * ldf, torch.bfloat16, float("nan"))
+    pat = lambda m, s: O.det_uniform((m,), s, 0.5, 1.0).to(DEV) * 2.0 ** -16
+    dW = _Guarded(F * lde, torch.float32, pat(F * lde, seed + 5))
+    dt = _Guarded(V * E, torch.float32, pat(V * E, seed + 6))
+    check(lib.nr_element_encoder_bwd(_p(ids), n, _p(dout), _p(out.all), F, _p(dY.all), ldf, _p(Eb.all), E, lde, _p(wT), _p(dW.all),
+                                     _p(dt.all), V, _stream()), "nr_element_encoder_bwd")
+    torch.cuda.synchronize()
+    exp_dy = torch.zeros(n, ldf, device=DEV)
+    exp_dy[:, :F] = torch.where(o > 0, dout, torch.zeros_like(dout))  # the kernel writes +0 where the ReLU was off
+    res["dY_relu_mask_exact"] = _bits_equal(dY.body.view(n, ldf), exp_dy.to(torch.bfloat16))
+    dy64 = dY.body.view(n, ldf)[:, :F].double()
+    e1 = torch.cat([e64, torch.ones(n, 1, dtype=torch.float64, device=DEV)], 1)
+    dW_k = dW.body.view(F, lde)[:, :E + 1].double() - dW.prefill.view(F, lde)[:, :E + 1].double()
+    res["dW_row_ratio"] = _abs_allow_rows(dW_k, dy64.t() @ e1, dy64.abs().t() @ e1.abs())
+    res["dW_bias_col_ratio"] = _worst(_safe_div((dW_k[:, E] - dy64.sum(0)).abs(), dy64.abs().sum(0)))
+    colmask = torch.zeros(F, lde, dtype=torch.bool, device=DEV)
+    colmask[:, E + 1:] = True
+    res["dW_pitch_cols_untouched"] = dW.unchanged(colmask)
+    scat = (ids >= 1) & (ids < V)
+    dX = dy64 @ W.double()
+    ref_t = torch.zeros(V, E, dtype=torch.float64, device=DEV).index_add_(0, ids[scat], dX[scat])
+    abs_t = torch.zeros(V, E, dtype=torch.float64, device=DEV).index_add_(0, ids[scat], (dy64.abs() @ W.double().abs())[scat])
+    touched = torch.zeros(V, dtype=torch.bool, device=DEV)
+    touched[ids[scat]] = True
+    dt_k = dt.body.view(V, E).double() - dt.prefill.view(V, E).double()
+    res["dtable_row_ratio"] = _abs_allow_rows(dt_k[touched], ref_t[touched], abs_t[touched])
+    res["dtable_untouched_rows_exact"] = dt.unchanged((~touched).view(V, 1).expand(V, E))
+    res["guards_intact"] = all(g.guard_ok() for g in (Eb, out, flag, dY, dW, dt))
+    return res
+
+
+def check_linear_rows(n=4000, K=300, N=275, relu=1, strided=False, with_dx=True, seed=5):
+    """nr_linear_rows_fwd / _bwd (TANR topic predictor, GRU projections): bf16 operand rows (exact), fp32 output per element,
+    masked bf16 dY (exact), dW_ext per row with its bias column (K + 1 > 512 columns are split across two weight-gradient
+    calls), dx per element, or dx = NULL."""
+    lib = load_library()
+    ldx, ldn = ru8(K + 1), ru8(N + 1)
+    ld_out = (N + 3) // 4 * 4
+    base = O.det_uniform((n, 2 * K if strided else K), seed).to(DEV)
+    x = base[:, ::2] if strided else base  # strided: element stride 2 inside a row
+    W = _rand_bf16((N, K), seed + 1, math.sqrt(3.0 / K)).to(DEV)
+    bias = O.det_uniform((N,), seed + 2, -0.2, 0.2).to(DEV)
+    w, wT = cast_pad(W, ldx), cast_pad(W, ldn, transpose=True)
+    X = _Guarded(n * ldx, torch.bfloat16, float("nan"))
+    out = _Guarded(n * ld_out, torch.float32, float("nan"))
+    check(lib.nr_linear_rows_fwd(_p(x), n, K, x.stride(0), x.stride(1), _p(X.all), ldx, _p(w), N, ldx, _p(bias), relu, _p(out.all),
+                                 ld_out, _stream()), "nr_linear_rows_fwd")
+    exp_x = torch.zeros(n, ldx, device=DEV)
+    exp_x[:, :K] = x
+    exp_x[:, K] = 1.0
+    x64 = X.body.view(n, ldx)[:, :K].double()
+    pre = x64 @ W.double().t() + bias.double()
+    ref = pre.clamp_min(0) if relu else pre
+    absum = x64.abs() @ W.double().abs().t() + bias.double().abs()
+    o = out.body.view(n, ld_out)[:, :N]
+    res = {"x_rows_exact": _bits_equal(X.body.view(n, ldx), exp_x.to(torch.bfloat16)),
+           "out_elem_ratio": _worst(_safe_div((o.double() - ref).abs(), 1e-6 * absum))}
+    dy = _Guarded(n * ld_out, torch.float32, 0.0)
+    dy.body.view(n, ld_out)[:, :N] = O.det_uniform((n, N), seed + 3).to(DEV)
+    dY = _Guarded(n * ldn, torch.bfloat16, float("nan"))
+    dW = _Guarded(N * ldx, torch.float32, O.det_uniform((N * ldx,), seed + 4, 0.5, 1.0).to(DEV) * 2.0 ** -16)
+    ld_dx = (K + 3) // 4 * 4
+    dx = _Guarded(n * ld_dx, torch.float32, float("nan")) if with_dx else None
+    check(lib.nr_linear_rows_bwd(_p(dy.all), _p(out.all) if relu else None, n, N, ld_out, _p(dY.all), ldn, _p(X.all), K, ldx, _p(wT),
+                                 ldn, _p(dW.all), _p(dx.all) if with_dx else None, ld_dx, _stream()), "nr_linear_rows_bwd")
+    torch.cuda.synchronize()
+    g = dy.body.view(n, ld_out)[:, :N]
+    exp_dy = torch.zeros(n, ldn, device=DEV)
+    exp_dy[:, :N] = torch.where(o > 0, g, torch.zeros_like(g)) if relu else g
+    res["dY_exact"] = _bits_equal(dY.body.view(n, ldn), exp_dy.to(torch.bfloat16))
+    dy64 = dY.body.view(n, ldn)[:, :N].double()
+    x1 = torch.cat([x64, torch.ones(n, 1, dtype=torch.float64, device=DEV)], 1)
+    dW_k = dW.body.view(N, ldx)[:, :K + 1].double() - dW.prefill.view(N, ldx)[:, :K + 1].double()
+    res["dW_row_ratio"] = _abs_allow_rows(dW_k, dy64.t() @ x1, dy64.abs().t() @ x1.abs())
+    res["dW_bias_col_ratio"] = _worst(_safe_div((dW_k[:, K] - dy64.sum(0)).abs(), dy64.abs().sum(0)))
+    colmask = torch.zeros(N, ldx, dtype=torch.bool, device=DEV)
+    colmask[:, K + 1:] = True
+    res["dW_pitch_cols_untouched"] = dW.unchanged(colmask)
+    if with_dx:
+        dxk = dx.body.view(n, ld_dx)[:, :K].double()
+        res["dx_elem_ratio"] = _worst(_safe_div((dxk - dy64 @ W.double()).abs(), 1e-6 * (dy64.abs() @ W.double().abs())))
+    res["guards_intact"] = all(b.guard_ok() for b in (X, out, dy, dY, dW) + ((dx,) if with_dx else ()))
+    return res
+
+
+def check_embedding_f32(n=512 * 55, V=300, D=100, seed=7):
+    """nr_embedding_f32_fwd / _bwd (LSTUR category and user embeddings): the lookup is bit exact (out-of-range ids read row 0
+    and raise the flag); the backward adds each touched row's fp64 sum, leaves row 0 and unused rows bit-identical."""
+    lib = load_library()
+    table = O.det_uniform((V, D), seed).to(DEV)
+    ids = O.det_randint((n,), seed + 1, 0, V)
+    ids[0], ids[-1] = 0, V - 1
+    if n >= 8:
+        ids[n // 3], ids[n // 2] = V + 5, -1
+    ids = ids.to(DEV)
+    out = _Guarded(n * D, torch.float32, float("nan"))
+    flag = _Guarded(1, torch.int32, 0, sentinel=-7)
+    check(lib.nr_embedding_f32_fwd(_p(ids), n, _p(table), V, D, _p(out.all), _p(flag.all), _stream()), "nr_embedding_f32_fwd")
+    bad = (ids < 0) | (ids >= V)
+    safe = torch.where(bad, torch.zeros_like(ids), ids)
+    res = {"fwd_exact": _bits_equal(out.body.view(n, D), table[safe]), "bad_id_flag": int(flag.body.item())}
+    dout = O.det_uniform((n, D), seed + 2).to(DEV)
+    dt = _Guarded(V * D, torch.float32, O.det_uniform((V * D,), seed + 3, 0.5, 1.0).to(DEV) * 2.0 ** -16)
+    check(lib.nr_embedding_f32_bwd(_p(ids), n, _p(dout), V, D, _p(dt.all), _stream()), "nr_embedding_f32_bwd")
+    torch.cuda.synchronize()
+    scat = (ids >= 1) & (ids < V)
+    ref = torch.zeros(V, D, dtype=torch.float64, device=DEV).index_add_(0, ids[scat], dout[scat].double())
+    absr = torch.zeros(V, D, dtype=torch.float64, device=DEV).index_add_(0, ids[scat], dout[scat].double().abs())
+    touched = torch.zeros(V, dtype=torch.bool, device=DEV)
+    touched[ids[scat]] = True
+    dk = dt.body.view(V, D).double() - dt.prefill.view(V, D).double()
+    res["bwd_row_ratio"] = _abs_allow_rows(dk[touched], ref[touched], absr[touched])
+    res["untouched_rows_exact"] = dt.unchanged((~touched).view(V, 1).expand(V, D))
+    res["row0_untouched"] = not bool(touched[0])
+    res["guards_intact"] = all(b.guard_ok() for b in (out, flag, dt))
+    return res

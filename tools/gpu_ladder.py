@@ -59,6 +59,17 @@ CHECKS = {
     "nrms_eval_api": ("check_nrms_eval_api", {}),
     "nrms_train_mode": ("check_nrms_train_mode", {}),
     "nrms_full_size": ("check_nrms_full_size_properties", {}),
+    "cnn_naml_title_full": ("check_cnn_encoder", dict(n_seq=512 * 55, T=20, d=300, F=400, q=200, V=70976, p_drop=0.2)),
+    "cnn_naml_abstract": ("check_cnn_encoder", dict(n_seq=128 * 55, T=50, d=300, F=400, q=200, V=5000, p_drop=0.2)),
+    "cnn_lstur_accurate": ("check_cnn_encoder", dict(n_seq=2000, T=20, d=300, F=300, q=200, V=3000, accurate=True)),
+    "cnn_tanr_eval": ("check_cnn_encoder", dict(n_seq=2000, T=20, d=300, F=400, q=200, V=3000, p_drop=0.0)),
+    "cnn_t1": ("check_cnn_encoder", dict(n_seq=999, T=1, d=300, F=300, q=200, V=3000)),
+    "cnn_t64": ("check_cnn_encoder", dict(n_seq=97, T=64, d=300, F=300, q=200, V=3000)),
+    "cnn_f8_q16": ("check_cnn_encoder", dict(n_seq=613, T=20, d=64, F=8, q=16, V=37, p_drop=0.5)),
+    "element_encoder": ("check_element_encoder", dict(n=512 * 55, E=100, F=400)),
+    "linear_rows_topic": ("check_linear_rows", dict(n=512 * 5, K=300, N=275, relu=1)),
+    "linear_rows_k900": ("check_linear_rows", dict(n=777, K=900, N=300, relu=1, strided=True)),
+    "embedding_f32": ("check_embedding_f32", dict(n=512 * 55, V=300, D=100)),
 }
 
 
