@@ -9,7 +9,6 @@
 // bf16 storage contract (mirrored by the oracle): A and dS are rounded to bf16 as tensor-core operands,
 // all softmax arithmetic is fp32.
 #include <algorithm>
-#include <cstdlib>
 
 #include "nr_common.cuh"
 #include "nr_mma.cuh"
@@ -28,6 +27,14 @@ constexpr int kPitch24 = 24; // fixed-shape d_k = 20 kernels: 48-byte rows (also
                              // quads); the second k-step over d_k is then an m16n8k8 MMA over columns 16..23 (20..23 stay zero).
                              // 40 % less shared memory per tile -> 4 instead of 3 resident CTAs (backward), 6 instead of 5 (forward):
                              // the kernels are latency bound (25-36 % issue-active under ncu), residency is what they lack.
+constexpr int kWarps = 4;    // warps per CTA
+constexpr int kStages = 2;   // tasks in flight per copy ring
+// Rows of a tile: 32 for the per-warp kernels (T <= 32), 64 for the cooperative ones (32 < T <= 64).
+__host__ __device__ constexpr int tile_rows(bool coop) { return coop ? 64 : 32; }
+// The reference's head shape (config.py: 15 heads x 20), at the sequence length each schedule sees in the reference:
+// 20 title words (per-warp kernels, dense-section callers) and 50 clicked news (cooperative kernels, user encoder).
+constexpr int kFixedDk = 20, kFixedHeads = 15;
+__host__ __device__ constexpr int fixed_T(bool coop) { return coop ? 50 : 20; }
 
 // A fragment (16 x 16) of a row-major [row][k] tile:           rows row0.., k columns k0..
 __device__ __forceinline__ void load_a(uint32_t* a, const __nv_bfloat16* tile, int pitch, int row0, int k0, int lane) {
@@ -283,52 +290,60 @@ __host__ __device__ inline int piece_bytes(int dk, int ld_a, int ld_b, int d) {
     if ((dk % 2) == 0 && (ld_a % 2) == 0 && (ld_b % 2) == 0 && (d % 2) == 0) return 4;
     return 2;
 }
+// the backward also stores dQ | dK | dV rows of pitch ld_out in pieces
+__host__ __device__ inline int piece_bytes_bwd(int dk, int ld_a, int ld_b, int d, int ld_out) {
+    const int piece = piece_bytes(dk, ld_a, ld_b, d);
+    return (piece == 8 && (ld_out % 4) == 0) ? 8 : ((piece >= 4 && (ld_out % 2) == 0) ? 4 : 2);
+}
 
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-// CT/CDK/CH > 0 pin the sequence length, head width and head count at compile time (8-byte pieces guaranteed by the
-// launcher): every shape guard, the piece plan and the task -> (sequence, head) division fold away.  ncu on the run-time
-// shaped kernel: 1200 warp instructions per 20x20 head, 650 of them integer/predicate/branch overhead.
-// COOP (history-level attention, T > 32): the WPS = TP/16 warps of a CTA share ONE task -- warp w owns the 16-row block w
-// -- instead of walking private tasks: 512 sequences x 15 heads are only 7,680 tasks, and one warp per 50x50 head left
-// 3 warps per SM resident (0.28 ms for 4 % of the tokens).  Tiles are loaded/stored by all threads, phases are separated
-// by __syncthreads instead of __syncwarp.
-template <int TP, int KSD, int NTD, int STG, int WPS, bool FAST, int CT, int CDK, int CH, bool COOP>
-__global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (COOP ? 3 : 1))) mhsa_mma_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, int sec, long long n_seq,
+// Template parameters:
+//   NTD   8-column n-tiles over d_k (2: d_k <= 16, 3: <= 24, 4: <= 32); KSD = 16-wide k-steps over d_k.
+//   FAST  per-lane copy plans (PieceMap) instead of the copy loops.
+//   FIXED the reference's head shape (T = fixed_T(COOP), d_k 20, 15 heads) at compile time (8-byte pieces guaranteed by
+//         the launcher): every shape guard, the piece plan and the task -> (sequence, head) division fold away.  ncu on
+//         the run-time shaped kernel: 1200 warp instructions per 20x20 head, 650 of them integer/predicate/branch overhead.
+//   COOP  history-level attention (T > 32): the kWarps = TP/16 warps of a CTA share ONE task -- warp w owns the 16-row
+//         block w -- instead of walking private tasks: 512 sequences x 15 heads are only 7,680 tasks, and one warp per
+//         50x50 head left 3 warps per SM resident (0.28 ms for 4 % of the tokens).  Tiles are loaded/stored by all
+//         threads, phases are separated by __syncthreads instead of __syncwarp.
+template <int NTD, bool FAST, bool FIXED, bool COOP>
+__global__ void __launch_bounds__(kWarps * 32, COOP ? 3 : (FIXED ? 8 : 5)) mhsa_mma_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, int sec, long long n_seq,
                                                                   int T_, int heads_, int dk_, __nv_bfloat16* __restrict__ ctx,
                                                                   int ld_ctx, float p, uint64_t seed) {
-    constexpr int NTJ = TP / 8, MT = TP / 16;
-    constexpr int PT = (CDK == 20) ? kPitch24 : kPitch;  // tile row pitch
-    constexpr bool K8T = (CDK == 20);                    // last k-step over d_k is an m16n8k8 (columns 16..23)
+    constexpr int TP = tile_rows(COOP), NTJ = TP / 8, MT = TP / 16, KSD = (NTD + 1) / 2;
+    constexpr int CT = FIXED ? fixed_T(COOP) : 0;
+    constexpr int PT = FIXED ? kPitch24 : kPitch;  // tile row pitch
+    constexpr bool K8T = FIXED;                    // last k-step over d_k is an m16n8k8 (columns 16..23)
     constexpr int KS16 = K8T ? KSD - 1 : KSD;
-    const int T = CT > 0 ? CT : T_, heads = CH > 0 ? CH : heads_, dk = CDK > 0 ? CDK : dk_;
+    const int T = FIXED ? CT : T_, heads = FIXED ? kFixedHeads : heads_, dk = FIXED ? kFixedDk : dk_;
     // A tile holds exactly T rows (pitch PT).  Fragment loads of rows >= T run into the neighbouring tile or the
     // zeroed slack behind the last one: finite bytes that only ever meet zero probabilities / unused output rows.
     const int TILE = T * PT;
     extern __shared__ __align__(16) __nv_bfloat16 sm[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
     const int d = heads * dk;
-    static_assert(!COOP || (WPS == TP / 16 && !FAST), "cooperative CTAs: one warp per 16-row block, generic copy loops");
-    for (int i = tid; i < ((COOP ? 1 : WPS) * STG * 3 * TILE + (TP - T) * PT) / 2; i += blockDim.x) reinterpret_cast<uint32_t*>(sm)[i] = 0u;
+    static_assert(!COOP || (kWarps == TP / 16 && !FAST), "cooperative CTAs: one warp per 16-row block, generic copy loops");
+    for (int i = tid; i < ((COOP ? 1 : kWarps) * kStages * 3 * TILE + (TP - T) * PT) / 2; i += blockDim.x) reinterpret_cast<uint32_t*>(sm)[i] = 0u;
     __syncthreads();
-    __nv_bfloat16* wbase = sm + (COOP ? 0 : warp) * STG * 3 * TILE;
-    const int ctid = COOP ? tid : lane, cnt = COOP ? WPS * 32 : 32;  // who copies a task's tiles
+    __nv_bfloat16* wbase = sm + (COOP ? 0 : warp) * kStages * 3 * TILE;
+    const int ctid = COOP ? tid : lane, cnt = COOP ? kWarps * 32 : 32;  // who copies a task's tiles
     auto phase_sync = [&]() { if (COOP) __syncthreads(); else __syncwarp(); };
     const float sc = rsqrtf(static_cast<float>(dk)) * 1.4426950408889634f;
     const uint32_t thresh = static_cast<uint32_t>(p * 65536.0f + 0.5f);
     const float dscale = p > 0.f ? 1.f / (1.f - p) : 1.f;
     const int ntj = (T + 7) >> 3;
-    const int piece = CT > 0 ? 8 : piece_bytes(dk, ld, ld_ctx, sec);
+    const int piece = FIXED ? 8 : piece_bytes(dk, ld, ld_ctx, sec);
     const int n_tasks = static_cast<int>(n_seq * heads);  // < 2^31, checked by the launcher
-    const int W = COOP ? gridDim.x : gridDim.x * WPS;
-    const int gw = COOP ? blockIdx.x : blockIdx.x * WPS + warp;
+    const int W = COOP ? gridDim.x : gridDim.x * kWarps;
+    const int gw = COOP ? blockIdx.x : blockIdx.x * kWarps + warp;
     PieceMap lmap, smap;
     if (FAST) {
         make_piece_map(lmap, T, dk, piece, ld, lane, PT);
         make_piece_map(smap, T, dk, piece, ld_ctx, lane, PT);
     }
-    constexpr bool fast = FAST;
     const uint32_t wbase_s = smem_u32(wbase);
 
     auto prefetch = [&](int task, int stage) {
@@ -336,7 +351,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
             const int seq = task / heads;
             const int h = task - seq * heads;
             const __nv_bfloat16* src = qkv + static_cast<long long>(seq) * T * ld + h * dk;
-            if constexpr (fast) {
+            if constexpr (FAST) {
                 const uint32_t t0s = wbase_s + 2 * stage * 3 * TILE;
                 tile_load_map(t0s, src, lmap, piece);
                 tile_load_map(t0s + 2 * TILE, src + sec, lmap, piece);
@@ -351,14 +366,14 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
         cp_commit();
     };
 #pragma unroll
-    for (int s0 = 0; s0 < STG - 1; ++s0) prefetch(gw + s0 * W, s0);
+    for (int s0 = 0; s0 < kStages - 1; ++s0) prefetch(gw + s0 * W, s0);
 
     int stage = 0;
     for (int task = gw; task < n_tasks; task += W) {
-        cp_wait<STG - 2>();
+        cp_wait<kStages - 2>();
         phase_sync();
         // the stage consumed in the previous iteration is free again: refill it before computing this task
-        prefetch(task + (STG - 1) * W, (stage + STG - 1) % STG);
+        prefetch(task + (kStages - 1) * W, (stage + kStages - 1) % kStages);
         const long long seq = task / heads;
         const int h = task - static_cast<int>(seq) * heads;
         __nv_bfloat16* q = wbase + stage * 3 * TILE;
@@ -394,7 +409,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
                     mma_bf16_k8(s[nt], a, b);
                 }
             }
-            const bool dead1 = CT > 0 && mt * 16 + 8 >= CT;  // folds after unrolling
+            const bool dead1 = FIXED && mt * 16 + 8 >= CT;  // folds after unrolling
             softmax_rows<NTJ>(s, T, t4, ntj, sc, dead1);
             float o[NTD][4];
 #pragma unroll
@@ -423,7 +438,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
                 const bool pair = col + 1 < dk;
 #pragma unroll
                 for (int hf = 0; hf < 2; ++hf) {
-                    if (CT > 0 && mt * 16 + hf * 8 >= CT) continue;  // whole half-block past T: folds after unrolling
+                    if (FIXED && mt * 16 + hf * 8 >= CT) continue;  // whole half-block past T: folds after unrolling
                     const int r = mt * 16 + g + hf * 8;
                     if (r >= T) continue;
                     const float v0 = o[nd][2 * hf], v1 = pair ? o[nd][2 * hf + 1] : 0.f;
@@ -433,7 +448,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
         }
         phase_sync();
         __nv_bfloat16* out = ctx + seq * T * static_cast<long long>(ld_ctx);
-        if constexpr (fast) {
+        if constexpr (FAST) {
             if (p > 0.f) tile_store_dropout_map(q, out + h * dk, smap, piece, ld_ctx, seq * T, h * dk, seed, thresh, dscale);
             else tile_store_map(q, out + h * dk, smap, piece);
         } else if (p > 0.f) {
@@ -448,7 +463,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
             }
         }
         phase_sync();
-        stage = (stage + 1) % STG;
+        stage = (stage + 1) % kStages;
     }
     cp_wait<0>();
 }
@@ -456,44 +471,43 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 8 : 5) : (C
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
-template <int TP, int KSD, int NTD, int STG, int WPS, bool FAST, int CT, int CDK, int CH, bool COOP>
-__global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (COOP ? 3 : 1))) mhsa_mma_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, int sec,
+template <int NTD, bool FAST, bool FIXED, bool COOP>
+__global__ void __launch_bounds__(kWarps * 32, COOP ? 3 : (FIXED ? 4 : 3)) mhsa_mma_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, int sec,
                                                                   const __nv_bfloat16* __restrict__ dctx, int ld_dctx,
                                                                   long long n_seq, int T_, int heads_, int dk_,
                                                                   __nv_bfloat16* __restrict__ dqkv, int ld_d) {
-    constexpr int NTJ = TP / 8, MT = TP / 16, SP = TP + 8;
-    constexpr int PT = (CDK == 20) ? kPitch24 : kPitch;
-    constexpr bool K8T = (CDK == 20);
+    constexpr int TP = tile_rows(COOP), NTJ = TP / 8, MT = TP / 16, SP = TP + 8, KSD = (NTD + 1) / 2;
+    constexpr int CT = FIXED ? fixed_T(COOP) : 0;
+    constexpr int PT = FIXED ? kPitch24 : kPitch;
+    constexpr bool K8T = FIXED;
     constexpr int KS16 = K8T ? KSD - 1 : KSD;
-    const int T = CT > 0 ? CT : T_, heads = CH > 0 ? CH : heads_, dk = CDK > 0 ? CDK : dk_;
+    const int T = FIXED ? CT : T_, heads = FIXED ? kFixedHeads : heads_, dk = FIXED ? kFixedDk : dk_;
     const int TILE = T * PT;  // packed rows, see the forward kernel
     extern __shared__ __align__(16) __nv_bfloat16 sm[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
     const int d = heads * dk;
-    const int PER_WARP = STG * 4 * TILE + 2 * TP * SP;  // the P/dS scratch behind a warp's tiles doubles as read slack
-    static_assert(!COOP || (WPS == TP / 16 && !FAST), "cooperative CTAs: one warp per 16-row block, generic copy loops");
-    for (int i = tid; i < (COOP ? 1 : WPS) * PER_WARP / 2; i += blockDim.x) reinterpret_cast<uint32_t*>(sm)[i] = 0u;
+    const int PER_WARP = kStages * 4 * TILE + 2 * TP * SP;  // the P/dS scratch behind a warp's tiles doubles as read slack
+    static_assert(!COOP || (kWarps == TP / 16 && !FAST), "cooperative CTAs: one warp per 16-row block, generic copy loops");
+    for (int i = tid; i < (COOP ? 1 : kWarps) * PER_WARP / 2; i += blockDim.x) reinterpret_cast<uint32_t*>(sm)[i] = 0u;
     __syncthreads();
     __nv_bfloat16* wbase = sm + (COOP ? 0 : warp) * PER_WARP;
-    const int ctid = COOP ? tid : lane, cnt = COOP ? WPS * 32 : 32;
+    const int ctid = COOP ? tid : lane, cnt = COOP ? kWarps * 32 : 32;
     auto phase_sync = [&]() { if (COOP) __syncthreads(); else __syncwarp(); };
-    __nv_bfloat16* ps = wbase + STG * 4 * TILE;  // [TP][SP] probabilities (bf16)
+    __nv_bfloat16* ps = wbase + kStages * 4 * TILE;  // [TP][SP] probabilities (bf16)
     __nv_bfloat16* ds = ps + TP * SP;                // [TP][SP] score gradients (bf16)
     const float rs = rsqrtf(static_cast<float>(dk));
     const float sc = rs * 1.4426950408889634f;
     const int ntj = (T + 7) >> 3;
-    const int piece = CT > 0 ? 8
-                             : (piece_bytes(dk, ld, ld_dctx, sec) == 8 && (ld_d % 4) == 0 ? 8 : (piece_bytes(dk, ld, ld_dctx, sec) >= 4 && (ld_d % 2) == 0 ? 4 : 2));
+    const int piece = FIXED ? 8 : piece_bytes_bwd(dk, ld, ld_dctx, sec, ld_d);
     const int n_tasks = static_cast<int>(n_seq * heads);
-    const int W = COOP ? gridDim.x : gridDim.x * WPS;
-    const int gw = COOP ? blockIdx.x : blockIdx.x * WPS + warp;
+    const int W = COOP ? gridDim.x : gridDim.x * kWarps;
+    const int gw = COOP ? blockIdx.x : blockIdx.x * kWarps + warp;
     PieceMap lmap, gmap, smap;
     if (FAST) {
         make_piece_map(lmap, T, dk, piece, ld, lane, PT);
         make_piece_map(gmap, T, dk, piece, ld_dctx, lane, PT);
         make_piece_map(smap, T, dk, piece, ld_d, lane, PT);
     }
-    constexpr bool fast = FAST;
     const uint32_t wbase_s = smem_u32(wbase);
 
     auto prefetch = [&](int task, int stage) {
@@ -502,7 +516,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
             const int h = task - seq * heads;
             const __nv_bfloat16* src = qkv + static_cast<long long>(seq) * T * ld + h * dk;
             const __nv_bfloat16* gsrc = dctx + static_cast<long long>(seq) * T * ld_dctx + h * dk;
-            if constexpr (fast) {
+            if constexpr (FAST) {
                 const uint32_t t0s = wbase_s + 2 * stage * 4 * TILE;
                 tile_load_map(t0s, src, lmap, piece);
                 tile_load_map(t0s + 2 * TILE, src + sec, lmap, piece);
@@ -519,14 +533,14 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
         cp_commit();
     };
 #pragma unroll
-    for (int s0 = 0; s0 < STG - 1; ++s0) prefetch(gw + s0 * W, s0);
+    for (int s0 = 0; s0 < kStages - 1; ++s0) prefetch(gw + s0 * W, s0);
 
     int stage = 0;
     for (int task = gw; task < n_tasks; task += W) {
-        cp_wait<STG - 2>();
+        cp_wait<kStages - 2>();
         phase_sync();
         // the stage consumed in the previous iteration is free again: refill it before computing this task
-        prefetch(task + (STG - 1) * W, (stage + STG - 1) % STG);
+        prefetch(task + (kStages - 1) * W, (stage + kStages - 1) % kStages);
         const long long seq = task / heads;
         const int h = task - static_cast<int>(seq) * heads;
         const __nv_bfloat16* q = wbase + stage * 4 * TILE;
@@ -610,7 +624,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
                     }
                 }
             }
-            const bool dead1 = CT > 0 && mt * 16 + 8 >= CT;  // rows g+8 of this block are all >= T (folds after unrolling)
+            const bool dead1 = FIXED && mt * 16 + 8 >= CT;  // rows g+8 of this block are all >= T (folds after unrolling)
             softmax_rows<NTJ>(s, T, t4, ntj, sc, dead1);
             float del0 = 0.f, del1 = 0.f;
 #pragma unroll
@@ -666,7 +680,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
                 if (col >= dk) continue;
 #pragma unroll
                 for (int hf = 0; hf < 2; ++hf) {
-                    if (CT > 0 && mt * 16 + hf * 8 >= CT) continue;  // whole half-block past T: folds after unrolling
+                    if (FIXED && mt * 16 + hf * 8 >= CT) continue;  // whole half-block past T: folds after unrolling
                     const int r = mt * 16 + g + hf * 8;
                     if (r >= T) continue;
                     __nv_bfloat16* o = gout + static_cast<size_t>(r) * ld_d + h * dk + col;
@@ -714,7 +728,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
                 const bool pair = col + 1 < dk;  // odd d_k: keep the zero padding column intact
 #pragma unroll
                 for (int hf = 0; hf < 2; ++hf) {
-                    if (CT > 0 && mt * 16 + hf * 8 >= CT) continue;  // whole half-block past T: folds after unrolling
+                    if (FIXED && mt * 16 + hf * 8 >= CT) continue;  // whole half-block past T: folds after unrolling
                     const int r = mt * 16 + g + hf * 8;
                     if (r >= T) continue;
                     *reinterpret_cast<uint32_t*>(k + r * PT + col) = pack_bf16x2(dkk[nd][2 * hf], pair ? dkk[nd][2 * hf + 1] : 0.f);
@@ -723,7 +737,7 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
             }
         }
         phase_sync();
-        if constexpr (fast) {
+        if constexpr (FAST) {
             tile_store_map(k, gout + sec + h * dk, smap, piece);
             tile_store_map(v, gout + 2 * sec + h * dk, smap, piece);
         } else {
@@ -738,112 +752,67 @@ __global__ void __launch_bounds__(WPS * 32, (TP <= 32 ? (CDK == 20 ? 4 : 3) : (C
             }
         }
         phase_sync();
-        stage = (stage + 1) % STG;
+        stage = (stage + 1) % kStages;
     }
     cp_wait<0>();
 }
 
-template <int TP, int KSD, int NTD, int STG, int WPS, bool FAST, int CT = 0, int CDK = 0, int CH = 0, bool COOP = false>
-int launch_mma_cfg2(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
+template <int NTD, bool FAST, bool FIXED, bool COOP>
+int launch_mma(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
                void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
     const long long tasks = n_seq * heads;
     NR_REQUIRE(tasks < (1ll << 31), "mhsa: too many (sequence, head) tasks");
-    constexpr int PT = (CDK == 20) ? kPitch24 : kPitch;
+    constexpr int TP = tile_rows(COOP);
+    constexpr int PT = FIXED ? kPitch24 : kPitch;
     const size_t tile = sizeof(__nv_bfloat16) * T * PT;
-    const int sets = COOP ? 1 : WPS;  // tile sets per CTA: one per warp, or one shared by the cooperative CTA
-    const size_t smem_f = sets * STG * 3 * tile + sizeof(__nv_bfloat16) * (TP - T) * PT;
-    const size_t smem_b = sets * (STG * 4 * tile + sizeof(__nv_bfloat16) * 2 * TP * (TP + 8));
+    const int sets = COOP ? 1 : kWarps;  // tile sets per CTA: one per warp, or one shared by the cooperative CTA
+    const size_t smem_f = sets * kStages * 3 * tile + sizeof(__nv_bfloat16) * (TP - T) * PT;
+    const size_t smem_b = sets * (kStages * 4 * tile + sizeof(__nv_bfloat16) * 2 * TP * (TP + 8));
     const size_t smem = bwd ? smem_b : smem_f;
     NR_REQUIRE(smem <= 227 * 1024, "mhsa: tile set of %zu bytes exceeds shared memory", smem);
     const int per_sm = std::max<int>(1, std::min<size_t>(COOP ? 3 : (bwd ? 6 : 8), (224 * 1024) / (smem + 1024)));
-    const int grid = static_cast<int>(std::min<long long>(ceil_div(static_cast<int>(std::min<long long>(tasks, 1 << 30)), COOP ? 1 : WPS),
+    const int grid = static_cast<int>(std::min<long long>(ceil_div(static_cast<int>(std::min<long long>(tasks, 1 << 30)), COOP ? 1 : kWarps),
                                                           static_cast<long long>(num_sms()) * per_sm));
     if (!bwd) {
-        NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_mma_fwd_kernel<TP, KSD, NTD, STG, WPS, FAST, CT, CDK, CH, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mhsa_mma_fwd_kernel<TP, KSD, NTD, STG, WPS, FAST, CT, CDK, CH, COOP><<<grid, WPS * 32, smem, stream>>>(static_cast<const __nv_bfloat16*>(qkv), ld_qkv, sec, n_seq, T,
-                                                                             heads, dk, static_cast<__nv_bfloat16*>(out), ld_out, drop.p,
-                                                                             drop.seed);
+        NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_mma_fwd_kernel<NTD, FAST, FIXED, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        mhsa_mma_fwd_kernel<NTD, FAST, FIXED, COOP><<<grid, kWarps * 32, smem, stream>>>(static_cast<const __nv_bfloat16*>(qkv), ld_qkv, sec, n_seq, T,
+                                                                                       heads, dk, static_cast<__nv_bfloat16*>(out), ld_out, drop.p,
+                                                                                       drop.seed);
     } else {
-        NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_mma_bwd_kernel<TP, KSD, NTD, STG, WPS, FAST, CT, CDK, CH, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mhsa_mma_bwd_kernel<TP, KSD, NTD, STG, WPS, FAST, CT, CDK, CH, COOP><<<grid, WPS * 32, smem, stream>>>(static_cast<const __nv_bfloat16*>(qkv), ld_qkv, sec,
-                                                                             static_cast<const __nv_bfloat16*>(dctx), ld_dctx, n_seq, T,
-                                                                             heads, dk, static_cast<__nv_bfloat16*>(out), ld_out);
+        NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_mma_bwd_kernel<NTD, FAST, FIXED, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        mhsa_mma_bwd_kernel<NTD, FAST, FIXED, COOP><<<grid, kWarps * 32, smem, stream>>>(static_cast<const __nv_bfloat16*>(qkv), ld_qkv, sec,
+                                                                                       static_cast<const __nv_bfloat16*>(dctx), ld_dctx, n_seq, T,
+                                                                                       heads, dk, static_cast<__nv_bfloat16*>(out), ld_out);
     }
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-
-// the per-lane copy plan covers tiles of up to 128 pieces of >= 4 bytes; anything else takes the generic loops
-template <int TP, int KSD, int NTD, int STG, int WPS>
-int launch_mma_cfg(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-                   void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
-    const int d = heads * dk;
-    int piece = piece_bytes(dk, ld_qkv, bwd ? ld_dctx : ld_out, sec);
-    if (bwd) piece = (piece == 8 && (ld_out % 4) == 0) ? 8 : ((piece >= 4 && (ld_out % 2) == 0) ? 4 : 2);
-#ifdef NEWSREC_TRIAGE
-    static const bool force_loops = getenv("NEWSREC_ATTN_LOOPS") != nullptr;  // tuning switch (tools/kbench.py), triage builds only
-#else
-    constexpr bool force_loops = false;
-#endif
-    const bool fast = !force_loops && piece >= 4 && T * (dk / (piece / 2)) <= kMaxP * 32;
-#ifdef NEWSREC_TRIAGE
-    static const bool no_fixed = getenv("NEWSREC_ATTN_GENERIC") != nullptr;  // tuning switch: skip the fixed-shape kernels
-#else
-    constexpr bool no_fixed = false;
-#endif
-    if constexpr (TP == 32 && KSD == 2 && NTD == 3) {
-        // the reference's title encoder (config.py: num_words_title 20, 15 heads x 20) gets a fully fixed-shape kernel
-        if (fast && !no_fixed && piece == 8 && T == 20 && dk == 20 && heads == 15)
-            return launch_mma_cfg2<TP, KSD, NTD, STG, WPS, true, 20, 20, 15>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out,
-                                                                             drop, stream);
-    }
-    if (fast)
-        return launch_mma_cfg2<TP, KSD, NTD, STG, WPS, true>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
-    return launch_mma_cfg2<TP, KSD, NTD, STG, WPS, false>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+template <bool FAST, bool COOP>
+int launch_dk(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
+              void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
+    if (dk <= 16) return launch_mma<2, FAST, false, COOP>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+    if (dk <= 24) return launch_mma<3, FAST, false, COOP>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+    return launch_mma<4, FAST, false, COOP>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
 }
 
-template <int TP, int KSD, int NTD>
-int launch_mma(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-               void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
-    // 64-row tiles (history-level attention): one cooperative CTA of TP/16 warps per (sequence, head)
-    if constexpr (TP > 32) {
-#ifdef NEWSREC_TRIAGE
-        static const bool no_coop = getenv("NEWSREC_ATTN_NOCOOP") != nullptr;  // tuning switch
-#else
-        constexpr bool no_coop = false;
-#endif
-        if (!no_coop) {
-            if constexpr (TP == 64 && KSD == 2 && NTD == 3) {
-                // the reference's user encoder (config.py: num_clicked_news_a_user 50, 15 heads x 20): fixed shape
-                const int d = heads * dk;
-                int piece = piece_bytes(dk, ld_qkv, bwd ? ld_dctx : ld_out, sec);
-                if (bwd && (ld_out % 4) != 0) piece = 0;
-#ifdef NEWSREC_TRIAGE
-                static const bool no_fixed = getenv("NEWSREC_ATTN_GENERIC") != nullptr;
-#else
-                constexpr bool no_fixed = false;
-#endif
-                if (!no_fixed && piece == 8 && T == 50 && dk == 20 && heads == 15)
-                    return launch_mma_cfg2<TP, KSD, NTD, 2, TP / 16, false, 50, 20, 15, true>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads,
-                                                                                              dk, out, ld_out, drop, stream);
-            }
-            return launch_mma_cfg2<TP, KSD, NTD, 2, TP / 16, false, 0, 0, 0, true>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out,
-                                                                                   ld_out, drop, stream);
-        }
-        if (bwd)
-            return launch_mma_cfg<TP, KSD, NTD, 2, 3>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+// Picks the kernel from the input.  T > 32 runs on cooperative CTAs (one task per CTA), T <= 32 on per-warp tasks.  Both take
+// the fixed-shape kernel for the reference's head shape when its rows move in 8-byte pieces.  Otherwise the per-warp tasks use
+// the per-lane copy plan when it covers the tile (up to kMaxP * 32 pieces of >= 4 bytes) and the copy loops when it does not.
+int dispatch(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
+             void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
+    const bool coop = T > 32;
+    const int piece = bwd ? piece_bytes_bwd(dk, ld_qkv, ld_dctx, sec, ld_out) : piece_bytes(dk, ld_qkv, ld_out, sec);
+    if (piece == 8 && T == fixed_T(coop) && dk == kFixedDk && heads == kFixedHeads) {  // d_k 20: the NTD 3 class
+        if (coop) return launch_mma<3, false, true, true>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+        // per-warp: the copy plan always covers it (20 rows x 5 pieces of 8 bytes)
+        return launch_mma<3, true, true, false>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
     }
-    return launch_mma_cfg<TP, KSD, NTD, 2, 4>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
-}
-
-template <int TP>
-int dispatch_dk(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-                void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
-    if (dk <= 16) return launch_mma<TP, 1, 2>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
-    if (dk <= 24) return launch_mma<TP, 2, 3>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
-    return launch_mma<TP, 2, 4>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+    if (coop) return launch_dk<false, true>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+    const bool fast = piece >= 4 && T * (dk / (piece / 2)) <= kMaxP * 32;
+    if (fast) return launch_dk<true, false>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
+    return launch_dk<false, false>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
 }
 
 }  // namespace
@@ -858,8 +827,7 @@ int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, 
     ProfScope ps("mhsa_core_fwd", static_cast<int>(n_seq), T, heads * dk, stream);
     if (mhsa_title_fwd_supported(T, dk, heads, sec, ld_qkv, ld_ctx))  // the news encoder's shape: whole titles per CTA, TMA in / out
         return mhsa_title_fwd(qkv, ld_qkv, sec, n_seq, heads, ctx, ld_ctx, drop, stream);
-    if (T <= 32) return dispatch_dk<32>(false, qkv, ld_qkv, sec, nullptr, 0, n_seq, T, heads, dk, ctx, ld_ctx, drop, stream);
-    return dispatch_dk<64>(false, qkv, ld_qkv, sec, nullptr, 0, n_seq, T, heads, dk, ctx, ld_ctx, drop, stream);
+    return dispatch(false, qkv, ld_qkv, sec, nullptr, 0, n_seq, T, heads, dk, ctx, ld_ctx, drop, stream);
 }
 
 int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
@@ -873,8 +841,7 @@ int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld
     const DropoutCfg nodrop{0.f, 0};
     if (mhsa_title_bwd_supported(T, dk, heads, sec, ld_qkv, ld_dctx, ld_dqkv))  // the news encoder's shape: whole titles per CTA, TMA in / out
         return mhsa_title_bwd(qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, heads, dqkv, ld_dqkv, stream);
-    if (T <= 32) return dispatch_dk<32>(true, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, nodrop, stream);
-    return dispatch_dk<64>(true, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, nodrop, stream);
+    return dispatch(true, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, nodrop, stream);
 }
 
 }  // namespace nr

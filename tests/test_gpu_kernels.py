@@ -70,6 +70,9 @@ def test_tcgen05_matches_simt_triage_backend():
 
 @pytest.mark.parametrize("kw", [dict(n_seq=7, T=20), dict(n_seq=3, T=50), dict(n_seq=2000, T=20), dict(n_seq=5, T=16, heads=30, dk=10),
                                 dict(n_seq=5, T=33, heads=20, dk=15), dict(n_seq=4, T=64, heads=10, dk=30), dict(n_seq=9, T=7, heads=12, dk=25),
+                                # the remaining per-warp / cooperative kernels: d_k class x copy plan / copy loops (dense sections)
+                                dict(n_seq=9, T=12, heads=8, dk=9), dict(n_seq=5, T=24, heads=15, dk=20), dict(n_seq=5, T=20, heads=5, dk=18),
+                                dict(n_seq=6, T=8, heads=4, dk=32), dict(n_seq=3, T=40, heads=6, dk=20),
                                 # the encoders' sectioned Q|K|V rows (sec = round_up(d, 8)); T=20, d_k=20 takes the title-level kernel
                                 dict(n_seq=7, T=20, sectioned=True), dict(n_seq=1, T=20, sectioned=True), dict(n_seq=2000, T=20, sectioned=True),
                                 dict(n_seq=301, T=20, heads=4, sectioned=True), dict(n_seq=40, T=20, heads=9, sectioned=True),
