@@ -12,14 +12,9 @@ void set_debug_simt_gemm(int on);
 int has_triage_backends();
 void set_debug_gemm_timing(void* dev_buf, int slots);
 void set_comm_reserved_sms(int n);
-extern int g_launches;
 }  // namespace nr
 
 using namespace nr;
-
-static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
-static const RowMapCfg kIdentity = {0, 0, 0, 0, 0};
-static const DropoutCfg kNoDrop = {0.f, 0};
 
 extern "C" {
 
@@ -39,44 +34,45 @@ int nr_profile_report(char* buf, int cap) { return prof_report(buf, cap); }
 int nr_cast_pad_bf16_many(int n, const float* const* src, const int* R, const int* C, const int* lds, void* const* dst, const int* ld,
                           const int* transpose, void* stream) {
     NR_REQUIRE(src && R && C && lds && dst && ld && transpose, "nr_cast_pad_bf16_many: null argument array");
-    return cast_pad_bf16_many(n, src, R, C, lds, dst, ld, transpose, S(stream));
+    return cast_pad_bf16_many(n, src, R, C, lds, dst, ld, transpose, as_stream(stream));
 }
 int nr_cast_pad_bf16(const float* src, int R, int C, int lds, void* dst, int ld, int transpose, void* stream) {
     NR_REQUIRE(src && dst && R >= 0 && C >= 0 && ld % 8 == 0 && ld >= (transpose ? R : C),
                "nr_cast_pad_bf16: R=%d C=%d ld=%d transpose=%d", R, C, ld, transpose);
-    return cast_pad_bf16(src, R, C, lds, dst, ld, transpose, S(stream));
+    return cast_pad_bf16(src, R, C, lds, dst, ld, transpose, as_stream(stream));
 }
 int nr_rows_to_bf16(const float* src, long long n, int D, long long s_row, long long s_col, void* dst, int ld,
                     void* stream) {
     NR_REQUIRE(src && dst && n >= 0 && ld % 8 == 0, "nr_rows_to_bf16: n=%lld ld=%d", n, ld);
-    return rows_to_bf16(src, n, 1, D, s_row, 0, s_col, dst, ld, S(stream));
+    return rows_to_bf16(src, n, 1, D, s_row, 0, s_col, dst, ld, as_stream(stream));
 }
 int nr_gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld, void* X,
                    int padded, float p_drop, unsigned long long seed, int* bad_id_flag, void* stream) {
     NR_REQUIRE(ids && table && X && bad_id_flag && T >= 1 && n_tok % T == 0 && p_drop >= 0.f && p_drop < 1.f,
                "nr_gather_rows: n_tok=%lld T=%d p=%f", n_tok, T, p_drop);
-    return gather_rows(ids, n_tok, T, table, V, D, ld, X, ld, padded, DropoutCfg{p_drop, seed}, bad_id_flag, S(stream));
+    return gather_rows(ids, n_tok, T, table, V, D, ld, X, ld, padded, DropoutCfg{p_drop, seed}, bad_id_flag, as_stream(stream));
 }
 int nr_linear(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,
               int rows_per_tile, const float* bias, int relu, void* out, int ld_out, int out_is_bf16, void* stream) {
     NR_REQUIRE(A && W && out && (taps == 1 || taps == 3), "nr_linear: null operand or taps=%d", taps);
-    return gemm_store(A, M, lda, W, N, ldw, K, taps, w_tap_rows, rows_per_tile, bias, relu, out, ld_out, out_is_bf16,
-                      kIdentity, 0, kNoDrop, -1, 0, S(stream));
+    return gemm_store({.A = A, .M = M, .lda = lda, .W = W, .N = N, .ldw = ldw, .K = K, .taps = taps, .w_tap_rows = w_tap_rows},
+                      {.out = out, .ld_out = ld_out, .out_bf16 = out_is_bf16, .relu = relu, .bias = bias, .rows_per_tile = rows_per_tile},
+                      as_stream(stream));
 }
 int nr_gemm_tn(const void* A, int Kr, int Ma, int lda, const void* B, int b_rows, int b_cols, int ldb, int b_col0,
                int Nb, int b_row_shift, float* D, int ldd, void* stream) {
     NR_REQUIRE(A && B && D, "nr_gemm_tn: null operand");
-    return gemm_tn_accumulate(A, Kr, Ma, lda, B, b_rows, b_cols, ldb, b_col0, Nb, b_row_shift, D, ldd, S(stream));
+    return gemm_tn_accumulate(A, Kr, Ma, lda, B, b_rows, b_cols, ldb, b_col0, Nb, b_row_shift, D, ldd, as_stream(stream));
 }
 int nr_mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, int heads, int dk, void* ctx, int ld_ctx,
                      float p_drop, unsigned long long seed, void* stream) {
     NR_REQUIRE(qkv && ctx, "nr_mhsa_core_fwd: null operand");
-    return mhsa_core_fwd(qkv, ld_qkv, sec, n_seq, T, heads, dk, ctx, ld_ctx, DropoutCfg{p_drop, seed}, S(stream));
+    return mhsa_core_fwd(qkv, ld_qkv, sec, n_seq, T, heads, dk, ctx, ld_ctx, DropoutCfg{p_drop, seed}, as_stream(stream));
 }
 int nr_mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads,
                      int dk, void* dqkv, int ld_dqkv, void* stream) {
     NR_REQUIRE(qkv && dctx && dqkv, "nr_mhsa_core_bwd: null operand");
-    return mhsa_core_bwd(qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, S(stream));
+    return mhsa_core_bwd(qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, as_stream(stream));
 }
 
 // ---- AdditiveAttention ---------------------------------------------------------------------------
@@ -85,12 +81,16 @@ int nr_additive_attention_fwd(const void* X, long long n_seg, int seg_len, int D
     NR_REQUIRE(X && Wa && ba && qv && out, "nr_additive_attention_fwd: null operand");
     NR_REQUIRE(n_seg * seg_len < (1ll << 31), "nr_additive_attention_fwd: too many rows");
     return gemm_additive_pool(X, static_cast<int>(n_seg * seg_len), ldx, D, Wa, q, ldw, ba, qv, seg_len, out, ldo, w_out,
-                              S(stream));
+                              as_stream(stream));
 }
-static inline long long align256(long long x) { return (x + 255) & ~255ll; }
+struct AdditiveBwdWorkspace : WorkspaceLayout {
+    float* dscore;
+    __nv_bfloat16* dpre;  // [rows][round_up(q, 16)]
+    AdditiveBwdWorkspace(void* base, long long rows, int q)
+        : WorkspaceLayout{static_cast<char*>(base)}, dscore(take<float>(rows)), dpre(take<__nv_bfloat16>(rows * round_up(q, 16))) {}
+};
 long long nr_additive_attention_bwd_workspace(long long n_seg, int seg_len, int q) {
-    const long long rows = n_seg * seg_len;
-    return align256(rows * 4) + align256(rows * ((q + 15) & ~15) * 2) + 256;
+    return AdditiveBwdWorkspace(nullptr, n_seg * seg_len, q).bytes();
 }
 int nr_additive_attention_bwd(const void* X, long long n_seg, int seg_len, int D, int ldx, const void* Wa,
                               const void* WaT, int q, int ldw, int ldwT, const float* ba, const float* qv, const float* w,
@@ -98,32 +98,28 @@ int nr_additive_attention_bwd(const void* X, long long n_seg, int seg_len, int D
                               void* workspace, long long workspace_bytes, void* stream) {
     NR_REQUIRE(X && Wa && WaT && ba && qv && w && dout && dX && dWa_ext && dqv && workspace,
                "nr_additive_attention_bwd: null operand");
-    NR_REQUIRE(workspace_bytes >= nr_additive_attention_bwd_workspace(n_seg, seg_len, q),
-               "nr_additive_attention_bwd: workspace too small");
     const long long rows = n_seg * seg_len;
+    const AdditiveBwdWorkspace ws(workspace, rows, q);
+    NR_REQUIRE(workspace_bytes >= ws.bytes(), "nr_additive_attention_bwd: workspace too small");
     NR_REQUIRE(rows < (1ll << 31), "nr_additive_attention_bwd: too many rows");
     const int M = static_cast<int>(rows);
-    const int ldq = (q + 15) & ~15;
-    char* ws = static_cast<char*>(workspace);
-    float* dscore = reinterpret_cast<float*>(ws);
-    void* dpre = ws + align256(rows * 4);
-    NR_PROPAGATE(pool_dscore(X, ldx, D, n_seg, seg_len, w, dout, ldo, dscore, S(stream)));
-    NR_PROPAGATE(gemm_additive_dpre(X, M, ldx, D, Wa, q, ldw, ba, qv, dscore, dpre, ldq, dqv, S(stream)));
-    NR_PROPAGATE(gemm_pool_dinput(dpre, M, ldq, q, WaT, D, ldwT, w, dout, ldo, seg_len, dX, ld_dx, kIdentity, 0, kNoDrop,
-                                  nullptr, 0, S(stream)));
-    // dWa_ext[q][0:D] += dPre^T . X ; column D (the ones column of X) accumulates d(bias)
-    NR_PROPAGATE(gemm_tn_accumulate(dpre, M, q, ldq, X, M, D + 1, ldx, 0, D + 1, 0, dWa_ext, ldx, S(stream)));
+    const int ldq = round_up(q, 16);
+    NR_PROPAGATE(pool_dscore(X, ldx, D, n_seg, seg_len, w, dout, ldo, ws.dscore, as_stream(stream)));
+    NR_PROPAGATE(gemm_additive_dpre(X, M, ldx, D, Wa, q, ldw, ba, qv, ws.dscore, ws.dpre, ldq, dqv, as_stream(stream)));
+    NR_PROPAGATE(gemm_pool_dinput({.A = ws.dpre, .M = M, .lda = ldq, .W = WaT, .N = D, .ldw = ldwT, .K = q},
+                                  {.w = w, .dout = dout, .ldo = ldo, .seg_len = seg_len, .dx = dX, .ld_dx = ld_dx}, as_stream(stream)));
+    NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, q, ldq, X, D, ldx, dWa_ext, as_stream(stream)));  // the ones column of X: d(bias)
     return 0;
 }
 
 int nr_dot_score_fwd(const float* cand, const float* user, int B, int C, int D, float* logits, void* stream) {
     NR_REQUIRE(cand && user && logits, "nr_dot_score_fwd: null operand");
-    return dot_score_fwd(cand, user, B, C, D, logits, S(stream));
+    return dot_score_fwd(cand, user, B, C, D, logits, as_stream(stream));
 }
 int nr_dot_score_bwd(const float* cand, const float* user, const float* dlogits, int B, int C, int D, float* dcand,
                      float* duser, void* stream) {
     NR_REQUIRE(cand && user && dlogits && dcand && duser, "nr_dot_score_bwd: null operand");
-    return dot_score_bwd(cand, user, dlogits, B, C, D, dcand, duser, S(stream));
+    return dot_score_bwd(cand, user, dlogits, B, C, D, dcand, duser, as_stream(stream));
 }
 
 
@@ -131,12 +127,12 @@ int nr_segment_dot(const float* news, long long n_news, int D, const long long* 
                    long long n_seg, const float* user, float* scores, int* bad_id_flag, void* stream) {
     NR_REQUIRE(news && cand && seg_offsets && user && scores && bad_id_flag && n_seg >= 1 && D >= 1 && n_cand >= 0,
                "nr_segment_dot: null operand or empty problem");
-    return segment_dot(news, n_news, D, cand, n_cand, seg_offsets, n_seg, user, scores, bad_id_flag, S(stream));
+    return segment_dot(news, n_news, D, cand, n_cand, seg_offsets, n_seg, user, scores, bad_id_flag, as_stream(stream));
 }
 
 int nr_accumulate_ext_grad(float* ext, int rows, int ld, int D, float* dW, float* db, void* stream) {
     NR_REQUIRE(ext && dW && rows >= 0 && D >= 1, "nr_accumulate_ext_grad: null operand");
-    return accumulate_ext_grad(ext, rows, ld, D, dW, db, S(stream));
+    return accumulate_ext_grad(ext, rows, ld, D, dW, db, as_stream(stream));
 }
 
 // ---- batch feed ------------------------------------------------------------------------------------
@@ -148,7 +144,7 @@ int nr_pack_slots(const void* const* slots, int n_clicked, int n_candidates, int
     NR_REQUIRE(slots && out && n_clicked >= 0 && n_candidates >= 0 && B >= 0 && L >= 1, "nr_pack_slots: bad arguments");
     for (int i = 0; i < n_clicked + n_candidates; ++i) NR_REQUIRE(slots[i] != nullptr, "nr_pack_slots: slot %d is null", i);
     prof_context("feed");
-    return pack_slots(slots, n_clicked, n_candidates, B, L, out, S(stream));
+    return pack_slots(slots, n_clicked, n_candidates, B, L, out, as_stream(stream));
 }
 
 // ---- NRMS encoders ---------------------------------------------------------------------------------
@@ -181,7 +177,8 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
     NR_REQUIRE(a->p_drop >= 0.f && a->p_drop < 1.f, "nr_mhsa_encoder_fwd: dropout p=%f", a->p_drop);
     if (a->n_seq == 0) return 0;
     const int M = static_cast<int>(a->n_seq * a->T);
-    const cudaStream_t st = S(stream);
+    const cudaStream_t st = as_stream(stream);
+    const int sec = qkv_section(a->d);
     prof_context(a->ids != nullptr ? "news.fwd" : "user.fwd");
     if (a->dense != nullptr && a->C_lo_bf16 != nullptr) {
         // precise user encoder (user_encoder.py:15-26 at fp32 accuracy): the input enters as a hi/lo pair against the
@@ -192,9 +189,10 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_bf16, a->ldx, st));
         NR_PROPAGATE(rows_to_bf16_hilo(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_kcat_bf16,
                                        a->ldx, st));
-        NR_PROPAGATE(gemm_store(a->X_kcat_bf16, M, 2 * a->ldx, a->wqkv_kcat_bf16, 3 * qkv_section(a->d), 2 * a->ldx, 2 * a->ldx, 1, 0, kGemmTileRows,
-                                a->bqkv, 0, a->QKV_f32, 3 * qkv_section(a->d), 0, kIdentity, 0, kNoDrop, -1, 0, st));
-        NR_PROPAGATE(mhsa_f32_fwd(a->QKV_f32, 3 * qkv_section(a->d), qkv_section(a->d), a->n_seq, a->T, a->heads, a->d / a->heads, a->C_bf16, a->C_lo_bf16, a->ldx, st));
+        NR_PROPAGATE(gemm_store({.A = a->X_kcat_bf16, .M = M, .lda = 2 * a->ldx, .W = a->wqkv_kcat_bf16, .N = 3 * sec, .ldw = 2 * a->ldx,
+                                 .K = 2 * a->ldx},
+                                {.out = a->QKV_f32, .ld_out = 3 * sec, .bias = a->bqkv}, st));
+        NR_PROPAGATE(mhsa_f32_fwd(a->QKV_f32, 3 * sec, sec, a->n_seq, a->T, a->heads, a->d / a->heads, a->C_bf16, a->C_lo_bf16, a->ldx, st));
         NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
                                         a->w, st, a->C_lo_bf16));
         return 0;
@@ -203,19 +201,19 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         // accurate news encoder on the unfused sequence: V, the attention probabilities and the context travel as hi/lo bf16
         // pairs (the projection GEMM emits the low plane of the V section, the title-level attention kernel splits the
         // probabilities in registers and writes both context planes, the pooled sum reads both)
-        const int sec = qkv_section(a->d);
         NR_REQUIRE(a->C_lo_bf16 != nullptr && a->table_bf16 && a->bad_id_flag && a->V >= 1,
                    "nr_mhsa_encoder_fwd: the accurate variant needs C_lo_bf16 (+ table / bad_id_flag)");
         NR_REQUIRE(mhsa_title_fwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx),
                    "nr_mhsa_encoder_fwd: the accurate variant needs the title-level attention kernel (T=20, d_k=20, <=15 heads); see nr_mhsa_accurate_supported");
         NR_PROPAGATE(gather_rows(a->ids, M, a->T, a->table_bf16, a->V, a->d, a->ldx, a->X_bf16, a->ldx, 0,
                                  DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
-        NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, kGemmTileRows, a->bqkv, 0, a->QKV_bf16, a->ld3, 1,
-                                kIdentity, 0, kNoDrop, -1, 0, st, a->V_lo_bf16, sec, 2 * sec));
-        const DropoutCfg cd = {a->p_drop, a->seed ^ 0x5bd1e995u};
+        NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
+                                {.out = a->QKV_bf16, .ld_out = a->ld3, .out_bf16 = 1, .bias = a->bqkv, .lo_out = a->V_lo_bf16, .ld_lo = sec,
+                                 .lo_col0 = 2 * sec}, st));
         {
             ProfScope ps("mhsa_core_fwd_hilo", static_cast<int>(a->n_seq), a->T, a->d, st);
-            NR_PROPAGATE(mhsa_title_fwd(a->QKV_bf16, a->ld3, sec, a->n_seq, a->heads, a->C_bf16, a->ldx, cd, st, a->V_lo_bf16, sec, a->C_lo_bf16));
+            NR_PROPAGATE(mhsa_title_fwd(a->QKV_bf16, a->ld3, sec, a->n_seq, a->heads, a->C_bf16, a->ldx, context_dropout(a->p_drop, a->seed), st,
+                                        a->V_lo_bf16, sec, a->C_lo_bf16));
         }
         NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
                                         a->w, st, a->C_lo_bf16));
@@ -230,23 +228,27 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
                                   a->X_bf16, a->ldx, st));
     }
     // Q|K|V = X . Wqkv^T + b   (multihead_self.py:53-58)
-    NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * qkv_section(a->d), a->ldx, a->d, 1, 0, kGemmTileRows, a->bqkv, 0,
-                            a->QKV_bf16, a->ld3, 1, kIdentity, 0, kNoDrop, -1, 0, st));
+    NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
+                            {.out = a->QKV_bf16, .ld_out = a->ld3, .out_bf16 = 1, .bias = a->bqkv}, st));
     // per-head attention (multihead_self.py:15-23), dropout on the context only in the news encoder
-    const DropoutCfg cdrop = {a->ids != nullptr ? a->p_drop : 0.f, a->seed ^ 0x5bd1e995u};
-    NR_PROPAGATE(mhsa_core_fwd(a->QKV_bf16, a->ld3, qkv_section(a->d), a->n_seq, a->T, a->heads, a->d / a->heads, a->C_bf16, a->ldx, cdrop,
-                               st));
+    const DropoutCfg cdrop = context_dropout(a->ids != nullptr ? a->p_drop : 0.f, a->seed);
+    NR_PROPAGATE(mhsa_core_fwd(a->QKV_bf16, a->ld3, sec, a->n_seq, a->T, a->heads, a->d / a->heads, a->C_bf16, a->ldx, cdrop, st));
     // additive pooling (additive.py:35-53)
     NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
                                     a->w, st));
     return 0;
 }
 
-long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q) {
-    const long long rows = n_seq * T;
-    const long long ldx = (d + 1 + 7) & ~7, ld3 = (3 * qkv_section(d) + 15) & ~15, ldq = (q + 15) & ~15;
-    return align256(rows * 4) + align256(rows * ldq * 2) + align256(rows * ldx * 2) + 2 * align256(rows * ld3 * 2) + 256;
-}
+// bf16 buffers at the canonical pitches ldq, ldx, ld3, ld3; QKV only for the precise dense forward, which keeps no bf16 Q|K|V
+struct MhsaBwdWorkspace : WorkspaceLayout {
+    float* dscore;
+    __nv_bfloat16 *dpre, *dC, *dQKV, *QKV;
+    MhsaBwdWorkspace(void* base, long long rows, int d, int q)
+        : WorkspaceLayout{static_cast<char*>(base)}, dscore(take<float>(rows)), dpre(take<__nv_bfloat16>(rows * round_up(q, 16))),
+          dC(take<__nv_bfloat16>(rows * round_up(d + 1, 8))), dQKV(take<__nv_bfloat16>(rows * round_up(3 * qkv_section(d), 16))),
+          QKV(take<__nv_bfloat16>(rows * round_up(3 * qkv_section(d), 16))) {}
+};
+long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q) { return MhsaBwdWorkspace(nullptr, n_seq * T, d, q).bytes(); }
 
 int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_mhsa_encoder_bwd: null args");
@@ -261,57 +263,45 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
                "nr_mhsa_encoder_bwd: Q|K|V was not saved (precise dense forward): pass wqkv_bf16 / bqkv so that it can be recomputed from X");
     NR_REQUIRE((a->ids != nullptr) ? (a->demb != nullptr) : (a->ddense != nullptr),
                "nr_mhsa_encoder_bwd: missing input-gradient buffer");
-    NR_REQUIRE(a->workspace_bytes >= nr_mhsa_encoder_bwd_workspace(a->n_seq, a->T, a->d, a->q),
-               "nr_mhsa_encoder_bwd: workspace too small (%lld bytes)", a->workspace_bytes);
+    const MhsaBwdWorkspace ws(a->workspace, a->n_seq * a->T, a->d, a->q);
+    NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_mhsa_encoder_bwd: workspace too small (%lld bytes)", a->workspace_bytes);
     if (a->n_seq == 0) return 0;
-    const long long rows = a->n_seq * a->T;
-    const int M = static_cast<int>(rows);
-    const cudaStream_t st = S(stream);
+    const int M = static_cast<int>(a->n_seq * a->T);
+    const cudaStream_t st = as_stream(stream);
     const int sec = qkv_section(a->d);
-    char* ws = static_cast<char*>(a->workspace);
-    float* dscore = reinterpret_cast<float*>(ws);
-    ws += align256(rows * 4);
-    void* dpre = ws;
-    ws += align256(rows * a->ldq * 2);
-    void* dC = ws;
-    ws += align256(rows * a->ldx * 2);
-    void* dQKV = ws;
-    ws += align256(rows * a->ld3 * 2);
 
     prof_context(a->ids != nullptr ? "news.bwd" : "user.bwd");
     const void* QKV = a->QKV_bf16;
     if (QKV == nullptr) {  // the precise dense forward keeps no bf16 Q|K|V: recompute it from the saved rows (multihead_self.py:53-58)
-        NR_PROPAGATE(gemm_store(a->X_bf16, M, a->ldx, a->wqkv_bf16, 3 * sec, a->ldx, a->d, 1, 0, kGemmTileRows, a->bqkv, 0, ws, a->ld3, 1,
-                                kIdentity, 0, kNoDrop, -1, 0, st));
-        QKV = ws;
+        NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
+                                {.out = ws.QKV, .ld_out = a->ld3, .out_bf16 = 1, .bias = a->bqkv}, st));
+        QKV = ws.QKV;
     }
     // --- additive pooling backward ---
-    NR_PROPAGATE(pool_dscore(a->C_bf16, a->ldx, a->d, a->n_seq, a->T, a->w, a->dout, a->d, dscore, st));
-    NR_PROPAGATE(gemm_additive_dpre(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, dscore, dpre, a->ldq,
+    NR_PROPAGATE(pool_dscore(a->C_bf16, a->ldx, a->d, a->n_seq, a->T, a->w, a->dout, a->d, ws.dscore, st));
+    NR_PROPAGATE(gemm_additive_dpre(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, ws.dscore, ws.dpre, a->ldq,
                                     a->dqv, st));
-    const DropoutCfg cdrop = {a->ids != nullptr ? a->p_drop : 0.f, a->seed ^ 0x5bd1e995u};
-    NR_PROPAGATE(gemm_pool_dinput(dpre, M, a->ldq, a->q, a->waT_bf16, a->d, a->ldq, a->w, a->dout, a->d, a->T, dC, a->ldx,
-                                  kIdentity, 0, cdrop, nullptr, 0, st));
+    NR_PROPAGATE(gemm_pool_dinput({.A = ws.dpre, .M = M, .lda = a->ldq, .W = a->waT_bf16, .N = a->d, .ldw = a->ldq, .K = a->q},
+                                  {.w = a->w, .dout = a->dout, .ldo = a->d, .seg_len = a->T, .dx = ws.dC, .ld_dx = a->ldx,
+                                   .drop = context_dropout(a->ids != nullptr ? a->p_drop : 0.f, a->seed)}, st));
     // --- attention backward ---
-    NR_PROPAGATE(mhsa_core_bwd(QKV, a->ld3, sec, dC, a->ldx, a->n_seq, a->T, a->heads, a->d / a->heads, dQKV, a->ld3, st));
+    NR_PROPAGATE(mhsa_core_bwd(QKV, a->ld3, sec, ws.dC, a->ldx, a->n_seq, a->T, a->heads, a->d / a->heads, ws.dQKV, a->ld3, st));
     // --- projection backward: the input first (the embedding gradient is 97 % of a data-parallel step's all-reduce: the
     //     caller's event lets the communication start under the weight-gradient GEMM), then the weights (+bias through the
     //     ones column of X) ---
     if (a->ids != nullptr) {
         NR_REQUIRE(a->V >= 1, "nr_mhsa_encoder_bwd: V=%d", a->V);
-        NR_PROPAGATE(gemm_scatter_emb(dQKV, M, a->ld3, a->wqkvT_bf16, a->d, a->ld3, 3 * sec, 1, 0, kGemmTileRows, a->ids, a->demb, a->V, a->d,
-                                      kIdentity, DropoutCfg{a->p_drop, a->seed}, a->ldx, st));
+        NR_PROPAGATE(gemm_scatter_emb({.A = ws.dQKV, .M = M, .lda = a->ld3, .W = a->wqkvT_bf16, .N = a->d, .ldw = a->ld3, .K = 3 * sec},
+                                      {.ids = a->ids, .demb = a->demb, .V = a->V, .drop = {a->p_drop, a->seed}, .drop_ld = a->ldx}, st));
         if (a->emb_grad_ready_event != nullptr) NR_CHECK_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(a->emb_grad_ready_event), st));
     } else {
-        NR_PROPAGATE(gemm_store(dQKV, M, a->ld3, a->wqkvT_bf16, a->d, a->ld3, 3 * sec, 1, 0, kGemmTileRows, nullptr, 0, a->ddense, a->d,
-                                0, kIdentity, 0, kNoDrop, -1, 0, st));
+        NR_PROPAGATE(gemm_store({.A = ws.dQKV, .M = M, .lda = a->ld3, .W = a->wqkvT_bf16, .N = a->d, .ldw = a->ld3, .K = 3 * sec},
+                                {.out = a->ddense, .ld_out = a->d}, st));
     }
     // both weight-gradient GEMMs run AFTER the embedding gradient is complete: together they are the window (~0.4 ms) under which
     // the caller's all-reduce of that gradient hides
-    NR_PROPAGATE(gemm_tn_accumulate(dpre, M, a->q, a->ldq, a->C_bf16, M, a->d + 1, a->ldx, 0, a->d + 1, 0, a->dWa_ext,
-                                    a->ldx, st));
-    NR_PROPAGATE(gemm_tn_accumulate(dQKV, M, 3 * sec, a->ld3, a->X_bf16, M, a->d + 1, a->ldx, 0, a->d + 1, 0, a->dWqkv_ext,
-                                    a->ldx, st));
+    NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, a->q, a->ldq, a->C_bf16, a->d, a->ldx, a->dWa_ext, st));
+    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st));
     return 0;
 }
 

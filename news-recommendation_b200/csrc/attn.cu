@@ -16,8 +16,6 @@
 
 namespace nr {
 
-extern int g_launches;
-
 namespace {
 
 using namespace mma;

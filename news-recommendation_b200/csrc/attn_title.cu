@@ -30,8 +30,6 @@
 
 namespace nr {
 
-extern int g_launches;
-
 int read_attn_device_error(int* out4) {
     return static_cast<int>(cudaMemcpyFromSymbol(out4, fused::g_attn_dev_error, sizeof(int) * 4));
 }

@@ -9,8 +9,6 @@
 
 namespace nr {
 
-extern int g_launches;
-
 // ------------------------------------------------------------------------------------------------
 // fp32 parameter -> zero-padded bf16 operand (optionally transposed)
 // ------------------------------------------------------------------------------------------------

@@ -513,6 +513,12 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     return 0;
 }
 
+int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int K, int ldx, float* dW_ext, cudaStream_t stream, int x_row_shift) {
+    for (int c0 = 0; c0 < K + 1; c0 += 512)
+        NR_PROPAGATE(gemm_tn_accumulate(dY, M, N, ld_dy, X, M, K + 1, ldx, c0, std::min(512, K + 1 - c0), x_row_shift, dW_ext + c0, ldx, stream));
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------------
 // epilogue instantiations
 // ------------------------------------------------------------------------------------------------
@@ -526,53 +532,51 @@ static Dropout to_drop(const DropoutCfg& c) {
     return d;
 }
 
-int gemm_store(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,
-               int rows_per_tile, const float* bias, int relu, void* out, int ld_out, int out_bf16, RowMapCfg rm,
-               int zero_pad_rows, DropoutCfg drop, int ones_col, int ones_zero_upto, cudaStream_t stream, void* lo_out, int ld_lo,
-               int lo_col0, int accumulate) {
-    if (M == 0) return 0;
-    rows_per_tile = std::min(rows_per_tile, kTileM);  // every row is owned by exactly one tile: whole tiles are fine
+int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
+    if (g.M == 0) return 0;
+    const int M = g.M, N = g.N, rows_per_tile = std::min(c.rows_per_tile, kTileM);  // every row is owned by exactly one tile
     GemmNTPlan plan;
-    NR_PROPAGATE(plan_gemm_nt(&plan, A, M, lda, W, N, ldw, K, taps, w_tap_rows, rows_per_tile, num_sms(), 0, EpiStore::kScratchBytes, 0));
-    NR_REQUIRE(out_bf16 ? (ld_out % 8 == 0) : (ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", ld_out);
+    NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, N, g.ldw, g.K, g.taps, g.w_tap_rows, rows_per_tile, num_sms(), 0,
+                              EpiStore::kScratchBytes, 0));
+    NR_REQUIRE(c.out_bf16 ? (c.ld_out % 8 == 0) : (c.ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", c.ld_out);
     EpiStore e;
     memset(&e, 0, sizeof(e));
-    e.use_tma = (out_bf16 && rm.seg_in == 0 && rows_per_tile == kTileM && N >= 32) ? 1 : 0;
-    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, out, M, N, ld_out, 32, 32, 64));
+    e.use_tma = (c.out_bf16 && c.rm.seg_in == 0 && rows_per_tile == kTileM && N >= 32) ? 1 : 0;
+    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.out, M, N, c.ld_out, 32, 32, 64));
     e.lo_col0 = -1;
-    NR_REQUIRE(!accumulate || !out_bf16, "gemm_store: accumulation needs an fp32 output");
-    e.accumulate = accumulate;
-    if (lo_out != nullptr) {
-        NR_REQUIRE(out_bf16 && lo_col0 >= 0 && lo_col0 < N && ld_lo % 8 == 0 && ld_lo >= N - lo_col0 && (e.use_tma || lo_col0 % 8 == 0),
+    NR_REQUIRE(!c.accumulate || !c.out_bf16, "gemm_store: accumulation needs an fp32 output");
+    e.accumulate = c.accumulate;
+    if (c.lo_out != nullptr) {
+        const int lo_col0 = c.lo_col0, ld_lo = c.ld_lo;
+        NR_REQUIRE(c.out_bf16 && lo_col0 >= 0 && lo_col0 < N && ld_lo % 8 == 0 && ld_lo >= N - lo_col0 && (e.use_tma || lo_col0 % 8 == 0),
                    "gemm_store: the low plane needs bf16 output and aligned columns (N=%d lo_col0=%d ld_lo=%d)", N, lo_col0, ld_lo);
         for (int sl = 0; sl < plan.p.n_slices; ++sl) {  // a 32-column chunk never straddles the first low-plane column
             const int c0 = sl * plan.p.n_stride;
             NR_REQUIRE(!(c0 < lo_col0 && lo_col0 < c0 + plan.p.n_stride) || (lo_col0 - c0) % 32 == 0,
                        "gemm_store: low-plane start %d is not chunk aligned in the slice at column %d", lo_col0, c0);
         }
-        if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_lo, lo_out, M, N - lo_col0, ld_lo, 32, 32, 64));
+        if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_lo, c.lo_out, M, N - lo_col0, ld_lo, 32, 32, 64));
         e.lo_col0 = lo_col0;
-        e.lo_out = static_cast<__nv_bfloat16*>(lo_out);
+        e.lo_out = static_cast<__nv_bfloat16*>(c.lo_out);
         e.ld_lo = ld_lo;
     }
-    e.out = out;
-    e.ld = ld_out;
-    e.out_bf16 = out_bf16;
-    e.bias = bias;
-    e.relu = relu;
+    e.out = c.out;
+    e.ld = c.ld_out;
+    e.out_bf16 = c.out_bf16;
+    e.bias = c.bias;
+    e.relu = c.relu;
     e.N = N;
-    e.rm = to_rm(rm);
-    e.zero_pad_rows = zero_pad_rows;
-    e.drop = to_drop(drop);
-    e.ones_col = ones_col;
-    e.ones_cols_zero_upto = ones_zero_upto;
+    e.rm = to_rm(c.rm);
+    e.drop = to_drop(c.drop);
+    e.ones_col = c.ones_col;
+    e.ones_cols_zero_upto = c.ones_zero_upto;
 #ifdef NEWSREC_TRIAGE
     static const int dbg_skip = [] { const char* v = getenv("NEWSREC_EPI_DBG"); return v != nullptr && v[0] == '1' ? 1 : 0; }();
     e.dbg_skip = dbg_skip;
 #endif
     g_launches += debug_simt_gemm() ? 2 : 1;
-    ProfScope ps("gemm_store", M, N, K * taps, stream);
-    return launch_gemm_nt(plan, e, A, lda, W, ldw, stream);
+    ProfScope ps("gemm_store", M, N, g.K * g.taps, stream);
+    return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
 }
 
 int gemm_additive_pool(const void* X, int M, int lda, int D, const void* Wa, int q, int ldw, const float* ba,
@@ -625,9 +629,8 @@ int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int
     return launch_gemm_nt(plan, e, X, lda, Wa, ldw, stream);
 }
 
-int gemm_pool_dinput(const void* dpre, int M, int ld_dpre, int q, const void* WaT, int D, int ldwT, const float* w,
-                     const float* dout, int ldo, int seg_len, void* dx, int ld_dx, RowMapCfg rm, int zero_pad_rows,
-                     DropoutCfg drop, const void* relu_src, int relu_ld, cudaStream_t stream) {
+int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t stream) {
+    const int M = g.M, D = g.N, seg_len = c.seg_len;
     if (M == 0) return 0;
     NR_REQUIRE(seg_len >= 1, "pool_dinput: seg_len=%d", seg_len);
     // the epilogue stages the dOut rows of every segment a tile touches: cap the slice width so that they fit
@@ -635,52 +638,29 @@ int gemm_pool_dinput(const void* dpre, int M, int ld_dpre, int q, const void* Wa
     const int max_stride = (EpiDPoolIn::kStageFloats / nseg_max) & ~15;
     NR_REQUIRE(max_stride >= 16, "pool_dinput: seg_len=%d needs %d staged segments per tile", seg_len, nseg_max);
     GemmNTPlan plan;
-    NR_PROPAGATE(plan_gemm_nt(&plan, dpre, M, ld_dpre, WaT, D, ldwT, q, 1, 0, kTileM, num_sms(), 0,
-                              EpiDPoolIn::kScratchBytes, max_stride));
-    NR_REQUIRE(ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", ld_dx);
-    EpiDPoolIn e;
-    memset(&e, 0, sizeof(e));
-    e.use_tma = (rm.seg_in == 0 && relu_src == nullptr && D >= 32) ? 1 : 0;
-    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, dx, M, D, ld_dx, 32, 32, 64));
-    e.w = w;
-    e.dout = dout;
-    e.ldo = ldo;
-    e.seg_len = seg_len;
-    e.dx = static_cast<__nv_bfloat16*>(dx);
-    e.ld = ld_dx;
-    e.N = D;
-    e.rm = to_rm(rm);
-    e.zero_pad_rows = zero_pad_rows;
-    e.drop = to_drop(drop);
-    e.relu_src = static_cast<const __nv_bfloat16*>(relu_src);
-    e.relu_ld = relu_ld;
-    e.M = M;
-    e.rows_per_tile = kTileM;
+    NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0, EpiDPoolIn::kScratchBytes,
+                              max_stride));
+    NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
+    EpiDPoolIn e{.use_tma = (c.rm.seg_in == 0 && c.relu_src == nullptr && D >= 32) ? 1 : 0, .w = c.w, .dout = c.dout, .ldo = c.ldo,
+                 .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx, .N = D, .rm = to_rm(c.rm),
+                 .zero_pad_rows = c.zero_pad_rows, .drop = to_drop(c.drop), .relu_src = static_cast<const __nv_bfloat16*>(c.relu_src),
+                 .relu_ld = c.relu_ld, .M = M, .rows_per_tile = kTileM};
+    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.dx, M, D, c.ld_dx, 32, 32, 64));
     g_launches += debug_simt_gemm() ? 2 : 1;
-    ProfScope ps("gemm_pool_dinput", M, D, q, stream);
-    return launch_gemm_nt(plan, e, dpre, ld_dpre, WaT, ldwT, stream);
+    ProfScope ps("gemm_pool_dinput", M, D, g.K, stream);
+    return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
 }
 
-int gemm_scatter_emb(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,
-                     int rows_per_tile, const long long* ids, float* demb, int V, int D, RowMapCfg rm, DropoutCfg drop,
-                     int drop_ld, cudaStream_t stream) {
-    if (M == 0) return 0;
-    NR_REQUIRE(N == D && D % 4 == 0 && V >= 1, "scatter_emb: N=%d D=%d V=%d", N, D, V);
-    rows_per_tile = std::min(rows_per_tile, kTileM);
-    GemmNTPlan plan;
-    NR_PROPAGATE(plan_gemm_nt(&plan, A, M, lda, W, N, ldw, K, taps, w_tap_rows, rows_per_tile, num_sms(), 0,
+int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t stream) {
+    if (g.M == 0) return 0;
+    NR_REQUIRE(g.N % 4 == 0 && c.V >= 1, "scatter_emb: N=%d V=%d", g.N, c.V);
+    GemmNTPlan plan;  // every row is computed independently: whole tiles
+    NR_PROPAGATE(plan_gemm_nt(&plan, g.A, g.M, g.lda, g.W, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                               EpiScatter::kScratchBytes, 0));
-    EpiScatter e;
-    e.ids = ids;
-    e.demb = demb;
-    e.V = V;
-    e.D = D;
-    e.rm = to_rm(rm);
-    e.drop = to_drop(drop);
-    e.drop_ld = drop_ld;
+    const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = to_drop(c.drop), .drop_ld = c.drop_ld};
     g_launches += debug_simt_gemm() ? 2 : 1;
-    ProfScope ps("gemm_scatter_emb", M, N, K * taps, stream);
-    return launch_gemm_nt(plan, e, A, lda, W, ldw, stream);
+    ProfScope ps("gemm_scatter_emb", g.M, g.N, g.K * g.taps, stream);
+    return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
 }
 
 }  // namespace nr

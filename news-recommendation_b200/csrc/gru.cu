@@ -15,7 +15,6 @@
 #include "nr_ops.h"
 
 namespace nr {
-extern int g_launches;
 
 // gi: fp32 [B*S][ldg] rows (b*S + t);  gh: fp32 [B][ldg];  h: fp32 [B][Hd] (in/out);
 // hb_next: bf16 [B][ldh] operand of the next step (ones column at Hd)
@@ -106,12 +105,6 @@ __global__ void zero_pad_cols_kernel(__nv_bfloat16* __restrict__ m, long long ro
 }  // namespace nr
 
 using namespace nr;
-static inline cudaStream_t S_(void* s) { return static_cast<cudaStream_t>(s); }
-static inline long long align256(long long x) { return (x + 255) & ~255ll; }
-static inline int ru8(int x) { return (x + 7) & ~7; }
-static inline int ru4(int x) { return (x + 3) & ~3; }
-static const RowMapCfg kIdentity = {0, 0, 0, 0, 0};
-static const DropoutCfg kNoDrop = {0.f, 0};
 static inline int blocks_for(long long n) { return static_cast<int>(std::min<long long>((n + 255) / 256, 148 * 8)); }
 
 extern "C" {
@@ -125,20 +118,21 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
     NR_REQUIRE(a->x && a->len && a->h0 && a->wih_bf16 && a->whh_bf16 && a->bih && a->bhh && a->xb && a->gi && a->gh && a->hs && a->hb && a->out,
                "nr_gru_fwd: null operand");
     if (B == 0) return 0;
-    const cudaStream_t st = S_(stream);
-    const int ldg = ru4(3 * Hd), ldh = ru8(Hd + 1), ldd = ru8(D + 1);
+    const cudaStream_t st = as_stream(stream);
+    const int ldg = round_up(3 * Hd, 4), ldh = round_up(Hd + 1, 8), ldd = round_up(D + 1, 8);
     const long long BH = static_cast<long long>(B) * Hd;
     prof_context("gru.fwd");
     // gi = X Wih^T + bih over all (user, step) rows
     NR_PROPAGATE(rows_to_bf16(a->x, B, S, D, a->x_s_b, a->x_s_t, a->x_s_c, a->xb, ldd, st));
-    NR_PROPAGATE(gemm_store(a->xb, B * S, ldd, a->wih_bf16, 3 * Hd, ldd, D, 1, 0, kGemmTileRows, a->bih, 0, a->gi, ldg, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+    NR_PROPAGATE(gemm_store({.A = a->xb, .M = B * S, .lda = ldd, .W = a->wih_bf16, .N = 3 * Hd, .ldw = ldd, .K = D},
+                            {.out = a->gi, .ld_out = ldg, .bias = a->bih}, st));
     if (a->x_lo_bf16 != nullptr) {
         // accurate mode: the news vectors enter as a hi/lo bf16 pair, gi = x_hi . W_ih^T + b + x_lo . W_ih^T.  Two passes over the
         // SAME resident weights with fp32 accumulation into gi: a K-concatenated single pass doubles K, which shrinks the weight-
         // stationary slices to N = 80 and costs 0.86 ms instead of 2 x 0.23
         NR_PROPAGATE(rows_to_bf16_lo(a->x, B, S, D, a->x_s_b, a->x_s_t, a->x_s_c, a->x_lo_bf16, ldd, st));
-        NR_PROPAGATE(gemm_store(a->x_lo_bf16, B * S, ldd, a->wih_bf16, 3 * Hd, ldd, D, 1, 0, kGemmTileRows, nullptr, 0, a->gi, ldg, 0, kIdentity, 0, kNoDrop,
-                                -1, 0, st, nullptr, 0, 0, 1));
+        NR_PROPAGATE(gemm_store({.A = a->x_lo_bf16, .M = B * S, .lda = ldd, .W = a->wih_bf16, .N = 3 * Hd, .ldw = ldd, .K = D},
+                                {.out = a->gi, .ld_out = ldg, .accumulate = 1}, st));
     }
     // h_0
     NR_CHECK_CUDA(cudaMemcpyAsync(a->hs, a->h0, sizeof(float) * BH, cudaMemcpyDeviceToDevice, st));
@@ -153,7 +147,8 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
         const void* hb_t = static_cast<const __nv_bfloat16*>(a->hb) + static_cast<size_t>(t) * B * ldh;
         __nv_bfloat16* hb_n = static_cast<__nv_bfloat16*>(a->hb) + static_cast<size_t>(t + 1) * B * ldh;
         float* h_n = a->hs + static_cast<size_t>(t + 1) * BH;
-        NR_PROPAGATE(gemm_store(hb_t, B, ldh, a->whh_bf16, 3 * Hd, ldh, Hd, 1, 0, kGemmTileRows, a->bhh, 0, gh_t, ldg, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+        NR_PROPAGATE(gemm_store({.A = hb_t, .M = B, .lda = ldh, .W = a->whh_bf16, .N = 3 * Hd, .ldw = ldh, .K = Hd},
+                                {.out = gh_t, .ld_out = ldg, .bias = a->bhh}, st));
         NR_CHECK_CUDA(cudaMemcpyAsync(h_n, a->hs + static_cast<size_t>(t) * BH, sizeof(float) * BH, cudaMemcpyDeviceToDevice, st));
         {
             ProfScope ps("gru_gate_fwd", B, Hd, t, st);
@@ -168,10 +163,16 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
 
 int nr_gru_persistent_supported(int B, int Hd) { return gru_persistent_supported(B, Hd); }
 
-long long nr_gru_bwd_workspace(int B, int S, int D, int Hd) {
-    const long long ldb = ru8(3 * Hd + 1), BP = static_cast<long long>(B) * ru4(Hd);
-    return align256(static_cast<long long>(B) * S * ldb * 2) * 2 + align256(BP * 4) * 2 + 256;
-}
+// dgi bf16 [B*S][ldb] (rows b*S+t), dgh bf16 [S][B][ldb] with ldb = round_up(3Hd+1, 8); dh_direct / dh_rec fp32 [B][round_up(Hd, 4)]
+struct GruBwdWorkspace : WorkspaceLayout {
+    __nv_bfloat16 *dgi, *dgh;
+    float *dh_direct, *dh_rec;
+    GruBwdWorkspace(void* base, long long B, int S, int Hd)
+        : WorkspaceLayout{static_cast<char*>(base)}, dgi(take<__nv_bfloat16>(B * S * round_up(3 * Hd + 1, 8))),
+          dgh(take<__nv_bfloat16>(B * S * round_up(3 * Hd + 1, 8))), dh_direct(take<float>(B * round_up(Hd, 4))),
+          dh_rec(take<float>(B * round_up(Hd, 4))) {}
+};
+long long nr_gru_bwd_workspace(int B, int S, int D, int Hd) { return GruBwdWorkspace(nullptr, B, S, Hd).bytes(); }
 
 int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_gru_bwd: null args");
@@ -179,24 +180,17 @@ int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream) {
     NR_REQUIRE(B >= 0 && S >= 1 && D % 4 == 0 && Hd % 2 == 0, "nr_gru_bwd: bad shape B=%d S=%d D=%d Hd=%d", B, S, D, Hd);
     NR_REQUIRE(a->len && a->wihT_bf16 && a->whhT_bf16 && a->xb && a->gi && a->gh && a->hs && a->hb && a->dout && a->dWih_ext && a->dWhh_ext &&
                    a->dx && a->dh0 && a->workspace, "nr_gru_bwd: null operand");
-    NR_REQUIRE(a->workspace_bytes >= nr_gru_bwd_workspace(B, S, D, Hd), "nr_gru_bwd: workspace too small");
+    const GruBwdWorkspace ws(a->workspace, B, S, Hd);
+    NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_gru_bwd: workspace too small");
     if (B == 0) return 0;
-    const cudaStream_t st = S_(stream);
-    const int ldg = ru4(3 * Hd), ldh = ru8(Hd + 1), ldd = ru8(D + 1), ldb = ru8(3 * Hd + 1);
+    const cudaStream_t st = as_stream(stream);
+    const int ldg = round_up(3 * Hd, 4), ldh = round_up(Hd + 1, 8), ldd = round_up(D + 1, 8), ldb = round_up(3 * Hd + 1, 8);
     const long long BH = static_cast<long long>(B) * Hd;
-    char* ws = static_cast<char*>(a->workspace);
-    __nv_bfloat16* dgi = reinterpret_cast<__nv_bfloat16*>(ws);            // [B*S][ldb]  rows b*S+t
-    ws += align256(static_cast<long long>(B) * S * ldb * 2);
-    __nv_bfloat16* dgh = reinterpret_cast<__nv_bfloat16*>(ws);            // [S][B][ldb]
-    ws += align256(static_cast<long long>(B) * S * ldb * 2);
-    const int P = ru4(Hd);  // pitch of the internal dh buffers (fp32 vector stores of the GEMM epilogue)
-    float* dh_direct = reinterpret_cast<float*>(ws);
-    ws += align256(static_cast<long long>(B) * P * 4);
-    float* dh_rec = reinterpret_cast<float*>(ws);
+    const int P = round_up(Hd, 4);  // pitch of the internal dh buffers (fp32 vector stores of the GEMM epilogue)
     prof_context("gru.bwd");
     {   // pad columns [3Hd, ldb) of both gradient matrices are K-extent-masked by TMA but read by nothing else: keep them clean
-        zero_pad_cols_kernel<<<blocks_for(static_cast<long long>(B) * S * (ldb - 3 * Hd)), 256, 0, st>>>(dgi, static_cast<long long>(B) * S, 3 * Hd, ldb);
-        zero_pad_cols_kernel<<<blocks_for(static_cast<long long>(B) * S * (ldb - 3 * Hd)), 256, 0, st>>>(dgh, static_cast<long long>(B) * S, 3 * Hd, ldb);
+        zero_pad_cols_kernel<<<blocks_for(static_cast<long long>(B) * S * (ldb - 3 * Hd)), 256, 0, st>>>(ws.dgi, static_cast<long long>(B) * S, 3 * Hd, ldb);
+        zero_pad_cols_kernel<<<blocks_for(static_cast<long long>(B) * S * (ldb - 3 * Hd)), 256, 0, st>>>(ws.dgh, static_cast<long long>(B) * S, 3 * Hd, ldb);
         g_launches += 2;
     }
     const float* dha = a->dout;
@@ -204,33 +198,29 @@ int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream) {
     int pa = Hd;
     for (int t = S - 1; t >= 0; --t) {
         const float* gh_t = a->gh + static_cast<size_t>(t) * B * ldg;
-        __nv_bfloat16* dgh_t = dgh + static_cast<size_t>(t) * B * ldb;
+        __nv_bfloat16* dgh_t = ws.dgh + static_cast<size_t>(t) * B * ldb;
         {
             ProfScope ps("gru_gate_bwd", B, Hd, t, st);
             gru_gate_bwd_kernel<<<blocks_for(BH), 256, 0, st>>>(a->gi, gh_t, ldg, a->hs + static_cast<size_t>(t) * BH, dha, pa, dhb, P, a->len, B, S,
-                                                               Hd, t, dgi, dgh_t, ldb, dh_direct, P);
+                                                               Hd, t, ws.dgi, dgh_t, ldb, ws.dh_direct, P);
             ++g_launches;
         }
         NR_CHECK_CUDA(cudaGetLastError());
         // recurrent path: dh_{t-1} += dgh_t . Whh
-        NR_PROPAGATE(gemm_store(dgh_t, B, ldb, a->whhT_bf16, Hd, ldb, 3 * Hd, 1, 0, kGemmTileRows, nullptr, 0, dh_rec, P, 0, kIdentity, 0, kNoDrop, -1, 0, st));
-        dha = dh_direct;
-        dhb = dh_rec;
+        NR_PROPAGATE(gemm_store({.A = dgh_t, .M = B, .lda = ldb, .W = a->whhT_bf16, .N = Hd, .ldw = ldb, .K = 3 * Hd},
+                                {.out = ws.dh_rec, .ld_out = P}, st));
+        dha = ws.dh_direct;
+        dhb = ws.dh_rec;
         pa = P;
     }
     add2_kernel<<<blocks_for(BH), 256, 0, st>>>(dha, pa, dhb, P, a->dh0, B, Hd);
     ++g_launches;
     // weight gradients over all (step, user) rows; the ones column of the saved operands yields the bias gradients
-    for (int c0 = 0; c0 < Hd + 1; c0 += 512) {
-        const int nb = std::min(512, Hd + 1 - c0);
-        NR_PROPAGATE(gemm_tn_accumulate(dgh, B * S, 3 * Hd, ldb, a->hb, B * S, Hd + 1, ldh, c0, nb, 0, a->dWhh_ext + c0, ldh, st));
-    }
-    for (int c0 = 0; c0 < D + 1; c0 += 512) {
-        const int nb = std::min(512, D + 1 - c0);
-        NR_PROPAGATE(gemm_tn_accumulate(dgi, B * S, 3 * Hd, ldb, a->xb, B * S, D + 1, ldd, c0, nb, 0, a->dWih_ext + c0, ldd, st));
-    }
+    NR_PROPAGATE(gemm_weight_grad(ws.dgh, B * S, 3 * Hd, ldb, a->hb, Hd, ldh, a->dWhh_ext, st));
+    NR_PROPAGATE(gemm_weight_grad(ws.dgi, B * S, 3 * Hd, ldb, a->xb, D, ldd, a->dWih_ext, st));
     // input gradient
-    NR_PROPAGATE(gemm_store(dgi, B * S, ldb, a->wihT_bf16, D, ldb, 3 * Hd, 1, 0, kGemmTileRows, nullptr, 0, a->dx, D, 0, kIdentity, 0, kNoDrop, -1, 0, st));
+    NR_PROPAGATE(gemm_store({.A = ws.dgi, .M = B * S, .lda = ldb, .W = a->wihT_bf16, .N = D, .ldw = ldb, .K = 3 * Hd},
+                            {.out = a->dx, .ld_out = D}, st));
     return 0;
 }
 

@@ -21,8 +21,6 @@
 
 namespace nr {
 
-extern int g_launches;
-
 int read_attn_device_error(int* out4);
 int read_gru_device_error(int* out4) {
     const int rc = static_cast<int>(cudaMemcpyFromSymbol(out4, fused::g_gru_dev_error, sizeof(int) * 4));

@@ -568,11 +568,4 @@ int launch_gemm_nt(const GemmNTPlan& plan, const Epi& epi, const void* A, int ld
     return 0;
 }
 
-// D[Ma x Nb] (+)= A[:, 0:Ma]^T . B[shifted rows, b_col0 : b_col0+Nb]
-int launch_gemm_tn(const void* A, int Kr, int Ma, int lda, const void* B, int b_rows, int b_cols, int ldb, int b_col0,
-                   int Nb, int b_row_shift, float* D, int ldd, int num_sms, cudaStream_t stream);
-
-int num_sms();
-extern int g_launches;  // kernels launched by this library (bench.py reports it)
-
 }  // namespace nr

@@ -16,19 +16,32 @@ struct RowMapCfg {  // see RowMap in nr_epilogues.cuh; seg_in == 0 => identity
 };
 
 // ---- wgmma GEMMs with fused epilogues (gemm.cu) ------------------------------------------------
-// rows_per_tile: rows of A owned by one 64-row tile (kGemmTileRows).  gemm_store / gemm_scatter_emb compute every row
-// independently (conv taps read their neighbour rows through shifted loads), so they take whole tiles; larger values are
-// clamped to the tile.
-constexpr int kGemmTileRows = 64;
-// out[rows x N] = act(A . W^T + bias) (bf16 or fp32).  A bf16 [M x K] pitch lda (taps>1: padded CNN layout),
-// W bf16 [taps*w_tap_rows x K] pitch ldw.
-int gemm_store(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,
-               int rows_per_tile, const float* bias, int relu, void* out, int ld_out, int out_bf16, RowMapCfg rm,
-               int zero_pad_rows, DropoutCfg drop, int ones_col, int ones_zero_upto, cudaStream_t stream,
-               void* lo_out = nullptr, int ld_lo = 0, int lo_col0 = 0, int accumulate = 0);
-// accumulate (fp32 output only): out += A . W^T (+ bias) instead of out =
-// lo_out (bf16 [M][ld_lo], identity rows, bf16 output only): columns [lo_col0, N) additionally leave as a LOW plane,
-// lo[r][c - lo_col0] = bf16(y - bf16(y)), so that a consumer can read y as a hi/lo bf16 pair (~16 mantissa bits)
+constexpr int kGemmTileRows = 64;  // rows of A per gemm_nt tile
+// Operands of the GEMMs with optional epilogue features, which callers name: gemm_store({.A = X, .M = M, ...}, {.out = Y, ...}, st).
+// A bf16 [M x K] pitch lda (taps 3: the zero-padded CNN layout, tap s reads row r + s - 1); W bf16 [taps * w_tap_rows x K] pitch ldw
+struct GemmOperands {
+    const void* A;
+    int M, lda;
+    const void* W;
+    int N, ldw, K, taps = 1, w_tap_rows = 0;
+};
+
+// out[M x N] = act(A . W^T + bias), bf16 or fp32; the defaults are fp32 "=", identity rows, no dropout
+struct StoreCfg {
+    void* out;
+    int ld_out, out_bf16 = 0, relu = 0;
+    const float* bias = nullptr;
+    RowMapCfg rm = {};
+    DropoutCfg drop = {};
+    int ones_col = -1, ones_zero_upto = 0;  // bf16 output: column ones_col = 1, (ones_col, ones_zero_upto) = 0 (bias of the next GEMM)
+    // bf16 output, identity rows: columns [lo_col0, N) also leave a LOW plane lo[r][c - lo_col0] = bf16(y - bf16(y)) in lo_out
+    // (bf16 [M][ld_lo]), so that a consumer can read y as a hi/lo bf16 pair (~16 mantissa bits)
+    void* lo_out = nullptr;
+    int ld_lo = 0, lo_col0 = 0;
+    int accumulate = 0;                 // fp32 output only: out += A . W^T (+ bias)
+    int rows_per_tile = kGemmTileRows;  // rows are computed independently: larger values are clamped to the tile
+};
+int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream);
 
 // additive-attention pooling: out[seg][D] = sum_r softmax_seg(tanh(X Wa^T + ba) . qv)_r X_r ; w_out[rows]
 // X_lo (may be null): a second bf16 plane with X = X_hi + X_lo; the scores use X_hi, the pooled sum both planes.
@@ -41,19 +54,39 @@ int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int
                        const float* qv, const float* dscore, void* dpre, int ld_dpre, float* dqv,
                        cudaStream_t stream);
 
-// dX = dPre . Wa + w (x) dOut  [* relu mask] [* dropout]  -> bf16 (optionally re-mapped to the padded layout)
-int gemm_pool_dinput(const void* dpre, int M, int ld_dpre, int q, const void* WaT, int D, int ldwT, const float* w,
-                     const float* dout, int ldo, int seg_len, void* dx, int ld_dx, RowMapCfg rm, int zero_pad_rows,
-                     DropoutCfg drop, const void* relu_src, int relu_ld, cudaStream_t stream);
+// dX = dPre . Wa + w (x) dOut [* relu mask] [* dropout] -> bf16, on {.A = dPre, .N = D, .K = q, .W = Wa^T}; w and dOut
+// (pitch ldo) are the pooling weights and output gradient of segments of seg_len rows
+struct PoolDInputCfg {
+    const float *w, *dout;
+    int ldo, seg_len;
+    void* dx;
+    int ld_dx;
+    RowMapCfg rm = {};
+    int zero_pad_rows = 0;  // with a compact -> padded row map: also zero the pad rows around each segment
+    DropoutCfg drop = {};
+    const void* relu_src = nullptr;  // non-null: multiply by (relu_src > 0), pitch relu_ld (ReLU backward of the CNN)
+    int relu_ld = 0;
+};
+int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t stream);
 
-// dEmb[ids[row]] += A . W^T  (embedding gradient; padding row 0 skipped) [* dropout of the gathered rows]
-int gemm_scatter_emb(const void* A, int M, int lda, const void* W, int N, int ldw, int K, int taps, int w_tap_rows,
-                     int rows_per_tile, const long long* ids, float* demb, int V, int D, RowMapCfg rm, DropoutCfg drop,
-                     int drop_ld, cudaStream_t stream);
+// dEmb[ids[row]] += A . W^T (embedding gradient of a [V x N] table; padding row 0 skipped) [* dropout of the gathered rows, pitch drop_ld]
+struct ScatterEmbCfg {
+    const long long* ids;
+    float* demb;
+    int V;
+    RowMapCfg rm = {};
+    DropoutCfg drop = {};
+    int drop_ld = 0;
+};
+int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t stream);
 
-// D[Ma x Nb] += A[:, :Ma]^T . B[rows + shift, b_col0 : b_col0 + Nb]   (fp32 accumulate into D, pitch ldd)
+// D[Ma x Nb] += A[:, :Ma]^T . B[rows + shift, b_col0 : b_col0 + Nb]   (fp32 accumulate into D, pitch ldd; Nb <= 512)
 int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, int b_rows, int b_cols, int ldb,
                        int b_col0, int Nb, int b_row_shift, float* D, int ldd, cudaStream_t stream);
+// Linear weight gradient: dW_ext[N][0..K] += dY^T . [X | 1] over M rows, dY pitch ld_dy, X read at row r + x_row_shift.  Column K of
+// X is its ones column, so column K of dW_ext (same pitch ldx) is the bias gradient.  Launches of <= 512 columns, left to right.
+int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int K, int ldx, float* dW_ext, cudaStream_t stream,
+                     int x_row_shift = 0);
 
 // ---- memory-bound companions (aux.cu) --------------------------------------------------------------
 // fp32 [R x C] (pitch lds) -> bf16 [R x ld] zero padded; transpose: out[c][r] = in[r][c] (out is [C x ld])
@@ -116,6 +149,7 @@ int segment_dot(const float* news, long long n_news, int D, const long long* can
 int slots_device_readable(const void* const* slots, int n);
 int pack_slots(const void* const* slots, int H, int C, int B, int L, long long* out, cudaStream_t stream);
 int num_sms();
+extern int g_launches;  // kernels launched by this library (nr_launch_count)
 
 // ---- live per-kernel timing (bench.py): CUDA events on the launching stream around every kernel ------
 // Off by default.  A ProfScope brackets one kernel launch; names are "<context>/<op>[shape]".
@@ -127,6 +161,25 @@ struct ProfScope {
     ~ProfScope();
     int idx;
     cudaStream_t stream;
+};
+
+// ---- host conventions of the C-ABI composites (abi.cu, abi_cnn.cu, gru.cu) --------------------------
+static inline cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
+static inline long long align256(long long x) { return (x + 255) & ~255ll; }
+// Dropout on the attention context / conv output: the forward and the backward of a composite must draw this same mask.
+// The Python reference model of the kernels (the oracle) restates the salt for the same two masks.
+static inline DropoutCfg context_dropout(float p, uint64_t seed) { return {p, seed ^ 0x5bd1e995u}; }
+// Back-to-back 256-byte aligned slots of a backward's workspace, plus 256 bytes at the end.  Over a null base it only
+// measures, so a composite's *_workspace() size and the buffers its backward carves come from one layout (derive from it).
+struct WorkspaceLayout {
+    char* base;
+    long long used = 0;
+    template <class T> T* take(long long count) {
+        T* p = base != nullptr ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += align256(count * static_cast<long long>(sizeof(T)));
+        return p;
+    }
+    long long bytes() const { return used + 256; }
 };
 
 }  // namespace nr
