@@ -224,7 +224,7 @@ int make_tmap_bytes_2d(CUtensorMap* out, const void* base, int64_t rows, int64_t
 // gemm_nt planning
 // ------------------------------------------------------------------------------------------------
 int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B, int N, int ldb, int K, int taps,
-                 int b_tap_rows, int rows_per_tile, int sms, int max_slices, int scratch_bytes, int max_n_stride) {
+                 int b_tap_rows, int rows_per_tile, int sms, int max_slices, int epi_smem_bytes, int max_n_stride) {
     NR_REQUIRE(M >= 0 && N >= 1 && K >= 1 && taps >= 1 && rows_per_tile >= 1 && rows_per_tile <= kTileM,
                "plan_gemm_nt: bad shape M=%d N=%d K=%d taps=%d rpt=%d", M, N, K, taps, rows_per_tile);
     NR_REQUIRE(sms > 0, "no CUDA device (SM count unknown)");
@@ -247,7 +247,7 @@ int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B,
         fprintf(stderr, "[nr] gemm timing slot %d: M=%d N=%d K=%d taps=%d\n", g_gemm_timing_next, M, N, K, taps);
         ++g_gemm_timing_next;
     }
-    const int fixed = 1024 + kXposeBytes + round_up(scratch_bytes, 16) + 512;
+    const int fixed = 1024 + round_up(epi_smem_bytes, 16) + 512;
     int slices = 1;
     long bbytes = 0;
     for (;; ++slices) {
@@ -537,12 +537,12 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
     const int M = g.M, N = g.N, rows_per_tile = std::min(c.rows_per_tile, kTileM);  // every row is owned by exactly one tile
     GemmNTPlan plan;
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, N, g.ldw, g.K, g.taps, g.w_tap_rows, rows_per_tile, num_sms(), 0,
-                              EpiStore::kScratchBytes, 0));
+                              kEpiSmemBytes<EpiStore>, 0));
     NR_REQUIRE(c.out_bf16 ? (c.ld_out % 8 == 0) : (c.ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", c.ld_out);
     EpiStore e;
     memset(&e, 0, sizeof(e));
     e.use_tma = (c.out_bf16 && c.rm.seg_in == 0 && rows_per_tile == kTileM && N >= 32) ? 1 : 0;
-    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.out, M, N, c.ld_out, 32, 32, 64));
+    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.out, M, N, c.ld_out, 32, 16, 64));
     e.lo_col0 = -1;
     NR_REQUIRE(!c.accumulate || !c.out_bf16, "gemm_store: accumulation needs an fp32 output");
     e.accumulate = c.accumulate;
@@ -555,7 +555,7 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
             NR_REQUIRE(!(c0 < lo_col0 && lo_col0 < c0 + plan.p.n_stride) || (lo_col0 - c0) % 32 == 0,
                        "gemm_store: low-plane start %d is not chunk aligned in the slice at column %d", lo_col0, c0);
         }
-        if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_lo, c.lo_out, M, N - lo_col0, ld_lo, 32, 32, 64));
+        if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_lo, c.lo_out, M, N - lo_col0, ld_lo, 32, 16, 64));
         e.lo_col0 = lo_col0;
         e.lo_out = static_cast<__nv_bfloat16*>(c.lo_out);
         e.ld_lo = ld_lo;
@@ -586,7 +586,7 @@ int gemm_additive_pool(const void* X, int M, int lda, int D, const void* Wa, int
     NR_REQUIRE(q <= 256 && (D % 2) == 0 && (ldo % 2) == 0, "additive_pool: q=%d D=%d ldo=%d unsupported", q, D, ldo);
     const int rpt = (kTileM / seg_len) * seg_len;
     GemmNTPlan plan;
-    NR_PROPAGATE(plan_gemm_nt(&plan, X, M, lda, Wa, q, ldw, D, 1, 0, rpt, num_sms(), 1, EpiPool::kScratchBytes, 0));
+    NR_PROPAGATE(plan_gemm_nt(&plan, X, M, lda, Wa, q, ldw, D, 1, 0, rpt, num_sms(), 1, kEpiSmemBytes<EpiPool>, 0));
     NR_REQUIRE(plan.p.n_slices == 1, "additive_pool: the query dimension must fit one weight slice (q=%d D=%d)", q, D);
     EpiPool e;
     e.bias = ba;
@@ -612,7 +612,7 @@ int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int
     if (M == 0) return 0;
     NR_REQUIRE(q <= 256 && ld_dpre % 8 == 0 && ld_dpre >= round_up(q, 8), "additive_dpre: q=%d ld=%d", q, ld_dpre);
     GemmNTPlan plan;
-    NR_PROPAGATE(plan_gemm_nt(&plan, X, M, lda, Wa, q, ldw, D, 1, 0, kTileM, num_sms(), 1, EpiDPre::kScratchBytes, 0));
+    NR_PROPAGATE(plan_gemm_nt(&plan, X, M, lda, Wa, q, ldw, D, 1, 0, kTileM, num_sms(), 1, kEpiSmemBytes<EpiDPre>, 0));
     NR_REQUIRE(plan.p.n_slices == 1, "additive_dpre: q=%d D=%d does not fit one weight slice", q, D);
     EpiDPre e;
     memset(&e, 0, sizeof(e));
@@ -638,7 +638,7 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
     const int max_stride = (EpiDPoolIn::kStageFloats / nseg_max) & ~15;
     NR_REQUIRE(max_stride >= 16, "pool_dinput: seg_len=%d needs %d staged segments per tile", seg_len, nseg_max);
     GemmNTPlan plan;
-    NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0, EpiDPoolIn::kScratchBytes,
+    NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0, kEpiSmemBytes<EpiDPoolIn>,
                               max_stride));
     NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
     EpiDPoolIn e{.use_tma = (c.rm.seg_in == 0 && c.relu_src == nullptr && D >= 32) ? 1 : 0, .w = c.w, .dout = c.dout, .ldo = c.ldo,
@@ -656,7 +656,7 @@ int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t
     NR_REQUIRE(g.N % 4 == 0 && c.V >= 1, "scatter_emb: N=%d V=%d", g.N, c.V);
     GemmNTPlan plan;  // every row is computed independently: whole tiles
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, g.M, g.lda, g.W, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
-                              EpiScatter::kScratchBytes, 0));
+                              kEpiSmemBytes<EpiScatter>, 0));
     const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = to_drop(c.drop), .drop_ld = c.drop_ld};
     g_launches += debug_simt_gemm() ? 2 : 1;
     ProfScope ps("gemm_scatter_emb", g.M, g.N, g.K * g.taps, stream);

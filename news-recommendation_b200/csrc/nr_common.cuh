@@ -153,11 +153,14 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 }
 
 // TMA store of one box from shared memory (bulk async-group completion)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                      reinterpret_cast<uint64_t>(m)),
-                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+                 "r"(smem_src), "r"(c0), "r"(c1)
                  : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+    tma_store_2d(m, smem_u32(smem_src), c0, c1);
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
@@ -177,6 +180,22 @@ __device__ __forceinline__ float lds_f(const float* p) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_u32(p)));
     return v;
+}
+__device__ __forceinline__ float2 lds_f2(const float* p) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(p)));
+    return v;
+}
+__device__ __forceinline__ uint4 lds_u4(uint32_t saddr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
+    return v;
+}
+// Four 8x8 b16 matrices to shared memory: lanes 8m .. 8m+7 give the row addresses of matrix m, and register m of lane t holds
+// row t/4, columns 2(t%4) and 2(t%4)+1 of matrix m -- the mma accumulator layout, packed to bf16 pairs.
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
 }
 // 4-byte cp.async with zero fill when !pred (src must still be a valid address)
 __device__ __forceinline__ void cp_async_f32(float* smem_dst, const float* gsrc, bool pred) {

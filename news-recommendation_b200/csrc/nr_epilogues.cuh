@@ -1,8 +1,10 @@
-// Fused epilogue functors for gemm_nt.  A tile (64 rows) belongs to one consumer warpgroup, 128 threads: thread t of the
+// Fused epilogue functors for gemm_nt.  A tile (64 rows) belongs to one consumer warpgroup, 128 threads.  A fragment-view
+// functor (kFragmentView, EpiStore) gets frag(acc, FragCtx): warp w of the warpgroup handles tile rows 16w .. 16w + 15 of every
+// column of the slice straight from the wgmma fragment.  A row-view functor gets operator()(acc, EpiCtx): thread t of the
 // warpgroup owns accumulator row r = 32*((t>>5)&1) + lane and column half t>>6; the two halves split the slice's 32-column
 // chunks as epi_chunk_range does ([ch0, ch1), warp-uniform).  Contract for every functor:
-//   * the accumulator is read through epi_chunks() (nr_gemm.cuh): c.rounds loads per tile, collective over the warpgroup,
-//     acc.release() exactly once per tile
+//   * row view: the accumulator is read through epi_chunks() (nr_gemm.cuh): c.rounds loads per tile, collective over the
+//     warpgroup, acc.release() exactly once per tile
 //   * operator() synchronises only its own warpgroup (epi_bar_sync(c.wg)); the other warpgroup is issuing wgmmas meanwhile
 //   * init()/finish() bracket the CTA's whole tile loop (all 256 consumer threads call them; consumers_bar_sync())
 //   * kScratchBytes of shared memory belong to the functor (the planner sizes the A ring around it); per-tile state is
@@ -60,12 +62,6 @@ struct Dropout {
     }
 };
 
-// 16 bf16 = one full 32-byte sector per thread, as two 16-byte stores (sm_90 has no 32-byte store).
-__device__ __forceinline__ void store_bf16x16(__nv_bfloat16* o, const float* y) {
-    uint4* q = reinterpret_cast<uint4*>(o);
-    q[0] = make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7]));
-    q[1] = make_uint4(pack_bf16x2(y[8], y[9]), pack_bf16x2(y[10], y[11]), pack_bf16x2(y[12], y[13]), pack_bf16x2(y[14], y[15]));
-}
 __device__ __forceinline__ bool aligned32(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 31) == 0; }
 
 __device__ __forceinline__ void store_bf16x8(__nv_bfloat16* o, const float* y, int nvalid) {
@@ -80,18 +76,28 @@ __device__ __forceinline__ void store_bf16x8(__nv_bfloat16* o, const float* y, i
 }
 
 // ------------------------------------------------------------------------------------------------
-// out = act(acc + bias) [* dropout]  ->  bf16 or fp32, optional row re-map, optional "ones" column
-// scratch floats: [0,256) bias of the slice | then the WarpTileStore staging region
+// out = act(acc + bias) [* dropout]  ->  bf16 or fp32, optional row re-map, optional "ones" column, optional low plane
+// Fragment view: every output element is independent, so each warp writes its own 16 rows of the tile straight from the
+// wgmma fragment, with no transpose and no barrier across warps.  A 32-column bf16 chunk is packed into one of the warp's
+// staging boxes with stmatrix and leaves by TMA (identity rows) or as 16-byte row pieces (mapped rows); fp32 output and bf16
+// chunks cut by the slice's end leave from the fragment, a quad of lanes covering 8 contiguous columns of a row.
+// scratch: [0, 1 KB) bias of the slice (zero past ncols) | kBoxes staging boxes per consumer warp (1 KB aligned)
 // ------------------------------------------------------------------------------------------------
 struct EpiStore {
-    static constexpr int kScratchBytes = 1024 + kTileStoreBytes;
-    CUtensorMap tm_out;  // bf16 output as a TMA tensor (32 x 32 boxes, SWIZZLE_64B); valid when use_tma
+    static constexpr bool kFragmentView = true;
+    // a box is 16 rows x 32 bf16 in the SWIZZLE_64B layout (16-byte piece q of row r at r*64 + ((q ^ (r>>1)) & 3)*16: the eight
+    // rows of one stmatrix matrix land in eight different bank groups).  A slice issues up to 2 x 8 stores per tile; the ring
+    // lets six of them be in flight before a box is reused.
+    static constexpr int kBoxBytes = 16 * 64;
+    static constexpr int kBoxes = 6;
+    static constexpr int kScratchBytes = 1024 + kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    CUtensorMap tm_out;  // bf16 output as a TMA tensor (32 x 16 boxes, SWIZZLE_64B); valid when use_tma
     CUtensorMap tm_lo;   // low plane of the columns >= lo_col0 (bf16(y - bf16(y))), its column 0 = output column lo_col0
     int accumulate;      // fp32 output only: out += result
     int lo_col0;         // < 0: no low plane
-    __nv_bfloat16* lo_out;  // the same plane for the (rare) partial chunks that leave through plain stores; pitch ld_lo
+    __nv_bfloat16* lo_out;  // the same plane for the chunks that leave without TMA; pitch ld_lo
     int ld_lo;
-    int use_tma;         // identity row map + bf16 output: full 32-column chunks leave through WarpTileStore
+    int use_tma;         // identity row map + bf16 output + whole 64-row tiles: bf16 chunks leave through tm_out / tm_lo
     void* out;
     int ld;
     int out_bf16;
@@ -99,145 +105,179 @@ struct EpiStore {
     int relu;
     int N;              // total valid columns
     RowMap rm;
-    int zero_pad_rows;  // compact->padded: the first/last token also zero the neighbouring pad row
     Dropout drop;
     int ones_col;       // >=0: column set to 1.0 (bias-gradient trick for the next weight-grad GEMM); -1 off
     int ones_cols_zero_upto;  // columns (ones_col, upto) are zeroed
-    int dbg_skip;       // tuning only (NEWSREC_EPI_DBG=1): release the accumulator untouched -> MMA/TMA pipeline alone
+    int dbg_skip;       // tuning only (NEWSREC_EPI_DBG=1): leave the accumulators untouched -> MMA/TMA pipeline alone
 
     __device__ void init(const EpiInit& e, int) const {
         for (int i = e.tid; i < 256; i += kEpiThreads) e.scratch[i] = (bias != nullptr && i < e.ncols) ? bias[e.col0 + i] : 0.f;
         consumers_bar_sync();
     }
     __device__ void finish(const EpiInit& e) const {
-        if (use_tma) WarpTileStore::drain(e.tid & 31);
+        if (use_tma && (e.tid & 31) == 0) bulk_wait_all();
     }
 
-    template <class Acc>
-    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
-        long long orow;
-        int t;
-        const bool v = rm.map(c.grow, orow, t) && c.valid;
+    __device__ __forceinline__ void frag(const float* acc, const FragCtx& f) const {
 #ifdef NEWSREC_TRIAGE
-        if (dbg_skip) {
-            acc.release();
-            return;
-        }
+        if (dbg_skip) return;
 #endif
-        const int lane = c.tid & 31;
-        WarpTileStore ts;
-        ts.attach(c.scratch + 256, c.tid >> 5);
-        if (use_tma) ts.begin_tile(lane);
-        epi_chunks(
-            acc, c, [](int) {},
-            [&](int ch, float* x) {
-                const int lc0 = ch * 32;
-                const bool whole = use_tma && lc0 + 32 <= c.ncols;  // warp-uniform
-                // row-mapped bf16 output (conv forward: padded rows -> compact rows): full chunks leave through the staging tile
-                // as coalesced stores (WarpTileStore::put_rows) instead of one 16/32-byte store per lane and row
-                const bool coop = !use_tma && out_bf16 && lc0 + 32 <= c.ncols && c.col0 + lc0 + 32 <= N && (ld & 7) == 0 &&
-                                  ((c.col0 + lc0) & 7) == 0;  // warp-uniform
-                if (!whole && !coop && !v) return;
+        const int lane = threadIdx.x & 31;
+        // this lane's rows e = 0, 1: tile row 16 wq + lane / 4 + 8e
+        long long orow[2];
+        bool v[2];
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {  // bias from shared memory (zero past ncols)
-                    const float4 b4 = lds_f4(c.scratch + lc0 + j);
-                    x[j] += b4.x; x[j + 1] += b4.y; x[j + 2] += b4.z; x[j + 3] += b4.w;
+        for (int e = 0; e < 2; ++e) {
+            const int r = 16 * f.wq + (lane >> 2) + 8 * e;
+            int t;
+            v[e] = rm.map(f.row0 + r, orow[e], t) && r < f.rows;
+        }
+        const uint32_t ring = ((smem_u32(f.scratch + 256) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
+        // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8 addressing row lane % 8
+        uint32_t st_off[2];
+#pragma unroll
+        for (int x = 0; x < 2; ++x) {
+            const int m = lane >> 3, jj = 2 * x + (m >> 1), r = 8 * (m & 1) + (lane & 7);
+            st_off[x] = r * 64 + ((jj ^ (r >> 1)) & 3) * 16;
+        }
+        if (use_tma) {  // the previous tile's stores have left the boxes (the other warpgroup's MMAs ran in between)
+            if (lane == 0) bulk_wait_read<0>();
+            __syncwarp();
+        }
+        int nbox = 0;
+        // w[k] = bf16 pair (2k, 2k+1) of the chunk's 16 values: fragment group jj = k / 2, row e = k % 2
+        auto stage = [&](const uint32_t* w) {
+            const uint32_t box = ring + (nbox % kBoxes) * kBoxBytes;
+            if (use_tma && nbox >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
+                if (lane == 0) bulk_wait_read<kBoxes - 1>();
+                __syncwarp();
+            }
+            stmatrix_x4(box + st_off[0], w[0], w[1], w[2], w[3]);
+            stmatrix_x4(box + st_off[1], w[4], w[5], w[6], w[7]);
+            ++nbox;
+            return box;
+        };
+        auto put_tma = [&](const CUtensorMap* tm, const uint32_t* w, int col) {  // rows >= M, columns >= N: clipped by the map
+            const uint32_t box = stage(w);
+            fence_proxy_async();
+            __syncwarp();
+            if (lane == 0) {
+                tma_store_2d(tm, box, col, f.row0 + 16 * f.wq);
+                bulk_commit();
+            }
+        };
+        // mapped rows: row r of the box leaves as 4 x 16 bytes, lane = 4 (r % 8) + piece owns row e = r / 8 (its own rows);
+        // the next stage() call's stmatrix is ordered after these reads by its __syncwarp (kBoxes >= 2)
+        auto put_rows = [&](__nv_bfloat16* base, int ldo, const uint32_t* w, int col) {
+            const uint32_t box = stage(w);
+            __syncwarp();
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int r = (lane >> 2) + 8 * e, q = lane & 3;
+                const uint4 u = lds_u4(box + r * 64 + ((q ^ (r >> 1)) & 3) * 16);
+                if (v[e]) *(reinterpret_cast<uint4*>(base + orow[e] * ldo + col) + q) = u;
+            }
+        };
+        auto put_direct = [&](const float* y, int lc0) {  // y[4jj + 2e + i]: row e, slice column lc0 + 8jj + 2 (lane % 4) + i
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int lc = lc0 + 8 * jj + 2 * (lane & 3);
+                    if (!v[e] || lc >= f.ncols) continue;
+                    const bool two = lc + 1 < f.ncols;
+                    const float y0 = y[4 * jj + 2 * e], y1 = y[4 * jj + 2 * e + 1];
+                    const int col = f.col0 + lc;
+                    if (out_bf16) {
+                        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out) + orow[e] * ld + col;
+                        if (two) *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y0, y1);
+                        else *o = __float2bfloat16_rn(y0);
+                        if (lo_col0 >= 0 && col >= lo_col0) {
+                            const float l0 = y0 - bf16_round(y0), l1 = y1 - bf16_round(y1);
+                            __nv_bfloat16* ol = lo_out + orow[e] * ld_lo + (col - lo_col0);
+                            if (two) *reinterpret_cast<uint32_t*>(ol) = pack_bf16x2(l0, l1);
+                            else *ol = __float2bfloat16_rn(l0);
+                        }
+                    } else {
+                        float* o = static_cast<float*>(out) + orow[e] * ld + col;
+                        if (two) {
+                            float2 r = make_float2(y0, y1);
+                            if (accumulate) {  // out += : second pass of a split-operand product (x_lo . W^T on top of x_hi . W^T)
+                                const float2 o2 = *reinterpret_cast<const float2*>(o);
+                                r.x += o2.x; r.y += o2.y;
+                            }
+                            *reinterpret_cast<float2*>(o) = r;
+                        } else {
+                            *o = accumulate ? *o + y0 : y0;
+                        }
+                    }
+                }
+        };
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            if (q < f.nch) {  // a compile-time chunk index keeps the fragment in registers
+                const int lc0 = 32 * q;
+                float y[16];
+#pragma unroll
+                for (int k = 0; k < 16; ++k) y[k] = acc[16 * q + k];
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {  // bias from shared memory (zero past ncols)
+                    const float2 b = lds_f2(f.scratch + lc0 + 8 * jj + 2 * (lane & 3));
+                    y[4 * jj] += b.x; y[4 * jj + 1] += b.y; y[4 * jj + 2] += b.x; y[4 * jj + 3] += b.y;
                 }
                 if (relu) {
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.f);
+                    for (int k = 0; k < 16; ++k) y[k] = fmaxf(y[k], 0.f);
                 }
                 if (drop.p > 0.f) {
+                    // the mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of the same
+                    // group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
+                    const int b = lane & 1;
+                    const long long my_row = b ? orow[1] : orow[0];
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float m[4];
-                        drop.mask4(orow, ld, c.col0 + lc0 + j, m);
-                        x[j] *= m[0]; x[j + 1] *= m[1]; x[j + 2] *= m[2]; x[j + 3] *= m[3];
-                    }
-                }
-                if (whole) {  // columns >= N and rows >= M are clipped by the tensor map
-                    uint32_t w[16];
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int col4 = f.col0 + lc0 + 8 * jj + 4 * ((lane >> 1) & 1);
+                        const uint64_t bits = dropout_bits4(drop.seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
+                        const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
+                        const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
+                        const uint32_t wd[2] = {b ? other : own, b ? own : other};
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) w[j] = pack_bf16x2(x[2 * j], x[2 * j + 1]);
-                    ts.put(&tm_out, w, c.col0 + lc0, c.grow - lane, lane);
-                    if (lo_col0 >= 0 && c.col0 + lc0 >= lo_col0) {  // warp-uniform (the host checked the chunk alignment)
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const float2 h = unpack_bf16x2(w[j]);
-                            w[j] = pack_bf16x2(x[2 * j] - h.x, x[2 * j + 1] - h.y);
-                        }
-                        ts.put(&tm_lo, w, c.col0 + lc0 - lo_col0, c.grow - lane, lane);
-                    }
-                    return;
-                }
-                if (coop) {
-                    uint32_t w[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) w[j] = pack_bf16x2(x[2 * j], x[2 * j + 1]);
-                    ts.put_rows(static_cast<__nv_bfloat16*>(out), ld, w, c.col0 + lc0, v ? static_cast<int>(orow) : -1, lane);
-                    if (lo_col0 >= 0 && c.col0 + lc0 >= lo_col0 && (ld_lo & 7) == 0) {  // low plane, same (mapped) rows
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const float2 h = unpack_bf16x2(w[j]);
-                            w[j] = pack_bf16x2(x[2 * j] - h.x, x[2 * j + 1] - h.y);
-                        }
-                        ts.put_rows(lo_out, ld_lo, w, c.col0 + lc0 - lo_col0, v ? static_cast<int>(orow) : -1, lane);
-                    }
-                    return;
-                }
-#pragma unroll
-                for (int g = 0; g < 2; ++g) {
-                    const int lc = lc0 + g * 16;  // column inside the slice
-                    if (lc >= c.ncols) break;
-                    const int col = c.col0 + lc;
-                    const float* y = x + g * 16;
-                    const int nvalid = min(16, min(c.ncols - lc, N - col));
-                    if (out_bf16) {
-                        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out) + orow * ld + col;
-                        if (nvalid == 16 && aligned32(o)) {
-                            store_bf16x16(o, y);
-                        } else {
-                            store_bf16x8(o, y, min(nvalid, 8));
-                            if (nvalid > 8) store_bf16x8(o + 8, y + 8, nvalid - 8);
-                        }
-                        if (lo_col0 >= 0 && col >= lo_col0) {  // low plane of a partial chunk (identity rows)
-                            float yl[16];
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) yl[j] = y[j] - bf16_round(y[j]);
-                            __nv_bfloat16* ol = lo_out + orow * ld_lo + (col - lo_col0);
-                            store_bf16x8(ol, yl, min(nvalid, 8));
-                            if (nvalid > 8) store_bf16x8(ol + 8, yl + 8, nvalid - 8);
-                        }
-                    } else {
-                        float* o = static_cast<float*>(out) + orow * ld + col;
-                        if (nvalid == 16) {
-#pragma unroll
-                            for (int j = 0; j < 16; j += 4) {
-                                float4 v4 = make_float4(y[j], y[j + 1], y[j + 2], y[j + 3]);
-                                if (accumulate) {  // out += : second pass of a split-operand product (x_lo . W^T on top of x_hi . W^T)
-                                    const float4 o4 = *reinterpret_cast<const float4*>(o + j);
-                                    v4.x += o4.x; v4.y += o4.y; v4.z += o4.z; v4.w += o4.w;
-                                }
-                                *reinterpret_cast<float4*>(o + j) = v4;
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j)
-                                if (j < nvalid) o[j] = accumulate ? o[j] + y[j] : y[j];
+                        for (int e = 0; e < 2; ++e) {
+                            y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= drop.thresh) ? drop.scale : 0.f;
+                            y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= drop.thresh) ? drop.scale : 0.f;
                         }
                     }
                 }
-            });
-        if (v && c.col0 == 0 && c.half == 0) {
-            if (ones_col >= 0 && out_bf16) {
-                __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out) + orow * ld;
+                // a chunk cut by the slice's end leaves from the fragment with predicated stores, which write exactly the
+                // columns < ncols (letting the tensor map clip it at N changed the outputs where N % 16 != 0)
+                const bool staged = out_bf16 && lc0 + 32 <= f.ncols;  // warp-uniform
+                if (staged) {
+                    uint32_t w[8];
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) w[k] = pack_bf16x2(y[2 * k], y[2 * k + 1]);
+                    if (use_tma) put_tma(&tm_out, w, f.col0 + lc0);
+                    else put_rows(static_cast<__nv_bfloat16*>(out), ld, w, f.col0 + lc0);
+                    if (lo_col0 >= 0 && f.col0 + lc0 >= lo_col0) {  // warp-uniform (the host checked the chunk alignment)
+#pragma unroll
+                        for (int k = 0; k < 8; ++k) {
+                            const float2 h = unpack_bf16x2(w[k]);
+                            w[k] = pack_bf16x2(y[2 * k] - h.x, y[2 * k + 1] - h.y);
+                        }
+                        if (use_tma) put_tma(&tm_lo, w, f.col0 + lc0 - lo_col0);
+                        else put_rows(lo_out, ld_lo, w, f.col0 + lc0 - lo_col0);
+                    }
+                } else {
+                    put_direct(y, lc0);
+                }
+            }
+        }
+        if (ones_col >= 0 && out_bf16 && f.col0 == 0 && (lane & 3) == 0) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (!v[e]) continue;
+                __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out) + orow[e] * ld;
                 o[ones_col] = __float2bfloat16_rn(1.0f);
                 for (int j = ones_col + 1; j < ones_cols_zero_upto; ++j) o[j] = __float2bfloat16_rn(0.f);
-            }
-            if (zero_pad_rows && out_bf16) {  // neighbours of the first / last token of a segment are pad rows
-                __nv_bfloat16* base = static_cast<__nv_bfloat16*>(out);
-                if (t == 0) zero_row_bf16(base + (orow - 1) * ld, ld);
-                if (t == rm.seg_len - 1) zero_row_bf16(base + (orow + 1) * ld, ld);
             }
         }
     }

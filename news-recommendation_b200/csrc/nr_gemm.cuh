@@ -13,8 +13,11 @@
 // last warpgroup is the TMA producer.  Ping-pong schedule: warpgroup w owns the CTA's tiles w, w + 2, w + 4, ... and computes
 // a whole tile (64 rows x the whole slice) with one m64nN wgmma per k-step, N = 32 * (chunks of the slice).  The two
 // warpgroups issue their MMAs in strict alternation (a pair of named barriers passes the tensor pipe from one to the other),
-// so one warpgroup's epilogue runs while the other's wgmmas execute.  Inside a warpgroup the epilogue view is row-per-thread:
-// the m64 fragment passes through a small shared-memory transpose buffer one 32-column chunk per column half at a time.
+// so one warpgroup's epilogue runs while the other's wgmmas execute.  An epilogue takes one of two views of the accumulators:
+//   * fragment view (Epi::kFragmentView): each warp reads its 16 rows of the m64 fragment in registers, with no shared memory
+//     and no barrier across warps -- for epilogues whose output elements are independent (EpiStore);
+//   * row view: row-per-thread, the fragment passes through a small shared-memory transpose buffer one 32-column chunk per
+//     column half at a time -- for epilogues that reduce along a row or a column.
 #pragma once
 #include "nr_common.cuh"
 
@@ -36,7 +39,7 @@ constexpr int kChunkK = 64;                     // bf16 elements per 128-byte sw
 constexpr int kAStageBytes = kTileM * 128;      // 8 KB
 constexpr int kMaxStages = 12;
 constexpr int kSmemLimit = 232448;              // 227 KB
-constexpr int kXposeBytes = 2 * kEpiHalves * kTileM * 16 * 4;  // per warpgroup and column half: 64 rows x 16 fp32 columns
+constexpr int kXposeBytes = 2 * kEpiHalves * kTileM * 16 * 4;  // row view: per warpgroup and column half 64 rows x 16 fp32 columns
 // named barriers of gemm_nt (0 is __syncthreads): all consumer threads, each warpgroup's own, each warpgroup's MMA turn
 constexpr int kBarConsumers = 1, kBarWg = 2, kBarTurn = 4;
 
@@ -79,6 +82,24 @@ struct EpiCtx {
     int it;          // how many tiles this warpgroup has finished before this one (double-buffer parity of the staging)
     int next_tile;   // the tile this warpgroup processes next, or -1
 };
+// What a fragment-view epilogue sees for one tile: frag(acc, f) is called by every thread of the warpgroup that owns the
+// tile, acc is its m64nN fragment (acc[4j + 2e + i] = tile row 16 * wq + lane / 4 + 8e, slice column 8j + 2 * (lane % 4) + i,
+// j < 4 * nch).
+struct FragCtx {
+    int row0;     // global A row of the tile's row 0
+    int rows;     // rows of the tile that exist (r < rows: rows_per_tile, fewer at the end of A)
+    int wq;       // warp in the warpgroup
+    int nch;      // 32-column chunks of the slice
+    int col0;     // first output column of this CTA's slice
+    int ncols;    // valid output columns in the slice
+    float* scratch;  // Epi::kScratchBytes of shared memory private to the epilogue (both warpgroups)
+};
+template <class Epi>
+concept FragmentEpilogue = Epi::kFragmentView;
+// shared memory an epilogue needs beside the pipeline: its scratch, plus the transpose buffers of the row view
+template <class Epi>
+constexpr int kEpiSmemBytes = Epi::kScratchBytes + (FragmentEpilogue<Epi> ? 0 : kXposeBytes);
+
 // What init()/finish() see (all kEpiThreads consumer threads call them).
 struct EpiInit {
     int col0, ncols, tid;
@@ -223,25 +244,6 @@ struct WarpTileStore {
         }
         ++nput;
     }
-    // Row-mapped destinations (no tensor map fits them): the same staging tile leaves as coalesced 16-byte stores, 8 rows x 64
-    // contiguous bytes per instruction.  my_orow = destination row of this lane's accumulator row, -1 for "drop the row".
-    __device__ __forceinline__ void put_rows(__nv_bfloat16* base, int ld, const uint32_t* w, int col, int my_orow, int lane) {
-        uint8_t* b = buf;
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-            *reinterpret_cast<uint4*>(b + lane * 64 + ((q ^ (lane >> 1)) & 3) * 16) =
-                make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-        __syncwarp();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int r = (lane >> 2) + 8 * k, q = lane & 3;
-            const int orr = __shfl_sync(0xffffffffu, my_orow, r);
-            if (orr >= 0)
-                *(reinterpret_cast<uint4*>(base + static_cast<long long>(orr) * ld + col) + q) =
-                    *reinterpret_cast<const uint4*>(b + r * 64 + ((q ^ (r >> 1)) & 3) * 16);
-        }
-        __syncwarp();
-    }
     static __device__ __forceinline__ void drain(int lane) {  // before the CTA exits
         if (lane == 0) bulk_wait_all();
     }
@@ -311,8 +313,8 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int b_region = p.n_box * 128;  // bytes of one (tap, k-chunk) box of the weight slice
     uint8_t* sB = smem;
     uint8_t* sA = sB + (p.b_stream ? 0 : p.taps * p.k_chunks * b_region);
-    float* xpose = reinterpret_cast<float*>(sA + p.stages * p.stage_bytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(xpose) + kXposeBytes);
+    float* xpose = reinterpret_cast<float*>(sA + p.stages * p.stage_bytes);  // row view only
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(xpose) + (FragmentEpilogue<Epi> ? 0 : kXposeBytes));
     uint64_t* full = bars;
     uint64_t* empty = bars + kMaxStages;
     uint64_t* bfull = bars + 2 * kMaxStages;
@@ -324,8 +326,8 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int col0 = slice * p.n_stride;
     const int ncols = min(p.n_stride, p.N - col0);
     const int tap_shift = p.taps / 2;
-    // tuning counters: [0] producer waits for a free A stage, [5] kernel; per consumer warpgroup w at [8 + 4w]: +0 waits for
-    // its MMA turn, +1 MMA loops incl. waits for A data (turn waits excluded), +2 epilogue, +3 tiles
+    // tuning counters: [0] producer waits for a free A stage, [1] the CTA's weight slice, [5] kernel; per consumer warpgroup w
+    // at [8 + 4w]: +0 waits for its MMA turn, +1 MMA loops incl. waits for A data (turn waits excluded), +2 epilogue, +3 tiles
     long long* tmr = p.timing != nullptr ? p.timing + blockIdx.x * 16 : nullptr;
     const long long t_begin = tmr != nullptr ? clock64() : 0;
 
@@ -422,31 +424,39 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
             skip_tile();
             if (tmr != nullptr) { const long long u = clock64(); tw_mma += u - t; t = u; }
-            EpiCtx c;
-            c.tile = tile;
-            c.r = 32 * (warp & 1) + lane;
-            c.grow = tile * p.rows_per_tile + c.r;
-            c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
-            c.col0 = col0;
-            c.ncols = ncols;
-            c.tid = threadIdx.x;
-            c.wg = wg;
-            c.wtid = threadIdx.x & 127;
-            c.half = half;
-            c.ch0 = ch0;
-            c.ch1 = ch1;
-            c.rounds = rounds;
-            c.scratch = scratch;
-            c.it = it;
-            c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
-            epi(racc, c);
+            if constexpr (FragmentEpilogue<Epi>) {
+                const int row0 = tile * p.rows_per_tile;
+                epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), warp & 3, nch, col0, ncols, scratch});
+            } else {
+                EpiCtx c;
+                c.tile = tile;
+                c.r = 32 * (warp & 1) + lane;
+                c.grow = tile * p.rows_per_tile + c.r;
+                c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
+                c.col0 = col0;
+                c.ncols = ncols;
+                c.tid = threadIdx.x;
+                c.wg = wg;
+                c.wtid = threadIdx.x & 127;
+                c.half = half;
+                c.ch0 = ch0;
+                c.ch1 = ch1;
+                c.rounds = rounds;
+                c.scratch = scratch;
+                c.it = it;
+                c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
+                epi(racc, c);
+            }
             if (tmr != nullptr) tw_epi += clock64() - t;
         }
         epi.finish(ei);
         if (tmr != nullptr && (threadIdx.x & 127) == 0) {
             long long* w = tmr + 8 + 4 * wg;
             w[0] = tw_turn; w[1] = tw_mma; w[2] = tw_epi; w[3] = it;
-            if (wg == 0) tmr[5] = clock64() - t_begin;
+            if (wg == 0) {
+                tmr[1] = slice;
+                tmr[5] = clock64() - t_begin;
+            }
         }
     }
 }
@@ -472,24 +482,36 @@ __global__ void __launch_bounds__(kEpiThreads, 1) gemm_nt_simt_epi_kernel(const 
     epi.init(ei, tile_step);
     int it = 0;
     for (int tile = tile0 + wg * tile_step; tile < p.num_m_tiles; tile += 2 * tile_step, ++it) {
-        EpiCtx c;
-        c.tile = tile;
-        c.r = 32 * ((threadIdx.x >> 5) & 1) + (threadIdx.x & 31);
-        c.grow = tile * p.rows_per_tile + c.r;
-        c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
-        c.col0 = col0;
-        c.ncols = ncols;
-        c.tid = threadIdx.x;
-        c.wg = wg;
-        c.wtid = threadIdx.x & 127;
-        c.half = (threadIdx.x >> 6) & 1;
-        epi_chunk_range(ncols, c.half, c.ch0, c.ch1);
-        c.rounds = (((ncols + 31) >> 5) + 1) >> 1;
-        c.scratch = scratch;
-        c.it = it;
-        c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
-        GlobalAcc acc{p.dbg_acc + (static_cast<size_t>(tile) * kTileM + c.r) * p.dbg_ld + col0, c.ch0, c.ch1};
-        epi(acc, c);
+        if constexpr (FragmentEpilogue<Epi>) {  // the same fragment layout as the wgmma accumulators
+            const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, nch = (ncols + 31) >> 5;
+            float acc[128];
+            for (int j = 0; j < 4 * nch; ++j)
+                for (int e = 0; e < 2; ++e)
+                    for (int i = 0; i < 2; ++i)
+                        acc[4 * j + 2 * e + i] = p.dbg_acc[(static_cast<size_t>(tile) * kTileM + 16 * wq + (lane >> 2) + 8 * e) * p.dbg_ld +
+                                                           col0 + 8 * j + 2 * (lane & 3) + i];
+            const int row0 = tile * p.rows_per_tile;
+            epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), wq, nch, col0, ncols, scratch});
+        } else {
+            EpiCtx c;
+            c.tile = tile;
+            c.r = 32 * ((threadIdx.x >> 5) & 1) + (threadIdx.x & 31);
+            c.grow = tile * p.rows_per_tile + c.r;
+            c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
+            c.col0 = col0;
+            c.ncols = ncols;
+            c.tid = threadIdx.x;
+            c.wg = wg;
+            c.wtid = threadIdx.x & 127;
+            c.half = (threadIdx.x >> 6) & 1;
+            epi_chunk_range(ncols, c.half, c.ch0, c.ch1);
+            c.rounds = (((ncols + 31) >> 5) + 1) >> 1;
+            c.scratch = scratch;
+            c.it = it;
+            c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
+            GlobalAcc acc{p.dbg_acc + (static_cast<size_t>(tile) * kTileM + c.r) * p.dbg_ld + col0, c.ch0, c.ch1};
+            epi(acc, c);
+        }
     }
     epi.finish(ei);
 }
@@ -525,10 +547,10 @@ struct GemmNTPlan {
     size_t smem;
 };
 // Fills slices/boxes/stages and encodes the tensor maps.  A: [M rows][K] pitch lda; B: [taps*b_tap_rows][K] pitch ldb.
-// scratch_bytes = Epi::kScratchBytes; max_n_stride (0 = none) caps the slice width for epilogues whose staging
+// epi_smem_bytes = kEpiSmemBytes<Epi>; max_n_stride (0 = none) caps the slice width for epilogues whose staging
 // grows with it.
 int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B, int N, int ldb, int K, int taps,
-                 int b_tap_rows, int rows_per_tile, int num_sms, int max_slices, int scratch_bytes, int max_n_stride);
+                 int b_tap_rows, int rows_per_tile, int num_sms, int max_slices, int epi_smem_bytes, int max_n_stride);
 bool debug_simt_gemm();
 
 template <class Epi>

@@ -48,9 +48,9 @@ lib.nr_debug_set_gemm_timing(buf.data_ptr(), SLOTS)
 step()
 lib.nr_debug_set_gemm_timing(None, 0)
 t = buf.cpu().double()
-# per CTA (gemm_nt_kernel): [0] producer waits for a free stage, [5] kernel; consumer warpgroup w at [8 + 4w]: +0 waits for
-# its MMA turn, +1 MMA loops (waits for A data included), +2 epilogue, +3 tiles.  With the epilogue overlapped, mma0 + mma1
-# approaches 100% of the kernel while each warpgroup's epilogue share stays large.
+# per CTA (gemm_nt_kernel): [0] producer waits for a free stage, [1] weight slice, [5] kernel; consumer warpgroup w at
+# [8 + 4w]: +0 waits for its MMA turn, +1 MMA loops (waits for A data included), +2 epilogue, +3 tiles.  With the epilogue
+# overlapped, mma0 + mma1 approaches 100% of the kernel while each warpgroup's epilogue share stays large.
 for s in range(SLOTS):
     used = t[s, :, 5] > 0
     if used.sum() == 0:
@@ -62,3 +62,14 @@ for s in range(SLOTS):
                     f"tiles={m[11 + 4 * w].item():6.1f} epi/tile={m[10 + 4 * w].item() / max(m[11 + 4 * w].item(), 1):6.0f} cyc"
                     for w in range(2))
     print(f"slot {s:2d} ctas={int(used.sum())} kernel={k / 1e3:8.1f} kcyc prod:empty={pct(0):5.1f}%  {wgs}", flush=True)
+    # per weight slice: the CTAs of one slice share its column range, so an epilogue that costs more on some columns (the
+    # low plane of the accurate V section) shows up as a slice whose CTAs run longer
+    slices = t[s, :, 1][used]
+    if int(slices.max()) == 0:
+        continue
+    for sl in range(int(slices.max()) + 1):
+        c = t[s][used][slices == sl]
+        tiles = c[:, 11] + c[:, 15]
+        print(f"         slice {sl}: ctas={c.shape[0]:3d} kernel={c[:, 5].mean().item() / 1e3:8.1f} kcyc "
+              f"(max {c[:, 5].max().item() / 1e3:8.1f})  mma/tile={(c[:, 9] + c[:, 13]).sum().item() / max(tiles.sum().item(), 1):6.0f} cyc "
+              f"epi/tile={(c[:, 10] + c[:, 14]).sum().item() / max(tiles.sum().item(), 1):6.0f} cyc", flush=True)
