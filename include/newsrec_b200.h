@@ -118,6 +118,19 @@ int nr_segment_dot(const float* news, long long n_news, int D, const long long* 
                    const long long* seg_offsets, long long n_seg, const float* user, float* scores, int* bad_id_flag,
                    void* stream);
 
+/* The evaluator's metrics (src/evaluate.py:160-168, 267-271: sklearn roc_auc_score + NumPy mrr / nDCG per impression):
+ * metrics[s] = {AUC, MRR, nDCG@5, nDCG@10} of impression s, whose candidates are
+ * scores[seg_offsets[s] .. seg_offsets[s+1]) with labels (0/1, uint8) at the same positions.  All fp64, [n_seg][4].
+ *   place_i = #{j : s_j > s_i} + #{j > i : s_j == s_i}: candidate i's 0-based position in the descending order, ties taken
+ *             as the stable reading of argsort(s)[::-1] (among equal scores the later candidate first; -0 == +0);
+ *   AUC     = sum_{i pos} (2 #{neg j : s_j < s_i} + #{neg j : s_j == s_i}) / (2 P N)  (Mann-Whitney, counted in integers);
+ *   MRR     = sum_{i pos} 1 / (place_i + 1) / P;
+ *   nDCG@k  = sum_{i pos, place_i < k} 1 / log2(place_i + 2)  /  sum_{r < min(P, k)} 1 / log2(r + 2).
+ * NaN rows: a non-finite score or a label other than 0/1 (all four); P == 0 (all four); N == 0 (AUC only).
+ * *bad_label_flag is set if a label is not 0 or 1.  Any segment length works (staged through shared memory in chunks). */
+int nr_impression_metrics(const float* scores, const unsigned char* labels, const long long* seg_offsets, long long n_seg,
+                          double* metrics, int* bad_label_flag, void* stream);
+
 /* Host-side glue of the weight-gradient GEMMs (nr_gemm_tn with the ones column): ext is [rows][ld] fp32 whose columns
  * [0,D) hold dW and column D holds db.  Adds them into the parameters' own gradient storage (dW [rows][D] contiguous,
  * db [rows] or null) and CLEARS ext, so the caller can keep it as a persistent accumulator across steps. */

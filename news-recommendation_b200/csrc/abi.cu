@@ -129,6 +129,12 @@ int nr_segment_dot(const float* news, long long n_news, int D, const long long* 
                "nr_segment_dot: null operand or empty problem");
     return segment_dot(news, n_news, D, cand, n_cand, seg_offsets, n_seg, user, scores, bad_id_flag, as_stream(stream));
 }
+int nr_impression_metrics(const float* scores, const unsigned char* labels, const long long* seg_offsets, long long n_seg,
+                          double* metrics, int* bad_label_flag, void* stream) {
+    NR_REQUIRE(scores && labels && seg_offsets && metrics && bad_label_flag && n_seg >= 0,
+               "nr_impression_metrics: null operand or n_seg=%lld", n_seg);
+    return impression_metrics(scores, labels, seg_offsets, n_seg, metrics, bad_label_flag, as_stream(stream));
+}
 
 int nr_accumulate_ext_grad(float* ext, int rows, int ld, int D, float* dW, float* db, void* stream) {
     NR_REQUIRE(ext && dW && rows >= 0 && D >= 1, "nr_accumulate_ext_grad: null operand");

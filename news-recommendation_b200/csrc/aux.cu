@@ -850,6 +850,146 @@ int segment_dot(const float* news, long long n_news, int D, const long long* can
 }
 
 // ------------------------------------------------------------------------------------------------
+// evaluation metrics (reference src/evaluate.py:160-168, 267-271: sklearn roc_auc_score + NumPy mrr / nDCG@5 / nDCG@10 once
+// per impression in a process pool): {AUC, MRR, nDCG@5, nDCG@10} of EVERY impression in one launch.  One warp per
+// impression; lane l owns candidates l, l+32, ... and counts, against every candidate of the impression, how many score
+// higher (its 0-based place in the descending order, ties broken as the stable reading of argsort(s)[::-1]: the later
+// candidate first) and, for a positive, how many negatives score lower / equal (Mann-Whitney AUC in integers).  The
+// impression's (score, label) pairs are staged in a per-warp shared-memory chunk, chunk by chunk when it is longer.
+// O(n^2) per impression: MIND impressions hold tens to a few hundred candidates.
+// ------------------------------------------------------------------------------------------------
+constexpr int kMetricWarps = 8, kMetricChunk = 512;
+template <typename T>
+__device__ __forceinline__ T warp_total(T v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+// finite fp32 score -> int32 with the same order and -0 == +0.  The library builds with --use_fast_math (-ftz=true), under
+// which fp32 comparisons treat subnormal scores as zero; integer keys keep every distinct finite score distinct.
+__device__ __forceinline__ int score_key(float x) {
+    const int b = __float_as_int(x) == static_cast<int>(0x80000000u) ? 0 : __float_as_int(x);
+    return b < 0 ? b ^ 0x7fffffff : b;
+}
+__device__ __forceinline__ bool finite_score(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
+
+__global__ void __launch_bounds__(kMetricWarps * 32) impression_metrics_kernel(const float* __restrict__ scores,
+                                                                               const unsigned char* __restrict__ labels,
+                                                                               const long long* __restrict__ seg_offsets, long long n_seg,
+                                                                               double* __restrict__ metrics, int* __restrict__ bad_flag) {
+    __shared__ int s_key[kMetricWarps][kMetricChunk];
+    __shared__ unsigned char s_neg[kMetricWarps][kMetricChunk];
+    const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
+    int* const ck = s_key[wl];
+    unsigned char* const cn = s_neg[wl];
+    const double qnan = __longlong_as_double(0x7ff8000000000000ll);
+    const long long nw = static_cast<long long>(gridDim.x) * kMetricWarps;
+    for (long long s = static_cast<long long>(blockIdx.x) * kMetricWarps + wl; s < n_seg; s += nw) {
+        const long long b = __ldg(seg_offsets + s);
+        const long long n = __ldg(seg_offsets + s + 1) - b;
+        const float* const sc = scores + b;
+        const unsigned char* const lb = labels + b;
+        // pass 1: positives, non-finite scores, labels other than 0 / 1
+        long long pos_cnt = 0;
+        bool bad_score = false, bad_label = false;
+        for (long long i = lane; i < n; i += 32) {
+            const unsigned char l = __ldg(lb + i);
+            pos_cnt += l == 1;
+            bad_label |= l > 1;
+            bad_score |= !finite_score(__ldg(sc + i));
+        }
+        const long long P = warp_total(pos_cnt);
+        bad_label = __any_sync(0xffffffffu, bad_label);
+        bad_score = __any_sync(0xffffffffu, bad_score);
+        if (bad_label && lane == 0) atomicExch(bad_flag, 1);
+        double* const out = metrics + 4 * s;
+        if (bad_label || bad_score || P == 0) {  // sklearn raises (the reference catches it: NaN row); no positive: 0/0
+            if (lane < 4) out[lane] = qnan;
+            continue;
+        }
+        const long long N = n - P;
+        // pass 2: lane l owns candidates i = l, l+32, ...; the comparison partners come from the shared-memory chunk
+        unsigned long long auc2 = 0;  // sum over positives of 2 #{negatives below} + #{negatives level}
+        double rr = 0.0, g5 = 0.0, g10 = 0.0;
+        const bool one_chunk = n <= kMetricChunk;
+        if (one_chunk) {
+            for (int j = lane; j < n; j += 32) {
+                ck[j] = score_key(__ldg(sc + j));
+                cn[j] = __ldg(lb + j) == 0;
+            }
+            __syncwarp();
+        }
+        for (long long i0 = 0; i0 < n; i0 += 32) {
+            const long long i = i0 + lane;
+            const bool own = i < n;
+            const int ki = own ? score_key(__ldg(sc + i)) : 0;
+            const bool pos_i = own && __ldg(lb + i) == 1;
+            long long place = 0, neg_lt = 0, neg_eq = 0;  // place: #{higher} + #{level and later} = position in the descending order
+            for (long long c0 = 0; c0 < n; c0 += kMetricChunk) {
+                const int len = static_cast<int>(min(static_cast<long long>(kMetricChunk), n - c0));
+                if (!one_chunk) {
+                    __syncwarp();
+                    for (int j = lane; j < len; j += 32) {
+                        ck[j] = score_key(__ldg(sc + c0 + j));
+                        cn[j] = __ldg(lb + c0 + j) == 0;
+                    }
+                    __syncwarp();
+                }
+                const int after = static_cast<int>(max(-1ll, min(static_cast<long long>(len), i - c0)));  // chunk slots j > after are later than i
+                int gt = 0, eq_after = 0, lt_neg = 0, eq_neg = 0;
+                for (int j = 0; j < len; ++j) {
+                    const int kj = ck[j];
+                    const int neg = cn[j];
+                    const int eq = kj == ki;
+                    gt += kj > ki;
+                    eq_after += eq & (j > after);
+                    lt_neg += neg & (kj < ki);
+                    eq_neg += neg & eq;
+                }
+                place += gt + eq_after;
+                neg_lt += lt_neg;
+                neg_eq += eq_neg;
+            }
+            if (pos_i) {
+                auc2 += static_cast<unsigned long long>(2 * neg_lt + neg_eq);
+                rr += 1.0 / static_cast<double>(place + 1);
+                const double g = place < 10 ? 1.0 / log2(static_cast<double>(place + 2)) : 0.0;
+                g10 += g;
+                g5 += place < 5 ? g : 0.0;
+            }
+        }
+        __syncwarp();  // the next impression restages this warp's chunk
+        auc2 = warp_total(auc2);
+        rr = warp_total(rr);
+        g5 = warp_total(g5);
+        g10 = warp_total(g10);
+        if (lane == 0) {
+            double ideal5 = 0.0, ideal10 = 0.0;  // DCG of the ideal order: the P positives first
+            for (int r = 0; r < 10 && r < P; ++r) {
+                const double g = 1.0 / log2(static_cast<double>(r + 2));
+                ideal10 += g;
+                ideal5 += r < 5 ? g : 0.0;
+            }
+            // one class (no negative): roc_auc_score warns and returns NaN, MRR / nDCG stay defined
+            out[0] = N > 0 ? static_cast<double>(auc2) / (2.0 * static_cast<double>(P) * static_cast<double>(N)) : qnan;
+            out[1] = rr / static_cast<double>(P);
+            out[2] = g5 / ideal5;
+            out[3] = g10 / ideal10;
+        }
+    }
+}
+int impression_metrics(const float* scores, const unsigned char* labels, const long long* seg_offsets, long long n_seg, double* metrics,
+                       int* bad_label_flag, cudaStream_t stream) {
+    if (n_seg == 0) return 0;
+    ProfScope ps("impression_metrics", static_cast<int>(std::min<long long>(n_seg, 1 << 30)), 0, 0, stream);
+    const int blocks = static_cast<int>(std::min<long long>((n_seg + kMetricWarps - 1) / kMetricWarps, 148 * 16));
+    impression_metrics_kernel<<<blocks, kMetricWarps * 32, 0, stream>>>(scores, labels, seg_offsets, n_seg, metrics, bad_label_flag);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Batch feed: the reference hands the model slot-major lists of per-slot (B, L) int64 tensors (default_collate over
 // src/dataset.py:64-85; pinned by the DataLoader, src/train.py:165-171).  ONE launch reads the payload of every slot
 // straight from page-locked host memory (unified addressing: the kernel's loads cross PCIe, no host staging copy, no

@@ -145,6 +145,9 @@ int mhsa_f32_fwd(const float* qkv, int ld, int sec, long long n_seq, int T, int 
 // scores[i] = news[cand[i]] . user[s] for seg_offsets[s] <= i < seg_offsets[s+1]  (batched evaluate.py:245-265)
 int segment_dot(const float* news, long long n_news, int D, const long long* cand, long long n_cand, const long long* seg_offsets,
                 long long n_seg, const float* user, float* scores, int* bad_flag, cudaStream_t stream);
+// metrics[s] = {AUC, MRR, nDCG@5, nDCG@10} of impression s (batched evaluate.py:160-168, 267-271)
+int impression_metrics(const float* scores, const unsigned char* labels, const long long* seg_offsets, long long n_seg, double* metrics,
+                       int* bad_label_flag, cudaStream_t stream);
 
 int slots_device_readable(const void* const* slots, int n);
 int pack_slots(const void* const* slots, int H, int C, int B, int L, long long* out, cudaStream_t stream);

@@ -122,6 +122,7 @@ SIGNATURES = {
     "nr_slots_device_readable": (_i, [_vp, _i]),
     "nr_pack_slots": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "nr_segment_dot": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp]),
+    "nr_impression_metrics": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),
     "nr_accumulate_ext_grad": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "nr_dot_score_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "nr_mhsa_accurate_supported": (_i, [_i, _i, _i]),

@@ -16,7 +16,8 @@ editing it:
   (`ddp.FlatGradients`: the kernels accumulate into it in place), `zero_grad()` clears that buffer, `step()` first
   all-reduces it (ONE NCCL collective, mean over ranks) -- every rank then applies the identical update;
 * rank 0 alone writes TensorBoard events and checkpoints and runs `evaluate()` (train.py:248); its metrics are broadcast
-  so that early stopping takes the same decision everywhere;
+  so that early stopping takes the same decision everywhere; `--device-evaluate` swaps the reference's evaluator for
+  `newsrec_b200.evaluate.evaluate` (same signature; scoring and metrics on the device);
 * compatibility shims the survey found necessary for the reference on current NumPy / pandas / torch.
 """
 from __future__ import annotations
@@ -122,14 +123,19 @@ def apply_compat_shims():
         torch.load = load
 
 
-def patch_trainer(train_module, rank, world, seed=0):
-    """Install the data-parallel pieces into an imported (reference) `train` module's namespace."""
+def patch_trainer(train_module, rank, world, seed=0, device_evaluate=False):
+    """Install the data-parallel pieces into an imported (reference) `train` module's namespace.  device_evaluate: the
+    trainer's `evaluate` becomes newsrec_b200.evaluate.evaluate (its docstring lists where its metrics can differ from a
+    given reference environment: ties across labels, one-class impressions)."""
     import torch
     train_module.DataLoader = make_sharded_dataloader(train_module.DataLoader, rank, world, seed)
     if world > 1 or os.environ.get("NEWSREC_FLAT_GRADS", "1") == "1":
         # the trainer reaches Adam through the global `torch.optim` module (train.py:127)
         torch.optim.Adam = make_all_reduce_adam(torch.optim.Adam, world)
-    if hasattr(train_module, "evaluate"):
+    if device_evaluate:
+        from newsrec_b200.evaluate import evaluate as device_evaluate_fn
+        train_module.evaluate = make_rank0_evaluate(device_evaluate_fn, rank, world)
+    elif hasattr(train_module, "evaluate"):
         train_module.evaluate = make_rank0_evaluate(train_module.evaluate, rank, world)
     if rank != 0:
         if hasattr(train_module, "SummaryWriter"):
@@ -145,6 +151,9 @@ def main(argv=None):
     ap.add_argument("--no-dropin", action="store_true", help="keep the reference's own model/config packages (CPU smoke runs)")
     ap.add_argument("--backend", default=None, help="torch.distributed backend (default: nccl with CUDA, else gloo)")
     ap.add_argument("--seed", type=int, default=0, help="seed of the sharded sampler's permutations")
+    ap.add_argument("--device-evaluate", action="store_true",
+                    help="validate with newsrec_b200.evaluate.evaluate (all impressions scored and their AUC / MRR / nDCG computed "
+                         "on the device) instead of the reference's evaluate.py")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
                     help="override a knob of the selected <MODEL_NAME>Config before the trainer is imported (repeatable), "
                          "e.g. --set batch_size=512 --set num_workers=8")
@@ -197,7 +206,7 @@ def main(argv=None):
                 pass  # keep the string
             setattr(cfg, key, val)
     train = importlib.import_module("train")
-    patch_trainer(train, rank, world, args.seed)
+    patch_trainer(train, rank, world, args.seed, device_evaluate=args.device_evaluate)
     try:
         train.train()
     finally:

@@ -482,3 +482,31 @@ def predict_impressions(news_matrix, cand_index, seg_offsets, user_vectors):
     check(lib.nr_segment_dot(_p(news_matrix), news_matrix.shape[0], news_matrix.shape[1], _p(cand_index), cand_index.numel(),
                              _p(seg_offsets), n_seg, _p(user_vectors), _p(scores), _p(flag), _stream()), "nr_segment_dot")
     return scores
+
+
+def impression_metrics(scores, labels, seg_offsets):
+    """{AUC, MRR, nDCG@5, nDCG@10} of every impression in one launch (nr_impression_metrics): reference src/evaluate.py
+    runs sklearn's roc_auc_score and NumPy's mrr / nDCG once per impression in a process pool.  scores (n_cand,) fp32,
+    labels (n_cand,) 0/1, seg_offsets (n_impressions + 1,) int64 with seg_offsets[0] = 0.  Returns the (n_impressions, 4)
+    fp64 device tensor; rows are NaN where the reference's metrics are undefined (include/newsrec_b200.h).  Raises
+    ValueError if a label is not 0 or 1 (reads the device flag: one synchronisation)."""
+    lib = load_library()
+    dev = require_cuda()
+    scores = scores.to(dev).float().contiguous()
+    labels = labels.to(dev)
+    if labels.dtype != torch.uint8:  # any value outside 0..255 must still reach the kernel as "not 0 / 1"
+        labels = torch.where((labels >= 0) & (labels <= 1), labels, 2).to(torch.uint8)
+    labels = labels.contiguous()
+    seg_offsets = seg_offsets.to(dev).long().contiguous()
+    if labels.numel() != scores.numel() or seg_offsets.dim() != 1 or seg_offsets.numel() < 1:
+        raise NewsrecError("impression_metrics: labels must match scores; seg_offsets must be (n_impressions + 1,)")
+    n_seg = seg_offsets.numel() - 1
+    metrics = torch.empty((n_seg, 4), dtype=torch.float64, device=dev)
+    if n_seg == 0:
+        return metrics
+    flag = torch.zeros(1, dtype=torch.int32, device=dev)
+    check(lib.nr_impression_metrics(_p(scores), _p(labels), _p(seg_offsets), n_seg, _p(metrics), _p(flag), _stream()),
+          "nr_impression_metrics")
+    if int(flag.item()):
+        raise ValueError("impression_metrics: a label is neither 0 nor 1")
+    return metrics
