@@ -1,4 +1,4 @@
-/* newsrec_b200 -- C ABI of the Hopper-native (sm_90a) NRMS / NAML / LSTUR / TANR hot path.
+/* newsrec_b200 -- C ABI of the Hopper-native (sm_90a) NRMS / NAML / LSTUR / TANR / Exp1 hot path.
  *
  * Drop-in boundary for the reference's Python modules (yusanshi/news-recommendation @ 8323a4f).  The
  * reference has no FFI of its own (pure PyTorch); these are the entry points a maintainer binds with
@@ -61,6 +61,10 @@ int nr_cast_pad_bf16_many(int n, const float* const* src, const int* R, const in
 /* fp32 rows [n][D] with element strides -> bf16 [n][ld] + ones column */
 int nr_rows_to_bf16(const float* src, long long n, int D, long long s_row, long long s_col, void* dst_bf16, int ld,
                     void* stream);
+/* the same rows as a hi/lo bf16 pair in one pass: hi [n][ld] = bf16(x) + ones column at D, lo [n][ld] = bf16(x - hi) with zeros
+ * from column D on (input of nr_additive_attention_fwd_hilo) */
+int nr_rows_to_bf16_hilo(const float* src, long long n, int D, long long s_row, long long s_col, void* hi_bf16, void* lo_bf16,
+                         int ld, void* stream);
 
 /* ---- reference: nn.Embedding lookup (src/model/NRMS/news_encoder.py:38 etc.) --------------------- */
 /* X[row(seg,t)] = table[ids[seg*T+t]]; padded!=0 writes the zero-padded CNN layout (T+2 rows per segment).
@@ -89,6 +93,11 @@ int nr_mhsa_core_bwd(const void* qkv_bf16, int ld_qkv, int sec, const void* dctx
 int nr_additive_attention_fwd(const void* X_bf16, long long n_seg, int seg_len, int D, int ldx, const void* Wa_bf16,
                               int q, int ldw, const float* ba, const float* qv, float* out, int ldo, float* w_out,
                               void* stream);
+/* the same with the input as a hi/lo pair X = X_bf16 + X_lo_bf16 (same pitch; nr_rows_to_bf16_hilo): the scores read the hi
+ * plane, the pooled sum both (~16 mantissa bits).  The backward is nr_additive_attention_bwd on the hi plane. */
+int nr_additive_attention_fwd_hilo(const void* X_bf16, const void* X_lo_bf16, long long n_seg, int seg_len, int D, int ldx,
+                                   const void* Wa_bf16, int q, int ldw, const float* ba, const float* qv, float* out, int ldo,
+                                   float* w_out, void* stream);
 /* backward.  dX bf16 [rows][ld_dx] (=), dWa_ext fp32 [q][ldx] (+=, column D is d(bias)), dqv [q] (+=).
  * workspace: nr_additive_attention_bwd_workspace(...) bytes. */
 long long nr_additive_attention_bwd_workspace(long long n_seg, int seg_len, int q);
@@ -181,6 +190,9 @@ typedef struct {
      * nr_mhsa_accurate_supported): V, the attention probabilities and the context are hi/lo bf16 pairs; X_bf16 and QKV_bf16
      * (the hi planes) are written as usual and saved for the backward. */
     void* V_lo_bf16;             /* [n_seq*T][sec] low plane of the V section                                            */
+    /* dense variants only (NULL otherwise): fp32 [T][d] contiguous positional addend; the rows entering the projection are
+     * X = dense + dense_pos[t], summed in fp32 before any rounding (Exp1's user encoder) */
+    const float* dense_pos;
 } nr_mhsa_encoder_fwd_args;
 int nr_mhsa_accurate_supported(int T, int d, int heads); /* 1: the accurate news variant exists for this shape */
 int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream);
@@ -216,6 +228,9 @@ typedef struct {
     /* optional cudaEvent_t recorded on `stream` as soon as demb is complete (before the weight-gradient GEMM): a data-
      * parallel caller starts the embedding-gradient all-reduce on a side stream that waits for it */
     void* emb_grad_ready_event;
+    /* dense variant only (NULL otherwise): fp32 [T][d] (+=) gradient of dense_pos = sum over the sequences of ddense, in a fixed
+     * order (bit-identical across runs) */
+    float* dpos;
 } nr_mhsa_encoder_bwd_args;
 long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q);
 int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream);

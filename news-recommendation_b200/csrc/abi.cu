@@ -46,6 +46,11 @@ int nr_rows_to_bf16(const float* src, long long n, int D, long long s_row, long 
     NR_REQUIRE(src && dst && n >= 0 && ld % 8 == 0, "nr_rows_to_bf16: n=%lld ld=%d", n, ld);
     return rows_to_bf16(src, n, 1, D, s_row, 0, s_col, dst, ld, as_stream(stream));
 }
+int nr_rows_to_bf16_hilo(const float* src, long long n, int D, long long s_row, long long s_col, void* hi, void* lo, int ld,
+                         void* stream) {
+    NR_REQUIRE(src && hi && lo && n >= 0 && D >= 1 && ld % 8 == 0, "nr_rows_to_bf16_hilo: n=%lld D=%d ld=%d", n, D, ld);
+    return rows_to_bf16_planes(src, n, D, s_row, s_col, hi, lo, ld, as_stream(stream));
+}
 int nr_gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld, void* X,
                    int padded, float p_drop, unsigned long long seed, int* bad_id_flag, void* stream) {
     NR_REQUIRE(ids && table && X && bad_id_flag && T >= 1 && n_tok % T == 0 && p_drop >= 0.f && p_drop < 1.f,
@@ -82,6 +87,13 @@ int nr_additive_attention_fwd(const void* X, long long n_seg, int seg_len, int D
     NR_REQUIRE(n_seg * seg_len < (1ll << 31), "nr_additive_attention_fwd: too many rows");
     return gemm_additive_pool(X, static_cast<int>(n_seg * seg_len), ldx, D, Wa, q, ldw, ba, qv, seg_len, out, ldo, w_out,
                               as_stream(stream));
+}
+int nr_additive_attention_fwd_hilo(const void* X, const void* X_lo, long long n_seg, int seg_len, int D, int ldx, const void* Wa,
+                                   int q, int ldw, const float* ba, const float* qv, float* out, int ldo, float* w_out, void* stream) {
+    NR_REQUIRE(X && X_lo && Wa && ba && qv && out, "nr_additive_attention_fwd_hilo: null operand");
+    NR_REQUIRE(n_seg * seg_len < (1ll << 31), "nr_additive_attention_fwd_hilo: too many rows");
+    return gemm_additive_pool(X, static_cast<int>(n_seg * seg_len), ldx, D, Wa, q, ldw, ba, qv, seg_len, out, ldo, w_out,
+                              as_stream(stream), X_lo);
 }
 struct AdditiveBwdWorkspace : WorkspaceLayout {
     float* dscore;
@@ -181,6 +193,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
     const bool precise_dense = a->dense != nullptr && a->C_lo_bf16 != nullptr;
     NR_REQUIRE(precise_dense || (a->wqkv_bf16 && a->bqkv && a->X_bf16 && a->QKV_bf16), "nr_mhsa_encoder_fwd: null operand");
     NR_REQUIRE(a->p_drop >= 0.f && a->p_drop < 1.f, "nr_mhsa_encoder_fwd: dropout p=%f", a->p_drop);
+    NR_REQUIRE(a->dense_pos == nullptr || a->dense != nullptr, "nr_mhsa_encoder_fwd: dense_pos needs the dense (user-level) variant");
     if (a->n_seq == 0) return 0;
     const int M = static_cast<int>(a->n_seq * a->T);
     const cudaStream_t st = as_stream(stream);
@@ -192,9 +205,10 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         NR_REQUIRE(a->wqkv_kcat_bf16 && a->X_kcat_bf16 && a->QKV_f32 && a->bqkv && a->X_bf16,
                    "nr_mhsa_encoder_fwd: precise dense variant needs wqkv_kcat_bf16 / X_kcat_bf16 / QKV_f32 / bqkv / X_bf16");
         NR_REQUIRE(a->QKV_bf16 == nullptr, "nr_mhsa_encoder_fwd: the precise dense variant writes no bf16 Q|K|V (pass NULL)");
-        NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_bf16, a->ldx, st));
+        NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_bf16, a->ldx, st,
+                                  a->dense_pos));
         NR_PROPAGATE(rows_to_bf16_hilo(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_kcat_bf16,
-                                       a->ldx, st));
+                                       a->ldx, st, a->dense_pos));
         NR_PROPAGATE(gemm_store({.A = a->X_kcat_bf16, .M = M, .lda = 2 * a->ldx, .W = a->wqkv_kcat_bf16, .N = 3 * sec, .ldw = 2 * a->ldx,
                                  .K = 2 * a->ldx},
                                 {.out = a->QKV_f32, .ld_out = 3 * sec, .bias = a->bqkv}, st));
@@ -231,7 +245,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
                                  DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
     } else {
         NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col,
-                                  a->X_bf16, a->ldx, st));
+                                  a->X_bf16, a->ldx, st, a->dense_pos));
     }
     // Q|K|V = X . Wqkv^T + b   (multihead_self.py:53-58)
     NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
@@ -269,6 +283,7 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
                "nr_mhsa_encoder_bwd: Q|K|V was not saved (precise dense forward): pass wqkv_bf16 / bqkv so that it can be recomputed from X");
     NR_REQUIRE((a->ids != nullptr) ? (a->demb != nullptr) : (a->ddense != nullptr),
                "nr_mhsa_encoder_bwd: missing input-gradient buffer");
+    NR_REQUIRE(a->dpos == nullptr || a->ids == nullptr, "nr_mhsa_encoder_bwd: dpos needs the dense (user-level) variant");
     const MhsaBwdWorkspace ws(a->workspace, a->n_seq * a->T, a->d, a->q);
     NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_mhsa_encoder_bwd: workspace too small (%lld bytes)", a->workspace_bytes);
     if (a->n_seq == 0) return 0;
@@ -303,6 +318,8 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     } else {
         NR_PROPAGATE(gemm_store({.A = ws.dQKV, .M = M, .lda = a->ld3, .W = a->wqkvT_bf16, .N = a->d, .ldw = a->ld3, .K = 3 * sec},
                                 {.out = a->ddense, .ld_out = a->d}, st));
+        // X = dense + pos[t]: the positional gradient is the input gradient summed over the sequences
+        if (a->dpos != nullptr) NR_PROPAGATE(sum_over_seq(a->ddense, a->n_seq, static_cast<long long>(a->T) * a->d, a->dpos, st));
     }
     // both weight-gradient GEMMs run AFTER the embedding gradient is complete: together they are the window (~0.4 ms) under which
     // the caller's all-reduce of that gradient hides

@@ -120,11 +120,13 @@ int cast_pad_bf16_many(int n, const float* const* src, const int* R, const int* 
 }
 
 // fp32 rows [n_seq][T][D] (arbitrary element strides) -> bf16 rows [n_seq*T x ld] with a ones column at D.
+// pos (fp32 [T][D] contiguous, or null): x + pos[tok] is formed in fp32 before the one rounding.
 // One thread per 8-column chunk column, a block walks kRowsThreads / chunks rows per iteration (no division in the loop).
 constexpr int kRowsThreads = 320;
 __global__ void __launch_bounds__(kRowsThreads) rows_to_bf16_kernel(const float* __restrict__ src, long long n_rows, int T, int D,
                                                                   long long s_seq, long long s_tok, long long s_col,
-                                                                  __nv_bfloat16* __restrict__ dst, int ld) {
+                                                                  __nv_bfloat16* __restrict__ dst, int ld,
+                                                                  const float* __restrict__ pos) {
     const int chunks = ld >> 3;
     const int rows_per_it = kRowsThreads / chunks;
     const int rl = threadIdx.x / chunks, c = threadIdx.x - rl * chunks;
@@ -143,12 +145,18 @@ __global__ void __launch_bounds__(kRowsThreads) rows_to_bf16_kernel(const float*
 #pragma unroll
             for (int j = 0; j < 8; ++j) v[j] = col + j < D ? sp[(col + j) * s_col] : (col + j == D ? 1.0f : 0.f);
         }
+        if (pos != nullptr) {
+            const float* pp = pos + tok * D;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                if (col + j < D) v[j] += pp[col + j];
+        }
         *reinterpret_cast<uint4*>(dst + r * ld + col) =
             make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
     }
 }
 int rows_to_bf16(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col,
-                 void* dst, int ld, cudaStream_t stream) {
+                 void* dst, int ld, cudaStream_t stream, const float* pos) {
     const long long n = n_seq * T;
     if (n == 0) return 0;
     NR_REQUIRE(ld >= D + 1 && ld % 8 == 0 && ld / 8 <= kRowsThreads, "rows_to_bf16: pitch %d for D=%d plus the ones column", ld, D);
@@ -156,7 +164,7 @@ int rows_to_bf16(const float* src, long long n_seq, int T, int D, long long s_se
     const int blocks = static_cast<int>(std::min<long long>((n + rows_per_it - 1) / rows_per_it, 148 * 6));
     ProfScope ps("rows_to_bf16", static_cast<int>(n), D, ld, stream);
     rows_to_bf16_kernel<<<blocks, kRowsThreads, 0, stream>>>(src, n, T, D, s_seq, s_tok, s_col, static_cast<__nv_bfloat16*>(dst),
-                                                             ld);
+                                                             ld, pos);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -569,10 +577,11 @@ int dot_score_bwd(const float* cand, const float* user, const float* dlogits, in
 // ------------------------------------------------------------------------------------------------
 // fp32 rows [n_seq][T][D] (element strides) -> bf16 [rows][2*ld]: columns [0, D) = hi = bf16(x), column D = 1.0, zeros up to
 // ld; columns [ld, ld + D) = lo = bf16(x - hi), zeros up to 2*ld.  Against the K-concatenated weight operand [W | W] the GEMM
-// computes (hi + lo) . W^T: the input enters with ~16 mantissa bits instead of 8.
+// computes (hi + lo) . W^T: the input enters with ~16 mantissa bits instead of 8.  pos: as in rows_to_bf16 (the hi plane stays
+// bitwise what rows_to_bf16 writes for the same src and pos).
 __global__ void __launch_bounds__(256) rows_to_bf16_hilo_kernel(const float* __restrict__ src, long long n_rows, int T, int D,
                                                                 long long s_seq, long long s_tok, long long s_col,
-                                                                __nv_bfloat16* __restrict__ dst, int ld) {
+                                                                __nv_bfloat16* __restrict__ dst, int ld, const float* __restrict__ pos) {
     const int chunks = (2 * ld) >> 3;
     const long long total = n_rows * chunks;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -582,12 +591,14 @@ __global__ void __launch_bounds__(256) rows_to_bf16_hilo_kernel(const float* __r
         const bool lo = c >= ld;
         const int col = lo ? c - ld : c;
         const long long seq = r / T;
-        const float* sp = src + seq * s_seq + (r - seq * T) * s_tok;
+        const long long tok = r - seq * T;
+        const float* sp = src + seq * s_seq + tok * s_tok;
         float v[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int cc = col + j;
             float x = cc < D ? sp[cc * s_col] : 0.f;
+            if (pos != nullptr && cc < D) x += pos[tok * D + cc];
             const float hi = bf16_round(x);
             v[j] = lo ? (x - hi) : (cc == D ? 1.0f : hi);
         }
@@ -596,13 +607,89 @@ __global__ void __launch_bounds__(256) rows_to_bf16_hilo_kernel(const float* __r
     }
 }
 int rows_to_bf16_hilo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst,
-                      int ld, cudaStream_t stream) {
+                      int ld, cudaStream_t stream, const float* pos) {
     const long long n = n_seq * T;
     if (n == 0) return 0;
     NR_REQUIRE(ld >= D + 1 && ld % 8 == 0, "rows_to_bf16_hilo: pitch %d for D=%d plus the ones column", ld, D);
     ProfScope ps("rows_to_bf16_hilo", static_cast<int>(n), D, ld, stream);
     const int blocks = static_cast<int>(std::min<long long>((n * (2 * ld / 8) + 255) / 256, 148 * 8));
-    rows_to_bf16_hilo_kernel<<<blocks, 256, 0, stream>>>(src, n, T, D, s_seq, s_tok, s_col, static_cast<__nv_bfloat16*>(dst), ld);
+    rows_to_bf16_hilo_kernel<<<blocks, 256, 0, stream>>>(src, n, T, D, s_seq, s_tok, s_col, static_cast<__nv_bfloat16*>(dst), ld,
+                                                         pos);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// fp32 rows [n][D] (element strides) -> two bf16 planes of pitch ld in one pass: hi = bf16(x) with the ones column at D, lo =
+// bf16(x - hi) with zeros from D on.  The hi/lo input of an additive attention (the pooled sum reads both planes).
+__global__ void __launch_bounds__(256) rows_to_bf16_planes_kernel(const float* __restrict__ src, long long n_rows, int D,
+                                                                  long long s_row, long long s_col, __nv_bfloat16* __restrict__ hi_out,
+                                                                  __nv_bfloat16* __restrict__ lo_out, int ld) {
+    const int chunks = ld >> 3;
+    const long long total = n_rows * chunks;
+    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += gridDim.x * 256ll) {
+        const long long r = i / chunks;
+        const int col = static_cast<int>(i - r * chunks) * 8;
+        const float* sp = src + r * s_row;
+        float h[8], l[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float x = col + j < D ? sp[(col + j) * s_col] : 0.f;
+            const float hi = bf16_round(x);
+            h[j] = col + j == D ? 1.0f : hi;
+            l[j] = x - hi;
+        }
+        *reinterpret_cast<uint4*>(hi_out + r * ld + col) =
+            make_uint4(pack_bf16x2(h[0], h[1]), pack_bf16x2(h[2], h[3]), pack_bf16x2(h[4], h[5]), pack_bf16x2(h[6], h[7]));
+        *reinterpret_cast<uint4*>(lo_out + r * ld + col) =
+            make_uint4(pack_bf16x2(l[0], l[1]), pack_bf16x2(l[2], l[3]), pack_bf16x2(l[4], l[5]), pack_bf16x2(l[6], l[7]));
+    }
+}
+int rows_to_bf16_planes(const float* src, long long n, int D, long long s_row, long long s_col, void* hi, void* lo, int ld,
+                        cudaStream_t stream) {
+    if (n == 0) return 0;
+    NR_REQUIRE(ld >= D + 1 && ld % 8 == 0, "rows_to_bf16_planes: pitch %d for D=%d plus the ones column", ld, D);
+    ProfScope ps("rows_to_bf16_planes", static_cast<int>(n), D, ld, stream);
+    const int blocks = static_cast<int>(std::min<long long>((n * (ld / 8) + 255) / 256, 148 * 8));
+    rows_to_bf16_planes_kernel<<<blocks, 256, 0, stream>>>(src, n, D, s_row, s_col, static_cast<__nv_bfloat16*>(hi),
+                                                           static_cast<__nv_bfloat16*>(lo), ld);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// dst[e] += sum_s src[s * L + e] for e < L, s < n_seq (the gradient of a per-position addend shared by every sequence).  A CTA owns
+// 32 consecutive e; warp w sums the sequences s = w (mod 8) in increasing order, the eight partials are added in warp order: the
+// result is the same bits on every run (no atomics).
+constexpr int kSeqSumWarps = 8;
+__global__ void __launch_bounds__(32 * kSeqSumWarps) sum_over_seq_kernel(const float* __restrict__ src, long long n_seq, long long L,
+                                                                        float* __restrict__ dst) {
+    __shared__ float part[kSeqSumWarps][32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const long long e = blockIdx.x * 32ll + lane;
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    if (e < L) {
+        long long s = w;
+        for (; s + 3 * kSeqSumWarps < n_seq; s += 4 * kSeqSumWarps) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) acc[k] += src[(s + k * kSeqSumWarps) * L + e];
+        }
+        for (; s < n_seq; s += kSeqSumWarps) acc[0] += src[s * L + e];
+    }
+    part[w][lane] = (acc[0] + acc[1]) + (acc[2] + acc[3]);
+    __syncthreads();
+    if (w == 0 && e < L) {
+        float t = part[0][lane];
+#pragma unroll
+        for (int k = 1; k < kSeqSumWarps; ++k) t += part[k][lane];
+        dst[e] += t;
+    }
+}
+int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cudaStream_t stream) {
+    if (n_seq == 0 || L == 0) return 0;
+    NR_REQUIRE(L > 0 && (L + 31) / 32 < (1ll << 31), "sum_over_seq: L=%lld", L);
+    ProfScope ps("sum_over_seq", static_cast<int>(n_seq), static_cast<int>(std::min<long long>(L, 1 << 30)), 0, stream);
+    sum_over_seq_kernel<<<static_cast<unsigned>((L + 31) / 32), 32 * kSeqSumWarps, 0, stream>>>(src, n_seq, L, dst);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -94,9 +94,15 @@ int cast_pad_bf16(const float* src, int R, int C, int lds, void* dst, int ld, in
 // up to 8 such casts in one launch
 int cast_pad_bf16_many(int n, const float* const* src, const int* R, const int* C, const int* lds, void* const* dst, const int* ld,
                        const int* transpose, cudaStream_t stream);
-// fp32 rows [n_seq][T][D] with element strides -> bf16 [n_seq*T x ld], ones column at D, zeros after
+// fp32 rows [n_seq][T][D] with element strides -> bf16 [n_seq*T x ld], ones column at D, zeros after.
+// pos (fp32 [T][D] contiguous, may be null): the rows converted are x + pos[t], summed in fp32 before the rounding
 int rows_to_bf16(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col,
-                 void* dst, int ld, cudaStream_t stream);
+                 void* dst, int ld, cudaStream_t stream, const float* pos = nullptr);
+// fp32 rows [n][D] -> hi = bf16(x) (ones column at D) and lo = bf16(x - hi) (zeros from D on), both [n x ld], one pass
+int rows_to_bf16_planes(const float* src, long long n, int D, long long s_row, long long s_col, void* hi, void* lo, int ld,
+                        cudaStream_t stream);
+// dst[e] += sum_s src[s*L + e] (e < L, s < n_seq): fixed summation order, bit-identical across runs
+int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cudaStream_t stream);
 // X[row(seg,t)] = table_bf16[ids[seg*T+t]] (bit-exact copy), ones column at D, optional dropout, optional padded layout
 int gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld_table, void* X,
                 int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream);
@@ -139,7 +145,7 @@ int gru_fwd_persistent(int B, int S, int Hd, int ldh, int ldg, const float* gi, 
 int rows_to_bf16_lo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst, int ld,
                     cudaStream_t stream);
 int rows_to_bf16_hilo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst,
-                      int ld, cudaStream_t stream);
+                      int ld, cudaStream_t stream, const float* pos = nullptr);
 int mhsa_f32_fwd(const float* qkv, int ld, int sec, long long n_seq, int T, int heads, int dk, void* c_hi, void* c_lo, int ldc,
                  cudaStream_t stream);
 // scores[i] = news[cand[i]] . user[s] for seg_offsets[s] <= i < seg_offsets[s+1]  (batched evaluate.py:245-265)

@@ -7,7 +7,7 @@ restatement of the knob surface, not a copy of the reference source.
 import os
 
 model_name = os.environ.get("MODEL_NAME", "NRMS")
-SUPPORTED_MODELS = ("NRMS", "NAML", "LSTUR", "TANR")  # the hot-path scope of this build (SURVEY.md section 8)
+SUPPORTED_MODELS = ("NRMS", "NAML", "LSTUR", "TANR", "Exp1")  # the hot-path scope of this build (SURVEY.md section 8)
 if model_name not in SUPPORTED_MODELS:
     raise AssertionError(f"MODEL_NAME={model_name!r}: this build accelerates {SUPPORTED_MODELS} only")
 
@@ -46,6 +46,10 @@ _PER_MODEL = {
                   precision=os.environ.get("NEWSREC_PRECISION", "accurate"), **_CNN),
     "TANR": dict(dataset_attributes={"news": ["category", "title"], "record": []},
                  topic_classification_loss_weight=0.1, **_CNN),
+    # the reference leaves "abstract" as a TODO for Exp1; this build raises if it is configured (DESIGN.md section 6).
+    # precision as NRMS: "accurate" also keeps the stacked views in front of final_attention as hi/lo bf16 pairs
+    "Exp1": dict(dataset_attributes={"news": ["category", "subcategory", "title"], "record": []}, num_attention_heads=15,
+                 ensemble_factor=1, precision=os.environ.get("NEWSREC_PRECISION", "accurate")),
 }
 for _name, _knobs in _PER_MODEL.items():
     globals()[f"{_name}Config"] = type(f"{_name}Config", (BaseConfig,), dict(_knobs))

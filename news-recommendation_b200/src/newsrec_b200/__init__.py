@@ -27,6 +27,7 @@ class MhsaEncoderFwdArgs(C.Structure):
         ("C_lo_bf16", _vp),
         ("wqkv_kcat_bf16", _vp), ("X_kcat_bf16", _vp), ("QKV_f32", _vp),
         ("V_lo_bf16", _vp),
+        ("dense_pos", _vp),
     ]
 
 
@@ -41,6 +42,7 @@ class MhsaEncoderBwdArgs(C.Structure):
         ("dWqkv_ext", _vp), ("dWa_ext", _vp), ("dqv", _vp), ("demb", _vp), ("ddense", _vp),
         ("workspace", _vp), ("workspace_bytes", _ll),
         ("wqkv_bf16", _vp), ("bqkv", _vp), ("emb_grad_ready_event", _vp),
+        ("dpos", _vp),
     ]
 
 
@@ -109,12 +111,14 @@ SIGNATURES = {
     "nr_cast_pad_bf16": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp]),
     "nr_cast_pad_bf16_many": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nr_rows_to_bf16": (_i, [_vp, _ll, _i, _ll, _ll, _vp, _i, _vp]),
+    "nr_rows_to_bf16_hilo": (_i, [_vp, _ll, _i, _ll, _ll, _vp, _vp, _i, _vp]),
     "nr_gather_rows": (_i, [_vp, _ll, _i, _vp, _i, _i, _i, _vp, _i, _f, _ull, _vp, _vp]),
     "nr_linear": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp]),
     "nr_gemm_tn": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "nr_mhsa_core_fwd": (_i, [_vp, _i, _i, _ll, _i, _i, _i, _vp, _i, _f, _ull, _vp]),
     "nr_mhsa_core_bwd": (_i, [_vp, _i, _i, _vp, _i, _ll, _i, _i, _i, _vp, _i, _vp]),
     "nr_additive_attention_fwd": (_i, [_vp, _ll, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp]),
+    "nr_additive_attention_fwd_hilo": (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp]),
     "nr_additive_attention_bwd_workspace": (_ll, [_ll, _i, _i]),
     "nr_additive_attention_bwd": (_i, [_vp, _ll, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i,
                                         _vp, _vp, _vp, _ll, _vp]),

@@ -5,7 +5,7 @@ collective on the path is the NCCL all-reduce of a flat fp32 gradient buffer per
 needs no packing copies and autograd accumulates straight into the communication buffer.  The largest
 parameter (the word-embedding table: 97 % of the buffer) sits FIRST in the buffer: its gradient is
 complete as soon as the news encoder's scatter GEMM has run, which the backward reports through a CUDA
-event (ops.grad_ready_hook), and its all-reduce is issued from a side stream that waits for that event --
+event attached to that gradient view (ops.GRAD_READY_ATTR), and its all-reduce is issued from a side stream that waits for that event --
 it runs under the weight-gradient GEMM that follows.  The rest of the buffer (a few hundred kB) is reduced
 after the backward.  The 1/world of the mean is folded into the reduction (ReduceOp.AVG): no extra pass
 over the 88 MB buffer.
@@ -69,14 +69,15 @@ class FlatGradients:
             off += pad4(n)
         self.big_numel = pad4(self.params[0].numel())
         self._side = None
-        self._event = None
+        self._hook = None
         if world > 1 and dev.type == "cuda" and dist.is_initialized() and dist.get_backend() == "nccl":
             from . import ops
             self._side = torch.cuda.Stream(device=dev)
-            self._event = torch.cuda.Event()
-            self._event.record()  # materialises the cudaEvent_t handle the backward records into
-            ops.grad_ready_hook["event"] = self._event
-            ops.grad_ready_hook["recorded"] = False
+            event = torch.cuda.Event()
+            event.record()  # materialises the cudaEvent_t handle the backward records into
+            # on this buffer's own view: the backward that writes it records THIS event, whichever other FlatGradients exist
+            self._hook = {"event": event, "recorded": False}
+            setattr(self.params[0].grad, ops.GRAD_READY_ATTR, self._hook)
             # NCCL's channel CTAs need SMs while the weight-gradient GEMM runs (it would otherwise hold all of them)
             from . import load_library
             load_library().nr_reserve_sms_for_comm(int(os.environ.get("NEWSREC_COMM_SMS", "32")))
@@ -98,11 +99,10 @@ class FlatGradients:
             dist.all_reduce(self.flat, op=dist.ReduceOp.SUM)
             self.flat.mul_(1.0 / self.world)
             return
-        from . import ops
         main = torch.cuda.current_stream()
-        if ops.grad_ready_hook["recorded"]:
+        if self._hook["recorded"]:
             # early slice: starts when the event the backward recorded behind the scatter GEMM fires
-            self._side.wait_event(self._event)
+            self._side.wait_event(self._hook["event"])
             with torch.cuda.stream(self._side):
                 if self._wire is not None:
                     self._wire.copy_(self.flat[:self.big_numel])
@@ -113,6 +113,6 @@ class FlatGradients:
             if self.big_numel < self.flat.numel():
                 dist.all_reduce(self.flat[self.big_numel:], op=dist.ReduceOp.AVG)
             main.wait_stream(self._side)
-            ops.grad_ready_hook["recorded"] = False
+            self._hook["recorded"] = False
         else:
             dist.all_reduce(self.flat, op=dist.ReduceOp.AVG)

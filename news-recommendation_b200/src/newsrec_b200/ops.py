@@ -30,9 +30,11 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-# Data-parallel hook (ddp.FlatGradients): a torch.cuda.Event the news-encoder backward records as soon as the embedding
-# gradient is complete, so that its all-reduce can start under the remaining backward kernels.  None = not armed.
-grad_ready_hook = {"event": None, "recorded": False}
+# Data-parallel hook (ddp.FlatGradients): the gradient view of the embedding table carries, under this attribute, the owning
+# buffer's {"event": torch.cuda.Event, "recorded": bool}; the news-encoder backward that writes that view records the event as
+# soon as the embedding gradient is complete, so that its all-reduce can start under the remaining backward kernels.  Keyed by the
+# gradient storage, so that models with a FlatGradients each (an ensemble) record into their own buffer's event.
+GRAD_READY_ATTR = "_newsrec_grad_ready"
 
 _seed_counter = [0x243F6A8885A308D3]
 
@@ -182,14 +184,18 @@ def table_operand(cache: OperandCache, name, weight):
 # NRMS NewsEncoder / UserEncoder: gather|dense -> MHSA -> additive pooling in ONE C call each way
 # ---------------------------------------------------------------------------------------------------
 class MhsaPoolEncoderFn(torch.autograd.Function):
-    """forward(ids|None, dense|None, emb_weight|None, Wq,bq,Wk,bk,Wv,bv, Wa,ba,qv, heads, p_drop, cache, prefix)
+    """forward(ids|None, dense|None, emb_weight|None, Wq,bq,Wk,bk,Wv,bv, Wa,ba,qv, heads, p_drop, cache, prefix, bad_flag,
+               precise, pos|None)
 
     ids   : int64 (n_seq, T) device tensor  (news encoder)   -- reference src/model/NRMS/news_encoder.py:27-48
     dense : fp32  (n_seq, T, d) any strides (user encoder)   -- reference src/model/NRMS/user_encoder.py:15-26
+    pos   : fp32  (T, d) added to every sequence of `dense` before the projection (reference src/model/Exp1/user_encoder.py:
+            26-27); its gradient is the input gradient summed over the sequences
     """
 
     @staticmethod
-    def forward(ctx, ids, dense, emb_w, Wq, bq, Wk, bk, Wv, bv, Wa, ba, qv, heads, p_drop, cache, prefix, bad_flag, precise=False):
+    def forward(ctx, ids, dense, emb_w, Wq, bq, Wk, bk, Wv, bv, Wa, ba, qv, heads, p_drop, cache, prefix, bad_flag, precise=False,
+                pos=None):
         lib = load_library()
         dev = require_cuda()
         d, q = Wq.shape[0], Wa.shape[0]
@@ -212,6 +218,12 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
             a.dense = _p(dense)
             a.dense_s_seq, a.dense_s_tok, a.dense_s_col = dense.stride()
             table = None
+        if pos is not None:
+            if ids is not None:
+                raise NewsrecError("a positional addend applies to the dense (user-level) input only")
+            if tuple(pos.shape) != (T, d):
+                raise NewsrecError(f"positional addend of shape {tuple(pos.shape)} for inputs of {T} positions x {d}")
+            a.dense_pos = _p(pos.detach().float().contiguous())
         n_tok = n_seq * T
         need_bwd = any(ctx.needs_input_grad)
         # precision modes (config.precision, DESIGN.md section 4):
@@ -252,7 +264,8 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
         ctx.meta = dict(n_seq=n_seq, T=T, d=d, q=q, heads=heads, p_drop=float(p_drop), seed=seed, ops=ops,
                         has_ids=ids is not None, V=emb_w.shape[0] if ids is not None else 0,
                         dense_shape=None if dense is None else tuple(dense.shape),
-                        params=(emb_w, Wq, bq, Wk, bk, Wv, bv, Wa, ba, qv), cache=cache, prefix=prefix)
+                        params=(emb_w, Wq, bq, Wk, bk, Wv, bv, Wa, ba, qv), cache=cache, prefix=prefix,
+                        pos=pos)
         return out
 
     @staticmethod
@@ -291,6 +304,12 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
                 demb = torch.zeros((m["V"], d), dtype=torch.float32, device=dev)
         else:
             ddense = torch.empty((n_seq * T, d), dtype=torch.float32, device=dev)
+        dpos, pos_direct = None, False
+        if m["pos"] is not None:  # the kernel adds into dpos: the parameter's own gradient storage, or a zeroed buffer returned below
+            dpos = grad_sink(m["pos"])
+            pos_direct = dpos is not None
+            if not pos_direct:
+                dpos = torch.zeros((T, d), dtype=torch.float32, device=dev)
         ws_bytes = int(lib.nr_mhsa_encoder_bwd_workspace(n_seq, T, d, q))
         ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
         a = MhsaEncoderBwdArgs()
@@ -301,38 +320,43 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
         a.p_drop, a.seed = m["p_drop"], m["seed"]
         a.X_bf16, a.QKV_bf16, a.C_bf16, a.w, a.dout = _p(X), (_p(QKV) if QKV.numel() else None), _p(Cx), _p(w), _p(dout)
         a.wqkv_bf16, a.bqkv = _p(ops["wqkv"]), _p(ops["bqkv"])
-        ev = grad_ready_hook["event"] if (m["has_ids"] and emb_direct) else None
-        if ev is not None:
-            a.emb_grad_ready_event = C.c_void_p(ev.cuda_event)
-            grad_ready_hook["recorded"] = True
+        hook = getattr(demb, GRAD_READY_ATTR, None) if (m["has_ids"] and emb_direct) else None
+        if hook is not None:
+            a.emb_grad_ready_event = C.c_void_p(hook["event"].cuda_event)
+            hook["recorded"] = True
         a.dWqkv_ext, a.dWa_ext, a.dqv = _p(dWqkv), _p(dWa), _p(dqv)
-        a.demb, a.ddense = _p(demb), _p(ddense)
+        a.demb, a.ddense, a.dpos = _p(demb), _p(ddense), _p(dpos)
         a.workspace, a.workspace_bytes = _p(ws), ws_bytes
         check(lib.nr_mhsa_encoder_bwd(C.byref(a), _stream()), "nr_mhsa_encoder_bwd")
         g_dense = ddense.view(m["dense_shape"]) if ddense is not None else None
         g_emb = None if emb_direct else demb
+        g_pos = None if pos_direct else dpos
         if direct:
             for i in range(3):
                 check(lib.nr_accumulate_ext_grad(_p(dWqkv[i * sec:i * sec + d]), d, ldx, d, _p(sinks[2 * i]), _p(sinks[2 * i + 1]),
                                                  _stream()), "nr_accumulate_ext_grad")
             check(lib.nr_accumulate_ext_grad(_p(dWa), q, ldx, d, _p(sinks[6]), _p(sinks[7]), _stream()), "nr_accumulate_ext_grad")
-            return (None, g_dense, g_emb) + (None,) * 15
+            return (None, g_dense, g_emb) + (None,) * 15 + (g_pos,)
         gW = [dWqkv[i * sec:i * sec + d, :d].contiguous() for i in range(3)]
         gb = [dWqkv[i * sec:i * sec + d, d].contiguous() for i in range(3)]
         return (None, g_dense, g_emb, gW[0], gb[0], gW[1], gb[1], gW[2], gb[2],
-                dWa[:, :d].contiguous(), dWa[:, d].contiguous(), dqv, None, None, None, None, None, None)
+                dWa[:, :d].contiguous(), dWa[:, d].contiguous(), dqv, None, None, None, None, None, None, g_pos)
 
 
 # ---------------------------------------------------------------------------------------------------
 # AdditiveAttention over dense fp32 rows (NAML / TANR user encoder, NAML 4-view fusion, standalone module)
 # ---------------------------------------------------------------------------------------------------
 class AdditiveAttentionFn(torch.autograd.Function):
-    """reference src/model/general/attention/additive.py:27-53;  x (N, S, D) fp32 -> (N, D)."""
+    """reference src/model/general/attention/additive.py:27-53;  x (N, S, D) fp32 -> (N, D).
+    precision "fast": x enters as bf16 rows; "accurate": as a hi/lo bf16 pair (the scores read the hi plane, the pooled sum
+    both: ~16 mantissa bits); the backward reads the hi plane in both modes."""
 
     @staticmethod
-    def forward(ctx, x, Wa, ba, qv, cache, prefix):
+    def forward(ctx, x, Wa, ba, qv, cache, prefix, precision="fast"):
         lib = load_library()
         dev = require_cuda()
+        if precision not in ("fast", "accurate"):
+            raise NewsrecError(f"additive attention precision must be 'fast' or 'accurate' (got {precision!r})")
         N, S, D = x.shape
         q = Wa.shape[0]
         ldx, ldq = ru8(D + 1), ru16(q)
@@ -342,11 +366,18 @@ class AdditiveAttentionFn(torch.autograd.Function):
         xf = x.float()
         X = torch.empty((N * S, ldx), dtype=torch.bfloat16, device=dev)
         xs = xf.reshape(N * S, D) if xf.is_contiguous() else xf.contiguous().view(N * S, D)
-        check(lib.nr_rows_to_bf16(_p(xs), N * S, D, xs.stride(0), xs.stride(1), _p(X), ldx, _stream()), "nr_rows_to_bf16")
         out = torch.empty((N, D), dtype=torch.float32, device=dev)
         w = torch.empty((N * S,), dtype=torch.float32, device=dev)
-        check(lib.nr_additive_attention_fwd(_p(X), N, S, D, ldx, _p(ops["wa"]), q, ldx, _p(ops["ba"]), _p(ops["qv"]),
-                                            _p(out), D, _p(w), _stream()), "nr_additive_attention_fwd")
+        if precision == "accurate":
+            X_lo = torch.empty((N * S, ldx), dtype=torch.bfloat16, device=dev)
+            check(lib.nr_rows_to_bf16_hilo(_p(xs), N * S, D, xs.stride(0), xs.stride(1), _p(X), _p(X_lo), ldx, _stream()),
+                  "nr_rows_to_bf16_hilo")
+            check(lib.nr_additive_attention_fwd_hilo(_p(X), _p(X_lo), N, S, D, ldx, _p(ops["wa"]), q, ldx, _p(ops["ba"]),
+                                                     _p(ops["qv"]), _p(out), D, _p(w), _stream()), "nr_additive_attention_fwd_hilo")
+        else:
+            check(lib.nr_rows_to_bf16(_p(xs), N * S, D, xs.stride(0), xs.stride(1), _p(X), ldx, _stream()), "nr_rows_to_bf16")
+            check(lib.nr_additive_attention_fwd(_p(X), N, S, D, ldx, _p(ops["wa"]), q, ldx, _p(ops["ba"]), _p(ops["qv"]),
+                                                _p(out), D, _p(w), _stream()), "nr_additive_attention_fwd")
         ctx.save_for_backward(X, w)
         ctx.meta = dict(N=N, S=S, D=D, q=q, ops=ops)
         return out
@@ -369,7 +400,7 @@ class AdditiveAttentionFn(torch.autograd.Function):
                                             _p(ops["qv"]), _p(w), _p(dout), D, _p(dX), ldx, _p(dWa), _p(dqv), _p(ws),
                                             ws_bytes, _stream()), "nr_additive_attention_bwd")
         gx = dX[:, :D].float().view(N, S, D)
-        return gx, dWa[:, :D].contiguous(), dWa[:, D].contiguous(), dqv, None, None
+        return gx, dWa[:, :D].contiguous(), dWa[:, D].contiguous(), dqv, None, None, None
 
 
 # ---------------------------------------------------------------------------------------------------

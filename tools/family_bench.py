@@ -7,6 +7,7 @@ inputs.  A coverage measurement next to bench.py (which is the contract benchmar
 import importlib
 import json
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -45,9 +46,16 @@ CASES = [
     ("TANR", {}, ("title", "category")),
     ("LSTUR", {"long_short_term_method": "ini"}, ("title", "category")),
     ("LSTUR", {"long_short_term_method": "con"}, ("title", "category")),
+    ("Exp1", {}, ("title", "category")),
 ]
 label = torch.zeros(B, dtype=torch.long, device=dev)
 res = {}
+try:  # the card and its power limit belong beside every number of this run
+    card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True, timeout=30).stdout.strip()
+except (OSError, subprocess.SubprocessError):
+    card = torch.cuda.get_device_name(dev) + ", power limit unknown"
+print("card:", card, flush=True)
 for name, over, want in CASES:
     cfg = type("Cfg", (getattr(cfgmod, name + "Config"),), over)
     model = getattr(importlib.import_module("model." + name), name)(cfg).to(dev)
@@ -85,4 +93,4 @@ for name, over, want in CASES:
     print(key, res[key], flush=True)
     del model, grads
     torch.cuda.empty_cache()
-print(json.dumps({"batch": B, "families": res}))
+print(json.dumps({"batch": B, "card": card, "families": res}))
