@@ -31,25 +31,39 @@ void nr_profile_enable(int on) { prof_enable(on); }
 void nr_profile_context(const char* ctx) { prof_context(ctx ? ctx : ""); }
 int nr_profile_report(char* buf, int cap) { return prof_report(buf, cap); }
 
+// the zero-padded bf16 operand of an fp32 [R][C] matrix of pitch lds, or of its transpose
+static Bf16Rows cast_pad_job(const float* src, int R, int C, int lds, void* dst, int ld, int transpose) {
+    if (transpose) return {.src = src, .n_rows = C, .D = R, .s_seq = 1, .s_col = lds, .width = ld, .hi = dst, .ld_hi = ld};
+    return {.src = src, .n_rows = R, .D = C, .s_seq = lds, .width = ld, .hi = dst, .ld_hi = ld};
+}
 int nr_cast_pad_bf16_many(int n, const float* const* src, const int* R, const int* C, const int* lds, void* const* dst, const int* ld,
                           const int* transpose, void* stream) {
     NR_REQUIRE(src && R && C && lds && dst && ld && transpose, "nr_cast_pad_bf16_many: null argument array");
-    return cast_pad_bf16_many(n, src, R, C, lds, dst, ld, transpose, as_stream(stream));
+    NR_REQUIRE(n >= 0 && n <= kBf16RowsJobs, "nr_cast_pad_bf16_many: %d matrices (at most %d per call)", n, kBf16RowsJobs);
+    Bf16Rows jobs[kBf16RowsJobs];
+    for (int i = 0; i < n; ++i) {
+        NR_REQUIRE(R[i] >= 1 && C[i] >= 1, "nr_cast_pad_bf16_many: bad matrix %d", i);
+        jobs[i] = cast_pad_job(src[i], R[i], C[i], lds[i], dst[i], ld[i], transpose[i]);
+    }
+    return rows_to_bf16(jobs, n, kCastPadMany, as_stream(stream));
 }
 int nr_cast_pad_bf16(const float* src, int R, int C, int lds, void* dst, int ld, int transpose, void* stream) {
     NR_REQUIRE(src && dst && R >= 0 && C >= 0 && ld % 8 == 0 && ld >= (transpose ? R : C),
                "nr_cast_pad_bf16: R=%d C=%d ld=%d transpose=%d", R, C, ld, transpose);
-    return cast_pad_bf16(src, R, C, lds, dst, ld, transpose, as_stream(stream));
+    return rows_to_bf16(cast_pad_job(src, R, C, lds, dst, ld, transpose), kCastPad, as_stream(stream));
 }
 int nr_rows_to_bf16(const float* src, long long n, int D, long long s_row, long long s_col, void* dst, int ld,
                     void* stream) {
     NR_REQUIRE(src && dst && n >= 0 && ld % 8 == 0, "nr_rows_to_bf16: n=%lld ld=%d", n, ld);
-    return rows_to_bf16(src, n, 1, D, s_row, 0, s_col, dst, ld, as_stream(stream));
+    return rows_to_bf16({.src = src, .n_rows = n, .D = D, .s_seq = s_row, .s_col = s_col, .width = ld, .hi = dst, .ld_hi = ld, .ones_col = 1},
+                        kRowsToBf16, as_stream(stream));
 }
 int nr_rows_to_bf16_hilo(const float* src, long long n, int D, long long s_row, long long s_col, void* hi, void* lo, int ld,
                          void* stream) {
     NR_REQUIRE(src && hi && lo && n >= 0 && D >= 1 && ld % 8 == 0, "nr_rows_to_bf16_hilo: n=%lld D=%d ld=%d", n, D, ld);
-    return rows_to_bf16_planes(src, n, D, s_row, s_col, hi, lo, ld, as_stream(stream));
+    return rows_to_bf16({.src = src, .n_rows = n, .D = D, .s_seq = s_row, .s_col = s_col, .width = ld, .hi = hi, .ld_hi = ld, .ones_col = 1,
+                         .lo = lo, .ld_lo = ld},
+                        kRowsToBf16Planes, as_stream(stream));
 }
 int nr_gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld, void* X,
                    int padded, float p_drop, unsigned long long seed, int* bad_id_flag, void* stream) {
@@ -185,6 +199,12 @@ int nr_mhsa_accurate_supported(int T, int d, int heads) {
     return mhsa_title_fwd_supported(T, d / heads, heads, sec, (3 * sec + 15) & ~15, (d + 8) & ~7) ? 1 : 0;
 }
 
+// the dense input rows [n_seq][T][d] (+ dense_pos) with the ones column at d, as the hi plane of pitch ld_hi
+static Bf16Rows dense_rows(const nr_mhsa_encoder_fwd_args* a, void* hi, int ld_hi) {
+    return {.src = a->dense, .n_rows = a->n_seq * a->T, .T = a->T, .D = a->d, .s_seq = a->dense_s_seq, .s_tok = a->dense_s_tok,
+            .s_col = a->dense_s_col, .pos = a->dense_pos, .width = a->ldx, .hi = hi, .ld_hi = ld_hi, .ones_col = 1};
+}
+
 int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_mhsa_encoder_fwd: null args");
     NR_PROPAGATE(check_mhsa_shape(a->n_seq, a->T, a->d, a->heads, a->q, a->ldx, a->ld3));
@@ -205,10 +225,12 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         NR_REQUIRE(a->wqkv_kcat_bf16 && a->X_kcat_bf16 && a->QKV_f32 && a->bqkv && a->X_bf16,
                    "nr_mhsa_encoder_fwd: precise dense variant needs wqkv_kcat_bf16 / X_kcat_bf16 / QKV_f32 / bqkv / X_bf16");
         NR_REQUIRE(a->QKV_bf16 == nullptr, "nr_mhsa_encoder_fwd: the precise dense variant writes no bf16 Q|K|V (pass NULL)");
-        NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_bf16, a->ldx, st,
-                                  a->dense_pos));
-        NR_PROPAGATE(rows_to_bf16_hilo(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col, a->X_kcat_bf16,
-                                       a->ldx, st, a->dense_pos));
+        NR_PROPAGATE(rows_to_bf16(dense_rows(a, a->X_bf16, a->ldx), kRowsToBf16, st));
+        // the same rows as [hi | lo] K-concatenated: against [W | W] the GEMM computes (hi + lo) . W^T
+        Bf16Rows kcat = dense_rows(a, a->X_kcat_bf16, 2 * a->ldx);
+        kcat.lo = static_cast<__nv_bfloat16*>(a->X_kcat_bf16) + a->ldx;
+        kcat.ld_lo = 2 * a->ldx;
+        NR_PROPAGATE(rows_to_bf16(kcat, kRowsToBf16Hilo, st));
         NR_PROPAGATE(gemm_store({.A = a->X_kcat_bf16, .M = M, .lda = 2 * a->ldx, .W = a->wqkv_kcat_bf16, .N = 3 * sec, .ldw = 2 * a->ldx,
                                  .K = 2 * a->ldx},
                                 {.out = a->QKV_f32, .ld_out = 3 * sec, .bias = a->bqkv}, st));
@@ -244,8 +266,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         NR_PROPAGATE(gather_rows(a->ids, M, a->T, a->table_bf16, a->V, a->d, a->ldx, a->X_bf16, a->ldx, 0,
                                  DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
     } else {
-        NR_PROPAGATE(rows_to_bf16(a->dense, a->n_seq, a->T, a->d, a->dense_s_seq, a->dense_s_tok, a->dense_s_col,
-                                  a->X_bf16, a->ldx, st, a->dense_pos));
+        NR_PROPAGATE(rows_to_bf16(dense_rows(a, a->X_bf16, a->ldx), kRowsToBf16, st));
     }
     // Q|K|V = X . Wqkv^T + b   (multihead_self.py:53-58)
     NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},

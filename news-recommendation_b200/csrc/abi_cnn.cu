@@ -102,7 +102,9 @@ int nr_linear_rows_fwd(const float* x, long long n, int K, long long s_row, long
                "nr_linear_rows_fwd: n=%lld K=%d ldx=%d ld_out=%d", n, K, ldx, ld_out);
     if (n == 0) return 0;
     prof_context("linear.fwd");
-    NR_PROPAGATE(rows_to_bf16(x, n, 1, K, s_row, 0, s_col, X_bf16, ldx, as_stream(stream)));
+    NR_PROPAGATE(rows_to_bf16({.src = x, .n_rows = n, .D = K, .s_seq = s_row, .s_col = s_col, .width = ldx, .hi = X_bf16, .ld_hi = ldx,
+                               .ones_col = 1},
+                              kRowsToBf16, as_stream(stream)));
     return gemm_store({.A = X_bf16, .M = static_cast<int>(n), .lda = ldx, .W = W_bf16, .N = N, .ldw = ldw, .K = K},
                       {.out = out, .ld_out = ld_out, .relu = relu, .bias = bias}, as_stream(stream));
 }

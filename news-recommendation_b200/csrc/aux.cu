@@ -1,7 +1,7 @@
-// Memory-bound companions of the wgmma GEMMs: operand preparation, the embedding-row gather,
-// the per-(sequence, head) self-attention core (fwd/bwd), pooling-backward row dots, the dot-product
-// click scorer.  All HBM-bound integer/byte or small-reduction work: coalesced 16-byte accesses,
-// warp-shuffle reductions, no tensor cores.
+// Memory-bound companions of the wgmma GEMMs: the fp32 -> bf16 row conversions, the embedding-row gather, pooling-backward
+// row dots, the dot-product click scorer, the fp32 attention of the precise user encoder, impression scoring and metrics,
+// the batch feed.  All HBM-bound integer/byte or small-reduction work: coalesced 16-byte accesses, warp-shuffle reductions,
+// no tensor cores.
 #include <algorithm>
 
 #include "nr_common.cuh"
@@ -10,161 +10,94 @@
 namespace nr {
 
 // ------------------------------------------------------------------------------------------------
-// fp32 parameter -> zero-padded bf16 operand (optionally transposed)
+// fp32 rows -> zero-padded bf16 planes (Bf16Rows, nr_ops.h)
 // ------------------------------------------------------------------------------------------------
-__global__ void cast_pad_kernel(const float* __restrict__ src, int R, int C, int lds, __nv_bfloat16* __restrict__ dst,
-                                int ld, int transpose) {
-    const long long n_rows = transpose ? C : R;
-    const long long total = n_rows * ld;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const long long r = i / ld;
-        const int c = static_cast<int>(i - r * ld);
-        float v = 0.f;
-        if (!transpose) {
-            if (c < C) v = src[r * lds + c];
-        } else {
-            if (c < R) v = src[static_cast<long long>(c) * lds + r];
-        }
-        dst[i] = __float2bfloat16_rn(v);
-    }
-}
-// non-transposed, 16-byte aligned rows: one thread per 8-column chunk (two float4 loads -> one 16-byte store), no division
-// per element.  The embedding table (85 MB of fp32 -> 43 MB of bf16) is rebuilt after every optimizer step: 0.07 -> 0.03 ms.
-__global__ void __launch_bounds__(256) cast_pad_rows_kernel(const float* __restrict__ src, long long R, int C, int lds,
-                                                            __nv_bfloat16* __restrict__ dst, int ld) {
-    const int chunks = ld >> 3;
-    const long long total = R * chunks;
-    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += gridDim.x * 256ll) {
-        const long long r = i / chunks;
-        const int col = static_cast<int>(i - r * chunks) * 8;
-        const float* sp = src + r * lds + col;
-        float v[8];
-        if (col + 8 <= C) {
-            const float4 a = __ldg(reinterpret_cast<const float4*>(sp)), b = __ldg(reinterpret_cast<const float4*>(sp) + 1);
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-        } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = col + j < C ? sp[j] : 0.f;
-        }
-        *reinterpret_cast<uint4*>(dst + r * ld + col) =
-            make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-    }
-}
-int cast_pad_bf16(const float* src, int R, int C, int lds, void* dst, int ld, int transpose, cudaStream_t stream) {
-    const long long total = static_cast<long long>(transpose ? C : R) * ld;
-    if (total == 0) return 0;
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148 * 16));
-    ProfScope ps("cast_pad", R, C, ld, stream);
-    if (!transpose && (ld & 7) == 0 && (lds & 3) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0 &&
-        (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-        const long long items = static_cast<long long>(R) * (ld >> 3);
-        cast_pad_rows_kernel<<<static_cast<int>(std::min<long long>((items + 255) / 256, 148 * 16)), 256, 0, stream>>>(
-            src, R, C, lds, static_cast<__nv_bfloat16*>(dst), ld);
-        ++g_launches;
-        NR_CHECK_CUDA(cudaGetLastError());
-        return 0;
-    }
-    cast_pad_kernel<<<blocks, 256, 0, stream>>>(src, R, C, lds, static_cast<__nv_bfloat16*>(dst), ld, transpose);
-    ++g_launches;
-    NR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// Several small operand casts in ONE launch (blockIdx.y = matrix): the packed / transposed projection and pooling weights of
-// an encoder are four matrices of a few hundred rows each -- as four launches they cost more in launch gaps than in work,
-// and they are rebuilt after every optimizer step.
-constexpr int kCastMany = 8;
-struct CastManyArgs {
-    const float* src[kCastMany];
-    __nv_bfloat16* dst[kCastMany];
-    int R[kCastMany], C[kCastMany], lds[kCastMany], ld[kCastMany], transpose[kCastMany];
+// One thread per 16-byte chunk (8 columns), grid-stride over the rows x chunks of a job: x is formed once per element and every
+// requested plane is written from it.  Chunks are taken row by row, so neighbouring threads read neighbouring columns; for strided
+// columns (a transpose) they are taken column by column instead, so that neighbouring threads read neighbouring rows and the
+// loads coalesce.  Several jobs share one launch (blockIdx.y = job): the packed and transposed weights of an encoder are a few
+// hundred rows each, and as separate launches they cost more in launch gaps than in work.  A single job runs in 512-thread
+// blocks with its descriptor at fixed parameter offsets; a batch runs in 128-thread blocks, so that its small jobs spread over
+// more SMs.
+template <int N>
+struct Bf16Jobs {
+    Bf16Rows job[N];
 };
-__global__ void __launch_bounds__(256) cast_pad_many_kernel(CastManyArgs a) {
-    const int m = blockIdx.y;
-    const float* __restrict__ src = a.src[m];
-    __nv_bfloat16* __restrict__ dst = a.dst[m];
-    const int R = a.R[m], C = a.C[m], lds = a.lds[m], ld = a.ld[m], transpose = a.transpose[m];
-    const long long total = static_cast<long long>(transpose ? C : R) * ld;
-    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += gridDim.x * 256ll) {
-        const long long r = i / ld;
-        const int c = static_cast<int>(i - r * ld);
-        float v = 0.f;
-        if (!transpose) {
-            if (c < C) v = src[r * lds + c];
-        } else {
-            if (c < R) v = src[static_cast<long long>(c) * lds + r];
-        }
-        dst[i] = __float2bfloat16_rn(v);
-    }
+__device__ __forceinline__ uint4 pack_bf16x8(const float (&v)[8]) {
+    return make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
 }
-int cast_pad_bf16_many(int n, const float* const* src, const int* R, const int* C, const int* lds, void* const* dst, const int* ld,
-                       const int* transpose, cudaStream_t stream) {
-    NR_REQUIRE(n >= 0 && n <= kCastMany, "cast_pad_bf16_many: %d matrices (at most %d per call)", n, kCastMany);
-    if (n == 0) return 0;
-    CastManyArgs a;
-    long long biggest = 0;
-    for (int i = 0; i < n; ++i) {
-        NR_REQUIRE(src[i] && dst[i] && R[i] >= 1 && C[i] >= 1 && ld[i] >= (transpose[i] ? R[i] : C[i]), "cast_pad_bf16_many: bad matrix %d", i);
-        a.src[i] = src[i];
-        a.dst[i] = static_cast<__nv_bfloat16*>(dst[i]);
-        a.R[i] = R[i], a.C[i] = C[i], a.lds[i] = lds[i], a.ld[i] = ld[i], a.transpose[i] = transpose[i];
-        biggest = std::max(biggest, static_cast<long long>(transpose[i] ? C[i] : R[i]) * ld[i]);
-    }
-    ProfScope ps("cast_pad_many", n, static_cast<int>(std::min<long long>(biggest, 1 << 30)), 0, stream);
-    const dim3 grid(static_cast<unsigned>(std::min<long long>((biggest + 255) / 256, 148 * 4)), static_cast<unsigned>(n));
-    cast_pad_many_kernel<<<grid, 256, 0, stream>>>(a);
-    ++g_launches;
-    NR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// fp32 rows [n_seq][T][D] (arbitrary element strides) -> bf16 rows [n_seq*T x ld] with a ones column at D.
-// pos (fp32 [T][D] contiguous, or null): x + pos[tok] is formed in fp32 before the one rounding.
-// One thread per 8-column chunk column, a block walks kRowsThreads / chunks rows per iteration (no division in the loop).
-constexpr int kRowsThreads = 320;
-__global__ void __launch_bounds__(kRowsThreads) rows_to_bf16_kernel(const float* __restrict__ src, long long n_rows, int T, int D,
-                                                                  long long s_seq, long long s_tok, long long s_col,
-                                                                  __nv_bfloat16* __restrict__ dst, int ld,
-                                                                  const float* __restrict__ pos) {
-    const int chunks = ld >> 3;
-    const int rows_per_it = kRowsThreads / chunks;
-    const int rl = threadIdx.x / chunks, c = threadIdx.x - rl * chunks;
-    if (rl >= rows_per_it) return;
-    const int col = c * 8;
-    for (long long r = static_cast<long long>(blockIdx.x) * rows_per_it + rl; r < n_rows;
-         r += static_cast<long long>(gridDim.x) * rows_per_it) {
-        const long long seq = r / T;
-        const long long tok = r - seq * T;
-        const float* sp = src + seq * s_seq + tok * s_tok;
-        float v[8];
-        if (s_col == 1 && col + 8 <= D && ((reinterpret_cast<uintptr_t>(sp + col) & 15) == 0)) {
-            const float4 a = *reinterpret_cast<const float4*>(sp + col), b = *reinterpret_cast<const float4*>(sp + col + 4);
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+template <int N, int kThreads>
+__global__ void __launch_bounds__(kThreads) rows_to_bf16_kernel(const __grid_constant__ Bf16Jobs<N> jobs) {
+    const Bf16Rows& j = jobs.job[N == 1 ? 0 : blockIdx.y];
+    const int D = j.D, T = j.T, chunks = j.width >> 3, n_rows = static_cast<int>(j.n_rows);  // n_rows * chunks < 2^30
+    const bool by_col = j.s_col != 1;
+    __nv_bfloat16* const hi = static_cast<__nv_bfloat16*>(j.hi);
+    __nv_bfloat16* const lo = static_cast<__nv_bfloat16*>(j.lo);
+    for (int i = blockIdx.x * kThreads + threadIdx.x; i < n_rows * chunks; i += gridDim.x * kThreads) {
+        const int c = by_col ? i / n_rows : i % chunks;
+        const int r = by_col ? i - c * n_rows : i / chunks;
+        const int col = c * 8;
+        const int seq = T == 1 ? r : r / T;
+        const int tok = r - seq * T;
+        const float* sp = j.src + seq * j.s_seq + tok * j.s_tok;
+        float x[8];
+        if (j.s_col == 1 && col + 8 <= D && (reinterpret_cast<uintptr_t>(sp + col) & 15) == 0) {
+            const float4 a = __ldg(reinterpret_cast<const float4*>(sp + col)), b = __ldg(reinterpret_cast<const float4*>(sp + col) + 1);
+            x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
         } else {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = col + j < D ? sp[(col + j) * s_col] : (col + j == D ? 1.0f : 0.f);
+            for (int e = 0; e < 8; ++e) x[e] = col + e < D ? __ldg(sp + (col + e) * j.s_col) : 0.f;
         }
-        if (pos != nullptr) {
-            const float* pp = pos + tok * D;
+        if (j.pos != nullptr) {
+            const float* pp = j.pos + tok * D;
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (col + j < D) v[j] += pp[col + j];
+            for (int e = 0; e < 8; ++e)
+                if (col + e < D) x[e] += __ldg(pp + col + e);
         }
-        *reinterpret_cast<uint4*>(dst + r * ld + col) =
-            make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+        if (hi != nullptr) {
+            float h[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) h[e] = j.ones_col && col + e == D ? 1.0f : x[e];
+            *reinterpret_cast<uint4*>(hi + static_cast<long long>(r) * j.ld_hi + col) = pack_bf16x8(h);
+        }
+        if (lo != nullptr) {
+            float l[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) l[e] = x[e] - bf16_round(x[e]);
+            *reinterpret_cast<uint4*>(lo + static_cast<long long>(r) * j.ld_lo + col) = pack_bf16x8(l);
+        }
     }
 }
-int rows_to_bf16(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col,
-                 void* dst, int ld, cudaStream_t stream, const float* pos) {
-    const long long n = n_seq * T;
+static bool plane_ok(const void* p, int ld, int width) {
+    return p == nullptr || ((reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld % 8 == 0 && ld >= width);
+}
+int rows_to_bf16(const Bf16Rows* jobs, int n_jobs, Bf16Op op, cudaStream_t stream) {
+    NR_REQUIRE(n_jobs >= 0 && n_jobs <= kBf16RowsJobs, "%s: %d jobs (at most %d per launch)", op.name, n_jobs, kBf16RowsJobs);
+    Bf16Jobs<kBf16RowsJobs> a;
+    int n = 0;
+    long long chunks = 0, biggest = 0;  // of the largest job
+    for (int i = 0; i < n_jobs; ++i) {
+        const Bf16Rows& j = jobs[i];
+        NR_REQUIRE(j.src && (j.hi || j.lo) && j.n_rows >= 0 && j.T >= 1 && j.D >= 0 && j.width % 8 == 0 &&
+                       j.width >= j.D + (j.hi && j.ones_col ? 1 : 0) && plane_ok(j.hi, j.ld_hi, j.width) && plane_ok(j.lo, j.ld_lo, j.width),
+                   "%s: job %d: n_rows=%lld T=%d D=%d width=%d ld_hi=%d ld_lo=%d (null or misaligned operand?)", op.name, i, j.n_rows, j.T,
+                   j.D, j.width, j.ld_hi, j.ld_lo);
+        NR_REQUIRE(j.n_rows * (j.width / 8) < (1ll << 30), "%s: job %d: %lld rows of %d columns", op.name, i, j.n_rows, j.width);
+        if (j.n_rows == 0 || j.width == 0) continue;
+        chunks = std::max(chunks, j.n_rows * (j.width / 8));
+        biggest = std::max(biggest, j.n_rows * j.width);
+        a.job[n++] = j;
+    }
     if (n == 0) return 0;
-    NR_REQUIRE(ld >= D + 1 && ld % 8 == 0 && ld / 8 <= kRowsThreads, "rows_to_bf16: pitch %d for D=%d plus the ones column", ld, D);
-    const int rows_per_it = kRowsThreads / (ld / 8);
-    const int blocks = static_cast<int>(std::min<long long>((n + rows_per_it - 1) / rows_per_it, 148 * 6));
-    ProfScope ps("rows_to_bf16", static_cast<int>(n), D, ld, stream);
-    rows_to_bf16_kernel<<<blocks, kRowsThreads, 0, stream>>>(src, n, T, D, s_seq, s_tok, s_col, static_cast<__nv_bfloat16*>(dst),
-                                                             ld, pos);
+    // one job: its shape; a batch: the job count and the largest job's elements
+    ProfScope ps(op.name, n_jobs == 1 ? static_cast<int>(a.job[0].n_rows) : n_jobs,
+                 n_jobs == 1 ? a.job[0].D : static_cast<int>(std::min<long long>(biggest, 1 << 30)), n_jobs == 1 ? a.job[0].width : 0,
+                 stream);
+    const int threads = n == 1 ? 512 : 128;
+    const dim3 grid(static_cast<unsigned>(std::min<long long>((chunks + threads - 1) / threads, 148ll * op.blocks_per_sm)),
+                    static_cast<unsigned>(n));
+    if (n == 1) rows_to_bf16_kernel<1, 512><<<grid, 512, 0, stream>>>(Bf16Jobs<1>{a.job[0]});
+    else rows_to_bf16_kernel<kBf16RowsJobs, 128><<<grid, 128, 0, stream>>>(a);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -572,92 +505,9 @@ int dot_score_bwd(const float* cand, const float* user, const float* dlogits, in
 }
 
 // ------------------------------------------------------------------------------------------------
-// Precise user encoder (NRMS precise mode): operand and attention kernels that keep the history-level path at fp32 accuracy.
+// Precise user encoder (NRMS precise mode): the kernels that keep the history-level path at fp32 accuracy.
 // The level is 4.6 % of the model's FLOPs (512 users x 50 news vectors), so plain CUDA-core arithmetic is affordable.
 // ------------------------------------------------------------------------------------------------
-// fp32 rows [n_seq][T][D] (element strides) -> bf16 [rows][2*ld]: columns [0, D) = hi = bf16(x), column D = 1.0, zeros up to
-// ld; columns [ld, ld + D) = lo = bf16(x - hi), zeros up to 2*ld.  Against the K-concatenated weight operand [W | W] the GEMM
-// computes (hi + lo) . W^T: the input enters with ~16 mantissa bits instead of 8.  pos: as in rows_to_bf16 (the hi plane stays
-// bitwise what rows_to_bf16 writes for the same src and pos).
-__global__ void __launch_bounds__(256) rows_to_bf16_hilo_kernel(const float* __restrict__ src, long long n_rows, int T, int D,
-                                                                long long s_seq, long long s_tok, long long s_col,
-                                                                __nv_bfloat16* __restrict__ dst, int ld, const float* __restrict__ pos) {
-    const int chunks = (2 * ld) >> 3;
-    const long long total = n_rows * chunks;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const long long r = i / chunks;
-        const int c = static_cast<int>(i - r * chunks) * 8;
-        const bool lo = c >= ld;
-        const int col = lo ? c - ld : c;
-        const long long seq = r / T;
-        const long long tok = r - seq * T;
-        const float* sp = src + seq * s_seq + tok * s_tok;
-        float v[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int cc = col + j;
-            float x = cc < D ? sp[cc * s_col] : 0.f;
-            if (pos != nullptr && cc < D) x += pos[tok * D + cc];
-            const float hi = bf16_round(x);
-            v[j] = lo ? (x - hi) : (cc == D ? 1.0f : hi);
-        }
-        *reinterpret_cast<uint4*>(dst + r * (2 * ld) + c) =
-            make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-    }
-}
-int rows_to_bf16_hilo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst,
-                      int ld, cudaStream_t stream, const float* pos) {
-    const long long n = n_seq * T;
-    if (n == 0) return 0;
-    NR_REQUIRE(ld >= D + 1 && ld % 8 == 0, "rows_to_bf16_hilo: pitch %d for D=%d plus the ones column", ld, D);
-    ProfScope ps("rows_to_bf16_hilo", static_cast<int>(n), D, ld, stream);
-    const int blocks = static_cast<int>(std::min<long long>((n * (2 * ld / 8) + 255) / 256, 148 * 8));
-    rows_to_bf16_hilo_kernel<<<blocks, 256, 0, stream>>>(src, n, T, D, s_seq, s_tok, s_col, static_cast<__nv_bfloat16*>(dst), ld,
-                                                         pos);
-    ++g_launches;
-    NR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// fp32 rows [n][D] (element strides) -> two bf16 planes of pitch ld in one pass: hi = bf16(x) with the ones column at D, lo =
-// bf16(x - hi) with zeros from D on.  The hi/lo input of an additive attention (the pooled sum reads both planes).
-__global__ void __launch_bounds__(256) rows_to_bf16_planes_kernel(const float* __restrict__ src, long long n_rows, int D,
-                                                                  long long s_row, long long s_col, __nv_bfloat16* __restrict__ hi_out,
-                                                                  __nv_bfloat16* __restrict__ lo_out, int ld) {
-    const int chunks = ld >> 3;
-    const long long total = n_rows * chunks;
-    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += gridDim.x * 256ll) {
-        const long long r = i / chunks;
-        const int col = static_cast<int>(i - r * chunks) * 8;
-        const float* sp = src + r * s_row;
-        float h[8], l[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float x = col + j < D ? sp[(col + j) * s_col] : 0.f;
-            const float hi = bf16_round(x);
-            h[j] = col + j == D ? 1.0f : hi;
-            l[j] = x - hi;
-        }
-        *reinterpret_cast<uint4*>(hi_out + r * ld + col) =
-            make_uint4(pack_bf16x2(h[0], h[1]), pack_bf16x2(h[2], h[3]), pack_bf16x2(h[4], h[5]), pack_bf16x2(h[6], h[7]));
-        *reinterpret_cast<uint4*>(lo_out + r * ld + col) =
-            make_uint4(pack_bf16x2(l[0], l[1]), pack_bf16x2(l[2], l[3]), pack_bf16x2(l[4], l[5]), pack_bf16x2(l[6], l[7]));
-    }
-}
-int rows_to_bf16_planes(const float* src, long long n, int D, long long s_row, long long s_col, void* hi, void* lo, int ld,
-                        cudaStream_t stream) {
-    if (n == 0) return 0;
-    NR_REQUIRE(ld >= D + 1 && ld % 8 == 0, "rows_to_bf16_planes: pitch %d for D=%d plus the ones column", ld, D);
-    ProfScope ps("rows_to_bf16_planes", static_cast<int>(n), D, ld, stream);
-    const int blocks = static_cast<int>(std::min<long long>((n * (ld / 8) + 255) / 256, 148 * 8));
-    rows_to_bf16_planes_kernel<<<blocks, 256, 0, stream>>>(src, n, D, s_row, s_col, static_cast<__nv_bfloat16*>(hi),
-                                                           static_cast<__nv_bfloat16*>(lo), ld);
-    ++g_launches;
-    NR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
 // dst[e] += sum_s src[s * L + e] for e < L, s < n_seq (the gradient of a per-position addend shared by every sequence).  A CTA owns
 // 32 consecutive e; warp w sums the sequences s = w (mod 8) in increasing order, the eight partials are added in warp order: the
 // result is the same bits on every run (no atomics).
@@ -690,41 +540,6 @@ int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cud
     NR_REQUIRE(L > 0 && (L + 31) / 32 < (1ll << 31), "sum_over_seq: L=%lld", L);
     ProfScope ps("sum_over_seq", static_cast<int>(n_seq), static_cast<int>(std::min<long long>(L, 1 << 30)), 0, stream);
     sum_over_seq_kernel<<<static_cast<unsigned>((L + 31) / 32), 32 * kSeqSumWarps, 0, stream>>>(src, n_seq, L, dst);
-    ++g_launches;
-    NR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// the low plane alone: dst bf16 [rows][ld], columns [0, D) = bf16(x - bf16(x)), zeros up to ld (no ones column: the bias
-// belongs to the hi pass).  Operand of the second pass of a two-pass hi/lo product (gru.cu).
-__global__ void __launch_bounds__(256) rows_to_bf16_lo_kernel(const float* __restrict__ src, long long n_rows, int T, int D,
-                                                              long long s_seq, long long s_tok, long long s_col,
-                                                              __nv_bfloat16* __restrict__ dst, int ld) {
-    const int chunks = ld >> 3;
-    const long long total = n_rows * chunks;
-    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += gridDim.x * 256ll) {
-        const long long r = i / chunks;
-        const int col = static_cast<int>(i - r * chunks) * 8;
-        const long long seq = r / T;
-        const float* sp = src + seq * s_seq + (r - seq * T) * s_tok;
-        float v[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float x = col + j < D ? sp[(col + j) * s_col] : 0.f;
-            v[j] = x - bf16_round(x);
-        }
-        *reinterpret_cast<uint4*>(dst + r * ld + col) =
-            make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-    }
-}
-int rows_to_bf16_lo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst, int ld,
-                    cudaStream_t stream) {
-    const long long n = n_seq * T;
-    if (n == 0) return 0;
-    NR_REQUIRE(ld >= D && ld % 8 == 0, "rows_to_bf16_lo: pitch %d for D=%d", ld, D);
-    ProfScope ps("rows_to_bf16_lo", static_cast<int>(n), D, ld, stream);
-    const int blocks = static_cast<int>(std::min<long long>((n * (ld / 8) + 255) / 256, 148 * 8));
-    rows_to_bf16_lo_kernel<<<blocks, 256, 0, stream>>>(src, n, T, D, s_seq, s_tok, s_col, static_cast<__nv_bfloat16*>(dst), ld);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -123,20 +123,27 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
     const long long BH = static_cast<long long>(B) * Hd;
     prof_context("gru.fwd");
     // gi = X Wih^T + bih over all (user, step) rows
-    NR_PROPAGATE(rows_to_bf16(a->x, B, S, D, a->x_s_b, a->x_s_t, a->x_s_c, a->xb, ldd, st));
+    const Bf16Rows x_rows{.src = a->x, .n_rows = static_cast<long long>(B) * S, .T = S, .D = D, .s_seq = a->x_s_b, .s_tok = a->x_s_t,
+                          .s_col = a->x_s_c, .width = ldd};
+    Bf16Rows x_hi = x_rows;
+    x_hi.hi = a->xb, x_hi.ld_hi = ldd, x_hi.ones_col = 1;
+    NR_PROPAGATE(rows_to_bf16(x_hi, kRowsToBf16, st));
     NR_PROPAGATE(gemm_store({.A = a->xb, .M = B * S, .lda = ldd, .W = a->wih_bf16, .N = 3 * Hd, .ldw = ldd, .K = D},
                             {.out = a->gi, .ld_out = ldg, .bias = a->bih}, st));
     if (a->x_lo_bf16 != nullptr) {
         // accurate mode: the news vectors enter as a hi/lo bf16 pair, gi = x_hi . W_ih^T + b + x_lo . W_ih^T.  Two passes over the
         // SAME resident weights with fp32 accumulation into gi: a K-concatenated single pass doubles K, which shrinks the weight-
         // stationary slices to N = 80 and costs 0.86 ms instead of 2 x 0.23
-        NR_PROPAGATE(rows_to_bf16_lo(a->x, B, S, D, a->x_s_b, a->x_s_t, a->x_s_c, a->x_lo_bf16, ldd, st));
+        Bf16Rows x_lo = x_rows;  // no ones column: the bias belongs to the hi pass
+        x_lo.lo = a->x_lo_bf16, x_lo.ld_lo = ldd;
+        NR_PROPAGATE(rows_to_bf16(x_lo, kRowsToBf16Lo, st));
         NR_PROPAGATE(gemm_store({.A = a->x_lo_bf16, .M = B * S, .lda = ldd, .W = a->wih_bf16, .N = 3 * Hd, .ldw = ldd, .K = D},
                                 {.out = a->gi, .ld_out = ldg, .accumulate = 1}, st));
     }
     // h_0
     NR_CHECK_CUDA(cudaMemcpyAsync(a->hs, a->h0, sizeof(float) * BH, cudaMemcpyDeviceToDevice, st));
-    NR_PROPAGATE(rows_to_bf16(a->h0, B, 1, Hd, Hd, 0, 1, a->hb, ldh, st));
+    NR_PROPAGATE(rows_to_bf16({.src = a->h0, .n_rows = B, .D = Hd, .s_seq = Hd, .width = ldh, .hi = a->hb, .ld_hi = ldh, .ones_col = 1},
+                              kRowsToBf16, st));
     static const bool no_persist = getenv("NEWSREC_GRU_STEPWISE") != nullptr;  // tests compare the two paths
     if (!no_persist && gru_persistent_supported(B, Hd)) {
         // one cooperative launch for the whole recurrence (gru_persist.cu); same saved state as the per-step sequence below

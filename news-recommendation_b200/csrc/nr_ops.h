@@ -89,18 +89,37 @@ int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int
                      int x_row_shift = 0);
 
 // ---- memory-bound companions (aux.cu) --------------------------------------------------------------
-// fp32 [R x C] (pitch lds) -> bf16 [R x ld] zero padded; transpose: out[c][r] = in[r][c] (out is [C x ld])
-int cast_pad_bf16(const float* src, int R, int C, int lds, void* dst, int ld, int transpose, cudaStream_t stream);
-// up to 8 such casts in one launch
-int cast_pad_bf16_many(int n, const float* const* src, const int* R, const int* C, const int* lds, void* const* dst, const int* ld,
-                       const int* transpose, cudaStream_t stream);
-// fp32 rows [n_seq][T][D] with element strides -> bf16 [n_seq*T x ld], ones column at D, zeros after.
-// pos (fp32 [T][D] contiguous, may be null): the rows converted are x + pos[t], summed in fp32 before the rounding
-int rows_to_bf16(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col,
-                 void* dst, int ld, cudaStream_t stream, const float* pos = nullptr);
-// fp32 rows [n][D] -> hi = bf16(x) (ones column at D) and lo = bf16(x - hi) (zeros from D on), both [n x ld], one pass
-int rows_to_bf16_planes(const float* src, long long n, int D, long long s_row, long long s_col, void* hi, void* lo, int ld,
-                        cudaStream_t stream);
+// fp32 rows -> zero-padded bf16 planes: every operand cast, dense-input conversion and hi/lo split in front of a GEMM.
+// Row r = seq * T + tok (r < n_rows), column col < D: x = src[seq * s_seq + tok * s_tok + col * s_col] (element strides), plus
+// pos[tok][col] when pos is set (fp32 [T][D] contiguous; the sum is formed in fp32 before the one rounding).  Columns [D, width)
+// hold 0, except column D of the hi plane when ones_col (1.0: the bias of the next GEMM).  Each plane takes `width` columns
+// (a multiple of 8, fewer than 2^33 columns in all the rows of a job) of 16-byte aligned rows of pitch ld_hi / ld_lo (multiples
+// of 8); either plane may be null:
+//   hi = bf16(x)          lo = bf16(x - bf16(x))   (hi + lo carries x to ~16 mantissa bits)
+// The transpose of an fp32 [R][C] matrix is the job n_rows = C, D = R, s_seq = 1, s_col = its pitch.
+struct Bf16Rows {
+    const float* src;
+    long long n_rows;
+    int T = 1, D;
+    long long s_seq, s_tok = 0, s_col = 1;
+    const float* pos = nullptr;
+    int width;
+    void* hi = nullptr;
+    int ld_hi = 0, ones_col = 0;
+    void* lo = nullptr;
+    int ld_lo = 0;
+};
+// Profiler key and grid cap (148 * blocks_per_sm blocks per job) of a conversion launch, one per kind of caller
+struct Bf16Op {
+    const char* name;
+    int blocks_per_sm;
+};
+inline constexpr Bf16Op kCastPad{"cast_pad", 16}, kCastPadMany{"cast_pad_many", 4}, kRowsToBf16{"rows_to_bf16", 6},
+    kRowsToBf16Hilo{"rows_to_bf16_hilo", 8}, kRowsToBf16Planes{"rows_to_bf16_planes", 8}, kRowsToBf16Lo{"rows_to_bf16_lo", 8};
+// up to kBf16RowsJobs jobs in ONE launch; jobs without rows or columns are skipped, no launch when none is left
+constexpr int kBf16RowsJobs = 8;
+int rows_to_bf16(const Bf16Rows* jobs, int n_jobs, Bf16Op op, cudaStream_t stream);
+inline int rows_to_bf16(const Bf16Rows& job, Bf16Op op, cudaStream_t stream) { return rows_to_bf16(&job, 1, op, stream); }
 // dst[e] += sum_s src[s*L + e] (e < L, s < n_seq): fixed summation order, bit-identical across runs
 int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cudaStream_t stream);
 // X[row(seg,t)] = table_bf16[ids[seg*T+t]] (bit-exact copy), ones column at D, optional dropout, optional padded layout
@@ -141,11 +160,7 @@ int gru_persistent_supported(int B, int Hd);
 int gru_fwd_persistent(int B, int S, int Hd, int ldh, int ldg, const float* gi, const void* whh, const float* bhh, const float* h0,
                        const long long* len, float* gh, float* hs, void* hb, float* out, cudaStream_t stream);
 
-// precise user encoder (NRMS precise mode): hi/lo K-concatenated operand rows, fp32 attention with hi/lo context planes
-int rows_to_bf16_lo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst, int ld,
-                    cudaStream_t stream);
-int rows_to_bf16_hilo(const float* src, long long n_seq, int T, int D, long long s_seq, long long s_tok, long long s_col, void* dst,
-                      int ld, cudaStream_t stream, const float* pos = nullptr);
+// precise user encoder (NRMS precise mode): fp32 attention with hi/lo context planes
 int mhsa_f32_fwd(const float* qkv, int ld, int sec, long long n_seq, int T, int heads, int dk, void* c_hi, void* c_lo, int ldc,
                  cudaStream_t stream);
 // scores[i] = news[cand[i]] . user[s] for seg_offsets[s] <= i < seg_offsets[s+1]  (batched evaluate.py:245-265)

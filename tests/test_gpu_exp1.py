@@ -137,7 +137,7 @@ def _dense_forward_planes(x, pos, accurate):
     a.dense = _p(x)
     a.dense_s_seq, a.dense_s_tok, a.dense_s_col = x.stride()
     a.wqkv_bf16, a.bqkv, a.wa_bf16, a.ba, a.qv = _p(ops["wqkv"]), _p(ops["bqkv"]), _p(ops["wa"]), _p(ops["ba"]), _p(ops["qv"])
-    X = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=DEV)
+    X = torch.full((n_tok, ldx), 7.0, dtype=torch.bfloat16, device=DEV)  # sentinel: every element must be written
     Cx = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=DEV)
     w = torch.empty((n_tok,), dtype=torch.float32, device=DEV)
     out = torch.empty((n_seq, d), dtype=torch.float32, device=DEV)
@@ -145,7 +145,7 @@ def _dense_forward_planes(x, pos, accurate):
     kcat = None
     if accurate:
         wk = cast_pad(torch.cat((torch.nn.functional.pad(stack_qkv(*prm[0:6:2]), (0, ldx - d)),) * 2, dim=1), 2 * ldx)
-        kcat = torch.empty((n_tok, 2 * ldx), dtype=torch.bfloat16, device=DEV)
+        kcat = torch.full((n_tok, 2 * ldx), 7.0, dtype=torch.bfloat16, device=DEV)
         qf = torch.empty((n_tok, 3 * sec), dtype=torch.float32, device=DEV)
         clo = torch.empty((n_tok, ldx), dtype=torch.bfloat16, device=DEV)
         keep += [wk, qf, clo]
