@@ -152,7 +152,7 @@ typedef struct {
     long long n_seq;          /* titles (news) or users                                             */
     int T;                    /* tokens per title / history length                                  */
     int d;                    /* model width (word_embedding_dim)                                   */
-    int heads;                /* num_attention_heads, d % heads == 0                                */
+    int heads;                /* num_attention_heads, d % heads == 0, head size 2 <= d/heads <= 32 (else -1 before any launch) */
     int q;                    /* query_vector_dim                                                   */
     int ldx;                  /* pitch of X / C / weight operands: multiple of 8, >= d+1            */
     int ld3;                  /* pitch of Q|K|V rows: round_up(3*sec, 16), sec = round_up(d, 8): sections at columns 0, sec, 2*sec;
@@ -164,8 +164,8 @@ typedef struct {
     const float* dense;       /* fp32 [n_seq][T][d] with element strides below, or NULL             */
     long long dense_s_seq, dense_s_tok, dense_s_col;
     /* parameters as prepared operands */
-    const void* wqkv_bf16;    /* [3d][ldx]  rows = W_Q | W_K | W_V                                  */
-    const float* bqkv;        /* [3d]                                                               */
+    const void* wqkv_bf16;    /* [3*sec][ldx]  rows = W_Q | 0 | W_K | 0 | W_V | 0 (zero rows at the section padding) */
+    const float* bqkv;        /* [3*sec]       b_Q | 0 | b_K | 0 | b_V | 0                                         */
     const void* wa_bf16;      /* [q][ldx]                                                           */
     const float* ba;          /* [q]                                                                */
     const float* qv;          /* [q]                                                                */
@@ -183,7 +183,7 @@ typedef struct {
     /* precise DENSE variant (user encoder of the precise mode; selected by dense != NULL and C_lo_bf16 != NULL): the fp32
      * input enters the projection as a hi/lo bf16 pair against K-concatenated weights, Q|K|V stays fp32, the attention runs
      * in fp32 on the CUDA cores, the context leaves as hi (C_bf16) + lo (C_lo_bf16) planes.  QKV_bf16 must be NULL. */
-    const void* wqkv_kcat_bf16;  /* [3d][2*ldx]: columns [0,d) = W, [ldx, ldx+d) = W again, zeros elsewhere            */
+    const void* wqkv_kcat_bf16;  /* [3*sec][2*ldx]: rows as wqkv_bf16; columns [0,d) = W, [ldx, ldx+d) = W again, zeros elsewhere */
     void* X_kcat_bf16;           /* [n_seq*T][2*ldx] workspace: hi | lo operand rows                                   */
     float* QKV_f32;              /* [n_seq*T][3*sec] workspace                                                           */
     /* accurate NEWS variant on the unfused kernels (selected by ids != NULL and V_lo_bf16 != NULL; needs C_lo_bf16 and
@@ -215,7 +215,8 @@ typedef struct {
     const float* w;
     const float* dout;                   /* [n_seq][d] fp32                                              */
     /* gradients */
-    float* dWqkv_ext;                    /* [3d][ldx] (+=)  column d = d(bias)                           */
+    float* dWqkv_ext;                    /* [3*sec][ldx] (+=)  sectioned rows as wqkv_bf16, column d = d(bias); the padding
+                                            rows receive exact zeros                                      */
     float* dWa_ext;                      /* [q][ldx]  (+=)  column d = d(bias)                           */
     float* dqv;                          /* [q] (+=)                                                     */
     float* demb;                         /* [V][d] (+=) embedding gradient (ids variant)                 */
@@ -223,8 +224,8 @@ typedef struct {
     void* workspace;
     long long workspace_bytes;
     /* QKV_bf16 == NULL (the precise dense forward keeps no bf16 Q|K|V): recomputed here from X_bf16 with these operands */
-    const void* wqkv_bf16;               /* [3d][ldx]                                                    */
-    const float* bqkv;                   /* [3d]                                                         */
+    const void* wqkv_bf16;               /* [3*sec][ldx] (sectioned, as in the forward arguments)        */
+    const float* bqkv;                   /* [3*sec]                                                      */
     /* optional cudaEvent_t recorded on `stream` as soon as demb is complete (before the weight-gradient GEMM): a data-
      * parallel caller starts the embedding-gradient all-reduce on a side stream that waits for it */
     void* emb_grad_ready_event;

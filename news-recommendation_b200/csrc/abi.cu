@@ -184,19 +184,28 @@ int nr_pack_slots(const void* const* slots, int n_clicked, int n_candidates, int
 // every head of every section) has the same 16-byte phase, which the title-level attention kernels rely on.  The packed
 // projection operands carry zero rows / columns at the section padding, so the padding columns of Q|K|V are exact zeros.
 static int qkv_section(int d) { return (d + 7) & ~7; }
+// Every attention kernel of both directions (title-level, head-level, fp32) covers head sizes 2 <= d_k <= 32: a shape outside
+// that range is rejected here, before the gather / row conversion and the projection GEMM have written anything.
 static int check_mhsa_shape(long long n_seq, int T, int d, int heads, int q, int ldx, int ld3) {
     NR_REQUIRE(n_seq >= 0 && T >= 1 && T <= 64 && d >= 8 && heads >= 1 && d % heads == 0 && q >= 1 && q <= 256,
                "mhsa encoder: bad shape n_seq=%lld T=%d d=%d heads=%d q=%d", n_seq, T, d, heads, q);
+    NR_REQUIRE(d / heads >= 2 && d / heads <= 32, "mhsa encoder: head size d_k=%d (d=%d, heads=%d) not in [2, 32]", d / heads, d,
+               heads);
     NR_REQUIRE(ldx % 8 == 0 && ldx >= d + 1 && ld3 % 8 == 0 && ld3 >= 3 * qkv_section(d), "mhsa encoder: bad pitches ldx=%d ld3=%d",
                ldx, ld3);
     NR_REQUIRE(n_seq * T < (1ll << 31), "mhsa encoder: too many tokens (%lld)", n_seq * T);
     return 0;
 }
 
-int nr_mhsa_accurate_supported(int T, int d, int heads) {
-    if (heads < 1 || d % heads != 0) return 0;
+// the accurate news variant needs the hi/lo title-level attention kernel and a projection GEMM that can emit the low plane of
+// the V section (whole 32-column chunks from column 2*sec: d = 20 and d = 40 have none)
+static bool mhsa_accurate_shape(int T, int d, int heads, int ld3, int ldx) {
+    if (heads < 1 || d % heads != 0) return false;
     const int sec = qkv_section(d);
-    return mhsa_title_fwd_supported(T, d / heads, heads, sec, (3 * sec + 15) & ~15, (d + 8) & ~7) ? 1 : 0;
+    return mhsa_title_fwd_supported(T, d / heads, heads, sec, ld3, ldx) && gemm_store_lo_supported(3 * sec, d, 2 * sec);
+}
+int nr_mhsa_accurate_supported(int T, int d, int heads) {
+    return mhsa_accurate_shape(T, d, heads, (3 * qkv_section(d) + 15) & ~15, (d + 8) & ~7) ? 1 : 0;
 }
 
 // the dense input rows [n_seq][T][d] (+ dense_pos) with the ones column at d, as the hi plane of pitch ld_hi
@@ -245,8 +254,9 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         // probabilities in registers and writes both context planes, the pooled sum reads both)
         NR_REQUIRE(a->C_lo_bf16 != nullptr && a->table_bf16 && a->bad_id_flag && a->V >= 1,
                    "nr_mhsa_encoder_fwd: the accurate variant needs C_lo_bf16 (+ table / bad_id_flag)");
-        NR_REQUIRE(mhsa_title_fwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx),
-                   "nr_mhsa_encoder_fwd: the accurate variant needs the title-level attention kernel (T=20, d_k=20, <=15 heads); see nr_mhsa_accurate_supported");
+        NR_REQUIRE(mhsa_accurate_shape(a->T, a->d, a->heads, a->ld3, a->ldx),
+                   "nr_mhsa_encoder_fwd: the accurate variant needs the title-level attention kernel (T=20, d_k=20, <=15 heads) and a "
+                   "chunk-aligned V section (d=%d); see nr_mhsa_accurate_supported", a->d);
         NR_PROPAGATE(gather_rows(a->ids, M, a->T, a->table_bf16, a->V, a->d, a->ldx, a->X_bf16, a->ldx, 0,
                                  DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
         NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},

@@ -532,6 +532,20 @@ static Dropout to_drop(const DropoutCfg& c) {
     return d;
 }
 
+// the chunk path of EpiStore emits the low plane by whole 32-column chunks of a weight slice: no chunk may straddle lo_col0
+static bool lo_plane_chunk_aligned(const GemmNTParams& p, int lo_col0) {
+    for (int sl = 0; sl < p.n_slices; ++sl) {
+        const int c0 = sl * p.n_stride;
+        if (c0 < lo_col0 && lo_col0 < c0 + p.n_stride && (lo_col0 - c0) % 32 != 0) return false;
+    }
+    return true;
+}
+bool gemm_store_lo_supported(int N, int K, int lo_col0) {
+    GemmNTPlan plan;  // the weight slicing depends on N and K only: plan an empty problem
+    if (plan_gemm_nt(&plan, nullptr, 0, K, nullptr, N, K, K, 1, 0, kTileM, 1, 0, kEpiSmemBytes<EpiStore>, 0) != 0) return false;
+    return lo_col0 >= 0 && lo_col0 < N && lo_plane_chunk_aligned(plan.p, lo_col0);
+}
+
 int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
     if (g.M == 0) return 0;
     const int M = g.M, N = g.N, rows_per_tile = std::min(c.rows_per_tile, kTileM);  // every row is owned by exactly one tile
@@ -550,11 +564,8 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
         const int lo_col0 = c.lo_col0, ld_lo = c.ld_lo;
         NR_REQUIRE(c.out_bf16 && lo_col0 >= 0 && lo_col0 < N && ld_lo % 8 == 0 && ld_lo >= N - lo_col0 && (e.use_tma || lo_col0 % 8 == 0),
                    "gemm_store: the low plane needs bf16 output and aligned columns (N=%d lo_col0=%d ld_lo=%d)", N, lo_col0, ld_lo);
-        for (int sl = 0; sl < plan.p.n_slices; ++sl) {  // a 32-column chunk never straddles the first low-plane column
-            const int c0 = sl * plan.p.n_stride;
-            NR_REQUIRE(!(c0 < lo_col0 && lo_col0 < c0 + plan.p.n_stride) || (lo_col0 - c0) % 32 == 0,
-                       "gemm_store: low-plane start %d is not chunk aligned in the slice at column %d", lo_col0, c0);
-        }
+        NR_REQUIRE(lo_plane_chunk_aligned(plan.p, lo_col0), "gemm_store: low-plane start %d is not chunk aligned in its weight slice (N=%d)",
+                   lo_col0, N);
         if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_lo, c.lo_out, M, N - lo_col0, ld_lo, 32, 16, 64));
         e.lo_col0 = lo_col0;
         e.lo_out = static_cast<__nv_bfloat16*>(c.lo_out);

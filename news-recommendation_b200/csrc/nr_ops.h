@@ -42,6 +42,8 @@ struct StoreCfg {
     int rows_per_tile = kGemmTileRows;  // rows are computed independently: larger values are clamped to the tile
 };
 int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream);
+// whether gemm_store can emit the low plane of the columns [lo_col0, N) of an N x K product (host-only, no launch)
+bool gemm_store_lo_supported(int N, int K, int lo_col0);
 
 // additive-attention pooling: out[seg][D] = sum_r softmax_seg(tanh(X Wa^T + ba) . qv)_r X_r ; w_out[rows]
 // X_lo (may be null): a second bf16 plane with X = X_hi + X_lo; the scores use X_hi, the pooled sum both planes.

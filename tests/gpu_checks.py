@@ -192,19 +192,26 @@ def check_mhsa_core(n_seq=7, T=20, heads=15, dk=20, sectioned=False):
             "bwd_rel": relerr(got, bf16r(qkv.grad)), "pad_zero": bool((pads == 0).all())}
 
 
-def check_additive(N=37, S=20, D=300, q=200):
+def check_additive(N=37, S=20, D=300, q=200, precision="fast"):
+    """precision "accurate": fp32 rows that are not bf16 values enter as hi/lo planes (nr_additive_attention_fwd_hilo, as
+    NAML's view fusion and Exp1's final attention run it).  The forward is compared with the oracle's hi/lo contract (scores
+    on the hi plane, the pooled sum on the fp32 rows); the backward reads the hi plane in both modes, so its gradients are
+    compared with the bf16 contract's gradients at the hi plane bf16(x)."""
     from newsrec_b200.ops import AdditiveAttentionFn, OperandCache
-    x = _rand_bf16((N, S, D), 31).requires_grad_(True)
+    accurate = precision == "accurate"
+    xf = O.det_uniform((N, S, D), 31) if accurate else _rand_bf16((N, S, D), 31)
+    x = bf16r(xf).requires_grad_(True)  # the leaf of the gradient reference: the plane the backward reads
     p = {"a.linear.weight": O.det_uniform((q, D), 32, -0.1, 0.1).requires_grad_(True),
          "a.linear.bias": O.det_uniform((q,), 33, -0.05, 0.05).requires_grad_(True),
          "a.attention_query_vector": O.det_uniform((q,), 34, -0.1, 0.1).requires_grad_(True)}
-    ref = O.additive_attention(x, p, "a", O.BF16)
     g = O.det_uniform((N, D), 35)
-    ref.backward(g)
-    xd = x.detach().to(DEV).requires_grad_(True)
+    O.additive_attention(x, p, "a", O.BF16).backward(g)
+    with torch.no_grad():
+        ref = O.additive_attention(xf, p, "a", O.BF16_FUSED if accurate else O.BF16)
+    xd = xf.to(DEV).requires_grad_(True)
     pd = {k: v.detach().to(DEV).requires_grad_(True) for k, v in p.items()}
     out = AdditiveAttentionFn.apply(xd, pd["a.linear.weight"], pd["a.linear.bias"], pd["a.attention_query_vector"],
-                                    OperandCache(), "t")
+                                    OperandCache(), "t", precision)
     out.backward(g.to(DEV))
     torch.cuda.synchronize()
     return {"fwd_rel": relerr(out, ref), "dx_rel": relerr(xd.grad, x.grad),
@@ -1320,4 +1327,424 @@ def check_embedding_f32(n=512 * 55, V=300, D=100, seed=7):
     res["untouched_rows_exact"] = dt.unchanged((~touched).view(V, 1).expand(V, D))
     res["row0_untouched"] = not bool(touched[0])
     res["guards_intact"] = all(b.guard_ok() for b in (out, flag, dt))
+    return res
+
+
+# ------------------------------------------------------------------------------------------------
+# The NRMS / Exp1 self-attention encoder (nr_mhsa_encoder_fwd / _bwd): the same treatment as the CNN encoder above, stage by
+# stage, for the four forward variants and their backward.  The fp64 backward chain is a plain function of tensors so that
+# tests/test_mhsa_encoder_host.py can check it against torch.autograd through the oracle on the CPU.
+# ------------------------------------------------------------------------------------------------
+def _bf16_round(t):
+    return t.to(torch.bfloat16).to(t.dtype)
+
+
+def mhsa_attention_probs(Q, K, heads):
+    """A = exp(S) / (sum_j exp(S) + 1e-8) with S = Q_h K_h^T / sqrt(d_k) per head (multihead_self.py:15-23), in its
+    max-subtracted form, in the inputs' dtype: Q, K (n, T, d) -> (n, heads, T, T)."""
+    n, T, d = Q.shape
+    dk = d // heads
+    sp = lambda t: t.reshape(n, T, heads, dk).transpose(1, 2)
+    S = sp(Q) @ sp(K).transpose(-1, -2) / math.sqrt(dk)
+    m = S.amax(-1, keepdim=True)
+    e = torch.exp(S - m)
+    return e / (e.sum(-1, keepdim=True) + 1e-8 * torch.exp(-m))
+
+
+def mhsa_pool_bwd_chain(X, Q, K, V, C, w, W3, Wa, ba, qv, dout, heads, ctx_mask=None, contract=False, dpre=None):
+    """The backward of one self-attention + additive-pooling encoder written out stage by stage, in the inputs' dtype, from
+    the forward values the kernels stored: X (n, T, d) the projection's input rows, Q, K, V (n, T, d), C (n, T, d) the
+    context the pooling read, w (n, T), W3 (3, d, d) = W_Q | W_K | W_V, Wa (q, d), ba, qv (q,), dout (n, d) and ctx_mask
+    (n, T, d) the context-dropout multipliers (None: no dropout).  contract=True rounds to bf16 where the kernels store bf16:
+    dPre, dC, dS (the gradient w.r.t. the unscaled product Q K^T, as oracle.scaled_dot_product_attention does), A as the
+    operand of dV, and dQ | dK | dV.  dpre (n T, q), if given, is used as the stored dPre instead (the kernels' own, which a
+    separate element bound judges).  Returns dqv (q,), dWa_ext (q, d + 1), dW3_ext (3, d, d + 1) (column d: the bias) and
+    dX (n, T, d), the gradient of the projection's input rows."""
+    r = _bf16_round if contract else (lambda t: t)
+    n, T, d = X.shape
+    dk = d // heads
+    one = torch.ones(n * T, 1, dtype=X.dtype, device=X.device)
+    C2 = C.reshape(n * T, d)
+    # additive pooling (additive.py:35-53): dscore -> dPre -> dqv, dWa_ext; dC = (dPre Wa + w dout) * context mask
+    dw = (C * dout.unsqueeze(1)).sum(2)
+    dscore = w * (dw - (w * dw).sum(1, keepdim=True))
+    th = torch.tanh(C2 @ Wa.t() + ba)
+    if dpre is None:
+        dpre = r(dscore.reshape(-1, 1) * qv * (1 - th * th))
+    dqv = (dscore.reshape(-1, 1) * th).sum(0)
+    dWa = dpre.t() @ torch.cat([C2, one], 1)
+    dC = dpre @ Wa + w.reshape(-1, 1) * dout.repeat_interleave(T, 0)
+    if ctx_mask is not None:
+        dC = dC * ctx_mask.reshape(n * T, d)
+    dC = r(dC)
+    # attention: A recomputed; dV = A^T dC, dA = dC V^T, dS = A (dA - sum A dA) / sqrt(d_k), dQ = dS K, dK = dS^T Q
+    sp = lambda t: t.reshape(n, T, heads, dk).transpose(1, 2)
+    mg = lambda t: t.transpose(1, 2).reshape(n * T, d)
+    A = mhsa_attention_probs(Q, K, heads)
+    G = sp(dC)
+    dV = r(A).transpose(-1, -2) @ G
+    dA = G @ sp(V).transpose(-1, -2)
+    dS = r(A * (dA - (A * dA).sum(-1, keepdim=True)) / math.sqrt(dk))
+    dQKV = [r(mg(t)) for t in (dS @ sp(K), dS.transpose(-1, -2) @ sp(Q), dV)]
+    # projection (multihead_self.py:53-58): dX = dQ|dK|dV . W_Q|W_K|W_V, dW_ext = dQKV^T [X, 1]
+    X1 = torch.cat([X.reshape(n * T, d), one], 1)
+    dX = dQKV[0] @ W3[0] + dQKV[1] @ W3[1] + dQKV[2] @ W3[2]
+    return dict(dqv=dqv, dWa=dWa, dW3=torch.stack([g.t() @ X1 for g in dQKV]), dX=dX.view(n, T, d))
+
+
+def check_mhsa_encoder(n_seq=37, T=20, d=300, heads=15, q=200, V=500, p_drop=0.2, level="ids", mode="accurate", pos=False,
+                       noncontig=False, seed=1, bad_ids=True, discriminate=False, grad_floor=2e-3):
+    """nr_mhsa_encoder_fwd / _bwd stage by stage against fp64 references built from the kernels' own stored X, Q|K|V, C, w.
+    level "ids" (news encoder: masked gather, context dropout, embedding scatter) or "dense" (user encoder: fp32 rows
+    [+ pos], input and positional gradient); mode "fast" or "accurate" (ids: V / probabilities / context as hi/lo pairs;
+    dense: the precise variant, fp32 Q|K|V and attention, hi/lo context).  Every "=" output starts as NaN, every "+=" output
+    with a small pattern, the workspace with 0xFF; every buffer, the packed operands included, is followed by a guard, and
+    the packed Q|K|V operands and dWqkv_ext are sized 3*sec rows (include/newsrec_b200.h).  Bounds: tests/test_gpu_mhsa_encoder.py."""
+    from newsrec_b200 import MhsaEncoderBwdArgs, MhsaEncoderFwdArgs
+    from newsrec_b200.ops import qkv_pitches, stack_qkv
+    lib = load_library()
+    ids_level = level == "ids"
+    accurate = mode == "accurate"
+    precise = accurate and not ids_level
+    ldx, ldq = ru8(d + 1), ru16(q)
+    sec, ld3 = qkv_pitches(d)
+    n_tok = n_seq * T
+    p_ctx = p_drop if ids_level else 0.0  # the dense (user-level) variant has no dropout
+    # ---- operands, built the way ops.mhsa_operands / MhsaPoolEncoderFn do; Q, K entries of about unit size
+    a_w = 3.0 / math.sqrt(d)
+    Wqkv = [_rand_bf16((d, d), seed + 1 + i, a_w).to(DEV) for i in range(3)]
+    bqkv_l = [O.det_uniform((d,), seed + 4 + i, -0.1, 0.1).to(DEV) for i in range(3)]
+    Wa = _rand_bf16((q, d), seed + 7, math.sqrt(3.0 / d)).to(DEV)
+    ba = O.det_uniform((q,), seed + 8, -0.1, 0.1).to(DEV)
+    qv = O.det_uniform((q,), seed + 9, -1.0, 1.0).to(DEV)
+    wqkv_f = stack_qkv(*Wqkv)
+    G_ = lambda t: _Guarded(t.numel(), t.dtype, t)  # a read-only operand followed by its guard
+    ops = dict(wqkv=G_(cast_pad(wqkv_f, ldx)), wqkvT=G_(cast_pad(wqkv_f, ld3, transpose=True)), bqkv=G_(stack_qkv(*bqkv_l)),
+               wa=G_(cast_pad(Wa, ldx)), waT=G_(cast_pad(Wa, ldq, transpose=True)), ba=G_(ba), qv=G_(qv))
+    assert ops["wqkv"].n == 3 * sec * ldx and ops["bqkv"].n == 3 * sec
+    if precise:
+        kc = torch.nn.functional.pad(wqkv_f, (0, ldx - d))
+        ops["kcat"] = G_(cast_pad(torch.cat((kc, kc), 1), 2 * ldx))
+    ids = table_f = dense = posv = None
+    if ids_level:
+        table_f = _rand_bf16((V, d), seed + 10).to(DEV)
+        ops["table"] = G_(cast_pad(table_f, ldx))
+        ids = _cnn_ids(n_seq, T, V, seed + 11, bad_ids)
+    else:
+        base = O.det_uniform((T, max(n_seq, 1), d), seed + 12).to(DEV)
+        dense = base.transpose(0, 1) if noncontig else base.transpose(0, 1).contiguous()  # (n, T, d)
+        if pos:
+            posv = O.det_uniform((T, d), seed + 13, -0.1, 0.1).to(DEV)
+    kseed = (0x9E3779B97F4A7C15 * (seed + 17)) & 0xFFFFFFFFFFFFFFFF
+
+    def forward():
+        nan = float("nan")
+        fb = dict(X=_Guarded(n_tok * ldx, torch.bfloat16, nan), C=_Guarded(n_tok * ldx, torch.bfloat16, nan),
+                  w=_Guarded(n_tok, torch.float32, nan), out=_Guarded(n_seq * d, torch.float32, nan),
+                  flag=_Guarded(1, torch.int32, 0, sentinel=-7))
+        if not precise:
+            fb["QKV"] = _Guarded(n_tok * ld3, torch.bfloat16, nan)
+        if accurate:
+            fb["Clo"] = _Guarded(n_tok * ldx, torch.bfloat16, nan)
+        if accurate and ids_level:
+            fb["Vlo"] = _Guarded(n_tok * sec, torch.bfloat16, nan)
+        if precise:
+            fb["Xk"] = _Guarded(n_tok * 2 * ldx, torch.bfloat16, nan)
+            fb["Q32"] = _Guarded(n_tok * 3 * sec, torch.float32, nan)
+        a = MhsaEncoderFwdArgs()
+        a.n_seq, a.T, a.d, a.heads, a.q, a.ldx, a.ld3 = n_seq, T, d, heads, q, ldx, ld3
+        if ids_level:
+            a.ids, a.table_bf16, a.V = _p(ids), _p(ops["table"].all), V
+        else:
+            a.dense = _p(dense)
+            a.dense_s_seq, a.dense_s_tok, a.dense_s_col = dense.stride()
+            a.dense_pos = _p(posv)
+        a.wqkv_bf16, a.bqkv, a.wa_bf16 = _p(ops["wqkv"].all), _p(ops["bqkv"].all), _p(ops["wa"].all)
+        a.ba, a.qv = _p(ops["ba"].all), _p(ops["qv"].all)
+        a.p_drop, a.seed = float(p_drop), kseed
+        a.X_bf16, a.C_bf16, a.w, a.out = _p(fb["X"].all), _p(fb["C"].all), _p(fb["w"].all), _p(fb["out"].all)
+        a.QKV_bf16 = _p(fb["QKV"].all) if "QKV" in fb else None
+        a.bad_id_flag = _p(fb["flag"].all)
+        if accurate:
+            a.C_lo_bf16 = _p(fb["Clo"].all)
+        if "Vlo" in fb:
+            a.V_lo_bf16 = _p(fb["Vlo"].all)
+        if precise:
+            a.wqkv_kcat_bf16, a.X_kcat_bf16, a.QKV_f32 = _p(ops["kcat"].all), _p(fb["Xk"].all), _p(fb["Q32"].all)
+        n0 = int(lib.nr_launch_count())
+        rc = lib.nr_mhsa_encoder_fwd(C.byref(a), _stream())
+        launches = int(lib.nr_launch_count()) - n0
+        if rc != 0:  # a refused shape: what the library said and how much it launched before saying it
+            return None, {"fwd_rejected": lib.nr_last_error().decode(), "fwd_launches": launches}
+        return fb, launches
+
+    fb, fwd_launches = forward()
+    if fb is None:
+        return fwd_launches
+    dout = O.det_uniform((max(n_seq, 1), d), seed + 14).to(DEV)
+    pat = lambda n, s: O.det_uniform((n,), s, 0.5, 1.0).to(DEV) * 2.0 ** -16  # small non-zero "+=" pre-fill
+    bb = dict(dW3=_Guarded(3 * sec * ldx, torch.float32, pat(3 * sec * ldx, seed + 20)),
+              dWa=_Guarded(q * ldx, torch.float32, pat(q * ldx, seed + 21)), dqv=_Guarded(q, torch.float32, pat(q, seed + 22)))
+    if ids_level:
+        bb["demb"] = _Guarded(V * d, torch.float32, pat(V * d, seed + 23))
+    else:
+        bb["ddense"] = _Guarded(n_tok * d, torch.float32, float("nan"))
+        if pos:
+            bb["dpos"] = _Guarded(T * d, torch.float32, pat(T * d, seed + 24))
+    ws_bytes = int(lib.nr_mhsa_encoder_bwd_workspace(n_seq, T, d, q))
+    ws = _Guarded(ws_bytes, torch.uint8, 0xFF, sentinel=0xA5)  # 0xFFFF.. = NaN in bf16 and fp32: unwritten rows poison results
+    b = MhsaEncoderBwdArgs()
+    b.n_seq, b.T, b.d, b.heads, b.q, b.ldx, b.ld3, b.ldq = n_seq, T, d, heads, q, ldx, ld3, ldq
+    b.ids, b.V = (_p(ids), V) if ids_level else (None, 0)
+    b.wqkvT_bf16, b.wa_bf16, b.waT_bf16 = _p(ops["wqkvT"].all), _p(ops["wa"].all), _p(ops["waT"].all)
+    b.ba, b.qv = _p(ops["ba"].all), _p(ops["qv"].all)
+    b.p_drop, b.seed = float(p_drop), kseed
+    b.X_bf16, b.C_bf16, b.w, b.dout = _p(fb["X"].all), _p(fb["C"].all), _p(fb["w"].all), _p(dout)
+    b.QKV_bf16 = _p(fb["QKV"].all) if "QKV" in fb else None  # precise: recomputed from X inside the backward
+    b.wqkv_bf16, b.bqkv = _p(ops["wqkv"].all), _p(ops["bqkv"].all)
+    b.dWqkv_ext, b.dWa_ext, b.dqv = _p(bb["dW3"].all), _p(bb["dWa"].all), _p(bb["dqv"].all)
+    if ids_level:
+        b.demb = _p(bb["demb"].all)
+    else:
+        b.ddense = _p(bb["ddense"].all)
+        b.dpos = _p(bb["dpos"].all) if pos else None
+    b.workspace, b.workspace_bytes = _p(ws.all), ws_bytes
+    n0 = int(lib.nr_launch_count())
+    check(lib.nr_mhsa_encoder_bwd(C.byref(b), _stream()), "nr_mhsa_encoder_bwd")
+    bwd_launches = int(lib.nr_launch_count()) - n0
+    torch.cuda.synchronize()
+    res = {"fwd_launches": fwd_launches, "bwd_launches": bwd_launches,
+           "guards_intact": all(g.guard_ok() for g in list(fb.values()) + list(bb.values()) + list(ops.values()) + [ws])}
+    # the backward's first two stages as the kernels stored them in the workspace (abi.cu MhsaBwdWorkspace: fp32 dscore
+    # [rows], then bf16 dPre [rows][ldq], each region 256-byte aligned), so that each is judged on its own inputs
+    ds_ws = ws.body[:n_tok * 4].view(torch.float32).clone()
+    off = (n_tok * 4 + 255) // 256 * 256
+    dpre_ws = ws.body[off:off + n_tok * ldq * 2].view(torch.bfloat16).view(n_tok, ldq)[:, :q].clone()
+    del ws
+    if n_seq == 0:
+        return res
+    if ids_level:
+        res["bad_id_flag"] = int(fb["flag"].body.item())
+        ids_flat = ids.reshape(-1)
+        bad = (ids_flat < 0) | (ids_flat >= V)
+        res["bad_ids_planted"] = int(bad.sum())
+        ids_safe = torch.where(bad, torch.zeros_like(ids_flat), ids_flat)
+        scat = (ids_flat >= 1) & (ids_flat < V)
+    res["fwd_outputs_finite"] = all(bool(torch.isfinite(fb[k].body.float()).all()) for k in ("X", "C", "w", "out") + (("Clo",) if accurate else ()))
+
+    # ---- fp64 references, a chunk of sequences at a time (a few hundred MB of fp64 temporaries at any n_seq)
+    X2, C2, w1 = fb["X"].body.view(n_tok, ldx), fb["C"].body.view(n_tok, ldx), fb["w"].body
+    Clo2 = fb["Clo"].body.view(n_tok, ldx) if accurate else None
+    QKV2 = fb["QKV"].body.view(n_tok, ld3) if "QKV" in fb else None
+    Vlo2 = fb["Vlo"].body.view(n_tok, sec) if "Vlo" in fb else None
+    Xk2, Q32 = (fb["Xk"].body.view(n_tok, 2 * ldx), fb["Q32"].body.view(n_tok, 3 * sec)) if precise else (None, None)
+    out2 = fb["out"].body.view(n_seq, d)
+    W3 = torch.stack(Wqkv).double()
+    b3 = torch.stack(bqkv_l).double()
+    Wa64, ba64, qv64 = Wa.double(), ba.double(), qv.double()
+    metrics = ("qkv_ratio", "vlo_ratio", "qkv32_ratio", "ctx_ratio", "ctx_hi_only_ratio", "ctx_no_vlo_ratio", "w_err", "w_sum_err",
+               "out_ratio", "dscore_ratio", "dpre_ratio")
+    acc = {k: 0.0 for k in metrics}
+    worst = lambda k, t: acc.__setitem__(k, max(acc[k], _worst(t)))
+    cnt = dict(x_mismatch_rows=0, xk_mismatch_rows=0, ctx_dropped_nonzero=0)
+    exact_flags = dict(qkv_pad_zero=True, ctx_ones_col=True, ctx_pitch_zero=True)
+    variants = ("exact", "contract") + (("exact_no_ctx_mask", "contract_no_ctx_mask") if discriminate else ())
+    grads = {v: dict(dW3=torch.zeros(3, d, d + 1, dtype=torch.float64, device=DEV),
+                     dWa=torch.zeros(q, d + 1, dtype=torch.float64, device=DEV),
+                     dqv=torch.zeros(q, dtype=torch.float64, device=DEV)) for v in variants}
+    for v in variants:
+        if ids_level:
+            grads[v]["demb"] = torch.zeros(V, d, dtype=torch.float64, device=DEV)
+        else:
+            grads[v]["ddense"] = torch.zeros(n_tok, d, dtype=torch.float64, device=DEV)
+    if discriminate and ids_level:
+        grads["exact_no_gather_mask"] = dict(demb=torch.zeros(V, d, dtype=torch.float64, device=DEV))
+        grads["contract_no_gather_mask"] = dict(demb=torch.zeros(V, d, dtype=torch.float64, device=DEV))
+    cs = max(1, min(40960 // T, (1 << 24) // (heads * T * T)))
+    for s0 in range(0, n_seq, cs):
+        s1 = min(n_seq, s0 + cs)
+        ns, r0, r1 = s1 - s0, s0 * T, s1 * T
+        rows = torch.arange(r0, r1, device=DEV)
+        # X: bit exact (masked gather or fp32 dense [+ pos] rounded once), ones column at d, zeros up to ldx
+        if ids_level:
+            mx = dropout_mask_dev(kseed, p_drop, rows, d, ldx)
+            src = table_f[ids_safe[r0:r1]] * mx
+        else:
+            src = (dense[s0:s1] + posv if pos else dense[s0:s1]).reshape(-1, d)
+        exp_x = torch.zeros(r1 - r0, ldx, dtype=torch.float32, device=DEV)
+        exp_x[:, :d] = src
+        exp_x[:, d] = 1.0
+        exp_hi = exp_x.to(torch.bfloat16)
+        cnt["x_mismatch_rows"] += int((X2[r0:r1].view(torch.int16) != exp_hi.view(torch.int16)).any(dim=1).sum())
+        X64 = X2[r0:r1, :d].double()
+        if precise:  # X_kcat = [hi | lo] of the same fp32 rows, as nr_rows_to_bf16_hilo writes them
+            exp_lo = torch.zeros_like(exp_hi)
+            exp_lo[:, :d] = (src - src.to(torch.bfloat16).float()).to(torch.bfloat16)
+            exp_k = torch.cat([exp_hi, exp_lo], 1)
+            cnt["xk_mismatch_rows"] += int((Xk2[r0:r1].view(torch.int16) != exp_k.view(torch.int16)).any(dim=1).sum())
+            Xin = Xk2[r0:r1, :d].double() + Xk2[r0:r1, ldx:ldx + d].double()
+        else:
+            Xin = X64
+        # Q|K|V against fp64 Xin . W^T + b, with the sum of |products| for the fp32 accumulation allowance
+        ref = torch.stack([Xin @ W3[i].t() + b3[i] for i in range(3)])  # (3, rows, d)
+        absum = torch.stack([Xin.abs() @ W3[i].abs().t() + b3[i].abs() for i in range(3)])
+        if precise:
+            got = torch.stack([Q32[r0:r1, i * sec:i * sec + d].double() for i in range(3)])
+            worst("qkv32_ratio", _safe_div((got - ref).abs(), 1e-6 * absum))
+            exact_flags["qkv_pad_zero"] &= all(bool((Q32[r0:r1, i * sec + d:(i + 1) * sec] == 0).all()) for i in range(3))
+            Qa, Ka, Va = got[0], got[1], got[2]
+        else:
+            got = torch.stack([QKV2[r0:r1, i * sec:i * sec + d].double() for i in range(3)])
+            worst("qkv_ratio", _safe_div((got - ref).abs(), _bf16_ulp(torch.maximum(got.abs(), ref.abs())) + 1e-6 * absum))
+            exact_flags["qkv_pad_zero"] &= all(bool((QKV2[r0:r1, i * sec + d:(i + 1) * sec] == 0).all()) for i in range(3))
+            Qa, Ka, Va = got[0], got[1], got[2]
+            if Vlo2 is not None:
+                Va = got[2] + Vlo2[r0:r1, :d].double()
+                rb = 2.0 ** -16 * ref[2].norm(dim=1) + 1e-6 * absum[2].norm(dim=1)
+                worst("vlo_ratio", _safe_div((Va - ref[2]).norm(dim=1), rb))
+                exact_flags["qkv_pad_zero"] &= bool((Vlo2[r0:r1, d:] == 0).all())
+        del ref, absum
+        # context against fp64 mask * (A V), A from the stored Q, K
+        sh = lambda t: t.reshape(ns, T, d)
+        A = mhsa_attention_probs(sh(Qa), sh(Ka), heads)
+        spv = lambda t: sh(t).reshape(ns, T, heads, d // heads).transpose(1, 2)
+        mg = lambda t: t.transpose(1, 2).reshape(ns * T, d)
+        AV, AabsV = mg(A @ spv(Va)), mg(A @ spv(Va.abs()))
+        cm = dropout_mask_dev(kseed ^ 0x5BD1E995, p_ctx, rows, d, ldx).double()
+        ref_c = AV * cm
+        chi = C2[r0:r1, :d].double()
+        if accurate:
+            clo = Clo2[r0:r1, :d].double()
+            bound = 2.0 ** -15 * AabsV * cm + 2.0 ** -16 * ref_c.abs()
+            worst("ctx_ratio", _safe_div((chi + clo - ref_c).abs(), bound))
+            worst("ctx_hi_only_ratio", _safe_div((chi - ref_c).abs(), bound))
+            if Vlo2 is not None:  # a reference that leaves out V_lo: the kernel's pair must be far from it
+                ref_nv = mg(A @ spv(got[2])) * cm
+                worst("ctx_no_vlo_ratio", _safe_div((chi + clo - ref_nv).abs(), 2.0 ** -15 * AabsV * cm + 2.0 ** -16 * ref_nv.abs()))
+            cnt["ctx_dropped_nonzero"] += int(((cm == 0) & ((chi != 0) | (clo != 0))).sum())
+            exact_flags["ctx_ones_col"] &= bool((C2[r0:r1, d] == 1).all()) and bool((Clo2[r0:r1, d] == 0).all())
+            exact_flags["ctx_pitch_zero"] &= bool((C2[r0:r1, d + 1:] == 0).all()) and bool((Clo2[r0:r1, d + 1:] == 0).all())
+        else:
+            ulps = _bf16_ulp(torch.maximum(chi.abs(), ref_c.abs())) * torch.where(cm > 1, 2.0, 1.0)
+            bound = (2.0 ** -8 + 2.0 ** -15) * AabsV * cm + ulps
+            rt = _safe_div((chi - ref_c).abs(), bound)
+            if _worst(rt) > acc["ctx_ratio"]:
+                i = int(torch.nan_to_num(rt, nan=float("inf")).argmax())
+                res["ctx_worst"] = [float(t.reshape(-1)[i]) for t in (chi, ref_c, AabsV, cm, ulps)] + [r0 + i // d, i % d]
+            worst("ctx_ratio", rt)
+            cnt["ctx_dropped_nonzero"] += int(((cm == 0) & (chi != 0)).sum())
+            exact_flags["ctx_ones_col"] &= bool((C2[r0:r1, d] == 1).all())
+            exact_flags["ctx_pitch_zero"] &= bool((C2[r0:r1, d + 1:] == 0).all())
+        del A, AV, AabsV, ref_c
+        # pooling from the kernel's own C_hi (scores) and C_hi [+ C_lo] (pooled sum)
+        score = torch.tanh(chi @ Wa64.t() + ba64) @ qv64
+        w_ref = torch.softmax(score.view(ns, T), dim=1)
+        wk = w1[r0:r1].double().view(ns, T)
+        worst("w_err", (wk - w_ref).abs())
+        worst("w_sum_err", (wk.sum(1) - 1).abs())
+        cc = (chi + clo if accurate else chi).view(ns, T, d)
+        o_ref, o_abs = (wk.unsqueeze(2) * cc).sum(1), (wk.unsqueeze(2) * cc.abs()).sum(1)
+        worst("out_ratio", _safe_div((out2[s0:s1].double() - o_ref).norm(dim=1), o_abs.norm(dim=1)))
+        # ---- backward, exact and under the bf16 contract, from the stored X, Q|K|V (the fp64 projection of the stored X where
+        #      the backward recomputes it), C_hi and w; the contract takes the kernels' stored dPre (judged above), so the
+        #      per-row rule measures the stages after it
+        do = dout[s0:s1].double()
+        # dscore = w (dw - sum w dw), dw = C_hi . dout: fp32 dot products of d terms (d 2^-24 sum |c||dout| each) and a few
+        # fp32 operations on w (dw, sum w dw)
+        cd = chi.view(ns, T, d) * do.unsqueeze(1)
+        dw, aw = cd.sum(2), cd.abs().sum(2)
+        ds_ref = wk * (dw - (wk * dw).sum(1, keepdim=True))
+        ds_bound = wk * (d * 2.0 ** -24 * (aw + (wk * aw).sum(1, keepdim=True)) + 4 * 2.0 ** -24 * (dw.abs() + (wk * dw.abs()).sum(1, keepdim=True)))
+        ds_k = ds_ws[r0:r1].double().view(ns, T)
+        worst("dscore_ratio", _safe_div((ds_k - ds_ref).abs(), ds_bound))
+        # dPre = dscore qv (1 - T^2) from the kernel's own dscore, T = tanh(C_hi Wa^T + ba): tanh.approx.f32 is within
+        # 2^-10.987 of T relatively (PTX ISA), the fp32 pre-activation within 1e-6 sum |c||wa| (+|ba|), which moves T by
+        # (1 - T^2) times that; 1 - T^2 then moves by up to 2|T| |dT| + dT^2; plus one bf16 ulp of the stored result
+        pre = chi @ Wa64.t() + ba64
+        th = torch.tanh(pre)
+        dT = th.abs() * 2.0 ** -10.987 + (1 - th * th) * 1e-6 * (chi.abs() @ Wa64.abs().t() + ba64.abs())
+        g1 = ds_k.reshape(-1, 1) * qv64
+        dp_ref = g1 * (1 - th * th)
+        dp_k = dpre_ws[r0:r1].double()
+        dp_bound = g1.abs() * (2 * th.abs() * dT + dT * dT + 4 * 2.0 ** -24) + _bf16_ulp(torch.maximum(dp_ref.abs(), dp_k.abs()))
+        worst("dpre_ratio", _safe_div((dp_k - dp_ref).abs(), dp_bound))
+        del cd, pre, th, dT, g1, dp_ref
+        if precise:
+            proj = torch.stack([X64 @ W3[i].t() + b3[i] for i in range(3)])
+        for v in variants:
+            contract = v.startswith("contract")
+            if precise:  # the backward recomputes Q|K|V from X_bf16 into a bf16 workspace
+                qkv_in = [_bf16_round(t) if contract else t for t in proj]
+            else:
+                qkv_in = [got[0], got[1], got[2]]
+            ch = mhsa_pool_bwd_chain(sh(X64), *[sh(t) for t in qkv_in], sh(chi), wk, W3, Wa64, ba64, qv64, do, heads,
+                                     ctx_mask=None if v.endswith("no_ctx_mask") else sh(cm), contract=contract,
+                                     dpre=dp_k if contract else None)
+            g = grads[v]
+            g["dqv"] += ch["dqv"]
+            g["dWa"] += ch["dWa"]
+            g["dW3"] += ch["dW3"]
+            dX = ch["dX"].reshape(-1, d)
+            if ids_level:
+                sc = scat[r0:r1]
+                g["demb"].index_add_(0, ids_flat[r0:r1][sc], (dX * mx.double())[sc])
+                if discriminate and not v.endswith("no_ctx_mask"):
+                    grads[v.split("_")[0] + "_no_gather_mask"]["demb"].index_add_(0, ids_flat[r0:r1][sc], dX[sc])
+            else:
+                g["ddense"][r0:r1] = dX
+            del ch, dX
+    res.update(acc)
+    res.update(cnt)
+    res.update(exact_flags)
+    # ---- gradients: per row, kernel error against exact next to the bf16 contract's error
+    ex, co = grads["exact"], grads["contract"]
+    body = lambda k: bb[k].body.double() - (bb[k].prefill.double() if bb[k].prefill is not None else 0.0)
+    dW3_k = body("dW3").view(3, sec, ldx)[:, :d, :d + 1]
+    dWa_k = body("dWa").view(q, ldx)[:, :d + 1]
+    dqv_k = body("dqv")
+    rr = lambda kern, e, c: _row_ratio(kern, e, c, floor=grad_floor)
+    # T = 1: A = 1 / (1 + 1e-8), so dS = A (dA - A dA) / sqrt(d_k) is 1e-8 of dA -- below fp32 resolution, the kernels' dQ, dK
+    # are 0 -- and the Q, K rows of dWqkv_ext are 1e-8 of the V rows: they are held to that scale, the V rows to the rule
+    s3 = slice(2, 3) if T == 1 else slice(0, 3)
+    n3 = (s3.stop - s3.start) * d
+    res["dWqkv_row_ratio"], res["dWqkv_ek"], res["dWqkv_ec"] = rr(dW3_k[s3].reshape(n3, -1), ex["dW3"][s3].reshape(n3, -1),
+                                                                  co["dW3"][s3].reshape(n3, -1))
+    if T == 1:
+        res["t1_dWqk_rel"] = _worst(dW3_k[:2].abs()) / max(_worst(ex["dW3"][2].abs()), 1e-300)
+    res["dWa_row_ratio"], res["dWa_ek"], res["dWa_ec"] = rr(dWa_k, ex["dWa"], co["dWa"])
+    res["dqv_ratio"], res["dqv_ek"], res["dqv_ec"] = rr(dqv_k.view(1, -1), ex["dqv"].view(1, -1), co["dqv"].view(1, -1))
+    if discriminate:
+        res["dWqkv_ratio_without_ctx_mask"] = rr(dW3_k.reshape(3 * d, -1), grads["exact_no_ctx_mask"]["dW3"].reshape(3 * d, -1),
+                                                 grads["contract_no_ctx_mask"]["dW3"].reshape(3 * d, -1))[0]
+    # the pre-fill outside what the kernels own: section-padding rows and pitch columns of dWqkv_ext, pitch columns of dWa_ext
+    m3 = torch.ones(3, sec, ldx, dtype=torch.bool, device=DEV)
+    m3[:, :d, :d + 1] = False
+    res["dWqkv_padding_untouched"] = bb["dW3"].unchanged(m3)
+    ma = torch.zeros(q, ldx, dtype=torch.bool, device=DEV)
+    ma[:, d + 1:] = True
+    res["dWa_pitch_cols_untouched"] = bb["dWa"].unchanged(ma)
+    if ids_level:
+        touched = torch.zeros(V, dtype=torch.bool, device=DEV)
+        touched[ids_flat[scat]] = True
+        res["demb_rows_touched"] = int(touched.sum())
+        demb_k = body("demb").view(V, d)
+        res["demb_row_ratio"], res["demb_ek"], res["demb_ec"] = rr(demb_k[touched], ex["demb"][touched], co["demb"][touched])
+        res["demb_untouched_rows_exact"] = bb["demb"].unchanged((~touched).view(V, 1).expand(V, d))
+        res["demb_row0_untouched"] = bb["demb"].unchanged(torch.arange(V, device=DEV).view(V, 1).expand(V, d) == 0)
+        if discriminate:
+            res["demb_ratio_without_gather_mask"] = rr(demb_k[touched], grads["exact_no_gather_mask"]["demb"][touched],
+                                                       grads["contract_no_gather_mask"]["demb"][touched])[0]
+    else:
+        dd_k = bb["ddense"].body.double().view(n_tok, d)
+        res["ddense_row_ratio"], res["ddense_ek"], res["ddense_ec"] = rr(dd_k, ex["ddense"], co["ddense"])
+        if pos:  # dpos = sum over the sequences of ddense
+            sum_seq = lambda t: t.view(n_seq, T, d).sum(0)
+            res["dpos_row_ratio"], res["dpos_ek"], res["dpos_ec"] = rr(body("dpos").view(T, d), sum_seq(ex["ddense"]),
+                                                                       sum_seq(co["ddense"]))
+    del grads, ex, co, bb
+
+    # ---- determinism: a second forward is bit-identical (run last, when the references are freed)
+    fb2, _ = forward()
+    torch.cuda.synchronize()
+    res["fwd_deterministic"] = all(_bits_equal(fb[k].body, fb2[k].body) for k in fb if k != "flag")
     return res

@@ -83,7 +83,9 @@ def test_attention_core(kw):
 
 
 @pytest.mark.parametrize("kw", [dict(), dict(N=9, S=50), dict(N=50, S=4, D=400), dict(N=1, S=20), dict(N=13, S=32, D=296),
-                                dict(N=700, S=20, q=64)])
+                                dict(N=700, S=20, q=64),
+                                # hi/lo input planes (NAML view fusion, Exp1 final attention): news-level and history-level lengths
+                                dict(S=20, precision="accurate"), dict(N=9, S=50, precision="accurate")])
 def test_additive_attention(kw):
     r = G.check_additive(**kw)
     assert r["fwd_rel"] < 1e-5, r
