@@ -7,6 +7,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #define NR_OWNS_WATCHDOG 1
@@ -328,51 +329,71 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint64_t* full = bars;
     uint64_t* empty = bars + kMaxStages;
 
-    const int mt = blockIdx.x % p.m_tiles;
-    const int rest = blockIdx.x / p.m_tiles;
-    const int nt = rest % p.n_tiles;
-    const int ks = rest / p.n_tiles;
+    const int mt = blockIdx.x, nt = blockIdx.y, ks = blockIdx.z;  // a cluster spans (m-tile, n-tile) pairs of one k-range
     const int total_chunks = (p.Kr + 63) >> 6;
     const int chunk0 = ks * p.chunks_per_slice;
     const int n_my = max(0, min(p.chunks_per_slice, total_chunks - chunk0));
     const int n0 = nt * NT;                       // first output column of this CTA
     const int ncol = min(NT, p.Nb - n0);
+    // cluster rank cx + cluster_m * cy; the A chunk of this m-tile goes to the ranks of column cx, the B chunk of this n-tile to
+    // those of row cy.  Every CTA issues its share of both by multicast, so a stage may be refilled only once the consumers of
+    // all those ranks have released it: the empty barriers count the warps of the row and the column.
+    const bool clustered = p.cluster_m * p.cluster_n > 1;
+    const int cx = mt % p.cluster_m, cy = nt % p.cluster_n;
+    uint32_t a_mask = 0, b_mask = 0;
+    for (int j = 0; j < p.cluster_n; ++j) a_mask |= 1u << (cx + p.cluster_m * j);
+    for (int i = 0; i < p.cluster_m; ++i) b_mask |= 1u << (i + p.cluster_m * cy);
 
     if (warp == kEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 8);
+            mbar_init(&empty[i], 8 * (p.cluster_m + p.cluster_n - 1));
         }
         fence_barrier_init();
     }
-    __syncthreads();
-    if (n_my == 0) return;
+    if (clustered) cluster_sync();  // the partners' barriers exist before the first multicast or remote arrive
+    else __syncthreads();
+    if (n_my == 0) return;  // the whole cluster: its CTAs share the k-range
 
     if (warp >= kEpiWarps) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
-        if (warp != kEpiWarps) return;
+        if (!clustered && warp != kEpiWarps) return;
+    }
+    if (warp == kEpiWarps) {
         // producer loop is warp-uniform, one elected lane issues
         int st = 0;
         uint32_t ph = 0;
         for (int c = 0; c < n_my; ++c) {
             const int k0 = (chunk0 + c) * 64;
-            mbar_wait(&empty[st], ph ^ 1, 201);
+            mbar_wait(&empty[st], ph ^ 1, clustered ? 203 : 201);
             if (elect_one()) {
                 mbar_arrive_expect_tx(&full[st], static_cast<uint32_t>(stage_bytes));
                 uint8_t* sa = smem + st * stage_bytes;
                 uint8_t* sb = sa + 2 * 8192;
-                tma_load_2d(sa, &tmA, &full[st], mt * 128, k0);
-                tma_load_2d(sa + 8192, &tmA, &full[st], mt * 128 + 64, k0);
+                if (!clustered) {
+                    tma_load_2d(sa, &tmA, &full[st], mt * 128, k0);
+                    tma_load_2d(sa + 8192, &tmA, &full[st], mt * 128 + 64, k0);
 #pragma unroll
-                for (int j = 0; j < kBoxes; ++j)
-                    tma_load_2d(sb + j * 8192, &tmB, &full[st], p.b_col0 + n0 + j * 64, k0 + p.b_row_shift);
+                    for (int j = 0; j < kBoxes; ++j)
+                        tma_load_2d(sb + j * 8192, &tmB, &full[st], p.b_col0 + n0 + j * 64, k0 + p.b_row_shift);
+                } else {  // box b of the A chunk from rank (cx, b % cluster_n), box j of the B chunk from rank (j % cluster_m, cy)
+#pragma unroll
+                    for (int b = 0; b < 2; ++b)
+                        if (b % p.cluster_n == cy)
+                            tma_load_2d_multicast(sa + b * 8192, &tmA, &full[st], mt * 128 + 64 * b, k0, static_cast<uint16_t>(a_mask));
+#pragma unroll
+                    for (int j = 0; j < kBoxes; ++j)
+                        if (j % p.cluster_m == cx)
+                            tma_load_2d_multicast(sb + j * 8192, &tmB, &full[st], p.b_col0 + n0 + j * 64, k0 + p.b_row_shift,
+                                                  static_cast<uint16_t>(b_mask));
+                }
             }
             __syncwarp();
             if (++st == p.stages) { st = 0; ph ^= 1; }
         }
-    } else {
+    } else if (warp < kEpiWarps) {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
         const int h = warp >> 2;
         float acc[NT / 2];
@@ -397,7 +418,13 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int i = 0; i < NT / 2; ++i) wgmma_reg_fence(acc[i]);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[st]);
+            if (lane == 0) {
+                if (!clustered) {
+                    mbar_arrive(&empty[st]);
+                } else {
+                    for (uint32_t m = a_mask | b_mask; m != 0; m &= m - 1) mbar_arrive_cluster(&empty[st], __ffs(m) - 1);
+                }
+            }
             if (++st == p.stages) { st = 0; ph ^= 1; }
         }
         // fragment: acc[4j + 2e + i] = row 16 * (warp % 4) + lane / 4 + 8e, column 8j + 2 * (lane % 4) + i
@@ -420,6 +447,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         }
     }
+    // no CTA leaves while a partner may still arrive on its barriers or multicast into its ring (the idle producer warps stay)
+    if (clustered) cluster_sync();
 }
 
 #ifdef NEWSREC_TRIAGE
@@ -445,16 +474,59 @@ __global__ void gemm_tn_simt_kernel(const __nv_bfloat16* A, int lda, const __nv_
 static int g_comm_reserved_sms = 0;
 void set_comm_reserved_sms(int n) { g_comm_reserved_sms = n < 0 ? 0 : n; }
 
+int max_active_clusters(const void* func, int threads, size_t smem, int cluster_x, int cluster_y) {
+    static std::map<std::tuple<const void*, int, size_t, int, int>, int> cache;
+    const auto key = std::make_tuple(func, threads, smem, cluster_x, cluster_y);
+    const auto it = cache.find(key);
+    if (it != cache.end()) return it->second;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = cluster_x;
+    attr[0].val.clusterDim.y = cluster_y;
+    attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3(cluster_x, cluster_y);
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, func, &cfg) != cudaSuccess) n = 0;
+    cache[key] = n;
+    return n;
+}
+
+// Splits the reduction over k-ranges so that the grid fills the GPU once (with clusters: as many as fit at once), then launches.
 template <int NT>
-static int launch_gemm_tn_kernel(dim3 grid, size_t smem, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmTNParams& p,
+static int launch_gemm_tn_kernel(int sms, int total_chunks, size_t smem, const CUtensorMap& tmA, const CUtensorMap& tmB, GemmTNParams p,
                                  cudaStream_t stream) {
     static bool attr_set = false;  // per instantiation
     if (!attr_set) {
         NR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tn_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
         attr_set = true;
     }
-    gemm_tn_kernel<NT><<<grid, kTnThreads, smem, stream>>>(tmA, tmB, p);
-    NR_CHECK_CUDA(cudaGetLastError());
+    const int tiles = p.m_tiles * p.n_tiles, csize = p.cluster_m * p.cluster_n;
+    int k_slices = std::max(1, std::min(sms / tiles, total_chunks));
+    if (csize > 1) {
+        const int fit = max_active_clusters(reinterpret_cast<const void*>(gemm_tn_kernel<NT>), kTnThreads, smem, p.cluster_m, p.cluster_n);
+        NR_REQUIRE(fit >= 1, "gemm_tn: no %d x %d cluster with %zu bytes of shared memory fits", p.cluster_m, p.cluster_n, smem);
+        k_slices = std::max(1, std::min(k_slices, fit / (tiles / csize)));
+    }
+    p.chunks_per_slice = ceil_div(total_chunks, k_slices);
+    p.k_slices = ceil_div(total_chunks, p.chunks_per_slice);
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = p.cluster_m;
+    attr[0].val.clusterDim.y = p.cluster_n;
+    attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3(p.m_tiles, p.n_tiles, p.k_slices);
+    cfg.blockDim = dim3(kTnThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = csize > 1 ? 1 : 0;
+    NR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tn_kernel<NT>, tmA, tmB, p));
     return 0;
 }
 
@@ -489,10 +561,9 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     p.n_tiles = ceil_div(Nb, 256);
     const int nt_cols = round_up(ceil_div(Nb, p.n_tiles), 64);
     const int total_chunks = ceil_div(Kr, 64);
-    int k_slices = std::max(1, std::min(sms / (p.m_tiles * p.n_tiles), total_chunks));
-    p.chunks_per_slice = ceil_div(total_chunks, k_slices);
-    k_slices = ceil_div(total_chunks, p.chunks_per_slice);
-    p.k_slices = k_slices;
+    // a cluster of 2 along each tile dimension that divides: the two CTAs share the chunk of the other operand
+    p.cluster_m = p.m_tiles % 2 == 0 ? 2 : 1;
+    p.cluster_n = p.n_tiles % 2 == 0 ? 2 : 1;
     p.n_boxes = nt_cols / 64;
     const int stage_bytes = (2 + p.n_boxes) * 8192;
     p.stages = std::min(kMaxStages, (kSmemLimit - 1024 - 512) / stage_bytes);
@@ -502,12 +573,11 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     NR_PROPAGATE(make_tmap_bf16_2d(&tmA, A, Kr, Ma, lda, 64, 64));
     NR_PROPAGATE(make_tmap_bf16_2d(&tmB, B, b_rows, b_cols, ldb, 64, 64));
     const size_t smem = static_cast<size_t>(p.stages) * stage_bytes + 1024 + 512;
-    const dim3 grid(p.m_tiles * p.n_tiles * k_slices);
     switch (p.n_boxes) {
-        case 1: NR_PROPAGATE(launch_gemm_tn_kernel<64>(grid, smem, tmA, tmB, p, stream)); break;
-        case 2: NR_PROPAGATE(launch_gemm_tn_kernel<128>(grid, smem, tmA, tmB, p, stream)); break;
-        case 3: NR_PROPAGATE(launch_gemm_tn_kernel<192>(grid, smem, tmA, tmB, p, stream)); break;
-        default: NR_PROPAGATE(launch_gemm_tn_kernel<256>(grid, smem, tmA, tmB, p, stream)); break;
+        case 1: NR_PROPAGATE(launch_gemm_tn_kernel<64>(sms, total_chunks, smem, tmA, tmB, p, stream)); break;
+        case 2: NR_PROPAGATE(launch_gemm_tn_kernel<128>(sms, total_chunks, smem, tmA, tmB, p, stream)); break;
+        case 3: NR_PROPAGATE(launch_gemm_tn_kernel<192>(sms, total_chunks, smem, tmA, tmB, p, stream)); break;
+        default: NR_PROPAGATE(launch_gemm_tn_kernel<256>(sms, total_chunks, smem, tmA, tmB, p, stream)); break;
     }
     ++g_launches;
     return 0;

@@ -152,6 +152,34 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
+// The same box landing at the same shared-memory offset in every CTA of cta_mask (bit r = cluster rank r); each receiver's
+// mbarrier at bar's offset sees the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+        : "memory");
+}
+
+// ---- thread-block clusters ---------------------------------------------------------------------
+// every thread of every CTA of the cluster; release / acquire: shared-memory writes (mbarrier inits included) before it are
+// visible to the partners after it
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at bar's offset in the shared memory of cluster rank `rank` (this CTA's own included).  Release at
+// CTA scope (the default) is what a consumer's "stage read" needs; .release.cluster would first wait for every earlier
+// global write of the thread, the epilogue's reductions and stores included.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    asm volatile(
+        "{\n\t.reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+        ::"r"(smem_u32(bar)), "r"(rank)
+        : "memory");
+}
+
 // TMA store of one box from shared memory (bulk async-group completion)
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(

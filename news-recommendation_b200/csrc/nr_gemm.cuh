@@ -528,6 +528,8 @@ struct GemmTNParams {
     int b_row_shift; // B row = A row + shift (conv taps)
     int m_tiles;
     int n_tiles;     // CTAs along Nb (<= 256 columns each)
+    int cluster_m;   // cluster shape over (m-tile, n-tile): the CTAs of one k-range that share an A chunk (same m-tile) or a
+    int cluster_n;   // B chunk (same n-tile) receive it by one TMA multicast; 1 x 1 = no cluster
     int k_slices;
     int chunks_per_slice;  // 64-row chunks per CTA
     int n_boxes;     // ceil(Nb/64)
@@ -552,6 +554,8 @@ struct GemmNTPlan {
 int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B, int N, int ldb, int K, int taps,
                  int b_tap_rows, int rows_per_tile, int num_sms, int max_slices, int epi_smem_bytes, int max_n_stride);
 bool debug_simt_gemm();
+// Thread-block clusters of cluster_x x cluster_y CTAs of `func` that fit on the device at once (cached per function and shape).
+int max_active_clusters(const void* func, int threads, size_t smem, int cluster_x, int cluster_y);
 
 template <class Epi>
 int launch_gemm_nt(const GemmNTPlan& plan, const Epi& epi, const void* A, int lda, const void* B, int ldb,
