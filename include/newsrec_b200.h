@@ -38,6 +38,9 @@ void nr_debug_set_simt_gemm(int on);
 /* 1 in a triage build (`make TRIAGE=1`), 0 in the release library, where nr_debug_set_simt_gemm is a no-op, the SIMT
  * kernels are not compiled and no environment switch is consulted on a launch path */
 int nr_has_triage_backends(void);
+/* Tests (release library too): on != 0 makes nr_gru_fwd run the per-step sequence even where the persistent recurrence applies,
+ * on == 0 restores the default.  Until the first call it follows NEWSREC_GRU_STEPWISE (set: per-step), read once. */
+void nr_debug_set_gru_stepwise(int on);
 /* TUNING ONLY (tools/kbench.py): dev_buf holds slots x 148 x 16 int64; the k-th gemm_nt planned after this call
  * writes, per CTA, cycle counters into slot k: [0] TMA producer waiting for a free A stage, [1] consumer warpgroups
  * waiting for A data, [4] epilogue body, [5] kernel, [6] tiles.  Null (default) switches the counters off. */
@@ -342,8 +345,8 @@ typedef struct {
 } nr_gru_fwd_args;
 int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream);
 /* 1 if nr_gru_fwd runs the whole recurrence as ONE cooperative launch for this shape on this device (users in 128-row tiles x
- * hidden units in slices of 32, one CTA each, all resident: tiles * slices <= SM count; Hd % 4 == 0, Hd <= 960); else it
- * runs three launches per step */
+ * hidden units in slices of 32, one CTA each, all resident): B >= 1, Hd % 4 == 0, 32 <= Hd <= 1024 (16 resident 64-column
+ * k-chunks of W_hh) and ceil(B / 128) * ceil(Hd / 32) <= SM count; else it runs a GEMM, a copy and a gate kernel per step */
 int nr_gru_persistent_supported(int B, int Hd);
 
 typedef struct {

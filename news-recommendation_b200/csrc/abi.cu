@@ -24,6 +24,7 @@ int nr_device_error(int out4[4]) { return read_device_error(out4); }
 long long nr_launch_count(void) { return g_launches; }
 int nr_num_sms(void) { return num_sms(); }
 void nr_debug_set_simt_gemm(int on) { set_debug_simt_gemm(on); }
+void nr_debug_set_gru_stepwise(int on) { set_gru_stepwise(on); }
 int nr_has_triage_backends(void) { return has_triage_backends(); }
 void nr_reserve_sms_for_comm(int n) { set_comm_reserved_sms(n); }
 void nr_debug_set_gemm_timing(void* dev_buf, int slots) { set_debug_gemm_timing(dev_buf, slots); }

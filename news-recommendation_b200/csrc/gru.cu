@@ -102,6 +102,24 @@ __global__ void zero_pad_cols_kernel(__nv_bfloat16* __restrict__ m, long long ro
     }
 }
 
+// Forward path switch: 1 = per-step sequence even where the persistent kernel applies.  Read lazily from NEWSREC_GRU_STEPWISE
+// (set: 1) on the first forward unless nr_debug_set_gru_stepwise set it before; -1 = not decided yet.
+static int g_gru_stepwise = -1;
+static bool gru_stepwise() {
+    if (g_gru_stepwise < 0) g_gru_stepwise = getenv("NEWSREC_GRU_STEPWISE") != nullptr ? 1 : 0;
+    return g_gru_stepwise == 1;
+}
+void set_gru_stepwise(int on) { g_gru_stepwise = on ? 1 : 0; }
+
+// the shape rules of nr_gru_fwd and nr_gru_bwd; the message names the rule a shape breaks
+static int check_gru_shape(const char* fn, int B, int S, int D, int Hd) {
+    NR_REQUIRE(B >= 0, "%s: B=%d is negative", fn, B);
+    NR_REQUIRE(S >= 1, "%s: S=%d, at least one step is needed", fn, S);
+    NR_REQUIRE(D >= 8 && D % 4 == 0, "%s: D=%d is not a multiple of 4 of at least 8", fn, D);
+    NR_REQUIRE(Hd >= 8 && Hd % 2 == 0, "%s: Hd=%d is not an even number of at least 8", fn, Hd);
+    return 0;
+}
+
 }  // namespace nr
 
 using namespace nr;
@@ -114,7 +132,7 @@ extern "C" {
 int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_gru_fwd: null args");
     const int B = a->B, S = a->S, D = a->D, Hd = a->Hd;
-    NR_REQUIRE(B >= 0 && S >= 1 && D >= 8 && Hd >= 8 && D % 4 == 0 && Hd % 2 == 0, "nr_gru_fwd: bad shape B=%d S=%d D=%d Hd=%d", B, S, D, Hd);
+    NR_PROPAGATE(check_gru_shape("nr_gru_fwd", B, S, D, Hd));
     NR_REQUIRE(a->x && a->len && a->h0 && a->wih_bf16 && a->whh_bf16 && a->bih && a->bhh && a->xb && a->gi && a->gh && a->hs && a->hb && a->out,
                "nr_gru_fwd: null operand");
     if (B == 0) return 0;
@@ -144,8 +162,7 @@ int nr_gru_fwd(const nr_gru_fwd_args* a, void* stream) {
     NR_CHECK_CUDA(cudaMemcpyAsync(a->hs, a->h0, sizeof(float) * BH, cudaMemcpyDeviceToDevice, st));
     NR_PROPAGATE(rows_to_bf16({.src = a->h0, .n_rows = B, .D = Hd, .s_seq = Hd, .width = ldh, .hi = a->hb, .ld_hi = ldh, .ones_col = 1},
                               kRowsToBf16, st));
-    static const bool no_persist = getenv("NEWSREC_GRU_STEPWISE") != nullptr;  // tests compare the two paths
-    if (!no_persist && gru_persistent_supported(B, Hd)) {
+    if (!gru_stepwise() && gru_persistent_supported(B, Hd)) {
         // one cooperative launch for the whole recurrence (gru_persist.cu); same saved state as the per-step sequence below
         return gru_fwd_persistent(B, S, Hd, ldh, ldg, a->gi, a->whh_bf16, a->bhh, a->h0, a->len, a->gh, a->hs, a->hb, a->out, st);
     }
@@ -184,11 +201,12 @@ long long nr_gru_bwd_workspace(int B, int S, int D, int Hd) { return GruBwdWorks
 int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_gru_bwd: null args");
     const int B = a->B, S = a->S, D = a->D, Hd = a->Hd;
-    NR_REQUIRE(B >= 0 && S >= 1 && D % 4 == 0 && Hd % 2 == 0, "nr_gru_bwd: bad shape B=%d S=%d D=%d Hd=%d", B, S, D, Hd);
+    NR_PROPAGATE(check_gru_shape("nr_gru_bwd", B, S, D, Hd));
     NR_REQUIRE(a->len && a->wihT_bf16 && a->whhT_bf16 && a->xb && a->gi && a->gh && a->hs && a->hb && a->dout && a->dWih_ext && a->dWhh_ext &&
                    a->dx && a->dh0 && a->workspace, "nr_gru_bwd: null operand");
     const GruBwdWorkspace ws(a->workspace, B, S, Hd);
-    NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_gru_bwd: workspace too small");
+    NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_gru_bwd: workspace too small: %lld bytes, nr_gru_bwd_workspace gives %lld",
+               a->workspace_bytes, ws.bytes());
     if (B == 0) return 0;
     const cudaStream_t st = as_stream(stream);
     const int ldg = round_up(3 * Hd, 4), ldh = round_up(Hd + 1, 8), ldd = round_up(D + 1, 8), ldb = round_up(3 * Hd + 1, 8);

@@ -157,6 +157,8 @@ __global__ void __launch_bounds__(kThreads, 1) gru_fwd_persistent_kernel(const _
                     h[bb][e][jj][1] = v.y;
                 }
             }
+        // the first wgmma reads the resident W_hh slice: its TMA loads, issued before the first A stage, may land after it
+        f_wait(wfull, 0, 403);
         int st = 0;
         uint32_t ph = 0;
         for (int t = 0; t < p.S; ++t) {

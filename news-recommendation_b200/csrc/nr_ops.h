@@ -161,6 +161,7 @@ int embedding_f32_bwd(const long long* ids, long long n, const float* dout, int 
 int gru_persistent_supported(int B, int Hd);
 int gru_fwd_persistent(int B, int S, int Hd, int ldh, int ldg, const float* gi, const void* whh, const float* bhh, const float* h0,
                        const long long* len, float* gh, float* hs, void* hb, float* out, cudaStream_t stream);
+void set_gru_stepwise(int on);  // nr_debug_set_gru_stepwise (gru.cu)
 
 // precise user encoder (NRMS precise mode): fp32 attention with hi/lo context planes
 int mhsa_f32_fwd(const float* qkv, int ld, int sec, long long n_seq, int T, int heads, int dk, void* c_hi, void* c_lo, int ldc,

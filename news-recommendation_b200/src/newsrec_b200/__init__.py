@@ -102,6 +102,7 @@ SIGNATURES = {
     "nr_launch_count": (_ll, []),
     "nr_num_sms": (_i, []),
     "nr_debug_set_simt_gemm": (None, [_i]),
+    "nr_debug_set_gru_stepwise": (None, [_i]),
     "nr_has_triage_backends": (_i, []),
     "nr_reserve_sms_for_comm": (None, [_i]),
     "nr_debug_set_gemm_timing": (None, [_vp, _i]),

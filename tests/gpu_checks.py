@@ -234,37 +234,6 @@ def check_dot_score(B=9, Cn=5, D=300):
 
 
 # ------------------------------------------------------------------------------------------------
-def check_gru(B=37, S=50, D=900, Hd=900, seed=3):
-    """LSTUR user-encoder GRU (pack_padded_sequence + nn.GRU, last hidden state; LSTUR/user_encoder.py:27-45) at the
-    reference's history length, mixed lengths including 0 (clamped to 1) and S: forward and every gradient against the
-    oracle under the bf16 operand contract.  B <= 128 * floor(SMs / 29) runs the persistent single-launch recurrence."""
-    from newsrec_b200.ops import OperandCache
-    from newsrec_b200.ops_gru import GruLastHiddenFn
-    a = math.sqrt(1.0 / Hd)
-    p = {"g.weight_ih_l0": O.det_uniform((3 * Hd, D), seed, -a, a), "g.weight_hh_l0": O.det_uniform((3 * Hd, Hd), seed + 1, -a, a),
-         "g.bias_ih_l0": O.det_uniform((3 * Hd,), seed + 2, -a, a), "g.bias_hh_l0": O.det_uniform((3 * Hd,), seed + 3, -a, a)}
-    p = {k: v.requires_grad_(True) for k, v in p.items()}
-    x = _rand_bf16((B, S, D), seed + 4, 0.5).requires_grad_(True)
-    h0 = O.det_uniform((B, Hd), seed + 5, -0.5, 0.5).requires_grad_(True)
-    lengths = O.det_randint((B,), seed + 6, 0, S + 1)
-    lengths[0], lengths[1 % B] = 0, S
-    ref = O.gru_last_hidden(x, lengths.clamp(min=1), h0, p, "g", O.BF16)
-    gout = O.det_uniform((B, Hd), seed + 7)
-    ref.backward(gout)
-    xd, hd = x.detach().to(DEV).requires_grad_(True), h0.detach().to(DEV).requires_grad_(True)
-    pd = {k: v.detach().to(DEV).requires_grad_(True) for k, v in p.items()}
-    out = GruLastHiddenFn.apply(xd, lengths.to(DEV), hd, pd["g.weight_ih_l0"], pd["g.weight_hh_l0"], pd["g.bias_ih_l0"],
-                                pd["g.bias_hh_l0"], OperandCache(), "gru")
-    out.backward(gout.to(DEV))
-    torch.cuda.synchronize()
-    res = {"fwd_rel": relerr(out, ref), "dx_rel": relerr(xd.grad, x.grad), "dh0_rel": relerr(hd.grad, h0.grad),
-           "persistent": bool(load_library().nr_gru_persistent_supported(B, Hd))}
-    for k in p:
-        res["d" + k.split(".")[1]] = relerr(pd[k].grad, p[k].grad)
-    return res
-
-
-# ------------------------------------------------------------------------------------------------
 def nrms_model_and_params(V, seed, heads=15, dropout=0.2, fused=False):
     import config as cfgmod
     from model.NRMS import NRMS
@@ -1747,4 +1716,419 @@ def check_mhsa_encoder(n_seq=37, T=20, d=300, heads=15, q=200, V=500, p_drop=0.2
     fb2, _ = forward()
     torch.cuda.synchronize()
     res["fwd_deterministic"] = all(_bits_equal(fb[k].body, fb2[k].body) for k in fb if k != "flag")
+    return res
+
+
+# ------------------------------------------------------------------------------------------------
+# The LSTUR GRU (nr_gru_fwd / _bwd) step by step.  The fp64 step functions below work in the (S, B, .) layout on any device;
+# tests/test_gru_host.py checks them against torch.autograd through the oracle on the CPU, tests/test_gpu_gru.py holds the
+# kernels to them (bounds derived there).
+# ------------------------------------------------------------------------------------------------
+def gru_gates(gi, gh, Hd):
+    """r, z, n of torch's gate order r | z | n and the pre-activations a_r, a_z, v = gi_n + r gh_n."""
+    a_r = gi[..., :Hd] + gh[..., :Hd]
+    a_z = gi[..., Hd:2 * Hd] + gh[..., Hd:2 * Hd]
+    r, z = torch.sigmoid(a_r), torch.sigmoid(a_z)
+    v = gi[..., 2 * Hd:] + r * gh[..., 2 * Hd:]
+    return dict(r=r, z=z, n=torch.tanh(v), a_r=a_r, a_z=a_z, v=v)
+
+
+def gru_proj(rows, w, b):
+    """rows . w^T + b and the sum of |products| (with |b|): gi from the stored bf16 x rows (hi, then lo), gh[t] from hb[t]."""
+    return rows @ w.t() + b, rows.abs() @ w.abs().t() + b.abs()
+
+
+def gru_step(gi_t, gh_t, h_t, active):
+    """hs[t+1] from gi[t], gh[t] and hs[t]; rows with active False (t >= max(len, 1)) keep h_t."""
+    g = gru_gates(gi_t, gh_t, h_t.shape[-1])
+    return torch.where(active.view(-1, 1), (1 - g["z"]) * g["n"] + g["z"] * h_t, h_t)
+
+
+def gru_bwd_chain(gi, gh, hs, L, w_ih, w_hh, x_ext, h_ext, dout, contract=False, dgh_stored=None):
+    """The backward of the recurrence written out step by step, in the inputs' dtype, from the forward values the kernels store:
+    gi, gh (S, B, 3Hd), hs (S+1, B, Hd), L (B,) = max(len, 1), w_ih (3Hd, D), w_hh (3Hd, Hd), x_ext (S, B, D+1) and h_ext
+    (S, B, Hd+1) the operand rows of the two projections with their ones column, dout (B, Hd).  contract=True rounds dgi and dgh
+    to bf16 where the kernels store them.  The dh entering step t - 1 is dh z (frozen rows: dh) + dgh[t] W_hh, with dgh[t] the
+    chain's own or, when dgh_stored is given, the kernel's stored one.  Returns dgi, dgh (S, B, 3Hd), dh (S, B, Hd) the gradient
+    entering each step, dh0, dx (S, B, D), dWih (3Hd, D+1), dWhh (3Hd, Hd+1) (last column: the bias)."""
+    S, B, H3 = gi.shape
+    Hd = H3 // 3
+    rnd = _bf16_round if contract else (lambda t: t)
+    dgi, dgh, dh_in = torch.empty_like(gi), torch.empty_like(gh), torch.empty_like(hs[1:])
+    dh = dout
+    for t in range(S - 1, -1, -1):
+        act = (t < L).view(-1, 1)
+        g = gru_gates(gi[t], gh[t], Hd)
+        r, z, n = g["r"], g["z"], g["n"]
+        dh_in[t] = dh
+        dn = dh * (1 - z)
+        dz = dh * (hs[t] - n)
+        dpn = dn * (1 - n * n)
+        dpz = dz * z * (1 - z)
+        dpr = dpn * gh[t, :, 2 * Hd:] * r * (1 - r)
+        dgi[t] = rnd(torch.where(act, torch.cat([dpr, dpz, dpn], 1), 0.0))
+        dgh[t] = rnd(torch.where(act, torch.cat([dpr, dpz, dpn * r], 1), 0.0))
+        rec = (dgh[t] if dgh_stored is None else dgh_stored[t]) @ w_hh
+        dh = torch.where(act, dh * z, dh) + rec
+    flat = lambda t: t.reshape(S * B, -1)
+    return dict(dgi=dgi, dgh=dgh, dh=dh_in, dh0=dh, dx=dgi @ w_ih, dWih=flat(dgi).t() @ flat(x_ext), dWhh=flat(dgh).t() @ flat(h_ext))
+
+
+def gru_bwd_workspace_layout(B, S, Hd):
+    """gru.cu GruBwdWorkspace: byte offsets of dgi bf16 [B*S][ldb] (rows b*S + t), dgh bf16 [S][B][ldb], dh_direct and dh_rec fp32
+    [B][round_up(Hd, 4)], each region rounded up to 256 bytes, and the total (one more 256-byte slot)."""
+    a256 = lambda n: (n + 255) // 256 * 256
+    ldb, P = ru8(3 * Hd + 1), (Hd + 3) // 4 * 4
+    off, lay = 0, {}
+    for k, n in (("dgi", B * S * ldb * 2), ("dgh", B * S * ldb * 2), ("dh_direct", B * P * 4), ("dh_rec", B * P * 4)):
+        lay[k] = off
+        off += a256(n)
+    return lay, off + 256
+
+
+def gru_lengths(B, S, seed):
+    """Lengths 1..S with 0, -3, 1, S - 1 and S planted at scattered rows (unsorted)."""
+    lens = O.det_randint((B,), seed, 1, S + 1)
+    for pos, v in zip((B // 2, 0, B - 1, B // 3, (2 * B) // 3), (0, -3, 1, S - 1, S)):
+        if B > 0:
+            lens[pos] = v
+    return lens
+
+
+_U = 2.0 ** -24      # fp32 unit roundoff
+_EX2 = 2.0 ** -22    # ex2.approx.f32: 2 ulp, at most 2^-22 relative
+_DIV = 2.0 ** -22    # div.approx.f32 (__fdividef): 2 ulp for divisors in [2^-126, 2^126]
+_TINY = 2.0 ** -100  # flush-to-zero of results below 2^-126 and the divisors above 2^126
+
+
+def gru_gate_errors(g, gh_n):
+    """Absolute error bounds of the kernels' fp32 gates on the stored gi, gh (tests/test_gpu_gru.py derives them): r, z, n."""
+    def sig(a, s):
+        return s * ((1 - s) * (3 * _U * a.abs() + _EX2) + _U + _DIV) + _TINY
+    Er, Ez = sig(g["a_r"], g["r"]), sig(g["a_z"], g["z"])
+    n, v = g["n"], g["v"]
+    Ev = gh_n.abs() * Er + _U * (g["r"] * gh_n).abs() + _U * v.abs()
+    En = (1 - n * n) * Ev + (1 - n * n) / 2 * (4 * _U * v.abs() + _EX2) + (1 - n) * (_U + _DIV) + _U * n.abs() + _TINY
+    return Er, Ez, En
+
+
+def _dev_error(lib):
+    e = (C.c_int * 4)()
+    lib.nr_device_error(C.byref(e))
+    return list(e)
+
+
+def check_gru_stages(B=37, S=50, D=900, Hd=900, accurate=True, h0_zero=False, x_layout="contig", wscale=1.0, seed=3,
+                     paths=("default",), e2e=True):
+    """nr_gru_fwd / _bwd stage by stage against fp64 references built from what the kernels stored (gi, gh, hs, hb, and the
+    workspace's dgi, dgh, dh_direct, dh_rec), per element.  paths: "default" (the library's choice), "persistent" / "stepwise"
+    (nr_debug_set_gru_stepwise 0 / 1); each path runs its own forward and backward on the same operands.  x_layout: "contig",
+    "perm" ([S][B][D] storage), "col2" (column stride 2), "slice" (s_b > S D); storage elements x does not cover are NaN.
+    Every "=" output starts as NaN, the "+=" outputs with a small pattern, the workspace with 0xFF; every buffer, the operands
+    included, is followed by a guard.  Bounds: tests/test_gpu_gru.py."""
+    import os
+    from newsrec_b200 import GruBwdArgs, GruFwdArgs
+    from newsrec_b200.ops_gru import ru4
+    lib = load_library()
+    ldd, ldh, ldg, ldb = ru8(D + 1), ru8(Hd + 1), ru4(3 * Hd), ru8(3 * Hd + 1)
+    H3, R = 3 * Hd, B * S
+    nan = float("nan")
+    G_ = lambda t: _Guarded(t.numel(), t.dtype, t)
+    a_w = wscale / math.sqrt(Hd)
+    Wih, Whh = _rand_bf16((H3, D), seed, a_w).to(DEV), _rand_bf16((H3, Hd), seed + 1, a_w).to(DEV)
+    bih = O.det_uniform((H3,), seed + 2, -a_w, a_w).to(DEV)
+    bhh = O.det_uniform((H3,), seed + 3, -a_w, a_w).to(DEV)
+    xv = O.det_uniform((B, S, D), seed + 4).to(DEV)
+    h0v = torch.zeros(B, Hd, device=DEV) if h0_zero else O.det_uniform((B, Hd), seed + 5, -0.5, 0.5).to(DEV)
+    lens = gru_lengths(B, S, seed + 6).to(DEV)
+    dout = O.det_uniform((B, Hd), seed + 7).to(DEV)
+    ops = dict(wih=G_(cast_pad(Wih, ldd)), whh=G_(cast_pad(Whh, ldh)), wihT=G_(cast_pad(Wih, ldb, transpose=True)),
+               whhT=G_(cast_pad(Whh, ldb, transpose=True)), bih=G_(bih), bhh=G_(bhh), h0=G_(h0v), len=G_(lens), dout=G_(dout))
+    # x: a strided view into guarded storage
+    shape, off = {"contig": ((B, S, D), 0), "perm": ((S, B, D), 0), "col2": ((B, S, 2 * D), 0), "slice": ((B, S + 3, D), D)}[x_layout]
+    xs = _Guarded(math.prod(shape), torch.float32, nan)
+    st = xs.body.view(shape)
+    x = {"contig": st, "perm": st.transpose(0, 1), "col2": st[..., ::2], "slice": st[:, 1:S + 1]}[x_layout]
+    x.copy_(xv)
+    ops["x"] = xs
+    assert x_layout != "slice" or x.stride()[0] > S * D
+    L = lens.clamp(min=1)
+    act = torch.arange(S, device=DEV).view(S, 1) < L.view(1, B)  # (S, B)
+    env_default = 1 if os.environ.get("NEWSREC_GRU_STEPWISE") is not None else 0
+
+    def forward(path):
+        fb = dict(xb=_Guarded(R * ldd, torch.bfloat16, nan), gi=_Guarded(R * ldg, torch.float32, nan),
+                  gh=_Guarded(S * B * ldg, torch.float32, nan), hs=_Guarded((S + 1) * B * Hd, torch.float32, nan),
+                  hb=_Guarded((S + 1) * B * ldh, torch.bfloat16, nan), out=_Guarded(B * Hd, torch.float32, nan))
+        if accurate:
+            fb["xlo"] = _Guarded(R * ldd, torch.bfloat16, nan)
+        a = GruFwdArgs()
+        a.B, a.S, a.D, a.Hd = B, S, D, Hd
+        a.x = _p(x if x.numel() else xs.all)  # an empty view may report a null data pointer
+        a.x_s_b, a.x_s_t, a.x_s_c = x.stride()
+        a.len, a.h0 = _p(ops["len"].all), _p(ops["h0"].all)
+        a.wih_bf16, a.whh_bf16, a.bih, a.bhh = _p(ops["wih"].all), _p(ops["whh"].all), _p(ops["bih"].all), _p(ops["bhh"].all)
+        a.xb, a.gi, a.gh, a.hs, a.hb, a.out = (_p(fb[k].all) for k in ("xb", "gi", "gh", "hs", "hb", "out"))
+        a.x_lo_bf16 = _p(fb["xlo"].all) if accurate else None
+        lib.nr_debug_set_gru_stepwise({"default": env_default, "persistent": 0, "stepwise": 1}[path])
+        try:
+            n0 = int(lib.nr_launch_count())
+            check(lib.nr_gru_fwd(C.byref(a), _stream()), "nr_gru_fwd")
+            launches = int(lib.nr_launch_count()) - n0
+        finally:
+            lib.nr_debug_set_gru_stepwise(env_default)
+        torch.cuda.synchronize()
+        return fb, launches, _dev_error(lib)
+
+    def backward(fb):
+        pat = lambda n, s: O.det_uniform((n,), s, 0.5, 1.0).to(DEV) * 2.0 ** -16  # small non-zero "+=" pre-fill
+        bb = dict(dWih=_Guarded(H3 * ldd, torch.float32, pat(H3 * ldd, seed + 20)),
+                  dWhh=_Guarded(H3 * ldh, torch.float32, pat(H3 * ldh, seed + 21)),
+                  dx=_Guarded(R * D, torch.float32, nan), dh0=_Guarded(B * Hd, torch.float32, nan))
+        ws_bytes = int(lib.nr_gru_bwd_workspace(B, S, D, Hd))
+        ws = _Guarded(ws_bytes, torch.uint8, 0xFF, sentinel=0xA5)  # 0xFFFF.. = NaN in bf16 and fp32
+        b = GruBwdArgs()
+        b.B, b.S, b.D, b.Hd = B, S, D, Hd
+        b.len, b.wihT_bf16, b.whhT_bf16 = _p(ops["len"].all), _p(ops["wihT"].all), _p(ops["whhT"].all)
+        b.xb, b.gi, b.gh, b.hs, b.hb = (_p(fb[k].all) for k in ("xb", "gi", "gh", "hs", "hb"))
+        b.dout, b.dWih_ext, b.dWhh_ext, b.dx, b.dh0 = _p(ops["dout"].all), _p(bb["dWih"].all), _p(bb["dWhh"].all), _p(bb["dx"].all), \
+            _p(bb["dh0"].all)
+        b.workspace, b.workspace_bytes = _p(ws.all), ws_bytes
+        n0 = int(lib.nr_launch_count())
+        check(lib.nr_gru_bwd(C.byref(b), _stream()), "nr_gru_bwd")
+        launches = int(lib.nr_launch_count()) - n0
+        torch.cuda.synchronize()
+        return bb, ws, launches, _dev_error(lib)
+
+    res = {"persistent_supported": bool(lib.nr_gru_persistent_supported(B, Hd)), "sms": int(lib.nr_num_sms()), "paths": {}}
+    saved = {}
+    ref = None
+    if B > 0 and e2e:
+        ref = _gru_end_to_end_refs(xv, L, h0v, Wih, Whh, bih, bhh, dout, accurate)
+    for path in paths:
+        fb, fl, fe = forward(path)
+        bb, ws, bl, be = backward(fb)
+        m = {"fwd_launches": fl, "bwd_launches": bl, "fwd_device_error": fe, "bwd_device_error": be,
+             "guards_intact": all(g.guard_ok() for g in list(fb.values()) + list(bb.values()) + list(ops.values()) + [ws])}
+        if B == 0:
+            res["paths"][path] = m
+            continue
+        m.update(_gru_judge(fb, bb, ws, xv, h0v, L, act, Wih, Whh, bih, bhh, dout, accurate, B, S, D, Hd, ref))
+        del ws, bb
+        fb2, _, _ = forward(path)
+        m["fwd_deterministic"] = all(_bits_equal(fb[k].body, fb2[k].body) for k in fb)
+        del fb2
+        res["paths"][path] = m
+        saved[path] = fb
+    if len(saved) == 2:
+        a_, b_ = saved.values()
+        res["paths_bit_identical"] = {k: _bits_equal(a_[k].body, b_[k].body) for k in a_}
+    return res
+
+
+def gru_reference(x, h0, L, w_ih, w_hh, b_ih, b_hh, dout, contract=None):
+    """The GRU in the inputs' dtype from x (B, S, D), forward and backward.  contract None: exact.  "bf16": x and every h rounded
+    to bf16 as GEMM operands, dgi and dgh stored in bf16 (oracle.BF16).  "hilo": the same, but x enters the input projection as a
+    hi/lo pair (taken as exact, oracle.BF16_FUSED) while the weight gradient reads the bf16 x rows, the only plane the kernels
+    keep for the backward.  Returns out (B, Hd), dx (B, S, D), dh0, dWih (3Hd, D+1), dWhh (3Hd, Hd+1) (last column: the bias)."""
+    B, S, D = x.shape
+    rnd = (lambda t: t) if contract is None else _bf16_round
+    xS = x.transpose(0, 1)
+    gi = gru_proj((rnd(xS) if contract == "bf16" else xS).reshape(S * B, D), w_ih, b_ih)[0].view(S, B, -1)
+    hs, gh, hop = [h0], [], []
+    for t in range(S):
+        hop.append(rnd(hs[t]))
+        gh.append(gru_proj(hop[t], w_hh, b_hh)[0])
+        hs.append(gru_step(gi[t], gh[t], hs[t], t < L))
+    one = torch.ones(S, B, 1, dtype=x.dtype, device=x.device)
+    ch = gru_bwd_chain(gi, torch.stack(gh), torch.stack(hs), L, w_ih, w_hh, torch.cat([rnd(xS), one], 2), torch.cat([torch.stack(hop), one], 2),
+                       dout, contract=contract is not None)
+    return dict(out=hs[S], dx=ch["dx"].transpose(0, 1), dh0=ch["dh0"], dWih=ch["dWih"], dWhh=ch["dWhh"])
+
+
+def _gru_end_to_end_refs(xv, L, h0v, Wih, Whh, bih, bhh, dout, accurate):
+    """The exact fp64 GRU and the bf16 storage contract of the mode, on the device (gru_reference)."""
+    args = [t.double() for t in (xv, h0v)] + [L] + [t.double() for t in (Wih, Whh, bih, bhh, dout)]
+    return {"exact": gru_reference(*args), "contract": gru_reference(*args, contract="hilo" if accurate else "bf16")}
+
+
+def _gru_judge(fb, bb, ws, xv, h0v, L, act, Wih, Whh, bih, bhh, dout, accurate, B, S, D, Hd, ref):
+    from newsrec_b200.ops_gru import ru4
+    ldd, ldh, ldg, ldb = ru8(D + 1), ru8(Hd + 1), ru4(3 * Hd), ru8(3 * Hd + 1)
+    H3, R = 3 * Hd, B * S
+    m = {}
+    i16 = lambda t: t.contiguous().view(torch.int16)
+    # ---- the operand rows: bit exact
+    exp_x = torch.zeros(B, S, ldd, device=DEV)
+    exp_x[..., :D] = xv
+    exp_x[..., D] = 1.0
+    xb = fb["xb"].body.view(B, S, ldd)
+    m["xb_mismatch_rows"] = int((i16(xb) != i16(exp_x.to(torch.bfloat16))).any(-1).sum())
+    if accurate:
+        exp_lo = torch.zeros(B, S, ldd, device=DEV)
+        exp_lo[..., :D] = xv - bf16r(xv)
+        m["xlo_mismatch_rows"] = int((i16(fb["xlo"].body.view(B, S, ldd)) != i16(exp_lo.to(torch.bfloat16))).any(-1).sum())
+    hs = fb["hs"].body.view(S + 1, B, Hd)
+    hb = fb["hb"].body.view(S + 1, B, ldh)
+    exp_hb = torch.zeros(S + 1, B, ldh, device=DEV)
+    exp_hb[..., :Hd] = hs
+    exp_hb[..., Hd] = 1.0
+    m["hs0_exact"] = _bits_equal(hs[0], h0v)
+    m["hb_mismatch_rows"] = int((i16(hb) != i16(exp_hb.to(torch.bfloat16))).any(-1).sum())  # hb[0] and every hb[t+1]
+    m["out_equals_hs_S"] = _bits_equal(fb["out"].body.view(B, Hd), hs[S])
+    m["fwd_outputs_finite"] = all(bool(torch.isfinite(t.float()).all()) for t in (
+        xb, fb["gi"].body.view(R, ldg)[:, :H3], fb["gh"].body.view(S, B, ldg)[..., :H3], hs, hb, fb["out"].body))
+    # ---- gi and every gh[t]: fp64 product of the stored bf16 operands plus the bias, within 1e-6 sum |x||w|
+    W1, W2 = Wih.double(), Whh.double()
+    gi = fb["gi"].body.view(B, S, ldg).transpose(0, 1)[..., :H3].double()  # (S, B, 3Hd)
+    gh = fb["gh"].body.view(S, B, ldg)[..., :H3].double()
+    xbS = xb.transpose(0, 1)[..., :D].double()
+    xloS = fb["xlo"].body.view(B, S, ldd).transpose(0, 1)[..., :D].double() if accurate else None
+    acc = {k: 0.0 for k in ("gi_ratio", "gi_no_lo_ratio", "gh_ratio", "hs_ratio", "hs_bhn_outside_r_ratio", "dg_ratio",
+                            "dgh_n_without_r_ratio", "dx_ratio", "dh0_ratio", "max_preact")}
+    worst = lambda k, t: acc.__setitem__(k, max(acc[k], _worst(t)))
+    frozen_ok = True
+    for t in range(S):
+        g_ref, g_abs = gru_proj(xbS[t], W1, bih.double())
+        if accurate:
+            lo_ref, lo_abs = gru_proj(xloS[t], W1, torch.zeros_like(bih, dtype=torch.float64))
+            worst("gi_no_lo_ratio", _safe_div((gi[t] - g_ref).abs(), 1e-6 * (g_abs + lo_abs)))
+            g_ref, g_abs = g_ref + lo_ref, g_abs + lo_abs
+        worst("gi_ratio", _safe_div((gi[t] - g_ref).abs(), 1e-6 * g_abs))
+        h_ref, h_abs = gru_proj(hb[t, :, :Hd].double(), W2, bhh.double())
+        worst("gh_ratio", _safe_div((gh[t] - h_ref).abs(), 1e-6 * h_abs))
+        # hs[t+1]: active rows within the gate bound, frozen rows bit-identical to hs[t]
+        h_t = hs[t].double()
+        g = gru_gates(gi[t], gh[t], Hd)
+        Er, Ez, En = gru_gate_errors(g, gh[t, :, 2 * Hd:])
+        r, z, n = g["r"], g["z"], g["n"]
+        hn = (1 - z) * n + z * h_t
+        bound = (h_t - n).abs() * Ez + (1 - z) * En + 3 * _U * ((1 - z) * n.abs() + z * h_t.abs())
+        a_t = act[t]
+        worst("max_preact", torch.cat([g["a_r"], g["a_z"], g["v"]], 1).abs()[a_t])
+        worst("hs_ratio", _safe_div((hs[t + 1].double() - hn).abs(), bound)[a_t])
+        bhn = bhh.double()[2 * Hd:]
+        n_cudnn = torch.tanh(gi[t, :, 2 * Hd:] + r * (gh[t, :, 2 * Hd:] - bhn) + bhn)  # b_hn outside r
+        worst("hs_bhn_outside_r_ratio", _safe_div((hs[t + 1].double() - ((1 - z) * n_cudnn + z * h_t)).abs(), bound)[a_t])
+        frozen_ok &= _bits_equal(hs[t + 1][~a_t], hs[t][~a_t])
+    m["hs_frozen_rows_exact"] = frozen_ok
+    # ---- backward: the workspace as the kernels left it
+    lay, total = gru_bwd_workspace_layout(B, S, Hd)
+    m["workspace_bytes_match"] = total == ws.n
+    wsb = ws.body
+    dgi_k = wsb[lay["dgi"]:lay["dgi"] + R * ldb * 2].view(torch.bfloat16).view(B, S, ldb)
+    dgh_k = wsb[lay["dgh"]:lay["dgh"] + R * ldb * 2].view(torch.bfloat16).view(S, B, ldb)
+    P = (Hd + 3) // 4 * 4
+    dh_dir = wsb[lay["dh_direct"]:lay["dh_direct"] + B * P * 4].view(torch.float32).view(B, P)[:, :Hd]
+    dh_rec = wsb[lay["dh_rec"]:lay["dh_rec"] + B * P * 4].view(torch.float32).view(B, P)[:, :Hd]
+    m["dg_pad_cols_zero"] = bool((i16(dgi_k[..., H3:]) == 0).all()) and bool((i16(dgh_k[..., H3:]) == 0).all())
+    dgiS = dgi_k.transpose(0, 1)[..., :H3].double()
+    dghS = dgh_k[..., :H3].double()
+    ones = torch.ones(S, B, 1, dtype=torch.float64, device=DEV)
+    x_ext = torch.cat([xbS, ones], 2)
+    h_ext = torch.cat([hb[:S, :, :Hd].double(), ones], 2)
+    ch = gru_bwd_chain(gi, gh, hs.double(), L, W1, W2, x_ext, h_ext, dout.double(), dgh_stored=dghS)
+    A = torch.zeros(B, Hd, dtype=torch.float64, device=DEV)  # bound on |dh_kernel - dh_reference| entering step t
+    dh_is_dout, dg_frozen_ok = True, True
+    for t in range(S - 1, -1, -1):
+        a_t = act[t].view(-1, 1)
+        g = gru_gates(gi[t], gh[t], Hd)
+        Er, Ez, En = gru_gate_errors(g, gh[t, :, 2 * Hd:])
+        r, z, n = g["r"], g["z"], g["n"]
+        ghn = gh[t, :, 2 * Hd:]
+        dh = ch["dh"][t]
+        last = (L - 1 == t) & (L < S)
+        dh_is_dout &= bool((dh[last] == dout.double()[last]).all())
+        hp = hs[t].double()
+        dn, dz = dh * (1 - z), dh * (hp - n)
+        dpn, dpz = dn * (1 - n * n), dz * z * (1 - z)
+        dpr = dpn * ghn * r * (1 - r)
+        E_dn = (1 - z) * A + dh.abs() * Ez + 2 * _U * dn.abs()
+        E_dpn = (1 - n * n) * E_dn + dn.abs() * 2 * n.abs() * En + 3 * _U * dpn.abs() + _TINY
+        E_dz = (hp - n).abs() * A + dh.abs() * En + 2 * _U * dz.abs()
+        E_dpz = z * (1 - z) * E_dz + dz.abs() * (1 - 2 * z).abs() * Ez + 3 * _U * dpz.abs() + _TINY
+        E_dpr = (ghn * r * (1 - r)).abs() * E_dpn + (dpn * ghn).abs() * (1 - 2 * r).abs() * Er + 4 * _U * dpr.abs() + _TINY
+        E_dghn = r * E_dpn + dpn.abs() * Er + _U * (dpn * r).abs() + _TINY
+        ref_gi = torch.cat([dpr, dpz, dpn], 1)
+        ref_gh = torch.cat([dpr, dpz, dpn * r], 1)
+        e_gi = torch.cat([E_dpr, E_dpz, E_dpn], 1)
+        e_gh = torch.cat([E_dpr, E_dpz, E_dghn], 1)
+        half_ulp = lambda k, rf: _bf16_ulp(torch.maximum(k.abs(), rf.abs())) / 2
+        for k, rf, e in ((dgiS[t], ref_gi, e_gi), (dghS[t], ref_gh, e_gh)):
+            worst("dg_ratio", _safe_div((k - rf).abs(), half_ulp(k, rf) + e)[a_t.view(-1)])
+        kn = dghS[t, :, 2 * Hd:]
+        worst("dgh_n_without_r_ratio", _safe_div((kn - dpn).abs(), half_ulp(kn, dpn) + E_dghn)[a_t.view(-1)])
+        dg_frozen_ok &= bool((i16(dgi_k[:, t, :H3])[~act[t]] == 0).all()) and bool((i16(dgh_k[t, :, :H3])[~act[t]] == 0).all())
+        # the dh entering step t - 1: dh z (fp32) + dgh[t] W_hh (fp32 GEMM, 1e-6 sum |dgh||w|), then one fp32 sum
+        nxt = ch["dh"][t - 1] if t > 0 else ch["dh0"]
+        G = 1e-6 * (dghS[t].abs() @ W2.abs())
+        A = torch.where(a_t, z * A + dh.abs() * Ez + _U * (dh * z).abs() + G + _U * nxt.abs(), A)
+    m["dg_frozen_zero"] = dg_frozen_ok
+    m["dh_at_last_active_step_is_dout"] = dh_is_dout
+    dh0_k = bb["dh0"].body.view(B, Hd)
+    ftz = lambda t_: torch.where(t_.abs() < 2.0 ** -126, torch.zeros_like(t_), t_)  # the kernels flush fp32 subnormals
+    m["dh0_equals_workspace_sum"] = _bits_equal(ftz(dh0_k), ftz(ftz(dh_dir) + ftz(dh_rec)))
+    worst("dh0_ratio", _safe_div((dh0_k.double() - ch["dh0"]).abs(), A + _TINY))
+    # ---- dx from the stored dgi: 1e-6 sum |dgi||w|, exactly 0 on frozen steps
+    dx_k = bb["dx"].body.view(B, S, D).transpose(0, 1)
+    for t in range(S):
+        worst("dx_ratio", _safe_div((dx_k[t].double() - dgiS[t] @ W1).abs(), 1e-6 * (dgiS[t].abs() @ W1.abs()) + _TINY))
+    m["dx_frozen_zero"] = bool((dx_k[~act] == 0).all())
+    m["bwd_outputs_finite"] = bool(torch.isfinite(bb["dx"].body).all()) and bool(torch.isfinite(dh0_k).all())
+    # ---- the weight gradients: pattern + dg^T [X | 1] from the stored operands, per element, against the split-K allowance
+    steps = 5 * ((R + 63) // 64) + 1
+    for key, dg, Xe, w in (("dWih", dgiS, x_ext, ldd), ("dWhh", dghS, h_ext, ldh)):
+        K1 = Xe.shape[-1]
+        pre = bb[key].prefill.double().view(H3, w)
+        got = bb[key].body.view(H3, w)
+        flat = lambda t_: t_.reshape(R, -1)
+        rf = pre[:, :K1] + flat(dg).t() @ flat(Xe)
+        ab = pre[:, :K1].abs() + flat(dg).abs().t() @ flat(Xe).abs()
+        m[key + "_elem_ratio"] = _worst(_safe_div((got[:, :K1].double() - rf).abs(), 2.0 ** -22 * steps * ab + _TINY))
+        cols = torch.zeros(H3, w, dtype=torch.bool, device=DEV)
+        cols[:, K1:] = True
+        m[key + "_pitch_cols_untouched"] = bb[key].unchanged(cols)
+    m.update(acc)
+    # ---- end to end: each row against the exact fp64 GRU, next to the bf16 contract's error (the project's gradient rule)
+    if ref is not None:
+        ex, co = ref["exact"], ref["contract"]
+        kern = dict(out=fb["out"].body.view(B, Hd).double(), dx=bb["dx"].body.view(R, D).double(), dh0=dh0_k.double(),
+                    dWih=(bb["dWih"].body.double() - bb["dWih"].prefill.double()).view(H3, ldd)[:, :D + 1],
+                    dWhh=(bb["dWhh"].body.double() - bb["dWhh"].prefill.double()).view(H3, ldh)[:, :Hd + 1])
+        for k, v in kern.items():
+            e_, c_ = ex[k].reshape(v.shape), co[k].reshape(v.shape)
+            m[k + "_tensor_rel_vs_contract"] = relerr(v, c_)
+            # rows whose exact norm is below fp32's normal range (a gradient that decays over hundreds of steps) cannot be
+            # held to a relative rule: the kernels flush subnormals to zero
+            keep = e_.norm(dim=1) > 2.0 ** -100
+            m[k + "_rows_below_fp32_range"] = int((~keep).sum())
+            m[k + "_row_ratio"], m[k + "_ek"], m[k + "_ec"] = _row_ratio(v[keep], e_[keep], c_[keep])
+    return m
+
+
+def check_gru_autograd(B=37, S=50, D=900, Hd=900, accurate=True, seed=3):
+    """GruLastHiddenFn (the model's entry: operand cache, dW_ext split into weight and bias gradients) end to end: each row of
+    the output and of every gradient against the exact fp64 GRU next to the bf16 contract's error."""
+    from newsrec_b200.ops import OperandCache
+    from newsrec_b200.ops_gru import GruLastHiddenFn
+    a_w = 1.0 / math.sqrt(Hd)
+    Wih, Whh = _rand_bf16((3 * Hd, D), seed, a_w).to(DEV), _rand_bf16((3 * Hd, Hd), seed + 1, a_w).to(DEV)
+    bih = O.det_uniform((3 * Hd,), seed + 2, -a_w, a_w).to(DEV)
+    bhh = O.det_uniform((3 * Hd,), seed + 3, -a_w, a_w).to(DEV)
+    xv = O.det_uniform((B, S, D), seed + 4).to(DEV)
+    h0v = O.det_uniform((B, Hd), seed + 5, -0.5, 0.5).to(DEV)
+    lens = gru_lengths(B, S, seed + 6).to(DEV)
+    dout = O.det_uniform((B, Hd), seed + 7).to(DEV)
+    ref = _gru_end_to_end_refs(xv, lens.clamp(min=1), h0v, Wih, Whh, bih, bhh, dout, accurate)
+    leaves = [t.clone().requires_grad_(True) for t in (xv, h0v, Wih, Whh, bih, bhh)]
+    x, h0, wi, wh, bi, bh = leaves
+    out = GruLastHiddenFn.apply(x, lens, h0, wi, wh, bi, bh, OperandCache(), "gru", accurate)
+    out.backward(dout)
+    torch.cuda.synchronize()
+    res = {}
+    ex, co = ref["exact"], ref["contract"]
+    kern = dict(out=out.detach().double(), dx=x.grad.double().reshape(B * S, D), dh0=h0.grad.double(),
+                dWih=torch.cat([wi.grad, bi.grad.view(-1, 1)], 1).double(), dWhh=torch.cat([wh.grad, bh.grad.view(-1, 1)], 1).double())
+    for k, v in kern.items():
+        res[k + "_row_ratio"], res[k + "_ek"], res[k + "_ec"] = _row_ratio(v, ex[k].reshape(v.shape), co[k].reshape(v.shape))
     return res
