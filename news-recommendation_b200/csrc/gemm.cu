@@ -698,7 +698,7 @@ int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int
     EpiDPre e;
     memset(&e, 0, sizeof(e));
     e.use_tma = q >= 32 ? 1 : 0;
-    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, dpre, M, ld_dpre, ld_dpre, 32, 32, 64));
+    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, dpre, M, ld_dpre, ld_dpre, 32, 16, 64));
     e.bias = ba;
     e.qv = qv;
     e.dscore = dscore;
@@ -718,15 +718,24 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
     const int nseg_max = kTileM / seg_len + 2;
     const int max_stride = (EpiDPoolIn::kStageFloats / nseg_max) & ~15;
     NR_REQUIRE(max_stride >= 16, "pool_dinput: seg_len=%d needs %d staged segments per tile", seg_len, nseg_max);
+    NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
     GemmNTPlan plan;
+    if (c.rm.seg_in == 0 && c.relu_src == nullptr && !c.zero_pad_rows && D >= 32) {  // identity rows, no mask: the fragment view
+        NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
+                                  kEpiSmemBytes<EpiDPoolInFrag>, max_stride));
+        EpiDPoolInFrag e{.w = c.w, .dout = c.dout, .ldo = c.ldo, .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx,
+                         .N = D, .drop = to_drop(c.drop), .M = M};
+        NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.dx, M, D, c.ld_dx, 32, 16, 64));
+        g_launches += debug_simt_gemm() ? 2 : 1;
+        ProfScope ps("gemm_pool_dinput", M, D, g.K, stream);
+        return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
+    }
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0, kEpiSmemBytes<EpiDPoolIn>,
                               max_stride));
-    NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
-    EpiDPoolIn e{.use_tma = (c.rm.seg_in == 0 && c.relu_src == nullptr && D >= 32) ? 1 : 0, .w = c.w, .dout = c.dout, .ldo = c.ldo,
+    EpiDPoolIn e{.w = c.w, .dout = c.dout, .ldo = c.ldo,
                  .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx, .N = D, .rm = to_rm(c.rm),
                  .zero_pad_rows = c.zero_pad_rows, .drop = to_drop(c.drop), .relu_src = static_cast<const __nv_bfloat16*>(c.relu_src),
                  .relu_ld = c.relu_ld, .M = M, .rows_per_tile = kTileM};
-    if (e.use_tma) NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.dx, M, D, c.ld_dx, 32, 32, 64));
     g_launches += debug_simt_gemm() ? 2 : 1;
     ProfScope ps("gemm_pool_dinput", M, D, g.K, stream);
     return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);

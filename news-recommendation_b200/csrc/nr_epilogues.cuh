@@ -413,11 +413,20 @@ struct EpiPool {
 // ------------------------------------------------------------------------------------------------
 // Backward of the additive scorer, fused behind the recomputed pre = X.Wa^T:
 //   T = tanh(pre + ba);  dPre_rc = dscore_r * qv_c * (1 - T^2)  -> bf16;   dqv_c += sum_r dscore_r * T_rc
-// scratch floats: [0,256) column sums | [256,512) bias | [512,768) query vector
+// Fragment view: every dPre element depends on its own row and column only, so each warp works on its 16 rows of the tile
+// straight from the wgmma fragment (the row view's shared-memory transpose was most of this GEMM's time).  A 32-column
+// chunk of dPre is packed into one of the warp's staging boxes with stmatrix and leaves by TMA; the dqv column sums of the
+// chunk are reduced over the warp's rows with a 7-shuffle butterfly and added to shared memory, one column per lane.
+// The output tensor map spans the whole pitch ld: the columns in [ncols, ld) are written as exact zeros (bias and query
+// vector are zero there), so GEMMs that read dPre with K = ld see zero padding.
+// scratch floats: [0,256) column sums | [256,512) bias | [512,768) query vector | kBoxes staging boxes per consumer warp
 // ------------------------------------------------------------------------------------------------
 struct EpiDPre {
-    static constexpr int kScratchBytes = 3072 + kTileStoreBytes;
-    CUtensorMap tm_out;       // dpre as a TMA tensor (32 x 32 boxes); valid when use_tma
+    static constexpr bool kFragmentView = true;
+    static constexpr int kBoxBytes = 16 * 64;  // 16 rows x 32 bf16, SWIZZLE_64B (as EpiStore)
+    static constexpr int kBoxes = 4;           // a smaller ring than EpiStore's keeps six A stages beside a 224 x 320 weight slice
+    static constexpr int kScratchBytes = 3072 + kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    CUtensorMap tm_out;       // dpre as a TMA tensor ([rows][ld], 32 x 16 boxes, SWIZZLE_64B); valid when use_tma
     int use_tma;
     const float* bias;
     const float* qv;
@@ -437,60 +446,94 @@ struct EpiDPre {
     __device__ void finish(const EpiInit& e) const {
         consumers_bar_sync();  // both warpgroups' column sums are in; one add per column and CTA
         for (int i = e.tid; i < e.ncols; i += kEpiThreads) atomicAdd(dqv + e.col0 + i, e.scratch[i]);
-        if (use_tma) WarpTileStore::drain(e.tid & 31);
+        if (use_tma && (e.tid & 31) == 0) bulk_wait_all();
     }
-    template <class Acc>
-    __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
-        const float ds = c.valid ? __ldg(dscore + c.grow) : 0.f;
-        const int lane = c.tid & 31;
-        WarpTileStore ts;
-        if (use_tma) {
-            ts.attach(c.scratch + 768, c.tid >> 5);
-            ts.begin_tile(lane);
+
+    __device__ __forceinline__ void frag(const float* acc, const FragCtx& f) const {
+        const int lane = threadIdx.x & 31;
+        // this lane's rows e = 0, 1: tile row 16 wq + lane / 4 + 8e (rows past the tile's end carry ds = 0: dPre = 0 there, and
+        // the tensor map clips them at the last row)
+        float ds[2];
+        long long grow[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int r = 16 * f.wq + (lane >> 2) + 8 * e;
+            grow[e] = static_cast<long long>(f.row0) + r;
+            ds[e] = r < f.rows ? __ldg(dscore + grow[e]) : 0.f;
         }
-        epi_chunks(
-            acc, c, [](int) {},
-            [&](int ch, float* x) {
-                // bias and query vector are zero past ncols in shared memory: dp = 0 there without a column test, and
-                // the column sums of those columns are never added to dqv.  dp leaves packed (bf16 pairs) as soon as a pair is
-                // done: x (reused for ds * tanh) and the packed pairs are all the chunk keeps in registers.
-                uint32_t w[16];
+        const uint32_t ring = ((smem_u32(f.scratch + 768) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
+        uint32_t st_off[2];  // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 b4 = lds_f4(c.scratch + 256 + ch * 32 + j);
-                    const float4 q4 = lds_f4(c.scratch + 512 + ch * 32 + j);
-                    const float bb[4] = {b4.x, b4.y, b4.z, b4.w}, qq[4] = {q4.x, q4.y, q4.z, q4.w};
-                    float dp[4];
+        for (int x = 0; x < 2; ++x) {
+            const int m = lane >> 3, jj = 2 * x + (m >> 1), r = 8 * (m & 1) + (lane & 7);
+            st_off[x] = r * 64 + ((jj ^ (r >> 1)) & 3) * 16;
+        }
+        if (use_tma) {  // the previous tile's stores have left the boxes
+            if (lane == 0) bulk_wait_read<0>();
+            __syncwarp();
+        }
+        const int b2 = (lane >> 2) & 1, b3 = (lane >> 3) & 1, b4 = (lane >> 4) & 1;
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float tt = tanh_approx(x[j + i] + bb[i]);
-                        dp[i] = (ds * qq[i]) * fmaf(-tt, tt, 1.f);
-                        x[j + i] = ds * tt;
+        for (int q = 0; q < 8; ++q) {
+            if (q < f.nch) {  // a compile-time chunk index keeps the fragment in registers
+                const int lc0 = 32 * q;
+                uint32_t w[8];   // bf16 pair k: fragment group jj = k / 2, row e = k % 2
+                float s[8];      // ds * T summed over the lane's two rows: s[2 jj + i] = column 8 jj + 2 (lane % 4) + i
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int lc = lc0 + 8 * jj + 2 * (lane & 3);
+                    const float2 b = lds_f2(f.scratch + 256 + lc), qq = lds_f2(f.scratch + 512 + lc);
+                    float t[2][2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        t[e][0] = tanh_approx(acc[16 * q + 4 * jj + 2 * e] + b.x);
+                        t[e][1] = tanh_approx(acc[16 * q + 4 * jj + 2 * e + 1] + b.y);
+                        w[2 * jj + e] = pack_bf16x2((ds[e] * qq.x) * fmaf(-t[e][0], t[e][0], 1.f), (ds[e] * qq.y) * fmaf(-t[e][1], t[e][1], 1.f));
                     }
-                    w[j / 2] = pack_bf16x2(dp[0], dp[1]);
-                    w[j / 2 + 1] = pack_bf16x2(dp[2], dp[3]);
+                    s[2 * jj] = fmaf(ds[0], t[0][0], ds[1] * t[1][0]);
+                    s[2 * jj + 1] = fmaf(ds[0], t[0][1], ds[1] * t[1][1]);
                 }
-                if (use_tma && ch * 32 + 32 <= c.ncols) {  // invalid rows carry ds = 0 and are clipped at M anyway
-                    ts.put(&tm_out, w, c.col0 + ch * 32, c.grow - lane, lane);
-                } else if (c.valid) {
-                    uint4* o = reinterpret_cast<uint4*>(dpre + static_cast<size_t>(c.grow) * ld + c.col0 + ch * 32);
-#pragma unroll
-                    for (int g = 0; g < 2; ++g) {  // 16-byte groups of 8 columns (ld and col0 are multiples of 8)
-                        const int lc = ch * 32 + g * 16;
-                        if (lc >= c.ncols) break;  // ld is padded to a multiple of 8: whole 8-groups are in bounds
-                        o[2 * g] = make_uint4(w[8 * g], w[8 * g + 1], w[8 * g + 2], w[8 * g + 3]);
-                        if ((lc + 16 <= ld - c.col0 && aligned32(o + 2 * g)) || lc + 8 < c.ncols)
-                            o[2 * g + 1] = make_uint4(w[8 * g + 4], w[8 * g + 5], w[8 * g + 6], w[8 * g + 7]);
+                if (use_tma) {
+                    const uint32_t box = ring + (q % kBoxes) * kBoxBytes;
+                    if (q >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
+                        if (lane == 0) bulk_wait_read<kBoxes - 1>();
+                        __syncwarp();
                     }
+                    stmatrix_x4(box + st_off[0], w[0], w[1], w[2], w[3]);
+                    stmatrix_x4(box + st_off[1], w[4], w[5], w[6], w[7]);
+                    fence_proxy_async();
+                    __syncwarp();
+                    if (lane == 0) {  // rows >= M and columns >= ld are clipped by the map
+                        tma_store_2d(&tm_out, box, f.col0 + lc0, f.row0 + 16 * f.wq);
+                        bulk_commit();
+                    }
+                } else {
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = f.col0 + lc0 + 8 * jj + 2 * (lane & 3);  // even: a pair never straddles ld
+                            if (16 * f.wq + (lane >> 2) + 8 * e < f.rows && col < ld)
+                                *reinterpret_cast<uint32_t*>(dpre + grow[e] * ld + col) = w[2 * jj + e];
+                        }
                 }
-                const float colsum = warp_transpose_sum32(x);
-                if (ch * 32 + lane < c.ncols) atomicAdd(c.scratch + ch * 32 + lane, colsum);
-            });
+                // column sums over the warp's 16 rows: reduce-scatter across lane bits 4, 3, 2 (the lanes holding the same
+                // columns); lane ends with the sum of column 8 (2 b4 + b3) + 2 (lane % 4) + b2
+                float s1[4], s2[2];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) s1[k] = (b4 ? s[k + 4] : s[k]) + __shfl_xor_sync(0xffffffffu, b4 ? s[k] : s[k + 4], 16);
+#pragma unroll
+                for (int k = 0; k < 2; ++k) s2[k] = (b3 ? s1[k + 2] : s1[k]) + __shfl_xor_sync(0xffffffffu, b3 ? s1[k] : s1[k + 2], 8);
+                const float s3 = (b2 ? s2[1] : s2[0]) + __shfl_xor_sync(0xffffffffu, b2 ? s2[0] : s2[1], 4);
+                atomicAdd(f.scratch + lc0 + 8 * (2 * b4 + b3) + 2 * (lane & 3) + b2, s3);  // zero past ncols: never added to dqv
+            }
+        }
     }
 };
 
 // ------------------------------------------------------------------------------------------------
 // dX_rc = acc_rc + w_r * dOut[seg(r)][c]  (pool backward, both paths into X) [* relu mask] [* dropout] -> bf16
+// Row view, for a row-mapped destination and/or a ReLU mask (the CNN encoders); the identity / no-mask case is EpiDPoolInFrag.
 // scratch floats: two staging buffers of kStageFloats per warpgroup: the dOut rows (slice columns only) of every segment
 // the tile touches (<= 64/seg_len + 2), [segment][pitch = slice width]; the buffer of the warpgroup's NEXT tile is filled by
 // cp.async while this one is used.
@@ -498,8 +541,6 @@ struct EpiDPre {
 struct EpiDPoolIn {
     static constexpr int kStageFloats = 1536;
     static constexpr int kScratchBytes = 4 * kStageFloats * 4 + kTileStoreBytes;
-    CUtensorMap tm_out;  // dx as a TMA tensor (32 x 32 boxes); valid when use_tma (identity row map, no ReLU mask)
-    int use_tma;
     const float* w;      // [rows]
     const float* dout;   // [segments][ldo]
     int ldo;
@@ -532,9 +573,7 @@ struct EpiDPoolIn {
         const int wg = e.tid >> 7, first = e.first_tile + wg * tile_step;
         if (first < e.num_tiles) stage_tile(first, e.col0, e.ncols, e.tid & 127, e.scratch + 2 * wg * kStageFloats);
     }
-    __device__ void finish(const EpiInit& e) const {
-        if (use_tma) WarpTileStore::drain(e.tid & 31);
-    }
+    __device__ void finish(const EpiInit&) const {}
 
     template <class Acc>
     __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
@@ -551,44 +590,15 @@ struct EpiDPoolIn {
         if (c.next_tile >= 0) stage_tile(c.next_tile, c.col0, c.ncols, c.wtid, mine + ((c.it + 1) & 1) * kStageFloats);
         const float* sd = cur + myseg * c.ncols;
         const int lane = c.tid & 31;
-        WarpTileStore ts;
-        if (use_tma) {
-            ts.attach(c.scratch + 4 * kStageFloats, c.tid >> 5);
-            ts.begin_tile(lane);
-        }
         epi_chunks(
             acc, c, [](int) {},
             [&](int ch, float* x) {
-                const bool whole = use_tma && ch * 32 + 32 <= c.ncols && (c.ncols & 3) == 0;  // warp-uniform
-                if (whole) {  // identity row map, no ReLU mask; rows >= M / columns >= N are clipped by the tensor map
-                    const float* sdc = c.valid ? sd + ch * 32 : cur;  // invalid rows: any staged address (wr = 0)
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 d4 = lds_f4(sdc + j);
-                        x[j] = fmaf(wr, d4.x, x[j]); x[j + 1] = fmaf(wr, d4.y, x[j + 1]);
-                        x[j + 2] = fmaf(wr, d4.z, x[j + 2]); x[j + 3] = fmaf(wr, d4.w, x[j + 3]);
-                    }
-                    if (drop.p > 0.f) {
-                        const uint64_t g0 = (static_cast<uint64_t>(c.grow) * ld + c.col0 + ch * 32) >> 2;  // ld, col0 are multiples of 4
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            float m[4];
-                            drop.mask4_group(g0 + (j >> 2), m);
-                            x[j] *= m[0]; x[j + 1] *= m[1]; x[j + 2] *= m[2]; x[j + 3] *= m[3];
-                        }
-                    }
-                    uint32_t pk[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) pk[j] = pack_bf16x2(x[2 * j], x[2 * j + 1]);
-                    ts.put(&tm_out, pk, c.col0 + ch * 32, c.grow - lane, lane);
-                    return;
-                }
-                // Row-mapped destination and/or ReLU mask (the CNN encoders): a full 32-column chunk goes through the warp's
-                // two staging tiles so that the mask rows are LOADED and the result rows STORED as 8 rows x 64 contiguous
-                // bytes per instruction (row-per-lane 16-byte accesses touch 32 half-used sectors per instruction and
-                // queue in the LSU: this epilogue ran at 0.64 ms against 0.26 ms for the identity/TMA form of the same GEMM).
+                // a full 32-column chunk goes through the warp's two staging tiles so that the mask rows are LOADED and the
+                // result rows STORED as 8 rows x 64 contiguous bytes per instruction (row-per-lane 16-byte accesses touch 32
+                // half-used sectors per instruction and queue in the LSU: this epilogue ran at 0.64 ms against 0.26 ms for the
+                // identity/TMA form of the same GEMM on a B200).
                 const int col = c.col0 + ch * 32;
-                const bool coop = !use_tma && ch * 32 + 32 <= c.ncols && col + 32 <= N && (col & 7) == 0 && (ld & 7) == 0 &&
+                const bool coop = ch * 32 + 32 <= c.ncols && col + 32 <= N && (col & 7) == 0 && (ld & 7) == 0 &&
                                   (relu_src == nullptr || (relu_ld & 7) == 0);  // warp-uniform
                 if (coop) {
                     uint8_t* stage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(c.scratch + 4 * kStageFloats) + 1023) & ~uintptr_t(1023)) +
@@ -710,6 +720,153 @@ struct EpiDPoolIn {
             } else if (v) {
                 if (t == 0) zero_row_bf16(dx + (orow - 1) * ld, ld);
                 if (t == rm.seg_len - 1) zero_row_bf16(dx + (orow + 1) * ld, ld);
+            }
+        }
+    }
+};
+
+// ------------------------------------------------------------------------------------------------
+// The same pool backward for an identity row map without a ReLU mask (the self-attention encoders, the additive attention):
+//   dX_rc = acc_rc + w_r * dOut[seg(r)][c] [* dropout] -> bf16
+// Fragment view, as EpiStore: each warp works on its 16 rows of the tile straight from the wgmma fragment and a whole 32-column
+// chunk leaves through a staging box (stmatrix) and TMA; a chunk cut by the slice's end leaves from the fragment with
+// predicated stores.  The dOut rows are staged per warpgroup exactly as in EpiDPoolIn (double buffer, cp.async one tile ahead),
+// at a pitch of round_up(ncols, 4) floats.
+// scratch: 4 x kStageFloats floats (two staging buffers per warpgroup) | kBoxes staging boxes per consumer warp (1 KB aligned)
+// ------------------------------------------------------------------------------------------------
+struct EpiDPoolInFrag {
+    static constexpr bool kFragmentView = true;
+    static constexpr int kStageFloats = EpiDPoolIn::kStageFloats;
+    static constexpr int kBoxBytes = 16 * 64;
+    static constexpr int kBoxes = 6;
+    static constexpr int kScratchBytes = 4 * kStageFloats * 4 + kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    CUtensorMap tm_out;  // dx as a TMA tensor (32 x 16 boxes, SWIZZLE_64B)
+    const float* w;      // [rows]
+    const float* dout;   // [segments][ldo]
+    int ldo;
+    int seg_len;
+    __nv_bfloat16* dx;   // [rows][ld]
+    int ld;
+    int N;
+    Dropout drop;
+    int M;
+
+    // the 128 threads of a warpgroup (wtid): queue the dOut rows of `tile` (columns [col0, col0 + ncols)) into buf, pitch sp
+    __device__ __forceinline__ void stage_tile(int tile, int col0, int ncols, int wtid, float* buf) const {
+        const int row0 = tile * kTileM, sp = (ncols + 3) & ~3;
+        const int seg_first = row0 / seg_len;
+        const int seg_last = min(row0 + kTileM - 1, M - 1) / seg_len;
+        const int total = (seg_last - seg_first + 1) * sp;
+        for (int i = wtid; i < total; i += kWgThreads) {
+            const int sgi = i / sp, j = i - sgi * sp;
+            const bool ok = j < ncols;
+            cp_async_f32(buf + i, dout + static_cast<size_t>(seg_first + sgi) * ldo + (ok ? col0 + j : 0), ok);
+        }
+        cp_async_commit();
+    }
+    __device__ void init(const EpiInit& e, int tile_step) const {  // each warpgroup queues its own first tile
+        const int wg = e.tid >> 7, first = e.first_tile + wg * tile_step;
+        if (first < e.num_tiles) stage_tile(first, e.col0, e.ncols, e.tid & 127, e.scratch + 2 * wg * kStageFloats);
+    }
+    __device__ void finish(const EpiInit& e) const {
+        if ((e.tid & 31) == 0) bulk_wait_all();
+    }
+
+    __device__ __forceinline__ void frag(const float* acc, const FragCtx& f) const {
+        const int lane = threadIdx.x & 31;
+        float* mine = f.scratch + 2 * f.wg * kStageFloats;
+        const float* cur = mine + (f.it & 1) * kStageFloats;
+        cp_async_wait_all();
+        named_bar_sync(kBarWg + f.wg, kWgThreads);  // this tile's dOut rows are visible; the warpgroup is done with its other buffer
+        if (f.next_tile >= 0) stage_tile(f.next_tile, f.col0, f.ncols, threadIdx.x & 127, mine + ((f.it + 1) & 1) * kStageFloats);
+        const int sp = (f.ncols + 3) & ~3, seg_first = f.row0 / seg_len;
+        // this lane's rows e = 0, 1: tile row 16 wq + lane / 4 + 8e
+        bool v[2];
+        float wr[2];
+        long long grow[2];
+        const float* sd[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int r = 16 * f.wq + (lane >> 2) + 8 * e;
+            grow[e] = static_cast<long long>(f.row0) + r;
+            v[e] = r < f.rows;
+            wr[e] = v[e] ? __ldg(w + grow[e]) : 0.f;
+            sd[e] = cur + (v[e] ? static_cast<int>(grow[e] / seg_len) - seg_first : 0) * sp;
+        }
+        const uint32_t ring = ((smem_u32(f.scratch + 4 * kStageFloats) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
+        uint32_t st_off[2];  // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8
+#pragma unroll
+        for (int x = 0; x < 2; ++x) {
+            const int m = lane >> 3, jj = 2 * x + (m >> 1), r = 8 * (m & 1) + (lane & 7);
+            st_off[x] = r * 64 + ((jj ^ (r >> 1)) & 3) * 16;
+        }
+        if (lane == 0) bulk_wait_read<0>();  // the previous tile's stores have left the boxes
+        __syncwarp();
+        int nbox = 0;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            if (q < f.nch) {  // a compile-time chunk index keeps the fragment in registers
+                const int lc0 = 32 * q;
+                float y[16];  // y[4jj + 2e + i]: row e, slice column lc0 + 8jj + 2 (lane % 4) + i
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int lc = lc0 + 8 * jj + 2 * (lane & 3);
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float2 d = lc < f.ncols ? lds_f2(sd[e] + lc) : make_float2(0.f, 0.f);
+                        y[4 * jj + 2 * e] = fmaf(wr[e], d.x, acc[16 * q + 4 * jj + 2 * e]);
+                        y[4 * jj + 2 * e + 1] = fmaf(wr[e], d.y, acc[16 * q + 4 * jj + 2 * e + 1]);
+                    }
+                }
+                if (drop.p > 0.f) {
+                    // the mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of the same
+                    // group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
+                    const int b = lane & 1;
+                    const long long my_row = b ? grow[1] : grow[0];
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int col4 = f.col0 + lc0 + 8 * jj + 4 * ((lane >> 1) & 1);
+                        const uint64_t bits = dropout_bits4(drop.seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
+                        const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
+                        const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
+                        const uint32_t wd[2] = {b ? other : own, b ? own : other};
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= drop.thresh) ? drop.scale : 0.f;
+                            y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= drop.thresh) ? drop.scale : 0.f;
+                        }
+                    }
+                }
+                if (lc0 + 32 <= f.ncols) {  // warp-uniform; rows >= M are clipped by the tensor map
+                    uint32_t wp[8];
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) wp[k] = pack_bf16x2(y[2 * k], y[2 * k + 1]);
+                    const uint32_t box = ring + (nbox % kBoxes) * kBoxBytes;
+                    if (nbox >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
+                        if (lane == 0) bulk_wait_read<kBoxes - 1>();
+                        __syncwarp();
+                    }
+                    stmatrix_x4(box + st_off[0], wp[0], wp[1], wp[2], wp[3]);
+                    stmatrix_x4(box + st_off[1], wp[4], wp[5], wp[6], wp[7]);
+                    ++nbox;
+                    fence_proxy_async();
+                    __syncwarp();
+                    if (lane == 0) {
+                        tma_store_2d(&tm_out, box, f.col0 + lc0, f.row0 + 16 * f.wq);
+                        bulk_commit();
+                    }
+                } else {  // the slice's last chunk: exactly the columns < ncols
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int lc = lc0 + 8 * jj + 2 * (lane & 3);
+                            if (!v[e] || lc >= f.ncols) continue;
+                            __nv_bfloat16* o = dx + grow[e] * ld + f.col0 + lc;
+                            if (lc + 1 < f.ncols) *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y[4 * jj + 2 * e], y[4 * jj + 2 * e + 1]);
+                            else *o = __float2bfloat16_rn(y[4 * jj + 2 * e]);
+                        }
+                }
             }
         }
     }

@@ -93,6 +93,9 @@ struct FragCtx {
     int col0;     // first output column of this CTA's slice
     int ncols;    // valid output columns in the slice
     float* scratch;  // Epi::kScratchBytes of shared memory private to the epilogue (both warpgroups)
+    int wg;          // consumer warpgroup (0, 1) that owns this tile
+    int it;          // how many tiles this warpgroup has finished before this one (double-buffer parity of the staging)
+    int next_tile;   // the tile this warpgroup processes next, or -1
 };
 template <class Epi>
 concept FragmentEpilogue = Epi::kFragmentView;
@@ -208,46 +211,11 @@ __device__ __forceinline__ void epi_chunks(const Acc& acc, const EpiCtx& c, Pre&
     acc.release();
 }
 
-// bf16 output tiles leave through TMA instead of 32 scattered rows per store instruction: a warp packs its 32 rows x 32
-// columns into a private staging buffer (SWIZZLE_64B layout: 16-byte chunk q of row r at r*64 + ((q ^ (r>>1)) & 3)*16,
-// conflict-free for row-per-lane 16-byte writes) and one lane issues cp.async.bulk.tensor.  Two buffers per warp.
-// Row-per-thread stores of 32 rows sit in the LSU queue and stall the warps on their source registers.
+// Row-view epilogues that move whole 32-row x 32-column bf16 tiles cooperatively stage them per warp (SWIZZLE_64B layout:
+// 16-byte chunk q of row r at r*64 + ((q ^ (r>>1)) & 3)*16, conflict-free for row-per-lane 16-byte accesses).  Row-per-thread
+// stores of 32 rows sit in the LSU queue and stall the warps on their source registers.
 constexpr int kTileStoreBufs = 2;                                  // staging tiles per warp (2 KB each)
 constexpr int kTileStoreBytes = kEpiWarps * kTileStoreBufs * 2048 + 1024;  // + alignment slack
-struct WarpTileStore {
-    uint8_t* buf;  // this warp's kTileStoreBufs x 2 KB (1024-byte aligned)
-    int nput;
-    __device__ __forceinline__ void attach(void* region, int warp_in_group) {
-        buf = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(region) + 1023) & ~uintptr_t(1023)) + warp_in_group * (kTileStoreBufs * 2048);
-    }
-    __device__ __forceinline__ void begin_tile(int lane) {
-        nput = 0;
-        if (lane == 0) bulk_wait_read<0>();
-        __syncwarp();
-    }
-    // w: this lane's row, 32 columns as 16 packed bf16 pairs; (col, row0) = global coordinates of the warp's tile
-    __device__ __forceinline__ void put(const CUtensorMap* tm, const uint32_t* w, int col, int row0, int lane) {
-        uint8_t* b = buf + (nput % kTileStoreBufs) * 2048;
-        if (nput >= kTileStoreBufs) {
-            if (lane == 0) bulk_wait_read<kTileStoreBufs - 1>();  // the store issued from this buffer has been read out
-            __syncwarp();
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-            *reinterpret_cast<uint4*>(b + lane * 64 + ((q ^ (lane >> 1)) & 3) * 16) =
-                make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-            tma_store_2d(tm, b, col, row0);
-            bulk_commit();
-        }
-        ++nput;
-    }
-    static __device__ __forceinline__ void drain(int lane) {  // before the CTA exits
-        if (lane == 0) bulk_wait_all();
-    }
-};
 
 // ---------------------------------------------------------------------------------------------
 // gemm_nt kernel: one CTA per (tile sequence, weight slice)
@@ -426,7 +394,8 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (tmr != nullptr) { const long long u = clock64(); tw_mma += u - t; t = u; }
             if constexpr (FragmentEpilogue<Epi>) {
                 const int row0 = tile * p.rows_per_tile;
-                epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), warp & 3, nch, col0, ncols, scratch});
+                epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), warp & 3, nch, col0, ncols, scratch, wg, it,
+                                      tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1});
             } else {
                 EpiCtx c;
                 c.tile = tile;
@@ -491,7 +460,8 @@ __global__ void __launch_bounds__(kEpiThreads, 1) gemm_nt_simt_epi_kernel(const 
                         acc[4 * j + 2 * e + i] = p.dbg_acc[(static_cast<size_t>(tile) * kTileM + 16 * wq + (lane >> 2) + 8 * e) * p.dbg_ld +
                                                            col0 + 8 * j + 2 * (lane & 3) + i];
             const int row0 = tile * p.rows_per_tile;
-            epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), wq, nch, col0, ncols, scratch});
+            epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), wq, nch, col0, ncols, scratch, wg, it,
+                                  tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1});
         } else {
             EpiCtx c;
             c.tile = tile;
