@@ -716,7 +716,7 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
     NR_REQUIRE(seg_len >= 1, "pool_dinput: seg_len=%d", seg_len);
     // the epilogue stages the dOut rows of every segment a tile touches: cap the slice width so that they fit
     const int nseg_max = kTileM / seg_len + 2;
-    const int max_stride = (EpiDPoolIn::kStageFloats / nseg_max) & ~15;
+    const int max_stride = (DOutStage::kStageFloats / nseg_max) & ~15;
     NR_REQUIRE(max_stride >= 16, "pool_dinput: seg_len=%d needs %d staged segments per tile", seg_len, nseg_max);
     NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
     GemmNTPlan plan;
@@ -735,7 +735,7 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
     EpiDPoolIn e{.w = c.w, .dout = c.dout, .ldo = c.ldo,
                  .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx, .N = D, .rm = to_rm(c.rm),
                  .zero_pad_rows = c.zero_pad_rows, .drop = to_drop(c.drop), .relu_src = static_cast<const __nv_bfloat16*>(c.relu_src),
-                 .relu_ld = c.relu_ld, .M = M, .rows_per_tile = kTileM};
+                 .relu_ld = c.relu_ld, .M = M};
     g_launches += debug_simt_gemm() ? 2 : 1;
     ProfScope ps("gemm_pool_dinput", M, D, g.K, stream);
     return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);

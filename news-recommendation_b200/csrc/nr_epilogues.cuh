@@ -60,6 +60,162 @@ struct Dropout {
         m[2] = ((hi & 0xffffu) >= thresh) ? scale : 0.f;
         m[3] = ((hi >> 16) >= thresh) ? scale : 0.f;
     }
+    // the same masks applied to one 32-column chunk of a wgmma fragment: y[4jj + 2e + i] is row[e], column col + 8jj +
+    // 2 (lane % 4) + i.  The mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of
+    // the same group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
+    __device__ __forceinline__ void apply_frag(float* y, const long long* row, int ld, int col) const {
+        const int lane = threadIdx.x & 31, b = lane & 1;
+        const long long my_row = b ? row[1] : row[0];
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int col4 = col + 8 * jj + 4 * ((lane >> 1) & 1);
+            const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
+            const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
+            const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
+            const uint32_t wd[2] = {b ? other : own, b ? own : other};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= thresh) ? scale : 0.f;
+                y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= thresh) ? scale : 0.f;
+            }
+        }
+    }
+};
+
+// SWIZZLE_64B layout of a tile with 64-byte rows (32 bf16): byte offset of 16-byte piece q of row r.  Eight consecutive
+// rows at the same q (the rows of one stmatrix matrix, or a row-per-lane 16-byte access) land in eight different bank groups.
+__device__ __forceinline__ int sw64_offset(int r, int q) { return r * 64 + ((q ^ (r >> 1)) & 3) * 16; }
+
+// A 32-column chunk of a fragment-view epilogue's output as bf16 pairs: w[2jj + e] holds row e of the lane, columns
+// 8jj + 2 (lane % 4) + {0, 1} of the chunk (the wgmma fragment's order).
+// Predicated stores straight from the fragment: row e goes to output row row[e] when ok[e], chunk column c to column col + c,
+// exactly the columns c < lim.
+__device__ __forceinline__ void store_frag_bf16(__nv_bfloat16* out, int ld, const long long* row, const bool* ok, int col, int lim,
+                                                const uint32_t* w) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int c = 8 * jj + 2 * (lane & 3);
+            if (!ok[e] || c >= lim) continue;
+            __nv_bfloat16* o = out + row[e] * ld + col + c;
+            if (c + 1 < lim) *reinterpret_cast<uint32_t*>(o) = w[2 * jj + e];
+            else *o = __ushort_as_bfloat16(static_cast<unsigned short>(w[2 * jj + e]));  // the pair's low half: column c
+        }
+}
+
+// The staging boxes of a fragment-view epilogue, built per tile by every lane of a consumer warp.  Each warp owns a ring of
+// kBoxes boxes of 16 rows x 32 bf16 (its rows of one chunk) in the SWIZZLE_64B layout; a chunk is packed into the next box
+// with two stmatrix and leaves by one lane's TMA store (send: rows >= M and columns past the map are clipped by the map) or
+// as 16-byte row pieces to mapped rows (put_rows).  With TMA the ring lets kBoxes - 1 of the warp's stores be in flight while
+// a box is written; the CTA's last ones are drained by finish().
+template <int kBoxes>
+struct FragStore {
+    static constexpr int kBoxBytes = 16 * 64;
+    static constexpr int kScratchBytes = kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    uint32_t ring;       // this warp's first box
+    uint32_t st_off[2];  // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8
+    int row;             // global row of the boxes' row 0
+    int tma;
+    int n = 0;           // chunks staged in this tile
+
+    // scratch: where the epilogue's boxes begin (aligned up to 1 KB here)
+    __device__ __forceinline__ FragStore(const float* scratch, const FragCtx& f, int use_tma)
+        : row(f.row0 + 16 * f.wq), tma(use_tma) {
+        const int lane = threadIdx.x & 31;
+        ring = ((smem_u32(scratch) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
+#pragma unroll
+        for (int x = 0; x < 2; ++x) {
+            const int m = lane >> 3;
+            st_off[x] = sw64_offset(8 * (m & 1) + (lane & 7), 2 * x + (m >> 1));
+        }
+        if (tma) {  // the previous tile's stores have left the boxes (the other warpgroup's MMAs ran in between)
+            if (lane == 0) bulk_wait_read<0>();
+            __syncwarp();
+        }
+    }
+    __device__ __forceinline__ uint32_t stage(const uint32_t* w) {
+        const uint32_t box = ring + (n % kBoxes) * kBoxBytes;
+        if (tma && n >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
+            if ((threadIdx.x & 31) == 0) bulk_wait_read<kBoxes - 1>();
+            __syncwarp();
+        }
+        stmatrix_x4(box + st_off[0], w[0], w[1], w[2], w[3]);
+        stmatrix_x4(box + st_off[1], w[4], w[5], w[6], w[7]);
+        ++n;
+        return box;
+    }
+    __device__ __forceinline__ void send(const CUtensorMap* tm, const uint32_t* w, int col) {
+        const uint32_t box = stage(w);
+        fence_proxy_async();
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) {
+            tma_store_2d(tm, box, col, row);
+            bulk_commit();
+        }
+    }
+    // row r of the box leaves as 4 x 16 bytes to output row orow[r / 8] (when v[r / 8]), lane = 4 (r % 8) + piece: each lane
+    // writes its own rows.  The next put_rows' __syncwarp orders these reads before the box is written again (kBoxes >= 2).
+    __device__ __forceinline__ void put_rows(__nv_bfloat16* out, int ld, const long long* orow, const bool* v, const uint32_t* w,
+                                             int col) {
+        const int lane = threadIdx.x & 31;
+        const uint32_t box = stage(w);
+        __syncwarp();
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int q = lane & 3;
+            const uint4 u = lds_u4(box + sw64_offset((lane >> 2) + 8 * e, q));
+            if (v[e]) *(reinterpret_cast<uint4*>(out + orow[e] * ld + col) + q) = u;
+        }
+    }
+    // end of the CTA's tile loop (every consumer thread)
+    static __device__ __forceinline__ void finish(const EpiInit& e) {
+        if ((e.tid & 31) == 0) bulk_wait_all();
+    }
+};
+
+// The dOut rows a pool-backward tile reads, staged per warpgroup in shared memory: every segment the 64-row tile touches
+// (<= 64/seg_len + 2), slice columns only, [segment][pitch round_up(ncols, 4)] so that every staged row is 16-byte aligned.
+// Two buffers of kStageFloats per warpgroup: the one of the warpgroup's NEXT tile is filled by cp.async while this one is read.
+struct DOutStage {
+    static constexpr int kStageFloats = 1536;
+    static constexpr int kScratchBytes = 4 * kStageFloats * 4;
+    const float* dout;  // [segments][ldo]
+    int ldo;
+    int seg_len;
+    int M;
+
+    static __device__ __forceinline__ int pitch(int ncols) { return (ncols + 3) & ~3; }
+    // the 128 threads of a warpgroup (wtid): queue the dOut rows of `tile` (columns [col0, col0 + ncols)) into buf
+    __device__ __forceinline__ void stage_tile(int tile, int col0, int ncols, int wtid, float* buf) const {
+        const int row0 = tile * kTileM, sp = pitch(ncols);
+        const int seg_first = row0 / seg_len;
+        const int seg_last = min(row0 + kTileM - 1, M - 1) / seg_len;
+        const int total = (seg_last - seg_first + 1) * sp;
+        for (int i = wtid; i < total; i += kWgThreads) {
+            const int sgi = i / sp, j = i - sgi * sp;
+            const bool ok = j < ncols;
+            cp_async_f32(buf + i, dout + static_cast<size_t>(seg_first + sgi) * ldo + (ok ? col0 + j : 0), ok);
+        }
+        cp_async_commit();
+    }
+    __device__ __forceinline__ void init(const EpiInit& e, int tile_step) const {  // each warpgroup queues its own first tile
+        const int wg = e.tid >> 7, first = e.first_tile + wg * tile_step;
+        if (first < e.num_tiles) stage_tile(first, e.col0, e.ncols, e.tid & 127, e.scratch + 2 * wg * kStageFloats);
+    }
+    // per tile, the whole warpgroup: wait for this tile's rows and queue the next tile's; returns this tile's buffer
+    __device__ __forceinline__ const float* begin(float* scratch, int wg, int it, int next_tile, int col0, int ncols) const {
+        float* mine = scratch + 2 * wg * kStageFloats;
+        cp_async_wait_all();
+        epi_bar_sync(wg);  // this tile's dOut rows are visible; the warpgroup is done with its other buffer
+        if (next_tile >= 0) stage_tile(next_tile, col0, ncols, threadIdx.x & 127, mine + ((it + 1) & 1) * kStageFloats);
+        return mine + (it & 1) * kStageFloats;
+    }
+    // the staged dOut row of global row grow, in the tile whose first row is row0 (the first staged row when !valid)
+    __device__ __forceinline__ const float* row(const float* buf, int row0, int grow, bool valid, int ncols) const {
+        return buf + (valid ? grow / seg_len - row0 / seg_len : 0) * pitch(ncols);
+    }
 };
 
 __device__ __forceinline__ bool aligned32(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 31) == 0; }
@@ -81,16 +237,13 @@ __device__ __forceinline__ void store_bf16x8(__nv_bfloat16* o, const float* y, i
 // wgmma fragment, with no transpose and no barrier across warps.  A 32-column bf16 chunk is packed into one of the warp's
 // staging boxes with stmatrix and leaves by TMA (identity rows) or as 16-byte row pieces (mapped rows); fp32 output and bf16
 // chunks cut by the slice's end leave from the fragment, a quad of lanes covering 8 contiguous columns of a row.
-// scratch: [0, 1 KB) bias of the slice (zero past ncols) | kBoxes staging boxes per consumer warp (1 KB aligned)
+// scratch: [0, 1 KB) bias of the slice (zero past ncols) | the staging boxes (FragStore, 1 KB aligned)
 // ------------------------------------------------------------------------------------------------
 struct EpiStore {
     static constexpr bool kFragmentView = true;
-    // a box is 16 rows x 32 bf16 in the SWIZZLE_64B layout (16-byte piece q of row r at r*64 + ((q ^ (r>>1)) & 3)*16: the eight
-    // rows of one stmatrix matrix land in eight different bank groups).  A slice issues up to 2 x 8 stores per tile; the ring
-    // lets six of them be in flight before a box is reused.
-    static constexpr int kBoxBytes = 16 * 64;
-    static constexpr int kBoxes = 6;
-    static constexpr int kScratchBytes = 1024 + kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    // a slice issues up to 2 x 8 stores per tile; the ring lets six of them be in flight before a box is reused
+    using Store = FragStore<6>;
+    static constexpr int kScratchBytes = 1024 + Store::kScratchBytes;
     CUtensorMap tm_out;  // bf16 output as a TMA tensor (32 x 16 boxes, SWIZZLE_64B); valid when use_tma
     CUtensorMap tm_lo;   // low plane of the columns >= lo_col0 (bf16(y - bf16(y))), its column 0 = output column lo_col0
     int accumulate;      // fp32 output only: out += result
@@ -115,7 +268,7 @@ struct EpiStore {
         consumers_bar_sync();
     }
     __device__ void finish(const EpiInit& e) const {
-        if (use_tma && (e.tid & 31) == 0) bulk_wait_all();
+        if (use_tma) Store::finish(e);
     }
 
     __device__ __forceinline__ void frag(const float* acc, const FragCtx& f) const {
@@ -132,84 +285,33 @@ struct EpiStore {
             int t;
             v[e] = rm.map(f.row0 + r, orow[e], t) && r < f.rows;
         }
-        const uint32_t ring = ((smem_u32(f.scratch + 256) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
-        // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8 addressing row lane % 8
-        uint32_t st_off[2];
-#pragma unroll
-        for (int x = 0; x < 2; ++x) {
-            const int m = lane >> 3, jj = 2 * x + (m >> 1), r = 8 * (m & 1) + (lane & 7);
-            st_off[x] = r * 64 + ((jj ^ (r >> 1)) & 3) * 16;
-        }
-        if (use_tma) {  // the previous tile's stores have left the boxes (the other warpgroup's MMAs ran in between)
-            if (lane == 0) bulk_wait_read<0>();
-            __syncwarp();
-        }
-        int nbox = 0;
-        // w[k] = bf16 pair (2k, 2k+1) of the chunk's 16 values: fragment group jj = k / 2, row e = k % 2
-        auto stage = [&](const uint32_t* w) {
-            const uint32_t box = ring + (nbox % kBoxes) * kBoxBytes;
-            if (use_tma && nbox >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
-                if (lane == 0) bulk_wait_read<kBoxes - 1>();
-                __syncwarp();
-            }
-            stmatrix_x4(box + st_off[0], w[0], w[1], w[2], w[3]);
-            stmatrix_x4(box + st_off[1], w[4], w[5], w[6], w[7]);
-            ++nbox;
-            return box;
+        Store st(f.scratch + 256, f, use_tma);
+        // a bf16 chunk of 32 output columns from column col: a chunk cut by the slice's end leaves from the fragment with
+        // predicated stores, which write exactly the columns < ncols (letting the tensor map clip it at N changed the outputs
+        // where N % 16 != 0)
+        auto put = [&](__nv_bfloat16* base, int ldo, const CUtensorMap* tm, const uint32_t* w, int lc0, int col) {
+            if (lc0 + 32 > f.ncols) store_frag_bf16(base, ldo, orow, v, col, f.ncols - lc0, w);  // warp-uniform
+            else if (use_tma) st.send(tm, w, col);
+            else st.put_rows(base, ldo, orow, v, w, col);
         };
-        auto put_tma = [&](const CUtensorMap* tm, const uint32_t* w, int col) {  // rows >= M, columns >= N: clipped by the map
-            const uint32_t box = stage(w);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-                tma_store_2d(tm, box, col, f.row0 + 16 * f.wq);
-                bulk_commit();
-            }
-        };
-        // mapped rows: row r of the box leaves as 4 x 16 bytes, lane = 4 (r % 8) + piece owns row e = r / 8 (its own rows);
-        // the next stage() call's stmatrix is ordered after these reads by its __syncwarp (kBoxes >= 2)
-        auto put_rows = [&](__nv_bfloat16* base, int ldo, const uint32_t* w, int col) {
-            const uint32_t box = stage(w);
-            __syncwarp();
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int r = (lane >> 2) + 8 * e, q = lane & 3;
-                const uint4 u = lds_u4(box + r * 64 + ((q ^ (r >> 1)) & 3) * 16);
-                if (v[e]) *(reinterpret_cast<uint4*>(base + orow[e] * ldo + col) + q) = u;
-            }
-        };
-        auto put_direct = [&](const float* y, int lc0) {  // y[4jj + 2e + i]: row e, slice column lc0 + 8jj + 2 (lane % 4) + i
+        auto put_f32 = [&](const float* y, int lc0) {  // y[4jj + 2e + i]: row e, slice column lc0 + 8jj + 2 (lane % 4) + i
 #pragma unroll
             for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int lc = lc0 + 8 * jj + 2 * (lane & 3);
                     if (!v[e] || lc >= f.ncols) continue;
-                    const bool two = lc + 1 < f.ncols;
                     const float y0 = y[4 * jj + 2 * e], y1 = y[4 * jj + 2 * e + 1];
-                    const int col = f.col0 + lc;
-                    if (out_bf16) {
-                        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out) + orow[e] * ld + col;
-                        if (two) *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y0, y1);
-                        else *o = __float2bfloat16_rn(y0);
-                        if (lo_col0 >= 0 && col >= lo_col0) {
-                            const float l0 = y0 - bf16_round(y0), l1 = y1 - bf16_round(y1);
-                            __nv_bfloat16* ol = lo_out + orow[e] * ld_lo + (col - lo_col0);
-                            if (two) *reinterpret_cast<uint32_t*>(ol) = pack_bf16x2(l0, l1);
-                            else *ol = __float2bfloat16_rn(l0);
+                    float* o = static_cast<float*>(out) + orow[e] * ld + f.col0 + lc;
+                    if (lc + 1 < f.ncols) {
+                        float2 r = make_float2(y0, y1);
+                        if (accumulate) {  // out += : second pass of a split-operand product (x_lo . W^T on top of x_hi . W^T)
+                            const float2 o2 = *reinterpret_cast<const float2*>(o);
+                            r.x += o2.x; r.y += o2.y;
                         }
+                        *reinterpret_cast<float2*>(o) = r;
                     } else {
-                        float* o = static_cast<float*>(out) + orow[e] * ld + col;
-                        if (two) {
-                            float2 r = make_float2(y0, y1);
-                            if (accumulate) {  // out += : second pass of a split-operand product (x_lo . W^T on top of x_hi . W^T)
-                                const float2 o2 = *reinterpret_cast<const float2*>(o);
-                                r.x += o2.x; r.y += o2.y;
-                            }
-                            *reinterpret_cast<float2*>(o) = r;
-                        } else {
-                            *o = accumulate ? *o + y0 : y0;
-                        }
+                        *o = accumulate ? *o + y0 : y0;
                     }
                 }
         };
@@ -229,45 +331,23 @@ struct EpiStore {
 #pragma unroll
                     for (int k = 0; k < 16; ++k) y[k] = fmaxf(y[k], 0.f);
                 }
-                if (drop.p > 0.f) {
-                    // the mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of the same
-                    // group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
-                    const int b = lane & 1;
-                    const long long my_row = b ? orow[1] : orow[0];
-#pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        const int col4 = f.col0 + lc0 + 8 * jj + 4 * ((lane >> 1) & 1);
-                        const uint64_t bits = dropout_bits4(drop.seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
-                        const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
-                        const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
-                        const uint32_t wd[2] = {b ? other : own, b ? own : other};
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= drop.thresh) ? drop.scale : 0.f;
-                            y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= drop.thresh) ? drop.scale : 0.f;
-                        }
-                    }
-                }
-                // a chunk cut by the slice's end leaves from the fragment with predicated stores, which write exactly the
-                // columns < ncols (letting the tensor map clip it at N changed the outputs where N % 16 != 0)
-                const bool staged = out_bf16 && lc0 + 32 <= f.ncols;  // warp-uniform
-                if (staged) {
+                if (drop.p > 0.f) drop.apply_frag(y, orow, ld, f.col0 + lc0);
+                if (out_bf16) {
+                    const int col = f.col0 + lc0;
                     uint32_t w[8];
 #pragma unroll
                     for (int k = 0; k < 8; ++k) w[k] = pack_bf16x2(y[2 * k], y[2 * k + 1]);
-                    if (use_tma) put_tma(&tm_out, w, f.col0 + lc0);
-                    else put_rows(static_cast<__nv_bfloat16*>(out), ld, w, f.col0 + lc0);
-                    if (lo_col0 >= 0 && f.col0 + lc0 >= lo_col0) {  // warp-uniform (the host checked the chunk alignment)
+                    put(static_cast<__nv_bfloat16*>(out), ld, &tm_out, w, lc0, col);
+                    if (lo_col0 >= 0 && col >= lo_col0) {  // warp-uniform (the host checked the chunk alignment)
 #pragma unroll
                         for (int k = 0; k < 8; ++k) {
                             const float2 h = unpack_bf16x2(w[k]);
                             w[k] = pack_bf16x2(y[2 * k] - h.x, y[2 * k + 1] - h.y);
                         }
-                        if (use_tma) put_tma(&tm_lo, w, f.col0 + lc0 - lo_col0);
-                        else put_rows(lo_out, ld_lo, w, f.col0 + lc0 - lo_col0);
+                        put(lo_out, ld_lo, &tm_lo, w, lc0, col - lo_col0);
                     }
                 } else {
-                    put_direct(y, lc0);
+                    put_f32(y, lc0);
                 }
             }
         }
@@ -419,13 +499,12 @@ struct EpiPool {
 // chunk are reduced over the warp's rows with a 7-shuffle butterfly and added to shared memory, one column per lane.
 // The output tensor map spans the whole pitch ld: the columns in [ncols, ld) are written as exact zeros (bias and query
 // vector are zero there), so GEMMs that read dPre with K = ld see zero padding.
-// scratch floats: [0,256) column sums | [256,512) bias | [512,768) query vector | kBoxes staging boxes per consumer warp
+// scratch floats: [0,256) column sums | [256,512) bias | [512,768) query vector | the staging boxes (FragStore)
 // ------------------------------------------------------------------------------------------------
 struct EpiDPre {
     static constexpr bool kFragmentView = true;
-    static constexpr int kBoxBytes = 16 * 64;  // 16 rows x 32 bf16, SWIZZLE_64B (as EpiStore)
-    static constexpr int kBoxes = 4;           // a smaller ring than EpiStore's keeps six A stages beside a 224 x 320 weight slice
-    static constexpr int kScratchBytes = 3072 + kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    using Store = FragStore<4>;  // a smaller ring than EpiStore's keeps six A stages beside a 224 x 320 weight slice
+    static constexpr int kScratchBytes = 3072 + Store::kScratchBytes;
     CUtensorMap tm_out;       // dpre as a TMA tensor ([rows][ld], 32 x 16 boxes, SWIZZLE_64B); valid when use_tma
     int use_tma;
     const float* bias;
@@ -446,7 +525,7 @@ struct EpiDPre {
     __device__ void finish(const EpiInit& e) const {
         consumers_bar_sync();  // both warpgroups' column sums are in; one add per column and CTA
         for (int i = e.tid; i < e.ncols; i += kEpiThreads) atomicAdd(dqv + e.col0 + i, e.scratch[i]);
-        if (use_tma && (e.tid & 31) == 0) bulk_wait_all();
+        if (use_tma) Store::finish(e);
     }
 
     __device__ __forceinline__ void frag(const float* acc, const FragCtx& f) const {
@@ -455,23 +534,15 @@ struct EpiDPre {
         // the tensor map clips them at the last row)
         float ds[2];
         long long grow[2];
+        bool v[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             const int r = 16 * f.wq + (lane >> 2) + 8 * e;
             grow[e] = static_cast<long long>(f.row0) + r;
-            ds[e] = r < f.rows ? __ldg(dscore + grow[e]) : 0.f;
+            v[e] = r < f.rows;
+            ds[e] = v[e] ? __ldg(dscore + grow[e]) : 0.f;
         }
-        const uint32_t ring = ((smem_u32(f.scratch + 768) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
-        uint32_t st_off[2];  // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8
-#pragma unroll
-        for (int x = 0; x < 2; ++x) {
-            const int m = lane >> 3, jj = 2 * x + (m >> 1), r = 8 * (m & 1) + (lane & 7);
-            st_off[x] = r * 64 + ((jj ^ (r >> 1)) & 3) * 16;
-        }
-        if (use_tma) {  // the previous tile's stores have left the boxes
-            if (lane == 0) bulk_wait_read<0>();
-            __syncwarp();
-        }
+        Store st(f.scratch + 768, f, use_tma);
         const int b2 = (lane >> 2) & 1, b3 = (lane >> 3) & 1, b4 = (lane >> 4) & 1;
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
@@ -493,30 +564,8 @@ struct EpiDPre {
                     s[2 * jj] = fmaf(ds[0], t[0][0], ds[1] * t[1][0]);
                     s[2 * jj + 1] = fmaf(ds[0], t[0][1], ds[1] * t[1][1]);
                 }
-                if (use_tma) {
-                    const uint32_t box = ring + (q % kBoxes) * kBoxBytes;
-                    if (q >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
-                        if (lane == 0) bulk_wait_read<kBoxes - 1>();
-                        __syncwarp();
-                    }
-                    stmatrix_x4(box + st_off[0], w[0], w[1], w[2], w[3]);
-                    stmatrix_x4(box + st_off[1], w[4], w[5], w[6], w[7]);
-                    fence_proxy_async();
-                    __syncwarp();
-                    if (lane == 0) {  // rows >= M and columns >= ld are clipped by the map
-                        tma_store_2d(&tm_out, box, f.col0 + lc0, f.row0 + 16 * f.wq);
-                        bulk_commit();
-                    }
-                } else {
-#pragma unroll
-                    for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            const int col = f.col0 + lc0 + 8 * jj + 2 * (lane & 3);  // even: a pair never straddles ld
-                            if (16 * f.wq + (lane >> 2) + 8 * e < f.rows && col < ld)
-                                *reinterpret_cast<uint32_t*>(dpre + grow[e] * ld + col) = w[2 * jj + e];
-                        }
-                }
+                if (use_tma) st.send(&tm_out, w, f.col0 + lc0);  // columns >= ld are clipped by the map
+                else store_frag_bf16(dpre, ld, grow, v, f.col0 + lc0, ld - f.col0 - lc0, w);  // even: a pair never straddles ld
                 // column sums over the warp's 16 rows: reduce-scatter across lane bits 4, 3, 2 (the lanes holding the same
                 // columns); lane ends with the sum of column 8 (2 b4 + b3) + 2 (lane % 4) + b2
                 float s1[4], s2[2];
@@ -534,13 +583,10 @@ struct EpiDPre {
 // ------------------------------------------------------------------------------------------------
 // dX_rc = acc_rc + w_r * dOut[seg(r)][c]  (pool backward, both paths into X) [* relu mask] [* dropout] -> bf16
 // Row view, for a row-mapped destination and/or a ReLU mask (the CNN encoders); the identity / no-mask case is EpiDPoolInFrag.
-// scratch floats: two staging buffers of kStageFloats per warpgroup: the dOut rows (slice columns only) of every segment
-// the tile touches (<= 64/seg_len + 2), [segment][pitch = slice width]; the buffer of the warpgroup's NEXT tile is filled by
-// cp.async while this one is used.
+// scratch: the dOut rows (DOutStage) | kTileStoreBufs staging tiles per consumer warp (1 KB aligned)
 // ------------------------------------------------------------------------------------------------
 struct EpiDPoolIn {
-    static constexpr int kStageFloats = 1536;
-    static constexpr int kScratchBytes = 4 * kStageFloats * 4 + kTileStoreBytes;
+    static constexpr int kScratchBytes = DOutStage::kScratchBytes + kTileStoreBytes;
     const float* w;      // [rows]
     const float* dout;   // [segments][ldo]
     int ldo;
@@ -554,25 +600,8 @@ struct EpiDPoolIn {
     const __nv_bfloat16* relu_src;  // non-null: multiply by (relu_src[r][c] > 0) (ReLU backward of the CNN); pitch relu_ld
     int relu_ld;
     int M;
-    int rows_per_tile;
 
-    // the 128 threads of a warpgroup (wtid): queue the dOut rows of `tile` (columns [col0, col0 + ncols)) into buf
-    __device__ __forceinline__ void stage_tile(int tile, int col0, int ncols, int wtid, float* buf) const {
-        const int row0 = tile * rows_per_tile;
-        const int seg_first = row0 / seg_len;
-        const int seg_last = min(row0 + kTileM - 1, M - 1) / seg_len;
-        const int total = (seg_last - seg_first + 1) * ncols;
-        for (int i = wtid; i < total; i += kWgThreads) {
-            const int sgi = i / ncols, j = i - sgi * ncols;
-            const bool ok = col0 + j < N;
-            cp_async_f32(buf + i, dout + static_cast<size_t>(seg_first + sgi) * ldo + (ok ? col0 + j : 0), ok);
-        }
-        cp_async_commit();
-    }
-    __device__ void init(const EpiInit& e, int tile_step) const {  // each warpgroup queues its own first tile
-        const int wg = e.tid >> 7, first = e.first_tile + wg * tile_step;
-        if (first < e.num_tiles) stage_tile(first, e.col0, e.ncols, e.tid & 127, e.scratch + 2 * wg * kStageFloats);
-    }
+    __device__ void init(const EpiInit& e, int tile_step) const { DOutStage{dout, ldo, seg_len, M}.init(e, tile_step); }
     __device__ void finish(const EpiInit&) const {}
 
     template <class Acc>
@@ -581,14 +610,8 @@ struct EpiDPoolIn {
         int t;
         const bool v = rm.map(c.grow, orow, t) && c.valid;
         const float wr = c.valid ? __ldg(w + c.grow) : 0.f;
-        const int seg_first = (c.tile * rows_per_tile) / seg_len;
-        const int myseg = (c.valid ? c.grow / seg_len : seg_first) - seg_first;
-        float* mine = c.scratch + 2 * c.wg * kStageFloats;
-        float* cur = mine + (c.it & 1) * kStageFloats;
-        cp_async_wait_all();
-        epi_bar_sync(c.wg);  // this tile's dOut rows are visible; the warpgroup is done with its other buffer
-        if (c.next_tile >= 0) stage_tile(c.next_tile, c.col0, c.ncols, c.wtid, mine + ((c.it + 1) & 1) * kStageFloats);
-        const float* sd = cur + myseg * c.ncols;
+        const DOutStage dst{dout, ldo, seg_len, M};
+        const float* sd = dst.row(dst.begin(c.scratch, c.wg, c.it, c.next_tile, c.col0, c.ncols), c.grow - c.r, c.grow, c.valid, c.ncols);
         const int lane = c.tid & 31;
         epi_chunks(
             acc, c, [](int) {},
@@ -601,7 +624,8 @@ struct EpiDPoolIn {
                 const bool coop = ch * 32 + 32 <= c.ncols && col + 32 <= N && (col & 7) == 0 && (ld & 7) == 0 &&
                                   (relu_src == nullptr || (relu_ld & 7) == 0);  // warp-uniform
                 if (coop) {
-                    uint8_t* stage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(c.scratch + 4 * kStageFloats) + 1023) & ~uintptr_t(1023)) +
+                    uint8_t* stage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(c.scratch + DOutStage::kScratchBytes / 4) + 1023) &
+                                                                ~uintptr_t(1023)) +
                                      (c.tid >> 5) * (kTileStoreBufs * 2048);
                     uint8_t* rb = stage;          // mask tile  (32 rows x 64 bytes, SWIZZLE_64B like WarpTileStore)
                     uint8_t* ob = stage + 2048;   // result tile
@@ -612,21 +636,20 @@ struct EpiDPoolIn {
                             const int r = (lane >> 2) + 8 * k, q = lane & 3;
                             const long long gr = row0 + r;
                             const uint4 u = gr < M ? __ldg(reinterpret_cast<const uint4*>(relu_src + gr * relu_ld + col) + q) : make_uint4(0, 0, 0, 0);
-                            *reinterpret_cast<uint4*>(rb + r * 64 + ((q ^ (r >> 1)) & 3) * 16) = u;
+                            *reinterpret_cast<uint4*>(rb + sw64_offset(r, q)) = u;
                         }
                         __syncwarp();
                     }
-                    const float* sdc = c.valid ? sd + ch * 32 : cur;
 #pragma unroll
                     for (int j = 0; j < 32; j += 4) {
-                        const float4 d4 = lds_f4(sdc + j);
+                        const float4 d4 = lds_f4(sd + ch * 32 + j);
                         x[j] = fmaf(wr, d4.x, x[j]); x[j + 1] = fmaf(wr, d4.y, x[j + 1]);
                         x[j + 2] = fmaf(wr, d4.z, x[j + 2]); x[j + 3] = fmaf(wr, d4.w, x[j + 3]);
                     }
                     if (relu_src != nullptr) {
 #pragma unroll
                         for (int q = 0; q < 4; ++q) {
-                            const uint4 ru = *reinterpret_cast<const uint4*>(rb + lane * 64 + ((q ^ (lane >> 1)) & 3) * 16);
+                            const uint4 ru = *reinterpret_cast<const uint4*>(rb + sw64_offset(lane, q));
                             const uint32_t rw[4] = {ru.x, ru.y, ru.z, ru.w};
 #pragma unroll
                             for (int j = 0; j < 4; ++j) {
@@ -648,7 +671,7 @@ struct EpiDPoolIn {
                     }
 #pragma unroll
                     for (int q = 0; q < 4; ++q)
-                        *reinterpret_cast<uint4*>(ob + lane * 64 + ((q ^ (lane >> 1)) & 3) * 16) =
+                        *reinterpret_cast<uint4*>(ob + sw64_offset(lane, q)) =
                             make_uint4(pack_bf16x2(x[8 * q], x[8 * q + 1]), pack_bf16x2(x[8 * q + 2], x[8 * q + 3]),
                                        pack_bf16x2(x[8 * q + 4], x[8 * q + 5]), pack_bf16x2(x[8 * q + 6], x[8 * q + 7]));
                     __syncwarp();
@@ -659,7 +682,7 @@ struct EpiDPoolIn {
                         const int orr = __shfl_sync(0xffffffffu, my_orow, r);
                         if (orr >= 0)
                             *(reinterpret_cast<uint4*>(dx + static_cast<long long>(orr) * ld + col) + q) =
-                                *reinterpret_cast<const uint4*>(ob + r * 64 + ((q ^ (r >> 1)) & 3) * 16);
+                                *reinterpret_cast<const uint4*>(ob + sw64_offset(r, q));
                     }
                     __syncwarp();
                     return;
@@ -672,7 +695,7 @@ struct EpiDPoolIn {
                     const int col = c.col0 + lc;
                     const int nvalid = min(8, min(c.ncols - lc, N - col));
                     float dd[8];
-                    if (((c.ncols & 3) == 0) && lc + 8 <= c.ncols) {
+                    if (lc + 8 <= c.ncols) {
                         const float4 d0 = lds_f4(sd + lc), d1 = lds_f4(sd + lc + 4);
                         dd[0] = d0.x; dd[1] = d0.y; dd[2] = d0.z; dd[3] = d0.w;
                         dd[4] = d1.x; dd[5] = d1.y; dd[6] = d1.z; dd[7] = d1.w;
@@ -730,16 +753,13 @@ struct EpiDPoolIn {
 //   dX_rc = acc_rc + w_r * dOut[seg(r)][c] [* dropout] -> bf16
 // Fragment view, as EpiStore: each warp works on its 16 rows of the tile straight from the wgmma fragment and a whole 32-column
 // chunk leaves through a staging box (stmatrix) and TMA; a chunk cut by the slice's end leaves from the fragment with
-// predicated stores.  The dOut rows are staged per warpgroup exactly as in EpiDPoolIn (double buffer, cp.async one tile ahead),
-// at a pitch of round_up(ncols, 4) floats.
-// scratch: 4 x kStageFloats floats (two staging buffers per warpgroup) | kBoxes staging boxes per consumer warp (1 KB aligned)
+// predicated stores.  The dOut rows are staged as in EpiDPoolIn.
+// scratch: the dOut rows (DOutStage) | the staging boxes (FragStore, 1 KB aligned)
 // ------------------------------------------------------------------------------------------------
 struct EpiDPoolInFrag {
     static constexpr bool kFragmentView = true;
-    static constexpr int kStageFloats = EpiDPoolIn::kStageFloats;
-    static constexpr int kBoxBytes = 16 * 64;
-    static constexpr int kBoxes = 6;
-    static constexpr int kScratchBytes = 4 * kStageFloats * 4 + kEpiWarps * kBoxes * kBoxBytes + 1024;  // + alignment slack
+    using Store = FragStore<6>;
+    static constexpr int kScratchBytes = DOutStage::kScratchBytes + Store::kScratchBytes;
     CUtensorMap tm_out;  // dx as a TMA tensor (32 x 16 boxes, SWIZZLE_64B)
     const float* w;      // [rows]
     const float* dout;   // [segments][ldo]
@@ -751,35 +771,13 @@ struct EpiDPoolInFrag {
     Dropout drop;
     int M;
 
-    // the 128 threads of a warpgroup (wtid): queue the dOut rows of `tile` (columns [col0, col0 + ncols)) into buf, pitch sp
-    __device__ __forceinline__ void stage_tile(int tile, int col0, int ncols, int wtid, float* buf) const {
-        const int row0 = tile * kTileM, sp = (ncols + 3) & ~3;
-        const int seg_first = row0 / seg_len;
-        const int seg_last = min(row0 + kTileM - 1, M - 1) / seg_len;
-        const int total = (seg_last - seg_first + 1) * sp;
-        for (int i = wtid; i < total; i += kWgThreads) {
-            const int sgi = i / sp, j = i - sgi * sp;
-            const bool ok = j < ncols;
-            cp_async_f32(buf + i, dout + static_cast<size_t>(seg_first + sgi) * ldo + (ok ? col0 + j : 0), ok);
-        }
-        cp_async_commit();
-    }
-    __device__ void init(const EpiInit& e, int tile_step) const {  // each warpgroup queues its own first tile
-        const int wg = e.tid >> 7, first = e.first_tile + wg * tile_step;
-        if (first < e.num_tiles) stage_tile(first, e.col0, e.ncols, e.tid & 127, e.scratch + 2 * wg * kStageFloats);
-    }
-    __device__ void finish(const EpiInit& e) const {
-        if ((e.tid & 31) == 0) bulk_wait_all();
-    }
+    __device__ void init(const EpiInit& e, int tile_step) const { DOutStage{dout, ldo, seg_len, M}.init(e, tile_step); }
+    __device__ void finish(const EpiInit& e) const { Store::finish(e); }
 
     __device__ __forceinline__ void frag(const float* acc, const FragCtx& f) const {
         const int lane = threadIdx.x & 31;
-        float* mine = f.scratch + 2 * f.wg * kStageFloats;
-        const float* cur = mine + (f.it & 1) * kStageFloats;
-        cp_async_wait_all();
-        named_bar_sync(kBarWg + f.wg, kWgThreads);  // this tile's dOut rows are visible; the warpgroup is done with its other buffer
-        if (f.next_tile >= 0) stage_tile(f.next_tile, f.col0, f.ncols, threadIdx.x & 127, mine + ((f.it + 1) & 1) * kStageFloats);
-        const int sp = (f.ncols + 3) & ~3, seg_first = f.row0 / seg_len;
+        const DOutStage dst{dout, ldo, seg_len, M};
+        const float* cur = dst.begin(f.scratch, f.wg, f.it, f.next_tile, f.col0, f.ncols);
         // this lane's rows e = 0, 1: tile row 16 wq + lane / 4 + 8e
         bool v[2];
         float wr[2];
@@ -791,18 +789,9 @@ struct EpiDPoolInFrag {
             grow[e] = static_cast<long long>(f.row0) + r;
             v[e] = r < f.rows;
             wr[e] = v[e] ? __ldg(w + grow[e]) : 0.f;
-            sd[e] = cur + (v[e] ? static_cast<int>(grow[e] / seg_len) - seg_first : 0) * sp;
+            sd[e] = dst.row(cur, f.row0, f.row0 + r, v[e], f.ncols);
         }
-        const uint32_t ring = ((smem_u32(f.scratch + 4 * kStageFloats) + 1023u) & ~1023u) + (threadIdx.x >> 5) * (kBoxes * kBoxBytes);
-        uint32_t st_off[2];  // stmatrix x of a chunk writes the 8 x 8 matrices (jj, e) = (2x + m/2, m%2), m = lane / 8
-#pragma unroll
-        for (int x = 0; x < 2; ++x) {
-            const int m = lane >> 3, jj = 2 * x + (m >> 1), r = 8 * (m & 1) + (lane & 7);
-            st_off[x] = r * 64 + ((jj ^ (r >> 1)) & 3) * 16;
-        }
-        if (lane == 0) bulk_wait_read<0>();  // the previous tile's stores have left the boxes
-        __syncwarp();
-        int nbox = 0;
+        Store st(f.scratch + DOutStage::kScratchBytes / 4, f, 1);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
             if (q < f.nch) {  // a compile-time chunk index keeps the fragment in registers
@@ -818,55 +807,12 @@ struct EpiDPoolInFrag {
                         y[4 * jj + 2 * e + 1] = fmaf(wr[e], d.y, acc[16 * q + 4 * jj + 2 * e + 1]);
                     }
                 }
-                if (drop.p > 0.f) {
-                    // the mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of the same
-                    // group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
-                    const int b = lane & 1;
-                    const long long my_row = b ? grow[1] : grow[0];
+                if (drop.p > 0.f) drop.apply_frag(y, grow, ld, f.col0 + lc0);
+                uint32_t wp[8];
 #pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        const int col4 = f.col0 + lc0 + 8 * jj + 4 * ((lane >> 1) & 1);
-                        const uint64_t bits = dropout_bits4(drop.seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
-                        const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
-                        const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
-                        const uint32_t wd[2] = {b ? other : own, b ? own : other};
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= drop.thresh) ? drop.scale : 0.f;
-                            y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= drop.thresh) ? drop.scale : 0.f;
-                        }
-                    }
-                }
-                if (lc0 + 32 <= f.ncols) {  // warp-uniform; rows >= M are clipped by the tensor map
-                    uint32_t wp[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) wp[k] = pack_bf16x2(y[2 * k], y[2 * k + 1]);
-                    const uint32_t box = ring + (nbox % kBoxes) * kBoxBytes;
-                    if (nbox >= kBoxes) {  // the store issued from this box kBoxes stores ago has been read out
-                        if (lane == 0) bulk_wait_read<kBoxes - 1>();
-                        __syncwarp();
-                    }
-                    stmatrix_x4(box + st_off[0], wp[0], wp[1], wp[2], wp[3]);
-                    stmatrix_x4(box + st_off[1], wp[4], wp[5], wp[6], wp[7]);
-                    ++nbox;
-                    fence_proxy_async();
-                    __syncwarp();
-                    if (lane == 0) {
-                        tma_store_2d(&tm_out, box, f.col0 + lc0, f.row0 + 16 * f.wq);
-                        bulk_commit();
-                    }
-                } else {  // the slice's last chunk: exactly the columns < ncols
-#pragma unroll
-                    for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            const int lc = lc0 + 8 * jj + 2 * (lane & 3);
-                            if (!v[e] || lc >= f.ncols) continue;
-                            __nv_bfloat16* o = dx + grow[e] * ld + f.col0 + lc;
-                            if (lc + 1 < f.ncols) *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y[4 * jj + 2 * e], y[4 * jj + 2 * e + 1]);
-                            else *o = __float2bfloat16_rn(y[4 * jj + 2 * e]);
-                        }
-                }
+                for (int k = 0; k < 8; ++k) wp[k] = pack_bf16x2(y[2 * k], y[2 * k + 1]);
+                if (lc0 + 32 <= f.ncols) st.send(&tm_out, wp, f.col0 + lc0);  // warp-uniform; rows >= M are clipped by the tensor map
+                else store_frag_bf16(dx, ld, grow, v, f.col0 + lc0, f.ncols - lc0, wp);  // the slice's last chunk
             }
         }
     }

@@ -211,6 +211,36 @@ __device__ __forceinline__ void epi_chunks(const Acc& acc, const EpiCtx& c, Pre&
     acc.release();
 }
 
+// What the calling consumer thread's epilogue sees of `tile`, the it-th tile of its warpgroup (both gemm_nt back-ends):
+// a FragCtx for a fragment-view functor, an EpiCtx for a row-view one.
+template <class Epi>
+__device__ __forceinline__ auto make_epi_ctx(const GemmNTParams& p, int tile, int tile_step, int it, int col0, int ncols, float* scratch) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, nch = (ncols + 31) >> 5;
+    const int next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
+    if constexpr (FragmentEpilogue<Epi>) {
+        const int row0 = tile * p.rows_per_tile;
+        return FragCtx{row0, min(p.rows_per_tile, p.M - row0), warp & 3, nch, col0, ncols, scratch, wg, it, next_tile};
+    } else {
+        EpiCtx c;
+        c.tile = tile;
+        c.r = 32 * (warp & 1) + lane;
+        c.grow = tile * p.rows_per_tile + c.r;
+        c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
+        c.col0 = col0;
+        c.ncols = ncols;
+        c.tid = threadIdx.x;
+        c.wg = wg;
+        c.wtid = threadIdx.x & 127;
+        c.half = (warp >> 1) & 1;
+        epi_chunk_range(ncols, c.half, c.ch0, c.ch1);
+        c.rounds = (nch + 1) >> 1;
+        c.scratch = scratch;
+        c.it = it;
+        c.next_tile = next_tile;
+        return c;
+    }
+}
+
 // Row-view epilogues that move whole 32-row x 32-column bf16 tiles cooperatively stage them per warp (SWIZZLE_64B layout:
 // 16-byte chunk q of row r at r*64 + ((q ^ (r>>1)) & 3)*16, conflict-free for row-per-lane 16-byte accesses).  Row-per-thread
 // stores of 32 rows sit in the LSU queue and stall the warps on their source registers.
@@ -354,9 +384,6 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // ===================== consumer warpgroups: whole tiles in turn, wgmma then the epilogue =====================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kNtConsumerRegs));
         const int wg = warp >> 2;
-        const int half = (warp >> 1) & 1;
-        int ch0, ch1;
-        epi_chunk_range(ncols, half, ch0, ch1);
         const int nch = (ncols + 31) >> 5;
         const int rounds = (nch + 1) >> 1;
         const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, p.num_m_tiles};
@@ -392,30 +419,9 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
             skip_tile();
             if (tmr != nullptr) { const long long u = clock64(); tw_mma += u - t; t = u; }
-            if constexpr (FragmentEpilogue<Epi>) {
-                const int row0 = tile * p.rows_per_tile;
-                epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), warp & 3, nch, col0, ncols, scratch, wg, it,
-                                      tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1});
-            } else {
-                EpiCtx c;
-                c.tile = tile;
-                c.r = 32 * (warp & 1) + lane;
-                c.grow = tile * p.rows_per_tile + c.r;
-                c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
-                c.col0 = col0;
-                c.ncols = ncols;
-                c.tid = threadIdx.x;
-                c.wg = wg;
-                c.wtid = threadIdx.x & 127;
-                c.half = half;
-                c.ch0 = ch0;
-                c.ch1 = ch1;
-                c.rounds = rounds;
-                c.scratch = scratch;
-                c.it = it;
-                c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
-                epi(racc, c);
-            }
+            const auto ctx = make_epi_ctx<Epi>(p, tile, tile_step, it, col0, ncols, scratch);
+            if constexpr (FragmentEpilogue<Epi>) epi.frag(acc, ctx);
+            else epi(racc, ctx);
             if (tmr != nullptr) tw_epi += clock64() - t;
         }
         epi.finish(ei);
@@ -451,34 +457,17 @@ __global__ void __launch_bounds__(kEpiThreads, 1) gemm_nt_simt_epi_kernel(const 
     epi.init(ei, tile_step);
     int it = 0;
     for (int tile = tile0 + wg * tile_step; tile < p.num_m_tiles; tile += 2 * tile_step, ++it) {
+        const auto c = make_epi_ctx<Epi>(p, tile, tile_step, it, col0, ncols, scratch);
         if constexpr (FragmentEpilogue<Epi>) {  // the same fragment layout as the wgmma accumulators
-            const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, nch = (ncols + 31) >> 5;
+            const int lane = threadIdx.x & 31;
             float acc[128];
-            for (int j = 0; j < 4 * nch; ++j)
+            for (int j = 0; j < 4 * c.nch; ++j)
                 for (int e = 0; e < 2; ++e)
                     for (int i = 0; i < 2; ++i)
-                        acc[4 * j + 2 * e + i] = p.dbg_acc[(static_cast<size_t>(tile) * kTileM + 16 * wq + (lane >> 2) + 8 * e) * p.dbg_ld +
+                        acc[4 * j + 2 * e + i] = p.dbg_acc[(static_cast<size_t>(tile) * kTileM + 16 * c.wq + (lane >> 2) + 8 * e) * p.dbg_ld +
                                                            col0 + 8 * j + 2 * (lane & 3) + i];
-            const int row0 = tile * p.rows_per_tile;
-            epi.frag(acc, FragCtx{row0, min(p.rows_per_tile, p.M - row0), wq, nch, col0, ncols, scratch, wg, it,
-                                  tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1});
+            epi.frag(acc, c);
         } else {
-            EpiCtx c;
-            c.tile = tile;
-            c.r = 32 * ((threadIdx.x >> 5) & 1) + (threadIdx.x & 31);
-            c.grow = tile * p.rows_per_tile + c.r;
-            c.valid = (c.r < p.rows_per_tile) && (c.grow < p.M);
-            c.col0 = col0;
-            c.ncols = ncols;
-            c.tid = threadIdx.x;
-            c.wg = wg;
-            c.wtid = threadIdx.x & 127;
-            c.half = (threadIdx.x >> 6) & 1;
-            epi_chunk_range(ncols, c.half, c.ch0, c.ch1);
-            c.rounds = (((ncols + 31) >> 5) + 1) >> 1;
-            c.scratch = scratch;
-            c.it = it;
-            c.next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
             GlobalAcc acc{p.dbg_acc + (static_cast<size_t>(tile) * kTileM + c.r) * p.dbg_ld + col0, c.ch0, c.ch1};
             epi(acc, c);
         }
