@@ -85,7 +85,11 @@ int nr_gemm_tn(const void* A_bf16, int Kr, int Ma, int lda, const void* B_bf16, 
                int b_col0, int Nb, int b_row_shift, float* D, int ldd, void* stream);
 
 /* ---- reference: MultiHeadSelfAttention core (src/model/general/attention/multihead_self.py:15-23) -- */
-/* Q | K | V sections of a row start at columns 0, sec, 2*sec (sec >= heads*dk; dQ|dK|dV likewise, padding written as zeros) */
+/* Q | K | V sections of a row start at columns 0, sec, 2*sec (sec >= heads*dk; dQ|dK|dV likewise, padding written as zeros).
+ * Shape: n_seq >= 0 (0 launches nothing), heads >= 1, 1 <= T <= 64, 2 <= dk <= 32; ld_qkv, ld_dqkv >= 3*sec, ld_ctx >= d+1 (ones
+ * column at d, zeros behind it), ld_dctx >= d, every pitch a multiple of 8 (the context dropout mask is the library's hash of
+ * row * ld_ctx + col); 0 <= p_drop < 1.  Nothing outside the head columns of qkv and columns [0, d) of dctx reaches a result
+ * (NaN there is harmless); dqkv columns [3*sec, ld_dqkv) are not written. */
 int nr_mhsa_core_fwd(const void* qkv_bf16, int ld_qkv, int sec, long long n_seq, int T, int heads, int dk, void* ctx_bf16,
                      int ld_ctx, float p_drop, unsigned long long seed, void* stream);
 int nr_mhsa_core_bwd(const void* qkv_bf16, int ld_qkv, int sec, const void* dctx_bf16, int ld_dctx, long long n_seq, int T,

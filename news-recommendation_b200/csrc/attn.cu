@@ -813,15 +813,29 @@ int dispatch(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, i
     return launch_dk<false, false>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
 }
 
+// The shape contract both directions share (include/newsrec_b200.h), checked before anything is launched.  Every pitch is a
+// multiple of 8: the context dropout picks the 16-bit lane of an element's hash from its column (gc & 3), which is the lane
+// (row * ld + col) & 3 of the library's hash only when the pitch is a multiple of 4.
+int check_core_shape(long long n_seq, int T, int heads, int dk, int sec, int ld_qkv) {
+    NR_REQUIRE(n_seq >= 0, "mhsa: n_seq=%lld is negative", n_seq);
+    NR_REQUIRE(heads >= 1, "mhsa: heads=%d, need at least one head", heads);
+    NR_REQUIRE(T >= 1 && T <= 64, "mhsa: sequence length %d not in [1,64]", T);
+    NR_REQUIRE(dk >= 2 && dk <= 32, "mhsa: head size d_k=%d not in [2,32]", dk);
+    NR_REQUIRE(sec >= static_cast<long long>(heads) * dk && ld_qkv >= 3ll * sec, "mhsa: Q|K|V section stride %d / pitch %d too small for d=%lld",
+               sec, ld_qkv, static_cast<long long>(heads) * dk);
+    NR_REQUIRE(ld_qkv % 8 == 0, "mhsa: Q|K|V pitch %d is not a multiple of 8", ld_qkv);
+    return 0;
+}
+
 }  // namespace
 
 int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, int heads, int dk, void* ctx, int ld_ctx, DropoutCfg drop,
                   cudaStream_t stream) {
-    if (n_seq == 0) return 0;
-    NR_REQUIRE(T >= 1 && T <= 64, "mhsa: sequence length %d not in [1,64]", T);
-    NR_REQUIRE(dk >= 2 && dk <= 32, "mhsa: head size d_k=%d not in [2,32]", dk);
+    NR_PROPAGATE(check_core_shape(n_seq, T, heads, dk, sec, ld_qkv));
     NR_REQUIRE(ld_ctx >= heads * dk + 1, "mhsa: context pitch %d has no room for the ones column", ld_ctx);
-    NR_REQUIRE(sec >= heads * dk && ld_qkv >= 3 * sec, "mhsa: Q|K|V section stride %d / pitch %d too small for d=%d", sec, ld_qkv, heads * dk);
+    NR_REQUIRE(ld_ctx % 8 == 0, "mhsa: context pitch %d is not a multiple of 8", ld_ctx);
+    NR_REQUIRE(drop.p >= 0.f && drop.p < 1.f, "mhsa: dropout p=%f not in [0, 1)", drop.p);
+    if (n_seq == 0) return 0;
     ProfScope ps("mhsa_core_fwd", static_cast<int>(n_seq), T, heads * dk, stream);
     if (mhsa_title_fwd_supported(T, dk, heads, sec, ld_qkv, ld_ctx))  // the news encoder's shape: whole titles per CTA, TMA in / out
         return mhsa_title_fwd(qkv, ld_qkv, sec, n_seq, heads, ctx, ld_ctx, drop, stream);
@@ -830,11 +844,12 @@ int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, 
 
 int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
                   void* dqkv, int ld_dqkv, cudaStream_t stream) {
+    NR_PROPAGATE(check_core_shape(n_seq, T, heads, dk, sec, ld_qkv));
+    NR_REQUIRE(ld_dqkv >= 3 * sec && ld_dctx >= heads * dk, "mhsa: dQ|dK|dV pitch %d / context-gradient pitch %d too small for sec=%d d=%d",
+               ld_dqkv, ld_dctx, sec, heads * dk);
+    NR_REQUIRE(ld_dctx % 8 == 0 && ld_dqkv % 8 == 0, "mhsa: context-gradient pitch %d / dQ|dK|dV pitch %d is not a multiple of 8", ld_dctx,
+               ld_dqkv);
     if (n_seq == 0) return 0;
-    NR_REQUIRE(T >= 1 && T <= 64, "mhsa: sequence length %d not in [1,64]", T);
-    NR_REQUIRE(dk >= 2 && dk <= 32, "mhsa: head size d_k=%d not in [2,32]", dk);
-    NR_REQUIRE(sec >= heads * dk && ld_qkv >= 3 * sec && ld_dqkv >= 3 * sec, "mhsa: Q|K|V section stride %d too small / pitches %d %d",
-               sec, ld_qkv, ld_dqkv);
     ProfScope ps("mhsa_core_bwd", static_cast<int>(n_seq), T, heads * dk, stream);
     const DropoutCfg nodrop{0.f, 0};
     if (mhsa_title_bwd_supported(T, dk, heads, sec, ld_qkv, ld_dctx, ld_dqkv))  // the news encoder's shape: whole titles per CTA, TMA in / out

@@ -480,8 +480,9 @@ class MhsaFn(torch.autograd.Function):
         check(lib.nr_mhsa_core_bwd(_p(QKV), ld3, d, _p(dC), ldx, N, T, heads, d // heads, _p(dQKV), ld3, _stream()),
               "nr_mhsa_core_bwd")
         dW = torch.zeros((3 * d, ldx), dtype=torch.float32, device=dev)
-        check(lib.nr_gemm_tn(_p(dQKV), N * T, 3 * d, ld3, _p(X), N * T, d + 1, ldx, 0, d + 1, 0, _p(dW), ldx, _stream()),
-              "nr_gemm_tn")
+        for c0 in range(0, d + 1, 512):  # nr_gemm_tn takes at most 512 columns of [X | 1] per launch
+            check(lib.nr_gemm_tn(_p(dQKV), N * T, 3 * d, ld3, _p(X), N * T, d + 1, ldx, c0, min(512, d + 1 - c0), 0, _p(dW[:, c0:]),
+                                 ldx, _stream()), "nr_gemm_tn")
         dx = torch.empty((N * T, d), dtype=torch.float32, device=dev)
         check(lib.nr_linear(_p(dQKV), N * T, ld3, _p(ops["wqkvT"]), d, ld3, 3 * d, 1, 0, 128, None, 0, _p(dx), d, 0, _stream()),
               "nr_linear")

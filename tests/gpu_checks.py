@@ -161,35 +161,235 @@ def check_gemm_tn(Kr=1000, Ma=900, Nb=301, shift=0):
 
 
 # ------------------------------------------------------------------------------------------------
-def check_mhsa_core(n_seq=7, T=20, heads=15, dk=20, sectioned=False):
-    """sectioned: Q | K | V at columns 0, sec, 2*sec with sec = round_up(d, 8) (the encoders' layout; padding columns
-    carry garbage on the way in and must come back as zeros in dQ|dK|dV), else dense sections (sec = d)."""
+def mhsa_core_inputs(n, T, heads, dk, regime, seed, device=DEV):
+    """Q, K, V, dC (n, T, d) as fp64 tensors of bf16 values in one of the score regimes of tests/test_gpu_mhsa_core.py:
+    "unit" (scores of standard deviation 1), "saturated" (standard deviation 16, |S| up to about 60: A nearly one-hot),
+    "negative" (every score in [-58, -25]: the +1e-8 dominates the softmax denominator) and "flush" (every score below -95:
+    the kernels' exp2(-max) overflows and the context flushes to zero)."""
+    d = heads * dk
+    u = lambda s, lo, hi: O.det_uniform((n, T, d), seed + s, lo, hi).to(device).double()
+    if regime in ("unit", "saturated"):
+        a = math.sqrt(3.0) if regime == "unit" else 7.0
+        Q, K = u(1, -a, a), u(2, -a, a)
+    else:  # S = -(c / d_k) sum_c u_c v_c with u, v in [0.8, 1.2]: S in -c [0.64, 1.44]
+        c = 40.0 if regime == "negative" else 150.0
+        a = math.sqrt(c / math.sqrt(dk))
+        Q, K = -a * u(1, 0.8, 1.2), a * u(2, 0.8, 1.2)
+    r = lambda t: t.to(torch.bfloat16).double()
+    return r(Q), r(K), r(u(3, -1.0, 1.0)), r(u(4, -1.0, 1.0))
+
+
+def core_launch_grid(T, dk, heads, bwd, sms, fixed=False):
+    """Tasks per full grid round of the head-level kernels (attn.cu launch_mma: per_sm from the tile sets' shared memory, the
+    grid capped at SMs x per_sm CTAs of kWarps = 4 per-warp tasks, or one task per cooperative CTA)."""
+    coop = T > 32
+    TP, PT = (64 if coop else 32), (24 if fixed else 40)
+    tile = 2 * T * PT
+    sets = 1 if coop else 4
+    smem = sets * (2 * 4 * tile + 2 * 2 * TP * (TP + 8)) if bwd else sets * 2 * 3 * tile + 2 * (TP - T) * PT
+    per_sm = max(1, min(3 if coop else (6 if bwd else 8), (224 * 1024) // (smem + 1024)))
+    return sms * per_sm * (1 if coop else 4)
+
+
+def check_mhsa_core(n_seq=7, T=20, heads=15, dk=20, sectioned=False, sec=None, pad=8, p_drop=0.0, regime="unit", seed=1,
+                    extra=True):
+    """nr_mhsa_core_fwd / _bwd through the C ABI against the fp64 references of tests/mhsa_core_ref.py, element by element.
+    Q | K | V at columns 0, sec, 2 sec of rows of pitch ld3 (sec = round_up(d, 8) when sectioned, else d, or as given);
+    pad = extra columns behind the natural pitches (ld3 = round_up(3 sec, 16), ldx = round_up(d + 1, 8), dCtx round_up(d, 8)).
+    Every input column the kernels must not read holds NaN (section padding, [3 sec, ld3), dCtx [d, ld_dctx)), every "="
+    output starts as NaN, every buffer is followed by a guard.  extra: discrimination references and the determinism reruns.
+    Bounds: tests/test_gpu_mhsa_core.py."""
+    import mhsa_core_ref as R
     lib = load_library()
     d = heads * dk
-    sec = ru8(d) if sectioned else d
-    ld3, ldx = ru16(3 * sec), ru8(d + 1)
-    qkv = _rand_bf16((n_seq * T, 3 * d), 21, 1.5).requires_grad_(True)
-    Q, K, V = [t.view(n_seq, T, heads, dk).transpose(1, 2) for t in qkv.split(d, dim=1)]
-    ctx = O.scaled_dot_product_attention(Q, K, V, O.BF16).transpose(1, 2).reshape(n_seq * T, d)
-    g = _rand_bf16((n_seq * T, d), 22)
-    ctx.backward(g)
-    qd = torch.zeros(n_seq * T, ld3)
-    for i in range(3):
-        qd[:, i * sec:i * sec + d] = qkv.detach()[:, i * d:(i + 1) * d]
-    qd = qd.to(torch.bfloat16).to(DEV)
-    cd = torch.full((n_seq * T, ldx), 9.0, dtype=torch.bfloat16, device=DEV)
-    check(lib.nr_mhsa_core_fwd(_p(qd), ld3, sec, n_seq, T, heads, dk, _p(cd), ldx, 0.0, 0, _stream()), "mhsa_fwd")
-    gd = torch.zeros(n_seq * T, ldx)
-    gd[:, :d] = g
-    gd = gd.to(torch.bfloat16).to(DEV)
-    dq = torch.full((n_seq * T, ld3), 9.0, dtype=torch.bfloat16, device=DEV)
-    check(lib.nr_mhsa_core_bwd(_p(qd), ld3, sec, _p(gd), ldx, n_seq, T, heads, dk, _p(dq), ld3, _stream()), "mhsa_bwd")
+    if sec is None:
+        sec = ru8(d) if sectioned else d
+    ld3, ldx, ldc = ru16(3 * sec) + pad, ru8(d + 1) + pad, ru8(d) + pad
+    n_tok = n_seq * T
+    nan = float("nan")
+    Q, K, V, dC = mhsa_core_inputs(max(n_seq, 1), T, heads, dk, regime, seed)
+    qkv = _Guarded(n_tok * ld3, torch.bfloat16, nan)
+    dct = _Guarded(n_tok * ldc, torch.bfloat16, nan)
+    if n_seq:
+        q2 = qkv.body.view(n_tok, ld3)
+        for i, t in enumerate((Q, K, V)):
+            q2[:, i * sec:i * sec + d] = t.reshape(n_tok, d).to(torch.bfloat16)
+        dct.body.view(n_tok, ldc)[:, :d] = dC.reshape(n_tok, d).to(torch.bfloat16)
+    kseed = (0x9E3779B97F4A7C15 * (seed + 17)) & 0xFFFFFFFFFFFFFFFF
+
+    def fwd():
+        out = _Guarded(n_tok * ldx, torch.bfloat16, nan)
+        n0 = int(lib.nr_launch_count())
+        rc = lib.nr_mhsa_core_fwd(_p(qkv.all), ld3, sec, n_seq, T, heads, dk, _p(out.all), ldx, float(p_drop), kseed, _stream())
+        return out, rc, int(lib.nr_launch_count()) - n0
+
+    def bwd():
+        out = _Guarded(n_tok * ld3, torch.bfloat16, nan)
+        n0 = int(lib.nr_launch_count())
+        rc = lib.nr_mhsa_core_bwd(_p(qkv.all), ld3, sec, _p(dct.all), ldc, n_seq, T, heads, dk, _p(out.all), ld3, _stream())
+        return out, rc, int(lib.nr_launch_count()) - n0
+
+    cb, rcf, lf = fwd()
+    db, rcb, lb = bwd()
     torch.cuda.synchronize()
-    c, dqc = cd.float().cpu(), dq.float().cpu()
-    got = torch.cat([dqc[:, i * sec:i * sec + d] for i in range(3)], dim=1)
-    pads = torch.cat([dqc[:, i * sec + d:(i + 1) * sec] for i in range(3)], dim=1)
-    return {"fwd_rel": relerr(c[:, :d], bf16r(ctx.detach())), "ones_col": bool((c[:, d] == 1).all()),
-            "bwd_rel": relerr(got, bf16r(qkv.grad)), "pad_zero": bool((pads == 0).all())}
+    res = {"fwd_rc": rcf, "bwd_rc": rcb, "fwd_launches": lf, "bwd_launches": lb,
+           "msg": lib.nr_last_error().decode() if (rcf or rcb) else ""}
+    if rcf or rcb or n_seq == 0:
+        res["guards_intact"] = all(g.guard_ok() for g in (qkv, dct, cb, db))
+        return res
+    C2, D2 = cb.body.view(n_seq, T, ldx), db.body.view(n_seq, T, ld3)
+    got_c = C2[..., :d].double()
+    got = {k: D2[..., i * sec:i * sec + d].double() for i, k in enumerate(("dQ", "dK", "dV"))}
+    rows = torch.arange(n_tok, device=DEV)
+    cm = dropout_mask_dev(kseed, p_drop, rows, d, ldx).double().view(n_seq, T, d)
+    # ---- exact outputs
+    res["ctx_ones_col"] = bool((C2[..., d] == 1).all())
+    res["ctx_tail_zero"] = bool((C2[..., d + 1:] == 0).all())
+    res["ctx_dropped_nonzero"] = int(((cm == 0) & (got_c != 0)).sum())
+    res["ctx_dropped"] = int((cm == 0).sum())
+    res["dqkv_section_pad_zero"] = all(bool((D2[..., i * sec + d:(i + 1) * sec] == 0).all()) for i in range(3))
+    res["dqkv_tail_prefill_kept"] = bool(torch.isnan(D2[..., 3 * sec:].float()).all())
+    res["guards_intact"] = all(g.guard_ok() for g in (qkv, dct, cb, db))
+    res["outputs_finite"] = bool(torch.isfinite(got_c).all()) and all(bool(torch.isfinite(g).all()) for g in got.values())
+    if regime == "flush":  # every exp2(-max) overflows: the context and every gradient are exactly zero
+        res["flushed_to_zero"] = bool((got_c == 0).all()) and all(bool((g == 0).all()) for g in got.values())
+    # ---- element bounds, a chunk of sequences at a time
+    acc = {k: 0.0 for k in ("ctx_ratio", "dQ_ratio", "dK_ratio", "dV_ratio", "ctx_neighbour_head_ratio", "ctx_no_last_key_ratio",
+                            "ctx_neighbour_row_mask_ratio", "dV_unrounded_A_ratio")}
+    worst = {}
+
+    def note(k, t, s0):
+        v = _worst(t)
+        if v >= acc[k]:
+            acc[k] = v
+            i = int(torch.nan_to_num(t, nan=float("inf")).reshape(-1).argmax())
+            worst[k] = [s0 + i // (T * d), (i // d) % T, i % d]
+
+    cm_next = dropout_mask_dev(kseed, p_drop, rows + 1, d, ldx).double().view(n_seq, T, d) if p_drop > 0 else None
+    cs = max(1, (1 << 22) // (heads * T * T))
+    for s0 in range(0, n_seq, cs):
+        s = slice(s0, min(n_seq, s0 + cs))
+        q, k, v, g, m = Q[s], K[s], V[s], dC[s], cm[s]
+        ref_c, spread_c = R.context_bound(q, k, v, heads, m)
+        note("ctx_ratio", R.judge_context(got_c[s], ref_c, spread_c, m), s0)
+        refs, spread = R.grad_bounds(q, k, v, g, heads)
+        for key in ("dQ", "dK", "dV"):
+            note(key + "_ratio", R.judge_grad(got[key][s], refs[key], spread[key]), s0)
+        if extra:  # discrimination: references a subtly wrong kernel would match instead
+            if heads > 1:
+                note("ctx_neighbour_head_ratio", R.judge_context(got_c[s], R.neighbour_head(ref_c, heads), spread_c, m), s0)
+            if T > 1:
+                ref_nl = R.forward(q, k, v, heads, keys=T - 1)[0] * m
+                note("ctx_no_last_key_ratio", R.judge_context(got_c[s], ref_nl, spread_c, m), s0)
+            if cm_next is not None:
+                ref_nm = R.forward(q, k, v, heads)[0] * cm_next[s]
+                note("ctx_neighbour_row_mask_ratio", R.judge_context(got_c[s], ref_nm, spread_c, m), s0)
+            ref_ua = R.backward(q, k, v, g, heads)["dV"]
+            note("dV_unrounded_A_ratio", R.judge_grad(got["dV"][s], ref_ua, spread["dV"]), s0)
+        del ref_c, spread_c, refs, spread
+    res.update(acc)
+    res["worst_at"] = worst
+    if extra:  # determinism: the core has no atomics
+        cb2, _, _ = fwd()
+        db2, _, _ = bwd()
+        torch.cuda.synchronize()
+        res["fwd_deterministic"] = _bits_equal(cb.body, cb2.body)
+        res["bwd_deterministic"] = _bits_equal(db.body, db2.body)
+    return res
+
+
+def mhsa_core_contract_call(which, **args):
+    """nr_mhsa_core_fwd / _bwd with the given arguments and a valid small shape for the others (2 sequences of 20 rows, 2 heads
+    of d_k 16), on real guarded buffers large enough for any shape the contract tests pass (2 x 65 rows of 256 columns).
+    Returns the return code, the message, the launches and whether every buffer (and its guard) is untouched."""
+    lib = load_library()
+    a = dict(n_seq=2, T=20, heads=2, dk=16, sec=32, ld_qkv=104, ld_ctx=40, ld_dctx=40, ld_dqkv=104, p_drop=0.0)
+    a.update(args)
+    n = 2 * 65 * 256
+    src = O.det_uniform((n,), 5).to(DEV)
+    bufs = [_Guarded(n, torch.bfloat16, src) for _ in range(3)]
+    n0 = int(lib.nr_launch_count())
+    if which == "fwd":
+        rc = lib.nr_mhsa_core_fwd(_p(bufs[0].all), a["ld_qkv"], a["sec"], a["n_seq"], a["T"], a["heads"], a["dk"], _p(bufs[1].all),
+                                  a["ld_ctx"], float(a["p_drop"]), 7, _stream())
+    else:
+        rc = lib.nr_mhsa_core_bwd(_p(bufs[0].all), a["ld_qkv"], a["sec"], _p(bufs[1].all), a["ld_dctx"], a["n_seq"], a["T"], a["heads"],
+                                  a["dk"], _p(bufs[2].all), a["ld_dqkv"], _stream())
+    launches = int(lib.nr_launch_count()) - n0
+    msg = lib.nr_last_error().decode() if rc else ""
+    torch.cuda.synchronize()
+    untouched = all(b.guard_ok() and b.unchanged(torch.ones(n, dtype=torch.bool, device=DEV)) for b in bufs)
+    return rc, msg, launches, untouched
+
+
+def check_mhsa_module(N=37, T=20, d=300, heads=15, seed=3, noncontig=False, step=False, grad_floor=2e-3):
+    """The standalone MultiHeadSelfAttention (ops.MhsaFn: bf16 rows, the Q|K|V projection, the dense-section core, and back)
+    against oracle.multihead_self_attention in fp64 on the module's bf16 operands: the context element by element from the
+    Q|K|V the forward stored, every gradient per row ([W | b] rows, input rows) against the exact chain next to the bf16
+    contract's error.  step: an SGD step first, then the same checks on the next call (the operand cache must rebuild), and
+    the context against the old weights' reference as a discrimination."""
+    import mhsa_core_ref as R
+    from model.general.attention.multihead_self import MultiHeadSelfAttention
+    torch.manual_seed(seed)
+    m = MultiHeadSelfAttention(d, heads).to(DEV)
+    base = O.det_uniform((T, N, d), seed + 1, -2.0, 2.0).to(DEV)
+    x = base.transpose(0, 1) if noncontig else base.transpose(0, 1).contiguous()
+    dout = O.det_uniform((N, T, d), seed + 2).to(DEV)
+    names = [f"W_{k}" for k in "QKV"]
+
+    def params64():
+        p = {}
+        for n in names:
+            lin = getattr(m, n)
+            p[f"m.{n}.weight"] = lin.weight.detach().to(torch.bfloat16).double().requires_grad_(True)
+            p[f"m.{n}.bias"] = lin.bias.detach().double().requires_grad_(True)
+        return p
+
+    def run():
+        m.zero_grad(set_to_none=True)
+        xi = x.detach().clone().requires_grad_(True) if not noncontig else x.detach().requires_grad_(True)
+        out = m(xi)
+        QKV = out.grad_fn.saved_tensors[1].double()
+        out.backward(dout)
+        return xi, out.detach().double(), QKV
+
+    res = {}
+    if step:
+        run()
+        old = params64()
+        # a step of up to 30 % of each weight (the backward's own gradients would move the scores past what the oracle's
+        # exp without max-subtraction can hold in fp64)
+        for i, t in enumerate(m.parameters()):
+            t.grad = 0.3 * t.detach() * O.det_uniform(tuple(t.shape), seed + 10 + i).to(DEV)
+        torch.optim.SGD(m.parameters(), lr=1.0).step()
+    xi, got, QKV = run()
+    xb = x.detach().to(torch.bfloat16).double()
+    Q, K, V = (QKV[:, i * d:(i + 1) * d].reshape(N, T, d) for i in range(3))
+    ones = torch.ones(N, T, d, dtype=torch.float64, device=DEV)
+    ref, spread = R.context_bound(Q, K, V, heads, ones)
+    res["ctx_ratio"] = _worst(R.judge_context(got, ref, spread, ones))
+    grads = {}
+    for v, c in (("exact", O.EXACT), ("contract", O.BF16)):
+        p = params64()
+        xr = xb.clone().requires_grad_(True)
+        O.multihead_self_attention(xr, p, "m", heads, c).backward(dout.double())
+        grads[v] = dict(x=xr.grad.reshape(N * T, d), **{n: torch.cat([p[f"m.{n}.weight"].grad, p[f"m.{n}.bias"].grad.view(-1, 1)], 1)
+                                                        for n in names})
+    kern = dict(x=xi.grad.double().reshape(N * T, d),
+                **{n: torch.cat([getattr(m, n).weight.grad, getattr(m, n).bias.grad.view(-1, 1)], 1).double() for n in names})
+    # T = 1: A = 1 / (1 + 1e-8), so dS = A (dA - A dA) / sqrt(d_k) is 1e-8 of dA -- below fp32 resolution, the kernels' dQ, dK
+    # are 0 -- and the W_Q, W_K gradients are 1e-8 of W_V's: they are held to that scale, the rest to the rule
+    judged = [k for k in kern if not (T == 1 and k in ("W_Q", "W_K"))]
+    for k in judged:
+        res[f"d{k}_row_ratio"], res[f"d{k}_ek"], res[f"d{k}_ec"] = _row_ratio(kern[k], grads["exact"][k], grads["contract"][k],
+                                                                              floor=grad_floor)
+    if T == 1:
+        res["t1_dWqk_rel"] = max(_worst(kern[k].abs()) for k in ("W_Q", "W_K")) / max(_worst(grads["exact"]["W_V"].abs()), 1e-300)
+    if step:  # the context of the old weights must be far from what the new call computed
+        with torch.no_grad():
+            old_ctx = O.multihead_self_attention(xb, old, "m", heads, O.EXACT)
+        res["ctx_old_weights_ratio"] = _worst(R.judge_context(got, old_ctx, spread, ones))
+    return res
 
 
 def check_additive(N=37, S=20, D=300, q=200, precision="fast"):
