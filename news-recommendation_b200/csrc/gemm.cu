@@ -741,6 +741,58 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
     return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
 }
 
+// The tiles of the embedding-gradient GEMM that scatter something: tile t (rows [64t, 64t + 64) of M) is live when one of its
+// rows maps through rm to a token whose id is in [1, V) -- EpiScatter's own test, so a dead tile would add nothing.  Padded
+// histories make runs of all-padding tiles (about 40 % of the NRMS batch), whose A loads and MMAs the scatter then skips.
+// Each warp flags whole tiles; the last block to finish (ticket) compacts the flags in ascending tile order into
+// list[0] = count, list[1 ..] = tiles (the layout of GemmNTParams::tile_list).
+constexpr int kLiveTilesThreads = 256;
+__global__ void __launch_bounds__(kLiveTilesThreads)
+scatter_live_tiles_kernel(const long long* ids, int V, RowMap rm, int M, int num_tiles, int* flags, unsigned* ticket, int* list) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
+    for (int t = blockIdx.x * warps + warp; t < num_tiles; t += gridDim.x * warps) {
+        bool live = false;
+#pragma unroll
+        for (int k = 0; k < kTileM / 32; ++k) {
+            const int grow = t * kTileM + 32 * k + lane;
+            long long trow;
+            int tt;
+            if (grow < M && rm.map(grow, trow, tt)) {
+                const long long id = ids[trow];
+                live = live || (id >= 1 && id < V);
+            }
+        }
+        live = __any_sync(0xffffffffu, live);
+        if (lane == 0) flags[t] = live ? 1 : 0;
+    }
+    __shared__ bool last;
+    __shared__ int warp_sums[kLiveTilesThreads / 32];
+    __threadfence();  // this block's flags are visible before its ticket
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    // thread i compacts the run of tiles [i * per, i * per + per): count, block-wide exclusive scan, then write
+    const int per = (num_tiles + kLiveTilesThreads - 1) / kLiveTilesThreads;
+    const int b = min(num_tiles, static_cast<int>(threadIdx.x) * per), e = min(num_tiles, b + per);
+    int n = 0;
+    for (int t = b; t < e; ++t) n += __ldcg(flags + t);
+    int incl = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+    }
+    if (lane == 31) warp_sums[warp] = incl;
+    __syncthreads();
+    int pos = incl - n;
+    for (int w = 0; w < warp; ++w) pos += warp_sums[w];
+    for (int t = b; t < e; ++t)
+        if (__ldcg(flags + t)) list[1 + pos++] = t;
+    if (threadIdx.x == kLiveTilesThreads - 1) list[0] = pos;  // the last run ends at the total
+}
+
 int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t stream) {
     if (g.M == 0) return 0;
     NR_REQUIRE(g.N % 4 == 0 && c.V >= 1, "scatter_emb: N=%d V=%d", g.N, c.V);
@@ -748,9 +800,29 @@ int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, g.M, g.lda, g.W, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                               kEpiSmemBytes<EpiScatter>, 0));
     const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = to_drop(c.drop), .drop_ld = c.drop_ld};
+    const int num_tiles = plan.p.num_m_tiles;
+    // [0, num_tiles) flags | ticket | list (count + tiles); stream-ordered, so the buffer lives exactly as long as the two launches
+    int* buf = nullptr;
+    NR_CHECK_CUDA(cudaMallocAsync(&buf, sizeof(int) * (2 * static_cast<size_t>(num_tiles) + 2), stream));
+    unsigned* ticket = reinterpret_cast<unsigned*>(buf + num_tiles);
+    int* list = buf + num_tiles + 1;
+    NR_CHECK_CUDA(cudaMemsetAsync(ticket, 0, sizeof(unsigned), stream));
+    {
+        ProfScope ps("scatter_live_tiles", g.M, num_tiles, 0, stream);
+        const int blocks = std::max(1, std::min(4 * num_sms(), ceil_div(num_tiles, kLiveTilesThreads / 32)));
+        scatter_live_tiles_kernel<<<blocks, kLiveTilesThreads, 0, stream>>>(c.ids, c.V, e.rm, g.M, num_tiles, buf, ticket, list);
+        NR_CHECK_CUDA(cudaGetLastError());
+        ++g_launches;
+    }
+    plan.p.tile_list = list;
     g_launches += debug_simt_gemm() ? 2 : 1;
-    ProfScope ps("gemm_scatter_emb", g.M, g.N, g.K * g.taps, stream);
-    return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
+    int rc;
+    {
+        ProfScope ps("gemm_scatter_emb", g.M, g.N, g.K * g.taps, stream);
+        rc = launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
+    }
+    NR_CHECK_CUDA(cudaFreeAsync(buf, stream));
+    return rc;
 }
 
 }  // namespace nr

@@ -58,6 +58,10 @@ struct GemmNTParams {
     int stages;
     int b_stream;       // 1: the weight slice does not fit beside the ring; its (tap, k-chunk) box travels with every A stage
     int stage_bytes;    // kAStageBytes (+ one weight box when b_stream)
+    // null: every tile 0 .. num_m_tiles-1.  Otherwise the tiles to process, written on the device before the launch:
+    // tile_list[0] = their count, tile_list[1 ..] = the tiles in ascending order.  The CTAs stride over list positions the way
+    // they stride over tiles without a list; a CTA whose first position is past the count leaves at once.
+    const int* tile_list;
     float* dbg_acc;     // debug backend only: fp32 accumulators [num_m_tiles*kTileM][dbg_ld]
     int dbg_ld;
     int dbg_flags;      // tuning only (NEWSREC_GEMM_DBG): bit 1 = the producer skips the A loads (MMA on stale data)
@@ -107,7 +111,7 @@ constexpr int kEpiSmemBytes = Epi::kScratchBytes + (FragmentEpilogue<Epi> ? 0 : 
 struct EpiInit {
     int col0, ncols, tid;
     float* scratch;
-    int first_tile;  // first tile of this CTA (warpgroup w starts at first_tile + w * tile_step)
+    int first_tile;  // first tile of this CTA (warpgroup w starts at first_tile + w * tile_step); a list position with a tile list
     int num_tiles;
 };
 
@@ -211,12 +215,18 @@ __device__ __forceinline__ void epi_chunks(const Acc& acc, const EpiCtx& c, Pre&
     acc.release();
 }
 
-// What the calling consumer thread's epilogue sees of `tile`, the it-th tile of its warpgroup (both gemm_nt back-ends):
-// a FragCtx for a fragment-view functor, an EpiCtx for a row-view one.
+// Tiles a gemm_nt launch processes, and the tile at list position i (see GemmNTParams::tile_list)
+__device__ __forceinline__ int gemm_nt_tile_count(const GemmNTParams& p) { return p.tile_list != nullptr ? p.tile_list[0] : p.num_m_tiles; }
+__device__ __forceinline__ int gemm_nt_tile_at(const GemmNTParams& p, int i) { return p.tile_list != nullptr ? p.tile_list[1 + i] : i; }
+
+// What the calling consumer thread's epilogue sees of the tile at list position i, the it-th tile of its warpgroup (both
+// gemm_nt back-ends; n_tiles = gemm_nt_tile_count): a FragCtx for a fragment-view functor, an EpiCtx for a row-view one.
 template <class Epi>
-__device__ __forceinline__ auto make_epi_ctx(const GemmNTParams& p, int tile, int tile_step, int it, int col0, int ncols, float* scratch) {
+__device__ __forceinline__ auto make_epi_ctx(const GemmNTParams& p, int i, int n_tiles, int tile_step, int it, int col0, int ncols,
+                                             float* scratch) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, nch = (ncols + 31) >> 5;
-    const int next_tile = tile + 2 * tile_step < p.num_m_tiles ? tile + 2 * tile_step : -1;
+    const int tile = gemm_nt_tile_at(p, i);
+    const int next_tile = i + 2 * tile_step < n_tiles ? gemm_nt_tile_at(p, i + 2 * tile_step) : -1;
     if constexpr (FragmentEpilogue<Epi>) {
         const int row0 = tile * p.rows_per_tile;
         return FragCtx{row0, min(p.rows_per_tile, p.M - row0), warp & 3, nch, col0, ncols, scratch, wg, it, next_tile};
@@ -321,6 +331,10 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int slice = blockIdx.x % p.n_slices;
     const int tile0 = blockIdx.x / p.n_slices;
     const int tile_step = gridDim.x / p.n_slices;
+    // tile0 .. n_tiles are list positions (tiles themselves without a list).  A CTA without a tile leaves before it issues the
+    // weight-slice load or touches a barrier.
+    const int n_tiles = gemm_nt_tile_count(p);
+    if (tile0 >= n_tiles) return;
     const int col0 = slice * p.n_stride;
     const int ncols = min(p.n_stride, p.N - col0);
     const int tap_shift = p.taps / 2;
@@ -355,8 +369,8 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         int st = 0;
         uint32_t ph = 0;
         long long tw_empty = 0;
-        for (int tile = tile0; tile < p.num_m_tiles; tile += tile_step) {
-            const int row0 = tile * p.rows_per_tile;
+        for (int i = tile0; i < n_tiles; i += tile_step) {
+            const int row0 = gemm_nt_tile_at(p, i) * p.rows_per_tile;
             for (int s = 0; s < p.taps; ++s)
                 for (int kc = 0; kc < p.k_chunks; ++kc) {
                     const long long t = tmr != nullptr ? clock64() : 0;
@@ -386,7 +400,7 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int wg = warp >> 2;
         const int nch = (ncols + 31) >> 5;
         const int rounds = (nch + 1) >> 1;
-        const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, p.num_m_tiles};
+        const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, n_tiles};
         epi.init(ei, tile_step);
         const uint32_t a_s = smem_u32(sA), b_s = smem_u32(sB);
         float acc[128];
@@ -402,11 +416,11 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (wg == 1) skip_tile();
         long long tw_turn = 0, tw_mma = 0, tw_epi = 0;
         int it = 0;
-        for (int tile = tile0 + wg * tile_step; tile < p.num_m_tiles; tile += 2 * tile_step, ++it) {
+        for (int i = tile0 + wg * tile_step; i < n_tiles; i += 2 * tile_step, ++it) {
             long long t = tmr != nullptr ? clock64() : 0;
-            if (tile != tile0) named_bar_sync(kBarTurn + wg, 2 * kWgThreads);  // the other warpgroup has issued its tile
+            if (i != tile0) named_bar_sync(kBarTurn + wg, 2 * kWgThreads);  // the other warpgroup has issued its tile
             if (tmr != nullptr) { const long long u = clock64(); tw_turn += u - t; t = u; }
-            const int pass_bar = tile + tile_step < p.num_m_tiles ? kBarTurn + (wg ^ 1) : -1;
+            const int pass_bar = i + tile_step < n_tiles ? kBarTurn + (wg ^ 1) : -1;
             switch (nch) {
                 case 1: gemm_nt_mma_tile<1>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
                 case 2: gemm_nt_mma_tile<2>(acc, p, full, empty, st, ph, a_s, b_s, b_region, lane, pass_bar); break;
@@ -419,7 +433,7 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
             skip_tile();
             if (tmr != nullptr) { const long long u = clock64(); tw_mma += u - t; t = u; }
-            const auto ctx = make_epi_ctx<Epi>(p, tile, tile_step, it, col0, ncols, scratch);
+            const auto ctx = make_epi_ctx<Epi>(p, i, n_tiles, tile_step, it, col0, ncols, scratch);
             if constexpr (FragmentEpilogue<Epi>) epi.frag(acc, ctx);
             else epi(racc, ctx);
             if (tmr != nullptr) tw_epi += clock64() - t;
@@ -453,11 +467,13 @@ __global__ void __launch_bounds__(kEpiThreads, 1) gemm_nt_simt_epi_kernel(const 
     const int wg = threadIdx.x >> 7;
     for (int i = threadIdx.x; i < Epi::kScratchBytes / 4; i += kEpiThreads) scratch[i] = 0.f;
     __syncthreads();
-    const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, p.num_m_tiles};
+    const int n_tiles = gemm_nt_tile_count(p);
+    const EpiInit ei{col0, ncols, static_cast<int>(threadIdx.x), scratch, tile0, n_tiles};
     epi.init(ei, tile_step);
     int it = 0;
-    for (int tile = tile0 + wg * tile_step; tile < p.num_m_tiles; tile += 2 * tile_step, ++it) {
-        const auto c = make_epi_ctx<Epi>(p, tile, tile_step, it, col0, ncols, scratch);
+    for (int i = tile0 + wg * tile_step; i < n_tiles; i += 2 * tile_step, ++it) {
+        const int tile = gemm_nt_tile_at(p, i);
+        const auto c = make_epi_ctx<Epi>(p, i, n_tiles, tile_step, it, col0, ncols, scratch);
         if constexpr (FragmentEpilogue<Epi>) {  // the same fragment layout as the wgmma accumulators
             const int lane = threadIdx.x & 31;
             float acc[128];

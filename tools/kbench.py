@@ -2,8 +2,15 @@
 between repetitions by a 256 MB memset).  A tuning tool; bench.py is the contract benchmark.
 
     python tools/kbench.py [op ...]      ops: mhsa_fwd mhsa_fwd_drop mhsa_bwd qkv pool tn900 tn200 gather dx_fp32 lin:N:K
+                                         scatter scatter_live
+
+scatter / scatter_live: the embedding-gradient scatter at the NRMS shape (M = 563,200, N = 300, K = 912) through
+nr_element_encoder_bwd, with ids drawn like bench.synth_slots (histories of U{1..50} news left-padded with all-zero news,
+titles of U{5..20} tokens right-padded) or all valid; the library's own launch timers give the scatter's kernels apart from
+the ReLU backward and weight gradient around them.
 """
 import ctypes as C
+import json
 import os
 import sys
 
@@ -51,6 +58,28 @@ demb_big = None
 names = sys.argv[1:] or ["mhsa_fwd", "mhsa_fwd_drop", "mhsa_bwd", "qkv", "pool", "tn900", "tn200", "gather"]
 if "dx_fp32" in names:
     demb_big = torch.empty(n_tok, d, device=dev)
+def synth_title_ids(B=512, H=50, C=5, T=20, V=70976, seed=0):
+    """news-level token ids in the encoder's order: the B x H browsed news, then the B x C candidates"""
+    g = torch.Generator().manual_seed(seed)
+    hl = torch.randint(1, H + 1, (B,), generator=g)
+    ids = torch.randint(1, V, (B, H + C, T), generator=g) * (torch.arange(T) < torch.randint(5, T + 1, (B, H + C, 1), generator=g))
+    ids[:, :H] *= (torch.arange(H).view(1, -1, 1) >= H - hl.view(-1, 1, 1))
+    return torch.cat([ids[:, :H].reshape(-1), ids[:, H:].reshape(-1)]).to(dev)
+
+
+def scatter_op(all_live):
+    """nr_element_encoder_bwd with E = d, F = 3 * sec: its scatter is gemm_scatter_emb at the NRMS shape"""
+    E, F, V = d, 3 * sec, 70976
+    lde, ldf = ru8(E + 1), ru8(F + 1)
+    sids = torch.randint(1, V, (n_tok,), device=dev) if all_live else synth_title_ids(V=V)
+    dout, out = torch.randn(n_tok, F, device=dev), torch.ones(n_tok, F, device=dev)
+    dY, Eb, WT = torch.empty(n_tok, ldf, device=dev, dtype=torch.bfloat16), bf(n_tok, lde), bf(E, ldf)
+    dWe, dt = torch.zeros(F, lde, device=dev), torch.zeros(V, E, device=dev)
+    print(f"scatter ids: {float(((sids >= 1) & (sids < V)).float().mean()):.3f} of the rows valid", flush=True)
+    return lambda: lib.nr_element_encoder_bwd(_p(sids), n_tok, _p(dout), _p(out), F, _p(dY), ldf, _p(Eb), E, lde, _p(WT), _p(dWe),
+                                              _p(dt), V, st)
+
+
 def lin_op(spec):
     """lin:N:K[:bf16out] -> nr_linear at M = n_tok with fresh operands"""
     parts = spec.split(":")
@@ -62,6 +91,22 @@ def lin_op(spec):
 
 
 for name in names:
+    if name in ("scatter", "scatter_live"):
+        fn = scatter_op(name == "scatter_live")
+        for _ in range(2):
+            check(fn(), name)
+        lib.nr_profile_enable(1)
+        for _ in range(5):
+            flush.zero_()
+            check(fn(), name)
+        torch.cuda.synchronize()
+        lib.nr_profile_enable(0)
+        buf = C.create_string_buffer(1 << 16)
+        assert lib.nr_profile_report(buf, len(buf)) >= 0
+        for key, (count, ms) in json.loads(buf.value.decode()).items():
+            if "scatter" in key:
+                print(f"{name:15s} {key:50s} {ms / count:.4f} ms per call ({count} calls)", flush=True)
+        continue
     fn = lin_op(name) if name.startswith("lin:") else OPS[name]
     for _ in range(2):
         check(fn(), name)
