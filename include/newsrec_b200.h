@@ -1,4 +1,4 @@
-/* newsrec_b200 -- C ABI of the Hopper-native (sm_90a) NRMS / NAML / LSTUR / TANR / Exp1 hot path.
+/* newsrec_b200 -- C ABI of the Hopper-native (sm_90a) NRMS / NAML / LSTUR / TANR / Exp1 / Hi-Fi Ark hot path.
  *
  * Drop-in boundary for the reference's Python modules (yusanshi/news-recommendation @ 8323a4f).  The
  * reference has no FFI of its own (pure PyTorch); these are the entry points a maintainer binds with
@@ -9,7 +9,7 @@
  *     (PyTorch caching allocator); the library allocates nothing persistent;
  *   - all work is enqueued asynchronously on `stream` (a cudaStream_t passed as void*); no implicit syncs;
  *   - return 0 on success, a positive cudaError_t on a CUDA failure, -1 on an argument/shape violation
- *     (detected before any launch); nr_last_error() returns the message for the calling thread;
+ *     (detected before any launch; the Hi-Fi Ark entry points return -2 for a shape outside their stated bounds); nr_last_error() returns the message for the calling thread;
  *   - bf16 operand matrices are row-major with a pitch ("ld", in elements) that is a multiple of 8;
  *     an activation matrix of logical width D carries a constant 1.0 in column D (it turns the next
  *     weight-gradient GEMM's extra column into the bias gradient) and zeros behind it;
@@ -373,6 +373,38 @@ typedef struct {
 } nr_gru_bwd_args;
 long long nr_gru_bwd_workspace(int B, int S, int D, int Hd);
 int nr_gru_bwd(const nr_gru_bwd_args* a, void* stream);
+
+/* ---- reference: Hi-Fi Ark after the news encoder, fp32 on the CUDA cores ---------------------------------------------------
+ *   user side  SelfAttention + residual + OMAP (src/model/general/attention/self.py, src/model/HiFiArk/OMAP.py):
+ *              X = hist[b] (H x F);  Y = softmax_row(X X^T) X + X;  archive[b] = softmax_over_h(Y W)^T Y  (P x F);  W is F x P
+ *   scorer     SimilarityAttention + DNNClickPredictor (src/model/general/attention/similarity.py, click_predictor/DNN.py):
+ *              w = softmax(A c);  u = w^T A;  logit = w2 . relu(W1 [c; u] + b1) + b2;  W1 is hidden x 2F, b2 one float
+ *   regulariser (src/model/HiFiArk/OMAP.py:36-44): reg_out = || (W^T W) * (1 - I) ||_F, its gradient 2 W (M * W^T W) / R (zero at R = 0)
+ * Supported bounds: 1 <= H <= 50, 4 <= F <= 400 with F % 4 == 0, 1 <= P <= 32, 1 <= hidden <= 32; a shape outside them returns -2
+ * before any launch.  Shared memory per CTA: user side 4 * ((max(H, P) + H)(F + 4) + 2H^2 + 2HP + P^2 + 8) bytes (198.5 KB at the
+ * bounds' corner), scorer forward 4 * (P (F + 4) + 2F + 128) bytes, scorer backward 4 * (2P (F + 4) + 2 hidden F + 4F + 260) bytes
+ * (213 KB at the corner).  hist, archive and darchive must be 16-byte aligned.  The kernels have no waits, so they never write the
+ * watchdog record (nr_device_error stays 0).
+ * Weight gradients (dW, dW1, db1, dw2, db2) are ADDED (+=) in a fixed order: per-CTA partial rows in the workspace, summed by one
+ * ordered reduction (bit-identical across runs).  dhist, dcand and darchive are written (=). */
+int nr_archive_user_fwd(const float* hist, long long B, int H, int F, int P, const float* W, float* archive, float* reg_out,
+                        void* stream);     /* hist [B][H][F], archive [B][P][F] (=); reg_out: device float or NULL (not computed) */
+long long nr_archive_user_bwd_workspace(long long B, int F, int P);
+/* dreg: device float, the gradient of reg_out, or NULL (no regulariser term) */
+int nr_archive_user_bwd(const float* hist, long long B, int H, int F, int P, const float* W, const float* darchive, const float* dreg,
+                        float* dhist, float* dW, void* workspace, long long workspace_bytes, void* stream);
+/* Segment s (a training user, an evaluation impression) scores candidates i in [seg_offsets[s], seg_offsets[s+1]) against
+ * archive[s] ([n_seg][P][F]): the candidate vector is news[cand[i]] (news [n_news][F]), or news[i] when cand is NULL.  A cand
+ * index outside [0, n_news) sets *bad_id_flag and leaves NaN as its logit.  logits [n_cand] (=). */
+int nr_archive_score_fwd(const float* news, long long n_news, int F, const long long* cand, long long n_cand,
+                         const long long* seg_offsets, long long n_seg, const float* archive, int P, const float* W1, const float* b1,
+                         int hidden, const float* w2, const float* b2, float* logits, int* bad_id_flag, void* stream);
+long long nr_archive_score_bwd_workspace(long long n_seg, int F, int hidden);
+/* dcand [n_cand][F] (=) by candidate POSITION i (not news row), darchive [n_seg][P][F] (=); dW1, db1, dw2, db2 (+=) */
+int nr_archive_score_bwd(const float* news, long long n_news, int F, const long long* cand, long long n_cand,
+                         const long long* seg_offsets, long long n_seg, const float* archive, int P, const float* W1, const float* b1,
+                         int hidden, const float* w2, const float* b2, const float* dlogits, float* dcand, float* darchive,
+                         float* dW1, float* db1, float* dw2, float* db2, void* workspace, long long workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -7,7 +7,7 @@ restatement of the knob surface, not a copy of the reference source.
 import os
 
 model_name = os.environ.get("MODEL_NAME", "NRMS")
-SUPPORTED_MODELS = ("NRMS", "NAML", "LSTUR", "TANR", "Exp1")  # the hot-path scope of this build (SURVEY.md section 8)
+SUPPORTED_MODELS = ("NRMS", "NAML", "LSTUR", "TANR", "Exp1", "HiFiArk")  # the hot-path scope of this build (SURVEY.md section 8)
 if model_name not in SUPPORTED_MODELS:
     raise AssertionError(f"MODEL_NAME={model_name!r}: this build accelerates {SUPPORTED_MODELS} only")
 
@@ -50,6 +50,8 @@ _PER_MODEL = {
     # precision as NRMS: "accurate" also keeps the stacked views in front of final_attention as hi/lo bf16 pairs
     "Exp1": dict(dataset_attributes={"news": ["category", "subcategory", "title"], "record": []}, num_attention_heads=15,
                  ensemble_factor=1, precision=os.environ.get("NEWSREC_PRECISION", "accurate")),
+    # plain bf16 storage in the news encoder meets the 1e-3 contract (DESIGN.md section 4): no precision knob
+    "HiFiArk": dict(dataset_attributes={"news": ["title"], "record": []}, num_pooling_heads=5, regularizer_loss_weight=0.1, **_CNN),
 }
 for _name, _knobs in _PER_MODEL.items():
     globals()[f"{_name}Config"] = type(f"{_name}Config", (BaseConfig,), dict(_knobs))

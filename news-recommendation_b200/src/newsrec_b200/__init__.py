@@ -147,6 +147,13 @@ SIGNATURES = {
     "nr_gru_persistent_supported": (_i, [_i, _i]),
     "nr_gru_bwd_workspace": (_ll, [_i, _i, _i, _i]),
     "nr_gru_bwd": (_i, [C.POINTER(GruBwdArgs), _vp]),
+    "nr_archive_user_fwd": (_i, [_vp, _ll, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "nr_archive_user_bwd_workspace": (_ll, [_ll, _i, _i]),
+    "nr_archive_user_bwd": (_i, [_vp, _ll, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "nr_archive_score_fwd": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "nr_archive_score_bwd_workspace": (_ll, [_ll, _i, _i]),
+    "nr_archive_score_bwd": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
 }
 
 _lib = None

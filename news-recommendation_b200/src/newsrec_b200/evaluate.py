@@ -154,11 +154,16 @@ def user_vectors(model, tables, matrix, flag):
     return torch.cat(out)
 
 
-def impression_scores(tables, matrix, users, flag):
-    """Stage 3: (n_cand,) fp32 scores of every impression (at least one), one launch (nr_segment_dot)."""
+def impression_scores(tables, matrix, users, flag, model=None):
+    """Stage 3: (n_cand,) fp32 scores of every impression (at least one), one launch: nr_segment_dot for user vectors (U, D);
+    for archives (U, P, D) (Hi-Fi Ark) the model's similarity-attention scorer against each impression's archive."""
     from .ops import predict_impressions
+    cand, seg = _device_long(tables.cand, matrix), _device_long(tables.seg_offsets, matrix)
+    if users.dim() == 3:
+        per_imp = _gather(tables.seg_user, users.reshape(users.shape[0], -1), flag).view(-1, *users.shape[1:])
+        return model.score_impressions(matrix, cand, seg, per_imp, flag)
     per_imp = _gather(tables.seg_user, users, flag)
-    return predict_impressions(matrix, _device_long(tables.cand, matrix), _device_long(tables.seg_offsets, matrix), per_imp)
+    return predict_impressions(matrix, cand, seg, per_imp)
 
 
 def _device_long(a, like):
@@ -185,7 +190,7 @@ def evaluate(model, directory, num_workers, max_count=sys.maxsize, *, user2int_p
             return (np.float64(np.nan),) * 4
         flag = new_flag(matrix.device)
         users = user_vectors(model, tables, matrix, flag)
-        scores = impression_scores(tables, matrix, users, flag)
+        scores = impression_scores(tables, matrix, users, flag, model)
         means = metric_means(scores, tables)  # synchronises
         if int(flag.item()):
             raise IndexError("evaluate: a history or impression row is outside the news / user tables")

@@ -47,7 +47,10 @@ CASES = [
     ("LSTUR", {"long_short_term_method": "ini"}, ("title", "category")),
     ("LSTUR", {"long_short_term_method": "con"}, ("title", "category")),
     ("Exp1", {}, ("title", "category")),
+    ("HiFiArk", {}, ("title",)),
 ]
+# weight of the second element of a tuple output in the training loss, per family (reference train.py)
+AUX_LOSS_WEIGHT = {"TANR": "topic_classification_loss_weight", "HiFiArk": "regularizer_loss_weight"}
 label = torch.zeros(B, dtype=torch.long, device=dev)
 res = {}
 try:  # the card and its power limit belong beside every number of this run
@@ -71,8 +74,8 @@ for name, over, want in CASES:
     def step():
         grads.zero()
         out = model(*extra, cand, clicked)
-        if isinstance(out, tuple):  # TANR: (click logits, topic loss)
-            loss = torch.nn.functional.cross_entropy(out[0], label) + cfg.topic_classification_loss_weight * out[1]
+        if isinstance(out, tuple):  # TANR: (click logits, topic loss); Hi-Fi Ark: (click logits, regulariser)
+            loss = torch.nn.functional.cross_entropy(out[0], label) + getattr(cfg, AUX_LOSS_WEIGHT[name]) * out[1]
         else:
             loss = torch.nn.functional.cross_entropy(out, label)
         loss.backward()
@@ -90,6 +93,12 @@ for name, over, want in CASES:
     ms = e0.elapsed_time(e1) / 5
     key = name + ("/" + over["long_short_term_method"] if over else "")
     res[key] = {"ms_per_step": round(ms, 3), "impressions_per_s": round(B / ms * 1e3), "launches_per_step": (newsrec_b200.launch_count() - l0) // 5}
+    if name == "HiFiArk":  # the kernels after the news encoder (the news encoder is TANR's: compare the two step times)
+        newsrec_b200.load_library().nr_profile_enable(1)
+        step()
+        torch.cuda.synchronize()
+        res[key]["kernels_ms"] = {k: round(v[1], 4) for k, v in newsrec_b200.profile_report().items() if "archive" in k}
+        newsrec_b200.load_library().nr_profile_enable(0)
     print(key, res[key], flush=True)
     del model, grads
     torch.cuda.empty_cache()
