@@ -299,6 +299,79 @@ typedef struct {
 long long nr_cnn_encoder_bwd_workspace(long long n_seq, int T, int F, int q);
 int nr_cnn_encoder_bwd(const nr_cnn_encoder_bwd_args* a, void* stream);
 
+/* ---- reference: DKN's knowledge-aware CNN (src/model/DKN/KCNN.py), without context embeddings --------------
+ * word embedding | tanh(entity embedding . M + b) stacked as two channels -> Conv2d(2, F, (x, d)) for every window x, no
+ * padding (T + 1 - x positions) -> ReLU -> ONE additive attention shared by the windows -> the windows' outputs side by side.
+ * Layouts (bf16 rows, 16-byte sections):
+ *   X2   [n_seq*T][ldx]   ldx = 2 sec, sec = round_up(d+1, 8): [word (d) | 1 | 0..] [tanh entity (d) | 1 | 0..] (saved)
+ *   E    [n_seq*T][lde]   lde = round_up(de+1, 8): gathered entity rows (saved)
+ *   Y    window w's relu(conv) rows [n_seq*(T+1-x_w)][ldf], ldf = round_up(F+1, 8), the windows back to back (saved); w likewise
+ *   out  [n_seq][ldo] fp32, ldo = n_win * Fs, Fs = round_up(F, 4): window w in columns [w Fs, w Fs + F), the rest 0 (=)
+ * Each conv is one wgmma GEMM of x_w row-shifted taps over the compact rows of X2.  The backward puts dY of every window into
+ * one [n_seq*T][n_win*ldf] block and runs the transposed conv of all windows as max(x) taps, split into the word half (scattered
+ * into dword) and the entity half (times 1 - t^2 -> dZ, then dM and dentity).  Row 0 of both tables is read as stored and gets
+ * no gradient (padding_idx).  dout's padding columns must be 0.
+ * Shapes: 1 <= n_win <= 4, 1 <= x_w <= 4, max(x) <= T <= 64, d and de multiples of 4 (>= 8), F even (>= 8), 1 <= q <= 256; both
+ * entry points reject any other shape with -1 before the first launch. */
+typedef struct {
+    long long n_seq;
+    int T, d, de, F, q, n_win;
+    int win[4];
+    int ldx, lde, ldf, ldo;
+    const long long* word_ids;      /* [n_seq*T]                                                          */
+    const long long* entity_ids;    /* [n_seq*T]                                                          */
+    const void* word_table_bf16;    /* [V][sec]                                                           */
+    int V;
+    const void* entity_table_bf16;  /* [Ve][lde]                                                          */
+    int Ve;
+    const void* mT_bf16;            /* [d][lde]  transform_matrix^T                                       */
+    const float* mb;                /* [d]       transform_bias                                           */
+    const void* wconv_bf16;         /* [sum x_w * F][ldx]; window w, tap s at rows (x_0 + .. + x_(w-1) + s) F, in X2's columns */
+    const float* bconv;             /* [n_win * F]                                                        */
+    const void* wa_bf16;            /* [q][ldf]                                                           */
+    const float* ba;
+    const float* qv;
+    void* X2_bf16;
+    void* E_bf16;
+    void* Y_bf16;
+    float* w;
+    float* out;
+    int* bad_id_flag;
+} nr_kcnn_encoder_fwd_args;
+int nr_kcnn_encoder_fwd(const nr_kcnn_encoder_fwd_args* a, void* stream);
+
+typedef struct {
+    long long n_seq;
+    int T, d, de, F, q, n_win;
+    int win[4];
+    int ldx, lde, ldf, ldo, ldq;    /* ldq = round_up(q, 16)                                              */
+    const long long* word_ids;
+    const long long* entity_ids;
+    int V, Ve;
+    const void* wT_word_bf16;       /* [max x][d][n_win*ldf]: tap s' holds W_(w, max x - 1 - s')^T in columns w ldf .. w ldf + F */
+    const void* wT_entity_bf16;     /* the same for the entity channel                                    */
+    const void* m_bf16;             /* [de][sec] transform_matrix                                          */
+    const void* wa_bf16;            /* [q][ldf]                                                           */
+    const void* waT_bf16;           /* [F][ldq]                                                           */
+    const float* ba;
+    const float* qv;
+    const void* X2_bf16;
+    const void* E_bf16;
+    const void* Y_bf16;
+    const float* w;
+    const float* dout;              /* [n_seq][ldo]                                                       */
+    float* dWconv_ext;              /* [sum x_w * F][ldx] (+=); column sec + d of each window's tap 0 is d(bias) */
+    float* dM_ext;                  /* [d][lde] (+=): d(transform_matrix)^T, column de = d(transform_bias)   */
+    float* dWa_ext;                 /* [q][ldf] (+=); column F is d(bias)                                   */
+    float* dqv;                     /* [q] (+=)                                                           */
+    float* dword;                   /* [V][d] (+=)                                                        */
+    float* dentity;                 /* [Ve][de] (+=)                                                      */
+    void* workspace;
+    long long workspace_bytes;
+} nr_kcnn_encoder_bwd_args;
+long long nr_kcnn_encoder_bwd_workspace(long long n_seq, int T, int d, int F, int q, int n_win);
+int nr_kcnn_encoder_bwd(const nr_kcnn_encoder_bwd_args* a, void* stream);
+
 /* ---- generic Linear over dense fp32 rows (TANR topic predictor src/model/TANR/__init__.py:58-61, GRU
  * projections).  fwd: X_bf16 = bf16(x | 1) (saved), out = act(X W^T + b).  bwd: dW_ext[N][ldx] += dY^T [X|1]
  * (column K = d(bias)), dx = dY W (optional).  relu_out masks dy with (relu_out > 0). */
@@ -405,6 +478,20 @@ int nr_archive_score_bwd(const float* news, long long n_news, int F, const long 
                          const long long* seg_offsets, long long n_seg, const float* archive, int P, const float* W1, const float* b1,
                          int hidden, const float* w2, const float* b2, const float* dlogits, float* dcand, float* darchive,
                          float* dW1, float* db1, float* dw2, float* db2, void* workspace, long long workspace_bytes, void* stream);
+
+/* ---- reference: DKN's history attention (src/model/DKN/attention.py), fp32 on the CUDA cores --------------------------------
+ * The reference scores history row h_j against candidate c as Linear(16,1)(Linear(2F,16)([c; h_j])), with nothing between the
+ * two Linears, so the score is alpha.c + beta.h_j + const with beta = W1[:, F:]^T w2: the softmax over j cancels everything
+ * but beta.h_j and the user vector is the same for every candidate:
+ *   user[b] = sum_j softmax_j(beta . hist[b][j]) hist[b][j]          W1 is hidden x 2F (the candidate half is never read)
+ * The gradients of W1[:, :F], b1 and b2 are exactly zero; the backward adds nothing there.  One CTA per user.
+ * Bounds: 1 <= H <= 64, 1 <= F <= 512, 1 <= hidden <= 32; a shape outside them returns -2 before any launch.
+ * dW1 (history half) and dw2 are ADDED (+=) in a fixed order (per-CTA partial rows, one ordered reduction); dhist is written (=). */
+int nr_dkn_user_fwd(const float* hist, long long B, int H, int F, const float* W1, int hidden, const float* w2, float* user,
+                    void* stream);     /* hist [B][H][F], user [B][F] (=) */
+long long nr_dkn_user_bwd_workspace(long long B, int F);
+int nr_dkn_user_bwd(const float* hist, long long B, int H, int F, const float* W1, int hidden, const float* w2, const float* duser,
+                    float* dhist, float* dW1, float* dw2, void* workspace, long long workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

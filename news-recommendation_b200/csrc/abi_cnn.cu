@@ -1,5 +1,6 @@
 // extern "C" surface, part 2: the title/abstract CNN encoder shared by NAML / LSTUR / TANR, the category
 // "element" encoder of NAML, fp32 embedding lookups, a generic Linear and the ReLU-backward helper.
+#include <algorithm>
 #include <cstring>
 
 #include "../../include/newsrec_b200.h"
@@ -93,6 +94,138 @@ int nr_cnn_encoder_bwd(const nr_cnn_encoder_bwd_args* a, void* stream) {
                                   {.ids = a->ids, .demb = a->demb, .V = a->V, .rm = to_compact, .drop = {a->p_drop, a->seed}, .drop_ld = a->ldx},
                                   st));
     return 0;
+}
+
+}  // extern "C"
+
+// ---- reference: DKN KCNN (src/model/DKN/KCNN.py:56-117, use_context=False) -------------------------------
+// Every shape limit of the chain, checked before the first launch: taps <= 4 per conv GEMM, a pooling tile holds whole segments
+// (T <= kGemmTileRows), d and de multiples of 4 for the embedding scatters, F even for the pooled rows.
+template <class Args>
+static int check_kcnn_shape(const Args* a) {
+    NR_REQUIRE(a->n_win >= 1 && a->n_win <= 4, "kcnn encoder: %d windows (1 .. 4)", a->n_win);
+    int max_x = 0;
+    for (int w = 0; w < a->n_win; ++w) {
+        NR_REQUIRE(a->win[w] >= 1 && a->win[w] <= 4, "kcnn encoder: window %d (1 .. 4)", a->win[w]);
+        max_x = std::max(max_x, a->win[w]);
+    }
+    NR_REQUIRE(a->n_seq >= 0 && a->T >= max_x && a->T <= kGemmTileRows && a->d >= 8 && a->de >= 8 && a->F >= 8 && a->q >= 1 && a->q <= 256,
+               "kcnn encoder: bad shape n_seq=%lld T=%d (max window %d .. %d) d=%d de=%d F=%d q=%d", a->n_seq, a->T, max_x, kGemmTileRows,
+               a->d, a->de, a->F, a->q);
+    NR_REQUIRE(a->d % 4 == 0 && a->de % 4 == 0 && a->F % 2 == 0, "kcnn encoder: d, de must be multiples of 4 and F even (d=%d de=%d F=%d)",
+               a->d, a->de, a->F);
+    NR_REQUIRE(a->ldx == 2 * round_up(a->d + 1, 8) && a->lde == round_up(a->de + 1, 8) && a->ldf == round_up(a->F + 1, 8) &&
+                   a->ldo == a->n_win * round_up(a->F, 4),
+               "kcnn encoder: pitches ldx=%d lde=%d ldf=%d ldo=%d", a->ldx, a->lde, a->ldf, a->ldo);
+    NR_REQUIRE(a->n_seq * a->T < (1ll << 31), "kcnn encoder: too many rows");
+    return 0;
+}
+static int kcnn_max_window(const int* win, int n_win) { return *std::max_element(win, win + n_win); }
+
+extern "C" {
+
+int nr_kcnn_encoder_fwd(const nr_kcnn_encoder_fwd_args* a, void* stream) {
+    NR_REQUIRE(a != nullptr, "nr_kcnn_encoder_fwd: null args");
+    NR_PROPAGATE(check_kcnn_shape(a));
+    NR_REQUIRE(a->word_ids && a->entity_ids && a->word_table_bf16 && a->entity_table_bf16 && a->mT_bf16 && a->mb && a->wconv_bf16 &&
+                   a->bconv && a->wa_bf16 && a->ba && a->qv && a->X2_bf16 && a->E_bf16 && a->Y_bf16 && a->w && a->out && a->bad_id_flag,
+               "nr_kcnn_encoder_fwd: null operand");
+    if (a->n_seq == 0) return 0;
+    const cudaStream_t st = as_stream(stream);
+    const int T = a->T, sec = a->ldx / 2, Fs = round_up(a->F, 4);
+    const long long n_tok = a->n_seq * T;
+    const int M = static_cast<int>(n_tok);
+    auto* X2 = static_cast<__nv_bfloat16*>(a->X2_bf16);
+    prof_context("kcnn.fwd");
+    // the two channels side by side in X2: the word rows, then tanh(E M + b) written by the GEMM into the entity section
+    NR_PROPAGATE(gather_rows(a->word_ids, n_tok, T, a->word_table_bf16, a->V, a->d, sec, X2, a->ldx, 0, DropoutCfg{}, a->bad_id_flag, st));
+    NR_PROPAGATE(gather_rows(a->entity_ids, n_tok, T, a->entity_table_bf16, a->Ve, a->de, a->lde, a->E_bf16, a->lde, 0, DropoutCfg{},
+                             a->bad_id_flag, st));
+    NR_PROPAGATE(gemm_store({.A = a->E_bf16, .M = M, .lda = a->lde, .W = a->mT_bf16, .N = a->d, .ldw = a->lde, .K = a->de},
+                            {.out = X2 + sec, .ld_out = a->ldx, .out_bf16 = 1, .tanh = 1, .bias = a->mb, .ones_col = a->d,
+                             .ones_zero_upto = sec}, st));
+    NR_CHECK_CUDA(cudaMemsetAsync(a->out, 0, sizeof(float) * a->n_seq * a->ldo, st));  // the section padding columns
+    long long row0 = 0;
+    int tap0 = 0;
+    for (int w = 0; w < a->n_win; ++w) {
+        const int x = a->win[w], L = T + 1 - x;
+        auto* Y = static_cast<__nv_bfloat16*>(a->Y_bf16) + row0 * a->ldf;
+        // position p of a title = sum_s W_s . X2[p + s]: the rows p > T - x read the next title and are dropped by the row map
+        NR_PROPAGATE(gemm_store({.A = X2, .M = M, .lda = a->ldx, .W = static_cast<const __nv_bfloat16*>(a->wconv_bf16) +
+                                     static_cast<size_t>(tap0) * a->F * a->ldx, .N = a->F, .ldw = a->ldx, .K = a->ldx, .taps = x,
+                                 .w_tap_rows = a->F, .tap_origin = 0},
+                                {.out = Y, .ld_out = a->ldf, .out_bf16 = 1, .relu = 1, .bias = a->bconv + w * a->F, .rm = {T, 0, L, L, 0},
+                                 .ones_col = a->F, .ones_zero_upto = a->ldf}, st));
+        NR_PROPAGATE(gemm_additive_pool(Y, static_cast<int>(a->n_seq * L), a->ldf, a->F, a->wa_bf16, a->q, a->ldf, a->ba, a->qv, L,
+                                        a->out + w * Fs, a->ldo, a->w + row0, st));
+        row0 += a->n_seq * L;
+        tap0 += x;
+    }
+    return 0;
+}
+
+struct KcnnBwdWorkspace : WorkspaceLayout {
+    float* dscore;
+    __nv_bfloat16 *dpre, *dY, *dZ;  // dY: every window's section in the T-row layout; dZ: the entity channel before tanh
+    KcnnBwdWorkspace(void* base, long long n_seq, int T, int d, int F, int q, int n_win)
+        : WorkspaceLayout{static_cast<char*>(base)}, dscore(take<float>(n_seq * T)), dpre(take<__nv_bfloat16>(n_seq * T * round_up(q, 16))),
+          dY(take<__nv_bfloat16>(n_seq * T * n_win * round_up(F + 1, 8))), dZ(take<__nv_bfloat16>(n_seq * T * round_up(d + 1, 8))) {}
+};
+long long nr_kcnn_encoder_bwd_workspace(long long n_seq, int T, int d, int F, int q, int n_win) {
+    return KcnnBwdWorkspace(nullptr, n_seq, T, d, F, q, n_win).bytes();
+}
+
+int nr_kcnn_encoder_bwd(const nr_kcnn_encoder_bwd_args* a, void* stream) {
+    NR_REQUIRE(a != nullptr, "nr_kcnn_encoder_bwd: null args");
+    NR_PROPAGATE(check_kcnn_shape(a));
+    NR_REQUIRE(a->ldq == round_up(a->q, 16), "nr_kcnn_encoder_bwd: ldq=%d (must be round_up(q, 16))", a->ldq);
+    NR_REQUIRE(a->word_ids && a->entity_ids && a->wT_word_bf16 && a->wT_entity_bf16 && a->m_bf16 && a->wa_bf16 && a->waT_bf16 && a->ba &&
+                   a->qv && a->X2_bf16 && a->E_bf16 && a->Y_bf16 && a->w && a->dout && a->dWconv_ext && a->dM_ext && a->dWa_ext && a->dqv &&
+                   a->dword && a->dentity && a->workspace, "nr_kcnn_encoder_bwd: null operand");
+    const KcnnBwdWorkspace ws(a->workspace, a->n_seq, a->T, a->d, a->F, a->q, a->n_win);
+    NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_kcnn_encoder_bwd: workspace too small");
+    if (a->n_seq == 0) return 0;
+    const cudaStream_t st = as_stream(stream);
+    const int T = a->T, sec = a->ldx / 2, Fs = round_up(a->F, 4), ldy = a->n_win * a->ldf;
+    const int M = static_cast<int>(a->n_seq * T);
+    const auto* X2 = static_cast<const __nv_bfloat16*>(a->X2_bf16);
+    prof_context("kcnn.bwd");
+    // the rows past each window's last position and the section padding stay 0: the taps below read them
+    NR_CHECK_CUDA(cudaMemsetAsync(ws.dY, 0, sizeof(__nv_bfloat16) * M * ldy, st));
+    long long row0 = 0;
+    int tap0 = 0;
+    for (int w = 0; w < a->n_win; ++w) {
+        const int x = a->win[w], L = T + 1 - x, Mw = static_cast<int>(a->n_seq * L);
+        const auto* Y = static_cast<const __nv_bfloat16*>(a->Y_bf16) + row0 * a->ldf;
+        const float* wr = a->w + row0;
+        const float* dout = a->dout + w * Fs;
+        __nv_bfloat16* dYw = ws.dY + w * a->ldf;
+        // the padding columns of dout are 0, so the dot over Fs columns (Y's ones column included) is the dot over F
+        NR_PROPAGATE(pool_dscore(Y, a->ldf, Fs, a->n_seq, L, wr, dout, a->ldo, ws.dscore, st));
+        NR_PROPAGATE(gemm_additive_dpre(Y, Mw, a->ldf, a->F, a->wa_bf16, a->q, a->ldf, a->ba, a->qv, ws.dscore, ws.dpre, a->ldq, a->dqv, st));
+        NR_PROPAGATE(gemm_pool_dinput({.A = ws.dpre, .M = Mw, .lda = a->ldq, .W = a->waT_bf16, .N = a->F, .ldw = a->ldq, .K = a->q},
+                                      {.w = wr, .dout = dout, .ldo = a->ldo, .seg_len = L, .dx = dYw, .ld_dx = ldy, .rm = {L, 0, L, T, 0},
+                                       .relu_src = Y, .relu_ld = a->ldf}, st));
+        NR_PROPAGATE(gemm_weight_grad(ws.dpre, Mw, a->q, a->ldq, Y, a->F, a->ldf, a->dWa_ext, st));
+        // dW_(w,s) = dY_w^T . X2[rows + s]; the entity section's ones column makes column sec + d the bias gradient
+        for (int s = 0; s < x; ++s)
+            NR_PROPAGATE(gemm_weight_grad(dYw, M, a->F, ldy, X2, sec + a->d, a->ldx,
+                                          a->dWconv_ext + static_cast<size_t>(tap0 + s) * a->F * a->ldx, st, s));
+        row0 += a->n_seq * L;
+        tap0 += x;
+    }
+    // transposed conv of all windows at once: dX2[r] = sum_(w, s) W_(w,s)^T dY_w[r - s], tap s' = max x - 1 - s reads row r + s' - (max x - 1)
+    const int taps = kcnn_max_window(a->win, a->n_win);
+    const GemmOperands tconv{.A = ws.dY, .M = M, .lda = ldy, .W = nullptr, .N = a->d, .ldw = ldy, .K = ldy, .taps = taps, .w_tap_rows = a->d,
+                             .tap_origin = taps - 1};
+    GemmOperands g = tconv;
+    g.W = a->wT_word_bf16;
+    NR_PROPAGATE(gemm_scatter_emb(g, {.ids = a->word_ids, .demb = a->dword, .V = a->V}, st));
+    g.W = a->wT_entity_bf16;
+    NR_PROPAGATE(gemm_store(g, {.out = ws.dZ, .ld_out = sec, .out_bf16 = 1, .dtanh_src = X2 + sec, .dtanh_ld = a->ldx}, st));
+    NR_PROPAGATE(gemm_weight_grad(ws.dZ, M, a->d, sec, a->E_bf16, a->de, a->lde, a->dM_ext, st));
+    return gemm_scatter_emb({.A = ws.dZ, .M = M, .lda = sec, .W = a->m_bf16, .N = a->de, .ldw = sec, .K = a->d},
+                            {.ids = a->entity_ids, .demb = a->dentity, .V = a->Ve}, st);
 }
 
 // ---- generic Linear on dense fp32 rows (topic predictor, element encoder, GRU projections) -------------

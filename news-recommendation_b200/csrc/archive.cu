@@ -440,6 +440,104 @@ __global__ void __launch_bounds__(kThreads, 1) archive_score_bwd_kernel(const __
     if (tid == 0) part_b2[seg] = db2;
 }
 
+// ---- DKN history attention (reference src/model/DKN/attention.py): user = sum_j softmax_j(beta . h_j) h_j -------------------
+// beta = W1[:, F:]^T w2 (the candidate half and both biases cancel in the softmax, include/newsrec_b200.h).  One CTA per user;
+// shared memory: beta, and the user's H scores / weights and their gradients.
+namespace dkn {
+constexpr int kMaxH = 64, kMaxF = 512, kMaxHid = 32;
+
+// beta (F) from the history half of W1 (hidden x 2F) and w2
+__device__ void load_beta(const float* __restrict__ W1, int Hd, const float* __restrict__ w2, int F, float* beta) {
+    for (int f = threadIdx.x; f < F; f += kThreads) {
+        float acc = 0.f;
+        for (int k = 0; k < Hd; ++k) acc = fmaf(__ldg(W1 + static_cast<size_t>(k) * 2 * F + F + f), __ldg(w2 + k), acc);
+        beta[f] = acc;
+    }
+}
+
+// wt[j] = softmax_j(beta . x_j) for the H rows of x (F wide)
+__device__ void history_weights(const float* __restrict__ x, int H, int F, const float* beta, float* wt) {
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+    __syncthreads();  // beta
+    for (int j = wp; j < H; j += kWarps) {
+        float acc = 0.f;
+        for (int f = lane; f < F; f += 32) acc = fmaf(__ldg(x + static_cast<size_t>(j) * F + f), beta[f], acc);
+        acc = warp_sum(acc);
+        if (lane == 0) wt[j] = acc;
+    }
+    __syncthreads();
+    if (wp == 0) warp_softmax(wt, H, 1);
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(kThreads) dkn_user_fwd_kernel(const float* __restrict__ hist, int H, int F, const float* __restrict__ W1,
+                                                                int Hd, const float* __restrict__ w2, float* __restrict__ user) {
+    __shared__ float beta[kMaxF], wt[kMaxH];
+    const float* x = hist + static_cast<size_t>(blockIdx.x) * H * F;
+    load_beta(W1, Hd, w2, F, beta);
+    history_weights(x, H, F, beta, wt);
+    for (int f = threadIdx.x; f < F; f += kThreads) {
+        float acc = 0.f;
+        for (int j = 0; j < H; ++j) acc = fmaf(wt[j], __ldg(x + static_cast<size_t>(j) * F + f), acc);
+        user[static_cast<size_t>(blockIdx.x) * F + f] = acc;
+    }
+}
+
+// dw_j = du . x_j ; ds_j = w_j (dw_j - sum w dw) ; dx_j = w_j du + ds_j beta ; part[b] = dbeta_b = sum_j ds_j x_j
+__global__ void __launch_bounds__(kThreads) dkn_user_bwd_kernel(const float* __restrict__ hist, int H, int F, const float* __restrict__ W1,
+                                                                int Hd, const float* __restrict__ w2, const float* __restrict__ duser,
+                                                                float* __restrict__ dhist, float* __restrict__ part) {
+    __shared__ float beta[kMaxF], du[kMaxF], wt[kMaxH], ds[kMaxH];
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+    const size_t b = blockIdx.x;
+    const float* x = hist + b * H * F;
+    load_beta(W1, Hd, w2, F, beta);
+    for (int f = threadIdx.x; f < F; f += kThreads) du[f] = __ldg(duser + b * F + f);
+    history_weights(x, H, F, beta, wt);
+    for (int j = wp; j < H; j += kWarps) {
+        float acc = 0.f;
+        for (int f = lane; f < F; f += 32) acc = fmaf(__ldg(x + static_cast<size_t>(j) * F + f), du[f], acc);
+        acc = warp_sum(acc);
+        if (lane == 0) ds[j] = acc;
+    }
+    __syncthreads();
+    if (wp == 0) {
+        float t = 0.f;
+        for (int j = lane; j < H; j += 32) t = fmaf(wt[j], ds[j], t);
+        t = warp_sum(t);
+        for (int j = lane; j < H; j += 32) ds[j] = wt[j] * (ds[j] - t);
+    }
+    __syncthreads();
+    for (int f = threadIdx.x; f < F; f += kThreads) {
+        const float uf = du[f], bf = beta[f];
+        float db = 0.f;
+        for (int j = 0; j < H; ++j) {
+            const float xj = __ldg(x + static_cast<size_t>(j) * F + f);
+            dhist[b * H * F + static_cast<size_t>(j) * F + f] = fmaf(wt[j], uf, ds[j] * bf);
+            db = fmaf(ds[j], xj, db);
+        }
+        part[b * F + f] = db;
+    }
+}
+
+// dW1[k][F + f] += w2[k] dbeta[f] ; dw2[k] += sum_f W1[k][F + f] dbeta[f]   (one CTA; dbeta is the ordered sum of the partial rows)
+__global__ void __launch_bounds__(kThreads) dkn_beta_bwd_kernel(int F, const float* __restrict__ W1, int Hd, const float* __restrict__ w2,
+                                                                const float* __restrict__ dbeta, float* __restrict__ dW1,
+                                                                float* __restrict__ dw2) {
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+    for (int e = threadIdx.x; e < Hd * F; e += kThreads) {
+        const int k = e / F, f = e - k * F;
+        dW1[static_cast<size_t>(k) * 2 * F + F + f] += __ldg(w2 + k) * dbeta[f];
+    }
+    for (int k = wp; k < Hd; k += kWarps) {
+        float acc = 0.f;
+        for (int f = lane; f < F; f += 32) acc = fmaf(__ldg(W1 + static_cast<size_t>(k) * 2 * F + F + f), dbeta[f], acc);
+        acc = warp_sum(acc);
+        if (lane == 0) dw2[k] += acc;
+    }
+}
+}  // namespace dkn
+
 }  // namespace archive
 
 using namespace archive;
@@ -591,6 +689,59 @@ int nr_archive_score_bwd(const float* news, long long n_news, int F, const long 
     NR_PROPAGATE(sum_over_seq(pb1, n_seg, Hd, db1, st));
     NR_PROPAGATE(sum_over_seq(pw2, n_seg, Hd, dw2, st));
     return sum_over_seq(pb2, n_seg, 1, db2, st);
+}
+
+static int check_dkn_user(long long B, int H, int F, int Hd) {
+    ARCHIVE_BOUNDS(B >= 0 && B < (1ll << 31) && H >= 1 && H <= dkn::kMaxH && F >= 1 && F <= dkn::kMaxF && Hd >= 1 && Hd <= dkn::kMaxHid,
+                   "dkn user: shape outside the supported bounds (B=%lld H=%d F=%d hidden=%d; need 1 <= H <= %d, 1 <= F <= %d, "
+                   "1 <= hidden <= %d)", B, H, F, Hd, dkn::kMaxH, dkn::kMaxF, dkn::kMaxHid);
+    return 0;
+}
+
+int nr_dkn_user_fwd(const float* hist, long long B, int H, int F, const float* W1, int Hd, const float* w2, float* user, void* stream) {
+    NR_PROPAGATE(check_dkn_user(B, H, F, Hd));
+    NR_REQUIRE(hist && W1 && w2 && user, "nr_dkn_user_fwd: null operand");
+    if (B == 0) return 0;
+    const cudaStream_t st = as_stream(stream);
+    prof_context("dkn.fwd");
+    ProfScope ps("dkn_user_fwd", static_cast<int>(B), H, F, st);
+    dkn::dkn_user_fwd_kernel<<<static_cast<unsigned>(B), kThreads, 0, st>>>(hist, H, F, W1, Hd, w2, user);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+long long nr_dkn_user_bwd_workspace(long long B, int F) {
+    WorkspaceLayout ws{nullptr};
+    ws.take<float>(B * F);
+    ws.take<float>(F);
+    return ws.bytes();
+}
+
+int nr_dkn_user_bwd(const float* hist, long long B, int H, int F, const float* W1, int Hd, const float* w2, const float* duser, float* dhist,
+                    float* dW1, float* dw2, void* workspace, long long workspace_bytes, void* stream) {
+    NR_PROPAGATE(check_dkn_user(B, H, F, Hd));
+    NR_REQUIRE(hist && W1 && w2 && duser && dhist && dW1 && dw2 && workspace, "nr_dkn_user_bwd: null operand");
+    NR_REQUIRE(workspace_bytes >= nr_dkn_user_bwd_workspace(B, F), "nr_dkn_user_bwd: workspace too small");
+    if (B == 0) return 0;
+    const cudaStream_t st = as_stream(stream);
+    prof_context("dkn.bwd");
+    WorkspaceLayout ws{static_cast<char*>(workspace)};
+    float* part = ws.take<float>(B * F);
+    float* dbeta = ws.take<float>(F);
+    {
+        ProfScope ps("dkn_user_bwd", static_cast<int>(B), H, F, st);
+        dkn::dkn_user_bwd_kernel<<<static_cast<unsigned>(B), kThreads, 0, st>>>(hist, H, F, W1, Hd, w2, duser, dhist, part);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    NR_CHECK_CUDA(cudaMemsetAsync(dbeta, 0, sizeof(float) * F, st));
+    NR_PROPAGATE(sum_over_seq(part, B, F, dbeta, st));
+    ProfScope ps("dkn_beta_bwd", static_cast<int>(B), Hd, F, st);
+    dkn::dkn_beta_bwd_kernel<<<1, kThreads, 0, st>>>(F, W1, Hd, w2, dbeta, dW1, dw2);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 }  // extern "C"

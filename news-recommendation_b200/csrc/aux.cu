@@ -119,9 +119,10 @@ __device__ __forceinline__ float drop_mult(uint64_t seed, uint32_t thresh, float
 constexpr int kGatherThreads = 320;
 __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long long* __restrict__ ids, long long n_tok, int T,
                                                                    const uint4* __restrict__ table, int V, int D, int ld,
-                                                                   uint4* __restrict__ X, int padded, float p, uint64_t seed,
-                                                                   int* bad_flag) {
-    const int chunks = ld >> 3;  // 16-byte chunks per row
+                                                                   uint4* __restrict__ X, int ld_x, int padded, float p,
+                                                                   uint64_t seed, int* bad_flag) {
+    const int chunks = ld >> 3;  // 16-byte chunks per table row
+    const int x_chunks = ld_x >> 3;
     const int rows_per_it = kGatherThreads / chunks;
     const int rl = threadIdx.x / chunks, c = threadIdx.x - rl * chunks;
     if (rl >= rows_per_it) return;
@@ -153,7 +154,7 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long 
         if (p > 0.f) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const uint64_t bits = dropout_bits4(seed, static_cast<uint64_t>(xr) * (ld >> 2) + (col >> 2) + h);  // ld % 8 == 0
+                const uint64_t bits = dropout_bits4(seed, static_cast<uint64_t>(xr) * (ld_x >> 2) + (col >> 2) + h);  // ld_x % 8 == 0
                 const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
                 float2 f0 = unpack_bf16x2(w[2 * h]), f1 = unpack_bf16x2(w[2 * h + 1]);
                 f0.x *= ((lo & 0xffffu) >= thresh) ? scale : 0.f;
@@ -168,23 +169,23 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long 
             __nv_bfloat16* e = reinterpret_cast<__nv_bfloat16*>(w);
             for (int j = D - col; j < 8; ++j) e[j] = __float2bfloat16_rn(j == D - col ? 1.0f : 0.f);
         }
-        X[xr * chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
+        X[xr * x_chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
         if (padded) {
-            if (t == 0) X[(xr - 1) * chunks + c] = make_uint4(0, 0, 0, 0);
-            if (t == T - 1) X[(xr + 1) * chunks + c] = make_uint4(0, 0, 0, 0);
+            if (t == 0) X[(xr - 1) * x_chunks + c] = make_uint4(0, 0, 0, 0);
+            if (t == T - 1) X[(xr + 1) * x_chunks + c] = make_uint4(0, 0, 0, 0);
         }
     }
 }
 int gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld_table, void* X,
                 int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream) {
     if (n_tok == 0) return 0;
-    NR_REQUIRE(ld_table == ld_x && ld_x % 8 == 0 && ld_x >= D + 1 && ld_x / 8 <= kGatherThreads,
+    NR_REQUIRE(ld_table % 8 == 0 && ld_x % 8 == 0 && ld_x >= ld_table && ld_table >= D + 1 && ld_table / 8 <= kGatherThreads,
                "gather_rows: pitch %d/%d for D=%d", ld_table, ld_x, D);
-    const int rows_per_it = kGatherThreads / (ld_x / 8);
+    const int rows_per_it = kGatherThreads / (ld_table / 8);
     const int blocks = static_cast<int>(std::min<long long>((n_tok + rows_per_it - 1) / rows_per_it, 148 * 6));
     ProfScope ps("gather_rows", static_cast<int>(n_tok), D, ld_x, stream);
-    gather_rows_kernel<<<blocks, kGatherThreads, 0, stream>>>(ids, n_tok, T, static_cast<const uint4*>(table), V, D, ld_x,
-                                                   static_cast<uint4*>(X), padded, drop.p, drop.seed, bad_id_flag);
+    gather_rows_kernel<<<blocks, kGatherThreads, 0, stream>>>(ids, n_tok, T, static_cast<const uint4*>(table), V, D, ld_table,
+                                                   static_cast<uint4*>(X), ld_x, padded, drop.p, drop.seed, bad_id_flag);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -226,7 +226,7 @@ int make_tmap_bytes_2d(CUtensorMap* out, const void* base, int64_t rows, int64_t
 // ------------------------------------------------------------------------------------------------
 int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B, int N, int ldb, int K, int taps,
                  int b_tap_rows, int rows_per_tile, int sms, int max_slices, int epi_smem_bytes, int max_n_stride) {
-    NR_REQUIRE(M >= 0 && N >= 1 && K >= 1 && taps >= 1 && rows_per_tile >= 1 && rows_per_tile <= kTileM,
+    NR_REQUIRE(M >= 0 && N >= 1 && K >= 1 && taps >= 1 && taps <= 4 && rows_per_tile >= 1 && rows_per_tile <= kTileM,
                "plan_gemm_nt: bad shape M=%d N=%d K=%d taps=%d rpt=%d", M, N, K, taps, rows_per_tile);
     NR_REQUIRE(sms > 0, "no CUDA device (SM count unknown)");
     GemmNTParams& p = plan->p;
@@ -238,6 +238,7 @@ int plan_gemm_nt(GemmNTPlan* plan, const void* A, int M, int lda, const void* B,
     p.K = K;
     p.k_chunks = ceil_div(K, kChunkK);
     p.taps = taps;
+    p.tap_origin = taps / 2;
     p.b_tap_rows = b_tap_rows;
 #ifdef NEWSREC_TRIAGE
     static const int dbg_flags = [] { const char* v = getenv("NEWSREC_GEMM_DBG"); return v != nullptr ? atoi(v) : 0; }();
@@ -293,7 +294,7 @@ __global__ void gemm_nt_simt_acc_kernel(const __nv_bfloat16* A, int lda, const _
     const int n = blockIdx.x * 128 + threadIdx.x;
     const int tile = blockIdx.y;
     if (n >= p.dbg_ld) return;
-    const int shift = p.taps / 2;
+    const int shift = p.tap_origin;
     for (int r = 0; r < kTileM; ++r) {
         float acc = 0.f;
         if (n < p.N) {
@@ -616,12 +617,21 @@ bool gemm_store_lo_supported(int N, int K, int lo_col0) {
     return lo_col0 >= 0 && lo_col0 < N && lo_plane_chunk_aligned(plan.p, lo_col0);
 }
 
+// the operands' tap origin (GemmOperands::tap_origin) over the planner's centred default
+static int apply_tap_origin(GemmNTPlan& plan, const GemmOperands& g) {
+    if (g.tap_origin < 0) return 0;
+    NR_REQUIRE(g.tap_origin < g.taps, "gemm: tap origin %d outside %d taps", g.tap_origin, g.taps);
+    plan.p.tap_origin = g.tap_origin;
+    return 0;
+}
+
 int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
     if (g.M == 0) return 0;
     const int M = g.M, N = g.N, rows_per_tile = std::min(c.rows_per_tile, kTileM);  // every row is owned by exactly one tile
     GemmNTPlan plan;
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, N, g.ldw, g.K, g.taps, g.w_tap_rows, rows_per_tile, num_sms(), 0,
                               kEpiSmemBytes<EpiStore>, 0));
+    NR_PROPAGATE(apply_tap_origin(plan, g));
     NR_REQUIRE(c.out_bf16 ? (c.ld_out % 8 == 0) : (c.ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", c.ld_out);
     EpiStore e;
     memset(&e, 0, sizeof(e));
@@ -646,6 +656,13 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
     e.out_bf16 = c.out_bf16;
     e.bias = c.bias;
     e.relu = c.relu;
+    NR_REQUIRE(!(c.relu && c.tanh), "gemm_store: one activation at a time");
+    e.act_tanh = c.tanh;
+    if (c.dtanh_src != nullptr)
+        NR_REQUIRE(c.dtanh_ld % 2 == 0 && (reinterpret_cast<uintptr_t>(c.dtanh_src) & 3) == 0,
+                   "gemm_store: the tanh-backward source needs 4-byte aligned column pairs (ld=%d)", c.dtanh_ld);
+    e.dtanh_src = static_cast<const __nv_bfloat16*>(c.dtanh_src);
+    e.dtanh_ld = c.dtanh_ld;
     e.N = N;
     e.rm = to_rm(c.rm);
     e.drop = to_drop(c.drop);
@@ -799,6 +816,7 @@ int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t
     GemmNTPlan plan;  // every row is computed independently: whole tiles
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, g.M, g.lda, g.W, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                               kEpiSmemBytes<EpiScatter>, 0));
+    NR_PROPAGATE(apply_tap_origin(plan, g));
     const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = to_drop(c.drop), .drop_ld = c.drop_ld};
     const int num_tiles = plan.p.num_m_tiles;
     // [0, num_tiles) flags | ticket | list (count + tiles); stream-ordered, so the buffer lives exactly as long as the two launches

@@ -256,6 +256,9 @@ struct EpiStore {
     int out_bf16;
     const float* bias;  // may be null
     int relu;
+    int act_tanh;       // y = tanh(acc + bias)
+    const __nv_bfloat16* dtanh_src;  // non-null: y *= 1 - t^2, t = dtanh_src[output row][output column] (pitch dtanh_ld)
+    int dtanh_ld;
     int N;              // total valid columns
     RowMap rm;
     Dropout drop;
@@ -330,6 +333,23 @@ struct EpiStore {
                 if (relu) {
 #pragma unroll
                     for (int k = 0; k < 16; ++k) y[k] = fmaxf(y[k], 0.f);
+                }
+                if (act_tanh) {
+#pragma unroll
+                    for (int k = 0; k < 16; ++k) y[k] = fast_tanh(y[k]);
+                }
+                if (dtanh_src != nullptr) {
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int lc = lc0 + 8 * jj + 2 * (lane & 3);
+                            if (!v[e] || lc >= f.ncols) continue;
+                            const float2 t = unpack_bf16x2(
+                                __ldg(reinterpret_cast<const unsigned*>(dtanh_src + orow[e] * dtanh_ld + f.col0 + lc)));
+                            y[4 * jj + 2 * e] *= 1.f - t.x * t.x;
+                            y[4 * jj + 2 * e + 1] *= 1.f - t.y * t.y;
+                        }
                 }
                 if (drop.p > 0.f) drop.apply_frag(y, orow, ld, f.col0 + lc0);
                 if (out_bf16) {

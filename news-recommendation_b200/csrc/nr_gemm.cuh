@@ -4,8 +4,8 @@
 //            * a CTA's weight slice (<=256 output columns, all K, all conv taps) is loaded ONCE by TMA and stays
 //              resident in shared memory; 64-row activation tiles stream through a TMA/mbarrier ring; two consumer
 //              warpgroups take the CTA's tiles in turn and run a fused epilogue functor on the accumulator rows.
-//            * conv taps: tap s re-loads the A tile shifted by (s - taps/2) rows (zero rows separate
-//              the segments in the padded layout), accumulating into the same registers.
+//            * conv taps: tap s re-loads the A tile shifted by (s - tap_origin) rows (tap_origin = taps/2 for the centred
+//              window, whose padded layout separates the segments by zero rows), accumulating into the same registers.
 //  gemm_tn : D[Ma x Nb] += A[Kr x Ma]^T . B[Kr x Nb]  (both MN-major; weight gradients, Kr = all tokens)
 //            split over Kr (and over Nb past 256 columns) across CTAs, fp32 red.global.add epilogue.
 //
@@ -53,7 +53,8 @@ struct GemmNTParams {
     int n_box;          // rows of one resident weight box (multiple of 32, <=256)
     int K;              // reduction length per tap (elements)
     int k_chunks;       // ceil(K/64)
-    int taps;           // 1, or 3 for the window-3 title CNN
+    int taps;           // 1 .. 4 conv taps (3 for the window-3 title CNN)
+    int tap_origin;     // tap s reads A rows shifted by s - tap_origin (plan_gemm_nt: taps / 2)
     int b_tap_rows;     // row offset between taps inside the weight operand
     int stages;
     int b_stream;       // 1: the weight slice does not fit beside the ring; its (tap, k-chunk) box travels with every A stage
@@ -337,7 +338,7 @@ gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (tile0 >= n_tiles) return;
     const int col0 = slice * p.n_stride;
     const int ncols = min(p.n_stride, p.N - col0);
-    const int tap_shift = p.taps / 2;
+    const int tap_shift = p.tap_origin;
     // tuning counters: [0] producer waits for a free A stage, [1] the CTA's weight slice, [5] kernel; per consumer warpgroup w
     // at [8 + 4w]: +0 waits for its MMA turn, +1 MMA loops incl. waits for A data (turn waits excluded), +2 epilogue, +3 tiles
     long long* tmr = p.timing != nullptr ? p.timing + blockIdx.x * 16 : nullptr;

@@ -18,18 +18,24 @@ struct RowMapCfg {  // see RowMap in nr_epilogues.cuh; seg_in == 0 => identity
 // ---- wgmma GEMMs with fused epilogues (gemm.cu) ------------------------------------------------
 constexpr int kGemmTileRows = 64;  // rows of A per gemm_nt tile
 // Operands of the GEMMs with optional epilogue features, which callers name: gemm_store({.A = X, .M = M, ...}, {.out = Y, ...}, st).
-// A bf16 [M x K] pitch lda (taps 3: the zero-padded CNN layout, tap s reads row r + s - 1); W bf16 [taps * w_tap_rows x K] pitch ldw
+// A bf16 [M x K] pitch lda; W bf16 [taps * w_tap_rows x K] pitch ldw.  Tap s (taps <= 4) reads row r + s - tap_origin of A;
+// tap_origin < 0 is the centred window taps / 2 (taps 3: the zero-padded CNN layout, tap s reads row r + s - 1)
 struct GemmOperands {
     const void* A;
     int M, lda;
     const void* W;
-    int N, ldw, K, taps = 1, w_tap_rows = 0;
+    int N, ldw, K, taps = 1, w_tap_rows = 0, tap_origin = -1;
 };
 
 // out[M x N] = act(A . W^T + bias), bf16 or fp32; the defaults are fp32 "=", identity rows, no dropout
 struct StoreCfg {
     void* out;
     int ld_out, out_bf16 = 0, relu = 0;
+    int tanh = 0;  // act = tanh (fast_tanh, absolute error ~2e-7: far below the bf16 store that follows it)
+    // non-null: the result is multiplied by 1 - t^2, t = dtanh_src[row][col] (bf16, pitch dtanh_ld; the output's own row and
+    // column): the tanh backward through a stored bf16 activation
+    const void* dtanh_src = nullptr;
+    int dtanh_ld = 0;
     const float* bias = nullptr;
     RowMapCfg rm = {};
     DropoutCfg drop = {};
@@ -124,7 +130,8 @@ int rows_to_bf16(const Bf16Rows* jobs, int n_jobs, Bf16Op op, cudaStream_t strea
 inline int rows_to_bf16(const Bf16Rows& job, Bf16Op op, cudaStream_t stream) { return rows_to_bf16(&job, 1, op, stream); }
 // dst[e] += sum_s src[s*L + e] (e < L, s < n_seq): fixed summation order, bit-identical across runs
 int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cudaStream_t stream);
-// X[row(seg,t)] = table_bf16[ids[seg*T+t]] (bit-exact copy), ones column at D, optional dropout, optional padded layout
+// X[row(seg,t)] = table_bf16[ids[seg*T+t]] (bit-exact copy), ones column at D, optional dropout, optional padded layout.
+// X may be wider than the table (ld_x >= ld_table): only its first ld_table columns are written.
 int gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld_table, void* X,
                 int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream);
 // multi-head self attention core on packed Q|K|V bf16 [n_seq*T x ld_qkv]: sections start at columns 0, sec, 2*sec

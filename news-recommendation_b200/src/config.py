@@ -7,7 +7,7 @@ restatement of the knob surface, not a copy of the reference source.
 import os
 
 model_name = os.environ.get("MODEL_NAME", "NRMS")
-SUPPORTED_MODELS = ("NRMS", "NAML", "LSTUR", "TANR", "Exp1", "HiFiArk")  # the hot-path scope of this build (SURVEY.md section 8)
+SUPPORTED_MODELS = ("NRMS", "NAML", "LSTUR", "TANR", "Exp1", "HiFiArk", "DKN")  # the hot-path scope of this build (SURVEY.md section 8)
 if model_name not in SUPPORTED_MODELS:
     raise AssertionError(f"MODEL_NAME={model_name!r}: this build accelerates {SUPPORTED_MODELS} only")
 
@@ -52,6 +52,9 @@ _PER_MODEL = {
                  ensemble_factor=1, precision=os.environ.get("NEWSREC_PRECISION", "accurate")),
     # plain bf16 storage in the news encoder meets the 1e-3 contract (DESIGN.md section 4): no precision knob
     "HiFiArk": dict(dataset_attributes={"news": ["title"], "record": []}, num_pooling_heads=5, regularizer_loss_weight=0.1, **_CNN),
+    # plain bf16 storage meets the 1e-3 contract (DESIGN.md section 4); use_context=True raises (context embeddings unavailable)
+    "DKN": dict(dataset_attributes={"news": ["title", "title_entities"], "record": []}, num_filters=50, window_sizes=[2, 3, 4],
+                use_context=False),
 }
 for _name, _knobs in _PER_MODEL.items():
     globals()[f"{_name}Config"] = type(f"{_name}Config", (BaseConfig,), dict(_knobs))

@@ -71,6 +71,30 @@ class CnnEncoderBwdArgs(C.Structure):
     ]
 
 
+class KcnnEncoderFwdArgs(C.Structure):
+    """nr_kcnn_encoder_fwd_args (include/newsrec_b200.h)."""
+    _fields_ = [
+        ("n_seq", _ll), ("T", _i), ("d", _i), ("de", _i), ("F", _i), ("q", _i), ("n_win", _i), ("win", _i * 4),
+        ("ldx", _i), ("lde", _i), ("ldf", _i), ("ldo", _i),
+        ("word_ids", _vp), ("entity_ids", _vp), ("word_table_bf16", _vp), ("V", _i), ("entity_table_bf16", _vp), ("Ve", _i),
+        ("mT_bf16", _vp), ("mb", _vp), ("wconv_bf16", _vp), ("bconv", _vp), ("wa_bf16", _vp), ("ba", _vp), ("qv", _vp),
+        ("X2_bf16", _vp), ("E_bf16", _vp), ("Y_bf16", _vp), ("w", _vp), ("out", _vp), ("bad_id_flag", _vp),
+    ]
+
+
+class KcnnEncoderBwdArgs(C.Structure):
+    """nr_kcnn_encoder_bwd_args (include/newsrec_b200.h)."""
+    _fields_ = [
+        ("n_seq", _ll), ("T", _i), ("d", _i), ("de", _i), ("F", _i), ("q", _i), ("n_win", _i), ("win", _i * 4),
+        ("ldx", _i), ("lde", _i), ("ldf", _i), ("ldo", _i), ("ldq", _i),
+        ("word_ids", _vp), ("entity_ids", _vp), ("V", _i), ("Ve", _i),
+        ("wT_word_bf16", _vp), ("wT_entity_bf16", _vp), ("m_bf16", _vp), ("wa_bf16", _vp), ("waT_bf16", _vp), ("ba", _vp),
+        ("qv", _vp), ("X2_bf16", _vp), ("E_bf16", _vp), ("Y_bf16", _vp), ("w", _vp), ("dout", _vp),
+        ("dWconv_ext", _vp), ("dM_ext", _vp), ("dWa_ext", _vp), ("dqv", _vp), ("dword", _vp), ("dentity", _vp),
+        ("workspace", _vp), ("workspace_bytes", _ll),
+    ]
+
+
 class GruFwdArgs(C.Structure):
     """nr_gru_fwd_args (include/newsrec_b200.h)."""
     _fields_ = [
@@ -137,6 +161,9 @@ SIGNATURES = {
     "nr_cnn_encoder_fwd": (_i, [C.POINTER(CnnEncoderFwdArgs), _vp]),
     "nr_cnn_encoder_bwd_workspace": (_ll, [_ll, _i, _i, _i]),
     "nr_cnn_encoder_bwd": (_i, [C.POINTER(CnnEncoderBwdArgs), _vp]),
+    "nr_kcnn_encoder_fwd": (_i, [C.POINTER(KcnnEncoderFwdArgs), _vp]),
+    "nr_kcnn_encoder_bwd_workspace": (_ll, [_ll, _i, _i, _i, _i, _i]),
+    "nr_kcnn_encoder_bwd": (_i, [C.POINTER(KcnnEncoderBwdArgs), _vp]),
     "nr_linear_rows_fwd": (_i, [_vp, _ll, _i, _ll, _ll, _vp, _i, _vp, _i, _i, _vp, _i, _vp, _i, _vp]),
     "nr_linear_rows_bwd": (_i, [_vp, _vp, _ll, _i, _i, _vp, _i, _vp, _i, _i, _vp, _i, _vp, _vp, _i, _vp]),
     "nr_embedding_f32_fwd": (_i, [_vp, _ll, _vp, _i, _i, _vp, _vp, _vp]),
@@ -154,6 +181,9 @@ SIGNATURES = {
     "nr_archive_score_bwd_workspace": (_ll, [_ll, _i, _i]),
     "nr_archive_score_bwd": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp,
                                    _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "nr_dkn_user_fwd": (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _vp, _vp]),
+    "nr_dkn_user_bwd_workspace": (_ll, [_ll, _i]),
+    "nr_dkn_user_bwd": (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
 }
 
 _lib = None

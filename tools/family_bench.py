@@ -31,6 +31,9 @@ def slots(n, seed, cfg, want):
         d = {}
         if "title" in want:
             d["title"] = torch.randint(1, cfg.num_words, (B, T), generator=g).to(dev)
+        if "title_entities" in want:  # MIND-like: most tokens carry no entity (id 0)
+            ents = torch.randint(1, cfg.num_entities, (B, T), generator=g)
+            d["title_entities"] = (ents * (torch.rand((B, T), generator=g) < 0.25)).to(dev)
         if "abstract" in want:
             d["abstract"] = torch.randint(1, cfg.num_words, (B, TA), generator=g).to(dev)
         if "category" in want:
@@ -48,6 +51,7 @@ CASES = [
     ("LSTUR", {"long_short_term_method": "con"}, ("title", "category")),
     ("Exp1", {}, ("title", "category")),
     ("HiFiArk", {}, ("title",)),
+    ("DKN", {}, ("title", "title_entities")),
 ]
 # weight of the second element of a tuple output in the training loss, per family (reference train.py)
 AUX_LOSS_WEIGHT = {"TANR": "topic_classification_loss_weight", "HiFiArk": "regularizer_loss_weight"}
@@ -93,11 +97,13 @@ for name, over, want in CASES:
     ms = e0.elapsed_time(e1) / 5
     key = name + ("/" + over["long_short_term_method"] if over else "")
     res[key] = {"ms_per_step": round(ms, 3), "impressions_per_s": round(B / ms * 1e3), "launches_per_step": (newsrec_b200.launch_count() - l0) // 5}
-    if name == "HiFiArk":  # the kernels after the news encoder (the news encoder is TANR's: compare the two step times)
+    # Hi-Fi Ark: the kernels after the news encoder (the news encoder is TANR's: compare the two step times); DKN: all of them
+    kernel_keys = {"HiFiArk": ("archive",), "DKN": ("kcnn", "dkn", "archive")}.get(name)
+    if kernel_keys:
         newsrec_b200.load_library().nr_profile_enable(1)
         step()
         torch.cuda.synchronize()
-        res[key]["kernels_ms"] = {k: round(v[1], 4) for k, v in newsrec_b200.profile_report().items() if "archive" in k}
+        res[key]["kernels_ms"] = {k: round(v[1], 4) for k, v in newsrec_b200.profile_report().items() if k.startswith(kernel_keys)}
         newsrec_b200.load_library().nr_profile_enable(0)
     print(key, res[key], flush=True)
     del model, grads
