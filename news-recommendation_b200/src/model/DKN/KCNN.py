@@ -16,6 +16,9 @@ class KCNN(torch.nn.Module):
         self.config = config
         if config.use_context:  # the reference marks context embeddings as unavailable
             raise NewsrecError("DKN use_context=True: context embeddings are not supported (DESIGN.md section 6)")
+        wins = list(config.window_sizes)
+        if not 1 <= len(wins) <= 4 or not all(1 <= x <= 4 for x in wins):  # the reference takes any; the kernels 1 .. 4 of 1 .. 4
+            raise NewsrecError(f"DKN window_sizes={wins}: the KCNN kernels take 1 to 4 windows of 1 to 4 words (include/newsrec_b200.h)")
         if pretrained_word_embedding is None:
             self.word_embedding = nn.Embedding(config.num_words, config.word_embedding_dim, padding_idx=0)
         else:

@@ -160,6 +160,10 @@ def main(argv=None):
     args = ap.parse_args(argv)
 
     rank, world, local = _env_int("RANK", 0), _env_int("WORLD_SIZE", 1), _env_int("LOCAL_RANK", 0)
+    # the ranks share one stdout pipe: with block buffering a flush can end mid-line and another rank's output then lands
+    # inside that line (train.py's loss lines run together); line buffering makes every line one write, which a pipe keeps whole
+    if world > 1 and hasattr(sys.stdout, "reconfigure"):
+        sys.stdout.reconfigure(line_buffering=True)
     if "CUDA_VISIBLE_DEVICES" not in os.environ or os.environ.get("NEWSREC_PIN_GPU", "1") == "1":
         vis = os.environ.get("CUDA_VISIBLE_DEVICES")
         if vis is None:

@@ -1,6 +1,10 @@
 """CPU oracle for DKN (reference src/model/DKN/**, general/click_predictor/DNN.py).  TEST INFRASTRUCTURE ONLY, like
 newsrec_oracle.py.  Pinned against tests/golden/dkn.npz (oracle/make_golden_dkn.py).
 
+The windows are a list in the order of config.window_sizes, repeats kept: the reference runs one Conv2d per entry (a repeated
+size runs the same conv twice) and concatenates the pooled vectors in that order.  The state_dict holds one conv per distinct
+size, so the order cannot be read back from it.
+
 Contract sites (newsrec_oracle.Contract) where the kernels store bf16: the word and entity rows and the transform matrix M
 (operands), tanh(E M + b) (stored in the entity section of X2), the conv weights (operands), the conv output (stored), and the
 attention weight Wa (operand).  Everything after the news encoder is fp32.
@@ -18,6 +22,7 @@ WINDOWS = (2, 3, 4)
 
 
 def dkn_shapes(V, VE, d=300, de=100, q=200, Fn=50, windows=WINDOWS):
+    """One conv per distinct window size (the reference's ModuleDict); the DNN widths count every entry of `windows`."""
     s = {"kcnn.word_embedding.weight": (V, d), "kcnn.entity_embedding.weight": (VE, de),
          "kcnn.transform_matrix": (de, d), "kcnn.transform_bias": (d,)}
     for x in windows:
@@ -44,18 +49,15 @@ def synth_entities(titles, VE, seed):
     return ids * keep * (titles != 0)
 
 
-def windows_of(p):
-    return sorted(int(k.split(".")[2]) for k in p if k.startswith("kcnn.conv_filters.") and k.endswith(".weight"))
-
-
-def kcnn(title, entities, p, c: O.Contract = O.EXACT):
-    """KCNN.py:56-117 (use_context=False).  title, entities (N, T) -> (N, len(windows) * F)."""
+def kcnn(title, entities, p, c: O.Contract = O.EXACT, windows=WINDOWS):
+    """KCNN.py:56-117 (use_context=False).  title, entities (N, T) -> (N, len(windows) * F), window after window in the
+    order of `windows`."""
     wv = O.embedding(title, p["kcnn.word_embedding.weight"], c)
     ev = O.embedding(entities, p["kcnn.entity_embedding.weight"], c)
     t = c.act(torch.tanh(torch.matmul(ev, c.operand(p["kcnn.transform_matrix"])) + p["kcnn.transform_bias"]))
     x2 = torch.stack([wv, t], dim=1)
     pooled = []
-    for x in windows_of(p):
+    for x in windows:
         y = F.conv2d(x2, c.operand(p[f"kcnn.conv_filters.{x}.weight"]), p[f"kcnn.conv_filters.{x}.bias"]).squeeze(3)
         y = c.act(F.relu(y).transpose(1, 2))
         pooled.append(O.additive_attention(y, p, "kcnn.additive_attention", c))
@@ -86,19 +88,22 @@ def score(cand, user, p):
     return F.linear(h, p["click_predictor.dnn.2.weight"], p["click_predictor.dnn.2.bias"]).squeeze(1)
 
 
-def dkn_forward(cand_title, cand_ent, clicked_title, clicked_ent, p, c: O.Contract = O.EXACT):
+def dkn_forward(cand_title, cand_ent, clicked_title, clicked_ent, p, c: O.Contract = O.EXACT, windows=WINDOWS):
     """__init__.py:26-64.  (B, C, T) / (B, H, T) id tensors -> (logits (B, C), cand vectors, clicked vectors, user (B, F'))."""
     B, C, T = cand_title.shape
     H = clicked_title.shape[1]
-    cv = kcnn(cand_title.reshape(B * C, T), cand_ent.reshape(B * C, T), p, c).view(B, C, -1)
-    hv = kcnn(clicked_title.reshape(B * H, T), clicked_ent.reshape(B * H, T), p, c).view(B, H, -1)
+    cv = kcnn(cand_title.reshape(B * C, T), cand_ent.reshape(B * C, T), p, c, windows).view(B, C, -1)
+    hv = kcnn(clicked_title.reshape(B * H, T), clicked_ent.reshape(B * H, T), p, c, windows).view(B, H, -1)
     u = user_vector(hv, p)
     Fp = cv.shape[2]
     logits = score(cv.reshape(B * C, Fp), u.repeat_interleave(C, dim=0), p).view(B, C)
     return logits, cv, hv, u
 
 
-def get_prediction(cand, clicked, p):
-    """__init__.py:90-104: cand (n, F'), clicked (H, F') -> (n,)."""
+def get_prediction(cand, clicked, p, windows=WINDOWS):
+    """__init__.py:90-104: cand (n, F'), clicked (H, F') -> (n,), F' = len(windows) * F."""
+    Fp = len(windows) * p["kcnn.additive_attention.linear.weight"].shape[1]
+    if cand.shape[-1] != Fp or clicked.shape[-1] != Fp:
+        raise ValueError(f"news vectors of width {cand.shape[-1]} / {clicked.shape[-1]} for {len(windows)} windows of {Fp // len(windows)}")
     u = user_vector(clicked.unsqueeze(0), p)
     return score(cand, u.expand(cand.shape[0], -1), p)

@@ -46,18 +46,21 @@ def make_cfg(VE, **kw):
     return type("Cfg", (config.DKNConfig,), dict(dict(num_words=V, num_entities=VE, num_clicked_news_a_user=6), **kw))
 
 
-def build(g):
+GOLDEN = {"dkn": (2, 3, 4), "dkn_w4133": (4, 1, 3, 3)}  # golden case -> config.window_sizes it was minted at
+
+
+def build(g, windows=DO.WINDOWS):
     from model.DKN import DKN
     VE = int(g["num_entities"])
     torch.manual_seed(0)
-    model = DKN(make_cfg(VE)).to(DEV)
-    model.load_state_dict(DO.dkn_state_dict(V, VE, int(g["seed"])))
+    model = DKN(make_cfg(VE, window_sizes=list(windows))).to(DEV)
+    model.load_state_dict(DO.dkn_state_dict(V, VE, int(g["seed"]), windows=windows))
     return model
 
 
-def params(g, requires_grad=True, dtype=torch.float32):
+def params(g, requires_grad=True, dtype=torch.float32, windows=DO.WINDOWS):
     return {k: v.to(dtype).clone().requires_grad_(requires_grad)
-            for k, v in DO.dkn_state_dict(V, int(g["num_entities"]), int(g["seed"])).items()}
+            for k, v in DO.dkn_state_dict(V, int(g["num_entities"]), int(g["seed"]), windows=windows).items()}
 
 
 def ids(g):
@@ -68,17 +71,17 @@ def slots(t, e):
     return [{"title": t[:, j].contiguous(), "title_entities": e[:, j].contiguous()} for j in range(t.shape[1])]
 
 
-def test_golden_case():
-    g = load_case("dkn")
-    model = build(g).train()  # DKN has no dropout: train and eval mode compute the same
+def _check_golden_case(case):
+    g, win = load_case(case), GOLDEN[case]
+    model = build(g, win).train()  # DKN has no dropout: train and eval mode compute the same
     ct, ce, ht, he = ids(g)
-    p_b, p_x = params(g), params(g)
-    lb = DO.dkn_forward(ct, ce, ht, he, p_b, O.BF16)[0]
+    p_b, p_x = params(g, windows=win), params(g, windows=win)
+    lb = DO.dkn_forward(ct, ce, ht, he, p_b, O.BF16, win)[0]
     O.click_loss(lb).backward()
-    lx = DO.dkn_forward(ct, ce, ht, he, p_x, O.EXACT)[0]
+    lx = DO.dkn_forward(ct, ce, ht, he, p_x, O.EXACT, win)[0]
     O.click_loss(lx).backward()
     with torch.no_grad():
-        lw = DO.dkn_forward(ct, ce, ht, he, params(g, False), O.WEIGHTS_BF16)[0]
+        lw = DO.dkn_forward(ct, ce, ht, he, params(g, False, windows=win), O.WEIGHTS_BF16, win)[0]
     logits = model(slots(ct, ce), slots(ht, he))
     loss = torch.nn.functional.cross_entropy(logits, torch.zeros(logits.shape[0], dtype=torch.long, device=DEV))
     loss.backward()
@@ -86,15 +89,20 @@ def test_golden_case():
     res = {"contract": relerr(logits, lb), "contract_centred": relerr(centred(logits), centred(lb)),
            "weights_bf16": relerr(logits, lw), "weights_bf16_centred": relerr(centred(logits), centred(lw)),
            "golden": relerr(logits, torch.from_numpy(g["logits"]))}
-    print("dkn golden", res)
+    print(case, "golden", res)
     assert res["contract"] < 1e-3 and res["contract_centred"] < 1e-3, res
     assert res["weights_bf16"] < 1e-3 and res["golden"] < 3e-3, res
-    Fp = 150
+    Fp = len(win) * 50
     worst = 0.0
     for k, prm in model.named_parameters():
         exact = p_x[k].grad
         if k in ("attention.dnn.0.bias", "attention.dnn.1.bias"):  # analytically zero: exact zeros, not rounding noise
             assert prm.grad is not None and bool((prm.grad == 0).all()), k
+            continue
+        if k == "click_predictor.dnn.2.bias":
+            # adds one constant to every logit of an impression, and the cross-entropy's logit gradients sum to 0 over the
+            # candidates: the exact gradient is 0, and every evaluation of it (fp32 oracle, contract, kernels) rounding noise
+            assert float(prm.grad.abs().max()) <= 1e-6 and float(exact.abs().max()) <= 1e-6, (k, prm.grad, exact)
             continue
         if k == "attention.dnn.0.weight":
             assert bool((prm.grad[:, :Fp] == 0).all()), k
@@ -108,6 +116,15 @@ def test_golden_case():
     print("worst gradient error over the contract's", worst)
     assert bool((model.kcnn.word_embedding.weight.grad[0] == 0).all())
     assert bool((model.kcnn.entity_embedding.weight.grad[0] == 0).all())
+
+
+def test_golden_case():
+    _check_golden_case("dkn")
+
+
+def test_golden_case_at_windows_4133():
+    """unsorted windows, a repeated size, window 1 and window 4"""
+    _check_golden_case("dkn_w4133")
 
 
 # ---- the KCNN encoder kernel pair against the fp64 oracle under its contract ---------------------------------------------------
@@ -124,27 +141,38 @@ def kcnn_case(n, T, VE, entities, seed):
     return title, ents
 
 
-@pytest.mark.parametrize("n,T,entities", [(96, 20, "mixed"),      # MIND title length
-                                          (70, 4, "mixed"),       # T = the widest window: one position for it
-                                          (9, 64, "mixed"),       # T = 64: whole pooling tiles per title
-                                          (37, 23, "mixed"),      # segments of 22 / 21 / 20 rows crossing 64-row tiles
-                                          (40, 20, "zero"),       # no entity anywhere: the entity scatter has no live tile
-                                          (40, 20, "last")])      # id = V - 1 in both tables
-def test_kcnn_encoder_against_fp64_contract(n, T, entities):
+def _kcnn_param(n, T, entities, windows=DO.WINDOWS, tag=None):
+    # the cases at the default windows keep the ids they had before the window sets were added
+    return pytest.param(n, T, entities, windows, id=f"{n}-{T}-{entities}" + (f"-{tag}" if tag else ""))
+
+
+@pytest.mark.parametrize("n,T,entities,windows", [
+    _kcnn_param(96, 20, "mixed"),      # MIND title length
+    _kcnn_param(70, 4, "mixed"),       # T = the widest window: one position for it
+    _kcnn_param(9, 64, "mixed"),       # T = 64: whole pooling tiles per title
+    _kcnn_param(37, 23, "mixed"),      # segments of 22 / 21 / 20 rows crossing 64-row tiles
+    _kcnn_param(40, 20, "zero"),       # no entity anywhere: the entity scatter has no live tile
+    _kcnn_param(40, 20, "last"),       # id = V - 1 in both tables
+    _kcnn_param(96, 20, "mixed", (1,), "w1"),                 # one window of one tap
+    _kcnn_param(96, 20, "mixed", (4, 2), "w42"),              # unsorted: the news vector keeps the list's order
+    _kcnn_param(96, 20, "mixed", (3, 3), "w33"),              # a repeated size: one conv, two blocks, two gradient parts
+    _kcnn_param(96, 20, "mixed", (1, 2, 3, 4), "w1234"),      # four windows
+    _kcnn_param(96, 20, "mixed", (4, 1, 3, 3), "w4133")])     # the second golden case's windows
+def test_kcnn_encoder_against_fp64_contract(n, T, entities, windows):
     from model.DKN.KCNN import KCNN
     VE = 30
-    cfg = make_cfg(VE, num_words_title=T)
+    cfg = make_cfg(VE, num_words_title=T, window_sizes=list(windows))
     torch.manual_seed(0)
     enc = KCNN(cfg, None, None, None).to(DEV)
-    sd = {k[len("kcnn."):]: v for k, v in DO.dkn_state_dict(V, VE, 7).items() if k.startswith("kcnn.")}
+    sd = {k[len("kcnn."):]: v for k, v in DO.dkn_state_dict(V, VE, 7, windows=windows).items() if k.startswith("kcnn.")}
     enc.load_state_dict(sd)
     title, ents = kcnn_case(n, T, VE, entities, 1000 + T)
-    dout = O.det_uniform((n, 150), 77, -1, 1, torch.float64)
+    dout = O.det_uniform((n, 50 * len(windows)), 77, -1, 1, torch.float64)
     p_c = {"kcnn." + k: v.double().clone().requires_grad_(True) for k, v in sd.items()}
     p_x = {"kcnn." + k: v.double().clone().requires_grad_(True) for k, v in sd.items()}
-    want = DO.kcnn(title, ents, p_c, O.BF16)
+    want = DO.kcnn(title, ents, p_c, O.BF16, windows)
     (want * dout).sum().backward()
-    exact = DO.kcnn(title, ents, p_x, O.EXACT)
+    exact = DO.kcnn(title, ents, p_x, O.EXACT, windows)
     (exact * dout).sum().backward()
     got = enc.encode_ids(title.to(DEV), ents.to(DEV))
     (got * dout.float().to(DEV)).sum().backward()
@@ -188,6 +216,21 @@ def test_kcnn_refuses_shapes_outside_its_bounds():
         enc.encode_ids(title, torch.zeros_like(title))
     with pytest.raises(NewsrecError):
         KCNN(make_cfg(30, use_context=True), None, None, None)
+
+
+def test_kcnn_refuses_a_window_of_5_before_any_launch():
+    """The reference accepts any window size; the kernels take 1 to 4 taps (include/newsrec_b200.h), so the drop-in refuses
+    a wider window when it is built, not at the first batch."""
+    from newsrec_b200 import NewsrecError
+    from model.DKN import DKN
+    from model.DKN.KCNN import KCNN
+    l0 = int(lib().nr_launch_count())
+    for wins in ([5], [2, 3, 5], [0, 2]):
+        with pytest.raises(NewsrecError, match="window"):
+            KCNN(make_cfg(30, window_sizes=wins), None, None, None)
+        with pytest.raises(NewsrecError, match="window"):
+            DKN(make_cfg(30, window_sizes=wins))
+    assert int(lib().nr_launch_count()) == l0
 
 
 # ---- nr_dkn_user_* through the C ABI --------------------------------------------------------------------------------------------

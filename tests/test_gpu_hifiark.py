@@ -314,6 +314,11 @@ def test_golden_case(train):
             assert prm.grad is None, k
             continue
         exact = p_x[k].grad
+        if k == "click_predictor.dnn.2.bias":
+            # adds one constant to every logit of an impression, and the cross-entropy's logit gradients sum to 0 over the
+            # candidates: the exact gradient is 0, and every evaluation of it (fp32 oracle, contract, kernels) rounding noise
+            assert float(prm.grad.abs().max()) <= 1e-6 and float(exact.abs().max()) <= 1e-6, (k, prm.grad, exact)
+            continue
         e_k = relerr(prm.grad, exact)
         e_c = float((p_b[k].grad - exact).norm() / exact.norm())
         worst = max(worst, e_k / max(e_c, 2e-3))
