@@ -679,9 +679,11 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
 
 int gemm_additive_pool(const void* X, int M, int lda, int D, const void* Wa, int q, int ldw, const float* ba,
                        const float* qv, int seg_len, float* out, int ldo, float* w_out, cudaStream_t stream, const void* X_lo) {
-    if (M == 0) return 0;
+    // the shape is checked before the empty case: seg_len = 0 makes M = n_seg * seg_len = 0 for any n_seg, and the segments'
+    // outputs would be left unwritten without an error
     NR_REQUIRE(seg_len >= 1 && seg_len <= kTileM && M % seg_len == 0, "additive_pool: M=%d seg_len=%d", M, seg_len);
-    NR_REQUIRE(q <= 256 && (D % 2) == 0 && (ldo % 2) == 0, "additive_pool: q=%d D=%d ldo=%d unsupported", q, D, ldo);
+    NR_REQUIRE(q >= 1 && q <= 256 && (D % 2) == 0 && (ldo % 2) == 0, "additive_pool: q=%d D=%d ldo=%d unsupported", q, D, ldo);
+    if (M == 0) return 0;
     const int rpt = (kTileM / seg_len) * seg_len;
     GemmNTPlan plan;
     NR_PROPAGATE(plan_gemm_nt(&plan, X, M, lda, Wa, q, ldw, D, 1, 0, rpt, num_sms(), 1, kEpiSmemBytes<EpiPool>, 0));

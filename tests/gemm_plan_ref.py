@@ -1,0 +1,135 @@
+"""Plain-Python restatement of the wgmma GEMM planners (importable without CUDA).
+
+plan_nt restates plan_gemm_nt (csrc/gemm.cu) line for line and adds the tiles each (CTA, consumer warpgroup) processes under
+gemm_nt_kernel's schedule; plan_tn restates gemm_tn_accumulate and launch_gemm_tn_kernel.  The GPU tests label every case
+with the regime it is there to reach (regimes_nt / regimes_tn), tests/test_gemm_plan_host.py checks those labels here, and
+tests/test_gpu_gemm_elements.py ties this restatement to the real planner through the kernel's per-CTA counters."""
+from __future__ import annotations
+
+# csrc/nr_gemm.cuh
+kSmemLimit = 232448            # kSmemLimit: 227 KB of dynamic shared memory per CTA
+kTileM = 64                    # kTileM: rows per gemm_nt tile (one m64 wgmma)
+kChunkK = 64                   # kChunkK: bf16 elements per 128-byte swizzle row
+kAStageBytes = kTileM * 128    # kAStageBytes: one 64 x 64 bf16 A box, 8 KB
+kMaxStages = 12                # kMaxStages
+# kEpiSmemBytes<Epi> = Epi::kScratchBytes (+ kXposeBytes for a row-view epilogue), csrc/nr_epilogues.cuh
+kXposeBytes = 2 * 2 * kTileM * 16 * 4                  # kXposeBytes (row view: 2 warpgroups x 2 column halves)
+EPI_STORE_SMEM = 1024 + (8 * 6 * 16 * 64 + 1024)       # EpiStore (fragment view): 1 KB bias + FragStore<6> = 51,200 B
+EPI_POOL_SMEM = 4096 + kXposeBytes                     # EpiPool (row view): 4 KB scratch + transpose = 20,480 B
+assert EPI_STORE_SMEM == 51200 and EPI_POOL_SMEM == 20480
+
+H100_SMS = 132                 # H100 SXM5; the GPU tests plan with the device's own count (nr_num_sms)
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def _round_up(a, b):
+    return _cdiv(a, b) * b
+
+
+def plan_nt(M, N, K, taps=1, rows_per_tile=kTileM, sms=H100_SMS, epi_smem_bytes=EPI_STORE_SMEM, max_slices=0, max_stride=0):
+    """plan_gemm_nt: the weight slicing, ring and grid, plus wg_tiles[b][w] = the tiles warpgroup w of CTA b processes
+    (CTA b takes slice b % n_slices and tiles b // n_slices + k * step, step = grid // n_slices; its warpgroup w takes every
+    second one of those, starting at the w-th)."""
+    assert M >= 0 and N >= 1 and K >= 1 and 1 <= taps <= 4 and 1 <= rows_per_tile <= kTileM and sms > 0
+    num_m_tiles = _cdiv(M, rows_per_tile)
+    k_chunks = _cdiv(K, kChunkK)
+    fixed = 1024 + _round_up(epi_smem_bytes, 16) + 512
+    slices, b_stream, bbytes = 1, 0, 0
+    while True:
+        assert slices <= 64, "cannot fit weight slice"
+        n_stride = _round_up(_cdiv(N, slices), 16)
+        n_box = _round_up(min(n_stride, N), 32)
+        if n_box > 256 or (max_stride > 0 and n_stride > max_stride):
+            slices += 1
+            continue
+        bbytes = taps * k_chunks * n_box * 128
+        if bbytes + 6 * kAStageBytes + fixed <= kSmemLimit:
+            break
+        if slices == max_slices or n_box <= 64:
+            if bbytes + 4 * kAStageBytes + fixed > kSmemLimit:
+                b_stream, bbytes = 1, 0
+            break
+        slices += 1
+    n_slices = _cdiv(N, n_stride)
+    stage_bytes = kAStageBytes + (n_box * 128 if b_stream else 0)
+    stages = min(kMaxStages, (kSmemLimit - fixed - bbytes) // stage_bytes)
+    assert stages >= 2
+    groups = max(1, min(sms // n_slices, num_m_tiles))
+    grid = groups * n_slices
+    step = grid // n_slices
+    wg_tiles = []
+    for b in range(grid):
+        t0 = b // n_slices
+        mine = list(range(t0, num_m_tiles, step))
+        wg_tiles.append((mine[0::2], mine[1::2]))
+    return {"n_stride": n_stride, "n_box": n_box, "n_slices": n_slices, "b_stream": b_stream, "stages": stages, "grid": grid,
+            "num_m_tiles": num_m_tiles, "k_chunks": k_chunks, "slice_of": [b % n_slices for b in range(grid)], "wg_tiles": wg_tiles,
+            "N": N, "taps": taps, "rows_per_tile": rows_per_tile}
+
+
+def plan_pool(M, D, q, seg_len, sms=H100_SMS):
+    """gemm_additive_pool's plan: pre = X . Wa^T with N = q, K = D, tiles of whole segments, one weight slice."""
+    return plan_nt(M, q, D, 1, (kTileM // seg_len) * seg_len, sms, EPI_POOL_SMEM, max_slices=1)
+
+
+def plan_tn(Kr, Ma, Nb, sms=H100_SMS, reserved=0):
+    """gemm_tn_accumulate: tiles, columns per CTA (NT), cluster shape and k_slices_max, an upper bound on the k-ranges.  With a
+    cluster the launch further caps k_slices by cudaOccupancyMaxActiveClusters, which only the device can answer, so the
+    exact count is known only there; without one k_slices_max is exact."""
+    assert 1 <= Nb <= 512 and Ma >= 1 and Kr >= 1
+    sms_eff = max(sms // 2, sms - max(0, reserved))
+    m_tiles = _cdiv(Ma, 128)
+    n_tiles = _cdiv(Nb, 256)
+    nt = _round_up(_cdiv(Nb, n_tiles), 64)
+    total_chunks = _cdiv(Kr, 64)
+    cluster = (2 if m_tiles % 2 == 0 else 1, 2 if n_tiles % 2 == 0 else 1)
+    k = max(1, min(sms_eff // (m_tiles * n_tiles), total_chunks))
+    cps = _cdiv(total_chunks, k)
+    return {"m_tiles": m_tiles, "n_tiles": n_tiles, "NT": nt, "cluster": cluster, "total_chunks": total_chunks,
+            "k_slices_max": _cdiv(total_chunks, cps), "exact": cluster == (1, 1)}
+
+
+# ------------------------------------------------------------------------------------------------
+# regimes: the labels the GPU case tables carry
+# ------------------------------------------------------------------------------------------------
+NT_REGIMES = ("1 slice", "slices > 1", "slice width % 32 != 0", "N < 32", "resident >= 6 stages", "resident < 6 stages",
+              "streamed weights", "taps 3", "rows_per_tile < 64", "warpgroup 1 idle", "odd tiles per CTA", "even tiles per CTA")
+TN_REGIMES = ("cluster 1x1", "cluster 2x1", "cluster 1x2", "cluster 2x2", "NT 64", "NT 128", "NT 192", "NT 256", "n_tiles 2",
+              "single k-range")
+
+
+def regimes_nt(p):
+    """Every regime of NT_REGIMES a gemm_nt plan is in."""
+    r = {"1 slice" if p["n_slices"] == 1 else "slices > 1"}
+    if p["n_stride"] % 32 != 0:
+        r.add("slice width % 32 != 0")
+    if p["N"] < 32:
+        r.add("N < 32")
+    if p["b_stream"]:
+        r.add("streamed weights")
+    else:
+        r.add("resident >= 6 stages" if p["stages"] >= 6 else "resident < 6 stages")
+    if p["taps"] == 3:
+        r.add("taps 3")
+    if p["rows_per_tile"] < kTileM:
+        r.add("rows_per_tile < 64")
+    for w0, w1 in p["wg_tiles"]:
+        if w0 and not w1:
+            r.add("warpgroup 1 idle")
+        if w0:
+            r.add("odd tiles per CTA" if (len(w0) + len(w1)) % 2 else "even tiles per CTA")
+    return r
+
+
+def regimes_tn(p):
+    """Every regime of TN_REGIMES a gemm_tn plan is in ("single k-range": the reduction has one 64-row chunk, so no launch
+    can split it, whatever the cluster occupancy)."""
+    r = {"cluster %dx%d" % p["cluster"], "NT %d" % p["NT"]}
+    if p["n_tiles"] == 2:
+        r.add("n_tiles 2")
+    if p["total_chunks"] == 1:
+        r.add("single k-range")
+    return r

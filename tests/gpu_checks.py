@@ -84,14 +84,14 @@ def _rand_bf16(shape, seed, scale=1.0):
 
 
 def check_linear(M=300, N=900, K=300, taps=1, seg=0, relu=0, out_bf16=1):
-    """nr_linear (wgmma gemm_nt + store epilogue) against an fp64 matmul of the same bf16 operands."""
+    """nr_linear (wgmma gemm_nt + store epilogue) against an fp64 matmul of the same bf16 operands: the norm-wise error and
+    the worst element against its bound (gemm_elem_ratio, <= 1)."""
     lib = load_library()
     lda, ldw = ru8(K + 1), ru8(K + 1)
     if taps == 1:
         A = _rand_bf16((M, K), 1)
         W = _rand_bf16((N, K), 2, 0.1)
         bias = O.det_uniform((N,), 3, -0.5, 0.5)
-        ref = A.double() @ W.double().t() + bias.double()
         Ad = torch.zeros(M, lda)
         Ad[:, :K] = A
         Wd = torch.zeros(N, ldw)
@@ -105,13 +105,6 @@ def check_linear(M=300, N=900, K=300, taps=1, seg=0, relu=0, out_bf16=1):
         bias = O.det_uniform((N,), 3, -0.5, 0.5)
         Xp = torch.zeros(n_seg, seg + 2, K)
         Xp[:, 1:seg + 1] = X
-        ref = torch.zeros(n_seg, seg + 2, N, dtype=torch.float64)
-        for s in range(taps):
-            sh = torch.zeros_like(Xp)
-            lo, hi = max(0, 1 - s), min(seg + 2, seg + 3 - s)
-            sh[:, lo:hi] = Xp[:, lo + s - 1:hi + s - 1]
-            ref += sh.double() @ W[:, s].double().t()
-        ref = (ref + bias.double()).view(Mrows, N)
         Ad = torch.zeros(Mrows, lda)
         Ad[:, :K] = Xp.view(Mrows, K)
         Wd = torch.zeros(taps * N, ldw)
@@ -119,34 +112,55 @@ def check_linear(M=300, N=900, K=300, taps=1, seg=0, relu=0, out_bf16=1):
             Wd[s * N:(s + 1) * N, :K] = W[:, s]
         M = Mrows
         rpt, w_tap_rows = (128 // (seg + 2)) * (seg + 2), N
-    if relu:
-        ref = ref.clamp(min=0)
     ld_out = ru8(N) if out_bf16 else (N + 3) // 4 * 4
     out = torch.full((M, ld_out), float("nan"), dtype=torch.bfloat16 if out_bf16 else torch.float32, device=DEV)
     Ad, Wd, bd = Ad.to(torch.bfloat16).to(DEV), Wd.to(torch.bfloat16).to(DEV), bias.to(DEV)
     check(lib.nr_linear(_p(Ad), M, lda, _p(Wd), N, ldw, K, taps, w_tap_rows, rpt, _p(bd), relu, _p(out), ld_out, out_bf16,
                         _stream()), "nr_linear")
     torch.cuda.synchronize()
-    got = out[:, :N].float().cpu()
+    pre, absum = linear_ref(Ad[:, :K].double(), Wd[:, :K].double(), bd.double(), N, taps, w_tap_rows)
+    got = out[:, :N]
+    ratio, zero_exact = gemm_elem_ratio(got, pre, absum, taps * -(-K // 16), out_bf16, relu)
+    ref = pre.clamp_min(0) if relu else pre
     if taps > 1:  # pad rows of the padded layout are not part of the result
-        keep = torch.ones(M, dtype=torch.bool).view(-1, seg + 2)
+        keep = torch.ones(M, dtype=torch.bool, device=DEV).view(-1, seg + 2)
         keep[:, 0] = keep[:, -1] = False
         keep = keep.view(-1)
         got, ref = got[keep], ref[keep]
-    return {"rel": relerr(got, ref), "maxabs": maxabs(got, ref), "nan": int(torch.isnan(got).sum())}
+    got = got.float()
+    return {"rel": relerr(got, ref), "maxabs": maxabs(got, ref), "nan": int(torch.isnan(got).sum()), "elem_ratio": ratio,
+            "relu_zero_exact": zero_exact}
+
+
+def linear_ref(A, W, bias, N, taps=1, w_tap_rows=0):
+    """fp64 pre-activation of nr_linear and the sum of |products| + |bias| per element: tap s reads A shifted by s - taps // 2
+    rows (zero outside A) against weight rows [s * w_tap_rows, + N).  A [M][K], W [rows][K], bias [N] or None (fp64 device)."""
+    M = A.shape[0]
+    pre = torch.zeros(M, N, dtype=torch.float64, device=A.device)
+    absum = torch.zeros_like(pre)
+    for s in range(taps):
+        d = s - taps // 2
+        As = torch.zeros_like(A)
+        lo, hi = max(0, -d), min(M, M - d)
+        if hi > lo:
+            As[lo:hi] = A[lo + d:hi + d]
+        Ws = W[s * w_tap_rows:s * w_tap_rows + N]
+        pre += As @ Ws.t()
+        absum += As.abs() @ Ws.abs().t()
+    if bias is not None:
+        pre += bias
+        absum += bias.abs()
+    return pre, absum
 
 
 def check_gemm_tn(Kr=1000, Ma=900, Nb=301, shift=0):
+    """nr_gemm_tn (+= onto ones) against an fp64 evaluation of the same bf16 operands: the norm-wise error and the worst element
+    against its bound (gemm_elem_ratio with n_acc = ceil(Kr/16) + the k-ranges' red.add, <= 1)."""
+    import gemm_plan_ref as P
     lib = load_library()
     lda, ldb = ru8(Ma), ru8(Nb)
     A = _rand_bf16((Kr, Ma), 11, 0.5)
     B = _rand_bf16((Kr, Nb), 12, 0.5)
-    Bs = torch.zeros_like(B)
-    if shift >= 0:
-        Bs[:Kr - shift] = B[shift:]
-    else:
-        Bs[-shift:] = B[:Kr + shift]
-    ref = A.double().t() @ Bs.double()
     Ad = torch.zeros(Kr, lda)
     Ad[:, :Ma] = A
     Bd = torch.zeros(Kr, ldb)
@@ -156,8 +170,21 @@ def check_gemm_tn(Kr=1000, Ma=900, Nb=301, shift=0):
     Ad, Bd = Ad.to(torch.bfloat16).to(DEV), Bd.to(torch.bfloat16).to(DEV)
     check(lib.nr_gemm_tn(_p(Ad), Kr, Ma, lda, _p(Bd), Kr, Nb, ldb, 0, Nb, shift, _p(D), ldd, _stream()), "nr_gemm_tn")
     torch.cuda.synchronize()
-    got = D[:, :Nb].cpu() - 1.0
-    return {"rel": relerr(got, ref), "maxabs": maxabs(got, ref), "nan": int(torch.isnan(got).sum())}
+    ref, absum = gemm_tn_ref(Ad[:, :Ma].double(), Bd[:, :Nb].double(), shift)
+    got = D[:, :Nb] - 1.0
+    n_acc = -(-Kr // 16) + P.plan_tn(Kr, Ma, Nb, sms=int(lib.nr_num_sms()))["k_slices_max"]
+    ratio, _ = gemm_elem_ratio(D[:, :Nb], ref + 1.0, absum + 1.0, n_acc, 0)
+    return {"rel": relerr(got, ref), "maxabs": maxabs(got, ref), "nan": int(torch.isnan(got).sum()), "elem_ratio": ratio}
+
+
+def gemm_tn_ref(A, B, shift):
+    """fp64 A^T . B[rows + shift] (rows of B outside [0, rows) are zero) and the sum of |products|; A [Kr][Ma], B [b_rows][Nb]."""
+    Kr, rows = A.shape[0], B.shape[0]
+    Bs = torch.zeros(Kr, B.shape[1], dtype=B.dtype, device=B.device)
+    lo, hi = max(0, -shift), min(Kr, rows - shift)
+    if hi > lo:
+        Bs[lo:hi] = B[lo + shift:hi + shift]
+    return A.t() @ Bs, A.abs().t() @ Bs.abs()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -414,7 +441,14 @@ def check_additive(N=37, S=20, D=300, q=200, precision="fast"):
                                     OperandCache(), "t", precision)
     out.backward(g.to(DEV))
     torch.cuda.synchronize()
-    return {"fwd_rel": relerr(out, ref), "dx_rel": relerr(xd.grad, x.grad),
+    # the forward element by element (additive_fwd_judge) from the operands it read: bf16(x) (and bf16(x - bf16(x)) in
+    # accurate mode), bf16(Wa), fp32 ba and qv
+    hi = bf16r(xf).to(DEV)
+    lo = bf16r(xf.to(DEV) - hi).double().reshape(N * S, D) if accurate else None
+    j = additive_fwd_judge(hi.double().reshape(N * S, D), bf16r(p["a.linear.weight"].detach()).double().to(DEV),
+                           p["a.linear.bias"].detach().double().to(DEV), p["a.attention_query_vector"].detach().double().to(DEV),
+                           S, out.detach(), X_lo=lo)
+    return {"fwd_rel": relerr(out, ref), "fwd_elem_ratio": j["out_ratio"], "dx_rel": relerr(xd.grad, x.grad),
             "dW_rel": relerr(pd["a.linear.weight"].grad, p["a.linear.weight"].grad),
             "db_rel": relerr(pd["a.linear.bias"].grad, p["a.linear.bias"].grad),
             "dq_rel": relerr(pd["a.attention_query_vector"].grad, p["a.attention_query_vector"].grad)}
@@ -1345,6 +1379,71 @@ def check_cnn_encoder(n_seq=37, T=20, d=300, F=400, q=200, V=500, p_drop=0.2, ac
 def _abs_allow_rows(got, ref, absref):
     """max over rows of |got - ref| / |absref| (row norms): fp32 accumulation error against the sum of |products|."""
     return _worst(_safe_div((got - ref).norm(dim=1), absref.norm(dim=1)))
+
+
+# ------------------------------------------------------------------------------------------------
+# Element bounds of the wgmma GEMMs and of the additive-attention forward (tests/test_gpu_gemm_elements.py,
+# tests/test_gpu_additive_fwd.py): each output element against an fp64 evaluation of the operands the kernel read.
+# ------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24  # unit roundoff of fp32
+TANH_ERR = 2e-7   # absolute error of fast_tanh (nr_common.cuh): ex2.approx, one division, one subtraction
+
+
+def gemm_elem_ratio(got, pre, absum, n_acc, out_bf16, relu=False):
+    """The GEMM element judge.  An element may miss its fp64 value ref (pre, after the ReLU) by e = 4u (n_acc + 2) S, with
+    S = sum of |products| + |bias| (+ |pre-fill| for a "+=" output) and n_acc the fp32 accumulations it went through (a
+    worst-case gamma_n, doubled because the tensor core's internal rounding is not documented); a bf16 output by e + half a
+    bf16 ulp of |ref| + e.  Returns the worst (|got - ref| - rounding allowance) / e, clamped at 0 -- the share of the
+    accumulation allowance used, <= 1 exactly when every element is inside its bound (+inf for a NaN) -- and whether every
+    element whose pre-activation lies below -e came out exactly 0 under a ReLU (True without one)."""
+    ref = pre.clamp_min(0) if relu else pre
+    e = 4 * U32 * (n_acc + 2) * absum
+    err = (got.double() - ref).abs()
+    if out_bf16:
+        err = (err - 0.5 * _bf16_ulp(ref.abs() + e)).clamp_min(0)
+    ratio = _worst(_safe_div(err, e))
+    zero_exact = bool((got[pre + e < 0] == 0).all()) if relu else True
+    return ratio, zero_exact
+
+
+def additive_fwd_judge(X, Wa, ba, qv, seg, out, w=None, X_lo=None):
+    """The pooling forward out_s = sum_r w_r X_r, w = softmax over the segment of score_r = sum_c qv_c tanh(X_r . Wa_c + ba_c),
+    judged element by element.  X [rows][D] (the plane the scores read), X_lo (or None) the low plane, Wa [q][D], ba and qv [q]:
+    the kernel's own operands as fp64 device tensors; out [n_seg][D] and w [rows] (or None) are the kernel's results.
+    The bound is carried stage by stage:
+      pre   e_rc = the GEMM bound (fp32 accumulation of ceil(D/16) k-steps, then the bias)
+      tanh  e_rc + TANH_ERR
+      score ds_r = sum_c |qv_c| (e_rc + TANH_ERR) + q u sum_c |qv_c t_rc|
+      w     |dw_r| <= w_r (2 max_seg ds + x_r + sum_t w_t x_t + (seg + 2) u) + 2^-126, with x_r = (2 |s_r - max| + 4) u the
+            error of __expf on the shifted score (the subtraction, the scaling by log2(e), ex2.approx), seg u the fp32 sum
+            and 2u the division; ex2.approx flushes results below 2^-126 to zero
+      out   |dout_d| <= sum_r |dw_r| |X_rd| + (n + 1) u sum_r w_r |X_rd|, n = seg fma steps (2 seg with the low plane, whose
+            rows enter |X| too)
+    Returns {"out_ratio", "w_ratio"}: the worst |kernel - ref| / bound of out, and of w the worst (|kernel - ref| - 2^-126) /
+    (the relative part of its bound), clamped at 0 -- both <= 1 exactly when every element is inside its bound (+inf for a
+    NaN); a weight that underflows to 0 in the kernel uses the flush allowance, not the relative one."""
+    rows, D = X.shape
+    q, n_seg = Wa.shape[0], rows // seg
+    pre = X @ Wa.t() + ba
+    e = 4 * U32 * (-(-D // 16) + 2) * (X.abs() @ Wa.abs().t() + ba.abs())
+    t = torch.tanh(pre)
+    s = (t @ qv).view(n_seg, seg)
+    ds = ((e + TANH_ERR) @ qv.abs() + q * U32 * (t.abs() @ qv.abs())).view(n_seg, seg)
+    wr = torch.softmax(s, dim=1)
+    xe = (2 * (s - s.max(dim=1, keepdim=True).values).abs() + 4) * U32
+    dw_rel = wr * (2 * ds.max(dim=1, keepdim=True).values + xe + (wr * xe).sum(dim=1, keepdim=True) + (seg + 2) * U32)
+    dw = dw_rel + 2.0 ** -126
+    Xs, Xa = X, X.abs()
+    if X_lo is not None:
+        Xs, Xa = X + X_lo, Xa + X_lo.abs()
+    n = 2 * seg if X_lo is not None else seg
+    ref = torch.einsum("ns,nsd->nd", wr, Xs.view(n_seg, seg, D))
+    bound = torch.einsum("ns,nsd->nd", dw, Xa.view(n_seg, seg, D)) + (n + 1) * U32 * torch.einsum("ns,nsd->nd", wr, Xa.view(n_seg, seg, D))
+    res = {"out_ratio": _worst(_safe_div((out.double() - ref).abs(), bound))}
+    if w is not None:
+        # like the bf16 rounding of the GEMM judge: the share of the relative allowance used beyond the flush to zero
+        res["w_ratio"] = _worst(_safe_div(((w.double().view(n_seg, seg) - wr).abs() - 2.0 ** -126).clamp_min(0), dw_rel))
+    return res
 
 
 def check_element_encoder(n=512 * 55, E=100, F=400, V=300, seed=3):
