@@ -247,17 +247,18 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream);
  *   NAML  TextEncoder      src/model/NAML/news_encoder.py:21-37
  *   LSTUR title branch     src/model/LSTUR/news_encoder.py:56-72
  *   TANR  NewsEncoder      src/model/TANR/news_encoder.py:40-52
- * embedding -> dropout -> Conv2d(1, F, (3, d), padding (1, 0)) -> ReLU -> dropout -> additive pooling.
- * The conv is three row-shifted wgmma GEMM taps over a zero-padded layout (T+2 rows per segment).
- * Shapes: 1 <= T <= 64 (the pooling tile holds whole segments), d and F multiples of 4, d, F >= 8, 1 <= q <= 256;
- * both entry points reject any other shape with -1 before the first launch. */
+ * embedding -> dropout -> Conv2d(1, F, (w, d), padding ((w-1)/2, 0)) -> ReLU -> dropout -> additive pooling, window w = 1 .. 4.
+ * With p = (w-1)/2 a segment has L = T + 2p - w + 1 output positions (T at odd w, T-1 at even w).  The conv is w row-shifted
+ * wgmma GEMM taps over a zero-padded layout (T+2 rows per segment, token t at row t+1), output j reading rows j+1-p+s, s < w.
+ * Shapes: 1 <= T <= 64 (the pooling tile holds whole segments), T >= w - 2p (T >= 2 at an even window), d and F multiples of
+ * 4, d, F >= 8, 1 <= q <= 256; both entry points reject any other shape or window with -1 before the first launch. */
 typedef struct {
     long long n_seq;
     int T, d, F, q, ldx, ldf;       /* ldx = round_up(d+1, 8), ldf = round_up(F+1, 8)                       */
     const long long* ids;           /* [n_seq*T]                                                          */
     const void* table_bf16;         /* [V][ldx]                                                           */
     int V;
-    const void* wconv_bf16;         /* [3*F][ldx]; rows s*F..(s+1)*F hold tap s = weight[:, 0, s, :]        */
+    const void* wconv_bf16;         /* [w*F][ldx]; rows s*F..(s+1)*F hold tap s = weight[:, 0, s, :]        */
     const float* bconv;             /* [F]                                                                */
     const void* wa_bf16;            /* [q][ldf]                                                           */
     const float* ba;
@@ -265,11 +266,12 @@ typedef struct {
     float p_drop;
     unsigned long long seed;
     void* Xp_bf16;                  /* [n_seq*(T+2)][ldx]  gathered rows, zero-padded layout (saved)        */
-    void* Y_bf16;                   /* [n_seq*T][ldf]      relu(conv) rows (saved)                          */
-    float* w;                       /* [n_seq*T]                                                          */
+    void* Y_bf16;                   /* [n_seq*L][ldf]      relu(conv) rows (saved)                          */
+    float* w;                       /* [n_seq*L]                                                          */
     float* out;                     /* [n_seq][F]                                                         */
     int* bad_id_flag;
-    void* Y_lo_bf16;          /* optional [n_seq*T][ldf]: low plane of the conv output (accurate mode: the pooled sum reads Y + Y_lo) */
+    void* Y_lo_bf16;          /* optional [n_seq*L][ldf]: low plane of the conv output (accurate mode: the pooled sum reads Y + Y_lo) */
+    int window;                     /* conv window w, 1 .. 4; 0 means 3 (the reference default)            */
 } nr_cnn_encoder_fwd_args;
 int nr_cnn_encoder_fwd(const nr_cnn_encoder_fwd_args* a, void* stream);
 
@@ -278,7 +280,7 @@ typedef struct {
     int T, d, F, q, ldx, ldf, ldq;
     const long long* ids;
     int V;
-    const void* wconvT_bf16;        /* [3*d][ldf]; rows s*d..(s+1)*d hold (weight[:, 0, 2-s, :])^T          */
+    const void* wconvT_bf16;        /* [w*d][ldf]; rows s*d..(s+1)*d hold (weight[:, 0, w-1-s, :])^T        */
     const void* wa_bf16;            /* [q][ldf]                                                           */
     const void* waT_bf16;           /* [F][ldq]                                                           */
     const float* ba;
@@ -289,12 +291,13 @@ typedef struct {
     const void* Y_bf16;
     const float* w;
     const float* dout;              /* [n_seq][F]                                                         */
-    float* dWconv_ext;              /* [3][F][ldx] (+=); column d of tap 1 is d(bias)                       */
+    float* dWconv_ext;              /* [w][F][ldx] (+=); column d of tap p = (w-1)/2 is d(bias)             */
     float* dWa_ext;                 /* [q][ldf] (+=); column F is d(bias)                                   */
     float* dqv;                     /* [q] (+=)                                                           */
     float* demb;                    /* [V][d] (+=)                                                        */
     void* workspace;
     long long workspace_bytes;
+    int window;                     /* as in the forward: 1 .. 4, 0 means 3                               */
 } nr_cnn_encoder_bwd_args;
 long long nr_cnn_encoder_bwd_workspace(long long n_seq, int T, int F, int q);
 int nr_cnn_encoder_bwd(const nr_cnn_encoder_bwd_args* a, void* stream);

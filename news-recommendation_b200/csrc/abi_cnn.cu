@@ -10,43 +10,57 @@
 using namespace nr;
 
 // Every shape limit of the kernels the encoder chains is checked here, before the first launch: T <= kGemmTileRows because
-// a pooling tile holds whole segments (gemm_additive_pool), F % 4 == 0 for the float4 dOut rows of pool_dscore.
-static int check_cnn_shape(long long n_seq, int T, int d, int F, int q, int ldx, int ldf) {
+// a pooling tile holds whole segments (gemm_additive_pool), F % 4 == 0 for the float4 dOut rows of pool_dscore, a window
+// of 1 to 4 taps (the conv GEMMs' limit; one zero pad row on each side of a segment covers all four) and at least one
+// output position per segment.
+static int check_cnn_shape(long long n_seq, int T, int d, int F, int q, int ldx, int ldf, int window) {
+    NR_REQUIRE(window >= 1 && window <= 4, "cnn encoder: window=%d (1 .. 4)", window);
     NR_REQUIRE(n_seq >= 0 && T >= 1 && T <= kGemmTileRows && d >= 8 && F >= 8 && q >= 1 && q <= 256,
                "cnn encoder: bad shape n_seq=%lld T=%d (at most %d) d=%d F=%d q=%d", n_seq, T, kGemmTileRows, d, F, q);
+    NR_REQUIRE(T >= window - 2 * ((window - 1) / 2), "cnn encoder: T=%d leaves no output position at window=%d", T, window);
     NR_REQUIRE(ldx == round_up(d + 1, 8) && ldf == round_up(F + 1, 8), "cnn encoder: pitches must be round_up(width+1, 8) (ldx=%d ldf=%d)", ldx, ldf);
     NR_REQUIRE(d % 4 == 0 && F % 4 == 0, "cnn encoder: d and F must be multiples of 4 (d=%d F=%d)", d, F);
     NR_REQUIRE(n_seq * (T + 2) < (1ll << 31), "cnn encoder: too many rows");
     return 0;
 }
 
+// The reference's Conv2d(1, F, (w, d), padding ((w - 1) / 2, 0)) over T tokens: pad rows p = (w - 1) / 2 on each side,
+// L = T + 2p - w + 1 output positions (T at odd w, T - 1 at even w).  In the padded layout (token t at row t + 1 of a
+// segment's T + 2 rows) output j reads rows j + 1 - p + s, s < w: the conv GEMM's taps with tap origin p.
+struct CnnWindow {
+    int w, p, L;
+    CnnWindow(int window, int T) : w(window == 0 ? 3 : window), p((w - 1) / 2), L(T + 2 * p - w + 1) {}
+};
+
 extern "C" {
 
 // ---- reference: TextEncoder / title_CNN + title_attention -------------------------------------------
 //   NAML  src/model/NAML/news_encoder.py:21-37 ; LSTUR src/model/LSTUR/news_encoder.py:56-72 ;
-//   TANR  src/model/TANR/news_encoder.py:40-52 :  embedding -> dropout -> Conv2d(1,F,(3,d),pad (1,0)) -> ReLU
+//   TANR  src/model/TANR/news_encoder.py:40-52 :  embedding -> dropout -> Conv2d(1,F,(w,d),pad ((w-1)/2,0)) -> ReLU
 //   -> dropout -> additive pooling
 int nr_cnn_encoder_fwd(const nr_cnn_encoder_fwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_cnn_encoder_fwd: null args");
-    NR_PROPAGATE(check_cnn_shape(a->n_seq, a->T, a->d, a->F, a->q, a->ldx, a->ldf));
+    const CnnWindow win(a->window, a->T);
+    NR_PROPAGATE(check_cnn_shape(a->n_seq, a->T, a->d, a->F, a->q, a->ldx, a->ldf, win.w));
     NR_REQUIRE(a->ids && a->table_bf16 && a->wconv_bf16 && a->bconv && a->wa_bf16 && a->ba && a->qv && a->Xp_bf16 && a->Y_bf16 &&
                    a->w && a->out && a->bad_id_flag, "nr_cnn_encoder_fwd: null operand");
     NR_REQUIRE(a->p_drop >= 0.f && a->p_drop < 1.f, "nr_cnn_encoder_fwd: dropout p=%f", a->p_drop);
     if (a->n_seq == 0) return 0;
     const cudaStream_t st = as_stream(stream);
-    const int T = a->T, Tp = T + 2;
+    const int T = a->T, Tp = T + 2, L = win.L;
     const long long n_tok = a->n_seq * T;
     const int Mp = static_cast<int>(a->n_seq * Tp);
     prof_context("cnn.fwd");
     NR_PROPAGATE(gather_rows(a->ids, n_tok, T, a->table_bf16, a->V, a->d, a->ldx, a->Xp_bf16, a->ldx, 1,
                              DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
-    const RowMapCfg to_compact = {Tp, 1, T, T, 0};
-    NR_PROPAGATE(gemm_store({.A = a->Xp_bf16, .M = Mp, .lda = a->ldx, .W = a->wconv_bf16, .N = a->F, .ldw = a->ldx, .K = a->d, .taps = 3,
-                             .w_tap_rows = a->F},
+    // padded row r of a segment is output j = r - 1 when j < L: the rows that read past the output positions are dropped
+    const RowMapCfg to_compact = {Tp, 1, L, L, 0};
+    NR_PROPAGATE(gemm_store({.A = a->Xp_bf16, .M = Mp, .lda = a->ldx, .W = a->wconv_bf16, .N = a->F, .ldw = a->ldx, .K = a->d, .taps = win.w,
+                             .w_tap_rows = a->F, .tap_origin = win.p},
                             {.out = a->Y_bf16, .ld_out = a->ldf, .out_bf16 = 1, .relu = 1, .bias = a->bconv, .rm = to_compact,
                              .drop = context_dropout(a->p_drop, a->seed), .ones_col = a->F, .ones_zero_upto = a->ldf, .lo_out = a->Y_lo_bf16,
                              .ld_lo = a->ldf}, st));
-    NR_PROPAGATE(gemm_additive_pool(a->Y_bf16, static_cast<int>(n_tok), a->ldf, a->F, a->wa_bf16, a->q, a->ldf, a->ba, a->qv, T,
+    NR_PROPAGATE(gemm_additive_pool(a->Y_bf16, static_cast<int>(a->n_seq * L), a->ldf, a->F, a->wa_bf16, a->q, a->ldf, a->ba, a->qv, L,
                                     a->out, a->F, a->w, st, a->Y_lo_bf16));
     return 0;
 }
@@ -62,34 +76,41 @@ long long nr_cnn_encoder_bwd_workspace(long long n_seq, int T, int F, int q) { r
 
 int nr_cnn_encoder_bwd(const nr_cnn_encoder_bwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_cnn_encoder_bwd: null args");
-    NR_PROPAGATE(check_cnn_shape(a->n_seq, a->T, a->d, a->F, a->q, a->ldx, a->ldf));
+    const CnnWindow win(a->window, a->T);
+    NR_PROPAGATE(check_cnn_shape(a->n_seq, a->T, a->d, a->F, a->q, a->ldx, a->ldf, win.w));
     NR_REQUIRE(a->ldq == round_up(a->q, 16), "nr_cnn_encoder_bwd: ldq=%d (must be round_up(q, 16))", a->ldq);
     NR_REQUIRE(a->ids && a->wconvT_bf16 && a->wa_bf16 && a->waT_bf16 && a->ba && a->qv && a->Xp_bf16 && a->Y_bf16 && a->w &&
                    a->dout && a->dWconv_ext && a->dWa_ext && a->dqv && a->demb && a->workspace, "nr_cnn_encoder_bwd: null operand");
-    const CnnBwdWorkspace ws(a->workspace, a->n_seq, a->T, a->F, a->q);
+    const CnnBwdWorkspace ws(a->workspace, a->n_seq, a->T, a->F, a->q);  // L <= T: sized for every window
     NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_cnn_encoder_bwd: workspace too small");
     if (a->n_seq == 0) return 0;
     const cudaStream_t st = as_stream(stream);
-    const int T = a->T, Tp = T + 2;
-    const int M = static_cast<int>(a->n_seq * T), Mp = static_cast<int>(a->n_seq * Tp);
-    const RowMapCfg to_padded = {T, 0, T, Tp, 1}, to_compact = {Tp, 1, T, T, 0};
+    const int T = a->T, Tp = T + 2, L = win.L;
+    const int M = static_cast<int>(a->n_seq * L), Mp = static_cast<int>(a->n_seq * Tp);
+    const RowMapCfg to_padded = {L, 0, L, Tp, 1}, to_compact = {Tp, 1, T, T, 0};
     prof_context("cnn.bwd");
     // additive pooling backward; the ReLU / dropout of the conv output are folded into the dY epilogue, which
     // also re-maps the rows into the zero-padded layout the shifted (tap) loads below need
-    NR_PROPAGATE(pool_dscore(a->Y_bf16, a->ldf, a->F, a->n_seq, T, a->w, a->dout, a->F, ws.dscore, st));
+    NR_PROPAGATE(pool_dscore(a->Y_bf16, a->ldf, a->F, a->n_seq, L, a->w, a->dout, a->F, ws.dscore, st));
     NR_PROPAGATE(gemm_additive_dpre(a->Y_bf16, M, a->ldf, a->F, a->wa_bf16, a->q, a->ldf, a->ba, a->qv, ws.dscore, ws.dpre, a->ldq,
                                     a->dqv, st));
+    // dY sits at rows 1 .. L of a segment; the epilogue zeroes rows 0 and L + 1.  At an even window L = T - 1, and row T + 1
+    // is zeroed here: every weight-gradient tap sums over all rows, and the transposed conv of w = 4 reads it
+    if (L < T)
+        NR_CHECK_CUDA(cudaMemset2DAsync(ws.dYp + static_cast<size_t>(T + 1) * a->ldf, sizeof(__nv_bfloat16) * Tp * a->ldf, 0,
+                                        sizeof(__nv_bfloat16) * a->ldf, a->n_seq, st));
     NR_PROPAGATE(gemm_pool_dinput({.A = ws.dpre, .M = M, .lda = a->ldq, .W = a->waT_bf16, .N = a->F, .ldw = a->ldq, .K = a->q},
-                                  {.w = a->w, .dout = a->dout, .ldo = a->F, .seg_len = T, .dx = ws.dYp, .ld_dx = a->ldf, .rm = to_padded,
+                                  {.w = a->w, .dout = a->dout, .ldo = a->F, .seg_len = L, .dx = ws.dYp, .ld_dx = a->ldf, .rm = to_padded,
                                    .zero_pad_rows = 1, .drop = context_dropout(a->p_drop, a->seed), .relu_src = a->Y_bf16, .relu_ld = a->ldf}, st));
     NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, a->q, a->ldq, a->Y_bf16, a->F, a->ldf, a->dWa_ext, st));
-    // conv weight gradient, one tap at a time: dW_s = dY^T . X[rows + (s-1)]; the ones column of X makes column d
-    // of the centre tap the bias gradient
-    for (int s = 0; s < 3; ++s)
+    // conv weight gradient, one tap at a time: dW_s = dY^T . X[rows + s - p]; the ones column of X makes column d
+    // of tap p (shift 0) the bias gradient
+    for (int s = 0; s < win.w; ++s)
         NR_PROPAGATE(gemm_weight_grad(ws.dYp, Mp, a->F, a->ldf, a->Xp_bf16, a->d, a->ldx,
-                                      a->dWconv_ext + static_cast<size_t>(s) * a->F * a->ldx, st, s - 1));
-    // embedding gradient: dX[r] = sum_s' W_(2-s')^T dY[r + s' - 1], scattered to the token ids
-    NR_PROPAGATE(gemm_scatter_emb({.A = ws.dYp, .M = Mp, .lda = a->ldf, .W = a->wconvT_bf16, .N = a->d, .ldw = a->ldf, .K = a->F, .taps = 3,
+                                      a->dWconv_ext + static_cast<size_t>(s) * a->F * a->ldx, st, s - win.p));
+    // embedding gradient, the transposed conv: dX[r] = sum_s' W_(w-1-s')^T dY[r + s' - (w - 1 - p)], w - 1 - p = w / 2 being the
+    // GEMM's centred tap origin; scattered to the token ids
+    NR_PROPAGATE(gemm_scatter_emb({.A = ws.dYp, .M = Mp, .lda = a->ldf, .W = a->wconvT_bf16, .N = a->d, .ldw = a->ldf, .K = a->F, .taps = win.w,
                                    .w_tap_rows = a->d},
                                   {.ids = a->ids, .demb = a->demb, .V = a->V, .rm = to_compact, .drop = {a->p_drop, a->seed}, .drop_ld = a->ldx},
                                   st));

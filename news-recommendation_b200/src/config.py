@@ -29,6 +29,8 @@ _COMMON = {
 }
 BaseConfig = type("BaseConfig", (), dict(_COMMON, __doc__="General configuration shared by all models"))
 
+# window_size: 1 to 4 (the conv GEMMs take at most 4 taps); building a CNN model with any other window raises NewsrecError.
+# The reference asserts an odd window in LSTUR, TANR and Hi-Fi Ark; this build runs 2 and 4 there as NAML's conv does
 _CNN = {"num_filters": 300, "window_size": 3}
 _PER_MODEL = {
     # precision is an extension knob of this build (not in the reference; DESIGN.md section 4):

@@ -16,7 +16,6 @@ class NewsEncoder(nn.Module):
             self.word_embedding = nn.Embedding(config.num_words, config.word_embedding_dim, padding_idx=0)
         else:
             self.word_embedding = nn.Embedding.from_pretrained(pretrained_word_embedding, freeze=False, padding_idx=0)
-        assert config.window_size >= 1 and config.window_size % 2 == 1
         self.title_CNN = make_title_cnn(config.num_filters, config.window_size, config.word_embedding_dim)
         self.abstract_CNN = make_title_cnn(config.num_filters, config.window_size, config.word_embedding_dim)
         self.title_attention = AdditiveAttention(config.query_vector_dim, config.num_filters)

@@ -19,7 +19,6 @@ class NewsEncoder(nn.Module):
         else:
             self.word_embedding = nn.Embedding.from_pretrained(pretrained_word_embedding, freeze=False, padding_idx=0)
         self.category_embedding = nn.Embedding(config.num_categories, config.num_filters, padding_idx=0)
-        assert config.window_size >= 1 and config.window_size % 2 == 1
         self.title_CNN = make_title_cnn(config.num_filters, config.window_size, config.word_embedding_dim)
         self.title_attention = AdditiveAttention(config.query_vector_dim, config.num_filters)
         self._cache, self._flag, self._cat_flag = OperandCache(), BadIdFlag(), BadIdFlag()

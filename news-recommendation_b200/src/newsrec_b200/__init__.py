@@ -54,7 +54,7 @@ class CnnEncoderFwdArgs(C.Structure):
         ("wconv_bf16", _vp), ("bconv", _vp), ("wa_bf16", _vp), ("ba", _vp), ("qv", _vp),
         ("p_drop", _f), ("seed", _ull),
         ("Xp_bf16", _vp), ("Y_bf16", _vp), ("w", _vp), ("out", _vp), ("bad_id_flag", _vp),
-        ("Y_lo_bf16", _vp),
+        ("Y_lo_bf16", _vp), ("window", _i),
     ]
 
 
@@ -67,7 +67,7 @@ class CnnEncoderBwdArgs(C.Structure):
         ("p_drop", _f), ("seed", _ull),
         ("Xp_bf16", _vp), ("Y_bf16", _vp), ("w", _vp), ("dout", _vp),
         ("dWconv_ext", _vp), ("dWa_ext", _vp), ("dqv", _vp), ("demb", _vp),
-        ("workspace", _vp), ("workspace_bytes", _ll),
+        ("workspace", _vp), ("workspace_bytes", _ll), ("window", _i),
     ]
 
 

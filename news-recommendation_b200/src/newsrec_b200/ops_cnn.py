@@ -7,30 +7,30 @@ import ctypes as C
 
 import torch
 
-from . import CnnEncoderBwdArgs, CnnEncoderFwdArgs, NewsrecError, check, load_library, require_cuda
+from . import CnnEncoderBwdArgs, CnnEncoderFwdArgs, check, load_library, require_cuda
 from .ops import _p, _stream, cast_pad, next_seed, ru8, ru16, table_operand
 
 
 class CnnPoolEncoderFn(torch.autograd.Function):
-    """ids (n_seq, T) int64 -> (n_seq, F):  embedding -> dropout -> Conv2d(1,F,(3,d)) -> ReLU -> dropout -> additive pool.
+    """ids (n_seq, T) int64 -> (n_seq, F):  embedding -> dropout -> Conv2d(1,F,(w,d), padding ((w-1)/2, 0)) -> ReLU -> dropout
+    -> additive pool, w = 1 .. 4 from the weight's shape; the pool runs over the L = T + 2 ((w-1)/2) - w + 1 conv outputs.
     reference: NAML/news_encoder.py:21-37, LSTUR/news_encoder.py:56-72, TANR/news_encoder.py:40-52."""
 
     @staticmethod
     def forward(ctx, ids, emb_w, Wc, bc, Wa, ba, qv, p_drop, cache, prefix, bad_flag, accurate=False):
         lib = load_library()
         dev = require_cuda()
-        Fn, _, win, d = Wc.shape
-        if win != 3:
-            raise NewsrecError(f"window_size={win}: the wgmma conv path implements the reference default window_size=3")
+        Fn, _, win, d = Wc.shape  # the C ABI refuses a window outside 1 .. 4 (make_title_cnn already has)
         q = Wa.shape[0]
         ldx, ldf, ldq = ru8(d + 1), ru8(Fn + 1), ru16(q)
         n_seq, T = ids.shape
+        L = T + 2 * ((win - 1) // 2) - win + 1
         ids = ids.contiguous()
 
         def build(Wc, bc, Wa, ba, qv):
-            taps = Wc[:, 0]                                                   # (F, 3, d)
-            wconv = taps.permute(1, 0, 2).reshape(3 * Fn, d)                  # tap-major rows
-            wconvT = torch.cat([taps[:, 2 - s, :].t() for s in range(3)], 0)  # (3d, F): tap s' = W_(2-s')^T
+            taps = Wc[:, 0]                                                           # (F, w, d)
+            wconv = taps.permute(1, 0, 2).reshape(win * Fn, d)                        # tap-major rows
+            wconvT = torch.cat([taps[:, win - 1 - s, :].t() for s in range(win)], 0)  # (w d, F): tap s' = W_(w-1-s')^T
             return dict(wconv=cast_pad(wconv, ldx), wconvT=cast_pad(wconvT, ldf), bconv=bc.float().contiguous(),
                         wa=cast_pad(Wa, ldf), waT=cast_pad(Wa, ldq, transpose=True), ba=ba.float().contiguous(),
                         qv=qv.float().contiguous())
@@ -38,23 +38,23 @@ class CnnPoolEncoderFn(torch.autograd.Function):
         ops = cache.get(prefix, (Wc, bc, Wa, ba, qv), build)
         table = table_operand(cache, prefix + ".table", emb_w)
         Xp = torch.empty((n_seq * (T + 2), ldx), dtype=torch.bfloat16, device=dev)
-        Y = torch.empty((n_seq * T, ldf), dtype=torch.bfloat16, device=dev)
-        w = torch.empty((n_seq * T,), dtype=torch.float32, device=dev)
+        Y = torch.empty((n_seq * L, ldf), dtype=torch.bfloat16, device=dev)
+        w = torch.empty((n_seq * L,), dtype=torch.float32, device=dev)
         out = torch.empty((n_seq, Fn), dtype=torch.float32, device=dev)
         seed = next_seed() if p_drop > 0 else 0
         a = CnnEncoderFwdArgs()
-        a.n_seq, a.T, a.d, a.F, a.q, a.ldx, a.ldf = n_seq, T, d, Fn, q, ldx, ldf
+        a.n_seq, a.T, a.d, a.F, a.q, a.ldx, a.ldf, a.window = n_seq, T, d, Fn, q, ldx, ldf, win
         a.ids, a.table_bf16, a.V = _p(ids), _p(table), emb_w.shape[0]
         a.wconv_bf16, a.bconv, a.wa_bf16, a.ba, a.qv = _p(ops["wconv"]), _p(ops["bconv"]), _p(ops["wa"]), _p(ops["ba"]), _p(ops["qv"])
         a.p_drop, a.seed = float(p_drop), seed
         a.Xp_bf16, a.Y_bf16, a.w, a.out, a.bad_id_flag = _p(Xp), _p(Y), _p(w), _p(out), _p(bad_flag)
         Y_lo = None
         if accurate:  # the conv output as a hi/lo bf16 pair: the pooled sum reads both planes (DESIGN.md section 4)
-            Y_lo = torch.empty((n_seq * T, ldf), dtype=torch.bfloat16, device=dev)
+            Y_lo = torch.empty((n_seq * L, ldf), dtype=torch.bfloat16, device=dev)
             a.Y_lo_bf16 = _p(Y_lo)
         check(lib.nr_cnn_encoder_fwd(C.byref(a), _stream()), "nr_cnn_encoder_fwd")
         ctx.save_for_backward(Xp, Y, w, ids)
-        ctx.meta = dict(n_seq=n_seq, T=T, d=d, F=Fn, q=q, p_drop=float(p_drop), seed=seed, ops=ops, V=emb_w.shape[0])
+        ctx.meta = dict(n_seq=n_seq, T=T, d=d, F=Fn, q=q, win=win, p_drop=float(p_drop), seed=seed, ops=ops, V=emb_w.shape[0])
         return out
 
     @staticmethod
@@ -63,17 +63,17 @@ class CnnPoolEncoderFn(torch.autograd.Function):
         Xp, Y, w, ids = ctx.saved_tensors
         m = ctx.meta
         dev = Xp.device
-        n_seq, T, d, Fn, q, ops = m["n_seq"], m["T"], m["d"], m["F"], m["q"], m["ops"]
+        n_seq, T, d, Fn, q, win, ops = m["n_seq"], m["T"], m["d"], m["F"], m["q"], m["win"], m["ops"]
         ldx, ldf, ldq = ru8(d + 1), ru8(Fn + 1), ru16(q)
         dout = dout.contiguous().float()
-        dWc = torch.zeros((3, Fn, ldx), dtype=torch.float32, device=dev)
+        dWc = torch.zeros((win, Fn, ldx), dtype=torch.float32, device=dev)
         dWa = torch.zeros((q, ldf), dtype=torch.float32, device=dev)
         dqv = torch.zeros((q,), dtype=torch.float32, device=dev)
         demb = torch.zeros((m["V"], d), dtype=torch.float32, device=dev)
         ws_bytes = int(lib.nr_cnn_encoder_bwd_workspace(n_seq, T, Fn, q))
         ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
         a = CnnEncoderBwdArgs()
-        a.n_seq, a.T, a.d, a.F, a.q, a.ldx, a.ldf, a.ldq = n_seq, T, d, Fn, q, ldx, ldf, ldq
+        a.n_seq, a.T, a.d, a.F, a.q, a.ldx, a.ldf, a.ldq, a.window = n_seq, T, d, Fn, q, ldx, ldf, ldq, win
         a.ids, a.V = _p(ids), m["V"]
         a.wconvT_bf16, a.wa_bf16, a.waT_bf16, a.ba, a.qv = _p(ops["wconvT"]), _p(ops["wa"]), _p(ops["waT"]), _p(ops["ba"]), _p(ops["qv"])
         a.p_drop, a.seed = m["p_drop"], m["seed"]
@@ -81,8 +81,8 @@ class CnnPoolEncoderFn(torch.autograd.Function):
         a.dWconv_ext, a.dWa_ext, a.dqv, a.demb = _p(dWc), _p(dWa), _p(dqv), _p(demb)
         a.workspace, a.workspace_bytes = _p(ws), ws_bytes
         check(lib.nr_cnn_encoder_bwd(C.byref(a), _stream()), "nr_cnn_encoder_bwd")
-        gWc = dWc[:, :, :d].permute(1, 0, 2).unsqueeze(1).contiguous()   # (F, 1, 3, d)
-        gbc = dWc[1, :, d].contiguous()
+        gWc = dWc[:, :, :d].permute(1, 0, 2).unsqueeze(1).contiguous()   # (F, 1, w, d)
+        gbc = dWc[(win - 1) // 2, :, d].contiguous()                      # the tap of shift 0 reads the ones column
         return (None, demb, gWc, gbc, dWa[:, :Fn].contiguous(), dWa[:, Fn].contiguous(), dqv, None, None, None, None, None)
 
 
