@@ -105,8 +105,16 @@ int nr_additive_attention_fwd(const void* X_bf16, long long n_seg, int seg_len, 
 int nr_additive_attention_fwd_hilo(const void* X_bf16, const void* X_lo_bf16, long long n_seg, int seg_len, int D, int ldx,
                                    const void* Wa_bf16, int q, int ldw, const float* ba, const float* qv, float* out, int ldo,
                                    float* w_out, void* stream);
-/* backward.  dX bf16 [rows][ld_dx] (=), dWa_ext fp32 [q][ldx] (+=, column D is d(bias)), dqv [q] (+=).
- * workspace: nr_additive_attention_bwd_workspace(...) bytes. */
+/* backward.  dX bf16 [rows][ld_dx] (=, columns [D, ld_dx) not written), dWa_ext fp32 [q][ldx] (+=, columns [0, D] only: column D
+ * is d(bias)), dqv [q] (+=).  w [rows] is the forward's saved softmax weights, dout fp32 [n_seg][ldo], WaT bf16 [D][ldwT] = Wa^T.
+ * Accepted shapes: n_seg >= 0 (0 launches nothing), 1 <= seg_len <= 64 (the forward's limit), 1 <= q <= 256, D >= 4 with
+ * D % 4 == 0, and q x D fitting one weight slice of the dPre GEMM (as in the forward); pitches ldx >= D + 1 (the ones column at
+ * D, 1.0), ldw >= D, ldwT >= q, ld_dx >= D, each a multiple of 8, and ldo >= D a multiple of 4; bf16 operands, dout and the
+ * workspace 16-byte aligned.  Every shape is checked before the first launch: a refused call returns -1 with dX, dWa_ext and
+ * dqv untouched.  Nothing outside X's columns [0, D], Wa's columns [0, D), WaT's columns [0, q) and dout's columns [0, D)
+ * reaches a result (NaN there is harmless).  dX is the same bits on every run; dWa_ext and dqv are sums of atomic adds.
+ * workspace: nr_additive_attention_bwd_workspace(...) bytes: dscore fp32 [rows] at 0, dPre bf16 [rows][round_up(q, 16)] at
+ * the next 256-byte boundary. */
 long long nr_additive_attention_bwd_workspace(long long n_seg, int seg_len, int q);
 int nr_additive_attention_bwd(const void* X_bf16, long long n_seg, int seg_len, int D, int ldx, const void* Wa_bf16,
                               const void* WaT_bf16, int q, int ldw, int ldwT, const float* ba, const float* qv,

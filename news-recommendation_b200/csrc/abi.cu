@@ -125,16 +125,30 @@ int nr_additive_attention_bwd(const void* X, long long n_seg, int seg_len, int D
                               void* workspace, long long workspace_bytes, void* stream) {
     NR_REQUIRE(X && Wa && WaT && ba && qv && w && dout && dX && dWa_ext && dqv && workspace,
                "nr_additive_attention_bwd: null operand");
+    // Every shape is checked before the first launch: the stages run in a row and dqv / dWa_ext accumulate, so a shape refused
+    // by a later stage would return an error after an earlier one had changed them.  w comes from the forward: seg_len <= 64.
+    NR_REQUIRE(n_seg >= 0 && seg_len >= 1 && seg_len <= 64 && q >= 1 && q <= 256 && D >= 4 && D % 4 == 0,
+               "nr_additive_attention_bwd: bad shape n_seg=%lld seg_len=%d D=%d q=%d", n_seg, seg_len, D, q);
+    NR_REQUIRE(ldx % 8 == 0 && ldx >= D + 1 && ldw % 8 == 0 && ldw >= D && ldwT % 8 == 0 && ldwT >= q && ldo % 4 == 0 && ldo >= D &&
+                   ld_dx % 8 == 0 && ld_dx >= D,
+               "nr_additive_attention_bwd: bad pitches ldx=%d ldw=%d ldwT=%d ldo=%d ld_dx=%d (D=%d q=%d)", ldx, ldw, ldwT, ldo, ld_dx, D, q);
+    const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };  // TMA bases, 16-byte dOut loads
+    NR_REQUIRE(a16(X) && a16(Wa) && a16(WaT) && a16(dout) && a16(dX) && a16(workspace), "nr_additive_attention_bwd: operand not 16-byte aligned");
     const long long rows = n_seg * seg_len;
+    NR_REQUIRE(rows < (1ll << 31), "nr_additive_attention_bwd: too many rows");
     const AdditiveBwdWorkspace ws(workspace, rows, q);
     NR_REQUIRE(workspace_bytes >= ws.bytes(), "nr_additive_attention_bwd: workspace too small");
-    NR_REQUIRE(rows < (1ll << 31), "nr_additive_attention_bwd: too many rows");
     const int M = static_cast<int>(rows);
     const int ldq = round_up(q, 16);
+    const GemmOperands dx_gemm{.A = ws.dpre, .M = M, .lda = ldq, .W = WaT, .N = D, .ldw = ldwT, .K = q};
+    const PoolDInputCfg dx_cfg{.w = w, .dout = dout, .ldo = ldo, .seg_len = seg_len, .dx = dX, .ld_dx = ld_dx};
+    NR_PROPAGATE(pool_dscore_check(ldx, D, seg_len, ldo));
+    NR_PROPAGATE(additive_dpre_check(q, D, ldq));
+    NR_PROPAGATE(pool_dinput_check(dx_gemm, dx_cfg));
+    if (M == 0) return 0;
     NR_PROPAGATE(pool_dscore(X, ldx, D, n_seg, seg_len, w, dout, ldo, ws.dscore, as_stream(stream)));
     NR_PROPAGATE(gemm_additive_dpre(X, M, ldx, D, Wa, q, ldw, ba, qv, ws.dscore, ws.dpre, ldq, dqv, as_stream(stream)));
-    NR_PROPAGATE(gemm_pool_dinput({.A = ws.dpre, .M = M, .lda = ldq, .W = WaT, .N = D, .ldw = ldwT, .K = q},
-                                  {.w = w, .dout = dout, .ldo = ldo, .seg_len = seg_len, .dx = dX, .ld_dx = ld_dx}, as_stream(stream)));
+    NR_PROPAGATE(gemm_pool_dinput(dx_gemm, dx_cfg, as_stream(stream)));
     NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, q, ldq, X, D, ldx, dWa_ext, as_stream(stream)));  // the ones column of X: d(bias)
     return 0;
 }

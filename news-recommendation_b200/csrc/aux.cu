@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(256) pool_dscore_warp_kernel(const __nv_bfloat
                                                                const float* __restrict__ dout, int ldo,
                                                                float* __restrict__ dscore) {
     const int lane = threadIdx.x & 31;
-    const int chunks = (D + 7) >> 3;  // the last one may be half valid (D % 8 == 4): its dOut half is zeroed below
+    const int chunks = (D + 7) >> 3;  // the last one may be half valid (D % 8 == 4): its dOut and X halves are zeroed below
     const long long wstride = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
     for (long long seg = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); seg < n_seg; seg += wstride) {
         const float* dob = dout + seg * ldo;
@@ -302,6 +302,8 @@ __global__ void __launch_bounds__(256) pool_dscore_warp_kernel(const __nv_bfloat
                 for (int h = 0; h < 2; ++h) {
                     const int c = lane + 32 * h;
                     u[k][h] = (t < seg_len && c < chunks) ? __ldg(xs + static_cast<long long>(t) * pitch16 + c) : make_uint4(0, 0, 0, 0);
+                    // the half past D of a half-valid chunk is X's pitch (the ones column, then anything): 0 * NaN would be NaN
+                    if (c * 8 + 8 > D) u[k][h].z = u[k][h].w = 0u;
                 }
             }
 #pragma unroll
@@ -329,10 +331,16 @@ __global__ void __launch_bounds__(256) pool_dscore_warp_kernel(const __nv_bfloat
     }
 }
 
+int pool_dscore_check(int lda, int D, int seg_len, int ldo) {
+    NR_REQUIRE(seg_len >= 1 && seg_len <= 128 && D % 4 == 0 && ldo % 4 == 0 && lda % 8 == 0, "pool_dscore: seg_len=%d D=%d ldo=%d lda=%d",
+               seg_len, D, ldo, lda);
+    return 0;
+}
+
 int pool_dscore(const void* X, int lda, int D, long long n_seg, int seg_len, const float* w, const float* dout, int ldo,
                 float* dscore, cudaStream_t stream) {
     if (n_seg == 0) return 0;
-    NR_REQUIRE(seg_len <= 128 && D % 4 == 0 && ldo % 4 == 0 && lda % 8 == 0, "pool_dscore: seg_len=%d D=%d ldo=%d lda=%d", seg_len, D, ldo, lda);
+    NR_PROPAGATE(pool_dscore_check(lda, D, seg_len, ldo));
     const long long groups = (n_seg + kDsSegs - 1) / kDsSegs;
     const int blocks = static_cast<int>(std::min<long long>(groups, 148 * 8));
     ProfScope ps("pool_dscore", static_cast<int>(n_seg), seg_len, D, stream);

@@ -706,14 +706,23 @@ int gemm_additive_pool(const void* X, int M, int lda, int D, const void* Wa, int
     return launch_gemm_nt(plan, e, X, lda, Wa, ldw, stream);
 }
 
+// The weight slicing of a plan depends on N, K, taps and the caps only: the shape checks below plan an empty problem, so that
+// nr_additive_attention_bwd can run them before its first launch.
+int additive_dpre_check(int q, int D, int ld_dpre) {
+    NR_REQUIRE(q >= 1 && q <= 256 && ld_dpre % 8 == 0 && ld_dpre >= round_up(q, 8), "additive_dpre: q=%d ld=%d", q, ld_dpre);
+    GemmNTPlan plan;
+    NR_PROPAGATE(plan_gemm_nt(&plan, nullptr, 0, D, nullptr, q, D, D, 1, 0, kTileM, 1, 1, kEpiSmemBytes<EpiDPre>, 0));
+    NR_REQUIRE(plan.p.n_slices == 1, "additive_dpre: q=%d D=%d does not fit one weight slice", q, D);
+    return 0;
+}
+
 int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int q, int ldw, const float* ba,
                        const float* qv, const float* dscore, void* dpre, int ld_dpre, float* dqv,
                        cudaStream_t stream) {
     if (M == 0) return 0;
-    NR_REQUIRE(q <= 256 && ld_dpre % 8 == 0 && ld_dpre >= round_up(q, 8), "additive_dpre: q=%d ld=%d", q, ld_dpre);
+    NR_PROPAGATE(additive_dpre_check(q, D, ld_dpre));
     GemmNTPlan plan;
     NR_PROPAGATE(plan_gemm_nt(&plan, X, M, lda, Wa, q, ldw, D, 1, 0, kTileM, num_sms(), 1, kEpiSmemBytes<EpiDPre>, 0));
-    NR_REQUIRE(plan.p.n_slices == 1, "additive_dpre: q=%d D=%d does not fit one weight slice", q, D);
     EpiDPre e;
     memset(&e, 0, sizeof(e));
     e.use_tma = q >= 32 ? 1 : 0;
@@ -729,17 +738,31 @@ int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int
     return launch_gemm_nt(plan, e, X, lda, Wa, ldw, stream);
 }
 
+// identity rows, no mask and at least one whole 32-column chunk: the fragment view; otherwise the row view
+static bool pool_dinput_frag(const GemmOperands& g, const PoolDInputCfg& c) {
+    return c.rm.seg_in == 0 && c.relu_src == nullptr && !c.zero_pad_rows && g.N >= 32;
+}
+// the epilogue stages the dOut rows of every segment a tile touches (<= 64 / seg_len + 2): cap the slice width so that they fit
+static int pool_dinput_max_stride(int seg_len) { return (DOutStage::kStageFloats / (kTileM / seg_len + 2)) & ~15; }
+
+int pool_dinput_check(const GemmOperands& g, const PoolDInputCfg& c) {
+    const int seg_len = c.seg_len;
+    NR_REQUIRE(seg_len >= 1, "pool_dinput: seg_len=%d", seg_len);
+    const int max_stride = pool_dinput_max_stride(seg_len);
+    NR_REQUIRE(max_stride >= 16, "pool_dinput: seg_len=%d needs %d staged segments per tile", seg_len, kTileM / seg_len + 2);
+    NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
+    GemmNTPlan plan;
+    return plan_gemm_nt(&plan, nullptr, 0, g.lda, nullptr, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, 1, 0,
+                        pool_dinput_frag(g, c) ? kEpiSmemBytes<EpiDPoolInFrag> : kEpiSmemBytes<EpiDPoolIn>, max_stride);
+}
+
 int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t stream) {
     const int M = g.M, D = g.N, seg_len = c.seg_len;
     if (M == 0) return 0;
-    NR_REQUIRE(seg_len >= 1, "pool_dinput: seg_len=%d", seg_len);
-    // the epilogue stages the dOut rows of every segment a tile touches: cap the slice width so that they fit
-    const int nseg_max = kTileM / seg_len + 2;
-    const int max_stride = (DOutStage::kStageFloats / nseg_max) & ~15;
-    NR_REQUIRE(max_stride >= 16, "pool_dinput: seg_len=%d needs %d staged segments per tile", seg_len, nseg_max);
-    NR_REQUIRE(c.ld_dx % 8 == 0, "pool_dinput: ld_dx=%d", c.ld_dx);
+    NR_PROPAGATE(pool_dinput_check(g, c));
+    const int max_stride = pool_dinput_max_stride(seg_len);
     GemmNTPlan plan;
-    if (c.rm.seg_in == 0 && c.relu_src == nullptr && !c.zero_pad_rows && D >= 32) {  // identity rows, no mask: the fragment view
+    if (pool_dinput_frag(g, c)) {
         NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                                   kEpiSmemBytes<EpiDPoolInFrag>, max_stride));
         EpiDPoolInFrag e{.w = c.w, .dout = c.dout, .ldo = c.ldo, .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx,

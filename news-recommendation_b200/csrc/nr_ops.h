@@ -61,6 +61,8 @@ int gemm_additive_pool(const void* X, int M, int lda, int D, const void* Wa, int
 int gemm_additive_dpre(const void* X, int M, int lda, int D, const void* Wa, int q, int ldw, const float* ba,
                        const float* qv, const float* dscore, void* dpre, int ld_dpre, float* dqv,
                        cudaStream_t stream);
+// gemm_additive_dpre's shape checks (host-only, no launch): q in [1, 256], the dPre pitch, one weight slice of q x D
+int additive_dpre_check(int q, int D, int ld_dpre);
 
 // dX = dPre . Wa + w (x) dOut [* relu mask] [* dropout] -> bf16, on {.A = dPre, .N = D, .K = q, .W = Wa^T}; w and dOut
 // (pitch ldo) are the pooling weights and output gradient of segments of seg_len rows
@@ -76,6 +78,8 @@ struct PoolDInputCfg {
     int relu_ld = 0;
 };
 int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t stream);
+// gemm_pool_dinput's shape checks (host-only, no launch): seg_len >= 1, the dOut staging cap, ld_dx % 8, the GEMM's plan
+int pool_dinput_check(const GemmOperands& g, const PoolDInputCfg& c);
 
 // dEmb[ids[row]] += A . W^T (embedding gradient of a [V x N] table; padding row 0 skipped) [* dropout of the gathered rows, pitch drop_ld]
 struct ScatterEmbCfg {
@@ -150,6 +154,8 @@ int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int l
 // dscore_r = w_r (dw_r - sum_seg w dw), dw_r = dOut[seg] . X_r
 int pool_dscore(const void* X, int lda, int D, long long n_seg, int seg_len, const float* w, const float* dout, int ldo,
                 float* dscore, cudaStream_t stream);
+// pool_dscore's shape checks (host-only, no launch): 1 <= seg_len <= 128, D % 4, ldo % 4, lda % 8
+int pool_dscore_check(int lda, int D, int seg_len, int ldo);
 // logits[b][c] = cand[b][c] . user[b]
 int dot_score_fwd(const float* cand, const float* user, int B, int C, int D, float* logits, cudaStream_t stream);
 int dot_score_bwd(const float* cand, const float* user, const float* dlogits, int B, int C, int D, float* dcand,

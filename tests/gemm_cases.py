@@ -1,5 +1,5 @@
-"""Case tables of the element-by-element GEMM and pooling-forward tests (tests/test_gpu_gemm_elements.py,
-tests/test_gpu_additive_fwd.py).  Each case names the planner regimes it is there to reach; tests/test_gemm_plan_host.py
+"""Case tables of the element-by-element GEMM and pooling tests (tests/test_gpu_gemm_elements.py,
+tests/test_gpu_additive_fwd.py, tests/test_gpu_additive_bwd_elements.py).  Each case names the planner regimes it is there to reach; tests/test_gemm_plan_host.py
 checks those names against the planner restatement (tests/gemm_plan_ref.py) on an H100 SXM's 132 SMs, and that every
 regime has a case.  Plain Python: importable without CUDA."""
 from __future__ import annotations
@@ -76,3 +76,29 @@ def linear_shape(c):
     taps = c.get("taps", 1)
     M = c["n_seg"] * (c["T"] + 2) if taps > 1 else c["M"]
     return M, c.get("rpt", 64), (c["N"] if taps > 1 else 0)
+
+# nr_additive_attention_bwd (tests/test_gpu_additive_bwd_elements.py): n_seg segments of seg rows, X [rows][D], Wa [q][D]; w
+# comes from the forward on the same operands (hilo: from nr_additive_attention_fwd_hilo).  scores as in POOL_CASES.  ldo: dout
+# pitch (default: D rounded up to 4, plus 4); ld_dx: dX pitch (default ldx = round_up(D + 1, 8)).  The regimes are those of
+# gemm_plan_ref.regimes_bwd: BWD_REGIMES plus the NT_REGIMES of the dPre and dX plans, prefixed "dPre " and "dX ".
+POOL_BWD_CASES = [
+    dict(id="bwd_S1_D300", n_seg=1000, seg=1, D=300, q=200,
+         regimes=("dscore warp", "dPre TMA", "dX fragment view", "dX slice capped by dOut staging", "dX slices > 1")),
+    dict(id="bwd_S2_D300", n_seg=777, seg=2, D=300, q=200, regimes=("dX slice capped by dOut staging", "dX slices > 1")),
+    dict(id="bwd_S3_D300", n_seg=2000, seg=3, D=300, q=200, regimes=("dX slice capped by dOut staging",)),
+    dict(id="bwd_S4_D400_view_fusion", n_seg=1000, seg=4, D=400, q=200,
+         regimes=("dX slice capped by dOut staging", "dPre streamed weights", "dX slice width % 32 != 0")),
+    dict(id="bwd_S20_D300_news_peaked", n_seg=3000, seg=20, D=300, q=200, scores="peaked", regimes=("dscore warp", "dX slices > 1")),
+    dict(id="bwd_S50_D300_user", n_seg=512, seg=50, D=300, q=200, regimes=("dscore block",)),
+    dict(id="bwd_S32_D300", n_seg=300, seg=32, D=300, q=200, regimes=("dscore warp",)),
+    dict(id="bwd_S33_D300", n_seg=300, seg=33, D=300, q=200, regimes=("dscore block",)),
+    dict(id="bwd_S64_D300_tied", n_seg=100, seg=64, D=300, q=200, scores="tied", regimes=("dscore block",)),
+    dict(id="bwd_S20_D604", n_seg=100, seg=20, D=604, q=200,
+         regimes=("dscore block D>512", "weight grad 2 launches", "dPre streamed weights")),
+    dict(id="bwd_S20_D24_q16", n_seg=500, seg=20, D=24, q=16, regimes=("dX row view", "dPre plain stores", "dX N < 32", "dPre N < 32")),
+    dict(id="bwd_S30_D64_q256", n_seg=50, seg=30, D=64, q=256, regimes=("dPre TMA", "dX 1 slice")),
+    dict(id="bwd_S3_D296_q24_many", n_seg=5000, seg=3, D=296, q=24, regimes=("dPre plain stores", "dX slices > 1")),
+    dict(id="bwd_S20_D300_one_tile", n_seg=1, seg=20, D=300, q=200, regimes=("dPre warpgroup 1 idle", "dX warpgroup 1 idle")),
+    dict(id="bwd_S20_D300_pitches", n_seg=37, seg=20, D=300, q=200, ldo=312, ld_dx=320, regimes=("dX fragment view",)),
+    dict(id="bwd_S50_D400_hilo", n_seg=64, seg=50, D=400, q=200, hilo=True, regimes=("dscore block", "dPre streamed weights")),
+]

@@ -1,7 +1,8 @@
 """Plain-Python restatement of the wgmma GEMM planners (importable without CUDA).
 
 plan_nt restates plan_gemm_nt (csrc/gemm.cu) line for line and adds the tiles each (CTA, consumer warpgroup) processes under
-gemm_nt_kernel's schedule; plan_tn restates gemm_tn_accumulate and launch_gemm_tn_kernel.  The GPU tests label every case
+gemm_nt_kernel's schedule; plan_tn restates gemm_tn_accumulate and launch_gemm_tn_kernel; plan_pool_bwd restates the kernel
+choices of the additive-attention backward's four launches.  The GPU tests label every case
 with the regime it is there to reach (regimes_nt / regimes_tn), tests/test_gemm_plan_host.py checks those labels here, and
 tests/test_gpu_gemm_elements.py ties this restatement to the real planner through the kernel's per-CTA counters."""
 from __future__ import annotations
@@ -17,6 +18,14 @@ kXposeBytes = 2 * 2 * kTileM * 16 * 4                  # kXposeBytes (row view: 
 EPI_STORE_SMEM = 1024 + (8 * 6 * 16 * 64 + 1024)       # EpiStore (fragment view): 1 KB bias + FragStore<6> = 51,200 B
 EPI_POOL_SMEM = 4096 + kXposeBytes                     # EpiPool (row view): 4 KB scratch + transpose = 20,480 B
 assert EPI_STORE_SMEM == 51200 and EPI_POOL_SMEM == 20480
+# the pooling backward's epilogues
+kStageFloats = 1536                                    # DOutStage::kStageFloats: staged dOut floats per buffer
+DOUT_STAGE_SMEM = 4 * kStageFloats * 4                 # DOutStage: 2 buffers per warpgroup = 24,576 B
+kTileStoreBytes = 8 * 2 * 2048 + 1024                  # kTileStoreBytes (nr_gemm.cuh): 2 staging tiles per epilogue warp
+EPI_DPRE_SMEM = 3072 + (8 * 4 * 16 * 64 + 1024)        # EpiDPre (fragment view): 3 KB + FragStore<4> = 36,864 B
+EPI_DPOOLIN_FRAG_SMEM = DOUT_STAGE_SMEM + (8 * 6 * 16 * 64 + 1024)   # EpiDPoolInFrag: dOut stage + FragStore<6> = 74,752 B
+EPI_DPOOLIN_SMEM = DOUT_STAGE_SMEM + kTileStoreBytes + kXposeBytes   # EpiDPoolIn (row view) + transpose = 74,752 B
+assert EPI_DPRE_SMEM == 36864 and EPI_DPOOLIN_FRAG_SMEM == 74752 and EPI_DPOOLIN_SMEM == 74752
 
 H100_SMS = 132                 # H100 SXM5; the GPU tests plan with the device's own count (nr_num_sms)
 
@@ -75,6 +84,31 @@ def plan_pool(M, D, q, seg_len, sms=H100_SMS):
     return plan_nt(M, q, D, 1, (kTileM // seg_len) * seg_len, sms, EPI_POOL_SMEM, max_slices=1)
 
 
+def pool_dinput_max_stride(seg_len):
+    """gemm_pool_dinput's cap on the slice width: the dOut rows of every segment a 64-row tile touches (<= 64 / seg_len + 2)
+    must fit one DOutStage buffer."""
+    return (kStageFloats // (kTileM // seg_len + 2)) & ~15
+
+
+def plan_pool_bwd(n_seg, seg_len, D, q, sms=H100_SMS):
+    """nr_additive_attention_bwd's four launches (csrc/abi.cu):
+      dscore   pool_dscore: the warp kernel when seg_len <= 32 and D <= 512, else the block kernel
+      dpre     gemm_additive_dpre: pre = X . Wa^T (N = q, K = D) in one weight slice; dPre leaves by TMA when q >= 32,
+               by plain stores otherwise
+      dx       gemm_pool_dinput: dPre . Wa (N = D, K = q), the slice width capped by the dOut staging; the fragment-view
+               EpiDPoolInFrag when D >= 32, the row-view EpiDPoolIn otherwise
+      wgrad    gemm_weight_grad: [dWa | dba] over the D + 1 columns of X (its ones column), one gemm_tn per 512 columns"""
+    M = n_seg * seg_len
+    frag = D >= 32
+    smem = EPI_DPOOLIN_FRAG_SMEM if frag else EPI_DPOOLIN_SMEM
+    dx = plan_nt(M, D, q, 1, kTileM, sms, smem, max_stride=pool_dinput_max_stride(seg_len))
+    wgrad = [plan_tn(M, q, min(512, D + 1 - c0), sms) for c0 in range(0, D + 1, 512)]
+    return {"dscore": "warp" if seg_len <= 32 and D <= 512 else "block",
+            "dpre": plan_nt(M, q, D, 1, kTileM, sms, EPI_DPRE_SMEM, max_slices=1), "dpre_tma": q >= 32,
+            "dx": dx, "dx_frag": frag, "dx_uncapped_stride": plan_nt(M, D, q, 1, kTileM, sms, smem)["n_stride"], "wgrad": wgrad,
+            "D": D}
+
+
 def plan_tn(Kr, Ma, Nb, sms=H100_SMS, reserved=0):
     """gemm_tn_accumulate: tiles, columns per CTA (NT), cluster shape and k_slices_max, an upper bound on the k-ranges.  With a
     cluster the launch further caps k_slices by cudaOccupancyMaxActiveClusters, which only the device can answer, so the
@@ -99,6 +133,8 @@ NT_REGIMES = ("1 slice", "slices > 1", "slice width % 32 != 0", "N < 32", "resid
               "streamed weights", "taps 3", "rows_per_tile < 64", "warpgroup 1 idle", "odd tiles per CTA", "even tiles per CTA")
 TN_REGIMES = ("cluster 1x1", "cluster 2x1", "cluster 1x2", "cluster 2x2", "NT 64", "NT 128", "NT 192", "NT 256", "n_tiles 2",
               "single k-range")
+BWD_REGIMES = ("dscore warp", "dscore block", "dscore block D>512", "dPre TMA", "dPre plain stores", "dX fragment view",
+               "dX row view", "dX slice capped by dOut staging", "dX slices > 1", "weight grad 2 launches")
 
 
 def regimes_nt(p):
@@ -132,4 +168,23 @@ def regimes_tn(p):
         r.add("n_tiles 2")
     if p["total_chunks"] == 1:
         r.add("single k-range")
+    return r
+
+
+def regimes_bwd(p):
+    """Every regime of BWD_REGIMES a backward plan (plan_pool_bwd) is in, plus the NT_REGIMES of its two gemm_nt plans
+    prefixed "dPre " and "dX " ("dX slice capped by dOut staging": the staging cap, not the 256-column box limit, sets the
+    slice width)."""
+    r = {"dscore " + p["dscore"], "dPre TMA" if p["dpre_tma"] else "dPre plain stores",
+         "dX fragment view" if p["dx_frag"] else "dX row view"}
+    if p["dscore"] == "block" and p["D"] > 512:
+        r.add("dscore block D>512")
+    dx = p["dx"]
+    if dx["n_slices"] > 1:
+        r.add("dX slices > 1")
+    if dx["n_stride"] < p["dx_uncapped_stride"]:
+        r.add("dX slice capped by dOut staging")
+    if len(p["wgrad"]) == 2:
+        r.add("weight grad 2 launches")
+    r |= {"dPre " + x for x in regimes_nt(p["dpre"])} | {"dX " + x for x in regimes_nt(dx)}
     return r
