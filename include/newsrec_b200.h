@@ -133,6 +133,27 @@ int nr_dot_score_bwd(const float* cand, const float* user, const float* dlogits,
 int nr_slots_device_readable(const void* const* slots, int n);
 int nr_pack_slots(const void* const* slots, int n_clicked, int n_candidates, int B, int L, long long* out, void* stream);
 
+/* ---- device-resident feed (newsrec_b200.feed.DeviceFeed): the parsed news and behaviour tables live on the device and ONE
+   launch gathers a batch from them.  Every pointer is device memory.
+     behaviors int32 [R][H + C]: the news rows of behaviour row r -- its first H browsed news left-padded with the padding news,
+                                 then its C candidates;
+     records   int32 [R][2 + C]: user, clicked_news_length (the history length after truncation), the C clicked labels;
+     rows      int64 [B]:        the batch's behaviour rows, each in [0, R).
+   For each field f, table int32 [n_news][width] (every value of behaviors is a row of it) and out int64 [B*H + B*C][width]:
+     out[(b*H + h)*width + t]         = table[behaviors[rows[b]][h]][t]       rows [0, B*H): browsed news, impression-major
+     out[(B*H + b*C + c)*width + t]   = table[behaviors[rows[b]][H + c]][t]   then the candidates
+   and, each only when not null, user_out[b] = records[rows[b]][0], length_out[b] = records[rows[b]][1] (int64 [B]) and
+   clicked_out[c*B + b] = records[rows[b]][2 + c] (int64 [C][B]); records may be null when all three are.  At most 8 fields;
+   H >= 0, C >= 1, B >= 0 (0 launches nothing), width >= 1.  Rows are copied with 16-byte stores where width is even and out
+   is 16-byte aligned, with 16-byte loads as well where width is a multiple of 4 and table is 16-byte aligned. */
+typedef struct {
+    const int* table;
+    int width;
+    long long* out;
+} nr_feed_field;
+int nr_feed_gather(const nr_feed_field* fields, int n_fields, const int* behaviors, int H, int C, const int* records,
+                   const long long* rows, int B, long long* user_out, long long* length_out, long long* clicked_out, void* stream);
+
 /* Batched form of the evaluator's scoring loop (src/evaluate.py:245-265 calls get_prediction once per impression and
  * synchronises on .tolist() each time): the news vectors live in ONE device matrix news[n_news][D]; the candidates of
  * impression s are cand[seg_offsets[s] .. seg_offsets[s+1]) (indices into news), user[s] its user vector;

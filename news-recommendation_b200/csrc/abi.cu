@@ -193,6 +193,20 @@ int nr_pack_slots(const void* const* slots, int n_clicked, int n_candidates, int
     prof_context("feed");
     return pack_slots(slots, n_clicked, n_candidates, B, L, out, as_stream(stream));
 }
+int nr_feed_gather(const nr_feed_field* fields, int n_fields, const int* behaviors, int H, int C, const int* records,
+                   const long long* rows, int B, long long* user_out, long long* length_out, long long* clicked_out, void* stream) {
+    NR_REQUIRE(n_fields >= 0 && n_fields <= kFeedFields && (fields || n_fields == 0) && H >= 0 && C >= 1 && B >= 0,
+               "nr_feed_gather: bad arguments n_fields=%d H=%d C=%d B=%d", n_fields, H, C, B);
+    NR_REQUIRE(behaviors && rows && (records || !(user_out || length_out || clicked_out)), "nr_feed_gather: null operand");
+    FeedField f[kFeedFields];
+    for (int i = 0; i < n_fields; ++i) {
+        NR_REQUIRE(fields[i].table && fields[i].out && fields[i].width >= 1, "nr_feed_gather: bad field %d", i);
+        f[i] = {.table = fields[i].table, .width = fields[i].width, .out = fields[i].out};
+    }
+    prof_context("feed");
+    return feed_gather(f, n_fields, behaviors, H, C, {.records = records, .user = user_out, .length = length_out, .clicked = clicked_out},
+                       rows, B, as_stream(stream));
+}
 
 // ---- NRMS encoders ---------------------------------------------------------------------------------
 // Q | K | V sections of the projected rows start at columns 0, sec, 2*sec with sec = round_up(d, 8): every section (and so

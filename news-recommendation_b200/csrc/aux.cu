@@ -956,4 +956,83 @@ int pack_slots(const void* const* slots, int H, int C, int B, int L, long long* 
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Device feed: the news tables (int32 [n_news][width] per field), the behaviour table (int32 [R][H + C] news rows) and the
+// per-row records live on the device; ONE launch writes the batch's impression-major int64 id block of every field (the
+// layout pack_slots writes) and its records.  blockIdx.y is the field, y == n_fields the records (each output its own buffer:
+// the trainer may change clicked_news_length in place while autograd holds user).  A thread item copies
+// `vec` ids of one row: 4 (one 16-byte load, two 16-byte stores), 2 (an 8-byte load, one 16-byte store) or 1.
+// ------------------------------------------------------------------------------------------------
+struct FeedJob {
+    const int* table;
+    long long* out;
+    int width, vec;
+};
+struct FeedJobs {
+    FeedJob f[kFeedFields];
+};
+__global__ void __launch_bounds__(256) feed_gather_kernel(FeedJobs jobs, int n_fields, const int* __restrict__ beh, int H, int C,
+                                                          FeedRecords rec, const long long* __restrict__ rows, int B) {
+    const long long stride = gridDim.x * 256ll;
+    if (static_cast<int>(blockIdx.y) == n_fields) {
+        const int n_rec = 2 + C;
+        for (long long i = blockIdx.x * 256ll + threadIdx.x; i < static_cast<long long>(n_rec) * B; i += stride) {
+            const int k = static_cast<int>(i / B), b = static_cast<int>(i - static_cast<long long>(k) * B);
+            long long* out = k == 0 ? rec.user : (k == 1 ? rec.length : rec.clicked);
+            if (out) out[k < 2 ? b : i - 2ll * B] = rec.records[rows[b] * n_rec + k];
+        }
+        return;
+    }
+    const FeedJob j = jobs.f[blockIdx.y];
+    const int per_row = j.width / j.vec;
+    const long long n_browsed = static_cast<long long>(B) * H, total = static_cast<long long>(B) * (H + C) * per_row;
+    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += stride) {
+        const long long r = i / per_row;
+        const int k = static_cast<int>(i - r * per_row);
+        long long b, s;
+        if (r < n_browsed) {
+            b = r / H;
+            s = r - b * H;
+        } else {
+            b = (r - n_browsed) / C;
+            s = H + (r - n_browsed - b * C);
+        }
+        const int news = beh[rows[b] * (H + C) + s];
+        const int* src = j.table + static_cast<long long>(news) * j.width + k * j.vec;
+        long long* dst = j.out + r * j.width + k * j.vec;
+        if (j.vec == 4) {
+            const int4 v = __ldg(reinterpret_cast<const int4*>(src));
+            reinterpret_cast<longlong2*>(dst)[0] = make_longlong2(v.x, v.y);
+            reinterpret_cast<longlong2*>(dst)[1] = make_longlong2(v.z, v.w);
+        } else if (j.vec == 2) {
+            const int2 v = __ldg(reinterpret_cast<const int2*>(src));
+            *reinterpret_cast<longlong2*>(dst) = make_longlong2(v.x, v.y);
+        } else {
+            *dst = __ldg(src);
+        }
+    }
+}
+int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int H, int C, FeedRecords rec, const long long* rows, int B,
+                cudaStream_t stream) {
+    const int n_rec = rec.user || rec.length || rec.clicked ? 2 + C : 0;
+    if (B == 0 || (n_fields == 0 && n_rec == 0)) return 0;
+    const auto aligned = [](const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; };
+    FeedJobs jobs{};
+    long long most = static_cast<long long>(n_rec) * B;
+    for (int f = 0; f < n_fields; ++f) {
+        const FeedField& x = fields[f];
+        const bool even = x.width % 2 == 0 && aligned(x.out, 16);
+        const int vec = even && x.width % 4 == 0 && aligned(x.table, 16) ? 4 : (even && aligned(x.table, 8) ? 2 : 1);
+        jobs.f[f] = {.table = x.table, .out = x.out, .width = x.width, .vec = vec};
+        most = std::max(most, static_cast<long long>(B) * (H + C) * (x.width / vec));
+    }
+    ProfScope ps("feed_gather", n_fields, B, H + C, stream);
+    const dim3 grid(static_cast<unsigned>(std::max<long long>(1, std::min<long long>((most + 255) / 256, num_sms() * 8ll))),
+                    static_cast<unsigned>(n_fields + (n_rec > 0 ? 1 : 0)));
+    feed_gather_kernel<<<grid, 256, 0, stream>>>(jobs, n_fields, behaviors, H, C, rec, rows, B);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace nr

@@ -188,6 +188,20 @@ int impression_metrics(const float* scores, const unsigned char* labels, const l
 
 int slots_device_readable(const void* const* slots, int n);
 int pack_slots(const void* const* slots, int H, int C, int B, int L, long long* out, cudaStream_t stream);
+// one launch: every field's impression-major id block and the per-row records of a batch from the device feed's tables
+// (records [R][2 + C]: user, clicked_news_length, labels -> user_out / length_out [B], clicked_out [C][B], each optional)
+constexpr int kFeedFields = 8;
+struct FeedField {
+    const int* table;
+    int width;
+    long long* out;
+};
+struct FeedRecords {
+    const int* records;
+    long long *user, *length, *clicked;
+};
+int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int H, int C, FeedRecords rec, const long long* rows, int B,
+                cudaStream_t stream);
 int num_sms();
 extern int g_launches;  // kernels launched by this library (nr_launch_count)
 

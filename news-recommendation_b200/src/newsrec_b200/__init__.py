@@ -117,6 +117,11 @@ class GruBwdArgs(C.Structure):
     ]
 
 
+class FeedField(C.Structure):
+    """nr_feed_field (include/newsrec_b200.h)."""
+    _fields_ = [("table", _vp), ("width", _i), ("out", _vp)]
+
+
 # name -> (restype, argtypes).  Must list EVERY symbol include/newsrec_b200.h declares
 # (tests/test_abi_symbols.py cross-checks this table against the header and the built .so).
 SIGNATURES = {
@@ -150,6 +155,7 @@ SIGNATURES = {
     "nr_dot_score_fwd": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "nr_slots_device_readable": (_i, [_vp, _i]),
     "nr_pack_slots": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    "nr_feed_gather": (_i, [C.POINTER(FeedField), _i, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "nr_segment_dot": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp]),
     "nr_impression_metrics": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),
     "nr_accumulate_ext_grad": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),

@@ -29,10 +29,10 @@ import numpy as np
 _LIST_COLUMNS = ("title", "abstract", "title_entities", "abstract_entities")
 
 
-def read_news(directory, attributes):
+def read_news(directory, attributes, filename="news_parsed.tsv"):
     """news_parsed.tsv columns id + attributes (reference NewsDataset, evaluate.py:54-76): (ids list, {attr: int64 array})."""
     import pandas as pd
-    df = pd.read_table(path.join(directory, "news_parsed.tsv"), usecols=["id"] + list(attributes),
+    df = pd.read_table(path.join(directory, filename), usecols=["id"] + list(attributes),
                        converters={a: literal_eval for a in set(attributes) & set(_LIST_COLUMNS)})
     cols = {a: np.asarray(df[a].tolist(), dtype=np.int64) for a in attributes}
     return df["id"].tolist(), cols

@@ -18,6 +18,9 @@ editing it:
 * rank 0 alone writes TensorBoard events and checkpoints and runs `evaluate()` (train.py:248); its metrics are broadcast
   so that early stopping takes the same decision everywhere; `--device-evaluate` swaps the reference's evaluator for
   `newsrec_b200.evaluate.evaluate` (same signature; scoring and metrics on the device);
+* `--device-feed` replaces the trainer's `BaseDataset` with `newsrec_b200.feed.DeviceFeed` (tables parsed once and held on
+  the device, one gather launch per batch; SURVEY.md row N3); the DataLoader factory returns the feed's loader for it,
+  over the same sharding, seed and epoch counter;
 * compatibility shims the survey found necessary for the reference on current NumPy / pandas / torch.
 """
 from __future__ import annotations
@@ -59,6 +62,24 @@ def make_sharded_dataloader(base_loader_cls, rank, world, seed=0):
         if not torch.cuda.is_available():
             kwargs.pop("pin_memory", None)
         return base_loader_cls(dataset, *args, **kwargs)
+
+    return factory
+
+
+def make_feed_dataloader(base_factory, rank, world, seed=0):
+    """DataLoader factory that hands a DeviceFeed its own loader (rows sharded by a DistributedSampler with `seed`, a new
+    epoch each time the trainer re-creates the loader) and every other dataset to `base_factory`."""
+    from newsrec_b200.feed import DeviceFeed
+
+    state = {"epoch": 0}
+
+    def factory(dataset, *args, **kwargs):
+        if not isinstance(dataset, DeviceFeed):
+            return base_factory(dataset, *args, **kwargs)
+        loader = dataset.loader(kwargs.get("batch_size", args[0] if args else 1), shuffle=kwargs.get("shuffle", False),
+                                drop_last=kwargs.get("drop_last", False), rank=rank, world=world, seed=seed, epoch=state["epoch"])
+        state["epoch"] += 1
+        return loader
 
     return factory
 
@@ -123,12 +144,17 @@ def apply_compat_shims():
         torch.load = load
 
 
-def patch_trainer(train_module, rank, world, seed=0, device_evaluate=False):
+def patch_trainer(train_module, rank, world, seed=0, device_evaluate=False, device_feed=False):
     """Install the data-parallel pieces into an imported (reference) `train` module's namespace.  device_evaluate: the
     trainer's `evaluate` becomes newsrec_b200.evaluate.evaluate (its docstring lists where its metrics can differ from a
-    given reference environment: ties across labels, one-class impressions)."""
+    given reference environment: ties across labels, one-class impressions).  device_feed: the trainer's `BaseDataset`
+    becomes newsrec_b200.feed.DeviceFeed and its DataLoader returns the feed's loader for it."""
     import torch
     train_module.DataLoader = make_sharded_dataloader(train_module.DataLoader, rank, world, seed)
+    if device_feed:
+        from newsrec_b200.feed import DeviceFeed
+        train_module.BaseDataset = DeviceFeed
+        train_module.DataLoader = make_feed_dataloader(train_module.DataLoader, rank, world, seed)
     if world > 1 or os.environ.get("NEWSREC_FLAT_GRADS", "1") == "1":
         # the trainer reaches Adam through the global `torch.optim` module (train.py:127)
         torch.optim.Adam = make_all_reduce_adam(torch.optim.Adam, world)
@@ -154,6 +180,9 @@ def main(argv=None):
     ap.add_argument("--device-evaluate", action="store_true",
                     help="validate with newsrec_b200.evaluate.evaluate (all impressions scored and their AUC / MRR / nDCG computed "
                          "on the device) instead of the reference's evaluate.py")
+    ap.add_argument("--device-feed", action="store_true",
+                    help="train from newsrec_b200.feed.DeviceFeed: news and behaviour tables parsed once and kept on the device, "
+                         "every batch gathered there by one kernel launch instead of the reference's BaseDataset / DataLoader")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
                     help="override a knob of the selected <MODEL_NAME>Config before the trainer is imported (repeatable), "
                          "e.g. --set batch_size=512 --set num_workers=8")
@@ -210,7 +239,8 @@ def main(argv=None):
                 pass  # keep the string
             setattr(cfg, key, val)
     train = importlib.import_module("train")
-    patch_trainer(train, rank, world, args.seed, device_evaluate=args.device_evaluate)
+    feed = {"device_feed": True} if args.device_feed else {}  # without the flag: the call (and the patch) of before
+    patch_trainer(train, rank, world, args.seed, device_evaluate=args.device_evaluate, **feed)
     try:
         train.train()
     finally:

@@ -94,7 +94,11 @@ class SlotPacker:
         return out
 
     def pack(self, clicked, candidates, field, dev):
-        """-> (ids (B*H + B*C, ...), B): rows [0, B*H) are the browsed news impression-major, then the candidates."""
+        """-> (ids (B*H + B*C, ...), B): rows [0, B*H) are the browsed news impression-major, then the candidates.
+        A batch of the device feed (newsrec_b200.feed) already holds that block: it is returned, nothing is launched."""
+        from .feed import FeedSlots
+        if isinstance(clicked, FeedSlots) and isinstance(candidates, FeedSlots) and clicked.blocks is candidates.blocks:
+            return clicked.blocks[field], clicked.B
         H = len(clicked)
         direct = self._pack_direct([x[field] for x in clicked], [x[field] for x in candidates], dev)
         if direct is not None:
