@@ -176,6 +176,24 @@ int nr_segment_dot(const float* news, long long n_news, int D, const long long* 
 int nr_impression_metrics(const float* scores, const unsigned char* labels, const long long* seg_offsets, long long n_seg,
                           double* metrics, int* bad_label_flag, void* stream);
 
+/* Test-set predictions (the leaderboard's prediction.txt).  Impressions are delimited by seg_offsets as above.
+ *   nr_impression_ranks: ranks[i] = place_i + 1 (int32), place_i exactly as nr_impression_metrics defines it, so every
+ *     impression's ranks are a permutation of 1..n.  An impression holding a non-finite score sets *bad_score_flag and
+ *     gets ranks 0 (its order is undefined).  An impression has fewer than 2^31 candidates.
+ *   nr_prediction_line_offsets: line s is "<impression_ids[s]> [r_0,r_1,...,r_{n-1}]\n" in decimal ("<id> []\n" when
+ *     empty); writes line_offsets[s] = its first byte (int64, n_seg + 1 entries, line_offsets[n_seg] = the total) with
+ *     one length kernel and a CUB exclusive scan in workspace (nr_prediction_line_offsets_workspace(n_seg) bytes, -1 if
+ *     the query fails or n_seg >= 2^31 - 1).  impression_ids are int64 and meant to be non-negative (a negative one prints as its unsigned value).
+ *   nr_prediction_text: writes the bytes of every line into text[line_offsets[s] .. line_offsets[s + 1]) in one launch.
+ * All pointers are device memory.  Null operands or n_seg < 0 return -1 before any launch. */
+int nr_impression_ranks(const float* scores, const long long* seg_offsets, long long n_seg, int* ranks, int* bad_score_flag,
+                        void* stream);
+long long nr_prediction_line_offsets_workspace(long long n_seg);
+int nr_prediction_line_offsets(const long long* impression_ids, const int* ranks, const long long* seg_offsets, long long n_seg,
+                               long long* line_offsets, void* workspace, long long workspace_bytes, void* stream);
+int nr_prediction_text(const long long* impression_ids, const int* ranks, const long long* seg_offsets, long long n_seg,
+                       const long long* line_offsets, char* text, void* stream);
+
 /* Host-side glue of the weight-gradient GEMMs (nr_gemm_tn with the ones column): ext is [rows][ld] fp32 whose columns
  * [0,D) hold dW and column D holds db.  Adds them into the parameters' own gradient storage (dW [rows][D] contiguous,
  * db [rows] or null) and CLEARS ext, so the caller can keep it as a persistent accumulator across steps. */

@@ -176,6 +176,26 @@ int nr_impression_metrics(const float* scores, const unsigned char* labels, cons
                "nr_impression_metrics: null operand or n_seg=%lld", n_seg);
     return impression_metrics(scores, labels, seg_offsets, n_seg, metrics, bad_label_flag, as_stream(stream));
 }
+int nr_impression_ranks(const float* scores, const long long* seg_offsets, long long n_seg, int* ranks, int* bad_score_flag, void* stream) {
+    NR_REQUIRE(scores && seg_offsets && ranks && bad_score_flag && n_seg >= 0, "nr_impression_ranks: null operand or n_seg=%lld", n_seg);
+    return impression_ranks(scores, seg_offsets, n_seg, ranks, bad_score_flag, as_stream(stream));
+}
+long long nr_prediction_line_offsets_workspace(long long n_seg) {
+    NR_REQUIRE(n_seg >= 0, "nr_prediction_line_offsets_workspace: n_seg=%lld", n_seg);
+    return prediction_scan_bytes(n_seg);
+}
+int nr_prediction_line_offsets(const long long* impression_ids, const int* ranks, const long long* seg_offsets, long long n_seg,
+                               long long* line_offsets, void* workspace, long long workspace_bytes, void* stream) {
+    NR_REQUIRE(impression_ids && ranks && seg_offsets && line_offsets && workspace && n_seg >= 0,
+               "nr_prediction_line_offsets: null operand or n_seg=%lld", n_seg);
+    return prediction_line_offsets(impression_ids, ranks, seg_offsets, n_seg, line_offsets, workspace, workspace_bytes, as_stream(stream));
+}
+int nr_prediction_text(const long long* impression_ids, const int* ranks, const long long* seg_offsets, long long n_seg,
+                       const long long* line_offsets, char* text, void* stream) {
+    NR_REQUIRE(impression_ids && ranks && seg_offsets && line_offsets && text && n_seg >= 0,
+               "nr_prediction_text: null operand or n_seg=%lld", n_seg);
+    return prediction_text(impression_ids, ranks, seg_offsets, n_seg, line_offsets, text, as_stream(stream));
+}
 
 int nr_accumulate_ext_grad(float* ext, int rows, int ld, int D, float* dW, float* db, void* stream) {
     NR_REQUIRE(ext && dW && rows >= 0 && D >= 1, "nr_accumulate_ext_grad: null operand");

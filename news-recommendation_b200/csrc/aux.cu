@@ -1,8 +1,10 @@
 // Memory-bound companions of the wgmma GEMMs: the fp32 -> bf16 row conversions, the embedding-row gather, pooling-backward
-// row dots, the dot-product click scorer, the fp32 attention of the precise user encoder, impression scoring and metrics,
-// the batch feed.  All HBM-bound integer/byte or small-reduction work: coalesced 16-byte accesses, warp-shuffle reductions,
-// no tensor cores.
+// row dots, the dot-product click scorer, the fp32 attention of the precise user encoder, impression scoring, metrics, ranks
+// and the prediction text, the batch feed.  All HBM-bound integer/byte or small-reduction work: coalesced 16-byte accesses,
+// warp-shuffle reductions, no tensor cores.
 #include <algorithm>
+
+#include <cub/device/device_scan.cuh>
 
 #include "nr_common.cuh"
 #include "nr_ops.h"
@@ -784,6 +786,59 @@ __device__ __forceinline__ int score_key(float x) {
 }
 __device__ __forceinline__ bool finite_score(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
 
+// The place of every candidate of one impression of n candidates, for one warp: lane l owns candidates i = l, l+32, ... and
+// calls visit(i, place_i, neg_lt_i, neg_eq_i) for each, where place_i = #{j : s_j > s_i} + #{j > i : s_j == s_i} and, with
+// kLabels, neg_lt_i / neg_eq_i count the negatives (label 0) scoring below / level with it (0 without).  ck / cn are the
+// warp's shared-memory chunk of kMetricChunk keys / negative marks; an impression longer than that is staged chunk by chunk.
+// Ends with __syncwarp, so the warp may restage the chunk for its next impression.
+template <bool kLabels, typename Visit>
+__device__ __forceinline__ void impression_places(const float* sc, const unsigned char* lb, long long n, int lane, int* ck,
+                                                  unsigned char* cn, Visit&& visit) {
+    const bool one_chunk = n <= kMetricChunk;
+    if (one_chunk) {
+        for (int j = lane; j < n; j += 32) {
+            ck[j] = score_key(__ldg(sc + j));
+            if constexpr (kLabels) cn[j] = __ldg(lb + j) == 0;
+        }
+        __syncwarp();
+    }
+    for (long long i0 = 0; i0 < n; i0 += 32) {
+        const long long i = i0 + lane;
+        const bool own = i < n;
+        const int ki = own ? score_key(__ldg(sc + i)) : 0;
+        long long place = 0, neg_lt = 0, neg_eq = 0;  // place: #{higher} + #{level and later} = position in the descending order
+        for (long long c0 = 0; c0 < n; c0 += kMetricChunk) {
+            const int len = static_cast<int>(min(static_cast<long long>(kMetricChunk), n - c0));
+            if (!one_chunk) {
+                __syncwarp();
+                for (int j = lane; j < len; j += 32) {
+                    ck[j] = score_key(__ldg(sc + c0 + j));
+                    if constexpr (kLabels) cn[j] = __ldg(lb + c0 + j) == 0;
+                }
+                __syncwarp();
+            }
+            const int after = static_cast<int>(max(-1ll, min(static_cast<long long>(len), i - c0)));  // chunk slots j > after are later than i
+            int gt = 0, eq_after = 0, lt_neg = 0, eq_neg = 0;
+            for (int j = 0; j < len; ++j) {
+                const int kj = ck[j];
+                const int eq = kj == ki;
+                gt += kj > ki;
+                eq_after += eq & (j > after);
+                if constexpr (kLabels) {
+                    const int neg = cn[j];
+                    lt_neg += neg & (kj < ki);
+                    eq_neg += neg & eq;
+                }
+            }
+            place += gt + eq_after;
+            neg_lt += lt_neg;
+            neg_eq += eq_neg;
+        }
+        if (own) visit(i, place, neg_lt, neg_eq);
+    }
+    __syncwarp();  // the next impression restages this warp's chunk
+}
+
 __global__ void __launch_bounds__(kMetricWarps * 32) impression_metrics_kernel(const float* __restrict__ scores,
                                                                                const unsigned char* __restrict__ labels,
                                                                                const long long* __restrict__ seg_offsets, long long n_seg,
@@ -822,54 +877,15 @@ __global__ void __launch_bounds__(kMetricWarps * 32) impression_metrics_kernel(c
         // pass 2: lane l owns candidates i = l, l+32, ...; the comparison partners come from the shared-memory chunk
         unsigned long long auc2 = 0;  // sum over positives of 2 #{negatives below} + #{negatives level}
         double rr = 0.0, g5 = 0.0, g10 = 0.0;
-        const bool one_chunk = n <= kMetricChunk;
-        if (one_chunk) {
-            for (int j = lane; j < n; j += 32) {
-                ck[j] = score_key(__ldg(sc + j));
-                cn[j] = __ldg(lb + j) == 0;
-            }
-            __syncwarp();
-        }
-        for (long long i0 = 0; i0 < n; i0 += 32) {
-            const long long i = i0 + lane;
-            const bool own = i < n;
-            const int ki = own ? score_key(__ldg(sc + i)) : 0;
-            const bool pos_i = own && __ldg(lb + i) == 1;
-            long long place = 0, neg_lt = 0, neg_eq = 0;  // place: #{higher} + #{level and later} = position in the descending order
-            for (long long c0 = 0; c0 < n; c0 += kMetricChunk) {
-                const int len = static_cast<int>(min(static_cast<long long>(kMetricChunk), n - c0));
-                if (!one_chunk) {
-                    __syncwarp();
-                    for (int j = lane; j < len; j += 32) {
-                        ck[j] = score_key(__ldg(sc + c0 + j));
-                        cn[j] = __ldg(lb + c0 + j) == 0;
-                    }
-                    __syncwarp();
-                }
-                const int after = static_cast<int>(max(-1ll, min(static_cast<long long>(len), i - c0)));  // chunk slots j > after are later than i
-                int gt = 0, eq_after = 0, lt_neg = 0, eq_neg = 0;
-                for (int j = 0; j < len; ++j) {
-                    const int kj = ck[j];
-                    const int neg = cn[j];
-                    const int eq = kj == ki;
-                    gt += kj > ki;
-                    eq_after += eq & (j > after);
-                    lt_neg += neg & (kj < ki);
-                    eq_neg += neg & eq;
-                }
-                place += gt + eq_after;
-                neg_lt += lt_neg;
-                neg_eq += eq_neg;
-            }
-            if (pos_i) {
+        impression_places<true>(sc, lb, n, lane, ck, cn, [&](long long i, long long place, long long neg_lt, long long neg_eq) {
+            if (__ldg(lb + i) == 1) {
                 auc2 += static_cast<unsigned long long>(2 * neg_lt + neg_eq);
                 rr += 1.0 / static_cast<double>(place + 1);
                 const double g = place < 10 ? 1.0 / log2(static_cast<double>(place + 2)) : 0.0;
                 g10 += g;
                 g5 += place < 5 ? g : 0.0;
             }
-        }
-        __syncwarp();  // the next impression restages this warp's chunk
+        });
         auc2 = warp_total(auc2);
         rr = warp_total(rr);
         g5 = warp_total(g5);
@@ -895,6 +911,162 @@ int impression_metrics(const float* scores, const unsigned char* labels, const l
     ProfScope ps("impression_metrics", static_cast<int>(std::min<long long>(n_seg, 1 << 30)), 0, 0, stream);
     const int blocks = static_cast<int>(std::min<long long>((n_seg + kMetricWarps - 1) / kMetricWarps, 148 * 16));
     impression_metrics_kernel<<<blocks, kMetricWarps * 32, 0, stream>>>(scores, labels, seg_offsets, n_seg, metrics, bad_label_flag);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// test-set predictions (the leaderboard's prediction.txt: one line "<impression_id> [r1,r2,...,rn]" per impression, r_i the
+// 1-based rank of candidate i).  ranks[i] = place_i + 1 with the place nr_impression_metrics uses, so MRR / nDCG recomputed
+// from the file agree with the evaluator; one warp per impression, the same shared-memory chunks.  An impression holding a
+// non-finite score sets the flag and gets ranks 0: its order is undefined.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kMetricWarps * 32) impression_ranks_kernel(const float* __restrict__ scores,
+                                                                             const long long* __restrict__ seg_offsets, long long n_seg,
+                                                                             int* __restrict__ ranks, int* __restrict__ bad_flag) {
+    __shared__ int s_key[kMetricWarps][kMetricChunk];
+    const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
+    const long long nw = static_cast<long long>(gridDim.x) * kMetricWarps;
+    for (long long s = static_cast<long long>(blockIdx.x) * kMetricWarps + wl; s < n_seg; s += nw) {
+        const long long b = __ldg(seg_offsets + s);
+        const long long n = __ldg(seg_offsets + s + 1) - b;
+        const float* const sc = scores + b;
+        int* const rk = ranks + b;
+        bool bad = false;
+        for (long long i = lane; i < n; i += 32) bad |= !finite_score(__ldg(sc + i));
+        if (__any_sync(0xffffffffu, bad)) {
+            if (lane == 0) atomicExch(bad_flag, 1);
+            for (long long i = lane; i < n; i += 32) rk[i] = 0;
+            continue;
+        }
+        impression_places<false>(sc, nullptr, n, lane, s_key[wl], nullptr,
+                                 [&](long long i, long long place, long long, long long) { rk[i] = static_cast<int>(place + 1); });
+    }
+}
+int impression_ranks(const float* scores, const long long* seg_offsets, long long n_seg, int* ranks, int* bad_score_flag,
+                     cudaStream_t stream) {
+    if (n_seg == 0) return 0;
+    ProfScope ps("impression_ranks", static_cast<int>(std::min<long long>(n_seg, 1 << 30)), 0, 0, stream);
+    const int blocks = static_cast<int>(std::min<long long>((n_seg + kMetricWarps - 1) / kMetricWarps, 148 * 16));
+    impression_ranks_kernel<<<blocks, kMetricWarps * 32, 0, stream>>>(scores, seg_offsets, n_seg, ranks, bad_score_flag);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// The text of the ranks: line s is "<ids[s]> [r_0,r_1,...,r_{n-1}]\n" (ids printed as unsigned decimal, ranks as unsigned
+// decimal), its bytes at text[line_offsets[s] .. line_offsets[s+1]).  The lengths kernel and the text kernel count the same
+// digits, so every line fills exactly its slot whatever the values.  One warp per impression; each lane writes the digits of
+// its candidates at the position a warp scan of the digit counts gives, followed by ',' (or ']' after the last).
+__device__ __forceinline__ int decimal_digits(unsigned long long v) {
+    int d = 1;
+    while (v >= 10ull) {
+        v /= 10ull;
+        ++d;
+    }
+    return d;
+}
+__device__ __forceinline__ void write_decimal(char* out, unsigned long long v, int digits) {
+    for (int k = digits - 1; k >= 0; --k) {
+        out[k] = static_cast<char>('0' + v % 10ull);
+        v /= 10ull;
+    }
+}
+constexpr int kTextWarps = 8;
+__global__ void __launch_bounds__(kTextWarps * 32) prediction_line_lengths_kernel(const long long* __restrict__ ids,
+                                                                                  const int* __restrict__ ranks,
+                                                                                  const long long* __restrict__ seg_offsets,
+                                                                                  long long n_seg, long long* __restrict__ lengths) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = static_cast<long long>(gridDim.x) * kTextWarps;
+    if (blockIdx.x == 0 && threadIdx.x == 0) lengths[n_seg] = 0;  // the scan's last entry becomes the total
+    for (long long s = static_cast<long long>(blockIdx.x) * kTextWarps + (threadIdx.x >> 5); s < n_seg; s += nw) {
+        const long long b = __ldg(seg_offsets + s);
+        const long long n = __ldg(seg_offsets + s + 1) - b;
+        long long body = 0;  // every rank's digits and the ',' or ']' after it
+        for (long long i = lane; i < n; i += 32) body += decimal_digits(static_cast<unsigned>(__ldg(ranks + b + i))) + 1;
+        body = warp_total(body);
+        if (lane == 0)  // "<id> [" body "\n"; an empty impression is "<id> []\n"
+            lengths[s] = decimal_digits(static_cast<unsigned long long>(__ldg(ids + s))) + 2 + body + (n == 0) + 1;
+    }
+}
+__global__ void __launch_bounds__(kTextWarps * 32) prediction_text_kernel(const long long* __restrict__ ids, const int* __restrict__ ranks,
+                                                                          const long long* __restrict__ seg_offsets, long long n_seg,
+                                                                          const long long* __restrict__ line_offsets, char* __restrict__ text) {
+    const int lane = threadIdx.x & 31;
+    const long long nw = static_cast<long long>(gridDim.x) * kTextWarps;
+    for (long long s = static_cast<long long>(blockIdx.x) * kTextWarps + (threadIdx.x >> 5); s < n_seg; s += nw) {
+        const long long b = __ldg(seg_offsets + s);
+        const long long n = __ldg(seg_offsets + s + 1) - b;
+        char* const line = text + __ldg(line_offsets + s);
+        const unsigned long long id = static_cast<unsigned long long>(__ldg(ids + s));
+        const int id_digits = decimal_digits(id);
+        if (lane == 0) {
+            write_decimal(line, id, id_digits);
+            line[id_digits] = ' ';
+            line[id_digits + 1] = '[';
+        }
+        long long pos = id_digits + 2;
+        for (long long i0 = 0; i0 < n; i0 += 32) {
+            const long long i = i0 + lane;
+            const unsigned r = i < n ? static_cast<unsigned>(__ldg(ranks + b + i)) : 0u;
+            const int d = i < n ? decimal_digits(r) : 0;
+            int incl = d + (i < n);
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += v;
+            }
+            if (i < n) {
+                char* const at = line + pos + incl - d - 1;
+                write_decimal(at, r, d);
+                at[d] = i == n - 1 ? ']' : ',';
+            }
+            pos += __shfl_sync(0xffffffffu, incl, 31);
+        }
+        if (lane == 0) {
+            if (n == 0) line[pos++] = ']';
+            line[pos] = '\n';
+        }
+    }
+}
+constexpr long long kMaxTextLines = (1ll << 31) - 1;  // the scan counts its n_seg + 1 entries in int32
+static int text_blocks(long long n_seg) {
+    return static_cast<int>(std::min<long long>((n_seg + kTextWarps - 1) / kTextWarps, 148 * 16));
+}
+long long prediction_scan_bytes(long long n_seg) {
+    size_t bytes = 0;
+    if (n_seg >= kMaxTextLines ||
+        cub::DeviceScan::ExclusiveSum(nullptr, bytes, static_cast<long long*>(nullptr), static_cast<int>(n_seg + 1)) != cudaSuccess) {
+        cudaGetLastError();
+        return -1;
+    }
+    return static_cast<long long>(bytes);
+}
+int prediction_line_offsets(const long long* ids, const int* ranks, const long long* seg_offsets, long long n_seg, long long* line_offsets,
+                            void* workspace, long long workspace_bytes, cudaStream_t stream) {
+    NR_REQUIRE(n_seg < kMaxTextLines, "nr_prediction_line_offsets: n_seg=%lld lines (at most 2^31 - 2 per call)", n_seg);
+    const long long need = prediction_scan_bytes(n_seg);
+    NR_REQUIRE(need >= 0, "nr_prediction_line_offsets: scan workspace query failed for n_seg=%lld", n_seg);
+    NR_REQUIRE(workspace_bytes >= need, "nr_prediction_line_offsets: workspace of %lld bytes, %lld needed", workspace_bytes, need);
+    {
+        ProfScope ps("prediction_line_lengths", static_cast<int>(std::min<long long>(n_seg, 1 << 30)), 0, 0, stream);
+        prediction_line_lengths_kernel<<<std::max(1, text_blocks(n_seg)), kTextWarps * 32, 0, stream>>>(ids, ranks, seg_offsets, n_seg,
+                                                                                                         line_offsets);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    size_t bytes = static_cast<size_t>(need);
+    NR_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(workspace, bytes, line_offsets, static_cast<int>(n_seg + 1), stream));
+    g_launches += 2;  // the scan's tile-state initialisation and the decoupled look-back scan
+    return 0;
+}
+int prediction_text(const long long* ids, const int* ranks, const long long* seg_offsets, long long n_seg, const long long* line_offsets,
+                    char* text, cudaStream_t stream) {
+    if (n_seg == 0) return 0;
+    ProfScope ps("prediction_text", static_cast<int>(std::min<long long>(n_seg, 1 << 30)), 0, 0, stream);
+    prediction_text_kernel<<<text_blocks(n_seg), kTextWarps * 32, 0, stream>>>(ids, ranks, seg_offsets, n_seg, line_offsets, text);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -185,6 +185,15 @@ int segment_dot(const float* news, long long n_news, int D, const long long* can
 // metrics[s] = {AUC, MRR, nDCG@5, nDCG@10} of impression s (batched evaluate.py:160-168, 267-271)
 int impression_metrics(const float* scores, const unsigned char* labels, const long long* seg_offsets, long long n_seg, double* metrics,
                        int* bad_label_flag, cudaStream_t stream);
+// ranks[i] = place_i + 1 (the place impression_metrics uses); the prediction.txt lines of the ranks: their byte offsets (a CUB
+// exclusive scan of the line lengths in the caller's workspace of prediction_scan_bytes), then every line's bytes
+int impression_ranks(const float* scores, const long long* seg_offsets, long long n_seg, int* ranks, int* bad_score_flag,
+                     cudaStream_t stream);
+long long prediction_scan_bytes(long long n_seg);
+int prediction_line_offsets(const long long* ids, const int* ranks, const long long* seg_offsets, long long n_seg, long long* line_offsets,
+                            void* workspace, long long workspace_bytes, cudaStream_t stream);
+int prediction_text(const long long* ids, const int* ranks, const long long* seg_offsets, long long n_seg, const long long* line_offsets,
+                    char* text, cudaStream_t stream);
 
 int slots_device_readable(const void* const* slots, int n);
 int pack_slots(const void* const* slots, int H, int C, int B, int L, long long* out, cudaStream_t stream);

@@ -158,6 +158,10 @@ SIGNATURES = {
     "nr_feed_gather": (_i, [C.POINTER(FeedField), _i, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "nr_segment_dot": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp]),
     "nr_impression_metrics": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),
+    "nr_impression_ranks": (_i, [_vp, _vp, _ll, _vp, _vp, _vp]),
+    "nr_prediction_line_offsets_workspace": (_ll, [_ll]),
+    "nr_prediction_line_offsets": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _ll, _vp]),
+    "nr_prediction_text": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),
     "nr_accumulate_ext_grad": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "nr_dot_score_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "nr_mhsa_accurate_supported": (_i, [_i, _i, _i]),

@@ -54,20 +54,22 @@ def _rows(news_index, ids):
     return [news_index[x] for x in ids]  # KeyError on an unknown news id, as the reference's news2vector[...]
 
 
-def build_tables(directory, news_index, H, max_count=sys.maxsize, user2int_path="data/train/user2int.tsv"):
-    """Host half of stages 2 and 3 (reference UserDataset / BehaviorsDataset and the loop at evaluate.py:243-265).
+def read_behaviors(directory, **kw):
+    """behaviors.tsv as a DataFrame (columns impression_id, user, time, clicked_news, impressions); an empty history
+    becomes ' ' (the reference's fillna).  kw goes to pandas.read_table."""
+    import pandas as pd
+    beh = pd.read_table(path.join(directory, "behaviors.tsv"), header=None, usecols=range(5),
+                        names=["impression_id", "user", "time", "clicked_news", "impressions"], **kw)
+    beh["clicked_news"] = beh["clicked_news"].fillna(" ")
+    return beh
 
-    news_index maps a news id to its matrix row and "PADDED_NEWS" to the zero row.  Users: behaviors.tsv columns 1 and 3,
-    empty history -> ' ', duplicate (user, history) rows dropped; the FIRST row of each distinct history string defines its user (user2int, 0 if
-    unknown) and its first H news ids.  Impressions: the first max_count - 1 rows (the reference increments its counter
-    and breaks on count == max_count before scoring)."""
+
+def user_tables(beh, news_index, H, user2int_path):
+    """The user half of build_tables: (user, history, history_length, hist_row) -- one row per distinct history string
+    of beh (read_behaviors), hist_row mapping each string to its row."""
     import pandas as pd
     pad = news_index["PADDED_NEWS"]
-    beh = pd.read_table(path.join(directory, "behaviors.tsv"), header=None, usecols=range(5),
-                        names=["impression_id", "user", "time", "clicked_news", "impressions"])
-    beh["clicked_news"] = beh["clicked_news"].fillna(" ")
     user2int = dict(pd.read_table(user2int_path).values.tolist())
-
     users = beh[["user", "clicked_news"]].drop_duplicates()
     users = users[~users["clicked_news"].duplicated()]        # first-wins user2vector (evaluate.py:226-230)
     hist_row = {}
@@ -82,7 +84,18 @@ def build_tables(directory, news_index, H, max_count=sys.maxsize, user2int_path=
         length[r] = len(ids)
         if ids:
             history[r, H - len(ids):] = _rows(news_index, ids)
+    return user, history, length, hist_row
 
+
+def build_tables(directory, news_index, H, max_count=sys.maxsize, user2int_path="data/train/user2int.tsv"):
+    """Host half of stages 2 and 3 (reference UserDataset / BehaviorsDataset and the loop at evaluate.py:243-265).
+
+    news_index maps a news id to its matrix row and "PADDED_NEWS" to the zero row.  Users: behaviors.tsv columns 1 and 3,
+    empty history -> ' ', duplicate (user, history) rows dropped; the FIRST row of each distinct history string defines its user (user2int, 0 if
+    unknown) and its first H news ids.  Impressions: the first max_count - 1 rows (the reference increments its counter
+    and breaks on count == max_count before scoring)."""
+    beh = read_behaviors(directory)
+    user, history, length, hist_row = user_tables(beh, news_index, H, user2int_path)
     n_imp = len(beh) if max_count < 1 else min(len(beh), max_count - 1)
     imp = beh.iloc[:n_imp]
     seg_user = np.asarray([hist_row[hs] for hs in imp["clicked_news"].tolist()], np.int64)

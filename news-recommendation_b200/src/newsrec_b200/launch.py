@@ -171,6 +171,23 @@ def patch_trainer(train_module, rank, world, seed=0, device_evaluate=False, devi
         torch.save._newsrec_original = _save
 
 
+def set_knobs(items):
+    """Apply KNOB=VALUE strings to the selected <MODEL_NAME>Config (VALUE read as a Python literal, else kept as the
+    string); returns the config class."""
+    import ast
+    import importlib
+    cfgmod = importlib.import_module("config")
+    cfg = getattr(cfgmod, f"{cfgmod.model_name}Config")
+    for item in items:
+        key, _, val = item.partition("=")
+        try:
+            val = ast.literal_eval(val)
+        except (ValueError, SyntaxError):
+            pass  # keep the string
+        setattr(cfg, key, val)
+    return cfg
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--reference-src", required=True, help="the reference repository's src/ directory (train.py, dataset.py, evaluate.py)")
@@ -228,16 +245,7 @@ def main(argv=None):
 
     import importlib
     if args.set:
-        import ast
-        cfgmod = importlib.import_module("config")
-        cfg = getattr(cfgmod, f"{cfgmod.model_name}Config")
-        for item in args.set:
-            key, _, val = item.partition("=")
-            try:
-                val = ast.literal_eval(val)
-            except (ValueError, SyntaxError):
-                pass  # keep the string
-            setattr(cfg, key, val)
+        set_knobs(args.set)
     train = importlib.import_module("train")
     feed = {"device_feed": True} if args.device_feed else {}  # without the flag: the call (and the patch) of before
     patch_trainer(train, rank, world, args.seed, device_evaluate=args.device_evaluate, **feed)

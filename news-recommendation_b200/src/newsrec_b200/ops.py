@@ -542,3 +542,53 @@ def impression_metrics(scores, labels, seg_offsets):
     if int(flag.item()):
         raise ValueError("impression_metrics: a label is neither 0 nor 1")
     return metrics
+
+
+def impression_ranks(scores, seg_offsets, bad_score_flag=None):
+    """1-based rank of every candidate within its impression, one launch (nr_impression_ranks): ranks[i] = place_i + 1 with
+    the place nr_impression_metrics uses (ties: the later candidate first; -0 == +0), so each impression's ranks are a
+    permutation of 1..n.  scores (n_cand,) fp32, seg_offsets (n_impressions + 1,) int64.  Returns (n_cand,) int32 on the
+    device.  An impression with a non-finite score sets bad_score_flag (a device int32 the caller checks); without one,
+    a fresh flag is read here (one synchronisation) and ValueError raised."""
+    lib = load_library()
+    dev = require_cuda()
+    scores = scores.to(dev).float().contiguous()
+    seg_offsets = seg_offsets.to(dev).long().contiguous()
+    if seg_offsets.dim() != 1 or seg_offsets.numel() < 1:
+        raise NewsrecError("impression_ranks: seg_offsets must be (n_impressions + 1,)")
+    ranks = torch.empty(scores.shape, dtype=torch.int32, device=dev)
+    own = bad_score_flag is None
+    flag = torch.zeros(1, dtype=torch.int32, device=dev) if own else bad_score_flag
+    check(lib.nr_impression_ranks(_p(scores), _p(seg_offsets), seg_offsets.numel() - 1, _p(ranks), _p(flag), _stream()),
+          "nr_impression_ranks")
+    if own and int(flag.item()):
+        raise ValueError("impression_ranks: an impression holds a non-finite score; its ranks are undefined")
+    return ranks
+
+
+def prediction_text(impression_ids, ranks, seg_offsets):
+    """The prediction.txt bytes of many impressions, "<impression_id> [r1,r2,...,rn]\\n" per impression, as a (n_bytes,)
+    uint8 device tensor: line lengths and their exclusive scan (nr_prediction_line_offsets, CUB in the library), one read of
+    the total (a synchronisation), then one launch writing every line (nr_prediction_text).  impression_ids
+    (n_impressions,) int64, non-negative; ranks (n_cand,) int32 from impression_ranks; seg_offsets as there."""
+    lib = load_library()
+    dev = require_cuda()
+    ids = impression_ids.to(dev).long().contiguous()
+    ranks = ranks.to(dev).int().contiguous()
+    seg_offsets = seg_offsets.to(dev).long().contiguous()
+    n_seg = seg_offsets.numel() - 1
+    if ids.dim() != 1 or ids.numel() != n_seg:
+        raise NewsrecError("prediction_text: impression_ids must be (len(seg_offsets) - 1,)")
+    if n_seg == 0:
+        return torch.empty(0, dtype=torch.uint8, device=dev)
+    line_offsets = torch.empty(n_seg + 1, dtype=torch.int64, device=dev)
+    ws_bytes = int(lib.nr_prediction_line_offsets_workspace(n_seg))
+    if ws_bytes < 0:
+        check(-1, "nr_prediction_line_offsets_workspace")
+    workspace = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    check(lib.nr_prediction_line_offsets(_p(ids), _p(ranks), _p(seg_offsets), n_seg, _p(line_offsets), _p(workspace), ws_bytes,
+                                         _stream()), "nr_prediction_line_offsets")
+    text = torch.empty(int(line_offsets[-1].item()), dtype=torch.uint8, device=dev)
+    check(lib.nr_prediction_text(_p(ids), _p(ranks), _p(seg_offsets), n_seg, _p(line_offsets), _p(text), _stream()),
+          "nr_prediction_text")
+    return text
