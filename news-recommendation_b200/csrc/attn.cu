@@ -58,11 +58,6 @@ __device__ __forceinline__ void load_b_t(uint32_t* b, const __nv_bfloat16* tile,
     ldsm_x2_t(b, tile + (k0 + (lane & 7) + (((lane >> 3) & 1) << 3)) * pitch + n0);
 }
 
-__device__ __forceinline__ float drop_mult(uint64_t seed, uint32_t thresh, float scale, long long row, int ld, int col) {
-    const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(row) * ld + col) >> 2);
-    return (((bits >> (16 * (col & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-}
-
 // Row-block softmax on the S fragments of one 16-row m-tile.  s[nt][4] holds (row g: c0,c1 ; row g+8: c2,c3)
 // for key columns nt*8 + 2t, +1.  Input scores are pre-scaled into the log2 domain.  Returns P in place.
 template <int NTJ>
@@ -225,25 +220,22 @@ __device__ __forceinline__ void tile_store_map(const __nv_bfloat16* tile, __nv_b
 }
 // context tile -> global with dropout (one counter hash per 4 aligned columns), offsets from the plan
 __device__ __forceinline__ void tile_store_dropout_map(const __nv_bfloat16* tile, __nv_bfloat16* g, const PieceMap& m, int piece, int ld,
-                                                       long long row0, int col0, uint64_t seed, uint32_t thresh, float scale) {
+                                                       long long row0, int col0, const Dropout& drop) {
 #pragma unroll
     for (int k = 0; k < kMaxP; ++k) {
         if (m.lane + 32 * k < m.total) {
+            const long long row = row0 + m.row[k];
             const int gc = col0 + m.col[k];
-            const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(row0 + m.row[k]) * ld + gc) >> 2);
             if (piece == 8) {
+                float mk[4];
+                drop.mask4(row, ld, gc, mk);
                 const uint2 u = *reinterpret_cast<const uint2*>(tile + m.dst[k]);
-                float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-                a.x *= ((bits & 0xffffu) >= thresh) ? scale : 0.f;
-                a.y *= (((bits >> 16) & 0xffffu) >= thresh) ? scale : 0.f;
-                b.x *= (((bits >> 32) & 0xffffu) >= thresh) ? scale : 0.f;
-                b.y *= (((bits >> 48) & 0xffffu) >= thresh) ? scale : 0.f;
-                *reinterpret_cast<uint2*>(g + m.src[k]) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(b.x, b.y));
+                const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
+                *reinterpret_cast<uint2*>(g + m.src[k]) = make_uint2(pack_bf16x2(a.x * mk[0], a.y * mk[1]), pack_bf16x2(b.x * mk[2], b.y * mk[3]));
             } else {
-                float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(tile + m.dst[k]));
-                a.x *= (((bits >> (16 * (gc & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-                a.y *= (((bits >> (16 * ((gc + 1) & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-                *reinterpret_cast<uint32_t*>(g + m.src[k]) = pack_bf16x2(a.x, a.y);
+                const float2 mk = drop.mask2(row, ld, gc);
+                const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(tile + m.dst[k]));
+                *reinterpret_cast<uint32_t*>(g + m.src[k]) = pack_bf16x2(a.x * mk.x, a.y * mk.y);
             }
         }
     }
@@ -251,8 +243,7 @@ __device__ __forceinline__ void tile_store_dropout_map(const __nv_bfloat16* tile
 
 // context tile -> global with the dropout mask applied on the fly (one counter hash per 4 aligned columns)
 __device__ __forceinline__ void tile_store_dropout(const __nv_bfloat16* tile, __nv_bfloat16* g, int ld, int T, int dk, int piece, int lane,
-                                                   long long row0, int col0, uint64_t seed, uint32_t thresh, float scale, int nthr = 32,
-                                                   int pitch = kPitch) {
+                                                   long long row0, int col0, const Dropout& drop, int nthr = 32, int pitch = kPitch) {
     const int epp = piece >> 1;
     const int ppr = dk / epp;
     const float inv = 1.0f / static_cast<float>(ppr);
@@ -263,23 +254,18 @@ __device__ __forceinline__ void tile_store_dropout(const __nv_bfloat16* tile, __
         const __nv_bfloat16* src = tile + r * pitch + c;
         __nv_bfloat16* dst = g + static_cast<size_t>(r) * ld + c;
         const int gc = col0 + c;
-        const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(row0 + r) * ld + gc) >> 2);
         if (piece == 8) {
+            float mk[4];
+            drop.mask4(row0 + r, ld, gc, mk);
             const uint2 u = *reinterpret_cast<const uint2*>(src);
-            float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-            a.x *= ((bits & 0xffffu) >= thresh) ? scale : 0.f;
-            a.y *= (((bits >> 16) & 0xffffu) >= thresh) ? scale : 0.f;
-            b.x *= (((bits >> 32) & 0xffffu) >= thresh) ? scale : 0.f;
-            b.y *= (((bits >> 48) & 0xffffu) >= thresh) ? scale : 0.f;
-            *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(b.x, b.y));
+            const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
+            *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16x2(a.x * mk[0], a.y * mk[1]), pack_bf16x2(b.x * mk[2], b.y * mk[3]));
         } else if (piece == 4) {
-            float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(src));
-            a.x *= (((bits >> (16 * (gc & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-            a.y *= (((bits >> (16 * ((gc + 1) & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-            *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(a.x, a.y);
+            const float2 mk = drop.mask2(row0 + r, ld, gc);
+            const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(src));
+            *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(a.x * mk.x, a.y * mk.y);
         } else {
-            const float m = (((bits >> (16 * (gc & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-            *dst = __float2bfloat16_rn(__bfloat162float(*src) * m);
+            *dst = __float2bfloat16_rn(__bfloat162float(*src) * drop.mask2(row0 + r, ld, gc).x);
         }
     }
 }
@@ -310,7 +296,7 @@ __host__ __device__ inline int piece_bytes_bwd(int dk, int ld_a, int ld_b, int d
 template <int NTD, bool FAST, bool FIXED, bool COOP>
 __global__ void __launch_bounds__(kWarps * 32, COOP ? 3 : (FIXED ? 8 : 5)) mhsa_mma_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, int sec, long long n_seq,
                                                                   int T_, int heads_, int dk_, __nv_bfloat16* __restrict__ ctx,
-                                                                  int ld_ctx, float p, uint64_t seed) {
+                                                                  int ld_ctx, Dropout drop) {
     constexpr int TP = tile_rows(COOP), NTJ = TP / 8, MT = TP / 16, KSD = (NTD + 1) / 2;
     constexpr int CT = FIXED ? fixed_T(COOP) : 0;
     constexpr int PT = FIXED ? kPitch24 : kPitch;  // tile row pitch
@@ -330,8 +316,6 @@ __global__ void __launch_bounds__(kWarps * 32, COOP ? 3 : (FIXED ? 8 : 5)) mhsa_
     const int ctid = COOP ? tid : lane, cnt = COOP ? kWarps * 32 : 32;  // who copies a task's tiles
     auto phase_sync = [&]() { if (COOP) __syncthreads(); else __syncwarp(); };
     const float sc = rsqrtf(static_cast<float>(dk)) * 1.4426950408889634f;
-    const uint32_t thresh = static_cast<uint32_t>(p * 65536.0f + 0.5f);
-    const float dscale = p > 0.f ? 1.f / (1.f - p) : 1.f;
     const int ntj = (T + 7) >> 3;
     const int piece = FIXED ? 8 : piece_bytes(dk, ld, ld_ctx, sec);
     const int n_tasks = static_cast<int>(n_seq * heads);  // < 2^31, checked by the launcher
@@ -447,10 +431,10 @@ __global__ void __launch_bounds__(kWarps * 32, COOP ? 3 : (FIXED ? 8 : 5)) mhsa_
         phase_sync();
         __nv_bfloat16* out = ctx + seq * T * static_cast<long long>(ld_ctx);
         if constexpr (FAST) {
-            if (p > 0.f) tile_store_dropout_map(q, out + h * dk, smap, piece, ld_ctx, seq * T, h * dk, seed, thresh, dscale);
+            if (drop.active()) tile_store_dropout_map(q, out + h * dk, smap, piece, ld_ctx, seq * T, h * dk, drop);
             else tile_store_map(q, out + h * dk, smap, piece);
-        } else if (p > 0.f) {
-            tile_store_dropout(q, out + h * dk, ld_ctx, T, dk, piece, ctid, seq * T, h * dk, seed, thresh, dscale, cnt, PT);
+        } else if (drop.active()) {
+            tile_store_dropout(q, out + h * dk, ld_ctx, T, dk, piece, ctid, seq * T, h * dk, drop, cnt, PT);
         } else {
             tile_store(q, out + h * dk, ld_ctx, T, dk, piece, ctid, cnt, PT);
         }
@@ -757,7 +741,7 @@ __global__ void __launch_bounds__(kWarps * 32, COOP ? 3 : (FIXED ? 4 : 3)) mhsa_
 
 template <int NTD, bool FAST, bool FIXED, bool COOP>
 int launch_mma(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-               void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
+               void* out, int ld_out, const Dropout& drop, cudaStream_t stream) {
     const long long tasks = n_seq * heads;
     NR_REQUIRE(tasks < (1ll << 31), "mhsa: too many (sequence, head) tasks");
     constexpr int TP = tile_rows(COOP);
@@ -774,8 +758,7 @@ int launch_mma(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx,
     if (!bwd) {
         NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_mma_fwd_kernel<NTD, FAST, FIXED, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         mhsa_mma_fwd_kernel<NTD, FAST, FIXED, COOP><<<grid, kWarps * 32, smem, stream>>>(static_cast<const __nv_bfloat16*>(qkv), ld_qkv, sec, n_seq, T,
-                                                                                       heads, dk, static_cast<__nv_bfloat16*>(out), ld_out, drop.p,
-                                                                                       drop.seed);
+                                                                                       heads, dk, static_cast<__nv_bfloat16*>(out), ld_out, drop);
     } else {
         NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_mma_bwd_kernel<NTD, FAST, FIXED, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         mhsa_mma_bwd_kernel<NTD, FAST, FIXED, COOP><<<grid, kWarps * 32, smem, stream>>>(static_cast<const __nv_bfloat16*>(qkv), ld_qkv, sec,
@@ -789,7 +772,7 @@ int launch_mma(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx,
 
 template <bool FAST, bool COOP>
 int launch_dk(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-              void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
+              void* out, int ld_out, const Dropout& drop, cudaStream_t stream) {
     if (dk <= 16) return launch_mma<2, FAST, false, COOP>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
     if (dk <= 24) return launch_mma<3, FAST, false, COOP>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
     return launch_mma<4, FAST, false, COOP>(bwd, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, out, ld_out, drop, stream);
@@ -799,7 +782,7 @@ int launch_dk(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, 
 // the fixed-shape kernel for the reference's head shape when its rows move in 8-byte pieces.  Otherwise the per-warp tasks use
 // the per-lane copy plan when it covers the tile (up to kMaxP * 32 pieces of >= 4 bytes) and the copy loops when it does not.
 int dispatch(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-             void* out, int ld_out, DropoutCfg drop, cudaStream_t stream) {
+             void* out, int ld_out, const Dropout& drop, cudaStream_t stream) {
     const bool coop = T > 32;
     const int piece = bwd ? piece_bytes_bwd(dk, ld_qkv, ld_dctx, sec, ld_out) : piece_bytes(dk, ld_qkv, ld_out, sec);
     if (piece == 8 && T == fixed_T(coop) && dk == kFixedDk && heads == kFixedHeads) {  // d_k 20: the NTD 3 class
@@ -814,8 +797,7 @@ int dispatch(bool bwd, const void* qkv, int ld_qkv, int sec, const void* dctx, i
 }
 
 // The shape contract both directions share (include/newsrec_b200.h), checked before anything is launched.  Every pitch is a
-// multiple of 8: the context dropout picks the 16-bit lane of an element's hash from its column (gc & 3), which is the lane
-// (row * ld + col) & 3 of the library's hash only when the pitch is a multiple of 4.
+// multiple of 8, which the context dropout's mask needs (Dropout in nr_common.cuh: a pitch that is a multiple of 4).
 int check_core_shape(long long n_seq, int T, int heads, int dk, int sec, int ld_qkv) {
     NR_REQUIRE(n_seq >= 0, "mhsa: n_seq=%lld is negative", n_seq);
     NR_REQUIRE(heads >= 1, "mhsa: heads=%d, need at least one head", heads);
@@ -839,7 +821,7 @@ int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, 
     ProfScope ps("mhsa_core_fwd", static_cast<int>(n_seq), T, heads * dk, stream);
     if (mhsa_title_fwd_supported(T, dk, heads, sec, ld_qkv, ld_ctx))  // the news encoder's shape: whole titles per CTA, TMA in / out
         return mhsa_title_fwd(qkv, ld_qkv, sec, n_seq, heads, ctx, ld_ctx, drop, stream);
-    return dispatch(false, qkv, ld_qkv, sec, nullptr, 0, n_seq, T, heads, dk, ctx, ld_ctx, drop, stream);
+    return dispatch(false, qkv, ld_qkv, sec, nullptr, 0, n_seq, T, heads, dk, ctx, ld_ctx, Dropout::make(drop.p, drop.seed), stream);
 }
 
 int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
@@ -851,10 +833,9 @@ int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld
                ld_dqkv);
     if (n_seq == 0) return 0;
     ProfScope ps("mhsa_core_bwd", static_cast<int>(n_seq), T, heads * dk, stream);
-    const DropoutCfg nodrop{0.f, 0};
     if (mhsa_title_bwd_supported(T, dk, heads, sec, ld_qkv, ld_dctx, ld_dqkv))  // the news encoder's shape: whole titles per CTA, TMA in / out
         return mhsa_title_bwd(qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, heads, dqkv, ld_dqkv, stream);
-    return dispatch(true, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, nodrop, stream);
+    return dispatch(true, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, Dropout::make(0.f, 0), stream);
 }
 
 }  // namespace nr

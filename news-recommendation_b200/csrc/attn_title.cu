@@ -354,9 +354,8 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
 struct FwdParams {
     int n_seq, heads, ld_ctx;
     uint32_t sec2, pq, pc, pv, qkv_tile, in_stage, out_tile, out_stage, tx;
-    float sc, dscale;
-    uint32_t thresh;
-    uint64_t seed;
+    float sc;
+    Dropout drop;
 };
 
 template <bool HILO>
@@ -440,7 +439,6 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
     const uint32_t r15q = (lane & 15) * pq, r7q = (lane & 7) * pq;
     const uint32_t hi = (lane >> 4) * 16u, mid = ((lane >> 3) & 1) * 16u;
     const float sc = p.sc;
-    const bool drop = p.thresh != 0u;
 
     for (int it = 0; it < n_my; ++it) {
         const int s = it % kIn, o = it % kOut;
@@ -564,7 +562,7 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                 }
             }
         }
-        if (drop) {
+        if (p.drop.active()) {
             // dropout acts on the context (multihead_self.py:23 -> news_encoder.py:43): second pass over the head's 20 x 20 block in
             // 8-byte pieces, ONE counter hash per 4 aligned columns (hashing per fragment pair in the loop above costs 3x the
             // hashes and made the kernel issue bound)
@@ -578,23 +576,21 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                     const uint32_t a = ob + r * pc + 40u * h + 8u * c4;
                     uint32_t u0, u1;
                     asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(u0), "=r"(u1) : "r"(a));
-                    const uint64_t bits = dropout_bits4(p.seed, gbase + r * (static_cast<uint32_t>(p.ld_ctx) >> 2) + c4);
-                    const uint32_t blo = static_cast<uint32_t>(bits), bhi = static_cast<uint32_t>(bits >> 32);
-                    const float m0 = ((blo & 0xffffu) >= p.thresh) ? p.dscale : 0.f, m1 = ((blo >> 16) >= p.thresh) ? p.dscale : 0.f;
-                    const float m2 = ((bhi & 0xffffu) >= p.thresh) ? p.dscale : 0.f, m3 = ((bhi >> 16) >= p.thresh) ? p.dscale : 0.f;
+                    float m[4];
+                    p.drop.mask4_group(gbase + r * (static_cast<uint32_t>(p.ld_ctx) >> 2) + c4, m);
                     float2 x = unpack_bf16x2(u0), y = unpack_bf16x2(u1);
                     if (HILO) {
                         uint32_t w0, w1;
                         asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w0), "=r"(w1) : "r"(a + p.out_tile));
                         const float2 xl = unpack_bf16x2(w0), yl = unpack_bf16x2(w1);
-                        x.x = (x.x + xl.x) * m0, x.y = (x.y + xl.y) * m1, y.x = (y.x + yl.x) * m2, y.y = (y.y + yl.y) * m3;
+                        x.x = (x.x + xl.x) * m[0], x.y = (x.y + xl.y) * m[1], y.x = (y.x + yl.x) * m[2], y.y = (y.y + yl.y) * m[3];
                         const uint32_t h0 = pack_bf16x2(x.x, x.y), h1 = pack_bf16x2(y.x, y.y);
                         const float2 hx = unpack_bf16x2(h0), hy = unpack_bf16x2(h1);
                         asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(a), "r"(h0), "r"(h1) : "memory");
                         asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(a + p.out_tile), "r"(pack_bf16x2(x.x - hx.x, x.y - hx.y)),
                                      "r"(pack_bf16x2(y.x - hy.x, y.y - hy.y)) : "memory");
                     } else {
-                        x.x *= m0, x.y *= m1, y.x *= m2, y.y *= m3;
+                        x.x *= m[0], x.y *= m[1], y.x *= m[2], y.y *= m[3];
                         asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(a), "r"(pack_bf16x2(x.x, x.y)), "r"(pack_bf16x2(y.x, y.y)) : "memory");
                     }
                 }
@@ -699,9 +695,7 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
     p.out_stage = (hilo ? 2u : 1u) * p.out_tile;
     p.tx = kT * p.pq + (hilo ? kT * p.pv : 0u);
     p.sc = 1.4426950408889634f / sqrtf(static_cast<float>(kDk));
-    p.thresh = static_cast<uint32_t>(drop.p * 65536.0f + 0.5f);
-    p.dscale = drop.p > 0.f ? 1.f / (1.f - drop.p) : 1.f;
-    p.seed = drop.seed;
+    p.drop = Dropout::make(drop.p, drop.seed);
     // fragment loads of rows 20..23 of a tile run into whatever follows it (the low-plane tile, the next stage, the result
     // tiles): always inside the allocation, always initialised
     const int n_in = hilo ? kInHilo : kIn;

@@ -109,11 +109,6 @@ int rows_to_bf16(const Bf16Rows* jobs, int n_jobs, Bf16Op op, cudaStream_t strea
 // Embedding-row gather: one warp per token, 16-byte lanes.  The copy is bit exact (bf16 table rows).
 // Column D of every gathered row is set to 1.0 (bias-gradient trick), columns after it stay 0.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float drop_mult(uint64_t seed, uint32_t thresh, float scale, long long row, int ld, int col) {
-    const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(row) * ld + col) >> 2);
-    return (((bits >> (16 * (col & 3))) & 0xffffu) >= thresh) ? scale : 0.f;
-}
-
 // one thread = one 16-byte chunk COLUMN: a block covers kGatherThreads / chunks consecutive token rows per iteration
 // (consecutive threads copy consecutive chunks: coalesced), so the chunk index and the row slot are computed once and
 // the loop carries no division (the flat-index version spent most of its instructions on 64-bit div/mod);
@@ -121,15 +116,13 @@ __device__ __forceinline__ float drop_mult(uint64_t seed, uint32_t thresh, float
 constexpr int kGatherThreads = 320;
 __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long long* __restrict__ ids, long long n_tok, int T,
                                                                    const uint4* __restrict__ table, int V, int D, int ld,
-                                                                   uint4* __restrict__ X, int ld_x, int padded, float p,
-                                                                   uint64_t seed, int* bad_flag) {
+                                                                   uint4* __restrict__ X, int ld_x, int padded, Dropout drop,
+                                                                   int* bad_flag) {
     const int chunks = ld >> 3;  // 16-byte chunks per table row
     const int x_chunks = ld_x >> 3;
     const int rows_per_it = kGatherThreads / chunks;
     const int rl = threadIdx.x / chunks, c = threadIdx.x - rl * chunks;
     if (rl >= rows_per_it) return;
-    const uint32_t thresh = static_cast<uint32_t>(p * 65536.0f + 0.5f);
-    const float scale = p > 0.f ? 1.f / (1.f - p) : 1.f;
     const long long stride = static_cast<long long>(gridDim.x) * rows_per_it;
     long long tok = static_cast<long long>(blockIdx.x) * rows_per_it + rl;
     // software pipeline: the (id -> table row) loads of the NEXT row are in flight while this one is stored
@@ -153,18 +146,14 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long 
             xr = seg * (T + 2) + 1 + t;
         }
         uint32_t w[4] = {u.x, u.y, u.z, u.w};
-        if (p > 0.f) {
+        if (drop.active()) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const uint64_t bits = dropout_bits4(seed, static_cast<uint64_t>(xr) * (ld_x >> 2) + (col >> 2) + h);  // ld_x % 8 == 0
-                const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
-                float2 f0 = unpack_bf16x2(w[2 * h]), f1 = unpack_bf16x2(w[2 * h + 1]);
-                f0.x *= ((lo & 0xffffu) >= thresh) ? scale : 0.f;
-                f0.y *= ((lo >> 16) >= thresh) ? scale : 0.f;
-                f1.x *= ((hi & 0xffffu) >= thresh) ? scale : 0.f;
-                f1.y *= ((hi >> 16) >= thresh) ? scale : 0.f;
-                w[2 * h] = pack_bf16x2(f0.x, f0.y);
-                w[2 * h + 1] = pack_bf16x2(f1.x, f1.y);
+                float m[4];
+                drop.mask4_group(static_cast<uint64_t>(xr) * (ld_x >> 2) + (col >> 2) + h, m);  // ld_x % 8 == 0
+                const float2 f0 = unpack_bf16x2(w[2 * h]), f1 = unpack_bf16x2(w[2 * h + 1]);
+                w[2 * h] = pack_bf16x2(f0.x * m[0], f0.y * m[1]);
+                w[2 * h + 1] = pack_bf16x2(f1.x * m[2], f1.y * m[3]);
             }
         }
         if (D >= col && D < col + 8) {  // ones column, zeros behind it
@@ -187,7 +176,8 @@ int gather_rows(const long long* ids, long long n_tok, int T, const void* table,
     const int blocks = static_cast<int>(std::min<long long>((n_tok + rows_per_it - 1) / rows_per_it, 148 * 6));
     ProfScope ps("gather_rows", static_cast<int>(n_tok), D, ld_x, stream);
     gather_rows_kernel<<<blocks, kGatherThreads, 0, stream>>>(ids, n_tok, T, static_cast<const uint4*>(table), V, D, ld_table,
-                                                   static_cast<uint4*>(X), ld_x, padded, drop.p, drop.seed, bad_id_flag);
+                                                   static_cast<uint4*>(X), ld_x, padded, Dropout::make(drop.p, drop.seed),
+                                                   bad_id_flag);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

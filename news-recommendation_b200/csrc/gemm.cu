@@ -594,14 +594,6 @@ int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int
 // epilogue instantiations
 // ------------------------------------------------------------------------------------------------
 static RowMap to_rm(const RowMapCfg& c) { return RowMap{c.seg_in, c.in_off, c.seg_len, c.seg_out, c.out_off}; }
-static Dropout to_drop(const DropoutCfg& c) {
-    Dropout d;
-    d.p = c.p;
-    d.scale = c.p > 0.f ? 1.f / (1.f - c.p) : 1.f;
-    d.thresh = static_cast<uint32_t>(c.p * 65536.0f + 0.5f);
-    d.seed = c.seed;
-    return d;
-}
 
 // the chunk path of EpiStore emits the low plane by whole 32-column chunks of a weight slice: no chunk may straddle lo_col0
 static bool lo_plane_chunk_aligned(const GemmNTParams& p, int lo_col0) {
@@ -665,7 +657,7 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
     e.dtanh_ld = c.dtanh_ld;
     e.N = N;
     e.rm = to_rm(c.rm);
-    e.drop = to_drop(c.drop);
+    e.drop = Dropout::make(c.drop.p, c.drop.seed);
     e.ones_col = c.ones_col;
     e.ones_cols_zero_upto = c.ones_zero_upto;
 #ifdef NEWSREC_TRIAGE
@@ -766,7 +758,7 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
         NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, D, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                                   kEpiSmemBytes<EpiDPoolInFrag>, max_stride));
         EpiDPoolInFrag e{.w = c.w, .dout = c.dout, .ldo = c.ldo, .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx,
-                         .N = D, .drop = to_drop(c.drop), .M = M};
+                         .N = D, .drop = Dropout::make(c.drop.p, c.drop.seed), .M = M};
         NR_PROPAGATE(make_tmap_bf16_2d(&e.tm_out, c.dx, M, D, c.ld_dx, 32, 16, 64));
         g_launches += debug_simt_gemm() ? 2 : 1;
         ProfScope ps("gemm_pool_dinput", M, D, g.K, stream);
@@ -776,7 +768,7 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
                               max_stride));
     EpiDPoolIn e{.w = c.w, .dout = c.dout, .ldo = c.ldo,
                  .seg_len = seg_len, .dx = static_cast<__nv_bfloat16*>(c.dx), .ld = c.ld_dx, .N = D, .rm = to_rm(c.rm),
-                 .zero_pad_rows = c.zero_pad_rows, .drop = to_drop(c.drop), .relu_src = static_cast<const __nv_bfloat16*>(c.relu_src),
+                 .zero_pad_rows = c.zero_pad_rows, .drop = Dropout::make(c.drop.p, c.drop.seed), .relu_src = static_cast<const __nv_bfloat16*>(c.relu_src),
                  .relu_ld = c.relu_ld, .M = M};
     g_launches += debug_simt_gemm() ? 2 : 1;
     ProfScope ps("gemm_pool_dinput", M, D, g.K, stream);
@@ -842,7 +834,7 @@ int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, g.M, g.lda, g.W, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                               kEpiSmemBytes<EpiScatter>, 0));
     NR_PROPAGATE(apply_tap_origin(plan, g));
-    const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = to_drop(c.drop), .drop_ld = c.drop_ld};
+    const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = Dropout::make(c.drop.p, c.drop.seed), .drop_ld = c.drop_ld};
     const int num_tiles = plan.p.num_m_tiles;
     // [0, num_tiles) flags | ticket | list (count + tiles); stream-ordered, so the buffer lives exactly as long as the two launches
     int* buf = nullptr;

@@ -304,17 +304,10 @@ __device__ __forceinline__ void red_add_v4_f32(float* addr, float a, float b, fl
                  : "memory");
 }
 
-// Counter-based dropout bits: (seed, element-group index) -> four 16-bit lanes.
-// keep(e) <=> lane16 >= thresh16, thresh16 = round(p * 65536).  Regenerated identically in backward.
+// Counter-based dropout bits: (seed, element-group index) -> four 16-bit lanes (Dropout below draws its masks from them).
 // Two chained 32-bit multiply-xorshift rounds (about half the instructions of the splitmix64 finaliser this replaced,
 // which was >50 % of the instructions of the gather and of the dropout-carrying GEMM epilogues); the statistical tests
 // (keep rate, scaling, train/eval mean) are the acceptance criterion for the mask quality.
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {  // splitmix64 finaliser (kept for non-hot uses)
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
 __device__ __forceinline__ uint64_t dropout_bits4(uint64_t seed, uint64_t group) {
     const uint32_t g_lo = static_cast<uint32_t>(group), g_hi = static_cast<uint32_t>(group >> 32);
     uint32_t x = (g_lo ^ static_cast<uint32_t>(seed)) + g_hi * 0x85EBCA6Bu + static_cast<uint32_t>(seed >> 32) * 0x165667B1u;
@@ -328,6 +321,65 @@ __device__ __forceinline__ uint64_t dropout_bits4(uint64_t seed, uint64_t group)
     y ^= y >> 15;
     return (static_cast<uint64_t>(y) << 32) | x;
 }
+
+// The library's dropout mask.  Element (row, col) of a matrix with pitch ld (a multiple of 4) is in group (row * ld + col) >> 2
+// and is kept iff 16-bit lane col & 3 of dropout_bits4(seed, group) is >= thresh; a kept element is multiplied by scale.  The
+// forward and the backward of a composite draw the same mask from the same (p, seed).  These members are the only code that
+// tests a lane against thresh; the Python reference model of the kernels (the oracle) restates the rule.
+struct Dropout {
+    float p;          // 0 => off
+    float scale;      // 1/(1-p); 1 when off
+    uint32_t thresh;  // round(p * 65536)
+    uint64_t seed;
+
+    static Dropout make(float p, uint64_t seed) {
+        return Dropout{p, p > 0.f ? 1.f / (1.f - p) : 1.f, static_cast<uint32_t>(p * 65536.0f + 0.5f), seed};
+    }
+    __device__ __forceinline__ bool active() const { return p > 0.f; }
+    // multipliers of the aligned 4-column group at col4 of a row
+    __device__ __forceinline__ void mask4(long long row, int ld, int col4, float* m) const {
+        mask4_group((static_cast<uint64_t>(row) * ld + col4) >> 2, m);
+    }
+    // the same for a precomputed group index ((row * ld + col) >> 2; callers that walk a row keep row * ld / 4 in a register);
+    // 32-bit field tests: the 64-bit shifts / compares of the straightforward form were a quarter of the instructions of the
+    // dropout-carrying epilogues (ncu source page)
+    __device__ __forceinline__ void mask4_group(uint64_t group, float* m) const {
+        const uint64_t bits = dropout_bits4(seed, group);
+        const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
+        m[0] = ((lo & 0xffffu) >= thresh) ? scale : 0.f;
+        m[1] = ((lo >> 16) >= thresh) ? scale : 0.f;
+        m[2] = ((hi & 0xffffu) >= thresh) ? scale : 0.f;
+        m[3] = ((hi >> 16) >= thresh) ? scale : 0.f;
+    }
+    // multipliers of element col (.x) and, for an even col, of its pair col + 1 (.y) of a row.  The lane is picked from the two
+    // 32-bit halves by selects: indexing a float[4] at a run-time position would put the array in local memory.
+    __device__ __forceinline__ float2 mask2(long long row, int ld, int col) const {
+        const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(row) * ld + col) >> 2);
+        const uint32_t w = (col & 2) ? static_cast<uint32_t>(bits >> 32) : static_cast<uint32_t>(bits);
+        const uint32_t own = (col & 1) ? (w >> 16) : (w & 0xffffu);
+        return make_float2(own >= thresh ? scale : 0.f, (w >> 16) >= thresh ? scale : 0.f);
+    }
+    // the same masks applied to one 32-column chunk of a wgmma fragment: y[4jj + 2e + i] is row[e], column col + 8jj +
+    // 2 (lane % 4) + i.  The mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of
+    // the same group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
+    __device__ __forceinline__ void apply_frag(float* y, const long long* row, int ld, int col) const {
+        const int lane = threadIdx.x & 31, b = lane & 1;
+        const long long my_row = b ? row[1] : row[0];
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int col4 = col + 8 * jj + 4 * ((lane >> 1) & 1);
+            const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
+            const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
+            const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
+            const uint32_t wd[2] = {b ? other : own, b ? own : other};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= thresh) ? scale : 0.f;
+                y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= thresh) ? scale : 0.f;
+            }
+        }
+    }
+};
 
 #endif  // __CUDACC__
 

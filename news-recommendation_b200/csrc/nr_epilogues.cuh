@@ -40,48 +40,6 @@ __device__ __forceinline__ void zero_row_bf16(__nv_bfloat16* row, int ld) {  // 
     for (int i = 0; i < ld; i += 8) *reinterpret_cast<uint4*>(row + i) = make_uint4(0u, 0u, 0u, 0u);
 }
 
-struct Dropout {
-    float p;          // 0 => off
-    float scale;      // 1/(1-p)
-    uint32_t thresh;  // keep iff 16-bit lane >= thresh
-    uint64_t seed;
-    // multiplier for element (row, col) of a matrix with pitch ld; cols are visited in aligned groups of 4
-    __device__ __forceinline__ void mask4(long long row, int ld, int col4, float* m) const {
-        mask4_group((static_cast<uint64_t>(row) * ld + col4) >> 2, m);
-    }
-    // the same for a precomputed group index ((row * ld + col) >> 2; callers that walk a row keep row * ld / 4 in a register);
-    // 32-bit field tests: the 64-bit shifts / compares of the straightforward form were a quarter of the instructions of the
-    // dropout-carrying epilogues (ncu source page)
-    __device__ __forceinline__ void mask4_group(uint64_t group, float* m) const {
-        const uint64_t bits = dropout_bits4(seed, group);
-        const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
-        m[0] = ((lo & 0xffffu) >= thresh) ? scale : 0.f;
-        m[1] = ((lo >> 16) >= thresh) ? scale : 0.f;
-        m[2] = ((hi & 0xffffu) >= thresh) ? scale : 0.f;
-        m[3] = ((hi >> 16) >= thresh) ? scale : 0.f;
-    }
-    // the same masks applied to one 32-column chunk of a wgmma fragment: y[4jj + 2e + i] is row[e], column col + 8jj +
-    // 2 (lane % 4) + i.  The mask of (row, aligned 4-column group) is one hash; lanes 2k and 2k+1 hold columns 0-1 and 2-3 of
-    // the same group in both rows: lane bit b hashes row e = b and passes the partner the 32-bit half it needs
-    __device__ __forceinline__ void apply_frag(float* y, const long long* row, int ld, int col) const {
-        const int lane = threadIdx.x & 31, b = lane & 1;
-        const long long my_row = b ? row[1] : row[0];
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int col4 = col + 8 * jj + 4 * ((lane >> 1) & 1);
-            const uint64_t bits = dropout_bits4(seed, (static_cast<uint64_t>(my_row) * ld + col4) >> 2);
-            const uint32_t lo = static_cast<uint32_t>(bits), hi = static_cast<uint32_t>(bits >> 32);
-            const uint32_t own = b ? hi : lo, other = __shfl_xor_sync(0xffffffffu, b ? lo : hi, 1);
-            const uint32_t wd[2] = {b ? other : own, b ? own : other};
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                y[4 * jj + 2 * e] *= ((wd[e] & 0xffffu) >= thresh) ? scale : 0.f;
-                y[4 * jj + 2 * e + 1] *= ((wd[e] >> 16) >= thresh) ? scale : 0.f;
-            }
-        }
-    }
-};
-
 // SWIZZLE_64B layout of a tile with 64-byte rows (32 bf16): byte offset of 16-byte piece q of row r.  Eight consecutive
 // rows at the same q (the rows of one stmatrix matrix, or a row-per-lane 16-byte access) land in eight different bank groups.
 __device__ __forceinline__ int sw64_offset(int r, int q) { return r * 64 + ((q ^ (r >> 1)) & 3) * 16; }
@@ -351,7 +309,7 @@ struct EpiStore {
                             y[4 * jj + 2 * e + 1] *= 1.f - t.y * t.y;
                         }
                 }
-                if (drop.p > 0.f) drop.apply_frag(y, orow, ld, f.col0 + lc0);
+                if (drop.active()) drop.apply_frag(y, orow, ld, f.col0 + lc0);
                 if (out_bf16) {
                     const int col = f.col0 + lc0;
                     uint32_t w[8];
@@ -680,7 +638,7 @@ struct EpiDPoolIn {
                                 x[q * 8 + 2 * j + 1] = f.y > 0.f ? x[q * 8 + 2 * j + 1] * drop.scale : 0.f;
                             }
                         }
-                    } else if (drop.p > 0.f) {
+                    } else if (drop.active()) {
                         const uint64_t g0 = (static_cast<uint64_t>(c.grow) * ld + col) >> 2;
 #pragma unroll
                         for (int j = 0; j < 32; j += 4) {
@@ -736,7 +694,7 @@ struct EpiDPoolIn {
                             if (!(f.y > 0.f)) y[2 * j + 1] = 0.f;
                         }
                     }
-                    if (drop.p > 0.f) {
+                    if (drop.active()) {
                         float m[8];
                         drop.mask4(c.grow, relu_src != nullptr ? relu_ld : ld, col, m);
                         drop.mask4(c.grow, relu_src != nullptr ? relu_ld : ld, col + 4, m + 4);
@@ -827,7 +785,7 @@ struct EpiDPoolInFrag {
                         y[4 * jj + 2 * e + 1] = fmaf(wr[e], d.y, acc[16 * q + 4 * jj + 2 * e + 1]);
                     }
                 }
-                if (drop.p > 0.f) drop.apply_frag(y, grow, ld, f.col0 + lc0);
+                if (drop.active()) drop.apply_frag(y, grow, ld, f.col0 + lc0);
                 uint32_t wp[8];
 #pragma unroll
                 for (int k = 0; k < 8; ++k) wp[k] = pack_bf16x2(y[2 * k], y[2 * k + 1]);
@@ -873,7 +831,7 @@ struct EpiScatter {
                     if (lc >= c.ncols) break;
                     const int col = c.col0 + lc;
                     float y[4] = {x[g * 4], x[g * 4 + 1], x[g * 4 + 2], x[g * 4 + 3]};
-                    if (drop.p > 0.f) {
+                    if (drop.active()) {
                         float m[4];
                         drop.mask4(c.grow, drop_ld, col, m);
 #pragma unroll

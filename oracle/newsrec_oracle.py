@@ -120,8 +120,8 @@ WEIGHTS_BF16 = Contract(True, False, False)   # bf16 operands (weights, embeddin
 
 
 # --------------------------------------------------------------------------- #
-# dropout: NumPy restatement of the kernels' counter hash (csrc/nr_common.cuh dropout_bits4,
-# nr_epilogues.cuh Dropout::mask4).  The reference draws its masks from torch's global RNG
+# dropout: NumPy restatement of the kernels' counter hash and mask (csrc/nr_common.cuh dropout_bits4
+# and Dropout).  The reference draws its masks from torch's global RNG
 # (news_encoder.py:38,43), which no kernel can reproduce; train-mode parity is therefore checked by
 # giving the ORACLE the kernel's masks: element (row, col) of a matrix with pitch ld belongs to group
 # (row*ld + col) >> 2 and is kept iff 16-bit lane (col & 3) of hash(seed, group) >= round(p * 65536).
