@@ -154,6 +154,27 @@ typedef struct {
 int nr_feed_gather(const nr_feed_field* fields, int n_fields, const int* behaviors, int H, int C, const int* records,
                    const long long* rows, int B, long long* user_out, long long* length_out, long long* clicked_out, void* stream);
 
+/* ---- negative sampling for the device feed (DeviceFeed(..., resample_negatives=True)): ONE launch redraws the candidate
+   columns of the behaviour table from MIND's raw impressions, for one (seed, epoch).  Every pointer is device memory.
+     cand_rows   int32 [n_cand], labels uint8 [n_cand]: impression i holds candidates [imp_offsets[i], imp_offsets[i+1]); label 1
+                 marks a positive, 0 a negative, any other value neither (the reference's endswith('1') / endswith('0'));
+     imp_offsets int64 [n_imp + 1];
+     row_offsets int64 [n_imp + 1]: impression i owns behaviour rows [row_offsets[i], row_offsets[i+1]), R_i = min(P, floor(N / K))
+                 of them for its P positives and N negatives (the reference's balancing count, the same for every draw);
+     behaviors   int32 [*][H + 1 + K].
+   The draw sorts impression i's negatives by (h_j, j) ascending, j being a negative's ordinal among them (file order) and h_j the
+   high 32 bits of
+       x = 0;  for v in (seed, epoch, i, j):  x = f((x ^ v) + 0x9E3779B97F4A7C15)          (all uint64, mod 2^64)
+       f(z): z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  z ^ (z >> 31)
+   (splitmix64's finaliser; epoch as its two's complement).  Owned row p gets behaviors[r][H] = the p-th positive in file order and
+   behaviors[r][H + 1 + k] = the negative of sorted place p*K + k, k < K, so no two rows of an impression share a negative.
+   Exactly columns H .. H + K of the owned rows are written, and never more than R_i rows of impression i; nothing else (history
+   columns, other rows) is touched.  Integer only: the same bits on every run and device.  Any number of candidates per
+   impression (fewer than 2^32 negatives); the work is O(N^2 / 32) per lane.  K >= 1, n_imp >= 0 (0 launches nothing), H >= 0. */
+int nr_sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp,
+                        const long long* row_offsets, int K, unsigned long long seed, long long epoch, int* behaviors, int H,
+                        void* stream);
+
 /* Batched form of the evaluator's scoring loop (src/evaluate.py:245-265 calls get_prediction once per impression and
  * synchronises on .tolist() each time): the news vectors live in ONE device matrix news[n_news][D]; the candidates of
  * impression s are cand[seg_offsets[s] .. seg_offsets[s+1]) (indices into news), user[s] its user vector;

@@ -227,6 +227,13 @@ int nr_feed_gather(const nr_feed_field* fields, int n_fields, const int* behavio
     return feed_gather(f, n_fields, behaviors, H, C, {.records = records, .user = user_out, .length = length_out, .clicked = clicked_out},
                        rows, B, as_stream(stream));
 }
+int nr_sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp,
+                        const long long* row_offsets, int K, unsigned long long seed, long long epoch, int* behaviors, int H, void* stream) {
+    NR_REQUIRE(cand_rows && labels && imp_offsets && row_offsets && behaviors, "nr_sample_negatives: null operand");
+    NR_REQUIRE(K >= 1 && n_imp >= 0 && H >= 0, "nr_sample_negatives: bad arguments K=%d n_imp=%lld H=%d", K, n_imp, H);
+    prof_context("feed");
+    return sample_negatives(cand_rows, labels, imp_offsets, n_imp, row_offsets, K, seed, epoch, behaviors, H, as_stream(stream));
+}
 
 // ---- NRMS encoders ---------------------------------------------------------------------------------
 // Q | K | V sections of the projected rows start at columns 0, sec, 2*sec with sec = round_up(d, 8): every section (and so

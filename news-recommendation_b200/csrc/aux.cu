@@ -1197,4 +1197,98 @@ int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Negative sampling (include/newsrec_b200.h, nr_sample_negatives): one warp per impression.  Pass 1 counts the positives P and
+// negatives N with ballots; the impression's R = min(P, N / K) rows are its owned rows.  Pass 2 walks the candidates again:
+// the p-th positive goes to row p, and a negative of ordinal j with sort key (h_j, j) -- one 64-bit integer, h_j in the high
+// half -- finds its rank among the impression's N keys by counting the smaller ones; rank r < R*K lands in row r / K,
+// candidate column 1 + r % K.  The keys are recomputed from j alone and staged in the warp's slice of shared memory: once per
+// impression when N <= kNegTile (MIND's impressions), else tile by tile for every 32 candidates.  The work is O(N^2 / 32) per
+// lane and integer only: the output is the same on every run and device.
+// ------------------------------------------------------------------------------------------------
+constexpr int kNegWarps = 8, kNegTile = 256;
+constexpr unsigned long long kNegGolden = 0x9E3779B97F4A7C15ull;
+// one link of the chained hash of (seed, epoch, impression, ordinal): x' = splitmix64's finaliser of (x ^ v) + golden ratio
+__host__ __device__ inline unsigned long long neg_hash_step(unsigned long long x, unsigned long long v) {
+    unsigned long long z = (x ^ v) + kNegGolden;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+__device__ inline unsigned long long neg_sort_key(unsigned long long imp_state, unsigned j) {
+    return (neg_hash_step(imp_state, j) & 0xFFFFFFFF00000000ull) | j;
+}
+__global__ void __launch_bounds__(kNegWarps * 32) sample_negatives_kernel(const int* __restrict__ cand_rows, const unsigned char* __restrict__ labels,
+                                                                          const long long* __restrict__ imp_offsets, long long n_imp,
+                                                                          const long long* __restrict__ row_offsets, int K,
+                                                                          unsigned long long epoch_state, int* __restrict__ beh, int H) {
+    __shared__ unsigned long long keys_all[kNegWarps][kNegTile];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long* keys = keys_all[warp];
+    const unsigned below = (1u << lane) - 1;
+    const long long W = H + 1ll + K;
+    for (long long i = blockIdx.x * static_cast<long long>(kNegWarps) + warp; i < n_imp; i += static_cast<long long>(gridDim.x) * kNegWarps) {
+        const long long beg = imp_offsets[i], end = imp_offsets[i + 1];
+        long long P = 0, N = 0;
+        for (long long c0 = beg; c0 < end; c0 += 32) {
+            const int l = c0 + lane < end ? labels[c0 + lane] : 255;
+            P += __popc(__ballot_sync(~0u, l == 1));
+            N += __popc(__ballot_sync(~0u, l == 0));
+        }
+        const long long row0 = row_offsets[i];
+        const long long rows = std::min(std::min(P, N / K), row_offsets[i + 1] - row0);  // never past the owned rows
+        if (rows <= 0) continue;
+        const unsigned long long imp_state = neg_hash_step(epoch_state, static_cast<unsigned long long>(i));
+        const long long taken = rows * K;
+        const bool one_tile = N <= kNegTile;
+        __syncwarp();  // the previous impression's compares are done with keys[]
+        if (one_tile) {
+            for (int t = lane; t < N; t += 32) keys[t] = neg_sort_key(imp_state, static_cast<unsigned>(t));
+            __syncwarp();
+        }
+        long long p_seen = 0, n_seen = 0;
+        for (long long c0 = beg; c0 < end; c0 += 32) {
+            const long long c = c0 + lane;
+            const int l = c < end ? labels[c] : 255;
+            const unsigned pos = __ballot_sync(~0u, l == 1), neg = __ballot_sync(~0u, l == 0);
+            if (l == 1) {
+                const long long p = p_seen + __popc(pos & below);
+                if (p < rows) beh[(row0 + p) * W + H] = cand_rows[c];
+            }
+            if (neg) {
+                const unsigned long long mine = neg_sort_key(imp_state, static_cast<unsigned>(n_seen + __popc(neg & below)));
+                long long rank = 0;
+                for (long long t0 = 0; t0 < N; t0 += kNegTile) {
+                    if (!one_tile) {
+                        __syncwarp();
+                        for (int t = lane; t < kNegTile && t0 + t < N; t += 32)
+                            keys[t] = neg_sort_key(imp_state, static_cast<unsigned>(t0 + t));
+                        __syncwarp();
+                    }
+                    const int n_t = static_cast<int>(std::min<long long>(kNegTile, N - t0));
+                    int smaller = 0;
+#pragma unroll 4
+                    for (int t = 0; t < n_t; ++t) smaller += keys[t] < mine;
+                    rank += smaller;
+                }
+                if (l == 0 && rank < taken) beh[(row0 + rank / K) * W + H + 1 + rank % K] = cand_rows[c];
+            }
+            p_seen += __popc(pos);
+            n_seen += __popc(neg);
+        }
+    }
+}
+int sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp, const long long* row_offsets,
+                     int K, unsigned long long seed, long long epoch, int* behaviors, int H, cudaStream_t stream) {
+    if (n_imp == 0) return 0;
+    const unsigned long long epoch_state = neg_hash_step(neg_hash_step(0, seed), static_cast<unsigned long long>(epoch));
+    ProfScope ps("sample_negatives", static_cast<int>(std::min<long long>(n_imp, 1 << 30)), K, H, stream);
+    const long long blocks = std::min<long long>((n_imp + kNegWarps - 1) / kNegWarps, num_sms() * 32ll);
+    sample_negatives_kernel<<<static_cast<unsigned>(blocks), kNegWarps * 32, 0, stream>>>(cand_rows, labels, imp_offsets, n_imp, row_offsets, K,
+                                                                                          epoch_state, behaviors, H);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace nr

@@ -211,6 +211,10 @@ struct FeedRecords {
 };
 int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int H, int C, FeedRecords rec, const long long* rows, int B,
                 cudaStream_t stream);
+// one launch: redraw the candidate columns [H, H + 1 + K] of the device feed's behaviour rows from each impression's
+// candidates (include/newsrec_b200.h, nr_sample_negatives)
+int sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp, const long long* row_offsets,
+                     int K, unsigned long long seed, long long epoch, int* behaviors, int H, cudaStream_t stream);
 int num_sms();
 extern int g_launches;  // kernels launched by this library (nr_launch_count)
 

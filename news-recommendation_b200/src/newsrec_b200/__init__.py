@@ -156,6 +156,7 @@ SIGNATURES = {
     "nr_slots_device_readable": (_i, [_vp, _i]),
     "nr_pack_slots": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "nr_feed_gather": (_i, [C.POINTER(FeedField), _i, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "nr_sample_negatives": (_i, [_vp, _vp, _vp, _ll, _vp, _i, _ull, _ll, _vp, _i, _vp]),
     "nr_segment_dot": (_i, [_vp, _ll, _i, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp]),
     "nr_impression_metrics": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),
     "nr_impression_ranks": (_i, [_vp, _vp, _ll, _vp, _vp, _vp]),

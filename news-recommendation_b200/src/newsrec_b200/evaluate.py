@@ -99,18 +99,24 @@ def build_tables(directory, news_index, H, max_count=sys.maxsize, user2int_path=
     n_imp = len(beh) if max_count < 1 else min(len(beh), max_count - 1)
     imp = beh.iloc[:n_imp]
     seg_user = np.asarray([hist_row[hs] for hs in imp["clicked_news"].tolist()], np.int64)
+    cand, labels, offsets = impression_candidates(imp["impressions"], news_index)
+    labels = np.where((labels >= 0) & (labels <= 1), labels, 2).astype(np.uint8)  # anything else is flagged on the device
+    return EvalTables(user=user, history=history, history_length=length, seg_user=seg_user,
+                      cand=cand, labels=labels, seg_offsets=offsets)
+
+
+def impression_candidates(impressions, news_index):
+    """The impressions column of read_behaviors ("N1-1 N2-0 ...") as CSR: (cand, labels, offsets) -- int64 news rows and
+    labels as written, impressions back to back, and the (n_imp + 1,) int64 offsets."""
     cand, labels, counts = [], [], []
-    for impressions in imp["impressions"].tolist():
-        items = impressions.split()
+    for items in impressions.tolist():
+        items = items.split()
         cand.extend(_rows(news_index, [x.split("-")[0] for x in items]))
         labels.extend(int(x.split("-")[1]) for x in items)
         counts.append(len(items))
-    labels = np.asarray(labels, np.int64)
-    labels = np.where((labels >= 0) & (labels <= 1), labels, 2).astype(np.uint8)  # anything else is flagged on the device
-    offsets = np.zeros(n_imp + 1, np.int64)
+    offsets = np.zeros(len(counts) + 1, np.int64)
     offsets[1:] = np.cumsum(counts)
-    return EvalTables(user=user, history=history, history_length=length, seg_user=seg_user,
-                      cand=np.asarray(cand, np.int64), labels=labels, seg_offsets=offsets)
+    return np.asarray(cand, np.int64), np.asarray(labels, np.int64), offsets
 
 
 def new_flag(device):

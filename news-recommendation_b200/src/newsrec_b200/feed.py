@@ -19,11 +19,20 @@ the blocks to the encoders without another launch.
 Row order: a ``DistributedSampler`` over the rows with a seed and an epoch counter (``newsrec_b200.launch --device-feed``
 advances the epoch each time the trainer re-creates its loader), with one replica at world size 1.  This is another random
 stream than the reference's ``RandomSampler``, with the same distribution.
+
+Negatives redrawn every epoch: ``DeviceFeed(behaviors_path, news_path, config, resample_negatives=True, seed=s)`` reads
+MIND's raw behaviors.tsv from behaviors_path's directory (users through user2int.tsv) instead of behaviors_parsed.tsv.  Its
+rows are the reference's balancing (parse_behaviors): impression i owns min(P, N // K) rows, row p holding the p-th positive
+and K negatives no other row of the impression holds.  The history columns and the records [user, clicked_news_length,
+1, 0, ..., 0] are written once; ``loader(..., epoch=e)`` redraws the candidate columns for (s, e) with ONE launch
+(``nr_sample_negatives``) on the stream the gathers use, before its first batch.  The table holds epoch 0's draw from
+construction on; ``behaviors`` and ``feed[idx]`` read the current draw back from the device.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+from dataclasses import dataclass
 
 import numpy as np
 import torch
@@ -66,9 +75,11 @@ class FeedSlots(list):
 
 class DeviceFeed(Dataset):
     """The reference BaseDataset's constructor signature and length; the tables are parsed once (host arrays
-    `news_tables`, `behaviors`, `records`) and copied to `device` (default: the current CUDA device, if any)."""
+    `news_tables`, `behaviors`, `records`) and copied to `device` (default: the current CUDA device, if any).
+    resample_negatives: rows from the raw behaviors.tsv beside behaviors_path, negatives drawn on the device per (seed,
+    epoch) (module docstring); user2int_path defaults to the user2int.tsv beside it.  Such a feed needs a CUDA device."""
 
-    def __init__(self, behaviors_path, news_path, config=None, device=None):
+    def __init__(self, behaviors_path, news_path, config=None, device=None, *, resample_negatives=False, user2int_path=None, seed=0):
         import pandas as pd
         from .evaluate import read_news
         super().__init__()
@@ -101,9 +112,40 @@ class DeviceFeed(Dataset):
                 raise ValueError(f"{news_path}: column {a!r} has {col.shape[1]} entries per news, the config says {L}")
             self.news_tables[a] = _int32(np.concatenate([col, np.zeros((1, L), np.int64)]), a)
 
-        beh = pd.read_table(behaviors_path)
-        R = len(beh)
-        C = None
+        self.resample_negatives, self.seed, self.epoch = bool(resample_negatives), int(seed), 0
+        self._stale = False  # the device table holds a draw the host copy does not
+        if self.resample_negatives:
+            directory = os.path.dirname(behaviors_path)
+            self.K = int(config.negative_sampling_ratio)
+            self.impressions = resample_tables(directory, dict(index, PADDED_NEWS=pad), H, self.K,
+                                               user2int_path or os.path.join(directory, "user2int.tsv"))
+            self.C = 1 + self.K
+            self._behaviors, self.records = self.impressions.behaviors, self.impressions.records
+        else:
+            self._parse_balanced(pd.read_table(behaviors_path), behaviors_path, index, pad)
+
+        if device is None and torch.cuda.is_available():
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.device = torch.device(device) if device is not None else None
+        if self.device is not None and self.device.type == "cuda" and self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self._dev = None
+        if self.device is not None and self.device.type == "cuda":
+            to = lambda a: torch.from_numpy(a).to(self.device)
+            self._dev = {"news": {a: to(t) for a, t in self.news_tables.items()}, "behaviors": to(self._behaviors),
+                         "records": to(self.records)}
+        if self.resample_negatives:
+            if self._dev is None:
+                from . import NewsrecError
+                raise NewsrecError("DeviceFeed(resample_negatives=True) needs a CUDA device: the negatives are drawn there only")
+            t = self.impressions
+            self._dev.update(cand_rows=to(t.cand_rows), labels=to(t.labels), imp_offsets=to(t.imp_offsets), row_offsets=to(t.row_offsets))
+            self.epoch = None
+            self.draw(0)
+
+    def _parse_balanced(self, beh, behaviors_path, index, pad):
+        """behaviors_parsed.tsv rows (user, clicked_news, candidate_news, clicked) -> self.behaviors, self.records, self.C."""
+        H, R, C = self.H, len(beh), None
         behaviors, records = [], []
         for r, (user, hist, cand, clicked) in enumerate(zip(beh["user"].tolist(), beh["clicked_news"].tolist(),
                                                             beh["candidate_news"].tolist(), beh["clicked"].tolist())):
@@ -120,22 +162,34 @@ class DeviceFeed(Dataset):
         if C is None or C < 1:
             raise ValueError(f"{behaviors_path}: no behaviour rows with candidates")
         self.C = C
-        self.behaviors = _int32(np.asarray(behaviors, np.int64).reshape(R, H + C), "behaviour table")
+        self._behaviors = _int32(np.asarray(behaviors, np.int64).reshape(R, H + C), "behaviour table")
         self.records = _int32(np.asarray(records, np.int64).reshape(R, 2 + C), "user / clicked columns")
 
-        if device is None and torch.cuda.is_available():
-            device = torch.device("cuda", torch.cuda.current_device())
-        self.device = torch.device(device) if device is not None else None
-        if self.device is not None and self.device.type == "cuda" and self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
-        self._dev = None
-        if self.device is not None and self.device.type == "cuda":
-            to = lambda a: torch.from_numpy(a).to(self.device)
-            self._dev = {"news": {a: to(t) for a, t in self.news_tables.items()}, "behaviors": to(self.behaviors),
-                         "records": to(self.records)}
+    @property
+    def behaviors(self):
+        """The behaviour table (R, H + C) int32 on the host; a resampling feed's candidate columns hold the current draw."""
+        if self._stale:
+            self._behaviors = self._dev["behaviors"].cpu().numpy()
+            self._stale = False
+        return self._behaviors
+
+    def draw(self, epoch):
+        """Redraw a resampling feed's candidate columns for (self.seed, epoch): one nr_sample_negatives launch on the feed
+        device's current stream, none when the table already holds that epoch."""
+        if epoch == self.epoch:
+            return
+        from . import check, load_library
+        d, t = self._dev, self.impressions
+        ptr = lambda x: C.c_void_p(x.data_ptr())
+        with torch.cuda.device(self.device):
+            check(load_library().nr_sample_negatives(ptr(d["cand_rows"]), ptr(d["labels"]), ptr(d["imp_offsets"]), len(t.imp_offsets) - 1,
+                                                     ptr(d["row_offsets"]), self.K, self.seed & 0xFFFFFFFFFFFFFFFF, int(epoch),
+                                                     ptr(d["behaviors"]), self.H, C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)),
+                  "nr_sample_negatives")
+        self.epoch, self._stale = epoch, True
 
     def __len__(self):
-        return len(self.behaviors)
+        return len(self._behaviors)
 
     def __getitem__(self, idx):
         """Row idx in the reference dataset's item format, from the host tables (CPU tensors)."""
@@ -157,7 +211,54 @@ class DeviceFeed(Dataset):
         if self._dev is None:
             from . import NewsrecError
             raise NewsrecError("DeviceFeed.loader needs the tables on a CUDA device: the feed has no host path")
+        if self.resample_negatives:
+            self.draw(epoch)
         return FeedLoader(self, batch_size, shuffle, drop_last, rank, world, seed, epoch)
+
+
+@dataclass
+class ImpressionTables:
+    """Host tables of a resampling feed (resample_tables); R = row_offsets[-1] rows."""
+    behaviors: np.ndarray    # (R, H + 1 + K) int32: the history columns; the candidate columns are the draw's (zero here)
+    records: np.ndarray      # (R, 3 + K) int32: user, clicked_news_length, then the labels 1, 0, ..., 0
+    cand_rows: np.ndarray    # (n_cand,) int32 news rows, impressions back to back
+    labels: np.ndarray       # (n_cand,) uint8, 1 positive / 0 negative
+    imp_offsets: np.ndarray  # (n_imp + 1,) int64
+    row_offsets: np.ndarray  # (n_imp + 1,) int64: impression i owns rows [row_offsets[i], row_offsets[i+1]), min(P, N // K) of them
+
+
+def resample_tables(directory, news_index, H, K, user2int_path):
+    """MIND's raw behaviors.tsv in `directory` as the tables of a resampling feed (no CUDA needed).  news_index maps news
+    ids (and "PADDED_NEWS") to news rows; histories are the first H browsed news, left-padded with the padding news; users
+    go through user2int.tsv.  Raises KeyError for an unknown news id, ValueError for a label other than 0 / 1 or a user
+    user2int.tsv does not list."""
+    import pandas as pd
+    from .evaluate import impression_candidates, read_behaviors, user_tables
+    beh = read_behaviors(directory)
+    _, history, length, hist_row = user_tables(beh, news_index, H, user2int_path)
+    user2int = dict(pd.read_table(user2int_path).values.tolist())
+    users = beh["user"].tolist()
+    unknown = sorted({u for u in users if u not in user2int})
+    if unknown:
+        raise ValueError(f"{directory}/behaviors.tsv: users not in {user2int_path}: {unknown[:5]}")
+    hist = np.asarray([hist_row[h] for h in beh["clicked_news"].tolist()], np.int64)
+    cand, labels, imp_offsets = impression_candidates(beh["impressions"], news_index)
+    if ((labels != 0) & (labels != 1)).any():
+        raise ValueError(f"{directory}/behaviors.tsv: a label other than 0 or 1 ({sorted(set(labels.tolist()) - {0, 1})[:5]})")
+    counts = np.diff(imp_offsets)
+    P = np.bincount(np.repeat(np.arange(len(counts)), counts), weights=labels, minlength=len(counts)).astype(np.int64)
+    rows = np.minimum(P, (counts - P) // K)
+    row_offsets = np.zeros(len(counts) + 1, np.int64)
+    row_offsets[1:] = np.cumsum(rows)
+    of_row = hist[np.repeat(np.arange(len(counts)), rows)]
+    user = np.asarray([user2int[u] for u in users], np.int64)[np.repeat(np.arange(len(counts)), rows)]
+    behaviors = np.zeros((len(of_row), H + 1 + K), np.int64)
+    behaviors[:, :H] = history[of_row]
+    records = np.zeros((len(of_row), 3 + K), np.int64)
+    records[:, 0], records[:, 1], records[:, 2] = user, length[of_row], 1
+    return ImpressionTables(behaviors=_int32(behaviors, "behaviour table"), records=_int32(records, "user column"),
+                            cand_rows=_int32(cand, "news rows"), labels=labels.astype(np.uint8), imp_offsets=imp_offsets,
+                            row_offsets=row_offsets)
 
 
 def epoch_rows(n, batch_size, shuffle=False, drop_last=False, rank=0, world=1, seed=0, epoch=0):

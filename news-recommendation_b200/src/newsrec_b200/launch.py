@@ -20,12 +20,14 @@ editing it:
   `newsrec_b200.evaluate.evaluate` (same signature; scoring and metrics on the device);
 * `--device-feed` replaces the trainer's `BaseDataset` with `newsrec_b200.feed.DeviceFeed` (tables parsed once and held on
   the device, one gather launch per batch; SURVEY.md row N3); the DataLoader factory returns the feed's loader for it,
-  over the same sharding, seed and epoch counter;
+  over the same sharding, seed and epoch counter; `--resample-negatives` makes it a feed over the raw behaviors.tsv
+  whose negatives are redrawn on the device every epoch from `--seed` and that epoch counter (the same on every rank);
 * compatibility shims the survey found necessary for the reference on current NumPy / pandas / torch.
 """
 from __future__ import annotations
 
 import argparse
+import functools
 import os
 import sys
 
@@ -144,16 +146,17 @@ def apply_compat_shims():
         torch.load = load
 
 
-def patch_trainer(train_module, rank, world, seed=0, device_evaluate=False, device_feed=False):
+def patch_trainer(train_module, rank, world, seed=0, device_evaluate=False, device_feed=False, resample_negatives=False):
     """Install the data-parallel pieces into an imported (reference) `train` module's namespace.  device_evaluate: the
     trainer's `evaluate` becomes newsrec_b200.evaluate.evaluate (its docstring lists where its metrics can differ from a
     given reference environment: ties across labels, one-class impressions).  device_feed: the trainer's `BaseDataset`
-    becomes newsrec_b200.feed.DeviceFeed and its DataLoader returns the feed's loader for it."""
+    becomes newsrec_b200.feed.DeviceFeed and its DataLoader returns the feed's loader for it.  resample_negatives (with
+    device_feed): that feed reads data/train/behaviors.tsv and redraws its negatives per (seed, epoch)."""
     import torch
     train_module.DataLoader = make_sharded_dataloader(train_module.DataLoader, rank, world, seed)
     if device_feed:
         from newsrec_b200.feed import DeviceFeed
-        train_module.BaseDataset = DeviceFeed
+        train_module.BaseDataset = functools.partial(DeviceFeed, resample_negatives=True, seed=seed) if resample_negatives else DeviceFeed
         train_module.DataLoader = make_feed_dataloader(train_module.DataLoader, rank, world, seed)
     if world > 1 or os.environ.get("NEWSREC_FLAT_GRADS", "1") == "1":
         # the trainer reaches Adam through the global `torch.optim` module (train.py:127)
@@ -200,10 +203,15 @@ def main(argv=None):
     ap.add_argument("--device-feed", action="store_true",
                     help="train from newsrec_b200.feed.DeviceFeed: news and behaviour tables parsed once and kept on the device, "
                          "every batch gathered there by one kernel launch instead of the reference's BaseDataset / DataLoader")
+    ap.add_argument("--resample-negatives", action="store_true",
+                    help="with --device-feed: train on MIND's raw behaviors.tsv and redraw each impression's negatives on the device "
+                         "every epoch (seeded by --seed) instead of the fixed draw in behaviors_parsed.tsv")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
                     help="override a knob of the selected <MODEL_NAME>Config before the trainer is imported (repeatable), "
                          "e.g. --set batch_size=512 --set num_workers=8")
     args = ap.parse_args(argv)
+    if args.resample_negatives and not args.device_feed:
+        ap.error("--resample-negatives needs --device-feed")
 
     rank, world, local = _env_int("RANK", 0), _env_int("WORLD_SIZE", 1), _env_int("LOCAL_RANK", 0)
     # the ranks share one stdout pipe: with block buffering a flush can end mid-line and another rank's output then lands
@@ -248,6 +256,8 @@ def main(argv=None):
         set_knobs(args.set)
     train = importlib.import_module("train")
     feed = {"device_feed": True} if args.device_feed else {}  # without the flag: the call (and the patch) of before
+    if args.resample_negatives:
+        feed["resample_negatives"] = True
     patch_trainer(train, rank, world, args.seed, device_evaluate=args.device_evaluate, **feed)
     try:
         train.train()
