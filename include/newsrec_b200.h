@@ -41,6 +41,34 @@ int nr_has_triage_backends(void);
 /* Tests (release library too): on != 0 makes nr_gru_fwd run the per-step sequence even where the persistent recurrence applies,
  * on == 0 restores the default.  Until the first call it follows NEWSREC_GRU_STEPWISE (set: per-step), read once. */
 void nr_debug_set_gru_stepwise(int on);
+/* Tests (release library too): the store GEMM with every option of its epilogue, out[M][N] = act(sum_s A[r + s - tap_origin] .
+ * W_s^T + bias) [* (1 - t^2)] [* dropout], fields one for one with the library's internal operands and store configuration.
+ * Tap s (taps 1..4) reads weight rows [s * w_tap_rows, + N) against row r + s - tap_origin of A, zero outside [0, M);
+ * tap_origin < 0 is taps / 2.  tanh and relu exclude each other; dtanh_src (bf16, pitch dtanh_ld, even; 4-byte aligned) multiplies
+ * by 1 - t^2 at the output's own row and column.  The row map sends A row r = s * rm_seg_in + t + rm_in_off to output row
+ * s * rm_seg_out + t + rm_out_off when 0 <= t < rm_seg_len (rm_seg_in == 0: identity).  Dropout (p_drop > 0) keys its mask on
+ * the output row and column with pitch ld_out.  ones_col >= N (bf16 output, < ld_out): column ones_col = 1 and columns
+ * (ones_col, ones_zero_upto) = 0, ones_zero_upto <= ld_out, in mapped rows.  lo_out (bf16 output): columns [lo_col0, N) also
+ * leave bf16(y - bf16(y)) at lo_out[row][col - lo_col0], pitch ld_lo.  accumulate (fp32 output): out += result.  out and lo_out
+ * must be 16-byte aligned.  Returns -1 before any launch for a configuration the GEMM does not support. */
+typedef struct {
+    const void* A;
+    int M, lda;
+    const void* W;
+    int N, ldw, K, taps, w_tap_rows, tap_origin;
+    void* out;
+    int ld_out, out_bf16, relu, tanh;
+    const void* dtanh_src;
+    int dtanh_ld;
+    const float* bias;
+    int rm_seg_in, rm_in_off, rm_seg_len, rm_seg_out, rm_out_off;
+    float p_drop;
+    unsigned long long seed;
+    int ones_col, ones_zero_upto;
+    void* lo_out;
+    int ld_lo, lo_col0, accumulate, rows_per_tile;
+} nr_gemm_store_args;
+int nr_debug_gemm_store(const nr_gemm_store_args* a, void* stream);
 /* TUNING ONLY (tools/kbench.py): dev_buf holds slots x 148 x 16 int64; the k-th gemm_nt planned after this call
  * writes, per CTA, cycle counters into slot k: [0] TMA producer waiting for a free A stage, [1] consumer warpgroups
  * waiting for A data, [4] epilogue body, [5] kernel, [6] tiles.  Null (default) switches the counters off. */

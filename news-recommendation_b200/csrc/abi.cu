@@ -25,6 +25,20 @@ long long nr_launch_count(void) { return g_launches; }
 int nr_num_sms(void) { return num_sms(); }
 void nr_debug_set_simt_gemm(int on) { set_debug_simt_gemm(on); }
 void nr_debug_set_gru_stepwise(int on) { set_gru_stepwise(on); }
+int nr_debug_gemm_store(const nr_gemm_store_args* a, void* stream) {
+    NR_REQUIRE(a && a->A && a->W && a->out, "nr_debug_gemm_store: null operand");
+    const auto misaligned = [](const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; };
+    NR_REQUIRE(!misaligned(a->out, 16) && !misaligned(a->lo_out, 16) && !misaligned(a->dtanh_src, 4),
+               "nr_debug_gemm_store: out and lo_out need 16-byte, dtanh_src 4-byte aligned bases");
+    return gemm_store({.A = a->A, .M = a->M, .lda = a->lda, .W = a->W, .N = a->N, .ldw = a->ldw, .K = a->K, .taps = a->taps,
+                       .w_tap_rows = a->w_tap_rows, .tap_origin = a->tap_origin},
+                      {.out = a->out, .ld_out = a->ld_out, .out_bf16 = a->out_bf16, .relu = a->relu, .tanh = a->tanh,
+                       .dtanh_src = a->dtanh_src, .dtanh_ld = a->dtanh_ld, .bias = a->bias,
+                       .rm = {a->rm_seg_in, a->rm_in_off, a->rm_seg_len, a->rm_seg_out, a->rm_out_off},
+                       .drop = {a->p_drop, a->seed}, .ones_col = a->ones_col, .ones_zero_upto = a->ones_zero_upto, .lo_out = a->lo_out,
+                       .ld_lo = a->ld_lo, .lo_col0 = a->lo_col0, .accumulate = a->accumulate, .rows_per_tile = a->rows_per_tile},
+                      as_stream(stream));
+}
 int nr_has_triage_backends(void) { return has_triage_backends(); }
 void nr_reserve_sms_for_comm(int n) { set_comm_reserved_sms(n); }
 void nr_debug_set_gemm_timing(void* dev_buf, int slots) { set_debug_gemm_timing(dev_buf, slots); }

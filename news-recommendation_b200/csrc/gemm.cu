@@ -625,6 +625,13 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
                               kEpiSmemBytes<EpiStore>, 0));
     NR_PROPAGATE(apply_tap_origin(plan, g));
     NR_REQUIRE(c.out_bf16 ? (c.ld_out % 8 == 0) : (c.ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", c.ld_out);
+    // the ones column is written by slice 0's CTA with plain stores after its chunk loop: only past the result columns (a chunk
+    // of another slice, or one of its own TMA stores still in flight, would race with it) and only inside the row's pitch
+    NR_REQUIRE(c.ones_col < 0 || (c.out_bf16 && c.ones_col >= N && c.ones_col < c.ld_out),
+               "gemm_store: the ones column needs a bf16 output and N <= ones_col < ld_out (N=%d ones_col=%d ld=%d)", N, c.ones_col,
+               c.ld_out);
+    NR_REQUIRE(c.ones_zero_upto <= c.ld_out, "gemm_store: zeroed columns up to %d run past the output pitch %d", c.ones_zero_upto,
+               c.ld_out);
     EpiStore e;
     memset(&e, 0, sizeof(e));
     e.use_tma = (c.out_bf16 && c.rm.seg_in == 0 && rows_per_tile == kTileM && N >= 32) ? 1 : 0;

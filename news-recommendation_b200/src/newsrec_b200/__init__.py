@@ -117,6 +117,20 @@ class GruBwdArgs(C.Structure):
     ]
 
 
+class GemmStoreArgs(C.Structure):
+    """nr_gemm_store_args (include/newsrec_b200.h)."""
+    _fields_ = [
+        ("A", _vp), ("M", _i), ("lda", _i), ("W", _vp), ("N", _i), ("ldw", _i), ("K", _i), ("taps", _i), ("w_tap_rows", _i),
+        ("tap_origin", _i),
+        ("out", _vp), ("ld_out", _i), ("out_bf16", _i), ("relu", _i), ("tanh", _i), ("dtanh_src", _vp), ("dtanh_ld", _i),
+        ("bias", _vp),
+        ("rm_seg_in", _i), ("rm_in_off", _i), ("rm_seg_len", _i), ("rm_seg_out", _i), ("rm_out_off", _i),
+        ("p_drop", _f), ("seed", _ull),
+        ("ones_col", _i), ("ones_zero_upto", _i), ("lo_out", _vp), ("ld_lo", _i), ("lo_col0", _i), ("accumulate", _i),
+        ("rows_per_tile", _i),
+    ]
+
+
 class FeedField(C.Structure):
     """nr_feed_field (include/newsrec_b200.h)."""
     _fields_ = [("table", _vp), ("width", _i), ("out", _vp)]
@@ -132,6 +146,7 @@ SIGNATURES = {
     "nr_num_sms": (_i, []),
     "nr_debug_set_simt_gemm": (None, [_i]),
     "nr_debug_set_gru_stepwise": (None, [_i]),
+    "nr_debug_gemm_store": (_i, [C.POINTER(GemmStoreArgs), _vp]),
     "nr_has_triage_backends": (_i, []),
     "nr_reserve_sms_for_comm": (None, [_i]),
     "nr_debug_set_gemm_timing": (None, [_vp, _i]),

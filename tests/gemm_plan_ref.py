@@ -133,6 +133,9 @@ NT_REGIMES = ("1 slice", "slices > 1", "slice width % 32 != 0", "N < 32", "resid
               "streamed weights", "taps 3", "rows_per_tile < 64", "warpgroup 1 idle", "odd tiles per CTA", "even tiles per CTA")
 TN_REGIMES = ("cluster 1x1", "cluster 2x1", "cluster 1x2", "cluster 2x2", "NT 64", "NT 128", "NT 192", "NT 256", "n_tiles 2",
               "single k-range")
+# how a 32-column chunk of gemm_store's output leaves EpiStore::frag (and the options of its configuration)
+STORE_PATHS = ("TMA", "row pieces", "cut chunk", "fp32 pairs", "fp32 scalar")
+STORE_OPTIONS = ("relu", "tanh", "dtanh", "dropout", "row map", "ones column", "low plane", "+=", "taps")
 BWD_REGIMES = ("dscore warp", "dscore block", "dscore block D>512", "dPre TMA", "dPre plain stores", "dX fragment view",
                "dX row view", "dX slice capped by dOut staging", "dX slices > 1", "weight grad 2 launches")
 
@@ -188,3 +191,57 @@ def regimes_bwd(p):
         r.add("weight grad 2 launches")
     r |= {"dPre " + x for x in regimes_nt(p["dpre"])} | {"dX " + x for x in regimes_nt(dx)}
     return r
+
+
+def store_use_tma(N, out_bf16, row_map, rows_per_tile):
+    """gemm_store's use_tma: bf16 chunks leave through the tensor maps for identity rows, whole 64-row tiles and N >= 32."""
+    return bool(out_bf16) and not row_map and min(rows_per_tile, kTileM) == kTileM and N >= 32
+
+
+def store_paths(plan, out_bf16, row_map=False, lo_col0=None):
+    """The paths of STORE_PATHS the chunks of every slice take in EpiStore::frag, as (output paths, low-plane paths).  A bf16
+    chunk at slice column lc0 is cut (predicated fragment stores) when lc0 + 32 > the slice's columns, else it leaves by TMA
+    (use_tma) or as 16-byte row pieces; fp32 leaves as column pairs (lc + 1 < ncols) and, where a slice has an odd column
+    count, one scalar.  The low plane takes the bf16 rule for the chunks at or past lo_col0 (None: no low plane)."""
+    tma = store_use_tma(plan["N"], out_bf16, row_map, plan["rows_per_tile"])
+    out, lo = set(), set()
+    for sl in range(plan["n_slices"]):
+        col0 = sl * plan["n_stride"]
+        ncols = min(plan["n_stride"], plan["N"] - col0)
+        for lc0 in range(0, ncols, 32):
+            if not out_bf16:
+                if ncols - lc0 >= 2:
+                    out.add("fp32 pairs")
+                if ncols % 2 and lc0 + 32 >= ncols:
+                    out.add("fp32 scalar")
+                continue
+            path = "cut chunk" if lc0 + 32 > ncols else ("TMA" if tma else "row pieces")
+            out.add(path)
+            if lo_col0 is not None and col0 + lc0 >= lo_col0:
+                lo.add(path)
+    return out, lo
+
+
+def lo_chunk_aligned(plan, lo_col0):
+    """lo_plane_chunk_aligned (csrc/gemm.cu): no 32-column chunk of a weight slice straddles lo_col0."""
+    s = plan["n_stride"]
+    return all(not (c0 < lo_col0 < c0 + s and (lo_col0 - c0) % 32) for c0 in range(0, plan["n_slices"] * s, s))
+
+
+def lo_supported(N, K, lo_col0):
+    """gemm_store_lo_supported: the low plane of the columns [lo_col0, N) of an N x K product is chunk aligned under the
+    weight slicing of plan_nt (which depends on N and K only)."""
+    return 0 <= lo_col0 < N and lo_chunk_aligned(plan_nt(0, N, K), lo_col0)
+
+
+def store_accepts(option, path):
+    """Whether gemm_store takes an option of STORE_OPTIONS on an output path of STORE_PATHS (for "low plane": a path of the
+    plane itself).  A row map leaves without TMA; the ones column and the low plane need a bf16 output, += an fp32 one."""
+    bf16 = path in ("TMA", "row pieces", "cut chunk")
+    if option == "row map":
+        return path != "TMA"
+    if option in ("ones column", "low plane"):
+        return bf16
+    if option == "+=":
+        return not bf16
+    return True

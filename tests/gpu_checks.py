@@ -132,14 +132,15 @@ def check_linear(M=300, N=900, K=300, taps=1, seg=0, relu=0, out_bf16=1):
             "relu_zero_exact": zero_exact}
 
 
-def linear_ref(A, W, bias, N, taps=1, w_tap_rows=0):
-    """fp64 pre-activation of nr_linear and the sum of |products| + |bias| per element: tap s reads A shifted by s - taps // 2
-    rows (zero outside A) against weight rows [s * w_tap_rows, + N).  A [M][K], W [rows][K], bias [N] or None (fp64 device)."""
+def linear_ref(A, W, bias, N, taps=1, w_tap_rows=0, tap_origin=None):
+    """fp64 pre-activation of nr_linear and the sum of |products| + |bias| per element: tap s reads A shifted by s - tap_origin
+    rows (tap_origin None: taps // 2; zero outside A) against weight rows [s * w_tap_rows, + N).  A [M][K], W [rows][K], bias [N]
+    or None (fp64 device)."""
     M = A.shape[0]
     pre = torch.zeros(M, N, dtype=torch.float64, device=A.device)
     absum = torch.zeros_like(pre)
     for s in range(taps):
-        d = s - taps // 2
+        d = s - (taps // 2 if tap_origin is None else tap_origin)
         As = torch.zeros_like(A)
         lo, hi = max(0, -d), min(M, M - d)
         if hi > lo:

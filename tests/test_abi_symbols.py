@@ -54,7 +54,8 @@ def test_struct_layouts_match_the_header_field_order():
     text = open(HEADER).read()
     for cname, cls in (("nr_mhsa_encoder_fwd_args", nb.MhsaEncoderFwdArgs), ("nr_mhsa_encoder_bwd_args", nb.MhsaEncoderBwdArgs),
                        ("nr_cnn_encoder_fwd_args", nb.CnnEncoderFwdArgs), ("nr_cnn_encoder_bwd_args", nb.CnnEncoderBwdArgs),
-                       ("nr_gru_fwd_args", nb.GruFwdArgs), ("nr_gru_bwd_args", nb.GruBwdArgs)):
+                       ("nr_gru_fwd_args", nb.GruFwdArgs), ("nr_gru_bwd_args", nb.GruBwdArgs),
+                       ("nr_gemm_store_args", nb.GemmStoreArgs)):
         end = re.search(r"\}\s*" + cname + r"\s*;", text).start()
         start = text.rfind("typedef struct {", 0, end) + len("typedef struct {")
         body = re.sub(r"/\*.*?\*/", "", text[start:end], flags=re.S)

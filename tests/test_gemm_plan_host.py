@@ -126,3 +126,76 @@ def test_schedule_covers_every_tile_once():
         p = P.plan_nt(M, N, K, 1, rpt)
         seen = [(t, p["slice_of"][b]) for b, (w0, w1) in enumerate(p["wg_tiles"]) for t in w0 + w1]
         assert sorted(seen) == [(t, s) for t in range(p["num_m_tiles"]) for s in range(p["n_slices"])]
+
+
+# ------------------------------------------------------------------------------------------------
+# gemm_store's options and store paths (tests/test_gpu_gemm_store.py)
+# ------------------------------------------------------------------------------------------------
+def _store_plan(c):
+    s = C.store_setup(c)
+    return P.plan_nt(s["M"], c["N"], c["K"], c.get("taps", 1), s["rpt"]), s
+
+
+def _store_paths(c):
+    plan, s = _store_plan(c)
+    out, lo = P.store_paths(plan, c.get("out_bf16", 1), c.get("rm") is not None, s["lo_col0"])
+    return out | {"lo " + x for x in lo}
+
+
+@pytest.mark.parametrize("c", C.STORE_CASES, ids=lambda c: c["id"])
+def test_store_case_labels(c):
+    """A case sets exactly the options it names, and its plan reaches the NT regimes and takes exactly the store paths it names."""
+    assert set(c["options"]) == C.store_options(c), (c["id"], sorted(C.store_options(c)))
+    assert set(c["options"]) <= set(P.STORE_OPTIONS)
+    plan, s = _store_plan(c)
+    got = P.regimes_nt(plan)
+    assert set(c["regimes"]) <= got, (c["id"], sorted(got))
+    assert set(c["paths"]) == _store_paths(c), (c["id"], sorted(_store_paths(c)))
+    if s["lo_col0"] is not None:  # gemm_store accepts the case's low plane
+        assert P.lo_chunk_aligned(plan, s["lo_col0"]) and (P.store_use_tma(c["N"], 1, c.get("rm"), s["rpt"]) or s["lo_col0"] % 8 == 0)
+
+
+def test_every_store_option_path_pair_has_a_case():
+    """Every (option, path) pair gemm_store accepts is reached by a case (the low plane by the paths of the plane itself)."""
+    want = {(o, p) for o in P.STORE_OPTIONS for p in P.STORE_PATHS if P.store_accepts(o, p)}
+    have = set()
+    for c in C.STORE_CASES:
+        paths = _store_paths(c)
+        for o in c["options"]:
+            have |= {(o, p[3:]) for p in paths if p.startswith("lo ")} if o == "low plane" else {(o, p) for p in paths if p in P.STORE_PATHS}
+    assert want <= have, sorted(want - have)
+    assert have <= want, sorted(have - want)
+    ids = [c["id"] for c in C.STORE_CASES]
+    assert len(ids) == len(set(ids))
+
+
+def test_store_case_table_reaches_the_edges():
+    """The slice edges and production shapes the table exists for: a slice width of 16 mod 32, N < 32, an odd fp32 tail, M = 1,
+    M not a multiple of 64, rows_per_tile 1 and 50, dropout at p = 0.2 and 0.5 on both output types with and without a row
+    map, taps 2 and 4 at tap_origin 0 and taps - 1, the low plane from column 0 and from a chunk boundary inside slice 1."""
+    cases = C.STORE_CASES
+    setups = [C.store_setup(c) for c in cases]
+    plans = [_store_plan(c)[0] for c in cases]
+    assert any(p["n_stride"] % 32 == 16 for p in plans)
+    assert any(c["N"] < 32 for c in cases) and any(c.get("out_bf16", 1) == 0 and c["N"] % 2 for c in cases)
+    assert any(s["M"] == 1 for s in setups) and any(s["M"] % 64 for s in setups)
+    assert {1, 50} <= {s["rpt"] for s in setups}
+    for p in (0.2, 0.5):
+        assert {(c.get("out_bf16", 1), c.get("rm") is not None) for c in cases if c.get("p") == p} >= {(0, False), (1, False), (1, True)} \
+            if p == 0.2 else {(0, False), (0, True), (1, False)}, p
+    for taps in (2, 4):
+        assert {0, taps - 1} <= {c.get("tap_origin") for c in cases if c.get("taps") == taps}, taps
+    lo = {(c["N"], c["K"], C.store_setup(c)["lo_col0"]) for c in cases if c.get("lo_col0") is not None}
+    assert any(l0 == 0 for _, _, l0 in lo)
+    assert any(P.plan_nt(1, N, K)["n_stride"] < l0 < 2 * P.plan_nt(1, N, K)["n_stride"] for N, K, l0 in lo)
+    assert any(c.get("dtanh") and c["N"] % 2 for c in cases)
+    assert any(c.get("relu") and c.get("p") for c in cases)
+
+
+@pytest.mark.parametrize("heads,supported", [(1, 0), (2, 0), (3, 1), (7, 1), (14, 1), (15, 1)])
+def test_lo_supported_matches_the_accurate_mhsa_head_counts(heads, supported):
+    """nr_mhsa_accurate_supported reaches the low-plane rule through gemm_store_lo_supported(3 sec, d, 2 sec), sec = round_up(d, 8):
+    at d_k = 20 the V section starts inside a 32-column chunk of the Q|K|V projection at 1 and 2 heads only."""
+    d = 20 * heads
+    sec = (d + 7) // 8 * 8
+    assert P.lo_supported(3 * sec, d, 2 * sec) == bool(supported)
