@@ -243,6 +243,24 @@ int nr_prediction_line_offsets(const long long* impression_ids, const int* ranks
 int nr_prediction_text(const long long* impression_ids, const int* ranks, const long long* seg_offsets, long long n_seg,
                        const long long* line_offsets, char* text, void* stream);
 
+/* Recommendation over a whole news pool: the k best news of every user, score[u][n] = users[u] . news[n], without the
+ * n_users x n_news score matrix ever reaching memory.  users fp32 [n_users][ld_users], news fp32 [n_news][ld_news] (row
+ * pitches in elements, >= D), 1 <= k <= 128, 1 <= D <= 4096, n_users and n_news below 2^31 - 64.  Optional exclusions in CSR
+ * form (both null, or both device int64): user u never gets the news rows excl_rows[excl_offsets[u] .. excl_offsets[u + 1])
+ * (a set: duplicates and any order are fine; a row outside [0, n_news) sets *bad_row_flag and is otherwise ignored).
+ * Outputs idx int64 [n_users][k] and score fp32 [n_users][k], best first: higher score, then lower news row (identical news
+ * rows come out in row order); when fewer than k news are eligible the trailing slots hold -1 / -inf.  A non-finite score of
+ * any (user, news) pair sets *bad_score_flag (the order is then undefined).  The same inputs give the same bits on every run.
+ * Scores: hi/lo bf16 planes of both operands, hi.hi + hi.lo + lo.hi on the tensor cores with fp32 accumulation, within
+ *     |score - u.n| <= (2^-15 + 3 round_up(D, 64) 2^-23) sum_i |u_i| |n_i|
+ * of the exact dot product of the fp32 inputs.  workspace: nr_topk_dot_workspace(...) bytes (256-byte aligned; -1 for a
+ * shape outside the limits above), which depends on the device's SM count.  Every limit is checked before the first launch;
+ * n_users == 0 or n_news == 0 launches nothing. */
+long long nr_topk_dot_workspace(long long n_users, long long n_news, int D, int k);
+int nr_topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
+                const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
+                int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
+
 /* Host-side glue of the weight-gradient GEMMs (nr_gemm_tn with the ones column): ext is [rows][ld] fp32 whose columns
  * [0,D) hold dW and column D holds db.  Adds them into the parameters' own gradient storage (dW [rows][D] contiguous,
  * db [rows] or null) and CLEARS ext, so the caller can keep it as a persistent accumulator across steps. */

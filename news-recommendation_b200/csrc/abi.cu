@@ -194,6 +194,14 @@ int nr_impression_ranks(const float* scores, const long long* seg_offsets, long 
     NR_REQUIRE(scores && seg_offsets && ranks && bad_score_flag && n_seg >= 0, "nr_impression_ranks: null operand or n_seg=%lld", n_seg);
     return impression_ranks(scores, seg_offsets, n_seg, ranks, bad_score_flag, as_stream(stream));
 }
+long long nr_topk_dot_workspace(long long n_users, long long n_news, int D, int k) { return topk_dot_workspace(n_users, n_news, D, k); }
+int nr_topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
+                const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
+                int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream) {
+    NR_REQUIRE(users && news && idx && score && bad_row_flag && bad_score_flag, "nr_topk_dot: null operand");
+    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, idx, score, bad_row_flag,
+                    bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+}
 long long nr_prediction_line_offsets_workspace(long long n_seg) {
     NR_REQUIRE(n_seg >= 0, "nr_prediction_line_offsets_workspace: n_seg=%lld", n_seg);
     return prediction_scan_bytes(n_seg);

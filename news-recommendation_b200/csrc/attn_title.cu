@@ -30,8 +30,11 @@
 
 namespace nr {
 
+int read_topk_device_error(int* out4);
 int read_attn_device_error(int* out4) {
-    return static_cast<int>(cudaMemcpyFromSymbol(out4, fused::g_attn_dev_error, sizeof(int) * 4));
+    const int rc = static_cast<int>(cudaMemcpyFromSymbol(out4, fused::g_attn_dev_error, sizeof(int) * 4));
+    if (rc != 0 || out4[0] != 0) return rc;
+    return read_topk_device_error(out4);  // the top-k kernel keeps its own record (topk.cu)
 }
 
 namespace title {

@@ -215,6 +215,11 @@ int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int
 // candidates (include/newsrec_b200.h, nr_sample_negatives)
 int sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp, const long long* row_offsets,
                      int K, unsigned long long seed, long long epoch, int* behaviors, int H, cudaStream_t stream);
+// top-k of users . news over a whole pool (topk.cu; include/newsrec_b200.h, nr_topk_dot)
+long long topk_dot_workspace(long long n_users, long long n_news, int D, int k);
+int topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
+             const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
+             int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
 int num_sms();
 extern int g_launches;  // kernels launched by this library (nr_launch_count)
 

@@ -64,14 +64,20 @@ def read_behaviors(directory, **kw):
     return beh
 
 
+def distinct_histories(beh):
+    """The (user, clicked_news) rows of beh (read_behaviors) that define the user tables: duplicate pairs dropped, then the
+    first row of each distinct history string, in first-appearance order."""
+    users = beh[["user", "clicked_news"]].drop_duplicates()
+    return users[~users["clicked_news"].duplicated()]        # first-wins user2vector (evaluate.py:226-230)
+
+
 def user_tables(beh, news_index, H, user2int_path):
     """The user half of build_tables: (user, history, history_length, hist_row) -- one row per distinct history string
     of beh (read_behaviors), hist_row mapping each string to its row."""
     import pandas as pd
     pad = news_index["PADDED_NEWS"]
     user2int = dict(pd.read_table(user2int_path).values.tolist())
-    users = beh[["user", "clicked_news"]].drop_duplicates()
-    users = users[~users["clicked_news"].duplicated()]        # first-wins user2vector (evaluate.py:226-230)
+    users = distinct_histories(beh)
     hist_row = {}
     U = len(users)
     user = np.zeros(U, np.int64)

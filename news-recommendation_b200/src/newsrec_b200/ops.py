@@ -592,3 +592,49 @@ def prediction_text(impression_ids, ranks, seg_offsets):
     check(lib.nr_prediction_text(_p(ids), _p(ranks), _p(seg_offsets), n_seg, _p(line_offsets), _p(text), _stream()),
           "nr_prediction_text")
     return text
+
+
+def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None):
+    """The k best news of every user over the whole pool, one pass (nr_topk_dot): users (U, D) and news (n, D) fp32, scores
+    users[u] . news[r] at fp32 level on the tensor cores (the bound is in include/newsrec_b200.h) without the U x n score
+    matrix.  Optional exclusions in CSR form: user u never gets rows excl_rows[excl_offsets[u] .. excl_offsets[u + 1]).
+    Returns (idx (U, k) int64, score (U, k) fp32) on the caller's stream, best first, equal scores by lower row; slots past
+    the eligible news hold -1 / -inf.  Raises NewsrecError on bad arguments (before any launch), IndexError on an exclusion
+    row outside [0, n) and ValueError on a non-finite score (both read device flags: one synchronisation)."""
+    lib = load_library()
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 128:
+        raise NewsrecError(f"top_k_scores: k={k!r} must be an integer in [1, 128]")
+    if users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]:
+        raise NewsrecError(f"top_k_scores: users {tuple(users.shape)} and news {tuple(news.shape)} must be (U, D) and (n, D)")
+    if (excl_rows is None) != (excl_offsets is None):
+        raise NewsrecError("top_k_scores: excl_rows and excl_offsets go together")
+    dev = require_cuda()
+    users = users.to(dev).float().contiguous()
+    news = news.to(dev).float().contiguous()
+    U, D = users.shape
+    n = news.shape[0]
+    if excl_offsets is not None:
+        excl_offsets = excl_offsets.to(dev).long().contiguous()
+        excl_rows = excl_rows.to(dev).long().contiguous()
+        if excl_offsets.dim() != 1 or excl_offsets.numel() != U + 1 or excl_rows.dim() != 1:
+            raise NewsrecError("top_k_scores: excl_offsets must be (U + 1,) and excl_rows 1-D")
+        if excl_rows.numel() == 0:
+            excl_rows = excl_rows.new_zeros(1)  # a valid address for an empty set
+    ws_bytes = int(lib.nr_topk_dot_workspace(U, n, D, k))
+    if ws_bytes < 0:
+        check(-1, "nr_topk_dot_workspace")
+    if U == 0 or n == 0:  # no user or nothing eligible: the library launches nothing
+        return (torch.full((U, k), -1, dtype=torch.int64, device=dev),
+                torch.full((U, k), float("-inf"), dtype=torch.float32, device=dev))
+    idx = torch.empty((U, k), dtype=torch.int64, device=dev)
+    score = torch.empty((U, k), dtype=torch.float32, device=dev)
+    flags = torch.zeros(2, dtype=torch.int32, device=dev)
+    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    check(lib.nr_topk_dot(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(idx), _p(score),
+                          _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes, _stream()), "nr_topk_dot")
+    bad_row, bad_score = (int(x) for x in flags.tolist())
+    if bad_row:
+        raise IndexError("top_k_scores: an exclusion row is outside the news pool")
+    if bad_score:
+        raise ValueError("top_k_scores: a score is not finite; the order is undefined")
+    return idx, score

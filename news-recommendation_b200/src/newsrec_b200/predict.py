@@ -136,9 +136,30 @@ def load_checkpoint(path, device):
         return torch.load(path, map_location=device, weights_only=True)
 
 
+def load_model(checkpoint, checkpoint_dir, knobs):
+    """(name, path, model): the drop-in's <MODEL_NAME> with the knobs applied, on the device in eval mode, loaded from
+    checkpoint or the latest ckpt-<n>.pth of checkpoint_dir (default ./checkpoint/<MODEL_NAME>)."""
+    import importlib
+    src = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))  # the drop-in's config / model packages
+    if src not in sys.path:
+        sys.path.insert(0, src)
+    from . import require_cuda
+    from .launch import set_knobs
+    cfgmod = importlib.import_module("config")
+    name = cfgmod.model_name
+    cfg = set_knobs(knobs)
+    path = checkpoint or latest_checkpoint(checkpoint_dir or os.path.join("checkpoint", name))
+    if path is None:
+        raise SystemExit(f"no checkpoint file found in {checkpoint_dir or os.path.join('checkpoint', name)}")
+    dev = require_cuda()
+    model = getattr(importlib.import_module(f"model.{name}"), name)(cfg).to(dev)
+    model.load_state_dict(load_checkpoint(path, dev)["model_state_dict"])
+    model.eval()
+    return name, path, model
+
+
 def main(argv=None):
     import argparse
-    import importlib
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--directory", default="./data/test", help="test split: news_parsed.tsv and behaviors.tsv")
     ap.add_argument("--out", default="prediction.txt", help="the file to write")
@@ -151,21 +172,7 @@ def main(argv=None):
                     help="override a knob of the selected <MODEL_NAME>Config (repeatable)")
     args = ap.parse_args(argv)
 
-    src = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))  # the drop-in's config / model packages
-    if src not in sys.path:
-        sys.path.insert(0, src)
-    from . import require_cuda
-    from .launch import set_knobs
-    cfgmod = importlib.import_module("config")
-    name = cfgmod.model_name
-    cfg = set_knobs(args.set)
-    path = args.checkpoint or latest_checkpoint(args.checkpoint_dir or os.path.join("checkpoint", name))
-    if path is None:
-        raise SystemExit(f"no checkpoint file found in {args.checkpoint_dir or os.path.join('checkpoint', name)}")
-    dev = require_cuda()
-    model = getattr(importlib.import_module(f"model.{name}"), name)(cfg).to(dev)
-    model.load_state_dict(load_checkpoint(path, dev)["model_state_dict"])
-    model.eval()
+    name, path, model = load_model(args.checkpoint, args.checkpoint_dir, args.set)
     n = predict(model, args.directory, args.out, user2int_path=args.user2int, chunk_impressions=args.chunk_impressions)
     print(f"{name} from {path}: {n} impressions written to {args.out}")
     return 0
