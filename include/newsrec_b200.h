@@ -261,6 +261,27 @@ int nr_topk_dot(const float* users, long long n_users, int ld_users, const float
                 const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
                 int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
 
+/* Ranks over a whole news pool under nr_topk_dot's scores.  Query row q (queries fp32 [n_rows][ld_queries]) has the target
+ * set T_q = tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) and the exclusion set X_q (excl_offsets / excl_rows as in
+ * nr_topk_dot: both null, or both device int64; a set, any length, order or duplicates).  For every target t of q:
+ *     rank(q, t) = |{ n in [0, n_news) \ X_q \ T_q : s(q, n) > s(q, t)  or  (s(q, n) == s(q, t) and n < t) }|
+ * where s is bit for bit the score nr_topk_dot computes for the pair (the same planes and tile code): rank(q, t) is t's 0-based
+ * position in the order nr_topk_dot returns over the pool without X_q and T_q.  A target is ranked even when it is also in X_q.
+ * rank int64 and score fp32 (s(q, t)) are written in target order, [tgt_offsets[0] .. tgt_offsets[n_rows]).  The same inputs
+ * give the same bits on every run.  Limits: 1 <= D <= 4096, 0 <= n_rows and 1 <= n_news, both below 2^31 - 64, pitches >= D;
+ * at most 32 targets per row: a row with more sets *target_flag and gets rank -1 (score NaN).  A target or exclusion outside
+ * [0, n_news) sets *bad_row_flag (such a target's row gets rank -1); a non-finite score of a row with targets sets
+ * *bad_score_flag (its ranks are then undefined).  With |s(q, n) - S(n)| <= e(n) (the bound of nr_topk_dot,
+ * e(n) = (2^-15 + 3 round_up(D, 64) 2^-23) sum_i |q_i| |n_i|, S(n) the exact dot product of the fp32 inputs):
+ *     |{n eligible : S(n) - S(t) > e(n) + e(t)}|  <=  rank(q, t)  <=  |{n eligible : S(n) - S(t) >= -(e(n) + e(t))}|
+ * workspace: nr_pool_ranks_workspace(...) bytes (256-byte aligned; -1 for a shape outside the limits), which depends on the
+ * device's SM count.  Every limit is checked before the first launch; n_rows == 0 launches nothing. */
+long long nr_pool_ranks_workspace(long long n_rows, long long n_news, int D);
+int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
+                  const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
+                  long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                  long long workspace_bytes, void* stream);
+
 /* Host-side glue of the weight-gradient GEMMs (nr_gemm_tn with the ones column): ext is [rows][ld] fp32 whose columns
  * [0,D) hold dW and column D holds db.  Adds them into the parameters' own gradient storage (dW [rows][D] contiguous,
  * db [rows] or null) and CLEARS ext, so the caller can keep it as a persistent accumulator across steps. */

@@ -202,6 +202,16 @@ int nr_topk_dot(const float* users, long long n_users, int ld_users, const float
     return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, idx, score, bad_row_flag,
                     bad_score_flag, workspace, workspace_bytes, as_stream(stream));
 }
+long long nr_pool_ranks_workspace(long long n_rows, long long n_news, int D) { return pool_ranks_workspace(n_rows, n_news, D); }
+int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
+                  const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
+                  long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                  long long workspace_bytes, void* stream) {
+    NR_REQUIRE(queries && news && tgt_offsets && tgt_rows && rank && score && bad_row_flag && bad_score_flag && target_flag,
+               "nr_pool_ranks: null operand");
+    return pool_ranks(queries, n_rows, ld_queries, news, n_news, ld_news, D, tgt_offsets, tgt_rows, excl_offsets, excl_rows, rank,
+                      score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes, as_stream(stream));
+}
 long long nr_prediction_line_offsets_workspace(long long n_seg) {
     NR_REQUIRE(n_seg >= 0, "nr_prediction_line_offsets_workspace: n_seg=%lld", n_seg);
     return prediction_scan_bytes(n_seg);

@@ -220,6 +220,12 @@ long long topk_dot_workspace(long long n_users, long long n_news, int D, int k);
 int topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
              const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
              int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
+// ranks of target news among a whole pool under the same scores (topk.cu; include/newsrec_b200.h, nr_pool_ranks)
+long long pool_ranks_workspace(long long n_rows, long long n_news, int D);
+int pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
+               const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
+               long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+               long long workspace_bytes, cudaStream_t stream);
 int num_sms();
 extern int g_launches;  // kernels launched by this library (nr_launch_count)
 

@@ -177,6 +177,8 @@ SIGNATURES = {
     "nr_impression_ranks": (_i, [_vp, _vp, _ll, _vp, _vp, _vp]),
     "nr_topk_dot_workspace": (_ll, [_ll, _ll, _i, _i]),
     "nr_topk_dot": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "nr_pool_ranks_workspace": (_ll, [_ll, _ll, _i]),
+    "nr_pool_ranks": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_prediction_line_offsets_workspace": (_ll, [_ll]),
     "nr_prediction_line_offsets": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _ll, _vp]),
     "nr_prediction_text": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),

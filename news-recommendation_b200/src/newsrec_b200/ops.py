@@ -638,3 +638,105 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None):
     if bad_score:
         raise ValueError("top_k_scores: a score is not finite; the order is undefined")
     return idx, score
+
+
+POOL_RANK_MAX_TARGETS = 32  # targets per kernel row (nr_pool_ranks)
+
+
+def target_parts(tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None, max_targets=POOL_RANK_MAX_TARGETS):
+    """Host CSR plumbing of pool_ranks: query q with c > 0 targets becomes ceil(c / max_targets) kernel rows, each holding
+    consecutive targets of q, so the kernel's targets are the caller's in the same order.  Each row excludes X_q and q's
+    targets outside the row, so a rank does not depend on the split; a query without targets gets no row.  Returns
+    (query (R,), offsets (R + 1,), excl_rows, excl_offsets (R + 1,)) as int64 NumPy arrays; offsets index tgt_rows."""
+    import numpy as np
+    tr, to = np.asarray(tgt_rows, np.int64), np.asarray(tgt_offsets, np.int64)
+    counts = np.diff(to)
+    nparts = (counts + max_targets - 1) // max_targets
+    R = int(nparts.sum())
+    query = np.repeat(np.arange(len(counts), dtype=np.int64), nparts)
+    first = np.repeat(np.cumsum(nparts) - nparts, nparts)
+    start = to[query] + max_targets * (np.arange(R, dtype=np.int64) - first)
+    end = np.minimum(start + max_targets, to[query + 1])
+    offsets = np.concatenate([start, end[-1:]]) if R else to[:1].copy()
+    xlen = np.zeros(R, np.int64) if excl_offsets is None else \
+        np.asarray(excl_offsets, np.int64)[query + 1] - np.asarray(excl_offsets, np.int64)[query]
+    split = np.flatnonzero(nparts[query] > 1)
+    extra = np.zeros(R, np.int64)
+    extra[split] = counts[query[split]] - (end - start)[split]
+    ex_off = np.zeros(R + 1, np.int64)
+    ex_off[1:] = np.cumsum(xlen + extra)
+    ex_rows = np.zeros(int(ex_off[-1]), np.int64)
+    if xlen.sum():
+        seg = np.repeat(np.arange(R), xlen)
+        within = np.arange(int(xlen.sum()), dtype=np.int64) - np.repeat(np.cumsum(xlen) - xlen, xlen)
+        ex_rows[ex_off[seg] + within] = np.asarray(excl_rows, np.int64)[np.asarray(excl_offsets, np.int64)[query[seg]] + within]
+    for p in split:
+        q = query[p]
+        ex_rows[ex_off[p] + xlen[p]:ex_off[p + 1]] = np.concatenate([tr[to[q]:start[p]], tr[end[p]:to[q + 1]]])
+    return query, offsets, ex_rows, ex_off
+
+
+def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None):
+    """Ranks of target news among the whole pool under nr_topk_dot's scores (nr_pool_ranks): query q (users (Q, D) fp32)
+    has targets tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) of news (n, D) fp32 and optional exclusions in CSR form.
+    rank(q, t) is t's 0-based position in the order top_k_scores returns for q over the pool without q's exclusions and
+    its other targets: higher score first, equal scores by lower row.  Returns (rank (n_targets,) int64, score
+    (n_targets,) fp32 = s(q, t)) in target order, on the caller's stream.  Queries with more than 32 targets run as several
+    kernel rows (target_parts).  Raises NewsrecError on bad arguments (before any launch), IndexError on a target or
+    exclusion row outside [0, n) and ValueError on a non-finite score (the device flags are read once: one
+    synchronisation)."""
+    import numpy as np
+    lib = load_library()
+    if users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]:
+        raise NewsrecError(f"pool_ranks: users {tuple(users.shape)} and news {tuple(news.shape)} must be (Q, D) and (n, D)")
+    if (excl_rows is None) != (excl_offsets is None):
+        raise NewsrecError("pool_ranks: excl_rows and excl_offsets go together")
+    to = torch.as_tensor(tgt_offsets).cpu().long().numpy()
+    Q, D = users.shape
+    n = news.shape[0]
+    if to.ndim != 1 or len(to) != Q + 1 or to[0] != 0 or (np.diff(to) < 0).any() or to[-1] != len(tgt_rows):
+        raise NewsrecError("pool_ranks: tgt_offsets must be (Q + 1,), start at 0, not decrease and end at len(tgt_rows)")
+    eo = er = None
+    if excl_offsets is not None:
+        eo = torch.as_tensor(excl_offsets).cpu().long().numpy()
+        er = torch.as_tensor(excl_rows).cpu().long().numpy()
+        if eo.ndim != 1 or len(eo) != Q + 1 or er.ndim != 1 or (np.diff(eo) < 0).any() or eo[0] < 0 or eo[-1] > len(er):
+            raise NewsrecError("pool_ranks: excl_offsets must be (Q + 1,) non-decreasing offsets into the 1-D excl_rows")
+    dev = require_cuda()
+    n_t = int(to[-1])
+    if int(lib.nr_pool_ranks_workspace(max(Q, 0), max(n, 1), D)) < 0:
+        check(-1, "nr_pool_ranks_workspace")
+    if n_t == 0:
+        return torch.zeros(0, dtype=torch.int64, device=dev), torch.zeros(0, dtype=torch.float32, device=dev)
+    if n == 0:
+        raise IndexError("pool_ranks: a target row is outside the news pool (the pool is empty)")
+    tr = torch.as_tensor(tgt_rows).cpu().long().numpy()
+    query, offsets, xr, xo = target_parts(tr, to, er, eo)
+    R = len(query)
+    users = users.to(dev).float()
+    same = R == Q and bool((query == np.arange(Q)).all())
+    rows = users.contiguous() if same else users.index_select(0, torch.from_numpy(query).to(dev)).contiguous()
+    news = news.to(dev).float().contiguous()
+    ws_bytes = int(lib.nr_pool_ranks_workspace(R, n, D))
+    if ws_bytes < 0:
+        check(-1, "nr_pool_ranks_workspace")
+    d_to = torch.from_numpy(offsets).to(dev)
+    d_tr = torch.from_numpy(tr).to(dev)
+    d_xo = d_xr = None
+    if eo is not None or len(xr):
+        d_xo = torch.from_numpy(xo).to(dev)
+        d_xr = torch.from_numpy(xr if len(xr) else np.zeros(1, np.int64)).to(dev)  # a valid address for an empty set
+    rank = torch.empty(n_t, dtype=torch.int64, device=dev)
+    score = torch.empty(n_t, dtype=torch.float32, device=dev)
+    flags = torch.zeros(3, dtype=torch.int32, device=dev)
+    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    check(lib.nr_pool_ranks(_p(rows), R, D, _p(news), n, D, D, _p(d_to), _p(d_tr), _p(d_xo), _p(d_xr), _p(rank), _p(score),
+                            _p(flags[0:1]), _p(flags[1:2]), _p(flags[2:3]), _p(workspace), ws_bytes, _stream()), "nr_pool_ranks")
+    bad_row, bad_score, too_many = (int(x) for x in flags.tolist())
+    if bad_row:
+        raise IndexError("pool_ranks: a target or exclusion row is outside the news pool")
+    if bad_score:
+        raise ValueError("pool_ranks: a score is not finite; the ranks are undefined")
+    if too_many:
+        raise NewsrecError("pool_ranks: a kernel row got more than 32 targets")
+    return rank, score
