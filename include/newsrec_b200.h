@@ -261,6 +261,24 @@ int nr_topk_dot(const float* users, long long n_users, int ld_users, const float
                 const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
                 int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
 
+/* nr_topk_dot with at most m = max_per_category news of one category per list (diversified recommendation).  categories is
+ * device int32 [n_news], one key per news row (any value: 0, negative keys and so on are ordinary keys).  With s(u, n) the bit
+ * pattern nr_topk_dot computes for the pair and E_u the pool without u's exclusions: walk E_u in nr_topk_dot's output order
+ * (score descending, then lower row) and take a news iff, at that moment, fewer than m taken news share its category and fewer
+ * than k news are taken in all.  The output is the taken news in walk order, with nr_topk_dot's shapes and padding: idx int64
+ * [n_users][k] and score fp32 [n_users][k], -1 / -inf after the last taken news (a user gets fewer than k news when the caps
+ * run out, e.g. with fewer than ceil(k / m) categories).  The result is exact with respect to the kernel's own scores, ties
+ * included; excluded news never count against a cap; m >= k gives nr_topk_dot's output bit for bit; the same inputs give the
+ * same bits on every run.  The walk is the greedy of a matroid (at most m per category, at most k in all), applied inside the
+ * kernel's candidate buffers, so the n_users x n_news score matrix still never reaches memory.  One cap field per call: two
+ * simultaneous caps (category and subcategory) are not a matroid and are not supported.  Every limit of nr_topk_dot, a null
+ * categories and max_per_category < 1 are refused (-1) before the first launch.  workspace: nr_topk_dot_workspace(...) bytes
+ * (the same layout).  Flags as nr_topk_dot. */
+int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D,
+                       int k, const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+                       long long* idx, float* score, int* bad_row_flag, int* bad_score_flag, void* workspace,
+                       long long workspace_bytes, void* stream);
+
 /* Ranks over a whole news pool under nr_topk_dot's scores.  Query row q (queries fp32 [n_rows][ld_queries]) has the target
  * set T_q = tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) and the exclusion set X_q (excl_offsets / excl_rows as in
  * nr_topk_dot: both null, or both device int64; a set, any length, order or duplicates).  For every target t of q:

@@ -199,8 +199,17 @@ int nr_topk_dot(const float* users, long long n_users, int ld_users, const float
                 const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
                 int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream) {
     NR_REQUIRE(users && news && idx && score && bad_row_flag && bad_score_flag, "nr_topk_dot: null operand");
-    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, idx, score, bad_row_flag,
-                    bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, nullptr, 0, idx, score,
+                    bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+}
+int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D,
+                       int k, const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+                       long long* idx, float* score, int* bad_row_flag, int* bad_score_flag, void* workspace,
+                       long long workspace_bytes, void* stream) {
+    NR_REQUIRE(users && news && categories && idx && score && bad_row_flag && bad_score_flag, "nr_topk_dot_capped: null operand");
+    NR_REQUIRE(max_per_category >= 1, "nr_topk_dot_capped: max_per_category=%d below 1", max_per_category);
+    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, categories, max_per_category,
+                    idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
 }
 long long nr_pool_ranks_workspace(long long n_rows, long long n_news, int D) { return pool_ranks_workspace(n_rows, n_news, D); }
 int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,

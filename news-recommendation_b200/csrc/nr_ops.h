@@ -215,11 +215,12 @@ int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int
 // candidates (include/newsrec_b200.h, nr_sample_negatives)
 int sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp, const long long* row_offsets,
                      int K, unsigned long long seed, long long epoch, int* behaviors, int H, cudaStream_t stream);
-// top-k of users . news over a whole pool (topk.cu; include/newsrec_b200.h, nr_topk_dot)
+// top-k of users . news over a whole pool, categories null, or at most max_per_category news of one category key per list
+// (topk.cu; include/newsrec_b200.h, nr_topk_dot and nr_topk_dot_capped)
 long long topk_dot_workspace(long long n_users, long long n_news, int D, int k);
 int topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
-             const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
-             int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
+             const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category, long long* idx,
+             float* score, int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
 // ranks of target news among a whole pool under the same scores (topk.cu; include/newsrec_b200.h, nr_pool_ranks)
 long long pool_ranks_workspace(long long n_rows, long long n_news, int D);
 int pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,

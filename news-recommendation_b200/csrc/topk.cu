@@ -16,6 +16,19 @@
 // never displaces it: "beats" is a strict >, and equal scores keep the lower row.  The matrix of scores never reaches
 // memory; per (user, split) k (score, row) pairs do, and with several splits one small kernel merges them.
 //
+// Diversified lists (nr_topk_dot_capped): the same kernels with kCapped = true; only merge_user and the split merge change.
+// The answer is the walk of the pool in output order that takes a news iff fewer than m taken news share its category and
+// fewer than k are taken.  The sets with at most m news per category and at most k in all are the independent sets of a
+// matroid (a partition matroid truncated to rank k), and the walk is its greedy: it takes x iff x is not spanned by the news
+// ranked above it.  Spans only grow as the ground set grows, so a news the walk rejects over a set S is rejected over every
+// superset of S.  Hence: (1) a merge sorts the buffer, walks it (capped_walk) and may drop every rejected entry for good;
+// (2) once a merge has taken k news, a score that does not beat the k-th taken can never enter (the strict > stays), and
+// while fewer than k are taken the threshold stays -inf; (3) the answer over the pool is contained in the union of the
+// splits' capped lists, so the split merge sorts the union and walks it.  Two caps at once (category and subcategory) are an
+// intersection of two partition matroids, which is not a matroid: a new entry could evict one whose slot then frees up, and
+// (1)-(3) fail, so a call caps one field.  Shared memory is full (kSmem), so no per-entry category is kept: a merge reads
+// categories[row] through the read-only path (the pool's keys stay in L2).
+//
 // Ranks over the pool (nr_pool_ranks): the same planes and the same tile pipeline (DotPlanes, produce_tile, consume_tile), so
 // every score is the bit pattern nr_topk_dot computes for that pair.  The CTA first runs the tiles that hold its rows'
 // targets and reads the target scores out of the fragments; those are the thresholds.  In the main pass a score that does not
@@ -136,6 +149,8 @@ struct Params {
     int* part_row;
     int* bad_row_flag;
     int* bad_score_flag;
+    const int* cat;                 // capped instantiation: [n_news] category keys, at most cap news of one key per list
+    int cap;
 };
 
 // a before b in the output order: higher score, then lower row
@@ -160,8 +175,60 @@ __device__ void warp_sort(float* s, int* r, int n) {
         }
 }
 
-// sorts user buffer u (pads [cnt, kCap) with (-inf, INT_MAX)), keeps the k best, sets the threshold
-__device__ void merge_user(float* bs, int* br, int* cnt, float* thr, int u, int k) {
+// The capped walk, one warp, over n (a multiple of 32) entries in output order, the live ones first (a dead entry has row
+// INT_MAX): an entry is kept iff fewer than m earlier entries share its category and fewer than k entries before it are kept.
+// The kept entries are compacted to the front, in order; returns their number (<= k <= 128).  While fewer than k are kept,
+// a category's kept count is min(m, its earlier entries), so "fewer than m earlier entries" is "fewer than m among the kept
+// entries of earlier chunks and the earlier entries of this chunk": the 32 lanes decide a chunk together, counting the chunk
+// with __match_any_sync and the kept entries by __shfl_sync broadcasts of their categories (kept entry 32 q + l: lane l's
+// kc[q]).  The categories are read through the read-only path (the pool's keys stay in L2).
+__device__ int capped_walk(float* s, int* r, int n, int k, const int* __restrict__ cat, int m) {
+    const int lane = threadIdx.x & 31;
+    const unsigned below = (1u << lane) - 1u;
+    int kc0 = 0, kc1 = 0, kc2 = 0, kc3 = 0;  // kc[q] (scalars: a register array indexed at run time would go to the stack)
+    int kept = 0;
+    for (int c0 = 0; c0 < n && kept < k; c0 += 32) {
+        const float sv = s[c0 + lane];
+        const int rv = r[c0 + lane];
+        const bool live = rv != 0x7fffffff;
+        const unsigned live_mask = __ballot_sync(~0u, live);
+        if (live_mask == 0) break;
+        const int cv = live ? __ldg(cat + rv) : 0;
+        int same = __popc(__match_any_sync(~0u, cv) & live_mask & below);
+        for (int j = 0; j < kept; ++j) {
+            const int q = j >> 5;
+            same += __shfl_sync(~0u, q == 0 ? kc0 : q == 1 ? kc1 : q == 2 ? kc2 : kc3, j & 31) == cv;
+        }
+        const unsigned take = __ballot_sync(~0u, live && same < m);
+        const int nt = min(__popc(take), k - kept);
+        const int pos = kept + __popc(take & below);
+        __syncwarp();  // every lane has read its entry: the kept ones move down to [kept, kept + nt)
+        if (((take >> lane) & 1u) && pos < kept + nt) {
+            s[pos] = sv;
+            r[pos] = rv;
+        }
+        // lane l receives new kept entry kept + t, t = (l - kept) mod 32: the category of the t-th taking lane
+        const int t = (lane - kept) & 31;
+        unsigned rest = take;
+        for (int i = 0; i < t && rest != 0u; ++i) rest &= rest - 1u;
+        const int v = __shfl_sync(~0u, cv, rest != 0u ? __ffs(rest) - 1 : lane);
+        if (t < nt) {
+            const int q = (kept + t) >> 5;
+            if (q == 0) kc0 = v;
+            else if (q == 1) kc1 = v;
+            else if (q == 2) kc2 = v;
+            else kc3 = v;
+        }
+        kept += nt;
+    }
+    __syncwarp();
+    return kept;
+}
+
+// sorts user buffer u (pads [cnt, kCap) with (-inf, INT_MAX)), keeps the k best (capped: the k the capped walk keeps), sets
+// the threshold
+template <bool kCapped>
+__device__ void merge_user(float* bs, int* br, int* cnt, float* thr, int u, int k, const int* cat, int m) {
     const int lane = threadIdx.x & 31;
     float* s = bs + u * kCap;
     int* r = br + u * kCap;
@@ -172,13 +239,20 @@ __device__ void merge_user(float* bs, int* br, int* cnt, float* thr, int u, int 
     }
     __syncwarp();
     warp_sort(s, r, kCap);
-    if (lane == 0) {
+    if constexpr (kCapped) {
+        const int kept = capped_walk(s, r, kCap, k, cat, m);
+        if (lane == 0) {
+            cnt[u] = kept;
+            thr[u] = kept >= k ? s[k - 1] : -INFINITY;
+        }
+    } else if (lane == 0) {
         cnt[u] = min(c, k);
         thr[u] = c >= k ? s[k - 1] : -INFINITY;
     }
     __syncwarp();
 }
 
+template <bool kCapped>
 __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_constant__ CUtensorMap tmUh, const __grid_constant__ CUtensorMap tmUl,
                                                                const __grid_constant__ CUtensorMap tmNh, const __grid_constant__ CUtensorMap tmNl,
                                                                const Params p) {
@@ -267,7 +341,7 @@ __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_cons
         asm volatile("bar.sync 1, 128;" ::: "memory");
         // a buffer that could not take another tile's 64 survivors is merged down to k
         for (int u = warp; u < kUsers; u += 4)
-            if (cnt[u] > kCap - kNews) merge_user(bs, br, cnt, thr, u, p.k);
+            if (cnt[u] > kCap - kNews) merge_user<kCapped>(bs, br, cnt, thr, u, p.k, p.cat, p.cap);
         asm volatile("bar.sync 1, 128;" ::: "memory");
     }
     if (bad_score) atomicOr(p.bad_score_flag, 1);
@@ -275,7 +349,7 @@ __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_cons
     for (int u = warp; u < kUsers; u += 4) {
         const long long ug = u0 + u;
         if (ug >= p.n_users) break;
-        merge_user(bs, br, cnt, thr, u, p.k);
+        merge_user<kCapped>(bs, br, cnt, thr, u, p.k, p.cat, p.cap);
         const float* s = bs + u * kCap;
         const int* r = br + u * kCap;
         const int c = cnt[u];
@@ -294,8 +368,10 @@ __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_cons
     }
 }
 
-// the splits' lists of a user (one warp per user) -> its k best
+// the splits' lists of a user (one warp per user) -> its k best (capped: the union's capped walk, which contains the answer
+// over the whole pool, since every split's list does over its part)
 constexpr int kMergeWarps = 4;
+template <bool kCapped>
 __global__ void __launch_bounds__(kMergeWarps * 32) topk_merge_kernel(const Params p) {
     __shared__ float ss[kMergeWarps][kMaxSplits * 128];
     __shared__ int sr[kMergeWarps][kMaxSplits * 128];
@@ -303,7 +379,7 @@ __global__ void __launch_bounds__(kMergeWarps * 32) topk_merge_kernel(const Para
     const long long u = static_cast<long long>(blockIdx.x) * kMergeWarps + w;
     if (u >= p.n_users) return;
     const int m = p.splits * p.k;
-    int n = 1;
+    int n = kCapped ? 32 : 1;  // the capped walk takes whole 32-entry chunks
     while (n < m) n <<= 1;
     float* s = ss[w];
     int* r = sr[w];
@@ -315,10 +391,18 @@ __global__ void __launch_bounds__(kMergeWarps * 32) topk_merge_kernel(const Para
     }
     __syncwarp();
     warp_sort(s, r, n);
-    for (int j = lane; j < p.k; j += 32) {
-        const bool live = s[j] != -INFINITY;
-        p.idx[u * p.k + j] = live ? r[j] : -1;
-        p.score[u * p.k + j] = s[j];
+    if constexpr (kCapped) {
+        const int kept = capped_walk(s, r, n, p.k, p.cat, p.cap);
+        for (int j = lane; j < p.k; j += 32) {
+            p.idx[u * p.k + j] = j < kept ? r[j] : -1;
+            p.score[u * p.k + j] = j < kept ? s[j] : -INFINITY;
+        }
+    } else {
+        for (int j = lane; j < p.k; j += 32) {
+            const bool live = s[j] != -INFINITY;
+            p.idx[u * p.k + j] = live ? r[j] : -1;
+            p.score[u * p.k + j] = s[j];
+        }
     }
 }
 
@@ -676,9 +760,34 @@ long long topk_dot_workspace(long long n_users, long long n_news, int D, int k) 
     return TopkWorkspace(nullptr, n_users, n_news, D, k, topk_splits(n_users, n_news)).bytes();
 }
 
+// the top-k kernel and, with several splits, the merge: plain or capped (the instantiation's own profile names)
+template <bool kCapped>
+static int topk_launch(const CUtensorMap (&tm)[4], const topk::Params& p, cudaStream_t stream) {
+    using namespace topk;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NR_CHECK_CUDA(cudaFuncSetAttribute(topk_dot_kernel<kCapped>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmem)));
+        attr_set = true;
+    }
+    const long long user_tiles = (p.n_users + kUsers - 1) / kUsers;
+    {
+        ProfScope ps(kCapped ? "topk_dot_capped" : "topk_dot", static_cast<int>(p.n_users), p.n_news, p.k, stream);
+        topk_dot_kernel<kCapped><<<dim3(static_cast<unsigned>(user_tiles), p.splits), kThreads, kSmem, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    if (p.splits > 1) {
+        ProfScope ps(kCapped ? "topk_merge_capped" : "topk_merge", static_cast<int>(p.n_users), p.splits, p.k, stream);
+        topk_merge_kernel<kCapped><<<static_cast<unsigned>((p.n_users + kMergeWarps - 1) / kMergeWarps), kMergeWarps * 32, 0, stream>>>(p);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    return 0;
+}
+
 int topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
-             const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
-             int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+             const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category, long long* idx,
+             float* score, int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
     using namespace topk;
     NR_PROPAGATE(topk_check(n_users, n_news, D, k));
     NR_REQUIRE(ld_users >= D && ld_news >= D, "nr_topk_dot: pitches ld_users=%d ld_news=%d below D=%d", ld_users, ld_news, D);
@@ -688,11 +797,6 @@ int topk_dot(const float* users, long long n_users, int ld_users, const float* n
     NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
                "nr_topk_dot: workspace of %lld bytes (256-byte aligned) needs %lld", workspace_bytes, ws.bytes());
     if (n_users == 0 || n_news == 0) return 0;
-    static bool attr_set = false;
-    if (!attr_set) {
-        NR_CHECK_CUDA(cudaFuncSetAttribute(topk_dot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmem)));
-        attr_set = true;
-    }
     CUtensorMap tm[4];
     NR_PROPAGATE(ws.planes.prepare(users, n_users, ld_users, news, n_news, ld_news, D, tm, stream));
     Params p;
@@ -710,20 +814,9 @@ int topk_dot(const float* users, long long n_users, int ld_users, const float* n
     p.part_row = ws.part_row;
     p.bad_row_flag = bad_row_flag;
     p.bad_score_flag = bad_score_flag;
-    const long long user_tiles = (n_users + kUsers - 1) / kUsers;
-    {
-        ProfScope ps("topk_dot", static_cast<int>(n_users), static_cast<int>(n_news), k, stream);
-        topk_dot_kernel<<<dim3(static_cast<unsigned>(user_tiles), splits), kThreads, kSmem, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
-        ++g_launches;
-        NR_CHECK_CUDA(cudaGetLastError());
-    }
-    if (splits > 1) {
-        ProfScope ps("topk_merge", static_cast<int>(n_users), splits, k, stream);
-        topk_merge_kernel<<<static_cast<unsigned>((n_users + kMergeWarps - 1) / kMergeWarps), kMergeWarps * 32, 0, stream>>>(p);
-        ++g_launches;
-        NR_CHECK_CUDA(cudaGetLastError());
-    }
-    return 0;
+    p.cat = categories;
+    p.cap = max_per_category;
+    return categories != nullptr ? topk_launch<true>(tm, p, stream) : topk_launch<false>(tm, p, stream);
 }
 
 struct RankWorkspace : WorkspaceLayout {

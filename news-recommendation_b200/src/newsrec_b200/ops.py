@@ -7,6 +7,7 @@ arithmetic happens here; `torch.cat`/slicing of parameters is layout plumbing on
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import os
 
 import torch
@@ -594,13 +595,18 @@ def prediction_text(impression_ids, ranks, seg_offsets):
     return text
 
 
-def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None):
+def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categories=None, max_per_category=None):
     """The k best news of every user over the whole pool, one pass (nr_topk_dot): users (U, D) and news (n, D) fp32, scores
     users[u] . news[r] at fp32 level on the tensor cores (the bound is in include/newsrec_b200.h) without the U x n score
     matrix.  Optional exclusions in CSR form: user u never gets rows excl_rows[excl_offsets[u] .. excl_offsets[u + 1]).
     Returns (idx (U, k) int64, score (U, k) fp32) on the caller's stream, best first, equal scores by lower row; slots past
     the eligible news hold -1 / -inf.  Raises NewsrecError on bad arguments (before any launch), IndexError on an exclusion
-    row outside [0, n) and ValueError on a non-finite score (both read device flags: one synchronisation)."""
+    row outside [0, n) and ValueError on a non-finite score (both read device flags: one synchronisation).
+
+    Diversified (nr_topk_dot_capped): with categories ((n,) integer keys, one per news row, any int32 value) and
+    max_per_category = m, each list holds at most m news of one category: the pool is walked in the order above and a news is
+    taken iff fewer than m taken news share its category and fewer than k are taken.  A user gets fewer than k news when the
+    caps run out; m >= k gives the plain answer bit for bit.  The two arguments go together."""
     lib = load_library()
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 128:
         raise NewsrecError(f"top_k_scores: k={k!r} must be an integer in [1, 128]")
@@ -608,6 +614,21 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None):
         raise NewsrecError(f"top_k_scores: users {tuple(users.shape)} and news {tuple(news.shape)} must be (U, D) and (n, D)")
     if (excl_rows is None) != (excl_offsets is None):
         raise NewsrecError("top_k_scores: excl_rows and excl_offsets go together")
+    capped = categories is not None or max_per_category is not None
+    if capped:
+        if categories is None or max_per_category is None:
+            raise NewsrecError("top_k_scores: categories and max_per_category go together")
+        if isinstance(max_per_category, bool) or not isinstance(max_per_category, numbers.Integral) or max_per_category < 1:
+            raise NewsrecError(f"top_k_scores: max_per_category={max_per_category!r} must be an integer >= 1")
+        max_per_category = min(int(max_per_category), k)  # a cap of k or more never binds
+        categories = torch.as_tensor(categories)
+        if categories.dim() != 1 or categories.shape[0] != news.shape[0]:
+            raise NewsrecError(f"top_k_scores: categories {tuple(categories.shape)} must be (n,) = ({news.shape[0]},)")
+        if categories.dtype.is_floating_point or categories.dtype.is_complex or categories.dtype == torch.bool:
+            raise NewsrecError(f"top_k_scores: categories must hold integer keys, not {categories.dtype}")
+        if categories.dtype != torch.int32 and categories.numel() and \
+                (int(categories.min()) < -2 ** 31 or int(categories.max()) >= 2 ** 31):
+            raise NewsrecError("top_k_scores: a category key does not fit in int32")
     dev = require_cuda()
     users = users.to(dev).float().contiguous()
     news = news.to(dev).float().contiguous()
@@ -630,8 +651,14 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None):
     score = torch.empty((U, k), dtype=torch.float32, device=dev)
     flags = torch.zeros(2, dtype=torch.int32, device=dev)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    check(lib.nr_topk_dot(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(idx), _p(score),
-                          _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes, _stream()), "nr_topk_dot")
+    if capped:
+        cat = categories.to(device=dev, dtype=torch.int32).contiguous()
+        check(lib.nr_topk_dot_capped(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(cat),
+                                     max_per_category, _p(idx), _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace),
+                                     ws_bytes, _stream()), "nr_topk_dot_capped")
+    else:
+        check(lib.nr_topk_dot(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(idx), _p(score),
+                              _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes, _stream()), "nr_topk_dot")
     bad_row, bad_score = (int(x) for x in flags.tolist())
     if bad_row:
         raise IndexError("top_k_scores: an exclusion row is outside the news pool")

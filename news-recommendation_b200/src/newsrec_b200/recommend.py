@@ -14,7 +14,14 @@ news without the U x n score matrix ever reaching memory (``ops.top_k_scores``, 
 
 The click predictor must be a dot product of a user vector and a news vector: NRMS, NAML, LSTUR, TANR and Exp1.
 
+Diversified lists: with ``max_per_category=m`` no line holds more than m news of one category (``diversify_by="category"``)
+or of one subcategory (``"subcategory"``), the column of ``news_parsed.tsv`` in the matrix's row order, copied once to the
+device as int32.  The cap is applied inside the kernel (``ops.top_k_scores(..., categories=, max_per_category=)``,
+nr_topk_dot_capped): the pool is walked best first and a news is taken iff fewer than m taken news share its category and
+fewer than k are taken, so a line can be shorter than k when the caps run out.  One field per call.
+
     python -m newsrec_b200.recommend --directory data/test --out recommendations.tsv [--k 10] [--keep-clicked]
+                                     [--max-per-category M [--diversify-by {category,subcategory}]]
                                      [--checkpoint PATH | --checkpoint-dir DIR] [--user2int data/train/user2int.tsv]
                                      [--chunk-users N] [--set KNOB=VALUE ...]
 """
@@ -30,6 +37,7 @@ from .evaluate import distinct_histories, new_flag, news_matrix, read_behaviors,
 
 DEFAULT_CHUNK = 65536
 MAX_K = 128
+DIVERSIFY_FIELDS = ("category", "subcategory")
 # Families whose click score is not users . news: Hi-Fi Ark's depends on the candidate through the similarity attention over
 # the user's archive; DKN's DNN scorer is separable (w2 . relu(W1c c + W1u u + b1)) but is not a single dot product.
 _REFUSED = {
@@ -39,17 +47,28 @@ _REFUSED = {
 }
 
 
-def check_request(model, directory, k):
-    """Everything recommend() refuses, checked before any device work: k outside [1, 128], a family whose click predictor is
-    not a dot product, a split without behaviors.tsv or news_parsed.tsv."""
+def check_request(model, directory, k, max_per_category=None, diversify_by="category"):
+    """Everything recommend() refuses, checked before any device work: k outside [1, 128], a cap that is not an integer >= 1,
+    a diversify_by other than "category" / "subcategory", a family whose click predictor is not a dot product, a split
+    without behaviors.tsv or news_parsed.tsv, and (with a cap) a news_parsed.tsv without the diversify_by column."""
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= MAX_K:
         raise NewsrecError(f"recommend: k={k!r} must be an integer in [1, {MAX_K}]")
+    if max_per_category is not None and (isinstance(max_per_category, bool) or
+                                         not isinstance(max_per_category, (int, np.integer)) or max_per_category < 1):
+        raise NewsrecError(f"recommend: max_per_category={max_per_category!r} must be an integer >= 1")
+    if diversify_by not in DIVERSIFY_FIELDS:
+        raise NewsrecError(f"recommend: diversify_by={diversify_by!r} must be one of {DIVERSIFY_FIELDS}")
     name = type(model).__name__
     if name in _REFUSED:
         raise NewsrecError(f"recommend: {name} is not supported: {_REFUSED[name]}")
     for f in ("behaviors.tsv", "news_parsed.tsv"):
         if not os.path.isfile(os.path.join(directory, f)):
             raise FileNotFoundError(f"recommend: {os.path.join(directory, f)} not found")
+    if max_per_category is not None:
+        with open(os.path.join(directory, "news_parsed.tsv")) as f:
+            header = f.readline().rstrip("\r\n").split("\t")
+        if diversify_by not in header:
+            raise NewsrecError(f"recommend: {os.path.join(directory, 'news_parsed.tsv')} has no {diversify_by} column")
 
 
 def exclusion_csr(history, pad):
@@ -79,13 +98,14 @@ class _Users:
 
 
 def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2int_path="data/train/user2int.tsv",
-              chunk_users=DEFAULT_CHUNK) -> int:
+              chunk_users=DEFAULT_CHUNK, max_per_category=None, diversify_by="category") -> int:
     """Write the k best news of the pool for every distinct history of directory/behaviors.tsv to out_path; returns the
     number of lines.  Runs under torch.no_grad() on the model as given (call .eval() first).  The file appears only when
-    every line is written; a non-finite score raises ValueError, a history row outside the news table IndexError."""
+    every line is written; a non-finite score raises ValueError, a history row outside the news table IndexError.  With
+    max_per_category=m a line holds at most m news of one diversify_by value (module docstring)."""
     import torch
     from .ops import top_k_scores
-    check_request(model, directory, k)
+    check_request(model, directory, k, max_per_category, diversify_by)
     if chunk_users < 1:
         raise ValueError(f"recommend: chunk_users={chunk_users}")
     with torch.no_grad():
@@ -96,6 +116,13 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
         user_ids = distinct_histories(beh)["user"].tolist()
         user, history, length, _ = user_tables(beh, news_index, model.config.num_clicked_news_a_user, user2int_path)
         pool = matrix[:pad]
+        cap = {}
+        if max_per_category is not None:
+            keys = read_news(directory, [diversify_by])[1][diversify_by]
+            if len(keys) and (keys.min() < -2 ** 31 or keys.max() >= 2 ** 31):
+                raise NewsrecError(f"recommend: a {diversify_by} id does not fit in int32")
+            cap = dict(categories=torch.from_numpy(keys.astype(np.int32)).to(matrix.device),
+                       max_per_category=int(max_per_category))
         U = len(user)
         flag = new_flag(matrix.device)
         tmp = f"{out_path}.partial"
@@ -108,7 +135,7 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
                     if exclude_clicked:
                         rows, offsets = exclusion_csr(history[a:b], pad)
                         excl = torch.from_numpy(rows), torch.from_numpy(offsets)
-                    idx, _ = top_k_scores(users, pool, int(k), *excl)  # reads its flags: synchronises
+                    idx, _ = top_k_scores(users, pool, int(k), *excl, **cap)  # reads its flags: synchronises
                     if int(flag.item()):
                         raise IndexError("recommend: a history row is outside the news table")
                     f.write(format_lines(user_ids[a:b], idx.cpu().numpy(), news_ids))
@@ -129,6 +156,10 @@ def parse_args(argv=None):
     g.add_argument("--checkpoint", help="a checkpoint file (a dict with model_state_dict, as the trainer saves)")
     g.add_argument("--checkpoint-dir", help="load its latest ckpt-<n>.pth (default: ./checkpoint/<MODEL_NAME>)")
     ap.add_argument("--keep-clicked", action="store_true", help="let a user's clicked news be recommended back")
+    ap.add_argument("--max-per-category", type=int, default=None, metavar="M",
+                    help="at most M news of one category (see --diversify-by) per line")
+    ap.add_argument("--diversify-by", choices=DIVERSIFY_FIELDS, default="category",
+                    help="the news_parsed.tsv column --max-per-category caps")
     ap.add_argument("--user2int", default="./data/train/user2int.tsv")
     ap.add_argument("--chunk-users", type=int, default=DEFAULT_CHUNK, help="users scored per device pass")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
@@ -138,6 +169,8 @@ def parse_args(argv=None):
         ap.error(f"--k must be in [1, {MAX_K}]")
     if args.chunk_users < 1:
         ap.error("--chunk-users must be at least 1")
+    if args.max_per_category is not None and args.max_per_category < 1:
+        ap.error("--max-per-category must be at least 1")
     return args
 
 
@@ -146,8 +179,9 @@ def main(argv=None):
     args = parse_args(argv)
     name, path, model = load_model(args.checkpoint, args.checkpoint_dir, args.set)
     n = recommend(model, args.directory, args.out, args.k, exclude_clicked=not args.keep_clicked, user2int_path=args.user2int,
-                  chunk_users=args.chunk_users)
-    print(f"{name} from {path}: top {args.k} news of {n} users written to {args.out}")
+                  chunk_users=args.chunk_users, max_per_category=args.max_per_category, diversify_by=args.diversify_by)
+    cap = "" if args.max_per_category is None else f" (at most {args.max_per_category} per {args.diversify_by})"
+    print(f"{name} from {path}: top {args.k} news{cap} of {n} users written to {args.out}")
     return 0
 
 

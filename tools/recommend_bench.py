@@ -3,7 +3,13 @@ D = 300 as NRMS's), against chunked torch.matmul in fp32 (TF32 off) + torch.topk
 alternately in the same run.  The baseline's answer also cross-checks the kernel's: every returned score within the bound of
 include/newsrec_b200.h of the fp32 product, and the set equal up to news within twice the bound of the k-th best.
 
+Diversified lists (--max-per-category M): every news gets a synthetic category, drawn from --categories N keys with
+probability proportional to 1 / rank^s (--zipf s; 0 is uniform), and nr_topk_dot_capped is timed against the plain
+nr_topk_dot at the same k, the two alternating in the same run (no matmul baseline).  The sampled users' capped lists are
+checked: no category over M, scores within the bound, and with M >= k the plain lists bit for bit.
+
     python tools/recommend_bench.py [--users 700000] [--news 120000] [--dim 300] [--k 10 100] [--reps 3] [--seed 0]
+                                    [--max-per-category M [--categories 17] [--zipf 0]]
 
 Time: CUDA events around the library's launches (operand planes, the top-k kernel, the split merge when there is one), after
 a warm-up, best and median over reps.  Rates: multiply-adds of the three bf16 products per score (3 n_users n_news
@@ -40,7 +46,13 @@ def main(argv=None):
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--baseline-chunk", type=int, default=8192, help="users per torch.matmul + torch.topk pass")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--max-per-category", type=int, default=None, metavar="M",
+                    help="time nr_topk_dot_capped with this cap against nr_topk_dot")
+    ap.add_argument("--categories", type=int, default=17, help="synthetic category keys (with --max-per-category)")
+    ap.add_argument("--zipf", type=float, default=0.0, help="Zipf exponent of the category draw, 0: uniform")
     a = ap.parse_args(argv)
+    if a.max_per_category is not None and (a.max_per_category < 1 or a.categories < 1):
+        ap.error("--max-per-category and --categories must be at least 1")
     import torch
     from newsrec_b200 import require_cuda
     from newsrec_b200.ops import top_k_scores
@@ -50,6 +62,8 @@ def main(argv=None):
     users = torch.randn(a.users, a.dim, device=dev, generator=g)
     news = torch.randn(a.news, a.dim, device=dev, generator=g)
     print(f"card: {card()}", flush=True)
+    if a.max_per_category is not None:
+        return capped(a, users, news, dev)
 
     def kernel(k):
         return top_k_scores(users, news, k)
@@ -104,6 +118,60 @@ def main(argv=None):
               f"{score_ok and set_ok}; same set as fp32 for {same:.3f} of the sampled users", flush=True)
         results.append(r)
     print(json.dumps(dict(card=card(), users=a.users, news=a.news, dim=a.dim, reps=a.reps, results=results)))
+    return 0
+
+
+def capped(a, users, news, dev):
+    """nr_topk_dot_capped against nr_topk_dot, alternating, at every k; prints one line per k and the JSON line."""
+    import torch
+    from newsrec_b200.ops import top_k_scores
+    g = torch.Generator(device=dev).manual_seed(a.seed + 1)
+    p = 1.0 / torch.arange(1, a.categories + 1, device=dev, dtype=torch.float64) ** a.zipf
+    cat = torch.multinomial(p / p.sum(), a.news, replacement=True, generator=g).int()
+    m = a.max_per_category
+    Dp = (a.dim + 63) // 64 * 64
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        out = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1), out
+
+    results = []
+    for k in a.k:
+        run_c = lambda: top_k_scores(users, news, k, categories=cat, max_per_category=m)  # noqa: E731
+        run_p = lambda: top_k_scores(users, news, k)  # noqa: E731
+        run_c(), run_p()  # warm-up
+        tc, tp = [], []
+        for _ in range(a.reps):
+            t, (ci, cs) = timed(run_c)
+            tc.append(t)
+            t, (pi, ps) = timed(run_p)
+            tp.append(t)
+        rows = torch.linspace(0, a.users - 1, 2000, device=dev).long()
+        live = ci[rows] >= 0
+        r = ci[rows].clamp(min=0)
+        u64, n64 = users[rows].double(), news.double()
+        s_k = (u64[:, None, :] * n64[r]).sum(-1)
+        e_k = (2.0 ** -15 + 3 * Dp * 2.0 ** -23) * (u64.abs()[:, None, :] * n64[r].abs()).sum(-1)
+        score_ok = bool(((cs[rows].double() - s_k).abs() <= e_k)[live].all())
+        c = torch.where(live, cat[r].long(), -1 - torch.arange(k, device=dev))  # dead slots: distinct keys
+        per_cat = (c[:, :, None] == c[:, None, :]).sum(-1)
+        caps_ok = bool((per_cat[live] <= m).all())
+        plain_ok = bool(torch.equal(ci, pi) and torch.equal(cs, ps)) if m >= k else None
+        mc, mp = sorted(tc)[len(tc) // 2], sorted(tp)[len(tp) // 2]
+        res = dict(k=k, capped_ms_best=min(tc), capped_ms_median=mc, plain_ms_best=min(tp), plain_ms_median=mp,
+                   capped_over_plain=mc / mp, mean_returned=float((ci >= 0).sum(1).float().mean()),
+                   scores_within_bound=score_ok, caps_obeyed=caps_ok, equal_to_plain=plain_ok)
+        print(f"k={k} m={m} over {a.categories} categories (zipf {a.zipf}): nr_topk_dot_capped {mc:.1f} ms (best "
+              f"{min(tc):.1f}), nr_topk_dot {mp:.1f} ms (best {min(tp):.1f}), {mc / mp:.2f}x; "
+              f"{res['mean_returned']:.1f} news per user; checks {score_ok and caps_ok and plain_ok is not False}", flush=True)
+        results.append(res)
+    print(json.dumps(dict(card=card(), users=a.users, news=a.news, dim=a.dim, reps=a.reps, max_per_category=m,
+                          categories=a.categories, zipf=a.zipf, results=results)))
     return 0
 
 
