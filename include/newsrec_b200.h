@@ -333,7 +333,8 @@ typedef struct {
     unsigned long long seed;
     /* outputs; X/QKV/C/w are what backward needs (the caller keeps them alive) */
     void* X_bf16;             /* [n_seq*T][ldx]                                                     */
-    void* QKV_bf16;           /* [n_seq*T][ld3]                                                     */
+    void* QKV_bf16;           /* [n_seq*T][ld3]; the accurate news variant leaves the rows of 64-row tiles that hold only
+                                 padding titles (all ids 0, zero table row 0) unwritten, and V_lo_bf16 likewise            */
     void* C_bf16;             /* [n_seq*T][ldx]                                                     */
     float* w;                 /* [n_seq*T] additive-attention weights                               */
     float* out;               /* [n_seq][d] fp32                                                    */
@@ -385,7 +386,7 @@ typedef struct {
     long long workspace_bytes;
     /* QKV_bf16 == NULL (the precise dense forward keeps no bf16 Q|K|V): recomputed here from X_bf16 with these operands */
     const void* wqkv_bf16;               /* [3*sec][ldx] (sectioned, as in the forward arguments)        */
-    const float* bqkv;                   /* [3*sec]                                                      */
+    const float* bqkv;                   /* [3*sec]; also required by the ids variant: the Q|K|V of its padding titles */
     /* optional cudaEvent_t recorded on `stream` as soon as demb is complete (before the weight-gradient GEMM): a data-
      * parallel caller starts the embedding-gradient all-reduce on a side stream that waits for it */
     void* emb_grad_ready_event;

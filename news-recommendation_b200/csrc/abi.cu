@@ -305,6 +305,13 @@ int nr_mhsa_accurate_supported(int T, int d, int heads) {
     return mhsa_accurate_shape(T, d, heads, (3 * qkv_section(d) + 15) & ~15, (d + 8) & ~7) ? 1 : 0;
 }
 
+// the padding-title buffers of one encoder call, released (stream-ordered) on every way out of it
+struct PaddingScope {
+    PaddingTitles pt;
+    cudaStream_t st;
+    ~PaddingScope() { free_padding_titles(pt, st); }
+};
+
 // the dense input rows [n_seq][T][d] (+ dense_pos) with the ones column at d, as the hi plane of pitch ld_hi
 static Bf16Rows dense_rows(const nr_mhsa_encoder_fwd_args* a, void* hi, int ld_hi) {
     return {.src = a->dense, .n_rows = a->n_seq * a->T, .T = a->T, .D = a->d, .s_seq = a->dense_s_seq, .s_tok = a->dense_s_tok,
@@ -356,13 +363,17 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
                    "chunk-aligned V section (d=%d); see nr_mhsa_accurate_supported", a->d);
         NR_PROPAGATE(gather_rows(a->ids, M, a->T, a->table_bf16, a->V, a->d, a->ldx, a->X_bf16, a->ldx, 0,
                                  DropoutCfg{a->p_drop, a->seed}, a->bad_id_flag, st));
+        // padding titles (all ids 0, zero table row 0; ~45 % of a batch of left-padded histories) share one Q|K|V tile: the
+        // projection computes only the live 64-row tiles, and the attention reads the shared tile for every padding title
+        PaddingScope pad{.st = st};
+        NR_PROPAGATE(padding_titles(a->ids, a->n_seq, a->T, a->d, a->table_bf16, a->ldx, 0, a->bqkv, sec, a->ld3, &pad.pt, st));
         NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
                                 {.out = a->QKV_bf16, .ld_out = a->ld3, .out_bf16 = 1, .bias = a->bqkv, .lo_out = a->V_lo_bf16, .ld_lo = sec,
-                                 .lo_col0 = 2 * sec}, st));
+                                 .lo_col0 = 2 * sec, .tile_list = pad.pt.live}, st));
         {
             ProfScope ps("mhsa_core_fwd_hilo", static_cast<int>(a->n_seq), a->T, a->d, st);
             NR_PROPAGATE(mhsa_title_fwd(a->QKV_bf16, a->ld3, sec, a->n_seq, a->heads, a->C_bf16, a->ldx, context_dropout(a->p_drop, a->seed), st,
-                                        a->V_lo_bf16, sec, a->C_lo_bf16));
+                                        a->V_lo_bf16, sec, a->C_lo_bf16, &pad.pt));
         }
         NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
                                         a->w, st, a->C_lo_bf16));
@@ -412,6 +423,7 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     NR_REQUIRE((a->ids != nullptr) ? (a->demb != nullptr) : (a->ddense != nullptr),
                "nr_mhsa_encoder_bwd: missing input-gradient buffer");
     NR_REQUIRE(a->dpos == nullptr || a->ids == nullptr, "nr_mhsa_encoder_bwd: dpos needs the dense (user-level) variant");
+    NR_REQUIRE(a->ids == nullptr || a->bqkv != nullptr, "nr_mhsa_encoder_bwd: the news variant needs bqkv (Q|K|V of its padding titles)");
     const MhsaBwdWorkspace ws(a->workspace, a->n_seq * a->T, a->d, a->q);
     NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_mhsa_encoder_bwd: workspace too small (%lld bytes)", a->workspace_bytes);
     if (a->n_seq == 0) return 0;
@@ -434,7 +446,14 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
                                   {.w = a->w, .dout = a->dout, .ldo = a->d, .seg_len = a->T, .dx = ws.dC, .ld_dx = a->ldx,
                                    .drop = context_dropout(a->ids != nullptr ? a->p_drop : 0.f, a->seed)}, st));
     // --- attention backward ---
-    NR_PROPAGATE(mhsa_core_bwd(QKV, a->ld3, sec, ws.dC, a->ldx, a->n_seq, a->T, a->heads, a->d / a->heads, ws.dQKV, a->ld3, st));
+    // padding titles (all ids 0 and zero rows in X): the attention reads their Q|K|V from the shared bias tile (the accurate
+    // forward left their rows unwritten), and the weight gradient skips the tiles that hold nothing else
+    PaddingScope pad{.st = st};
+    const bool title_bwd = mhsa_title_bwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx, a->ld3);
+    if (a->ids != nullptr && title_bwd)
+        NR_PROPAGATE(padding_titles(a->ids, a->n_seq, a->T, a->d, a->X_bf16, a->ldx, 1, a->bqkv, sec, a->ld3, &pad.pt, st));
+    NR_PROPAGATE(mhsa_core_bwd(QKV, a->ld3, sec, ws.dC, a->ldx, a->n_seq, a->T, a->heads, a->d / a->heads, ws.dQKV, a->ld3, st,
+                               pad.pt.pad != nullptr ? &pad.pt : nullptr));
     // --- projection backward: the input first (the embedding gradient is 97 % of a data-parallel step's all-reduce: the
     //     caller's event lets the communication start under the weight-gradient GEMM), then the weights (+bias through the
     //     ones column of X) ---
@@ -452,7 +471,9 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     // both weight-gradient GEMMs run AFTER the embedding gradient is complete: together they are the window (~0.4 ms) under which
     // the caller's all-reduce of that gradient hides
     NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, a->q, a->ldq, a->C_bf16, a->d, a->ldx, a->dWa_ext, st));
-    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st));
+    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st, 0, pad.pt.live));
+    // the skipped tiles' rows of X are [0 .. 0, 1]: their whole term is their dQ|dK|dV column sums in the bias column
+    if (pad.pt.live != nullptr) NR_PROPAGATE(dead_tiles_colsum(ws.dQKV, a->ld3, 3 * sec, M, pad.pt.tile_flags, a->dWqkv_ext + a->d, a->ldx, st));
     return 0;
 }
 

@@ -61,13 +61,14 @@ struct Params {
     uint32_t out_stage;   // == qkv_tile
     uint32_t tx;          // bytes one stage's two boxes deliver
     float rs, sc;         // 1/sqrt(dk), log2(e)/sqrt(dk)
+    const unsigned char* pad;  // PaddingTitles::pad or null
 };
 
 __device__ __forceinline__ uint32_t sel(bool keep, uint32_t v) { return keep ? v : 0u; }
 
 __global__ void __launch_bounds__((kMaxHeads + 1) * 32, 1)
 mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_dc,
-                      const __grid_constant__ CUtensorMap tm_out, const Params p) {
+                      const __grid_constant__ CUtensorMap tm_out, const __grid_constant__ CUtensorMap tm_pad, const Params p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     uint8_t* const base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -104,11 +105,13 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
             tma_prefetch_desc(&tm_qkv);
             tma_prefetch_desc(&tm_dc);
             tma_prefetch_desc(&tm_out);
+            if (p.pad != nullptr) tma_prefetch_desc(&tm_pad);
             auto load = [&](int it) {
                 const int s = it % kIn;
-                const int row = (static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x)) * kT;
+                const int title = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x), row = title * kT;
+                const bool pad = p.pad != nullptr && p.pad[title] != 0;  // a padding title reads the shared bias tile
                 mbar_arrive_expect_tx(&full[s], p.tx);
-                tma_load_2d(base_ptr + s * p.in_stage, &tm_qkv, &full[s], 0, row);
+                tma_load_2d(base_ptr + s * p.in_stage, pad ? &tm_pad : &tm_qkv, &full[s], 0, pad ? 0 : row);
                 tma_load_2d(base_ptr + s * p.in_stage + p.qkv_tile, &tm_dc, &full[s], 0, row);
             };
             for (int it = 0; it < kIn && it < n_my; ++it) load(it);
@@ -359,12 +362,14 @@ struct FwdParams {
     uint32_t sec2, pq, pc, pv, qkv_tile, in_stage, out_tile, out_stage, tx;
     float sc;
     Dropout drop;
+    const unsigned char* pad;  // PaddingTitles::pad or null
 };
 
 template <bool HILO>
 __global__ void __launch_bounds__((kMaxHeads + 1) * 32, HILO ? 1 : 2)
 mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_vlo,
-                      const __grid_constant__ CUtensorMap tm_ctx, const __grid_constant__ CUtensorMap tm_clo, const FwdParams p) {
+                      const __grid_constant__ CUtensorMap tm_ctx, const __grid_constant__ CUtensorMap tm_clo,
+                      const __grid_constant__ CUtensorMap tm_pad, const __grid_constant__ CUtensorMap tm_padlo, const FwdParams p) {
     constexpr int kIn = HILO ? kInHilo : title::kIn;  // input stages (one CTA per SM in the hi/lo variant, two otherwise)
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
@@ -405,12 +410,18 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                 tma_prefetch_desc(&tm_vlo);
                 tma_prefetch_desc(&tm_clo);
             }
+            if (p.pad != nullptr) {
+                tma_prefetch_desc(&tm_pad);
+                if (HILO) tma_prefetch_desc(&tm_padlo);
+            }
             auto load = [&](int it) {
                 const int s = it % kIn;
-                const int row = (static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x)) * kT;
+                const int title = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
+                const bool pad = p.pad != nullptr && p.pad[title] != 0;  // a padding title reads the shared bias tile
+                const int row = pad ? 0 : title * kT;
                 mbar_arrive_expect_tx(&full[s], p.tx);
-                tma_load_2d(base_ptr + s * p.in_stage, &tm_qkv, &full[s], 0, row);
-                if (HILO) tma_load_2d(base_ptr + s * p.in_stage + p.qkv_tile, &tm_vlo, &full[s], 0, row);
+                tma_load_2d(base_ptr + s * p.in_stage, pad ? &tm_pad : &tm_qkv, &full[s], 0, row);
+                if (HILO) tma_load_2d(base_ptr + s * p.in_stage + p.qkv_tile, pad ? &tm_padlo : &tm_vlo, &full[s], 0, row);
             };
             for (int it = 0; it < kIn && it < n_my; ++it) load(it);
             for (int j = 0; j < n_my; ++j) {
@@ -625,7 +636,7 @@ bool mhsa_title_bwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int
 }
 
 int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int heads, void* dqkv,
-                   int ld_dqkv, cudaStream_t stream) {
+                   int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad) {
     using namespace title;
     NR_REQUIRE(mhsa_title_bwd_supported(kT, kDk, heads, sec, ld_qkv, ld_dctx, ld_dqkv), "mhsa_title_bwd: unsupported layout");
     NR_REQUIRE(n_seq * kT < (1ll << 31), "mhsa_title_bwd: too many rows");
@@ -645,21 +656,27 @@ int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int l
     p.tx = kT * p.pq + kT * p.pc;
     p.rs = 1.0f / sqrtf(static_cast<float>(kDk));
     p.sc = p.rs * 1.4426950408889634f;
+    NR_REQUIRE(pad == nullptr || (pad->pad != nullptr && pad->qkv != nullptr), "mhsa_title_bwd: padding titles without their Q|K|V tile");
+    p.pad = pad != nullptr ? pad->pad : nullptr;
     const size_t smem = 128 + static_cast<size_t>(kIn) * p.in_stage + static_cast<size_t>(kOut) * p.out_stage +
                        static_cast<size_t>(heads) * kScrWarp + (2 * kIn + 2 * kOut) * sizeof(uint64_t) + 64;
     NR_REQUIRE(smem <= 227 * 1024, "mhsa_title_bwd: %zu bytes of shared memory", smem);
     const long long rows = n_seq * kT;
-    CUtensorMap tq, tc, to;
+    CUtensorMap tq, tc, to, tp;
     NR_PROPAGATE(make_tmap_bytes_2d(&tq, qkv, rows, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
     NR_PROPAGATE(make_tmap_bytes_2d(&tc, dctx, rows, dc_row, static_cast<int64_t>(ld_dctx) * 2, static_cast<int>(p.pc), kT));
     NR_PROPAGATE(make_tmap_bytes_2d(&to, dqkv, rows, qkv_row, static_cast<int64_t>(ld_dqkv) * 2, static_cast<int>(p.pq), kT));
+    if (pad != nullptr)
+        NR_PROPAGATE(make_tmap_bytes_2d(&tp, pad->qkv, kT, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
+    else
+        tp = tq;
     static bool attr_set = false;
     if (!attr_set) {
         NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_title_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
     const int grid = static_cast<int>(std::min<long long>(n_seq, num_sms()));
-    mhsa_title_bwd_kernel<<<grid, (heads + 1) * 32, smem, stream>>>(tq, tc, to, p);
+    mhsa_title_bwd_kernel<<<grid, (heads + 1) * 32, smem, stream>>>(tq, tc, to, tp, p);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -675,7 +692,7 @@ bool mhsa_title_fwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int
 // v_lo / ctx_lo both non-null: the accurate (hi/lo) variant.  v_lo bf16 [rows][ld_vlo] = low plane of the V section (column 0
 // = first V column); ctx_lo bf16 [rows][ld_ctx] = low plane of the context (no ones column).
 int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int heads, void* ctx, int ld_ctx, DropoutCfg drop,
-                   cudaStream_t stream, const void* v_lo, int ld_vlo, void* ctx_lo) {
+                   cudaStream_t stream, const void* v_lo, int ld_vlo, void* ctx_lo, const PaddingTitles* pad) {
     using namespace title;
     NR_REQUIRE(mhsa_title_fwd_supported(kT, kDk, heads, sec, ld_qkv, ld_ctx), "mhsa_title_fwd: unsupported layout");
     NR_REQUIRE(n_seq * kT < (1ll << 31), "mhsa_title_fwd: too many rows");
@@ -699,6 +716,9 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
     p.tx = kT * p.pq + (hilo ? kT * p.pv : 0u);
     p.sc = 1.4426950408889634f / sqrtf(static_cast<float>(kDk));
     p.drop = Dropout::make(drop.p, drop.seed);
+    NR_REQUIRE(pad == nullptr || (pad->pad != nullptr && pad->qkv != nullptr && (!hilo || (pad->v_lo != nullptr && ld_vlo == sec))),
+               "mhsa_title_fwd: padding titles without their Q|K|V tile (or its V low plane at pitch sec)");
+    p.pad = pad != nullptr ? pad->pad : nullptr;
     // fragment loads of rows 20..23 of a tile run into whatever follows it (the low-plane tile, the next stage, the result
     // tiles): always inside the allocation, always initialised
     const int n_in = hilo ? kInHilo : kIn;
@@ -707,7 +727,7 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
     const size_t cap = hilo ? 227 * 1024 : 113 * 1024;
     NR_REQUIRE(smem <= cap, "mhsa_title_fwd: %zu bytes of shared memory", smem);
     const long long rows = n_seq * kT;
-    CUtensorMap tq, tc, tv, tl;
+    CUtensorMap tq, tc, tv, tl, tp, tpl;
     NR_PROPAGATE(make_tmap_bytes_2d(&tq, qkv, rows, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
     NR_PROPAGATE(make_tmap_bytes_2d(&tc, ctx, rows, ctx_row, static_cast<int64_t>(ld_ctx) * 2, static_cast<int>(p.pc), kT));
     if (hilo) {
@@ -717,6 +737,12 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
         tv = tq;
         tl = tc;
     }
+    tp = tq;
+    tpl = tv;
+    if (pad != nullptr) {
+        NR_PROPAGATE(make_tmap_bytes_2d(&tp, pad->qkv, kT, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
+        if (hilo) NR_PROPAGATE(make_tmap_bytes_2d(&tpl, pad->v_lo, kT, vlo_row, static_cast<int64_t>(ld_vlo) * 2, static_cast<int>(p.pv), kT));
+    }
     static bool attr_set = false;
     if (!attr_set) {
         NR_CHECK_CUDA(cudaFuncSetAttribute(mhsa_title_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 113 * 1024));
@@ -725,9 +751,9 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
     }
     const int grid = static_cast<int>(std::min<long long>(n_seq, (hilo ? 1ll : 2ll) * num_sms()));
     if (hilo)
-        mhsa_title_fwd_kernel<true><<<grid, (heads + 1) * 32, smem, stream>>>(tq, tv, tc, tl, p);
+        mhsa_title_fwd_kernel<true><<<grid, (heads + 1) * 32, smem, stream>>>(tq, tv, tc, tl, tp, tpl, p);
     else
-        mhsa_title_fwd_kernel<false><<<grid, (heads + 1) * 32, smem, stream>>>(tq, tv, tc, tl, p);
+        mhsa_title_fwd_kernel<false><<<grid, (heads + 1) * 32, smem, stream>>>(tq, tv, tc, tl, tp, tpl, p);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

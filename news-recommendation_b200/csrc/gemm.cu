@@ -331,9 +331,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint64_t* empty = bars + kMaxStages;
 
     const int mt = blockIdx.x, nt = blockIdx.y, ks = blockIdx.z;  // a cluster spans (m-tile, n-tile) pairs of one k-range
-    const int total_chunks = (p.Kr + 63) >> 6;
-    const int chunk0 = ks * p.chunks_per_slice;
-    const int n_my = max(0, min(p.chunks_per_slice, total_chunks - chunk0));
+    // with a chunk list the k-ranges split the listed chunks evenly (the count is known on the device only)
+    const int total_chunks = p.k_list != nullptr ? p.k_list[0] : (p.Kr + 63) >> 6;
+    const int per_slice = p.k_list != nullptr ? (total_chunks + p.k_slices - 1) / p.k_slices : p.chunks_per_slice;
+    const int chunk0 = ks * per_slice;
+    const int n_my = max(0, min(per_slice, total_chunks - chunk0));
     const int n0 = nt * NT;                       // first output column of this CTA
     const int ncol = min(NT, p.Nb - n0);
     // cluster rank cx + cluster_m * cy; the A chunk of this m-tile goes to the ranks of column cx, the B chunk of this n-tile to
@@ -367,7 +369,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         int st = 0;
         uint32_t ph = 0;
         for (int c = 0; c < n_my; ++c) {
-            const int k0 = (chunk0 + c) * 64;
+            const int k0 = (p.k_list != nullptr ? p.k_list[1 + chunk0 + c] : chunk0 + c) * 64;
             mbar_wait(&empty[st], ph ^ 1, clustered ? 203 : 201);
             if (elect_one()) {
                 mbar_arrive_expect_tx(&full[st], static_cast<uint32_t>(stage_bytes));
@@ -532,7 +534,7 @@ static int launch_gemm_tn_kernel(int sms, int total_chunks, size_t smem, const C
 }
 
 int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, int b_rows, int b_cols, int ldb,
-                       int b_col0, int Nb, int b_row_shift, float* D, int ldd, cudaStream_t stream) {
+                       int b_col0, int Nb, int b_row_shift, float* D, int ldd, cudaStream_t stream, const int* k_list) {
     NR_REQUIRE(Nb >= 1 && Nb <= 512 && Ma >= 1 && Kr >= 0, "gemm_tn: bad shape Kr=%d Ma=%d Nb=%d", Kr, Ma, Nb);
     if (Kr == 0) return 0;
     GemmTNParams p;
@@ -544,6 +546,7 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     p.b_row_shift = b_row_shift;
     p.D = D;
     p.ldd = ldd;
+    p.k_list = k_list;
     ProfScope ps("gemm_tn", Kr, Ma, Nb, stream);
 #ifdef NEWSREC_TRIAGE
     if (debug_simt_gemm()) {
@@ -584,9 +587,11 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
     return 0;
 }
 
-int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int K, int ldx, float* dW_ext, cudaStream_t stream, int x_row_shift) {
+int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int K, int ldx, float* dW_ext, cudaStream_t stream, int x_row_shift,
+                     const int* k_list) {
     for (int c0 = 0; c0 < K + 1; c0 += 512)
-        NR_PROPAGATE(gemm_tn_accumulate(dY, M, N, ld_dy, X, M, K + 1, ldx, c0, std::min(512, K + 1 - c0), x_row_shift, dW_ext + c0, ldx, stream));
+        NR_PROPAGATE(gemm_tn_accumulate(dY, M, N, ld_dy, X, M, K + 1, ldx, c0, std::min(512, K + 1 - c0), x_row_shift, dW_ext + c0, ldx, stream,
+                                        k_list));
     return 0;
 }
 
@@ -624,6 +629,8 @@ int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream) {
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, M, g.lda, g.W, N, g.ldw, g.K, g.taps, g.w_tap_rows, rows_per_tile, num_sms(), 0,
                               kEpiSmemBytes<EpiStore>, 0));
     NR_PROPAGATE(apply_tap_origin(plan, g));
+    NR_REQUIRE(c.tile_list == nullptr || rows_per_tile == kTileM, "gemm_store: a tile list needs whole 64-row tiles");
+    plan.p.tile_list = c.tile_list;
     NR_REQUIRE(c.out_bf16 ? (c.ld_out % 8 == 0) : (c.ld_out % 4 == 0), "gemm_store: output pitch %d breaks vector stores", c.ld_out);
     // the ones column is written by slice 0's CTA with plain stores after its chunk loop: only past the result columns (a chunk
     // of another slice, or one of its own TMA stores still in flight, would race with it) and only inside the row's pitch
@@ -782,30 +789,11 @@ int gemm_pool_dinput(const GemmOperands& g, const PoolDInputCfg& c, cudaStream_t
     return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
 }
 
-// The tiles of the embedding-gradient GEMM that scatter something: tile t (rows [64t, 64t + 64) of M) is live when one of its
-// rows maps through rm to a token whose id is in [1, V) -- EpiScatter's own test, so a dead tile would add nothing.  Padded
-// histories make runs of all-padding tiles (about 40 % of the NRMS batch), whose A loads and MMAs the scatter then skips.
-// Each warp flags whole tiles; the last block to finish (ticket) compacts the flags in ascending tile order into
-// list[0] = count, list[1 ..] = tiles (the layout of GemmNTParams::tile_list).
 constexpr int kLiveTilesThreads = 256;
-__global__ void __launch_bounds__(kLiveTilesThreads)
-scatter_live_tiles_kernel(const long long* ids, int V, RowMap rm, int M, int num_tiles, int* flags, unsigned* ticket, int* list) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
-    for (int t = blockIdx.x * warps + warp; t < num_tiles; t += gridDim.x * warps) {
-        bool live = false;
-#pragma unroll
-        for (int k = 0; k < kTileM / 32; ++k) {
-            const int grow = t * kTileM + 32 * k + lane;
-            long long trow;
-            int tt;
-            if (grow < M && rm.map(grow, trow, tt)) {
-                const long long id = ids[trow];
-                live = live || (id >= 1 && id < V);
-            }
-        }
-        live = __any_sync(0xffffffffu, live);
-        if (lane == 0) flags[t] = live ? 1 : 0;
-    }
+// The last block of a tile-flagging kernel to finish (ticket) compacts flags[0 .. num_tiles) in ascending tile order into
+// list[0] = count, list[1 ..] = the flagged tiles.  Every block calls it after writing its own flags.
+__device__ void compact_live_tiles(const int* flags, int num_tiles, unsigned* ticket, int* list) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     __shared__ bool last;
     __shared__ int warp_sums[kLiveTilesThreads / 32];
     __threadfence();  // this block's flags are visible before its ticket
@@ -832,6 +820,168 @@ scatter_live_tiles_kernel(const long long* ids, int V, RowMap rm, int M, int num
     for (int t = b; t < e; ++t)
         if (__ldcg(flags + t)) list[1 + pos++] = t;
     if (threadIdx.x == kLiveTilesThreads - 1) list[0] = pos;  // the last run ends at the total
+}
+
+// The tiles of the embedding-gradient GEMM that scatter something: tile t (rows [64t, 64t + 64) of M) is live when one of its
+// rows maps through rm to a token whose id is in [1, V) -- EpiScatter's own test, so a dead tile would add nothing.  Padded
+// histories make runs of all-padding tiles (about 40 % of the NRMS batch), whose A loads and MMAs the scatter then skips.
+// Each warp flags whole tiles; compact_live_tiles lists them (the layout of GemmNTParams::tile_list).
+__global__ void __launch_bounds__(kLiveTilesThreads)
+scatter_live_tiles_kernel(const long long* ids, int V, RowMap rm, int M, int num_tiles, int* flags, unsigned* ticket, int* list) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
+    for (int t = blockIdx.x * warps + warp; t < num_tiles; t += gridDim.x * warps) {
+        bool live = false;
+#pragma unroll
+        for (int k = 0; k < kTileM / 32; ++k) {
+            const int grow = t * kTileM + 32 * k + lane;
+            long long trow;
+            int tt;
+            if (grow < M && rm.map(grow, trow, tt)) {
+                const long long id = ids[trow];
+                live = live || (id >= 1 && id < V);
+            }
+        }
+        live = __any_sync(0xffffffffu, live);
+        if (lane == 0) flags[t] = live ? 1 : 0;
+    }
+    compact_live_tiles(flags, num_tiles, ticket, list);
+}
+
+// ------------------------------------------------------------------------------------------------
+// padding titles of the news encoder (PaddingTitles in nr_ops.h).  A warp owns a 64-row tile and classifies every title that
+// has a row in it (a title across a tile edge is classified by both tiles, the same way); the tile whose rows include a
+// title's first row writes its flag.
+// ------------------------------------------------------------------------------------------------
+struct PaddingJob {
+    const long long* ids;
+    int n_seq, T, d, M, num_tiles;
+    const uint32_t* rows;  // bf16 pairs: row 0 of the table (per_title 0) or the gathered rows X (per_title 1)
+    long long ld_words;    // row pitch in 32-bit words
+    int per_title;
+    const float* bqkv;     // non-null: also write the shared padding tile
+    int sec, ld3;
+    PaddingTitles out;
+    unsigned* ticket;
+};
+
+__global__ void __launch_bounds__(kLiveTilesThreads) padding_titles_kernel(const PaddingJob j) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
+    const int half_d = j.d / 2;
+    // forward: one verdict for every title, from row 0 of the table
+    const int row0_nonzero = __syncthreads_or(!j.per_title && threadIdx.x < half_d && (j.rows[threadIdx.x] & 0x7fff7fffu) != 0);
+    if (j.bqkv != nullptr) {  // Q|K|V of a zero row: what the projection's store epilogue writes for it, bf16(0 + b) and bf16(y - bf16(y))
+        const int n3 = 3 * j.sec;
+        auto* qkv = static_cast<__nv_bfloat16*>(j.out.qkv);
+        auto* vlo = static_cast<__nv_bfloat16*>(j.out.v_lo);
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < j.T * j.ld3; i += gridDim.x * blockDim.x) {
+            const int c = i % j.ld3, r = i / j.ld3;
+            const float y = c < n3 ? j.bqkv[c] : 0.f;
+            const __nv_bfloat16 h = __float2bfloat16_rn(y);
+            qkv[i] = h;
+            if (c >= 2 * j.sec && c < n3) vlo[r * j.sec + c - 2 * j.sec] = __float2bfloat16_rn(y - __bfloat162float(h));
+        }
+    }
+    for (int t = blockIdx.x * warps + warp; t < j.num_tiles; t += gridDim.x * warps) {
+        const int r0 = t * kTileM, r1 = min(j.M, r0 + kTileM);
+        bool live = false;
+        for (int s = r0 / j.T; s * j.T < r1; ++s) {
+            const long long id = lane < j.T ? j.ids[static_cast<long long>(s) * j.T + lane] : 0;
+            bool pad = __all_sync(0xffffffffu, id == 0);
+            if (pad && j.per_title) {
+                // the title's T rows are one contiguous run of 16-byte pieces (pitch % 8 == 0): OR every bit of columns < d
+                const uint4* x = reinterpret_cast<const uint4*>(j.rows + static_cast<long long>(s) * j.T * j.ld_words);
+                const int per_row = static_cast<int>(j.ld_words / 4);
+                uint32_t nz = 0;
+#pragma unroll 8
+                for (int i = lane; i < j.T * per_row; i += 32) {
+                    const uint4 v = __ldg(x + i);
+                    const int c0 = 8 * (i % per_row), n = min(8, max(0, j.d - c0));  // columns of this piece below d
+                    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        nz |= w[k] & (2 * k + 1 < n ? 0x7fff7fffu : 2 * k < n ? 0x00007fffu : 0u);
+                }
+                pad = !__any_sync(0xffffffffu, nz != 0);
+            } else if (pad) {
+                pad = !row0_nonzero;
+            }
+            live = live || !pad;
+            if (lane == 0 && s * j.T >= r0) j.out.pad[s] = pad ? 1 : 0;
+        }
+        if (lane == 0) j.out.tile_flags[t] = live ? 1 : 0;
+    }
+    compact_live_tiles(j.out.tile_flags, j.num_tiles, j.ticket, j.out.live);
+}
+
+int padding_titles(const long long* ids, long long n_seq, int T, int d, const void* rows, int ld_rows, int per_title,
+                   const float* bqkv, int sec, int ld3, PaddingTitles* out, cudaStream_t stream) {
+    NR_REQUIRE(T >= 1 && T <= 32 && d % 2 == 0 && d <= 2 * kLiveTilesThreads && ld_rows % 8 == 0 && n_seq * T < (1ll << 31),
+               "padding_titles: T=%d d=%d ld=%d", T, d, ld_rows);
+    const int M = static_cast<int>(n_seq * T), num_tiles = ceil_div(M, kTileM);
+    // pad flags | tile flags | ticket | live list | shared Q|K|V tile | its V low plane; stream-ordered, freed by the caller
+    const size_t pad_b = round_up(static_cast<int>(n_seq), 16), head_b = round_up(static_cast<int>(pad_b) + 4 * (2 * num_tiles + 2), 128);
+    const size_t qkv_b = bqkv ? round_up(T * ld3 * 2, 128) : 0, vlo_b = bqkv ? static_cast<size_t>(T) * sec * 2 : 0;
+    char* buf = nullptr;
+    NR_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), head_b + qkv_b + vlo_b, stream));
+    out->base = buf;
+    out->pad = reinterpret_cast<unsigned char*>(buf);
+    out->tile_flags = reinterpret_cast<int*>(buf + pad_b);
+    unsigned* ticket = reinterpret_cast<unsigned*>(out->tile_flags + num_tiles);
+    out->live = out->tile_flags + num_tiles + 1;
+    out->qkv = bqkv ? buf + head_b : nullptr;
+    out->v_lo = bqkv ? static_cast<char*>(out->qkv) + qkv_b : nullptr;
+    if (n_seq == 0) return 0;
+    NR_CHECK_CUDA(cudaMemsetAsync(ticket, 0, sizeof(unsigned), stream));
+    const PaddingJob j{.ids = ids, .n_seq = static_cast<int>(n_seq), .T = T, .d = d, .M = M, .num_tiles = num_tiles,
+                       .rows = static_cast<const uint32_t*>(rows), .ld_words = ld_rows / 2, .per_title = per_title, .bqkv = bqkv,
+                       .sec = sec, .ld3 = ld3, .out = *out, .ticket = ticket};
+    ProfScope ps("padding_titles", M, num_tiles, per_title, stream);
+    const int blocks = std::max(1, std::min(4 * num_sms(), ceil_div(num_tiles, kLiveTilesThreads / 32)));
+    padding_titles_kernel<<<blocks, kLiveTilesThreads, 0, stream>>>(j);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+void free_padding_titles(PaddingTitles& pt, cudaStream_t stream) {
+    if (pt.base != nullptr) cudaFreeAsync(pt.base, stream);
+    pt = PaddingTitles{};
+}
+
+// dst[c * ld_dst] += sum of A[r][c] over the rows r of the tiles flagged 0 (c < N, N even): the bias column of a weight gradient
+// whose GEMM skipped those tiles because their X rows are [0 .. 0, 1].  Thread = column pair, block = 64-row tile (grid stride)
+constexpr int kDeadSumThreads = 128;
+__global__ void __launch_bounds__(kDeadSumThreads)
+dead_tiles_colsum_kernel(const __nv_bfloat16* A, int lda, int N, int M, const int* tile_flags, int num_tiles, float* dst, int ld_dst) {
+    const int cp = blockIdx.y * kDeadSumThreads + threadIdx.x;
+    if (2 * cp >= N) return;
+    float s0 = 0.f, s1 = 0.f;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        if (__ldg(tile_flags + t)) continue;
+        const int r1 = min(M, t * kTileM + kTileM);
+        const uint32_t* a = reinterpret_cast<const uint32_t*>(A + static_cast<size_t>(t) * kTileM * lda) + cp;
+#pragma unroll 8
+        for (int r = t * kTileM; r < r1; ++r, a += lda / 2) {
+            const float2 v = unpack_bf16x2(__ldg(a));
+            s0 += v.x;
+            s1 += v.y;
+        }
+    }
+    red_add_f32(dst + static_cast<size_t>(2 * cp) * ld_dst, s0);
+    red_add_f32(dst + static_cast<size_t>(2 * cp + 1) * ld_dst, s1);
+}
+
+int dead_tiles_colsum(const void* A, int lda, int N, int M, const int* tile_flags, float* dst, int ld_dst, cudaStream_t stream) {
+    NR_REQUIRE(N % 2 == 0 && lda % 2 == 0, "dead_tiles_colsum: N=%d lda=%d", N, lda);
+    if (M == 0) return 0;
+    const int num_tiles = ceil_div(M, kTileM);
+    ProfScope ps("dead_tiles_colsum", M, N, 0, stream);
+    const dim3 grid(std::max(1, std::min(2 * num_sms(), num_tiles)), ceil_div(N / 2, kDeadSumThreads));
+    dead_tiles_colsum_kernel<<<grid, kDeadSumThreads, 0, stream>>>(static_cast<const __nv_bfloat16*>(A), lda, N, M, tile_flags,
+                                                                  num_tiles, dst, ld_dst);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t stream) {

@@ -507,7 +507,10 @@ struct GemmTNParams {
     int cluster_m;   // cluster shape over (m-tile, n-tile): the CTAs of one k-range that share an A chunk (same m-tile) or a
     int cluster_n;   // B chunk (same n-tile) receive it by one TMA multicast; 1 x 1 = no cluster
     int k_slices;
-    int chunks_per_slice;  // 64-row chunks per CTA
+    int chunks_per_slice;  // 64-row chunks per CTA (without k_list)
+    // null: every 64-row chunk of the Kr rows.  Otherwise the chunks to reduce over, written on the device before the launch
+    // (GemmNTParams::tile_list layout); the k_slices ranges split them evenly
+    const int* k_list;
     int n_boxes;     // ceil(Nb/64)
     int stages;
     float* D;        // fp32 [Ma][ldd], accumulated with red.global.add

@@ -46,6 +46,7 @@ struct StoreCfg {
     int ld_lo = 0, lo_col0 = 0;
     int accumulate = 0;                 // fp32 output only: out += A . W^T (+ bias)
     int rows_per_tile = kGemmTileRows;  // rows are computed independently: larger values are clamped to the tile
+    const int* tile_list = nullptr;     // device list of the 64-row tiles to compute (GemmNTParams::tile_list); the others are not written
 };
 int gemm_store(const GemmOperands& g, const StoreCfg& c, cudaStream_t stream);
 // whether gemm_store can emit the low plane of the columns [lo_col0, N) of an N x K product (host-only, no launch)
@@ -92,13 +93,36 @@ struct ScatterEmbCfg {
 };
 int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t stream);
 
-// D[Ma x Nb] += A[:, :Ma]^T . B[rows + shift, b_col0 : b_col0 + Nb]   (fp32 accumulate into D, pitch ldd; Nb <= 512)
+// D[Ma x Nb] += A[:, :Ma]^T . B[rows + shift, b_col0 : b_col0 + Nb]   (fp32 accumulate into D, pitch ldd; Nb <= 512).
+// k_list (device, GemmNTParams::tile_list layout): only the listed 64-row chunks of the rows are summed.
 int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, int b_rows, int b_cols, int ldb,
-                       int b_col0, int Nb, int b_row_shift, float* D, int ldd, cudaStream_t stream);
+                       int b_col0, int Nb, int b_row_shift, float* D, int ldd, cudaStream_t stream, const int* k_list = nullptr);
 // Linear weight gradient: dW_ext[N][0..K] += dY^T . [X | 1] over M rows, dY pitch ld_dy, X read at row r + x_row_shift.  Column K of
 // X is its ones column, so column K of dW_ext (same pitch ldx) is the bias gradient.  Launches of <= 512 columns, left to right.
 int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int K, int ldx, float* dW_ext, cudaStream_t stream,
-                     int x_row_shift = 0);
+                     int x_row_shift = 0, const int* k_list = nullptr);
+
+// Padding titles of the news encoder.  Title s is padding when its T ids are all 0 and the rows the projection reads for it are
+// exact zeros: row 0 of the bf16 table in the forward (per_title 0; padding_idx=0 keeps it zero, a pretrained table may not),
+// the title's own gathered rows X in the backward (per_title 1).  Such a title's X rows are [0 .. 0, 1], so its Q|K|V rows are
+// the bias rows in `qkv` below and its only weight-gradient term is its dQ|dK|dV rows in the bias column.  A 64-row tile is
+// live when it holds a row of a title that is not padding.  Nothing is read back to the host.
+struct PaddingTitles {
+    unsigned char* pad = nullptr;  // [n_seq] 1 = padding title
+    int* tile_flags = nullptr;     // [ceil(n_seq * T / 64)] 1 = live tile
+    int* live = nullptr;           // the live tiles in GemmNTParams::tile_list layout
+    void* qkv = nullptr;           // with bqkv: bf16 [T][ld3] Q|K|V of a padding title (every row bf16(b_qkv))
+    void* v_lo = nullptr;          // with bqkv: bf16 [T][sec] low plane of its V section, bf16(b - bf16(b))
+    void* base = nullptr;          // the one stream-ordered allocation behind the buffers above
+};
+// rows: the table (per_title 0) or X (per_title 1), pitch ld_rows; d even, T <= 32.  Allocates on `stream`; free_padding_titles
+// releases the buffers once every launch that reads them has been enqueued.
+int padding_titles(const long long* ids, long long n_seq, int T, int d, const void* rows, int ld_rows, int per_title,
+                   const float* bqkv, int sec, int ld3, PaddingTitles* out, cudaStream_t stream);
+void free_padding_titles(PaddingTitles& pt, cudaStream_t stream);
+// dst[c * ld_dst] += sum over the rows of the tiles with tile_flags 0 of A[r][c], c < N (the bias column of a weight gradient
+// whose GEMM skipped those tiles)
+int dead_tiles_colsum(const void* A, int lda, int N, int M, const int* tile_flags, float* dst, int ld_dst, cudaStream_t stream);
 
 // ---- memory-bound companions (aux.cu) --------------------------------------------------------------
 // fp32 rows -> zero-padded bf16 planes: every operand cast, dense-input conversion and hi/lo split in front of a GEMM.
@@ -143,14 +167,17 @@ int gather_rows(const long long* ids, long long n_tok, int T, const void* table,
 int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, int heads, int dk, void* ctx, int ld_ctx,
                   DropoutCfg drop, cudaStream_t stream);
 int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-                  void* dqkv, int ld_dqkv, cudaStream_t stream);
+                  void* dqkv, int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad = nullptr);
 // title-level backward (attn_title.cu): T = 20, d_k = 20, <= 15 heads, sections with a 16-byte phase (sec % 8 == 0)
 bool mhsa_title_fwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int ld_ctx);
+// pad (PaddingTitles, may be null): the padding titles take their Q|K|V rows (and V low plane) from pad->qkv / pad->v_lo, not
+// from qkv / v_lo, whose rows they may have left unwritten
 int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int heads, void* ctx, int ld_ctx, DropoutCfg drop,
-                   cudaStream_t stream, const void* v_lo = nullptr, int ld_vlo = 0, void* ctx_lo = nullptr);
+                   cudaStream_t stream, const void* v_lo = nullptr, int ld_vlo = 0, void* ctx_lo = nullptr,
+                   const PaddingTitles* pad = nullptr);
 bool mhsa_title_bwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int ld_dctx, int ld_dqkv);
 int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int heads, void* dqkv,
-                   int ld_dqkv, cudaStream_t stream);
+                   int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad = nullptr);
 // dscore_r = w_r (dw_r - sum_seg w dw), dw_r = dOut[seg] . X_r
 int pool_dscore(const void* X, int lda, int D, long long n_seg, int seg_len, const float* w, const float* dout, int ldo,
                 float* dscore, cudaStream_t stream);
