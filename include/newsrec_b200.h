@@ -73,6 +73,14 @@ int nr_debug_gemm_store(const nr_gemm_store_args* a, void* stream);
  * writes, per CTA, cycle counters into slot k: [0] TMA producer waiting for a free A stage, [1] consumer warpgroups
  * waiting for A data, [4] epilogue body, [5] kernel, [6] tiles.  Null (default) switches the counters off. */
 void nr_debug_set_gemm_timing(void* dev_buf, int slots);
+/* The live-token compaction of the news encoder's backward (see table_bf16 of nr_mhsa_encoder_bwd_args), on its own: ids
+ * [n_seq*T] (T <= 32), the bf16 table (pitch ldx, or NULL) and the gathered rows X [n_seq*T][ldx] in; out the per-title live
+ * mask [n_seq] and padding flag [n_seq], the offsets [n_seq+1], the compact -> token index [n_seq*T], the compact tile list
+ * [1 + ceil(n_seq*T/64)] (count first), the compact copy of X into Xc [n_seq*T][ldx] and the zero tail rows of Xc and of
+ * dqkv_c [n_seq*T][ld3], ld3 = round_up(3*round_up(d, 8), 16).  bqkv [3*round_up(d, 8)]: the padding Q|K|V tile's bias. */
+int nr_debug_live_tokens(const long long* ids, long long n_seq, int T, int d, const void* table, int V, const void* X, int ldx,
+                         const float* bqkv, unsigned* mask, unsigned char* pad, int* offset, int* index, int* tiles, void* Xc,
+                         void* dqkv_c, void* stream);
 /* Data parallel: the weight-gradient GEMMs (nr_gemm_tn and the composites' internal calls) leave n SMs free, so that the
  * channel CTAs of a gradient all-reduce running on a side stream have somewhere to run (0 = use every SM, the default). */
 void nr_reserve_sms_for_comm(int n);
@@ -393,6 +401,11 @@ typedef struct {
     /* dense variant only (NULL otherwise): fp32 [T][d] (+=) gradient of dense_pos = sum over the sequences of ddense, in a fixed
      * order (bit-identical across runs) */
     float* dpos;
+    /* ids variant: the bf16 table of the forward (pitch ldx).  The projection backward runs over the live tokens only -- id in
+     * [1, V), or every token when row 0 of the table is nonzero -- and, like the accurate forward, takes a title without one
+     * for padding.  NULL: the same verdict from the gathered rows X instead (a token is live when its id is in [1, V) or its
+     * row of X is nonzero below column d), which costs a read of the dead tokens' rows.  NULL for the dense variant. */
+    const void* table_bf16;
 } nr_mhsa_encoder_bwd_args;
 long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q);
 int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream);

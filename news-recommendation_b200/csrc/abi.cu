@@ -1,5 +1,6 @@
 // extern "C" surface declared in include/newsrec_b200.h: argument validation + kernel sequencing.
 #include <cstring>
+#include <utility>
 
 #include "../../include/newsrec_b200.h"
 #include "nr_common.cuh"
@@ -38,6 +39,27 @@ int nr_debug_gemm_store(const nr_gemm_store_args* a, void* stream) {
                        .drop = {a->p_drop, a->seed}, .ones_col = a->ones_col, .ones_zero_upto = a->ones_zero_upto, .lo_out = a->lo_out,
                        .ld_lo = a->ld_lo, .lo_col0 = a->lo_col0, .accumulate = a->accumulate, .rows_per_tile = a->rows_per_tile},
                       as_stream(stream));
+}
+int nr_debug_live_tokens(const long long* ids, long long n_seq, int T, int d, const void* table, int V, const void* X, int ldx,
+                         const float* bqkv, unsigned* mask, unsigned char* pad, int* offset, int* index, int* tiles, void* Xc,
+                         void* dqkv_c, void* stream) {
+    NR_REQUIRE(ids && X && bqkv && mask && pad && offset && index && tiles && Xc && dqkv_c && n_seq >= 0 && d >= 2,
+               "nr_debug_live_tokens: null operand or n_seq=%lld d=%d", n_seq, d);
+    const cudaStream_t st = as_stream(stream);
+    const int sec = (d + 7) & ~7, ld3 = (3 * sec + 15) & ~15;
+    const long long bytes = live_tokens_bytes(n_seq, T, ld3);
+    char* buf = nullptr;
+    NR_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), bytes, st));
+    LiveTokens lt;
+    int rc = live_tokens(ids, n_seq, T, d, table, ldx, V, bqkv, sec, ld3, X, ldx, Xc, dqkv_c, buf, bytes, &lt, st);
+    const size_t n = static_cast<size_t>(n_seq), M = n * T;
+    const std::pair<void*, const void*> copies[] = {{mask, lt.mask}, {pad, lt.pad}, {offset, lt.offset}, {index, lt.index}, {tiles, lt.tiles}};
+    const size_t sizes[] = {4 * n, n, 4 * (n + 1), 4 * M, 4 * (1 + (M + 63) / 64)};
+    for (int i = 0; i < 5 && rc == 0 && n > 0; ++i)
+        if (cudaMemcpyAsync(copies[i].first, copies[i].second, sizes[i], cudaMemcpyDeviceToDevice, st) != cudaSuccess) rc = -1;
+    NR_CHECK_CUDA(cudaFreeAsync(buf, st));
+    NR_REQUIRE(rc != -1, "nr_debug_live_tokens: copy-out failed");
+    return rc;
 }
 int nr_has_triage_backends(void) { return has_triage_backends(); }
 void nr_reserve_sms_for_comm(int n) { set_comm_reserved_sms(n); }
@@ -312,6 +334,7 @@ struct PaddingScope {
     ~PaddingScope() { free_padding_titles(pt, st); }
 };
 
+
 // the dense input rows [n_seq][T][d] (+ dense_pos) with the ones column at d, as the hi plane of pitch ld_hi
 static Bf16Rows dense_rows(const nr_mhsa_encoder_fwd_args* a, void* hi, int ld_hi) {
     return {.src = a->dense, .n_rows = a->n_seq * a->T, .T = a->T, .D = a->d, .s_seq = a->dense_s_seq, .s_tok = a->dense_s_tok,
@@ -366,7 +389,7 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
         // padding titles (all ids 0, zero table row 0; ~45 % of a batch of left-padded histories) share one Q|K|V tile: the
         // projection computes only the live 64-row tiles, and the attention reads the shared tile for every padding title
         PaddingScope pad{.st = st};
-        NR_PROPAGATE(padding_titles(a->ids, a->n_seq, a->T, a->d, a->table_bf16, a->ldx, 0, a->bqkv, sec, a->ld3, &pad.pt, st));
+        NR_PROPAGATE(padding_titles(a->ids, a->n_seq, a->T, a->d, a->table_bf16, a->ldx, a->bqkv, sec, a->ld3, &pad.pt, st));
         NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
                                 {.out = a->QKV_bf16, .ld_out = a->ld3, .out_bf16 = 1, .bias = a->bqkv, .lo_out = a->V_lo_bf16, .ld_lo = sec,
                                  .lo_col0 = 2 * sec, .tile_list = pad.pt.live}, st));
@@ -398,16 +421,23 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
     return 0;
 }
 
-// bf16 buffers at the canonical pitches ldq, ldx, ld3, ld3; QKV only for the precise dense forward, which keeps no bf16 Q|K|V
+// bf16 buffers at the canonical pitches ldq, ldx, ld3, ld3; QKV holds the precise dense forward's recomputed Q|K|V (it keeps
+// none) or, in the news variant, the compact copy of X (pitch ldx)
+// live: the news variant's LiveTokens buffers (live_tokens_bytes)
 struct MhsaBwdWorkspace : WorkspaceLayout {
     float* dscore;
     __nv_bfloat16 *dpre, *dC, *dQKV, *QKV;
-    MhsaBwdWorkspace(void* base, long long rows, int d, int q)
-        : WorkspaceLayout{static_cast<char*>(base)}, dscore(take<float>(rows)), dpre(take<__nv_bfloat16>(rows * round_up(q, 16))),
-          dC(take<__nv_bfloat16>(rows * round_up(d + 1, 8))), dQKV(take<__nv_bfloat16>(rows * round_up(3 * qkv_section(d), 16))),
-          QKV(take<__nv_bfloat16>(rows * round_up(3 * qkv_section(d), 16))) {}
+    char* live;
+    long long live_bytes;
+    MhsaBwdWorkspace(void* base, long long n_seq, int T, int d, int q)
+        : WorkspaceLayout{static_cast<char*>(base)}, dscore(take<float>(n_seq * T)), dpre(take<__nv_bfloat16>(n_seq * T * round_up(q, 16))),
+          dC(take<__nv_bfloat16>(n_seq * T * round_up(d + 1, 8))), dQKV(take<__nv_bfloat16>(n_seq * T * round_up(3 * qkv_section(d), 16))),
+          QKV(take<__nv_bfloat16>(n_seq * T * round_up(3 * qkv_section(d), 16))),
+          live_bytes(live_tokens_bytes(n_seq, T, round_up(3 * qkv_section(d), 16))) {
+        live = take<char>(live_bytes);
+    }
 };
-long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q) { return MhsaBwdWorkspace(nullptr, n_seq * T, d, q).bytes(); }
+long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q) { return MhsaBwdWorkspace(nullptr, n_seq, T, d, q).bytes(); }
 
 int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     NR_REQUIRE(a != nullptr, "nr_mhsa_encoder_bwd: null args");
@@ -424,7 +454,8 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
                "nr_mhsa_encoder_bwd: missing input-gradient buffer");
     NR_REQUIRE(a->dpos == nullptr || a->ids == nullptr, "nr_mhsa_encoder_bwd: dpos needs the dense (user-level) variant");
     NR_REQUIRE(a->ids == nullptr || a->bqkv != nullptr, "nr_mhsa_encoder_bwd: the news variant needs bqkv (Q|K|V of its padding titles)");
-    const MhsaBwdWorkspace ws(a->workspace, a->n_seq * a->T, a->d, a->q);
+    NR_REQUIRE(a->table_bf16 == nullptr || a->ids != nullptr, "nr_mhsa_encoder_bwd: table_bf16 needs the ids (news) variant");
+    const MhsaBwdWorkspace ws(a->workspace, a->n_seq, a->T, a->d, a->q);
     NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_mhsa_encoder_bwd: workspace too small (%lld bytes)", a->workspace_bytes);
     if (a->n_seq == 0) return 0;
     const int M = static_cast<int>(a->n_seq * a->T);
@@ -446,21 +477,29 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
                                   {.w = a->w, .dout = a->dout, .ldo = a->d, .seg_len = a->T, .dx = ws.dC, .ld_dx = a->ldx,
                                    .drop = context_dropout(a->ids != nullptr ? a->p_drop : 0.f, a->seed)}, st));
     // --- attention backward ---
-    // padding titles (all ids 0 and zero rows in X): the attention reads their Q|K|V from the shared bias tile (the accurate
-    // forward left their rows unwritten), and the weight gradient skips the tiles that hold nothing else
-    PaddingScope pad{.st = st};
-    const bool title_bwd = mhsa_title_bwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx, a->ld3);
-    if (a->ids != nullptr && title_bwd)
-        NR_PROPAGATE(padding_titles(a->ids, a->n_seq, a->T, a->d, a->X_bf16, a->ldx, 1, a->bqkv, sec, a->ld3, &pad.pt, st));
+    // the news variant at the title-level kernel's shape runs the projection backward over live tokens only (id in [1, V), or
+    // a nonzero table row 0; about a third of a batch of padded titles and left-padded histories): the attention stores their
+    // dQ|dK|dV rows in compact order and sums the dead tokens' rows into the bias column, the dead tokens' only weight-gradient
+    // term (their X rows are [0 .. 0, 1]); padding titles read their Q|K|V from the shared bias tile (the accurate forward left
+    // their rows unwritten)
+    LiveTokens live;
+    const bool compact = a->ids != nullptr && mhsa_title_bwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx, a->ld3);
+    if (compact) {
+        NR_REQUIRE(a->V >= 1, "nr_mhsa_encoder_bwd: V=%d", a->V);
+        NR_PROPAGATE(live_tokens(a->ids, a->n_seq, a->T, a->d, a->table_bf16, a->ldx, a->V, a->bqkv, sec, a->ld3, a->X_bf16, a->ldx, ws.QKV,
+                                 ws.dQKV, ws.live, ws.live_bytes, &live, st));
+    }
+    const TitleBwdLive title_live{.tokens = &live, .dbias = a->dWqkv_ext + a->d, .ld_dbias = a->ldx};
     NR_PROPAGATE(mhsa_core_bwd(QKV, a->ld3, sec, ws.dC, a->ldx, a->n_seq, a->T, a->heads, a->d / a->heads, ws.dQKV, a->ld3, st,
-                               pad.pt.pad != nullptr ? &pad.pt : nullptr));
+                               compact ? &title_live : nullptr));
     // --- projection backward: the input first (the embedding gradient is 97 % of a data-parallel step's all-reduce: the
     //     caller's event lets the communication start under the weight-gradient GEMM), then the weights (+bias through the
     //     ones column of X) ---
     if (a->ids != nullptr) {
         NR_REQUIRE(a->V >= 1, "nr_mhsa_encoder_bwd: V=%d", a->V);
         NR_PROPAGATE(gemm_scatter_emb({.A = ws.dQKV, .M = M, .lda = a->ld3, .W = a->wqkvT_bf16, .N = a->d, .ldw = a->ld3, .K = 3 * sec},
-                                      {.ids = a->ids, .demb = a->demb, .V = a->V, .drop = {a->p_drop, a->seed}, .drop_ld = a->ldx}, st));
+                                      {.ids = a->ids, .demb = a->demb, .V = a->V, .drop = {a->p_drop, a->seed}, .drop_ld = a->ldx,
+                                       .rows = live.index, .tile_list = live.tiles}, st));
         if (a->emb_grad_ready_event != nullptr) NR_CHECK_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(a->emb_grad_ready_event), st));
     } else {
         NR_PROPAGATE(gemm_store({.A = ws.dQKV, .M = M, .lda = a->ld3, .W = a->wqkvT_bf16, .N = a->d, .ldw = a->ld3, .K = 3 * sec},
@@ -471,9 +510,9 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     // both weight-gradient GEMMs run AFTER the embedding gradient is complete: together they are the window (~0.4 ms) under which
     // the caller's all-reduce of that gradient hides
     NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, a->q, a->ldq, a->C_bf16, a->d, a->ldx, a->dWa_ext, st));
-    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st, 0, pad.pt.live));
-    // the skipped tiles' rows of X are [0 .. 0, 1]: their whole term is their dQ|dK|dV column sums in the bias column
-    if (pad.pt.live != nullptr) NR_PROPAGATE(dead_tiles_colsum(ws.dQKV, a->ld3, 3 * sec, M, pad.pt.tile_flags, a->dWqkv_ext + a->d, a->ldx, st));
+    // compact: the live tokens' dQ|dK|dV against the compact copy of their X rows (+ bias through its ones column)
+    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, compact ? ws.QKV : a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st, 0,
+                                  live.tiles));
     return 0;
 }
 

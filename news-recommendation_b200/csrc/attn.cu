@@ -825,7 +825,7 @@ int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, 
 }
 
 int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-                  void* dqkv, int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad) {
+                  void* dqkv, int ld_dqkv, cudaStream_t stream, const TitleBwdLive* live) {
     NR_PROPAGATE(check_core_shape(n_seq, T, heads, dk, sec, ld_qkv));
     NR_REQUIRE(ld_dqkv >= 3 * sec && ld_dctx >= heads * dk, "mhsa: dQ|dK|dV pitch %d / context-gradient pitch %d too small for sec=%d d=%d",
                ld_dqkv, ld_dctx, sec, heads * dk);
@@ -834,8 +834,8 @@ int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld
     if (n_seq == 0) return 0;
     ProfScope ps("mhsa_core_bwd", static_cast<int>(n_seq), T, heads * dk, stream);
     if (mhsa_title_bwd_supported(T, dk, heads, sec, ld_qkv, ld_dctx, ld_dqkv))  // the news encoder's shape: whole titles per CTA, TMA in / out
-        return mhsa_title_bwd(qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, heads, dqkv, ld_dqkv, stream, pad);
-    NR_REQUIRE(pad == nullptr, "mhsa: padding titles need the title-level kernel");
+        return mhsa_title_bwd(qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, heads, dqkv, ld_dqkv, stream, live);
+    NR_REQUIRE(live == nullptr, "mhsa: live tokens need the title-level kernel");
     return dispatch(true, qkv, ld_qkv, sec, dctx, ld_dctx, n_seq, T, heads, dk, dqkv, ld_dqkv, Dropout::make(0.f, 0), stream);
 }
 

@@ -61,7 +61,15 @@ struct Params {
     uint32_t out_stage;   // == qkv_tile
     uint32_t tx;          // bytes one stage's two boxes deliver
     float rs, sc;         // 1/sqrt(dk), log2(e)/sqrt(dk)
-    const unsigned char* pad;  // PaddingTitles::pad or null
+    const unsigned char* pad;  // LiveTokens::pad or null
+    // with live tokens (mask non-null): title s stores its live rows at rows offset[s] .. of dqkv (pitch ld_out bytes, row_bytes
+    // each), and the dead rows' bf16 dQ|dK|dV go into dbias[c * ld_dbias]
+    const uint32_t* mask;
+    const int* offset;
+    char* dqkv;
+    uint32_t ld_out, row_bytes;
+    float* dbias;
+    int ld_dbias;
 };
 
 __device__ __forceinline__ uint32_t sel(bool keep, uint32_t v) { return keep ? v : 0u; }
@@ -117,9 +125,20 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
             for (int it = 0; it < kIn && it < n_my; ++it) load(it);
             for (int j = 0; j < n_my; ++j) {
                 const int o = j % kOut;
+                const int title = static_cast<int>(blockIdx.x) + j * static_cast<int>(gridDim.x);
+                const uint32_t tile = out_base + o * p.out_stage;
+                uint32_t live = 0;
+                char* dst = nullptr;
+                if (p.mask != nullptr) {
+                    live = p.mask[title];
+                    dst = p.dqkv + static_cast<size_t>(p.offset[title]) * p.ld_out;
+                }
                 f_wait(&ofull[o], (j / kOut) & 1, 70);
-                tma_store_2d(&tm_out, base_ptr + kIn * p.in_stage + o * p.out_stage, 0,
-                             (static_cast<int>(blockIdx.x) + j * static_cast<int>(gridDim.x)) * kT);
+                if (p.mask == nullptr) {
+                    tma_store_2d(&tm_out, tile, 0, title * kT);
+                } else {  // the live rows, one bulk copy each, to consecutive compact rows
+                    for (; live != 0; live &= live - 1, dst += p.ld_out) bulk_store_1d(dst, tile + (__ffs(live) - 1) * p.pq, p.row_bytes);
+                }
                 bulk_commit();
                 if (j + kIn < n_my) {
                     f_wait(&empty[j % kIn], (j / kIn) & 1, 71);
@@ -152,11 +171,19 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
     const uint32_t at1 = (lane & 15) * kScrPitch + 32u;                      // x2.trans, key rows 16..23 as m
     const uint32_t st_scr = g * kScrPitch + t4 * 4u;
     const float rs = p.rs, sc = p.sc;
+    // the dead rows' dQ | dK | dV as stored (bf16), per section, column group and column of the pair: the bias-column term
+    float dsum[3][3][2] = {};
+    const auto add_dead = [](float* acc, uint32_t packed) {
+        const float2 v = unpack_bf16x2(packed);
+        acc[0] += v.x;
+        acc[1] += v.y;
+    };
 
     for (int it = 0; it < n_my; ++it) {
         const int s = it % kIn, o = it % kOut;
         const uint32_t Q = in_base + s * p.in_stage, K = Q + p.sec2, V = K + p.sec2, G = Q + p.qkv_tile;
         const uint32_t ob = out_base + o * p.out_stage;
+        const uint32_t dead = p.mask != nullptr ? ~__ldg(p.mask + static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x)) : 0u;
         f_wait(&full[s], (it / kIn) & 1, 72);
 
         // ---- phase A (query rows i): A, dS -> scratch; dQ -> result tile ----
@@ -284,8 +311,16 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                 mma_bf16_k8(dq, a8, &kt8[nd]);
                 const bool cok = nd == 1 || (nd == 0 ? c0ok : c2ok);
                 const uint32_t oa = ob + (mt * 16 + g) * pq + gb + 16 * nd + 4 * t4;
-                if (cok && row0) sts32(oa, pack_bf16x2(dq[0], dq[1]));
-                if (mt == 0 && cok) sts32(oa + 8 * pq, pack_bf16x2(dq[2], dq[3]));
+                if (cok && row0) {
+                    const uint32_t v = pack_bf16x2(dq[0], dq[1]);
+                    sts32(oa, v);
+                    if ((dead >> (mt * 16 + g)) & 1u) add_dead(dsum[0][nd], v);
+                }
+                if (mt == 0 && cok) {
+                    const uint32_t v = pack_bf16x2(dq[2], dq[3]);
+                    sts32(oa + 8 * pq, v);
+                    if ((dead >> (8 + g)) & 1u) add_dead(dsum[0][nd], v);
+                }
             }
         }
         __syncwarp();
@@ -329,12 +364,16 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                 const bool cok = nd == 1 || (nd == 0 ? c0ok : c2ok);
                 const uint32_t oa = ob + p.sec2 + (mt * 16 + g) * pq + gb + 16 * nd + 4 * t4;
                 if (cok && row0) {
-                    sts32(oa, pack_bf16x2(dk[0], dk[1]));
-                    sts32(oa + p.sec2, pack_bf16x2(dv[0], dv[1]));
+                    const uint32_t k = pack_bf16x2(dk[0], dk[1]), v = pack_bf16x2(dv[0], dv[1]);
+                    sts32(oa, k);
+                    sts32(oa + p.sec2, v);
+                    if ((dead >> (mt * 16 + g)) & 1u) add_dead(dsum[1][nd], k), add_dead(dsum[2][nd], v);
                 }
                 if (mt == 0 && cok) {
-                    sts32(oa + 8 * pq, pack_bf16x2(dk[2], dk[3]));
-                    sts32(oa + p.sec2 + 8 * pq, pack_bf16x2(dv[2], dv[3]));
+                    const uint32_t k = pack_bf16x2(dk[2], dk[3]), v = pack_bf16x2(dv[2], dv[3]);
+                    sts32(oa + 8 * pq, k);
+                    sts32(oa + p.sec2 + 8 * pq, v);
+                    if ((dead >> (8 + g)) & 1u) add_dead(dsum[1][nd], k), add_dead(dsum[2][nd], v);
                 }
             }
         }
@@ -343,6 +382,25 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
         if (lane == 0) {
             mbar_arrive(&empty[s]);
             mbar_arrive(&ofull[o]);
+        }
+    }
+    if (p.mask != nullptr) {  // one add per column and CTA: the column sums over the warp's eight row groups g
+        const int sec = static_cast<int>(p.sec2 / 2u);
+#pragma unroll
+        for (int nd = 0; nd < 3; ++nd) {
+            const bool cok = nd == 1 || (nd == 0 ? c0ok : c2ok);
+            const int col = static_cast<int>(gb / 2u) + 8 * nd + 2 * t4;
+#pragma unroll
+            for (int sct = 0; sct < 3; ++sct) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float v = dsum[sct][nd][e];
+                    v += __shfl_xor_sync(0xffffffffu, v, 4);
+                    v += __shfl_xor_sync(0xffffffffu, v, 8);
+                    v += __shfl_xor_sync(0xffffffffu, v, 16);
+                    if (g == 0 && cok) red_add_f32(p.dbias + static_cast<size_t>(sct * sec + col + e) * p.ld_dbias, v);
+                }
+            }
         }
     }
 }
@@ -636,7 +694,7 @@ bool mhsa_title_bwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int
 }
 
 int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int heads, void* dqkv,
-                   int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad) {
+                   int ld_dqkv, cudaStream_t stream, const TitleBwdLive* live) {
     using namespace title;
     NR_REQUIRE(mhsa_title_bwd_supported(kT, kDk, heads, sec, ld_qkv, ld_dctx, ld_dqkv), "mhsa_title_bwd: unsupported layout");
     NR_REQUIRE(n_seq * kT < (1ll << 31), "mhsa_title_bwd: too many rows");
@@ -656,8 +714,18 @@ int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int l
     p.tx = kT * p.pq + kT * p.pc;
     p.rs = 1.0f / sqrtf(static_cast<float>(kDk));
     p.sc = p.rs * 1.4426950408889634f;
-    NR_REQUIRE(pad == nullptr || (pad->pad != nullptr && pad->qkv != nullptr), "mhsa_title_bwd: padding titles without their Q|K|V tile");
-    p.pad = pad != nullptr ? pad->pad : nullptr;
+    const LiveTokens* lt = live != nullptr ? live->tokens : nullptr;
+    NR_REQUIRE(live == nullptr || (lt != nullptr && lt->pad && lt->mask && lt->offset && lt->qkv && live->dbias),
+               "mhsa_title_bwd: live tokens without their flags, offsets, padding Q|K|V tile or bias column");
+    NR_REQUIRE(live == nullptr || (reinterpret_cast<uintptr_t>(dqkv) & 15) == 0, "mhsa_title_bwd: compact rows not 16-byte aligned");
+    p.pad = lt != nullptr ? lt->pad : nullptr;
+    p.mask = lt != nullptr ? lt->mask : nullptr;
+    p.offset = lt != nullptr ? lt->offset : nullptr;
+    p.dqkv = static_cast<char*>(dqkv);
+    p.ld_out = static_cast<uint32_t>(ld_dqkv) * 2u;
+    p.row_bytes = qkv_row;
+    p.dbias = live != nullptr ? live->dbias : nullptr;
+    p.ld_dbias = live != nullptr ? live->ld_dbias : 0;
     const size_t smem = 128 + static_cast<size_t>(kIn) * p.in_stage + static_cast<size_t>(kOut) * p.out_stage +
                        static_cast<size_t>(heads) * kScrWarp + (2 * kIn + 2 * kOut) * sizeof(uint64_t) + 64;
     NR_REQUIRE(smem <= 227 * 1024, "mhsa_title_bwd: %zu bytes of shared memory", smem);
@@ -666,8 +734,8 @@ int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int l
     NR_PROPAGATE(make_tmap_bytes_2d(&tq, qkv, rows, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
     NR_PROPAGATE(make_tmap_bytes_2d(&tc, dctx, rows, dc_row, static_cast<int64_t>(ld_dctx) * 2, static_cast<int>(p.pc), kT));
     NR_PROPAGATE(make_tmap_bytes_2d(&to, dqkv, rows, qkv_row, static_cast<int64_t>(ld_dqkv) * 2, static_cast<int>(p.pq), kT));
-    if (pad != nullptr)
-        NR_PROPAGATE(make_tmap_bytes_2d(&tp, pad->qkv, kT, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
+    if (lt != nullptr)
+        NR_PROPAGATE(make_tmap_bytes_2d(&tp, lt->qkv, kT, qkv_row, static_cast<int64_t>(ld_qkv) * 2, static_cast<int>(p.pq), kT));
     else
         tp = tq;
     static bool attr_set = false;

@@ -848,63 +848,51 @@ scatter_live_tiles_kernel(const long long* ids, int V, RowMap rm, int M, int num
 }
 
 // ------------------------------------------------------------------------------------------------
-// padding titles of the news encoder (PaddingTitles in nr_ops.h).  A warp owns a 64-row tile and classifies every title that
-// has a row in it (a title across a tile edge is classified by both tiles, the same way); the tile whose rows include a
-// title's first row writes its flag.
+// padding titles of the news encoder's forward (PaddingTitles in nr_ops.h).  A warp owns a 64-row tile and classifies every
+// title that has a row in it (a title across a tile edge is classified by both tiles, the same way); the tile whose rows
+// include a title's first row writes its flag.
 // ------------------------------------------------------------------------------------------------
 struct PaddingJob {
     const long long* ids;
     int n_seq, T, d, M, num_tiles;
-    const uint32_t* rows;  // bf16 pairs: row 0 of the table (per_title 0) or the gathered rows X (per_title 1)
-    long long ld_words;    // row pitch in 32-bit words
-    int per_title;
+    const uint32_t* row0;  // bf16 pairs: row 0 of the table
     const float* bqkv;     // non-null: also write the shared padding tile
     int sec, ld3;
     PaddingTitles out;
     unsigned* ticket;
 };
 
+// whether the first d columns of a bf16 row are nonzero (any block thread may ask; every thread of the block must)
+__device__ __forceinline__ bool block_row_nonzero(const uint32_t* row, int d) {
+    bool nz = false;
+    for (int i = threadIdx.x; i < d / 2; i += blockDim.x) nz = nz || (row[i] & 0x7fff7fffu) != 0;
+    return __syncthreads_or(nz) != 0;
+}
+
+// Q|K|V of a zero row: what the projection's store epilogue writes for it, bf16(0 + b) (and with vlo, bf16(y - bf16(y)))
+__device__ __forceinline__ void write_padding_qkv(const float* bqkv, int T, int sec, int ld3, void* qkv_out, void* vlo_out) {
+    const int n3 = 3 * sec;
+    auto* qkv = static_cast<__nv_bfloat16*>(qkv_out);
+    auto* vlo = static_cast<__nv_bfloat16*>(vlo_out);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < T * ld3; i += gridDim.x * blockDim.x) {
+        const int c = i % ld3, r = i / ld3;
+        const float y = c < n3 ? bqkv[c] : 0.f;
+        const __nv_bfloat16 h = __float2bfloat16_rn(y);
+        qkv[i] = h;
+        if (vlo != nullptr && c >= 2 * sec && c < n3) vlo[r * sec + c - 2 * sec] = __float2bfloat16_rn(y - __bfloat162float(h));
+    }
+}
+
 __global__ void __launch_bounds__(kLiveTilesThreads) padding_titles_kernel(const PaddingJob j) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
-    const int half_d = j.d / 2;
-    // forward: one verdict for every title, from row 0 of the table
-    const int row0_nonzero = __syncthreads_or(!j.per_title && threadIdx.x < half_d && (j.rows[threadIdx.x] & 0x7fff7fffu) != 0);
-    if (j.bqkv != nullptr) {  // Q|K|V of a zero row: what the projection's store epilogue writes for it, bf16(0 + b) and bf16(y - bf16(y))
-        const int n3 = 3 * j.sec;
-        auto* qkv = static_cast<__nv_bfloat16*>(j.out.qkv);
-        auto* vlo = static_cast<__nv_bfloat16*>(j.out.v_lo);
-        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < j.T * j.ld3; i += gridDim.x * blockDim.x) {
-            const int c = i % j.ld3, r = i / j.ld3;
-            const float y = c < n3 ? j.bqkv[c] : 0.f;
-            const __nv_bfloat16 h = __float2bfloat16_rn(y);
-            qkv[i] = h;
-            if (c >= 2 * j.sec && c < n3) vlo[r * j.sec + c - 2 * j.sec] = __float2bfloat16_rn(y - __bfloat162float(h));
-        }
-    }
+    const bool row0_nonzero = block_row_nonzero(j.row0, j.d);  // one verdict for every title
+    if (j.bqkv != nullptr) write_padding_qkv(j.bqkv, j.T, j.sec, j.ld3, j.out.qkv, j.out.v_lo);
     for (int t = blockIdx.x * warps + warp; t < j.num_tiles; t += gridDim.x * warps) {
         const int r0 = t * kTileM, r1 = min(j.M, r0 + kTileM);
         bool live = false;
         for (int s = r0 / j.T; s * j.T < r1; ++s) {
             const long long id = lane < j.T ? j.ids[static_cast<long long>(s) * j.T + lane] : 0;
-            bool pad = __all_sync(0xffffffffu, id == 0);
-            if (pad && j.per_title) {
-                // the title's T rows are one contiguous run of 16-byte pieces (pitch % 8 == 0): OR every bit of columns < d
-                const uint4* x = reinterpret_cast<const uint4*>(j.rows + static_cast<long long>(s) * j.T * j.ld_words);
-                const int per_row = static_cast<int>(j.ld_words / 4);
-                uint32_t nz = 0;
-#pragma unroll 8
-                for (int i = lane; i < j.T * per_row; i += 32) {
-                    const uint4 v = __ldg(x + i);
-                    const int c0 = 8 * (i % per_row), n = min(8, max(0, j.d - c0));  // columns of this piece below d
-                    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        nz |= w[k] & (2 * k + 1 < n ? 0x7fff7fffu : 2 * k < n ? 0x00007fffu : 0u);
-                }
-                pad = !__any_sync(0xffffffffu, nz != 0);
-            } else if (pad) {
-                pad = !row0_nonzero;
-            }
+            const bool pad = __all_sync(0xffffffffu, id == 0) && !row0_nonzero;
             live = live || !pad;
             if (lane == 0 && s * j.T >= r0) j.out.pad[s] = pad ? 1 : 0;
         }
@@ -913,10 +901,10 @@ __global__ void __launch_bounds__(kLiveTilesThreads) padding_titles_kernel(const
     compact_live_tiles(j.out.tile_flags, j.num_tiles, j.ticket, j.out.live);
 }
 
-int padding_titles(const long long* ids, long long n_seq, int T, int d, const void* rows, int ld_rows, int per_title,
-                   const float* bqkv, int sec, int ld3, PaddingTitles* out, cudaStream_t stream) {
-    NR_REQUIRE(T >= 1 && T <= 32 && d % 2 == 0 && d <= 2 * kLiveTilesThreads && ld_rows % 8 == 0 && n_seq * T < (1ll << 31),
-               "padding_titles: T=%d d=%d ld=%d", T, d, ld_rows);
+int padding_titles(const long long* ids, long long n_seq, int T, int d, const void* table, int ld_table, const float* bqkv, int sec,
+                   int ld3, PaddingTitles* out, cudaStream_t stream) {
+    NR_REQUIRE(T >= 1 && T <= 32 && d % 2 == 0 && ld_table % 8 == 0 && n_seq * T < (1ll << 31), "padding_titles: T=%d d=%d ld=%d", T,
+               d, ld_table);
     const int M = static_cast<int>(n_seq * T), num_tiles = ceil_div(M, kTileM);
     // pad flags | tile flags | ticket | live list | shared Q|K|V tile | its V low plane; stream-ordered, freed by the caller
     const size_t pad_b = round_up(static_cast<int>(n_seq), 16), head_b = round_up(static_cast<int>(pad_b) + 4 * (2 * num_tiles + 2), 128);
@@ -933,9 +921,8 @@ int padding_titles(const long long* ids, long long n_seq, int T, int d, const vo
     if (n_seq == 0) return 0;
     NR_CHECK_CUDA(cudaMemsetAsync(ticket, 0, sizeof(unsigned), stream));
     const PaddingJob j{.ids = ids, .n_seq = static_cast<int>(n_seq), .T = T, .d = d, .M = M, .num_tiles = num_tiles,
-                       .rows = static_cast<const uint32_t*>(rows), .ld_words = ld_rows / 2, .per_title = per_title, .bqkv = bqkv,
-                       .sec = sec, .ld3 = ld3, .out = *out, .ticket = ticket};
-    ProfScope ps("padding_titles", M, num_tiles, per_title, stream);
+                       .row0 = static_cast<const uint32_t*>(table), .bqkv = bqkv, .sec = sec, .ld3 = ld3, .out = *out, .ticket = ticket};
+    ProfScope ps("padding_titles", M, num_tiles, 0, stream);
     const int blocks = std::max(1, std::min(4 * num_sms(), ceil_div(num_tiles, kLiveTilesThreads / 32)));
     padding_titles_kernel<<<blocks, kLiveTilesThreads, 0, stream>>>(j);
     ++g_launches;
@@ -948,37 +935,204 @@ void free_padding_titles(PaddingTitles& pt, cudaStream_t stream) {
     pt = PaddingTitles{};
 }
 
-// dst[c * ld_dst] += sum of A[r][c] over the rows r of the tiles flagged 0 (c < N, N even): the bias column of a weight gradient
-// whose GEMM skipped those tiles because their X rows are [0 .. 0, 1].  Thread = column pair, block = 64-row tile (grid stride)
-constexpr int kDeadSumThreads = 128;
-__global__ void __launch_bounds__(kDeadSumThreads)
-dead_tiles_colsum_kernel(const __nv_bfloat16* A, int lda, int N, int M, const int* tile_flags, int num_tiles, float* dst, int ld_dst) {
-    const int cp = blockIdx.y * kDeadSumThreads + threadIdx.x;
-    if (2 * cp >= N) return;
-    float s0 = 0.f, s1 = 0.f;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        if (__ldg(tile_flags + t)) continue;
-        const int r1 = min(M, t * kTileM + kTileM);
-        const uint32_t* a = reinterpret_cast<const uint32_t*>(A + static_cast<size_t>(t) * kTileM * lda) + cp;
-#pragma unroll 8
-        for (int r = t * kTileM; r < r1; ++r, a += lda / 2) {
-            const float2 v = unpack_bf16x2(__ldg(a));
-            s0 += v.x;
-            s1 += v.y;
+// ------------------------------------------------------------------------------------------------
+// live tokens of the news encoder's backward (LiveTokens in nr_ops.h).  Block b of both kernels owns the titles
+// [32 b, 32 b + 32); one warp classifies or compacts one title at a time.
+//   classify: live mask, padding flag and live count of every title, the block's total; the last block to finish (ticket)
+//             scans the block totals into block bases and writes M' and the tile count.  Also the shared padding Q|K|V
+//             tile and the tile list body.
+//   compact:  the block's per-title offsets (a block scan of its counts on top of its base), the compact -> token index,
+//             the compact copy of the live X rows, and the zero tail rows [M', round_up(M', 64)).
+// ------------------------------------------------------------------------------------------------
+constexpr int kLiveTitlesPerBlock = 32;  // four titles per warp: about 900 blocks for a bench batch
+
+struct LiveJob {
+    const long long* ids;
+    int n_seq, T, d, M, V, n_blocks;
+    const uint32_t* row0;  // bf16 pairs: row 0 of the table, or null (the verdict from X)
+    const float* bqkv;
+    int sec, ld3, ldx;
+    const uint4* X;        // bf16 rows of pitch ldx (16-byte pieces)
+    uint4* Xc;
+    uint4* dqkv_c;
+    int* counts;           // [n_seq] live tokens per title
+    int* block_base;       // [n_blocks] live tokens of the titles before the block
+    unsigned* ticket;
+    LiveTokens out;
+};
+
+__global__ void __launch_bounds__(kLiveTilesThreads) live_classify_kernel(const LiveJob j) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
+    const bool all_live = j.row0 != nullptr && block_row_nonzero(j.row0, j.d);
+    write_padding_qkv(j.bqkv, j.T, j.sec, j.ld3, j.out.qkv, nullptr);
+    const int gtid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
+    for (int i = gtid; i < (j.M + kTileM - 1) / kTileM; i += nthreads) j.out.tiles[1 + i] = i;
+    const int px = j.ldx / 8;  // 16-byte pieces per row of X
+    const int s0 = blockIdx.x * kLiveTitlesPerBlock, s1 = min(j.n_seq, s0 + kLiveTitlesPerBlock);
+    int total = 0;  // lane 0: the live tokens of this warp's titles
+    for (int s = s0 + warp; s < s1; s += warps) {
+        const long long id = lane < j.T ? j.ids[static_cast<long long>(s) * j.T + lane] : 0;
+        uint32_t mask = __ballot_sync(0xffffffffu, lane < j.T && (all_live || (id >= 1 && id < j.V)));
+        if (j.row0 == nullptr) {  // no table: a token whose gathered row is nonzero below column d is live as well
+            for (uint32_t cand = ((j.T == 32 ? 0u : 1u << j.T) - 1u) & ~mask; cand != 0; cand &= cand - 1) {
+                const int r = __ffs(cand) - 1;
+                const uint4* x = j.X + (static_cast<long long>(s) * j.T + r) * px;
+                uint32_t nz = 0;
+                for (int c = lane; c < px; c += 32) {
+                    const uint4 v = __ldg(x + c);
+                    const int n = min(8, max(0, j.d - 8 * c));  // columns of this piece below d
+                    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) nz |= w[k] & (2 * k + 1 < n ? 0x7fff7fffu : 2 * k < n ? 0x00007fffu : 0u);
+                }
+                if (__any_sync(0xffffffffu, nz != 0)) mask |= 1u << r;
+            }
+        }
+        if (lane == 0) {
+            j.out.mask[s] = mask;
+            j.out.pad[s] = mask == 0 ? 1 : 0;
+            j.counts[s] = __popc(mask);
+            total += __popc(mask);
         }
     }
-    red_add_f32(dst + static_cast<size_t>(2 * cp) * ld_dst, s0);
-    red_add_f32(dst + static_cast<size_t>(2 * cp + 1) * ld_dst, s1);
+    __shared__ int warp_tot[kLiveTilesThreads / 32];
+    __shared__ bool last;
+    if (lane == 0) warp_tot[warp] = total;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int w = 0; w < warps; ++w) t += warp_tot[w];
+        j.block_base[blockIdx.x] = t;  // the block's total until the last block turns the totals into bases
+        __threadfence();               // the total and this block's counts are visible before its ticket
+        last = atomicAdd(j.ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    // exclusive scan of the block totals, kLiveTilesThreads at a time with a running carry
+    __shared__ int carry;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int b0 = 0; b0 < j.n_blocks; b0 += kLiveTilesThreads) {
+        const int b = b0 + threadIdx.x;
+        const int v = b < j.n_blocks ? __ldcg(j.block_base + b) : 0;
+        int incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) warp_tot[warp] = incl;
+        __syncthreads();
+        int base = carry;
+        for (int w = 0; w < warp; ++w) base += warp_tot[w];
+        if (b < j.n_blocks) j.block_base[b] = base + incl - v;
+        __syncthreads();
+        if (threadIdx.x == kLiveTilesThreads - 1) carry = base + incl;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        j.out.offset[j.n_seq] = carry;
+        j.out.tiles[0] = (carry + kTileM - 1) / kTileM;
+    }
 }
 
-int dead_tiles_colsum(const void* A, int lda, int N, int M, const int* tile_flags, float* dst, int ld_dst, cudaStream_t stream) {
-    NR_REQUIRE(N % 2 == 0 && lda % 2 == 0, "dead_tiles_colsum: N=%d lda=%d", N, lda);
-    if (M == 0) return 0;
-    const int num_tiles = ceil_div(M, kTileM);
-    ProfScope ps("dead_tiles_colsum", M, N, 0, stream);
-    const dim3 grid(std::max(1, std::min(2 * num_sms(), num_tiles)), ceil_div(N / 2, kDeadSumThreads));
-    dead_tiles_colsum_kernel<<<grid, kDeadSumThreads, 0, stream>>>(static_cast<const __nv_bfloat16*>(A), lda, N, M, tile_flags,
-                                                                  num_tiles, dst, ld_dst);
+__global__ void __launch_bounds__(kLiveTilesThreads) live_compact_kernel(const LiveJob j) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
+    const int s0 = blockIdx.x * kLiveTitlesPerBlock, s1 = min(j.n_seq, s0 + kLiveTitlesPerBlock);
+    // offsets of the block's titles: lane t of warp 0 scans title s0 + t
+    static_assert(kLiveTitlesPerBlock == 32, "one warp scans the block's titles");
+    __shared__ int off[kLiveTitlesPerBlock];
+    if (warp == 0) {
+        const int v = s0 + lane < s1 ? j.counts[s0 + lane] : 0;
+        int incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        off[lane] = j.block_base[blockIdx.x] + incl - v;
+        if (s0 + lane < s1) j.out.offset[s0 + lane] = off[lane];
+    }
+    __syncthreads();
+    // the tail rows [M', round_up(M', 64)) below M: no token, zero X and dQ|dK|dV rows (the last block)
+    const int px = j.ldx / 8, p3 = j.ld3 / 8;  // 16-byte pieces per row
+    if (blockIdx.x == gridDim.x - 1) {
+        const int m_live = j.out.offset[j.n_seq];
+        const int tail_end = min(j.M, (m_live + kTileM - 1) / kTileM * kTileM);
+        for (int r = m_live + threadIdx.x; r < tail_end; r += blockDim.x) j.out.index[r] = -1;
+        for (int i = threadIdx.x; i < (tail_end - m_live) * px; i += blockDim.x)
+            j.Xc[static_cast<long long>(m_live) * px + i] = make_uint4(0, 0, 0, 0);
+        for (int i = threadIdx.x; i < (tail_end - m_live) * p3; i += blockDim.x)
+            j.dqkv_c[static_cast<long long>(m_live) * p3 + i] = make_uint4(0, 0, 0, 0);
+    }
+    // a warp per title: the index entries, then every 16-byte piece of the title's live rows spread over the lanes
+    __shared__ int src_row[kLiveTilesThreads / 32][32];
+    for (int s = s0 + warp; s < s1; s += warps) {
+        const uint32_t mask = j.out.mask[s];
+        const int dst = off[s - s0], n_live = __popc(mask);
+        const int rank = __popc(mask & ((1u << lane) - 1u));
+        if (lane < j.T && ((mask >> lane) & 1u)) {
+            j.out.index[dst + rank] = s * j.T + lane;
+            src_row[warp][rank] = s * j.T + lane;
+        }
+        __syncwarp();
+        const uint4* X = j.X;
+        uint4* Xc = j.Xc + static_cast<long long>(dst) * px;
+#pragma unroll 4
+        for (int i = lane; i < n_live * px; i += 32) {
+            const int k = i / px, c = i - k * px;
+            Xc[i] = __ldg(X + static_cast<long long>(src_row[warp][k]) * px + c);
+        }
+        __syncwarp();
+    }
+}
+
+// bytes of the LiveTokens buffers of a call (live_tokens carves them from `buf`)
+long long live_tokens_bytes(long long n_seq, int T, int ld3) {
+    const long long n = n_seq, M = n_seq * T, nb = (n + kLiveTitlesPerBlock - 1) / kLiveTitlesPerBlock;
+    WorkspaceLayout l{nullptr};
+    l.take<unsigned char>(n);           // pad
+    l.take<uint32_t>(n);                // mask
+    l.take<int>(n);                     // counts
+    l.take<int>(n + 1);                 // offset
+    l.take<int>(M);                     // index
+    l.take<int>(M / kTileM + 2);        // tiles
+    l.take<int>(nb + 1);                // block bases | ticket
+    l.take<__nv_bfloat16>(static_cast<long long>(T) * ld3);  // shared Q|K|V tile
+    return l.bytes();
+}
+
+int live_tokens(const long long* ids, long long n_seq, int T, int d, const void* table, int ld_table, int V, const float* bqkv,
+                int sec, int ld3, const void* X, int ldx, void* Xc, void* dqkv_c, void* buf, long long buf_bytes, LiveTokens* out,
+                cudaStream_t stream) {
+    NR_REQUIRE(ids && bqkv && X && Xc && dqkv_c && buf, "live_tokens: null operand");
+    NR_REQUIRE(T >= 1 && T <= 32 && d % 2 == 0 && ld_table % 8 == 0 && ldx % 8 == 0 && ld3 % 8 == 0 && V >= 1 && n_seq * T < (1ll << 31),
+               "live_tokens: T=%d d=%d ld_table=%d ldx=%d ld3=%d V=%d", T, d, ld_table, ldx, ld3, V);
+    const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    NR_REQUIRE(a16(X) && a16(Xc) && a16(dqkv_c) && a16(buf), "live_tokens: rows not 16-byte aligned");
+    NR_REQUIRE(buf_bytes >= live_tokens_bytes(n_seq, T, ld3), "live_tokens: buffer too small (%lld bytes)", buf_bytes);
+    const int n = static_cast<int>(n_seq), M = n * T, nb = ceil_div(n, kLiveTitlesPerBlock);
+    WorkspaceLayout l{static_cast<char*>(buf)};
+    out->pad = l.take<unsigned char>(n);
+    out->mask = l.take<uint32_t>(n);
+    int* counts = l.take<int>(n);
+    out->offset = l.take<int>(n + 1);
+    out->index = l.take<int>(M);
+    out->tiles = l.take<int>(M / kTileM + 2);
+    int* block_base = l.take<int>(nb + 1);
+    out->qkv = l.take<__nv_bfloat16>(static_cast<long long>(T) * ld3);
+    if (n == 0) return 0;
+    unsigned* ticket = reinterpret_cast<unsigned*>(block_base + nb);
+    NR_CHECK_CUDA(cudaMemsetAsync(ticket, 0, sizeof(unsigned), stream));
+    const LiveJob j{.ids = ids, .n_seq = n, .T = T, .d = d, .M = M, .V = V, .n_blocks = nb, .row0 = static_cast<const uint32_t*>(table),
+                    .bqkv = bqkv, .sec = sec, .ld3 = ld3, .ldx = ldx, .X = static_cast<const uint4*>(X), .Xc = static_cast<uint4*>(Xc),
+                    .dqkv_c = static_cast<uint4*>(dqkv_c), .counts = counts, .block_base = block_base, .ticket = ticket, .out = *out};
+    ProfScope ps("live_tokens", M, n, 0, stream);
+    live_classify_kernel<<<nb, kLiveTilesThreads, 0, stream>>>(j);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    live_compact_kernel<<<nb, kLiveTilesThreads, 0, stream>>>(j);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -991,7 +1145,15 @@ int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t
     NR_PROPAGATE(plan_gemm_nt(&plan, g.A, g.M, g.lda, g.W, g.N, g.ldw, g.K, g.taps, g.w_tap_rows, kTileM, num_sms(), 0,
                               kEpiSmemBytes<EpiScatter>, 0));
     NR_PROPAGATE(apply_tap_origin(plan, g));
-    const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = Dropout::make(c.drop.p, c.drop.seed), .drop_ld = c.drop_ld};
+    const EpiScatter e{.ids = c.ids, .demb = c.demb, .V = c.V, .D = g.N, .rm = to_rm(c.rm), .drop = Dropout::make(c.drop.p, c.drop.seed),
+                       .drop_ld = c.drop_ld, .rows = c.rows};
+    NR_REQUIRE(c.rows == nullptr || c.rm.seg_in == 0, "scatter_emb: compact rows need the identity row map");
+    if (c.tile_list != nullptr) {  // the caller knows the tiles with a live token
+        plan.p.tile_list = c.tile_list;
+        g_launches += debug_simt_gemm() ? 2 : 1;
+        ProfScope ps("gemm_scatter_emb", g.M, g.N, g.K * g.taps, stream);
+        return launch_gemm_nt(plan, e, g.A, g.lda, g.W, g.ldw, stream);
+    }
     const int num_tiles = plan.p.num_m_tiles;
     // [0, num_tiles) flags | ticket | list (count + tiles); stream-ordered, so the buffer lives exactly as long as the two launches
     int* buf = nullptr;

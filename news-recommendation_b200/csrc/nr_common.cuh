@@ -190,6 +190,10 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
     tma_store_2d(m, smem_u32(smem_src), c0, c1);
 }
+// bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) from shared to global memory (bulk async-group completion)
+__device__ __forceinline__ void bulk_store_1d(void* gdst, uint32_t smem_src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_src), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() {  // at most N groups of this thread still reading shared memory

@@ -809,6 +809,7 @@ struct EpiScatter {
     RowMap rm;             // maps the GEMM row to the token index in ids
     Dropout drop;
     int drop_ld;           // pitch used when the forward mask was drawn
+    const int* rows;       // null, or compact rows: GEMM row r is token rows[r] (none when negative), its id and dropout row
 
     __device__ void init(const EpiInit&, int) const {}
     __device__ void finish(const EpiInit&) const {}
@@ -817,7 +818,15 @@ struct EpiScatter {
     __device__ __forceinline__ void operator()(const Acc& acc, const EpiCtx& c) const {
         long long trow;
         int t;
-        const bool v = rm.map(c.grow, trow, t) && c.valid;
+        bool v;
+        int drow = c.grow;  // the row the forward's dropout mask was drawn at
+        if (rows != nullptr) {
+            drow = c.valid ? rows[c.grow] : -1;
+            trow = drow;
+            v = drow >= 0;
+        } else {
+            v = rm.map(c.grow, trow, t) && c.valid;
+        }
         long long id = v ? ids[trow] : 0;
         if (id < 0 || id >= V) id = 0;  // out of range: skipped like the padding row
         float* dst = demb + static_cast<size_t>(id) * D;
@@ -833,7 +842,7 @@ struct EpiScatter {
                     float y[4] = {x[g * 4], x[g * 4 + 1], x[g * 4 + 2], x[g * 4 + 3]};
                     if (drop.active()) {
                         float m[4];
-                        drop.mask4(c.grow, drop_ld, col, m);
+                        drop.mask4(drow, drop_ld, col, m);
 #pragma unroll
                         for (int j = 0; j < 4; ++j) y[j] *= m[j];
                     }

@@ -90,6 +90,10 @@ struct ScatterEmbCfg {
     RowMapCfg rm = {};
     DropoutCfg drop = {};
     int drop_ld = 0;
+    // compact rows (LiveTokens): GEMM row r is token rows[r] (no token when negative; rm must be the identity), whose id and
+    // dropout row it takes; tile_list (device, GemmNTParams::tile_list layout) replaces the scan for tiles with a live token
+    const int* rows = nullptr;
+    const int* tile_list = nullptr;
 };
 int gemm_scatter_emb(const GemmOperands& g, const ScatterEmbCfg& c, cudaStream_t stream);
 
@@ -102,11 +106,10 @@ int gemm_tn_accumulate(const void* A, int Kr, int Ma, int lda, const void* B, in
 int gemm_weight_grad(const void* dY, int M, int N, int ld_dy, const void* X, int K, int ldx, float* dW_ext, cudaStream_t stream,
                      int x_row_shift = 0, const int* k_list = nullptr);
 
-// Padding titles of the news encoder.  Title s is padding when its T ids are all 0 and the rows the projection reads for it are
-// exact zeros: row 0 of the bf16 table in the forward (per_title 0; padding_idx=0 keeps it zero, a pretrained table may not),
-// the title's own gathered rows X in the backward (per_title 1).  Such a title's X rows are [0 .. 0, 1], so its Q|K|V rows are
-// the bias rows in `qkv` below and its only weight-gradient term is its dQ|dK|dV rows in the bias column.  A 64-row tile is
-// live when it holds a row of a title that is not padding.  Nothing is read back to the host.
+// Padding titles of the news encoder's forward.  Title s is padding when its T ids are all 0 and row 0 of the bf16 table is an
+// exact zero row (padding_idx=0 keeps it zero, a pretrained table may not).  Such a title's X rows are [0 .. 0, 1], so its
+// Q|K|V rows are the bias rows in `qkv` below.  A 64-row tile is live when it holds a row of a title that is not padding.
+// Nothing is read back to the host.
 struct PaddingTitles {
     unsigned char* pad = nullptr;  // [n_seq] 1 = padding title
     int* tile_flags = nullptr;     // [ceil(n_seq * T / 64)] 1 = live tile
@@ -115,14 +118,34 @@ struct PaddingTitles {
     void* v_lo = nullptr;          // with bqkv: bf16 [T][sec] low plane of its V section, bf16(b - bf16(b))
     void* base = nullptr;          // the one stream-ordered allocation behind the buffers above
 };
-// rows: the table (per_title 0) or X (per_title 1), pitch ld_rows; d even, T <= 32.  Allocates on `stream`; free_padding_titles
-// releases the buffers once every launch that reads them has been enqueued.
-int padding_titles(const long long* ids, long long n_seq, int T, int d, const void* rows, int ld_rows, int per_title,
-                   const float* bqkv, int sec, int ld3, PaddingTitles* out, cudaStream_t stream);
+// table: the bf16 embedding table, pitch ld_table; d even, T <= 32.  Allocates on `stream`; free_padding_titles releases the
+// buffers once every launch that reads them has been enqueued.
+int padding_titles(const long long* ids, long long n_seq, int T, int d, const void* table, int ld_table, const float* bqkv, int sec,
+                   int ld3, PaddingTitles* out, cudaStream_t stream);
 void free_padding_titles(PaddingTitles& pt, cudaStream_t stream);
-// dst[c * ld_dst] += sum over the rows of the tiles with tile_flags 0 of A[r][c], c < N (the bias column of a weight gradient
-// whose GEMM skipped those tiles)
-int dead_tiles_colsum(const void* A, int lda, int N, int M, const int* tile_flags, float* dst, int ld_dst, cudaStream_t stream);
+
+// Live tokens of the news encoder's backward.  Token r is live when its id is in [1, V), or when row 0 of the bf16 table is
+// nonzero (then every token is).  A dead token's gathered row is [0 .. 0, 1] (gather_rows reads an out-of-range id as row 0),
+// so its dQ|dK|dV row adds nothing to the embedding gradient and reaches the weight gradient only through the bias column.
+// The compact order lists the live tokens in ascending token order.  A title without a live token is a padding title: the
+// same verdict as padding_titles, from the same ids and table row.  Nothing is read back to the host.
+struct LiveTokens {
+    unsigned char* pad = nullptr;  // [n_seq] 1 = padding title (mask 0)
+    uint32_t* mask = nullptr;      // [n_seq] bit t: token t of the title is live
+    int* offset = nullptr;         // [n_seq + 1] exclusive scan of the masks' popcounts; offset[n_seq] = M', the live tokens
+    int* index = nullptr;          // [n_seq * T] compact row -> token; -1 on the rows [M', round_up(M', 64)) below n_seq * T
+    int* tiles = nullptr;          // the compact 64-row tiles 0 .. ceil(M' / 64) - 1 in GemmNTParams::tile_list layout
+    void* qkv = nullptr;           // bf16 [T][ld3] Q|K|V of a padding title (every row bf16(b_qkv))
+};
+// table null: a token is live when its id is in [1, V) or its row of X is nonzero below column d (the same tokens, found by
+// reading X; a dead token's row is [0 .. 0, 1] either way).  Also copies the live rows of X (bf16, pitch ldx) to Xc in
+// compact order and writes zeros to the rows [M', round_up(M', 64)) below n_seq * T of Xc and of dqkv_c (bf16, pitch ld3),
+// the rows a 64-row tile of the compact GEMMs reads past M'.  d even, T <= 32.  The buffers of `out` are carved from `buf`
+// (16-byte aligned, live_tokens_bytes(n_seq, T, ld3) bytes): nothing is allocated, nothing is read back to the host.
+long long live_tokens_bytes(long long n_seq, int T, int ld3);
+int live_tokens(const long long* ids, long long n_seq, int T, int d, const void* table, int ld_table, int V, const float* bqkv,
+                int sec, int ld3, const void* X, int ldx, void* Xc, void* dqkv_c, void* buf, long long buf_bytes, LiveTokens* out,
+                cudaStream_t stream);
 
 // ---- memory-bound companions (aux.cu) --------------------------------------------------------------
 // fp32 rows -> zero-padded bf16 planes: every operand cast, dense-input conversion and hi/lo split in front of a GEMM.
@@ -162,12 +185,18 @@ int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cud
 // X may be wider than the table (ld_x >= ld_table): only its first ld_table columns are written.
 int gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld_table, void* X,
                 int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream);
+// the news encoder's backward over live tokens (LiveTokens above): what the title-level attention backward needs of it
+struct TitleBwdLive {
+    const LiveTokens* tokens;
+    float* dbias;  // the bias column of the Q|K|V weight gradient
+    int ld_dbias;
+};
 // multi-head self attention core on packed Q|K|V bf16 [n_seq*T x ld_qkv]: sections start at columns 0, sec, 2*sec
 // (sec >= d = heads*dk; dQKV uses the same sections)
 int mhsa_core_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int T, int heads, int dk, void* ctx, int ld_ctx,
                   DropoutCfg drop, cudaStream_t stream);
 int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int T, int heads, int dk,
-                  void* dqkv, int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad = nullptr);
+                  void* dqkv, int ld_dqkv, cudaStream_t stream, const TitleBwdLive* live = nullptr);
 // title-level backward (attn_title.cu): T = 20, d_k = 20, <= 15 heads, sections with a 16-byte phase (sec % 8 == 0)
 bool mhsa_title_fwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int ld_ctx);
 // pad (PaddingTitles, may be null): the padding titles take their Q|K|V rows (and V low plane) from pad->qkv / pad->v_lo, not
@@ -176,8 +205,11 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
                    cudaStream_t stream, const void* v_lo = nullptr, int ld_vlo = 0, void* ctx_lo = nullptr,
                    const PaddingTitles* pad = nullptr);
 bool mhsa_title_bwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int ld_dctx, int ld_dqkv);
+// live (may be null): the padding titles take their Q|K|V rows from live->tokens->qkv; only the live tokens' dQ|dK|dV rows are
+// stored, in compact order (row live->tokens->offset[s] + rank of the token among its title's live tokens); the bf16-rounded
+// dQ|dK|dV rows of the dead tokens are summed into dbias[c * ld_dbias] (+=), c < 3 * sec
 int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld_dctx, long long n_seq, int heads, void* dqkv,
-                   int ld_dqkv, cudaStream_t stream, const PaddingTitles* pad = nullptr);
+                   int ld_dqkv, cudaStream_t stream, const TitleBwdLive* live = nullptr);
 // dscore_r = w_r (dw_r - sum_seg w dw), dw_r = dOut[seg] . X_r
 int pool_dscore(const void* X, int lda, int D, long long n_seg, int seg_len, const float* w, const float* dout, int ldo,
                 float* dscore, cudaStream_t stream);

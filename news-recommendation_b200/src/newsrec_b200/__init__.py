@@ -42,7 +42,7 @@ class MhsaEncoderBwdArgs(C.Structure):
         ("dWqkv_ext", _vp), ("dWa_ext", _vp), ("dqv", _vp), ("demb", _vp), ("ddense", _vp),
         ("workspace", _vp), ("workspace_bytes", _ll),
         ("wqkv_bf16", _vp), ("bqkv", _vp), ("emb_grad_ready_event", _vp),
-        ("dpos", _vp),
+        ("dpos", _vp), ("table_bf16", _vp),
     ]
 
 
@@ -150,6 +150,7 @@ SIGNATURES = {
     "nr_has_triage_backends": (_i, []),
     "nr_reserve_sms_for_comm": (None, [_i]),
     "nr_debug_set_gemm_timing": (None, [_vp, _i]),
+    "nr_debug_live_tokens": (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nr_profile_enable": (None, [_i]),
     "nr_profile_context": (None, [C.c_char_p]),
     "nr_profile_report": (_i, [C.c_char_p, _i]),

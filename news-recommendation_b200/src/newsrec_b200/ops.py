@@ -266,7 +266,7 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
                         has_ids=ids is not None, V=emb_w.shape[0] if ids is not None else 0,
                         dense_shape=None if dense is None else tuple(dense.shape),
                         params=(emb_w, Wq, bq, Wk, bk, Wv, bv, Wa, ba, qv), cache=cache, prefix=prefix,
-                        pos=pos)
+                        pos=pos, table=table)
         return out
 
     @staticmethod
@@ -317,6 +317,7 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
         a.n_seq, a.T, a.d, a.heads, a.q, a.ldx, a.ld3, a.ldq = n_seq, T, d, m["heads"], q, ldx, ld3, ldq
         a.ids = _p(ids) if m["has_ids"] else None
         a.V = m["V"]
+        a.table_bf16 = _p(m["table"]) if m["has_ids"] else None  # the forward's table: its row 0 decides which tokens are live
         a.wqkvT_bf16, a.wa_bf16, a.waT_bf16, a.ba, a.qv = _p(ops["wqkvT"]), _p(ops["wa"]), _p(ops["waT"]), _p(ops["ba"]), _p(ops["qv"])
         a.p_drop, a.seed = m["p_drop"], m["seed"]
         a.X_bf16, a.QKV_bf16, a.C_bf16, a.w, a.dout = _p(X), (_p(QKV) if QKV.numel() else None), _p(Cx), _p(w), _p(dout)
