@@ -287,6 +287,39 @@ int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, cons
                        long long* idx, float* score, int* bad_row_flag, int* bad_score_flag, void* workspace,
                        long long workspace_bytes, void* stream);
 
+/* Maximal-marginal-relevance (MMR) re-ranking of nr_topk_dot's shortlists (content-diversified recommendation).  news fp32
+ * [n_news][ld_news] (pitch >= D), the pool nr_topk_dot scored; shortlist_idx int64 / shortlist_score fp32 [n_users][depth],
+ * nr_topk_dot's output at k = depth.  For user u:
+ *   shortlist  C_u = the entries before the first -1 (the live ones, L_u <= depth of them; entries after the first -1 are
+ *              ignored), in their order (nr_topk_dot's: score descending, then lower row);
+ *   relevance  rel_i = (s_i - s_min) / (s_max - s_min) over C_u, s_i the score bits given; rel_i = 1 for all i when
+ *              s_max == s_min.  Dot-product scores have a model-dependent scale, so lambda means the same for every model;
+ *   similarity sim(i, j) = the cosine of the fp32 news rows i and j, 0 when either row is all zeros;
+ *   greedy     S = {}; for t = 0 .. min(k, L_u) - 1 take the i of C_u \ S that maximises
+ *                  obj_i = lambda rel_i - (1 - lambda) max_{j in S} sim(i, j)      (the max over {} is 0),
+ *              equal objectives going to the lower shortlist position.
+ * Outputs idx int64 [n_users][k] and score fp32 [n_users][k] in pick order; score holds the shortlist's own score bits of
+ * the picked rows; the slots after the last pick hold -1 / -inf (nr_topk_dot's shapes and padding).  Exact, bit for bit:
+ * lambda = 1 gives nr_topk_dot's k-list (obj is rel exactly, and rel never increases along the shortlist); depth == k gives
+ * the shortlist's set, reordered; the same inputs give the same bits on every run.
+ * Bounds.  Each block of 64 columns of the live rows is gathered and split into hi/lo bf16 (hi = bf16(x), lo = bf16(x - hi))
+ * and the Gram G = hi.lo + lo.hi + hi.hi runs on the tensor cores with fp32 accumulation, so, as for nr_topk_dot's scores,
+ *     |G_ij - x_i.x_j| <= eps sum_d |x_id||x_jd| <= eps |x_i||x_j|,    eps = 2^-15 + 3 round_up(D, 64) 2^-23.
+ * The norms come from the diagonal (G_ii = |x_i|^2 (1 + t_i), |t_i| <= eps) and sim(i, j) = (G_ji rsqrt(G_jj)) rsqrt(G_ii)
+ * in correctly rounded fp32 (0 when G_ii or G_jj is 0), so with c = 2 / (1 - eps), against the exact cosine of the inputs:
+ *     e_sim = c eps + 2^-21
+ * (the 1 / sqrt((1 + t_i)(1 + t_j)) factor is within eps / (1 - eps) of 1 and the error of G_ij is within eps / (1 - eps) of the
+ * cosine's scale after it; four roundings on a value below 1 + c eps add at most 2^-21).  rel and obj are rounded once per
+ * operation (no contraction), so against obj evaluated in fp64 on the same score bits, the same fp32 lambda and the exact
+ * cosines:
+ *     e_obj = (1 - lambda) e_sim + 2^-20,
+ * and each pick's fp64 objective is within 2 e_obj of the best remaining one.  The bounds assume finite scores and rows whose
+ * squared norms are fp32 normal numbers.  Limits: 1 <= D <= 4096; 1 <= k <= depth <= 128; lambda finite in [0, 1];
+ * n_users and n_news in [0, 2^31 - 64).  A live shortlist row outside [0, n_news) sets *bad_row_flag (the user's list is then
+ * undefined).  Every limit is refused (-1) before the first launch; n_users == 0 launches nothing.  Runs on the stream given. */
+int nr_mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* shortlist_idx, const float* shortlist_score,
+                  long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag, void* stream);
+
 /* Ranks over a whole news pool under nr_topk_dot's scores.  Query row q (queries fp32 [n_rows][ld_queries]) has the target
  * set T_q = tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) and the exclusion set X_q (excl_offsets / excl_rows as in
  * nr_topk_dot: both null, or both device int64; a set, any length, order or duplicates).  For every target t of q:

@@ -233,6 +233,12 @@ int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, cons
     return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, categories, max_per_category,
                     idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
 }
+int nr_mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* shortlist_idx, const float* shortlist_score,
+                  long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag, void* stream) {
+    NR_REQUIRE(news && shortlist_idx && shortlist_score && idx && score && bad_row_flag, "nr_mmr_rerank: null operand");
+    return mmr_rerank(news, n_news, ld_news, D, shortlist_idx, shortlist_score, n_users, depth, k, lambda, idx, score, bad_row_flag,
+                      as_stream(stream));
+}
 long long nr_pool_ranks_workspace(long long n_rows, long long n_news, int D) { return pool_ranks_workspace(n_rows, n_news, D); }
 int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
                   const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,

@@ -286,6 +286,10 @@ int pool_ranks(const float* queries, long long n_rows, int ld_queries, const flo
                const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
                long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                long long workspace_bytes, cudaStream_t stream);
+// maximal-marginal-relevance re-ranking of nr_topk_dot's shortlists (topk.cu; include/newsrec_b200.h, nr_mmr_rerank)
+int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* sl_idx, const float* sl_score,
+               long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag,
+               cudaStream_t stream);
 int num_sms();
 extern int g_launches;  // kernels launched by this library (nr_launch_count)
 

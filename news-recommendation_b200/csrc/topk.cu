@@ -37,6 +37,10 @@
 // output order).  Membership goes through a per-row bit filter of the targets and exclusions: a filter hit is queued and
 // checked after the tile by the whole warpgroup, one entry per thread, so one lane's scan never stalls its warp.  Splits add
 // integer counts, so the ranks do not depend on the order of anything.
+//
+// MMR re-ranking (nr_mmr_rerank): one block per user re-ranks nr_topk_dot's shortlist (<= 128 entries).  The live rows are
+// gathered and split into hi/lo planes in the swizzled layout the TMA boxes above have, their Gram runs on the same three
+// products, and the greedy reads the Gram from shared memory.  The bounds and their derivation are in the header and DESIGN §3.
 #include <algorithm>
 #include <cmath>
 
@@ -699,6 +703,208 @@ __global__ void __launch_bounds__(128) pool_ranks_merge_kernel(const RankParams 
     }
 }
 
+// ---- maximal-marginal-relevance re-ranking of a shortlist (nr_mmr_rerank) ----
+constexpr int kMmrDepth = 128;                 // shortlist entries per user, at most
+constexpr int kMmrThreads = 256;               // two warpgroups: Gram rows [0, 64) and [64, 128)
+constexpr int kMmrPlane = kMmrDepth * 128;     // one 64-column chunk of 128 rows, bf16, 128-byte swizzled (two kBox)
+constexpr int kMmrGramLd = kMmrDepth + 8;      // fp32 Gram pitch: the fragment stores and the row reads are conflict free
+constexpr size_t kMmrBuf = 2 * 2 * kMmrPlane;  // two chunk buffers of hi | lo planes
+constexpr size_t kMmrGram = size_t(kMmrDepth) * kMmrGramLd * 4;  // aliases the buffers once the last chunk is done
+constexpr size_t kMmrSmem = 1024 + (kMmrBuf > kMmrGram ? kMmrBuf : kMmrGram) + 1024;
+static_assert(kMmrSmem <= 232448, "mmr_rerank_kernel: shared memory");
+
+struct MmrParams {
+    const float* news;
+    long long n_news, n_users;
+    int ld, D, k_chunks, depth, k;
+    bool vec4;                // news and ld allow 16-byte loads
+    float lam, one_minus_lam;
+    const long long* sl_idx;  // [n_users][depth] nr_topk_dot's list
+    const float* sl_score;
+    long long* idx;           // [n_users][k]
+    float* score;
+    int* bad_row_flag;
+};
+
+// chunk c (columns [64c, 64c + 64)) of the shortlist's rows into hi / lo planes, rows at and past live zero: thread t
+// converts the 16-byte pieces t, t + 256, ... (row q / 8, piece q % 8, which lands at piece (q % 8) ^ (row % 8))
+__device__ __forceinline__ void mmr_gather_chunk(const MmrParams& p, const int* rows, int live, int c, uint8_t* buf) {
+    for (int q = threadIdx.x; q < kMmrDepth * 8; q += kMmrThreads) {
+        const int r = q >> 3, j = q & 7, col0 = c * 64 + 8 * j;
+        float x[8];
+        const int row = r < live ? rows[r] : -1;
+        const float* src = p.news + static_cast<long long>(row < 0 ? 0 : row) * p.ld + col0;
+        if (row >= 0 && p.vec4 && col0 + 8 <= p.D) {
+            const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src + 4));
+            x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w;
+            x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) x[e] = row >= 0 && col0 + e < p.D ? __ldg(src + e) : 0.f;
+        }
+        uint32_t h[4], l[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float h0 = bf16_round(x[2 * e]), h1 = bf16_round(x[2 * e + 1]);
+            h[e] = pack_bf16x2(h0, h1);
+            l[e] = pack_bf16x2(x[2 * e] - h0, x[2 * e + 1] - h1);
+        }
+        const int off = r * 128 + ((j ^ (r & 7)) << 4);
+        *reinterpret_cast<uint4*>(buf + off) = make_uint4(h[0], h[1], h[2], h[3]);
+        *reinterpret_cast<uint4*>(buf + kMmrPlane + off) = make_uint4(l[0], l[1], l[2], l[3]);
+    }
+}
+
+// one block per user.  Gram G[i][j] of the live rows (hi.lo + lo.hi + hi.hi on wgmma, m64n128 per warpgroup, the gather of
+// chunk c + 1 under the MMAs of chunk c), then the greedy on warpgroup 0, one thread per shortlist position
+__global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    float* G = reinterpret_cast<float*>(base);  // [kMmrDepth][kMmrGramLd], after the last chunk
+    __shared__ int rows[kMmrDepth];
+    __shared__ float rn[kMmrDepth];                    // 1 / |row| from the diagonal, 0 for a zero row
+    __shared__ float red_s[2][4];                      // per-warp (objective or score) and position of a step
+    __shared__ int red_i[2][4];
+    __shared__ int s_live;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const long long u = blockIdx.x;
+    const long long* sl_idx = p.sl_idx + u * p.depth;
+    const float* sl_score = p.sl_score + u * p.depth;
+
+    // ---- the live entries: those before the first -1; a row outside [0, n_news) is flagged and reads as zeros ----
+    if (tid == 0) s_live = p.depth;
+    __syncthreads();
+    const long long r = tid < p.depth ? sl_idx[tid] : -1;
+    if (tid < p.depth && r == -1) atomicMin(&s_live, tid);
+    __syncthreads();
+    const int live = s_live;
+    if (tid < live) {
+        const bool ok = r >= 0 && r < p.n_news;
+        if (!ok) atomicOr(p.bad_row_flag, 1);
+        rows[tid] = ok ? static_cast<int>(r) : -1;
+    }
+    __syncthreads();
+
+    // ---- Gram ----
+    float acc[kMmrDepth / 2];
+#pragma unroll
+    for (int i = 0; i < kMmrDepth / 2; ++i) acc[i] = 0.f;
+    mmr_gather_chunk(p, rows, live, 0, base);
+    fence_proxy_async();
+    __syncthreads();
+    // every warpgroup issues its MMAs on every chunk (rows past live are zeros): a warpgroup-divergent wgmma is serialised
+    for (int c = 0; c < p.k_chunks; ++c) {
+        const uint32_t a = smem_u32(base + (c & 1) * 2 * kMmrPlane);
+        const uint64_t dAh = make_sw128_desc(a + wg * kBox, 16, 1024), dAl = make_sw128_desc(a + kMmrPlane + wg * kBox, 16, 1024);
+        const uint64_t dBh = make_sw128_desc(a, 16, 1024), dBl = make_sw128_desc(a + kMmrPlane, 16, 1024);
+#pragma unroll
+        for (int i = 0; i < kMmrDepth / 2; ++i) wgmma_reg_fence(acc[i]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            Wgmma<kMmrDepth, 0, 0>::mma(acc, dAh + 2 * k, dBl + 2 * k, 1);
+            Wgmma<kMmrDepth, 0, 0>::mma(acc, dAl + 2 * k, dBh + 2 * k, 1);
+            Wgmma<kMmrDepth, 0, 0>::mma(acc, dAh + 2 * k, dBh + 2 * k, 1);
+        }
+        wgmma_commit();
+        // the other buffer was last read by chunk c - 1's MMAs, which every warpgroup waited for before the barrier
+        if (c + 1 < p.k_chunks) mmr_gather_chunk(p, rows, live, c + 1, base + ((c + 1) & 1) * 2 * kMmrPlane);
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < kMmrDepth / 2; ++i) wgmma_reg_fence(acc[i]);
+        fence_proxy_async();
+        __syncthreads();
+    }
+    // fragment of m64n128 (nr_wgmma.cuh): acc[4j + 2e + i] = row 64 wg + 16 (warp % 4) + lane / 4 + 8e, column 8j + 2 (lane % 4) + i
+#pragma unroll
+    for (int j = 0; j < kMmrDepth / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int row = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * e, col = 8 * j + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(G + row * kMmrGramLd + col) = make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]);
+        }
+    __syncthreads();
+    if (wg != 0) return;
+
+    // ---- relevance: (s_i - s_min) / (s_max - s_min) over the live entries, 1 when they are all equal ----
+    const int i = tid;
+    const bool is_live = i < live;
+    const float s = is_live ? sl_score[i] : 0.f;
+    float smax = is_live ? s : -INFINITY, smin = is_live ? s : INFINITY;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        smax = fmaxf(smax, __shfl_xor_sync(~0u, smax, o));
+        smin = fminf(smin, __shfl_xor_sync(~0u, smin, o));
+    }
+    if (lane == 0) {
+        red_s[0][warp] = smax;
+        red_s[1][warp] = smin;
+    }
+    if (is_live) {
+        const float g = G[i * kMmrGramLd + i];
+        rn[i] = g > 0.f ? __frsqrt_rn(g) : 0.f;
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    smax = fmaxf(fmaxf(red_s[0][0], red_s[0][1]), fmaxf(red_s[0][2], red_s[0][3]));
+    smin = fminf(fminf(red_s[1][0], red_s[1][1]), fminf(red_s[1][2], red_s[1][3]));
+    const float rel = smax == smin ? 1.f : __fdiv_rn(__fsub_rn(s, smin), __fsub_rn(smax, smin));
+    const float rn_i = is_live ? rn[i] : 0.f;
+    asm volatile("bar.sync 1, 128;" ::: "memory");  // red_s is reused by the steps
+
+    // ---- greedy: obj_i = lam rel_i - (1 - lam) max_{j in S} sim(i, j) (0 over the empty S), the largest wins, equal
+    // objectives go to the lower position; every product and difference is rounded on its own (no contraction), so lam = 1
+    // gives obj = rel exactly ----
+    const int picks = min(p.k, live);
+    bool taken = !is_live;
+    float msim = 0.f;
+    long long* out_idx = p.idx + u * p.k;
+    float* out_score = p.score + u * p.k;
+    for (int t = 0; t < picks; ++t) {
+        // a taken or dead entry is (-inf, i + 128): it loses to every open one, and best is always a position
+        float ob = taken ? -INFINITY : __fsub_rn(__fmul_rn(p.lam, rel), __fmul_rn(p.one_minus_lam, msim));
+        if (ob != ob) ob = -INFINITY;  // only a non-finite input gets here
+        int pos = taken ? i + 128 : i;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob2 = __shfl_xor_sync(~0u, ob, o);
+            const int pos2 = __shfl_xor_sync(~0u, pos, o);
+            if (ob2 > ob || (ob2 == ob && pos2 < pos)) {
+                ob = ob2;
+                pos = pos2;
+            }
+        }
+        if (lane == 0) {
+            red_s[t & 1][warp] = ob;
+            red_i[t & 1][warp] = pos;
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");  // one barrier per step: the slots alternate
+        int best = red_i[t & 1][0];
+        float bo = red_s[t & 1][0];
+#pragma unroll
+        for (int w = 1; w < 4; ++w) {
+            const float o2 = red_s[t & 1][w];
+            const int p2 = red_i[t & 1][w];
+            if (o2 > bo || (o2 == bo && p2 < best)) {
+                bo = o2;
+                best = p2;
+            }
+        }
+        best &= kMmrDepth - 1;
+        if (i == best) {
+            taken = true;
+            out_idx[t] = sl_idx[i];
+            out_score[t] = s;
+        }
+        // sim(i, best) = (G[best][i] / |best|) / |i|: row best of the Gram
+        const float sim = __fmul_rn(__fmul_rn(G[best * kMmrGramLd + i], rn[best]), rn_i);
+        msim = t == 0 ? sim : fmaxf(msim, sim);
+    }
+    for (int t = picks + i; t < p.k; t += 128) {
+        out_idx[t] = -1;
+        out_score[t] = -INFINITY;
+    }
+}
+
 }  // namespace topk
 
 static int topk_splits(long long n_users, long long n_news) {
@@ -889,6 +1095,47 @@ int pool_ranks(const float* queries, long long n_rows, int ld_queries, const flo
         ++g_launches;
         NR_CHECK_CUDA(cudaGetLastError());
     }
+    return 0;
+}
+
+int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* sl_idx, const float* sl_score,
+               long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag,
+               cudaStream_t stream) {
+    using namespace topk;
+    NR_REQUIRE(D >= 1 && D <= 4096, "nr_mmr_rerank: D=%d outside [1, 4096]", D);
+    NR_REQUIRE(ld_news >= D, "nr_mmr_rerank: pitch ld_news=%d below D=%d", ld_news, D);
+    NR_REQUIRE(n_news >= 0 && n_news < (1ll << 31) - kNews, "nr_mmr_rerank: n_news=%lld outside [0, 2^31 - 64)", n_news);
+    NR_REQUIRE(n_users >= 0 && n_users < (1ll << 31) - kUsers, "nr_mmr_rerank: n_users=%lld outside [0, 2^31 - 64)", n_users);
+    NR_REQUIRE(depth >= 1 && depth <= kMmrDepth, "nr_mmr_rerank: depth=%d outside [1, %d]", depth, kMmrDepth);
+    NR_REQUIRE(k >= 1 && k <= depth, "nr_mmr_rerank: k=%d outside [1, depth=%d]", k, depth);
+    NR_REQUIRE(lambda >= 0.f && lambda <= 1.f, "nr_mmr_rerank: lambda=%g outside [0, 1]", static_cast<double>(lambda));
+    if (n_users == 0) return 0;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NR_CHECK_CUDA(cudaFuncSetAttribute(mmr_rerank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kMmrSmem)));
+        attr_set = true;
+    }
+    MmrParams p;
+    p.news = news;
+    p.n_news = n_news;
+    p.n_users = n_users;
+    p.ld = ld_news;
+    p.D = D;
+    p.k_chunks = ceil_div(D, 64);
+    p.depth = depth;
+    p.k = k;
+    p.vec4 = ld_news % 4 == 0 && (reinterpret_cast<uintptr_t>(news) & 15) == 0;
+    p.lam = lambda;
+    p.one_minus_lam = 1.f - lambda;
+    p.sl_idx = sl_idx;
+    p.sl_score = sl_score;
+    p.idx = idx;
+    p.score = score;
+    p.bad_row_flag = bad_row_flag;
+    ProfScope ps("mmr_rerank", static_cast<int>(n_users), depth, k, stream);
+    mmr_rerank_kernel<<<static_cast<unsigned>(n_users), kMmrThreads, kMmrSmem, stream>>>(p);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 

@@ -596,7 +596,28 @@ def prediction_text(impression_ids, ranks, seg_offsets):
     return text
 
 
-def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categories=None, max_per_category=None):
+MMR_MAX_DEPTH = 128  # shortlist entries per user (nr_mmr_rerank)
+
+
+def mmr_request(k, mmr_lambda, mmr_depth):
+    """The (lambda, depth) top_k_scores re-ranks with, or None without MMR; raises NewsrecError on a bad request: a lambda
+    that is not a real number in [0, 1] (NaN and bools included), a depth that is not an integer in [k, 128], or a depth
+    without a lambda.  The depth defaults to min(128, 4k)."""
+    if mmr_lambda is None:
+        if mmr_depth is not None:
+            raise NewsrecError(f"mmr_depth={mmr_depth!r} needs mmr_lambda")
+        return None
+    if isinstance(mmr_lambda, bool) or not isinstance(mmr_lambda, numbers.Real) or not 0.0 <= float(mmr_lambda) <= 1.0:
+        raise NewsrecError(f"mmr_lambda={mmr_lambda!r} must be a real number in [0, 1]")
+    if mmr_depth is None:
+        mmr_depth = min(MMR_MAX_DEPTH, 4 * k)
+    if isinstance(mmr_depth, bool) or not isinstance(mmr_depth, numbers.Integral) or not k <= mmr_depth <= MMR_MAX_DEPTH:
+        raise NewsrecError(f"mmr_depth={mmr_depth!r} must be an integer in [k, {MMR_MAX_DEPTH}] = [{k}, {MMR_MAX_DEPTH}]")
+    return float(mmr_lambda), int(mmr_depth)
+
+
+def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categories=None, max_per_category=None,
+                 mmr_lambda=None, mmr_depth=None):
     """The k best news of every user over the whole pool, one pass (nr_topk_dot): users (U, D) and news (n, D) fp32, scores
     users[u] . news[r] at fp32 level on the tensor cores (the bound is in include/newsrec_b200.h) without the U x n score
     matrix.  Optional exclusions in CSR form: user u never gets rows excl_rows[excl_offsets[u] .. excl_offsets[u + 1]).
@@ -607,10 +628,22 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     Diversified (nr_topk_dot_capped): with categories ((n,) integer keys, one per news row, any int32 value) and
     max_per_category = m, each list holds at most m news of one category: the pool is walked in the order above and a news is
     taken iff fewer than m taken news share its category and fewer than k are taken.  A user gets fewer than k news when the
-    caps run out; m >= k gives the plain answer bit for bit.  The two arguments go together."""
+    caps run out; m >= k gives the plain answer bit for bit.  The two arguments go together.
+
+    Diversified by content (nr_mmr_rerank): with mmr_lambda = lambda in [0, 1] the list is the maximal-marginal-relevance
+    re-ranking of the plain top mmr_depth (k <= depth <= 128, default min(128, 4k)): k times, the news of the shortlist not
+    yet taken with the largest lambda rel - (1 - lambda) max cosine to the news taken, rel the score scaled to [0, 1] over
+    the shortlist (include/newsrec_b200.h).  Scores are the picked news' own scores, in pick order; lambda = 1 gives the plain
+    answer bit for bit.  lambda is used as fp32.  Not together with a category cap."""
     lib = load_library()
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 128:
         raise NewsrecError(f"top_k_scores: k={k!r} must be an integer in [1, 128]")
+    try:
+        mmr = mmr_request(k, mmr_lambda, mmr_depth)
+    except NewsrecError as e:
+        raise NewsrecError(f"top_k_scores: {e}") from None
+    if mmr is not None and (categories is not None or max_per_category is not None):
+        raise NewsrecError("top_k_scores: mmr_lambda and a category cap do not combine")
     if users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]:
         raise NewsrecError(f"top_k_scores: users {tuple(users.shape)} and news {tuple(news.shape)} must be (U, D) and (n, D)")
     if (excl_rows is None) != (excl_offsets is None):
@@ -642,14 +675,15 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
             raise NewsrecError("top_k_scores: excl_offsets must be (U + 1,) and excl_rows 1-D")
         if excl_rows.numel() == 0:
             excl_rows = excl_rows.new_zeros(1)  # a valid address for an empty set
-    ws_bytes = int(lib.nr_topk_dot_workspace(U, n, D, k))
+    kk = k if mmr is None else mmr[1]  # the shortlist's length
+    ws_bytes = int(lib.nr_topk_dot_workspace(U, n, D, kk))
     if ws_bytes < 0:
         check(-1, "nr_topk_dot_workspace")
     if U == 0 or n == 0:  # no user or nothing eligible: the library launches nothing
         return (torch.full((U, k), -1, dtype=torch.int64, device=dev),
                 torch.full((U, k), float("-inf"), dtype=torch.float32, device=dev))
-    idx = torch.empty((U, k), dtype=torch.int64, device=dev)
-    score = torch.empty((U, k), dtype=torch.float32, device=dev)
+    idx = torch.empty((U, kk), dtype=torch.int64, device=dev)
+    score = torch.empty((U, kk), dtype=torch.float32, device=dev)
     flags = torch.zeros(2, dtype=torch.int32, device=dev)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
     if capped:
@@ -658,8 +692,14 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
                                      max_per_category, _p(idx), _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace),
                                      ws_bytes, _stream()), "nr_topk_dot_capped")
     else:
-        check(lib.nr_topk_dot(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(idx), _p(score),
+        check(lib.nr_topk_dot(_p(users), U, D, _p(news), n, D, D, kk, _p(excl_offsets), _p(excl_rows), _p(idx), _p(score),
                               _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes, _stream()), "nr_topk_dot")
+    if mmr is not None:
+        shortlist_idx, shortlist_score = idx, score
+        idx = torch.empty((U, k), dtype=torch.int64, device=dev)
+        score = torch.empty((U, k), dtype=torch.float32, device=dev)
+        check(lib.nr_mmr_rerank(_p(news), n, D, D, _p(shortlist_idx), _p(shortlist_score), U, kk, k, mmr[0], _p(idx),
+                                _p(score), _p(flags[0:1]), _stream()), "nr_mmr_rerank")
     bad_row, bad_score = (int(x) for x in flags.tolist())
     if bad_row:
         raise IndexError("top_k_scores: an exclusion row is outside the news pool")

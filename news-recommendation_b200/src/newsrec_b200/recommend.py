@@ -20,8 +20,16 @@ device as int32.  The cap is applied inside the kernel (``ops.top_k_scores(..., 
 nr_topk_dot_capped): the pool is walked best first and a news is taken iff fewer than m taken news share its category and
 fewer than k are taken, so a line can be shorter than k when the caps run out.  One field per call.
 
+Diversified by content: with ``mmr_lambda=lambda`` each line is the maximal-marginal-relevance re-ranking of the user's top
+``mmr_depth`` news (default min(128, 4k)): k times, the shortlisted news not yet taken with the largest
+lambda rel - (1 - lambda) max cosine to the news already taken, rel the click score scaled to [0, 1] over the shortlist and the
+cosine that of the model's news vectors (``ops.top_k_scores(..., mmr_lambda=, mmr_depth=)``, nr_mmr_rerank).  lambda = 1 gives
+the plain lines byte for byte; lower lambda trades relevance for lines that do not repeat one story.  Not together with a
+category cap.
+
     python -m newsrec_b200.recommend --directory data/test --out recommendations.tsv [--k 10] [--keep-clicked]
-                                     [--max-per-category M [--diversify-by {category,subcategory}]]
+                                     [--max-per-category M [--diversify-by {category,subcategory}]
+                                      | --mmr-lambda X [--mmr-depth L]]
                                      [--checkpoint PATH | --checkpoint-dir DIR] [--user2int data/train/user2int.tsv]
                                      [--chunk-users N] [--set KNOB=VALUE ...]
 """
@@ -47,10 +55,11 @@ _REFUSED = {
 }
 
 
-def check_request(model, directory, k, max_per_category=None, diversify_by="category"):
+def check_request(model, directory, k, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None):
     """Everything recommend() refuses, checked before any device work: k outside [1, 128], a cap that is not an integer >= 1,
-    a diversify_by other than "category" / "subcategory", a family whose click predictor is not a dot product, a split
-    without behaviors.tsv or news_parsed.tsv, and (with a cap) a news_parsed.tsv without the diversify_by column."""
+    a diversify_by other than "category" / "subcategory", a family whose click predictor is not a dot product, an MMR
+    request ops.mmr_request refuses or one together with a cap, a split without behaviors.tsv or news_parsed.tsv, and (with
+    a cap) a news_parsed.tsv without the diversify_by column."""
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= MAX_K:
         raise NewsrecError(f"recommend: k={k!r} must be an integer in [1, {MAX_K}]")
     if max_per_category is not None and (isinstance(max_per_category, bool) or
@@ -61,6 +70,13 @@ def check_request(model, directory, k, max_per_category=None, diversify_by="cate
     name = type(model).__name__
     if name in _REFUSED:
         raise NewsrecError(f"recommend: {name} is not supported: {_REFUSED[name]}")
+    from .ops import mmr_request
+    try:
+        mmr = mmr_request(int(k), mmr_lambda, mmr_depth)
+    except NewsrecError as e:
+        raise NewsrecError(f"recommend: {e}") from None
+    if mmr is not None and max_per_category is not None:
+        raise NewsrecError("recommend: mmr_lambda and max_per_category do not combine")
     for f in ("behaviors.tsv", "news_parsed.tsv"):
         if not os.path.isfile(os.path.join(directory, f)):
             raise FileNotFoundError(f"recommend: {os.path.join(directory, f)} not found")
@@ -98,14 +114,15 @@ class _Users:
 
 
 def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2int_path="data/train/user2int.tsv",
-              chunk_users=DEFAULT_CHUNK, max_per_category=None, diversify_by="category") -> int:
+              chunk_users=DEFAULT_CHUNK, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None) -> int:
     """Write the k best news of the pool for every distinct history of directory/behaviors.tsv to out_path; returns the
     number of lines.  Runs under torch.no_grad() on the model as given (call .eval() first).  The file appears only when
     every line is written; a non-finite score raises ValueError, a history row outside the news table IndexError.  With
-    max_per_category=m a line holds at most m news of one diversify_by value (module docstring)."""
+    max_per_category=m a line holds at most m news of one diversify_by value; with mmr_lambda the lines are the MMR
+    re-rankings of each user's top mmr_depth (module docstring)."""
     import torch
     from .ops import top_k_scores
-    check_request(model, directory, k, max_per_category, diversify_by)
+    check_request(model, directory, k, max_per_category, diversify_by, mmr_lambda, mmr_depth)
     if chunk_users < 1:
         raise ValueError(f"recommend: chunk_users={chunk_users}")
     with torch.no_grad():
@@ -116,7 +133,7 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
         user_ids = distinct_histories(beh)["user"].tolist()
         user, history, length, _ = user_tables(beh, news_index, model.config.num_clicked_news_a_user, user2int_path)
         pool = matrix[:pad]
-        cap = {}
+        cap = {} if mmr_lambda is None else dict(mmr_lambda=mmr_lambda, mmr_depth=mmr_depth)
         if max_per_category is not None:
             keys = read_news(directory, [diversify_by])[1][diversify_by]
             if len(keys) and (keys.min() < -2 ** 31 or keys.max() >= 2 ** 31):
@@ -156,10 +173,16 @@ def parse_args(argv=None):
     g.add_argument("--checkpoint", help="a checkpoint file (a dict with model_state_dict, as the trainer saves)")
     g.add_argument("--checkpoint-dir", help="load its latest ckpt-<n>.pth (default: ./checkpoint/<MODEL_NAME>)")
     ap.add_argument("--keep-clicked", action="store_true", help="let a user's clicked news be recommended back")
-    ap.add_argument("--max-per-category", type=int, default=None, metavar="M",
-                    help="at most M news of one category (see --diversify-by) per line")
+    d = ap.add_mutually_exclusive_group()
+    d.add_argument("--max-per-category", type=int, default=None, metavar="M",
+                   help="at most M news of one category (see --diversify-by) per line")
+    d.add_argument("--mmr-lambda", type=float, default=None, metavar="X",
+                   help="re-rank each user's shortlist by maximal marginal relevance: X in [0, 1] weighs the click score "
+                        "against similarity to the news already listed (1: the plain lines)")
     ap.add_argument("--diversify-by", choices=DIVERSIFY_FIELDS, default="category",
                     help="the news_parsed.tsv column --max-per-category caps")
+    ap.add_argument("--mmr-depth", type=int, default=None, metavar="L",
+                    help=f"shortlist length --mmr-lambda re-ranks, k .. {MAX_K} (default min({MAX_K}, 4k))")
     ap.add_argument("--user2int", default="./data/train/user2int.tsv")
     ap.add_argument("--chunk-users", type=int, default=DEFAULT_CHUNK, help="users scored per device pass")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
@@ -171,6 +194,13 @@ def parse_args(argv=None):
         ap.error("--chunk-users must be at least 1")
     if args.max_per_category is not None and args.max_per_category < 1:
         ap.error("--max-per-category must be at least 1")
+    if args.mmr_lambda is not None and not 0.0 <= args.mmr_lambda <= 1.0:
+        ap.error("--mmr-lambda must be in [0, 1]")
+    if args.mmr_depth is not None:
+        if args.mmr_lambda is None:
+            ap.error("--mmr-depth needs --mmr-lambda")
+        if not args.k <= args.mmr_depth <= MAX_K:
+            ap.error(f"--mmr-depth must be in [--k, {MAX_K}]")
     return args
 
 
@@ -179,8 +209,11 @@ def main(argv=None):
     args = parse_args(argv)
     name, path, model = load_model(args.checkpoint, args.checkpoint_dir, args.set)
     n = recommend(model, args.directory, args.out, args.k, exclude_clicked=not args.keep_clicked, user2int_path=args.user2int,
-                  chunk_users=args.chunk_users, max_per_category=args.max_per_category, diversify_by=args.diversify_by)
+                  chunk_users=args.chunk_users, max_per_category=args.max_per_category, diversify_by=args.diversify_by,
+                  mmr_lambda=args.mmr_lambda, mmr_depth=args.mmr_depth)
     cap = "" if args.max_per_category is None else f" (at most {args.max_per_category} per {args.diversify_by})"
+    if args.mmr_lambda is not None:
+        cap = f" (MMR re-ranked, lambda {args.mmr_lambda})"
     print(f"{name} from {path}: top {args.k} news{cap} of {n} users written to {args.out}")
     return 0
 

@@ -8,8 +8,17 @@ probability proportional to 1 / rank^s (--zipf s; 0 is uniform), and nr_topk_dot
 nr_topk_dot at the same k, the two alternating in the same run (no matmul baseline).  The sampled users' capped lists are
 checked: no category over M, scores within the bound, and with M >= k the plain lists bit for bit.
 
+Diversified by content (--mmr-lambda X [--mmr-depth L]): the news are clustered (--stories centroids plus noise, as near-copies
+of one story are), and four arms alternate in the same run at every k: nr_topk_dot at k (plain), nr_topk_dot at L (the
+shortlist), nr_mmr_rerank alone on that shortlist, and a batched torch restatement of the re-ranking (gather, bmm Gram in fp32
+with TF32 off, the k-step greedy, in chunks of --baseline-chunk users).  The MMR end to end is ops.top_k_scores(...,
+mmr_lambda=, mmr_depth=): the shortlist plus the rerank.  Quality over a sample of users, plain lists against MMR lists: the
+mean cosine of the pairs within a list, and the mean relevance (the score scaled to [0, 1] over the user's shortlist).  The
+sampled MMR lists go through the fp64 path verifier of tests/mmr_ref.py.
+
     python tools/recommend_bench.py [--users 700000] [--news 120000] [--dim 300] [--k 10 100] [--reps 3] [--seed 0]
                                     [--max-per-category M [--categories 17] [--zipf 0]]
+                                    [--mmr-lambda X [--mmr-depth 40] [--stories 2000]]
 
 Time: CUDA events around the library's launches (operand planes, the top-k kernel, the split merge when there is one), after
 a warm-up, best and median over reps.  Rates: multiply-adds of the three bf16 products per score (3 n_users n_news
@@ -50,7 +59,14 @@ def main(argv=None):
                     help="time nr_topk_dot_capped with this cap against nr_topk_dot")
     ap.add_argument("--categories", type=int, default=17, help="synthetic category keys (with --max-per-category)")
     ap.add_argument("--zipf", type=float, default=0.0, help="Zipf exponent of the category draw, 0: uniform")
+    ap.add_argument("--mmr-lambda", type=float, default=None, metavar="X",
+                    help="time nr_mmr_rerank at this lambda against nr_topk_dot and a torch restatement")
+    ap.add_argument("--mmr-depth", type=int, default=40, metavar="L", help="shortlist length (with --mmr-lambda)")
+    ap.add_argument("--stories", type=int, default=2000, help="story centroids of the clustered pool (with --mmr-lambda)")
     a = ap.parse_args(argv)
+    if a.mmr_lambda is not None and (a.max_per_category is not None or not 0 <= a.mmr_lambda <= 1 or
+                                     not max(a.k) <= a.mmr_depth <= 128):
+        ap.error("--mmr-lambda takes a lambda in [0, 1], a --mmr-depth in [max(--k), 128] and no --max-per-category")
     if a.max_per_category is not None and (a.max_per_category < 1 or a.categories < 1):
         ap.error("--max-per-category and --categories must be at least 1")
     import torch
@@ -62,6 +78,10 @@ def main(argv=None):
     users = torch.randn(a.users, a.dim, device=dev, generator=g)
     news = torch.randn(a.news, a.dim, device=dev, generator=g)
     print(f"card: {card()}", flush=True)
+    if a.mmr_lambda is not None:
+        news = news[torch.randint(0, a.stories, (a.news,), device=dev, generator=g) % a.news]
+        news = news + 0.3 * torch.randn(a.news, a.dim, device=dev, generator=g)  # near-copies of a.stories stories
+        return mmr(a, users, news, dev)
     if a.max_per_category is not None:
         return capped(a, users, news, dev)
 
@@ -172,6 +192,118 @@ def capped(a, users, news, dev):
         results.append(res)
     print(json.dumps(dict(card=card(), users=a.users, news=a.news, dim=a.dim, reps=a.reps, max_per_category=m,
                           categories=a.categories, zipf=a.zipf, results=results)))
+    return 0
+
+
+def torch_mmr(news, sl_idx, sl_score, k, lam, chunk):
+    """The re-ranking restated in torch, chunk users at a time: (idx (U, k), score (U, k))."""
+    import torch
+    U, L = sl_idx.shape
+    nn = torch.nn.functional.normalize(news, dim=1)
+    out_i, out_s = [], []
+    for lo in range(0, U, chunk):
+        si, ss = sl_idx[lo:lo + chunk], sl_score[lo:lo + chunk]
+        live = si >= 0
+        X = nn[si.clamp(min=0)] * live[..., None]
+        Gm = torch.bmm(X, X.transpose(1, 2))
+        smax = torch.where(live, ss, -torch.inf).amax(1, keepdim=True)
+        smin = torch.where(live, ss, torch.inf).amin(1, keepdim=True)
+        rel = torch.where(smax == smin, torch.ones_like(ss), (ss - smin) / (smax - smin))
+        msim = torch.zeros_like(ss)
+        open_ = live.clone()
+        rows = torch.arange(len(si), device=si.device)
+        picks = []
+        for t in range(k):
+            obj = torch.where(open_, lam * rel - (1 - lam) * msim, -torch.inf)
+            p = obj.argmax(1)  # the first maximum: the lower position
+            ok = open_[rows, p]
+            picks.append(torch.where(ok, p, -1))
+            open_[rows, p] = False
+            sim = Gm[rows, p]
+            msim = sim if t == 0 else torch.maximum(msim, sim)
+        P = torch.stack(picks, 1)
+        out_i.append(torch.where(P >= 0, torch.gather(si, 1, P.clamp(min=0)), -1))
+        out_s.append(torch.where(P >= 0, torch.gather(ss, 1, P.clamp(min=0)), -torch.inf))
+    return torch.cat(out_i), torch.cat(out_s)
+
+
+def mmr(a, users, news, dev):
+    """nr_mmr_rerank against nr_topk_dot and the torch restatement, alternating, at every k; one line per k, the JSON line."""
+    import torch
+    from newsrec_b200 import load_library
+    from newsrec_b200.ops import _p, _stream, top_k_scores
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import mmr_ref
+    lib = load_library()
+    L, lam = a.mmr_depth, a.mmr_lambda
+    n, D = news.shape
+    flag = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        out = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1), out
+
+    results = []
+    for k in a.k:
+        sl = top_k_scores(users, news, L)
+        idx = torch.empty((a.users, k), dtype=torch.int64, device=dev)
+        score = torch.empty((a.users, k), dtype=torch.float32, device=dev)
+
+        def rerank():
+            rc = lib.nr_mmr_rerank(_p(news), n, D, D, _p(sl[0]), _p(sl[1]), a.users, L, k, lam, _p(idx), _p(score), _p(flag),
+                                   _stream())
+            assert rc == 0, lib.nr_last_error().decode()
+            return idx, score
+        arms = dict(plain=lambda: top_k_scores(users, news, k), shortlist=lambda: top_k_scores(users, news, L),
+                    rerank=rerank, end_to_end=lambda: top_k_scores(users, news, k, mmr_lambda=lam, mmr_depth=L),
+                    torch=lambda: torch_mmr(news, sl[0], sl[1], k, lam, a.baseline_chunk))
+        times = {name: [] for name in arms}
+        outs = {}
+        for name, fn in arms.items():
+            outs[name] = fn()  # warm-up
+        for _ in range(a.reps):
+            for name, fn in arms.items():
+                t, outs[name] = timed(fn)
+                times[name].append(t)
+        med = {name: sorted(t)[len(t) // 2] for name, t in times.items()}
+        same_e2e = bool(torch.equal(outs["end_to_end"][0], outs["rerank"][0]))
+        agree_torch = float((outs["torch"][0] == outs["rerank"][0]).all(1).float().mean())
+        # quality and the path verifier over a sample of users
+        rows = torch.linspace(0, a.users - 1, 2000, device=dev).long()
+        nn = torch.nn.functional.normalize(news.double(), dim=1)
+        sl_i, sl_s = sl[0][rows], sl[1][rows].double()
+        smax, smin = sl_s[:, :1], sl_s.min(1, keepdim=True).values
+
+        def quality(i):
+            X = nn[i.clamp(min=0)]
+            C = torch.bmm(X, X.transpose(1, 2))
+            off = ~torch.eye(k, dtype=torch.bool, device=dev)
+            pos = (i[:, :, None] == sl_i[:, None, :]).float().argmax(2)
+            rel = ((torch.gather(sl_s, 1, pos) - smin) / (smax - smin).clamp(min=1e-30))
+            return float(C[:, off].mean()), float(rel.mean())
+        cos_p, rel_p = quality(outs["plain"][0][rows])
+        cos_m, rel_m = quality(outs["rerank"][0][rows])
+        mmr_ref.verify_path(news.cpu().numpy(), sl_i.cpu().numpy(), sl[1][rows].cpu().numpy(), idx[rows].cpu().numpy(),
+                            score[rows].cpu().numpy(), k, lam)
+        gathered = a.users * L * D * 4.0
+        res = dict(k=k, depth=L, mmr_lambda=lam, **{f"{name}_ms_median": m for name, m in med.items()},
+                   **{f"{name}_ms_best": min(t) for name, t in times.items()},
+                   rerank_row_gather_gb=gathered / 1e9, rerank_gather_tb_per_s=gathered / (med["rerank"] * 1e-3) / 1e12,
+                   end_to_end_equals_rerank=same_e2e, torch_same_lists_share=agree_torch,
+                   intra_list_cosine_plain=cos_p, intra_list_cosine_mmr=cos_m, relevance_plain=rel_p, relevance_mmr=rel_m,
+                   path_verified=True)
+        print(f"k={k} depth={L} lambda={lam}: nr_topk_dot@k {med['plain']:.1f} ms, nr_topk_dot@depth {med['shortlist']:.1f} "
+              f"ms, nr_mmr_rerank {med['rerank']:.2f} ms, top_k_scores with MMR {med['end_to_end']:.1f} ms, torch "
+              f"restatement {med['torch']:.1f} ms (same lists for {agree_torch:.3f} of users); intra-list cosine "
+              f"{cos_p:.3f} plain / {cos_m:.3f} MMR, relevance {rel_p:.3f} / {rel_m:.3f}", flush=True)
+        results.append(res)
+    print(json.dumps(dict(card=card(), users=a.users, news=a.news, dim=a.dim, reps=a.reps, stories=a.stories,
+                          results=results)))
     return 0
 
 
