@@ -341,6 +341,51 @@ int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const 
                   long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                   long long workspace_bytes, void* stream);
 
+/* Recommendation over a whole news pool under the archive DNN click score of Hi-Fi Ark and DKN (the scorer of
+ * nr_archive_score_fwd).  archive fp32 [n_users][P][F] contiguous (DKN: P = 1, the user vector), news fp32 [n_news][F]
+ * contiguous, W1 fp32 [hidden][2F] over [c; u], b1 [hidden], w2 [hidden], b2 [1], all device.  For user u and news c:
+ *     w = softmax_p(A_u[p] . c)   (P = 1: w = 1 exactly),   score = b2 + sum_j w2_j relu(X_j + sum_p w_p Y_pj)
+ *     X = W1[:, :F] c + b1,   Y_p = W1[:, F:] A_u[p]
+ * Exclusions, categories (nullable) / max_per_category (>= 1 with categories), outputs, padding, ordering, flags and
+ * determinism are nr_topk_dot's (nr_topk_dot_capped's with categories), with these scores in place of the dot products.
+ * One routine computes every pair's score in a fixed operation order, so a pair's score is the same bits in nr_topk_archive
+ * and nr_pool_ranks_archive and does not depend on k, the cap, the split count or where the user sits in the call.
+ * Computation: X and Y in fp32 on the CUDA cores (sequential fma over f, then + b1); the P logits on the tensor cores from
+ * hi/lo bf16 planes, as nr_topk_dot's scores; m = max_p l_p, e_p = __expf(l_p - m), z = sum_p e_p (in p order),
+ * w_p = e_p rcp(z); pre_j = fma over p of w_p Y_pj onto X_j; out = fma over j of w2_j relu(pre_j) onto b2.
+ * Bound.  With L_p, W_p, X_j, Y_pj, pre_j the exact values from the fp32 inputs, u = 2^-24, g(n) = n u / (1 - n u):
+ *   logits   |l_p - L_p| <= d_p = (2^-15 + 3 round_up(F, 64) 2^-23) sum_f |A_pf| |c_f|         (nr_topk_dot, per head)
+ *   softmax  sum_p |w_p - W_p| <= e_w = (1 + 2^-10) (2 max_p d_p + 2 sum_p W_p (2 + 2 |L_p - L_max| + 4 max_p d_p) 2^-23
+ *                                                    + g(P + 2))
+ *            (a logit shift moves the softmax by at most 2 max_p d_p in l1; __expf(x) is within 2 + 1.173 |x| ulp of e^x and
+ *            the subtraction adds |x| u; each relative error enters w_p and z; the sum, the reciprocal and the product add
+ *            g(P + 2); the factor covers the second-order terms)
+ *   X, Y     |dX_j| <= g(F + 1) (sum_f |W1_jf| |c_f| + |b1_j|),   |dY_pj| <= g(F) sum_f |W1_j,F+f| |A_pf|
+ *   mix      |pre_j - PRE_j| <= E_j = |dX_j| + sum_p W_p |dY_pj| + e_w max_p (|Y_pj| + |dY_pj|)
+ *                                   + g(P) (|X_j| + |dX_j| + sum_p (W_p + e_w)(|Y_pj| + |dY_pj|))
+ *   output   e = sum_j |w2_j| E_j + g(hidden) (|b2| + sum_j |w2_j| (|PRE_j| + E_j))      (relu is 1-Lipschitz)
+ * so |score - SCORE| <= e per pair, SCORE the exact score of the fp32 inputs (finite inputs; normal-range exponentials).
+ * The rank band of nr_pool_ranks carries over with this e(n).  Limits: 1 <= k <= 128, 1 <= P <= 32, 1 <= hidden <= 32,
+ * 1 <= F <= 4096, n_users P and n_news below 2^31 - 64.  Every limit is refused (-1) before the first launch; n_users == 0
+ * or n_news == 0 launches nothing.  workspace: nr_topk_archive_workspace(...) bytes (256-byte aligned; -1 outside the
+ * limits), which depends on the device's SM count. */
+long long nr_topk_archive_workspace(long long n_users, int P, long long n_news, int F, int hidden, int k);
+int nr_topk_archive(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
+                    const float* b1, int hidden, const float* w2, const float* b2, int k, const long long* excl_offsets,
+                    const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
+                    int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
+
+/* nr_pool_ranks under nr_topk_archive's scores (the same bits per pair): targets, exclusions, 32-target rows, flags and the
+ * rank definition are nr_pool_ranks'; archive [n_rows][P][F] as nr_topk_archive's, one archive per query row.  The band
+ * holds with nr_topk_archive's e(n).  Limits as nr_topk_archive's without k, with 1 <= n_news.  workspace:
+ * nr_pool_ranks_archive_workspace(...) bytes (256-byte aligned; -1 outside the limits). */
+long long nr_pool_ranks_archive_workspace(long long n_rows, int P, long long n_news, int F, int hidden);
+int nr_pool_ranks_archive(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F, const float* W1,
+                          const float* b1, int hidden, const float* w2, const float* b2, const long long* tgt_offsets,
+                          const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
+                          float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                          long long workspace_bytes, void* stream);
+
 /* Host-side glue of the weight-gradient GEMMs (nr_gemm_tn with the ones column): ext is [rows][ld] fp32 whose columns
  * [0,D) hold dW and column D holds db.  Adds them into the parameters' own gradient storage (dW [rows][D] contiguous,
  * db [rows] or null) and CLEARS ext, so the caller can keep it as a persistent accumulator across steps. */

@@ -249,6 +249,33 @@ int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const 
     return pool_ranks(queries, n_rows, ld_queries, news, n_news, ld_news, D, tgt_offsets, tgt_rows, excl_offsets, excl_rows, rank,
                       score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes, as_stream(stream));
 }
+long long nr_topk_archive_workspace(long long n_users, int P, long long n_news, int F, int hidden, int k) {
+    return topk_archive_workspace(n_users, P, n_news, F, hidden, k);
+}
+int nr_topk_archive(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
+                    const float* b1, int hidden, const float* w2, const float* b2, int k, const long long* excl_offsets,
+                    const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
+                    int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream) {
+    NR_REQUIRE(archive && news && W1 && b1 && w2 && b2 && idx && score && bad_row_flag && bad_score_flag,
+               "nr_topk_archive: null operand");
+    return topk_archive(archive, n_users, P, news, n_news, F, W1, b1, hidden, w2, b2, k, excl_offsets, excl_rows, categories,
+                        max_per_category, idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+}
+long long nr_pool_ranks_archive_workspace(long long n_rows, int P, long long n_news, int F, int hidden) {
+    return pool_ranks_archive_workspace(n_rows, P, n_news, F, hidden);
+}
+int nr_pool_ranks_archive(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F, const float* W1,
+                          const float* b1, int hidden, const float* w2, const float* b2, const long long* tgt_offsets,
+                          const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
+                          float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                          long long workspace_bytes, void* stream) {
+    NR_REQUIRE(archive && news && W1 && b1 && w2 && b2 && tgt_offsets && tgt_rows && rank && score && bad_row_flag &&
+                   bad_score_flag && target_flag,
+               "nr_pool_ranks_archive: null operand");
+    return pool_ranks_archive(archive, n_rows, P, news, n_news, F, W1, b1, hidden, w2, b2, tgt_offsets, tgt_rows, excl_offsets,
+                              excl_rows, rank, score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes,
+                              as_stream(stream));
+}
 long long nr_prediction_line_offsets_workspace(long long n_seg) {
     NR_REQUIRE(n_seg >= 0, "nr_prediction_line_offsets_workspace: n_seg=%lld", n_seg);
     return prediction_scan_bytes(n_seg);

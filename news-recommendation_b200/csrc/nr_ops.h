@@ -286,6 +286,19 @@ int pool_ranks(const float* queries, long long n_rows, int ld_queries, const flo
                const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
                long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                long long workspace_bytes, cudaStream_t stream);
+// top-k and ranks over a whole pool under the archive DNN scorer (topk.cu; include/newsrec_b200.h, nr_topk_archive and
+// nr_pool_ranks_archive)
+long long topk_archive_workspace(long long n_users, int P, long long n_news, int F, int hidden, int k);
+int topk_archive(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
+                 const float* b1, int hidden, const float* w2, const float* b2, int k, const long long* excl_offsets,
+                 const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
+                 int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
+long long pool_ranks_archive_workspace(long long n_rows, int P, long long n_news, int F, int hidden);
+int pool_ranks_archive(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F, const float* W1,
+                       const float* b1, int hidden, const float* w2, const float* b2, const long long* tgt_offsets,
+                       const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
+                       float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                       long long workspace_bytes, cudaStream_t stream);
 // maximal-marginal-relevance re-ranking of nr_topk_dot's shortlists (topk.cu; include/newsrec_b200.h, nr_mmr_rerank)
 int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* sl_idx, const float* sl_score,
                long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag,

@@ -905,6 +905,470 @@ __global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams
     }
 }
 
+// ---- the archive DNN scorer over the pool (nr_topk_archive, nr_pool_ranks_archive) ----
+// score(u, n) = b2 + sum_j w2_j relu(X[n][j] + sum_p w_p Y[u p][j]),  w = softmax_p(A_u[p] . c_n),  X = W1c c + b1, Y = W1u A_u[p].
+// A CTA owns G = 64 / P users, i.e. the G P archive rows [u0 P, u0 P + G P) as the wgmma M side of the tile pipeline above
+// (produce_tile / consume_tile at row offset u0 P); the 64 x 64 logit tile goes to shared memory and the consumer warpgroup
+// scores the tile's G x 64 pairs against the tile's X rows and the CTA's Y rows, both staged in shared memory.  P = 1 (DKN)
+// has w = 1 and runs no TMA ring and no wgmma.
+constexpr int kArchMaxP = 32;            // archive rows per user
+constexpr int kArchMaxHid = 32;          // DNN hidden width
+constexpr int kArchTileLd = kNews + 8;   // fp32 pitch of the logit / score tile
+
+struct ArchOperands {
+    int P, G, hid, hp;                   // archive rows per user, users per CTA, hidden width, hidden rounded up to 8
+    const float* X;                      // [n_news][hp]          W1[:, :F] c + b1, zeros past hid
+    const float* Y;                      // [n_users * P][hp]     W1[:, F:] a, zeros past hid
+    const float* w2;                     // [hid]
+    const float* b2;                     // [1]
+};
+
+// Shared memory of the archive kernels, byte offsets from the 1024-aligned base: the TMA ring (P > 1), the logit / score
+// tile, the per-thread softmax weights (P > 1), the tile's X rows (pitch hp + 4: conflict-free 16-byte reads), the CTA's
+// Y rows, w2 | b2, then the kernel's own region of `rest` bytes.
+struct ArchSmem {
+    int tile, w, x, y, w2, rest, bytes;
+    __host__ __device__ constexpr ArchSmem(int P, int G, int hp, int rest_bytes) {
+        tile = P > 1 ? kStages * kStage : 0;
+        w = tile + kUsers * kArchTileLd * 4;
+        x = w + (P > 1 ? kArchMaxP * 128 * 4 : 0);
+        y = x + kNews * (hp + 4) * 4;
+        w2 = y + G * P * hp * 4;
+        rest = w2 + (kArchMaxHid + 4) * 4;
+        bytes = rest + rest_bytes;
+    }
+};
+__host__ __device__ constexpr int topk_archive_rest(int G) { return G * kCap * 8 + 2 * kStages * 8 + 2 * kUsers * 4; }
+__host__ __device__ constexpr int ranks_archive_rest(int G) {
+    // hist and tiles hold kUsers * kMaxTargets entries: the tile sort needs a power of two
+    return G * kFiltWords * 8 + 3 * G * kMaxTargets * 4 + 2 * kUsers * kMaxTargets * 4 + 3 * G * kNews * 4 + 2 * kStages * 8 +
+           3 * G * 4 + 16;
+}
+
+// X or Y: out[r][j] = (sum_f W[j][f] src[r][f]) (+ b[j]) for j < hid, in f order, 0 for hid <= j < hp; one warp per row
+__global__ void __launch_bounds__(256) arch_project_kernel(const float* __restrict__ src, long long rows, int F,
+                                                           const float* __restrict__ W, int ldw, const float* __restrict__ b,
+                                                           int hid, int hp, float* __restrict__ out) {
+    const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+    const int j = threadIdx.x & 31;
+    if (r >= rows || j >= hp) return;
+    float acc = 0.f;
+    if (j < hid) {
+        const float* w = W + static_cast<long long>(j) * ldw;
+        const float* x = src + r * F;
+        for (int f = 0; f < F; ++f) acc = __fmaf_rn(__ldg(w + f), __ldg(x + f), acc);
+        if (b != nullptr) acc = __fadd_rn(acc, __ldg(b + j));
+    }
+    out[r * hp + j] = acc;
+}
+
+// THE score of one pair, in one fixed operation order (both kernels call it, so a pair has the same bits in both):
+//   m = max_p l_p;  e_p = __expf(l_p - m);  z = ((e_0 + e_1) + ...) + e_{P-1};  w_p = e_p rcp_rn(z)        (P = 1: w_0 = 1)
+//   pre_j = fma(w_{P-1}, Y_{P-1,j}, ... fma(w_0, Y_0j, X_j));  out = fma(w2_{hp-1}, relu(pre_{hp-1}), ... fma(w2_0, relu(pre_0), b2))
+// lg: the pair's logit column (rows p of pitch kArchTileLd); xr: the news' X row; yr: the user's P Y rows (pitch hp); ws: the
+// thread's weight slots (stride 128).  relu keeps a NaN, so a non-finite operand gives a non-finite score.
+__device__ __forceinline__ float arch_pair_score(const float* lg, const float* xr, const float* yr, const float* w2, float b2,
+                                                 float* ws, int P, int hp) {
+    if (P > 1) {
+        float m = lg[0];
+        for (int p = 1; p < P; ++p) m = fmaxf(m, lg[p * kArchTileLd]);
+        float z = 0.f;
+        for (int p = 0; p < P; ++p) {
+            const float e = __expf(__fsub_rn(lg[p * kArchTileLd], m));
+            ws[p * 128] = e;
+            z = __fadd_rn(z, e);
+        }
+        const float rz = __frcp_rn(z);
+        for (int p = 0; p < P; ++p) ws[p * 128] = __fmul_rn(ws[p * 128], rz);
+    }
+    float out = b2;
+    for (int jb = 0; jb < hp; jb += 8) {
+        const float4 xa = *reinterpret_cast<const float4*>(xr + jb), xb = *reinterpret_cast<const float4*>(xr + jb + 4);
+        float a[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
+        for (int p = 0; p < P; ++p) {
+            const float w = P > 1 ? ws[p * 128] : 1.f;
+            const float4 ya = *reinterpret_cast<const float4*>(yr + p * hp + jb);
+            const float4 yb = *reinterpret_cast<const float4*>(yr + p * hp + jb + 4);
+            a[0] = __fmaf_rn(w, ya.x, a[0]);
+            a[1] = __fmaf_rn(w, ya.y, a[1]);
+            a[2] = __fmaf_rn(w, ya.z, a[2]);
+            a[3] = __fmaf_rn(w, ya.w, a[3]);
+            a[4] = __fmaf_rn(w, yb.x, a[4]);
+            a[5] = __fmaf_rn(w, yb.y, a[5]);
+            a[6] = __fmaf_rn(w, yb.z, a[6]);
+            a[7] = __fmaf_rn(w, yb.w, a[7]);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) out = __fmaf_rn(w2[jb + i], a[i] < 0.f ? 0.f : a[i], out);
+    }
+    return out;
+}
+
+// Per tile, consumer warpgroup: (P > 1) the logits of news tile t into T; the tile's X rows into Xs.  The caller syncs.
+__device__ __forceinline__ void arch_stage_tile(Ring& r, const ArchOperands& o, int t, int n_news, int k_chunks, float* T, float* Xs) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (o.P > 1) {
+        float acc[kNews / 2];
+        consume_tile(r, acc, k_chunks);
+#pragma unroll
+        for (int j = 0; j < kNews / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int row = 16 * warp + (lane >> 2) + 8 * e, col = 8 * j + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(T + row * kArchTileLd + col) = make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]);
+            }
+    }
+    const int q4 = o.hp / 4;
+    for (int i = threadIdx.x; i < kNews * q4; i += 128) {
+        const int row = i / q4, q = i - row * q4;
+        const long long n = static_cast<long long>(t) * kNews + row;
+        const float4 v = n < n_news ? __ldg(reinterpret_cast<const float4*>(o.X + n * o.hp) + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(Xs + row * (o.hp + 4) + 4 * q) = v;
+    }
+}
+
+// Every (user g < here, column c) pair of the staged tile, scored and handed to visit(g, c, s): thread i takes column i % 64
+// and users i / 64, i / 64 + 2, ... (a warp shares its user: the Y reads are broadcasts)
+template <class Visit>
+__device__ __forceinline__ void arch_tile_pairs(const ArchOperands& o, const float* T, const float* Xs, const float* Ys,
+                                                const float* w2s, float* Ws, int here, Visit&& visit) {
+    const int c = threadIdx.x & (kNews - 1);
+    const float b2 = w2s[kArchMaxHid];
+    for (int g = threadIdx.x >> 6; g < here; g += 2)
+        visit(g, c, arch_pair_score(T + g * o.P * kArchTileLd + c, Xs + c * (o.hp + 4), Ys + g * o.P * o.hp, w2s, b2,
+                                    Ws + threadIdx.x, o.P, o.hp));
+}
+
+// Y rows of users [u0, u0 + here) and w2 | b2 into shared memory (all threads; the caller syncs)
+__device__ __forceinline__ void arch_stage_users(const ArchOperands& o, long long u0, int here, float* Ys, float* w2s) {
+    const long long y0 = u0 * o.P * o.hp;
+    for (int i = threadIdx.x; i < o.G * o.P * o.hp; i += kThreads) Ys[i] = i < here * o.P * o.hp ? __ldg(o.Y + y0 + i) : 0.f;
+    for (int i = threadIdx.x; i < kArchMaxHid; i += kThreads) w2s[i] = i < o.hid ? __ldg(o.w2 + i) : 0.f;
+    if (threadIdx.x == 0) w2s[kArchMaxHid] = __ldg(o.b2);
+}
+
+template <bool kCapped>
+__global__ void __launch_bounds__(kThreads, 1) topk_archive_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+                                                                   const __grid_constant__ CUtensorMap tmNh, const __grid_constant__ CUtensorMap tmNl,
+                                                                   const Params p, const ArchOperands o) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const int G = o.G;
+    const ArchSmem L(o.P, G, o.hp, topk_archive_rest(G));
+    float* T = reinterpret_cast<float*>(base + L.tile);
+    float* Ws = reinterpret_cast<float*>(base + L.w);
+    float* Xs = reinterpret_cast<float*>(base + L.x);
+    float* Ys = reinterpret_cast<float*>(base + L.y);
+    float* w2s = reinterpret_cast<float*>(base + L.w2);
+    float* bs = reinterpret_cast<float*>(base + L.rest);            // [G][kCap] candidate scores
+    int* br = reinterpret_cast<int*>(bs + G * kCap);                // [G][kCap] candidate rows
+    uint64_t* full = reinterpret_cast<uint64_t*>(br + G * kCap);    // [kStages]
+    uint64_t* empty = full + kStages;                               // [kStages]
+    int* cnt = reinterpret_cast<int*>(empty + kStages);             // [G]
+    float* thr = reinterpret_cast<float*>(cnt + kUsers);            // [G]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long u0 = static_cast<long long>(blockIdx.x) * G;
+    const int here = static_cast<int>(min(static_cast<long long>(G), p.n_users - u0));
+    const int split = blockIdx.y;
+    const int t0 = static_cast<int>(static_cast<long long>(p.tiles) * split / p.splits);
+    const int t1 = static_cast<int>(static_cast<long long>(p.tiles) * (split + 1) / p.splits);
+
+    Ring ring{base, full, empty};
+    if (o.P > 1 && warp == 4 && lane == 0) ring_init(ring, &tmAh, &tmAl, &tmNh, &tmNl);
+    if (threadIdx.x < G) {
+        cnt[threadIdx.x] = 0;
+        thr[threadIdx.x] = -INFINITY;
+    }
+    arch_stage_users(o, u0, here, Ys, w2s);
+    __syncthreads();
+
+    if (warp == 4) {
+        // ===================== TMA producer (P > 1): archive rows [u0 P, u0 P + 64) and the news of every tile =====================
+        if (o.P > 1 && elect_one())
+            for (int t = t0; t < t1; ++t) produce_tile(ring, &tmAh, &tmAl, &tmNh, &tmNl, static_cast<int>(u0 * o.P), t, p.k_chunks);
+        return;
+    }
+
+    // ===================== consumer warpgroup =====================
+    if (p.excl_offsets != nullptr && split == 0) {
+        bool bad = false;
+        for (long long i = p.excl_offsets[u0] + threadIdx.x; i < p.excl_offsets[u0 + here]; i += 128) {
+            const long long r = p.excl_rows[i];
+            bad |= r < 0 || r >= p.n_news;
+        }
+        if (bad) atomicOr(p.bad_row_flag, 1);
+    }
+    bool bad_score = false;
+    for (int t = t0; t < t1; ++t) {
+        arch_stage_tile(ring, o, t, p.n_news, p.k_chunks, T, Xs);
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        // ---- survivors of the tile into the candidate buffers ----
+        arch_tile_pairs(o, T, Xs, Ys, w2s, Ws, here, [&](int g, int c, float s) {
+            const int n = t * kNews + c;
+            if (n >= p.n_news) return;
+            bad_score |= !(fabsf(s) <= 3.402823466e38f);
+            if (!(s > thr[g])) return;
+            if (p.excl_offsets != nullptr) {
+                const long long x1 = p.excl_offsets[u0 + g + 1];
+                for (long long x = p.excl_offsets[u0 + g]; x < x1; ++x)
+                    if (__ldg(p.excl_rows + x) == n) return;
+            }
+            const int pos = atomicAdd(&cnt[g], 1);
+            bs[g * kCap + pos] = s;
+            br[g * kCap + pos] = n;
+        });
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        for (int u = warp; u < here; u += 4)
+            if (cnt[u] > kCap - kNews) merge_user<kCapped>(bs, br, cnt, thr, u, p.k, p.cat, p.cap);
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+    }
+    if (bad_score) atomicOr(p.bad_score_flag, 1);
+    // ---- the k best of every user of the CTA: sorted, padded with (-inf, -1) ----
+    for (int u = warp; u < here; u += 4) {
+        const long long ug = u0 + u;
+        merge_user<kCapped>(bs, br, cnt, thr, u, p.k, p.cat, p.cap);
+        const float* s = bs + u * kCap;
+        const int* r = br + u * kCap;
+        const int c = cnt[u];
+        for (int j = lane; j < p.k; j += 32) {
+            const float sv = j < c ? s[j] : -INFINITY;
+            const int rv = j < c ? r[j] : -1;
+            if (p.splits == 1) {
+                p.idx[ug * p.k + j] = rv;
+                p.score[ug * p.k + j] = sv;
+            } else {
+                const long long off = (ug * p.splits + split) * p.k + j;
+                p.part_score[off] = sv;
+                p.part_row[off] = rv;
+            }
+        }
+    }
+}
+
+// nr_pool_ranks_kernel's algorithm over the CTA's G users, on the archive scores: the target tiles first (their scores read
+// out of the score tile), then the split's tiles, each pair counted against the first target it comes before
+__global__ void __launch_bounds__(kThreads, 1) pool_ranks_archive_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+                                                                         const __grid_constant__ CUtensorMap tmNh, const __grid_constant__ CUtensorMap tmNl,
+                                                                         const RankParams p, const ArchOperands o) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const int G = o.G;
+    const ArchSmem L(o.P, G, o.hp, ranks_archive_rest(G));
+    float* T = reinterpret_cast<float*>(base + L.tile);
+    float* Ws = reinterpret_cast<float*>(base + L.w);
+    float* Xs = reinterpret_cast<float*>(base + L.x);
+    float* Ys = reinterpret_cast<float*>(base + L.y);
+    float* w2s = reinterpret_cast<float*>(base + L.w2);
+    unsigned long long* filt = reinterpret_cast<unsigned long long*>(base + L.rest);  // [G][kFiltWords]
+    float* ts = reinterpret_cast<float*>(filt + G * kFiltWords);    // [G][kMaxTargets] target scores, then sorted
+    int* tr = reinterpret_cast<int*>(ts + G * kMaxTargets);         // target rows
+    int* tp = tr + G * kMaxTargets;                                 // target slot in the row's CSR range
+    int* hist = tp + G * kMaxTargets;                               // counts by first target beaten (the sort's keys first)
+    int* tiles = hist + kUsers * kMaxTargets;                       // [kUsers * kMaxTargets] pool tiles holding targets
+    float* qs = reinterpret_cast<float*>(tiles + kUsers * kMaxTargets);  // [G * kNews] filter hits: score, news row, query row
+    int* qn = reinterpret_cast<int*>(qs + G * kNews);
+    int* qr = qn + G * kNews;
+    uint64_t* full = reinterpret_cast<uint64_t*>(qr + G * kNews);
+    uint64_t* empty = full + kStages;
+    float* lo_s = reinterpret_cast<float*>(empty + kStages);        // [G] per row: its last target in output order
+    int* lo_r = reinterpret_cast<int*>(lo_s + G);
+    int* tm = lo_r + G;                                             // [G] targets of the row, -1: bad row
+    int* n_pro = tm + G;
+    int* qc = n_pro + 1;                                            // [2] queue length, by tile parity
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long q0 = static_cast<long long>(blockIdx.x) * G;
+    const int here = static_cast<int>(min(static_cast<long long>(G), p.n_rows - q0));
+    const int split = blockIdx.y;
+    const int t0 = static_cast<int>(static_cast<long long>(p.tiles) * split / p.splits);
+    const int t1 = static_cast<int>(static_cast<long long>(p.tiles) * (split + 1) / p.splits);
+
+    Ring ring{base, full, empty};
+    if (o.P > 1 && warp == 4 && lane == 0) ring_init(ring, &tmAh, &tmAl, &tmNh, &tmNl);
+    for (int i = threadIdx.x; i < G * kFiltWords; i += kThreads) filt[i] = 0;
+    if (threadIdx.x < 2) qc[threadIdx.x] = 0;
+    arch_stage_users(o, q0, here, Ys, w2s);
+    __syncthreads();
+    // ---- the rows' targets and the membership filter of targets and exclusions ----
+    if (threadIdx.x < G) {
+        const int r = threadIdx.x;
+        int m = 0;
+        if (r < here) {
+            const long long q = q0 + r, a = p.tgt_offsets[q], cnt = p.tgt_offsets[q + 1] - a;
+            if (cnt > kMaxTargets) {
+                m = -1;
+                atomicOr(p.target_flag, 1);
+            } else {
+                m = static_cast<int>(cnt);
+                for (int j = 0; j < m; ++j) {
+                    const long long n = p.tgt_rows[a + j];
+                    if (n < 0 || n >= p.n_news) {
+                        m = -1;
+                        break;
+                    }
+                    tr[r * kMaxTargets + j] = static_cast<int>(n);
+                    tp[r * kMaxTargets + j] = j;
+                    atomicOr(&filt[r * kFiltWords + ((n >> 6) & (kFiltWords - 1))], 1ull << (n & 63));
+                }
+                if (m < 0) atomicOr(p.bad_row_flag, 1);
+            }
+        }
+        tm[r] = m;
+    }
+    if (p.excl_offsets != nullptr) {
+        bool bad = false;
+        for (int r = 0; r < here; ++r)
+            for (long long i = p.excl_offsets[q0 + r] + threadIdx.x; i < p.excl_offsets[q0 + r + 1]; i += kThreads) {
+                const long long n = p.excl_rows[i];
+                if (n < 0 || n >= p.n_news) bad = true;
+                else atomicOr(&filt[r * kFiltWords + ((n >> 6) & (kFiltWords - 1))], 1ull << (n & 63));
+            }
+        if (bad) atomicOr(p.bad_row_flag, 1);
+    }
+    __syncthreads();
+    // ---- the distinct tiles holding the CTA's targets, ascending (one warp) ----
+    if (warp == 0) {
+        int c = 0;
+        if (lane == 0)
+            for (int r = 0; r < G; ++r)
+                for (int j = 0; j < tm[r]; ++j) tiles[c++] = tr[r * kMaxTargets + j] / kNews;
+        c = __shfl_sync(0xffffffffu, c, 0);
+        int n = 1;
+        while (n < c) n <<= 1;
+        float* keys = reinterpret_cast<float*>(hist);  // equal keys: warp_sort orders by the int
+        for (int i = lane; i < n; i += 32) {
+            keys[i] = 0.f;
+            if (i >= c) tiles[i] = 0x7fffffff;
+        }
+        __syncwarp();
+        warp_sort(keys, tiles, n);
+        if (lane == 0) {
+            int d = 0;
+            for (int i = 0; i < c; ++i)
+                if (d == 0 || tiles[i] != tiles[d - 1]) tiles[d++] = tiles[i];
+            *n_pro = d;
+        }
+    }
+    __syncthreads();
+    const int npro = *n_pro;
+
+    if (warp == 4) {
+        // ===================== TMA producer (P > 1): the target tiles, then the split's tiles =====================
+        if (o.P > 1 && elect_one()) {
+            const int a0 = static_cast<int>(q0 * o.P);
+            for (int i = 0; i < npro; ++i) produce_tile(ring, &tmAh, &tmAl, &tmNh, &tmNl, a0, tiles[i], p.k_chunks);
+            for (int t = t0; t < t1; ++t) produce_tile(ring, &tmAh, &tmAl, &tmNh, &tmNl, a0, t, p.k_chunks);
+        }
+        return;
+    }
+
+    // ===================== consumer warpgroup =====================
+    // prologue: the target scores, from the score tiles of the tiles that hold them (user g's scores in T's row g P)
+    for (int i = 0; i < npro; ++i) {
+        const int t = tiles[i];
+        arch_stage_tile(ring, o, t, p.n_news, p.k_chunks, T, Xs);
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        arch_tile_pairs(o, T, Xs, Ys, w2s, Ws, here, [&](int g, int c, float s) { T[g * o.P * kArchTileLd + c] = s; });
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        if (threadIdx.x < here) {
+            const int r = threadIdx.x;
+            for (int j = 0; j < tm[r]; ++j) {
+                const int col = tr[r * kMaxTargets + j] - t * kNews;
+                if (col >= 0 && col < kNews) ts[r * kMaxTargets + j] = T[r * o.P * kArchTileLd + col];
+            }
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+    }
+    // each row's targets into output order (score descending, row ascending); counts start at zero
+    bool bad_score = false;
+    if (threadIdx.x < G) {
+        const int r = threadIdx.x, m = tm[r];
+        float* s = ts + r * kMaxTargets;
+        int* n = tr + r * kMaxTargets;
+        int* ord = tp + r * kMaxTargets;
+        for (int j = 0; j < m; ++j) bad_score |= !(fabsf(s[j]) <= 3.402823466e38f);
+        for (int j = 1; j < m; ++j) {
+            const float sj = s[j];
+            const int nj = n[j], oj = ord[j];
+            int i = j;
+            for (; i > 0 && before(sj, nj, s[i - 1], n[i - 1]); --i) {
+                s[i] = s[i - 1];
+                n[i] = n[i - 1];
+                ord[i] = ord[i - 1];
+            }
+            s[i] = sj;
+            n[i] = nj;
+            ord[i] = oj;
+        }
+        for (int j = 0; j < kMaxTargets; ++j) hist[r * kMaxTargets + j] = 0;
+        // threshold: a score counts when it comes before the row's last target
+        lo_s[r] = m > 0 ? s[m - 1] : INFINITY;  // nothing comes before (+inf, -1)
+        lo_r[r] = m > 0 ? n[m - 1] : -1;
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    for (int t = t0; t < t1; ++t) {
+        arch_stage_tile(ring, o, t, p.n_news, p.k_chunks, T, Xs);
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        arch_tile_pairs(o, T, Xs, Ys, w2s, Ws, here, [&](int g, int c, float s) {
+            const int n = t * kNews + c;
+            if (lo_r[g] < 0 || n >= p.n_news) return;  // no target, or a bad row
+            bad_score |= !(fabsf(s) <= 3.402823466e38f);
+            if (!before(s, n, lo_s[g], lo_r[g])) return;
+            if ((filt[g * kFiltWords + (t & (kFiltWords - 1))] >> c) & 1ull) {  // maybe a target or an exclusion of the row: queued
+                const int k = atomicAdd(&qc[t & 1], 1);
+                qs[k] = s;
+                qn[k] = n;
+                qr[k] = g;
+                return;
+            }
+            int b = 0;  // the first target it comes before: exists, the last one
+            while (!before(s, n, ts[g * kMaxTargets + b], tr[g * kMaxTargets + b])) ++b;
+            atomicAdd(&hist[g * kMaxTargets + b], 1);
+        });
+        // the queued scores, one per thread: counted unless a target or an exclusion of their row
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        const int nq = qc[t & 1];
+        if (threadIdx.x == 0) qc[(t + 1) & 1] = 0;  // every thread read it before the previous tile's second barrier
+        for (int k = threadIdx.x; k < nq; k += 128) {
+            const float s = qs[k];
+            const int n = qn[k], r = qr[k];
+            bool member = false;
+            for (int x = 0; x < tm[r] && !member; ++x) member = tr[r * kMaxTargets + x] == n;
+            if (p.excl_offsets != nullptr)
+                for (long long x = p.excl_offsets[q0 + r]; x < p.excl_offsets[q0 + r + 1] && !member; ++x)
+                    member = __ldg(p.excl_rows + x) == n;
+            if (member) continue;
+            int b = 0;
+            while (!before(s, n, ts[r * kMaxTargets + b], tr[r * kMaxTargets + b])) ++b;
+            atomicAdd(&hist[r * kMaxTargets + b], 1);
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+    }
+    if (bad_score) atomicOr(p.bad_score_flag, 1);
+    // ---- rank of the b-th target in output order: the counts of bins 0 .. b ----
+    if (threadIdx.x < here) {
+        const int r = threadIdx.x, m = tm[r];
+        const long long q = q0 + r;
+        const long long a = p.tgt_offsets[q];
+        if (m < 0) {
+            if (split == 0)
+                for (long long j = a; j < p.tgt_offsets[q + 1]; ++j) {
+                    if (p.splits == 1) p.rank[j] = -1;
+                    p.score[j] = NAN;
+                }
+            if (p.splits > 1) p.part[(q * p.splits + split) * kMaxTargets] = -1;
+            return;
+        }
+        int c = 0;
+        for (int b = 0; b < m; ++b) {
+            c += hist[r * kMaxTargets + b];
+            const int j = tp[r * kMaxTargets + b];
+            if (split == 0) p.score[a + j] = ts[r * kMaxTargets + b];
+            if (p.splits == 1) p.rank[a + j] = c;
+            else p.part[(q * p.splits + split) * kMaxTargets + j] = c;
+        }
+    }
+}
+
 }  // namespace topk
 
 static int topk_splits(long long n_users, long long n_news) {
@@ -1138,5 +1602,223 @@ int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const lo
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
+
+// ---- the archive DNN scorer over the pool ----
+static int archive_check(const char* who, long long n_users, int P, long long n_news, long long min_news, int F, int hidden) {
+    NR_REQUIRE(P >= 1 && P <= topk::kArchMaxP, "%s: P=%d outside [1, 32]", who, P);
+    NR_REQUIRE(hidden >= 1 && hidden <= topk::kArchMaxHid, "%s: hidden=%d outside [1, 32]", who, hidden);
+    NR_REQUIRE(F >= 1 && F <= 4096, "%s: F=%d outside [1, 4096]", who, F);
+    NR_REQUIRE(n_users >= 0 && n_users < ((1ll << 31) - topk::kUsers) / P, "%s: n_users=%lld x P=%d outside [0, 2^31 - 64)", who,
+               n_users, P);
+    NR_REQUIRE(n_news >= min_news && n_news < (1ll << 31) - topk::kNews, "%s: n_news=%lld outside [%lld, 2^31 - 64)", who, n_news,
+               min_news);
+    return 0;
+}
+
+// the planes of the archive rows and the news (P > 1 only: P = 1 needs no logits), X and Y
+struct ArchPlanes {
+    DotPlanes planes;
+    float *X, *Y;
+    ArchPlanes(WorkspaceLayout& ws, long long n_users, int P, long long n_news, int F, int hidden)
+        : planes(ws, P > 1 ? n_users * P : 0, P > 1 ? n_news : 0, F) {
+        const int hp = round_up(hidden, 8);
+        X = ws.take<float>(n_news * hp);
+        Y = ws.take<float>(n_users * P * hp);
+    }
+    // the TMA maps and planes (P > 1), then X and Y; fills o
+    int prepare(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
+                const float* b1, int hidden, const float* w2, const float* b2, CUtensorMap (&tm)[4], topk::ArchOperands& o,
+                cudaStream_t stream) const {
+        o.P = P;
+        o.G = topk::kUsers / P;
+        o.hid = hidden;
+        o.hp = round_up(hidden, 8);
+        o.X = X;
+        o.Y = Y;
+        o.w2 = w2;
+        o.b2 = b2;
+        if (P > 1) NR_PROPAGATE(planes.prepare(archive, n_users * P, F, news, n_news, F, F, tm, stream));
+        const struct { const float* src; long long rows; int col0; const float* b; float* out; } jobs[2] = {
+            {news, n_news, 0, b1, X}, {archive, n_users * P, F, nullptr, Y}};
+        for (const auto& j : jobs) {
+            if (j.rows == 0) continue;
+            ProfScope ps("archive_project", static_cast<int>(j.rows), F, hidden, stream);
+            topk::arch_project_kernel<<<static_cast<unsigned>((j.rows + 7) / 8), 256, 0, stream>>>(j.src, j.rows, F, W1 + j.col0, 2 * F,
+                                                                                                     j.b, hidden, o.hp, j.out);
+            ++g_launches;
+            NR_CHECK_CUDA(cudaGetLastError());
+        }
+        return 0;
+    }
+};
+
+static int archive_ctas(long long n_users, int P) { return static_cast<int>((n_users + topk::kUsers / P - 1) / (topk::kUsers / P)); }
+
+struct TopkArchiveWorkspace : WorkspaceLayout {
+    ArchPlanes ops;
+    float* part_score;
+    int* part_row;
+    TopkArchiveWorkspace(void* base, long long n_users, int P, long long n_news, int F, int hidden, int k, int splits)
+        : WorkspaceLayout{static_cast<char*>(base)}, ops(*this, n_users, P, n_news, F, hidden) {
+        part_score = take<float>(splits > 1 ? n_users * splits * k : 0);
+        part_row = take<int>(splits > 1 ? n_users * splits * k : 0);
+    }
+};
+
+static int topk_archive_check(long long n_users, int P, long long n_news, int F, int hidden, int k) {
+    NR_REQUIRE(k >= 1 && k <= 128, "nr_topk_archive: k=%d outside [1, 128]", k);
+    return archive_check("nr_topk_archive", n_users, P, n_news, 0, F, hidden);
+}
+
+static int archive_splits(long long n_users, int P, long long n_news) {
+    return topk_splits(static_cast<long long>(archive_ctas(n_users, P)) * topk::kUsers, n_news);
+}
+
+long long topk_archive_workspace(long long n_users, int P, long long n_news, int F, int hidden, int k) {
+    if (topk_archive_check(n_users, P, n_news, F, hidden, k) != 0) return -1;
+    return TopkArchiveWorkspace(nullptr, n_users, P, n_news, F, hidden, k, archive_splits(n_users, P, n_news)).bytes();
+}
+
+template <bool kCapped>
+static int topk_archive_launch(const CUtensorMap (&tm)[4], const topk::Params& p, const topk::ArchOperands& o, cudaStream_t stream) {
+    using namespace topk;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NR_CHECK_CUDA(cudaFuncSetAttribute(topk_archive_kernel<kCapped>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+        attr_set = true;
+    }
+    const size_t smem = 1024 + ArchSmem(o.P, o.G, o.hp, topk_archive_rest(o.G)).bytes;
+    {
+        ProfScope ps(kCapped ? "topk_archive_capped" : "topk_archive", static_cast<int>(p.n_users), p.n_news, p.k, stream);
+        topk_archive_kernel<kCapped><<<dim3(static_cast<unsigned>(archive_ctas(p.n_users, o.P)), p.splits), kThreads, smem, stream>>>(
+            tm[0], tm[1], tm[2], tm[3], p, o);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    if (p.splits > 1) {
+        ProfScope ps(kCapped ? "topk_merge_capped" : "topk_merge", static_cast<int>(p.n_users), p.splits, p.k, stream);
+        topk_merge_kernel<kCapped><<<static_cast<unsigned>((p.n_users + kMergeWarps - 1) / kMergeWarps), kMergeWarps * 32, 0, stream>>>(p);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    return 0;
+}
+
+int topk_archive(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
+                 const float* b1, int hidden, const float* w2, const float* b2, int k, const long long* excl_offsets,
+                 const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
+                 int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+    using namespace topk;
+    NR_PROPAGATE(topk_archive_check(n_users, P, n_news, F, hidden, k));
+    NR_REQUIRE((excl_offsets == nullptr) == (excl_rows == nullptr), "nr_topk_archive: excl_offsets and excl_rows go together");
+    NR_REQUIRE(categories == nullptr || max_per_category >= 1, "nr_topk_archive: max_per_category=%d below 1", max_per_category);
+    const int splits = archive_splits(n_users, P, n_news);
+    TopkArchiveWorkspace ws(workspace, n_users, P, n_news, F, hidden, k, splits);
+    NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
+               "nr_topk_archive: workspace of %lld bytes (256-byte aligned) needs %lld", workspace_bytes, ws.bytes());
+    if (n_users == 0 || n_news == 0) return 0;
+    CUtensorMap tm[4] = {};
+    ArchOperands o;
+    NR_PROPAGATE(ws.ops.prepare(archive, n_users, P, news, n_news, F, W1, b1, hidden, w2, b2, tm, o, stream));
+    Params p;
+    p.n_users = n_users;
+    p.n_news = static_cast<int>(n_news);
+    p.k = k;
+    p.k_chunks = ceil_div(F, 64);
+    p.tiles = static_cast<int>((n_news + kNews - 1) / kNews);
+    p.splits = splits;
+    p.excl_offsets = excl_offsets;
+    p.excl_rows = excl_rows;
+    p.idx = idx;
+    p.score = score;
+    p.part_score = ws.part_score;
+    p.part_row = ws.part_row;
+    p.bad_row_flag = bad_row_flag;
+    p.bad_score_flag = bad_score_flag;
+    p.cat = categories;
+    p.cap = max_per_category;
+    return categories != nullptr ? topk_archive_launch<true>(tm, p, o, stream) : topk_archive_launch<false>(tm, p, o, stream);
+}
+
+struct RankArchiveWorkspace : WorkspaceLayout {
+    ArchPlanes ops;
+    int* part;
+    RankArchiveWorkspace(void* base, long long n_rows, int P, long long n_news, int F, int hidden, int splits)
+        : WorkspaceLayout{static_cast<char*>(base)}, ops(*this, n_rows, P, n_news, F, hidden) {
+        part = take<int>(splits > 1 ? n_rows * splits * topk::kMaxTargets : 0);
+    }
+};
+
+long long pool_ranks_archive_workspace(long long n_rows, int P, long long n_news, int F, int hidden) {
+    if (archive_check("nr_pool_ranks_archive", n_rows, P, n_news, 1, F, hidden) != 0) return -1;
+    return RankArchiveWorkspace(nullptr, n_rows, P, n_news, F, hidden, archive_splits(n_rows, P, n_news)).bytes();
+}
+
+int pool_ranks_archive(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F, const float* W1,
+                       const float* b1, int hidden, const float* w2, const float* b2, const long long* tgt_offsets,
+                       const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
+                       float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                       long long workspace_bytes, cudaStream_t stream) {
+    using namespace topk;
+    NR_PROPAGATE(archive_check("nr_pool_ranks_archive", n_rows, P, n_news, 1, F, hidden));
+    NR_REQUIRE((excl_offsets == nullptr) == (excl_rows == nullptr), "nr_pool_ranks_archive: excl_offsets and excl_rows go together");
+    const int splits = archive_splits(n_rows, P, n_news);
+    RankArchiveWorkspace ws(workspace, n_rows, P, n_news, F, hidden, splits);
+    NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
+               "nr_pool_ranks_archive: workspace of %lld bytes (256-byte aligned) needs %lld", workspace_bytes, ws.bytes());
+    if (n_rows == 0) return 0;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NR_CHECK_CUDA(cudaFuncSetAttribute(pool_ranks_archive_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+        attr_set = true;
+    }
+    CUtensorMap tm[4] = {};
+    ArchOperands o;
+    NR_PROPAGATE(ws.ops.prepare(archive, n_rows, P, news, n_news, F, W1, b1, hidden, w2, b2, tm, o, stream));
+    RankParams p;
+    p.n_rows = n_rows;
+    p.n_news = static_cast<int>(n_news);
+    p.k_chunks = ceil_div(F, 64);
+    p.tiles = static_cast<int>((n_news + kNews - 1) / kNews);
+    p.splits = splits;
+    p.tgt_offsets = tgt_offsets;
+    p.tgt_rows = tgt_rows;
+    p.excl_offsets = excl_offsets;
+    p.excl_rows = excl_rows;
+    p.rank = rank;
+    p.score = score;
+    p.part = ws.part;
+    p.bad_row_flag = bad_row_flag;
+    p.bad_score_flag = bad_score_flag;
+    p.target_flag = target_flag;
+    const size_t smem = 1024 + ArchSmem(o.P, o.G, o.hp, ranks_archive_rest(o.G)).bytes;
+    {
+        ProfScope ps("pool_ranks_archive", static_cast<int>(n_rows), static_cast<int>(n_news), splits, stream);
+        pool_ranks_archive_kernel<<<dim3(static_cast<unsigned>(archive_ctas(n_rows, P)), splits), kThreads, smem, stream>>>(
+            tm[0], tm[1], tm[2], tm[3], p, o);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    if (splits > 1) {
+        ProfScope ps("pool_ranks_merge", static_cast<int>(n_rows), splits, 0, stream);
+        pool_ranks_merge_kernel<<<static_cast<unsigned>((n_rows + 127) / 128), 128, 0, stream>>>(p);
+        ++g_launches;
+        NR_CHECK_CUDA(cudaGetLastError());
+    }
+    return 0;
+}
+
+// the largest shared memory either archive kernel asks for, over every P (G = 64 / P users per CTA)
+static constexpr int archive_smem_max() {
+    int m = 0;
+    for (int P = 1; P <= topk::kArchMaxP; ++P) {
+        const int G = topk::kUsers / P;
+        const int a = topk::ArchSmem(P, G, topk::kArchMaxHid, topk::topk_archive_rest(G)).bytes;
+        const int b = topk::ArchSmem(P, G, topk::kArchMaxHid, topk::ranks_archive_rest(G)).bytes;
+        m = std::max(m, std::max(a, b));
+    }
+    return 1024 + m;
+}
+static_assert(archive_smem_max() <= 232448, "topk_archive_kernel / pool_ranks_archive_kernel: shared memory");
 
 }  // namespace nr

@@ -40,6 +40,13 @@ class DKN(torch.nn.Module):
         """(batch, H, len(window_sizes) * num_filters) -> the same, as the reference"""
         return clicked_news_vector
 
+    def pool_user_vector(self, clicked_news_vector):
+        """(batch, H, F') -> (batch, F'): the one attention vector per user that the click predictor scores against, the user
+        operand of the whole-pool kernels (newsrec_b200.recommend, pool_eval)"""
+        require_cuda()
+        W1a, _, w2a, _ = self.attention.weights()
+        return DknUserFn.apply(clicked_news_vector, W1a, w2a)
+
     def get_prediction(self, candidate_news_vector, clicked_news_vector):
         """candidates (n, F'), clicked (H, F') -> click logits (n,)"""
         dev = require_cuda()

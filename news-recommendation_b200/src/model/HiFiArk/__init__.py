@@ -62,6 +62,10 @@ class HiFiArk(torch.nn.Module):
         require_cuda()
         return ArchiveUserFn.apply(clicked_news_vector, self.omap.W)
 
+    def pool_user_vector(self, clicked_news_vector):
+        """The user operand of the whole-pool kernels (newsrec_b200.recommend, pool_eval): the archive, as get_user_vector"""
+        return self.get_user_vector(clicked_news_vector)
+
     def get_prediction(self, candidate_news_vector, user_archive_vector):
         """(num_filters,) -> 0-dim logit, as the reference; (n, num_filters) -> (n,), what the reference's evaluate.py passes.
         user_archive_vector: (num_pooling_heads, num_filters)."""

@@ -616,8 +616,31 @@ def mmr_request(k, mmr_lambda, mmr_depth):
     return float(mmr_lambda), int(mmr_depth)
 
 
+def _pool_dnn(who, users, news, dnn):
+    """The archive DNN scorer's operands (nr_topk_archive): users (U, F) (P = 1) or (U, P, F), news (n, F), dnn = (W1 (hidden,
+    2F), b1 (hidden,), w2 (1, hidden) or (hidden,), b2 (1,)).  Returns (users (U, P, F), W1, b1, w2, b2), fp32 contiguous on
+    the device; raises NewsrecError on a shape the kernels refuse."""
+    if not isinstance(dnn, (tuple, list)) or len(dnn) != 4:
+        raise NewsrecError(f"{who}: dnn must be the predictor's (W1, b1, w2, b2)")
+    if news.dim() != 2 or users.dim() not in (2, 3) or users.shape[-1] != news.shape[1]:
+        raise NewsrecError(f"{who}: users {tuple(users.shape)} and news {tuple(news.shape)} must be (U, F) or (U, P, F) "
+                           "and (n, F)")
+    F = news.shape[1]
+    W1, b1, w2, b2 = dnn
+    hidden = W1.shape[0] if W1.dim() == 2 else -1
+    if W1.dim() != 2 or W1.shape[1] != 2 * F or b1.numel() != hidden or w2.numel() != hidden or b2.numel() != 1:
+        raise NewsrecError(f"{who}: dnn shapes W1 {tuple(W1.shape)}, b1 {tuple(b1.shape)}, w2 {tuple(w2.shape)}, "
+                           f"b2 {tuple(b2.shape)} do not fit news vectors of width {F}")
+    dev = require_cuda()
+    users = users.to(dev).float()
+    if users.dim() == 2:
+        users = users.unsqueeze(1)
+    return (users.contiguous(),) + tuple(t.detach().to(dev).float().reshape(s).contiguous()
+                                         for t, s in ((W1, (hidden, 2 * F)), (b1, (-1,)), (w2, (-1,)), (b2, (1,))))
+
+
 def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categories=None, max_per_category=None,
-                 mmr_lambda=None, mmr_depth=None):
+                 mmr_lambda=None, mmr_depth=None, dnn=None):
     """The k best news of every user over the whole pool, one pass (nr_topk_dot): users (U, D) and news (n, D) fp32, scores
     users[u] . news[r] at fp32 level on the tensor cores (the bound is in include/newsrec_b200.h) without the U x n score
     matrix.  Optional exclusions in CSR form: user u never gets rows excl_rows[excl_offsets[u] .. excl_offsets[u + 1]).
@@ -634,7 +657,12 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     re-ranking of the plain top mmr_depth (k <= depth <= 128, default min(128, 4k)): k times, the news of the shortlist not
     yet taken with the largest lambda rel - (1 - lambda) max cosine to the news taken, rel the score scaled to [0, 1] over
     the shortlist (include/newsrec_b200.h).  Scores are the picked news' own scores, in pick order; lambda = 1 gives the plain
-    answer bit for bit.  lambda is used as fp32.  Not together with a category cap."""
+    answer bit for bit.  lambda is used as fp32.  Not together with a category cap.
+
+    DNN click scores (nr_topk_archive): with dnn = the (W1, b1, w2, b2) of Hi-Fi Ark's or DKN's click predictor, users is
+    (U, F) (one vector per user, P = 1) or (U, P, F) (an archive per user) and the score of user u and news c is
+    b2 + w2 . relu(W1 [c; softmax_p(A_u c)^T A_u] + b1), fp32-accurate (the bound is in include/newsrec_b200.h).  The
+    exclusions, the category cap and MMR work as above."""
     lib = load_library()
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 128:
         raise NewsrecError(f"top_k_scores: k={k!r} must be an integer in [1, 128]")
@@ -644,8 +672,10 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
         raise NewsrecError(f"top_k_scores: {e}") from None
     if mmr is not None and (categories is not None or max_per_category is not None):
         raise NewsrecError("top_k_scores: mmr_lambda and a category cap do not combine")
-    if users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]:
+    if dnn is None and (users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]):
         raise NewsrecError(f"top_k_scores: users {tuple(users.shape)} and news {tuple(news.shape)} must be (U, D) and (n, D)")
+    if dnn is not None:
+        users, *dnn = _pool_dnn("top_k_scores", users, news, dnn)
     if (excl_rows is None) != (excl_offsets is None):
         raise NewsrecError("top_k_scores: excl_rows and excl_offsets go together")
     capped = categories is not None or max_per_category is not None
@@ -666,7 +696,7 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     dev = require_cuda()
     users = users.to(dev).float().contiguous()
     news = news.to(dev).float().contiguous()
-    U, D = users.shape
+    U, D = users.shape[0], users.shape[-1]
     n = news.shape[0]
     if excl_offsets is not None:
         excl_offsets = excl_offsets.to(dev).long().contiguous()
@@ -676,9 +706,15 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
         if excl_rows.numel() == 0:
             excl_rows = excl_rows.new_zeros(1)  # a valid address for an empty set
     kk = k if mmr is None else mmr[1]  # the shortlist's length
-    ws_bytes = int(lib.nr_topk_dot_workspace(U, n, D, kk))
-    if ws_bytes < 0:
-        check(-1, "nr_topk_dot_workspace")
+    if dnn is None:
+        ws_bytes = int(lib.nr_topk_dot_workspace(U, n, D, kk))
+        if ws_bytes < 0:
+            check(-1, "nr_topk_dot_workspace")
+    else:
+        P, hidden = users.shape[1], dnn[0].shape[0]
+        ws_bytes = int(lib.nr_topk_archive_workspace(U, P, n, D, hidden, kk))
+        if ws_bytes < 0:
+            check(-1, "nr_topk_archive_workspace")
     if U == 0 or n == 0:  # no user or nothing eligible: the library launches nothing
         return (torch.full((U, k), -1, dtype=torch.int64, device=dev),
                 torch.full((U, k), float("-inf"), dtype=torch.float32, device=dev))
@@ -686,7 +722,14 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     score = torch.empty((U, kk), dtype=torch.float32, device=dev)
     flags = torch.zeros(2, dtype=torch.int32, device=dev)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    if capped:
+    if dnn is not None:
+        cat = categories.to(device=dev, dtype=torch.int32).contiguous() if capped else None
+        W1, b1, w2, b2 = dnn
+        check(lib.nr_topk_archive(_p(users), U, P, _p(news), n, D, _p(W1), _p(b1), hidden, _p(w2), _p(b2), kk,
+                                  _p(excl_offsets), _p(excl_rows), _p(cat), max_per_category if capped else 0, _p(idx),
+                                  _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes, _stream()),
+              "nr_topk_archive")
+    elif capped:
         cat = categories.to(device=dev, dtype=torch.int32).contiguous()
         check(lib.nr_topk_dot_capped(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(cat),
                                      max_per_category, _p(idx), _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace),
@@ -744,7 +787,7 @@ def target_parts(tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None, max_t
     return query, offsets, ex_rows, ex_off
 
 
-def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None):
+def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None, *, dnn=None):
     """Ranks of target news among the whole pool under nr_topk_dot's scores (nr_pool_ranks): query q (users (Q, D) fp32)
     has targets tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) of news (n, D) fp32 and optional exclusions in CSR form.
     rank(q, t) is t's 0-based position in the order top_k_scores returns for q over the pool without q's exclusions and
@@ -752,15 +795,18 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
     (n_targets,) fp32 = s(q, t)) in target order, on the caller's stream.  Queries with more than 32 targets run as several
     kernel rows (target_parts).  Raises NewsrecError on bad arguments (before any launch), IndexError on a target or
     exclusion row outside [0, n) and ValueError on a non-finite score (the device flags are read once: one
-    synchronisation)."""
+    synchronisation).  With dnn = (W1, b1, w2, b2) the scores are top_k_scores(..., dnn=)'s (nr_pool_ranks_archive) and
+    users is (Q, F) or (Q, P, F)."""
     import numpy as np
     lib = load_library()
-    if users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]:
+    if dnn is None and (users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]):
         raise NewsrecError(f"pool_ranks: users {tuple(users.shape)} and news {tuple(news.shape)} must be (Q, D) and (n, D)")
+    if dnn is not None:
+        users, *dnn = _pool_dnn("pool_ranks", users, news, dnn)
     if (excl_rows is None) != (excl_offsets is None):
         raise NewsrecError("pool_ranks: excl_rows and excl_offsets go together")
     to = torch.as_tensor(tgt_offsets).cpu().long().numpy()
-    Q, D = users.shape
+    Q, D = users.shape[0], users.shape[-1]
     n = news.shape[0]
     if to.ndim != 1 or len(to) != Q + 1 or to[0] != 0 or (np.diff(to) < 0).any() or to[-1] != len(tgt_rows):
         raise NewsrecError("pool_ranks: tgt_offsets must be (Q + 1,), start at 0, not decrease and end at len(tgt_rows)")
@@ -772,8 +818,18 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
             raise NewsrecError("pool_ranks: excl_offsets must be (Q + 1,) non-decreasing offsets into the 1-D excl_rows")
     dev = require_cuda()
     n_t = int(to[-1])
-    if int(lib.nr_pool_ranks_workspace(max(Q, 0), max(n, 1), D)) < 0:
-        check(-1, "nr_pool_ranks_workspace")
+    if dnn is None:
+        def workspace_bytes(rows):
+            return int(lib.nr_pool_ranks_workspace(rows, max(n, 1), D))
+        ws_name = "nr_pool_ranks_workspace"
+    else:
+        P, hidden = users.shape[1], dnn[0].shape[0]
+
+        def workspace_bytes(rows):
+            return int(lib.nr_pool_ranks_archive_workspace(rows, P, max(n, 1), D, hidden))
+        ws_name = "nr_pool_ranks_archive_workspace"
+    if workspace_bytes(max(Q, 0)) < 0:
+        check(-1, ws_name)
     if n_t == 0:
         return torch.zeros(0, dtype=torch.int64, device=dev), torch.zeros(0, dtype=torch.float32, device=dev)
     if n == 0:
@@ -785,9 +841,9 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
     same = R == Q and bool((query == np.arange(Q)).all())
     rows = users.contiguous() if same else users.index_select(0, torch.from_numpy(query).to(dev)).contiguous()
     news = news.to(dev).float().contiguous()
-    ws_bytes = int(lib.nr_pool_ranks_workspace(R, n, D))
+    ws_bytes = workspace_bytes(R)
     if ws_bytes < 0:
-        check(-1, "nr_pool_ranks_workspace")
+        check(-1, ws_name)
     d_to = torch.from_numpy(offsets).to(dev)
     d_tr = torch.from_numpy(tr).to(dev)
     d_xo = d_xr = None
@@ -798,8 +854,15 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
     score = torch.empty(n_t, dtype=torch.float32, device=dev)
     flags = torch.zeros(3, dtype=torch.int32, device=dev)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    check(lib.nr_pool_ranks(_p(rows), R, D, _p(news), n, D, D, _p(d_to), _p(d_tr), _p(d_xo), _p(d_xr), _p(rank), _p(score),
-                            _p(flags[0:1]), _p(flags[1:2]), _p(flags[2:3]), _p(workspace), ws_bytes, _stream()), "nr_pool_ranks")
+    if dnn is None:
+        check(lib.nr_pool_ranks(_p(rows), R, D, _p(news), n, D, D, _p(d_to), _p(d_tr), _p(d_xo), _p(d_xr), _p(rank), _p(score),
+                                _p(flags[0:1]), _p(flags[1:2]), _p(flags[2:3]), _p(workspace), ws_bytes, _stream()),
+              "nr_pool_ranks")
+    else:
+        W1, b1, w2, b2 = dnn
+        check(lib.nr_pool_ranks_archive(_p(rows), R, P, _p(news), n, D, _p(W1), _p(b1), hidden, _p(w2), _p(b2), _p(d_to),
+                                        _p(d_tr), _p(d_xo), _p(d_xr), _p(rank), _p(score), _p(flags[0:1]), _p(flags[1:2]),
+                                        _p(flags[2:3]), _p(workspace), ws_bytes, _stream()), "nr_pool_ranks_archive")
     bad_row, bad_score, too_many = (int(x) for x in flags.tolist())
     if bad_row:
         raise IndexError("pool_ranks: a target or exclusion row is outside the news pool")

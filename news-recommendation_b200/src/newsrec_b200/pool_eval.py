@@ -13,8 +13,10 @@ question: does the news the user clicked come near the top of the whole pool?  P
 5. metrics  recall@K = |{p : c_p < K}| / |P_i|,  nDCG@K = sum_{c_p < K} 1 / log2(c_p + 2) / sum_{j < min(|P_i|, K)} 1 / log2(j + 2),
             MRR = 1 / (1 + min_p c_p), fp64 means over the counted impressions.
 
-Device memory is bounded by the chunk and the pool, and the result does not depend on the chunk.  The click predictor must be
-a dot product of a user vector and a news vector: NRMS, NAML, LSTUR, TANR and Exp1.
+Device memory is bounded by the chunk and the pool, and the result does not depend on the chunk.  NRMS, NAML, LSTUR, TANR and
+Exp1 are ranked under the dot product of user and news vectors; Hi-Fi Ark and DKN under their DNN click predictor, through
+their models' ``pool_user_vector`` and ``ops.pool_ranks(..., dnn=)`` (nr_pool_ranks_archive: the scores nr_topk_archive
+computes).  A model of those two families without ``pool_user_vector`` is refused.
 
     python -m newsrec_b200.pool_eval --directory data/val [--ks 5,10,20,50,100] [--keep-clicked]
                                      [--checkpoint PATH | --checkpoint-dir DIR] [--user2int data/train/user2int.tsv]
@@ -29,8 +31,8 @@ import sys
 import numpy as np
 
 from . import NewsrecError
-from .evaluate import build_tables, new_flag, news_matrix, read_behaviors, user_vectors, _gather
-from .recommend import _REFUSED, _Users, exclusion_csr
+from .evaluate import build_tables, new_flag, news_matrix, read_behaviors, _gather
+from .recommend import _Users, exclusion_csr, pool_operands, refuse_family
 
 DEFAULT_KS = (5, 10, 20, 50, 100)
 DEFAULT_CHUNK = 65536
@@ -42,9 +44,7 @@ def check_request(model, directory, ks):
     ks = tuple(ks)
     if not ks or any(isinstance(k, bool) or not isinstance(k, (int, np.integer)) or k < 1 for k in ks):
         raise NewsrecError(f"evaluate_pool: ks={ks!r} must be positive integers")
-    name = type(model).__name__
-    if name in _REFUSED:
-        raise NewsrecError(f"evaluate_pool: {name} is not supported: {_REFUSED[name]}")
+    refuse_family("evaluate_pool", model)
     for f in ("behaviors.tsv", "news_parsed.tsv"):
         if not os.path.isfile(os.path.join(directory, f)):
             raise FileNotFoundError(f"evaluate_pool: {os.path.join(directory, f)} not found")
@@ -116,14 +116,15 @@ def pool_positions(model, directory, *, exclude_clicked=True, max_count=sys.maxs
         for a in range(0, len(imp), chunk_impressions):
             b = min(len(imp), a + chunk_impressions)
             who, inv = np.unique(t.seg_user[imp[a:b]], return_inverse=True)
-            uv = user_vectors(model, _Users(t.user[who], t.history[who], t.history_length[who]), matrix, flag)
-            queries = _gather(inv.astype(np.int64), uv, flag)
+            uv, dnn = pool_operands(model, _Users(t.user[who], t.history[who], t.history_length[who]), matrix, flag)
+            queries = _gather(inv.astype(np.int64), uv.reshape(uv.shape[0], -1), flag).view(-1, *uv.shape[1:])
             excl = None, None
             if exclude_clicked:
                 xr, xo = exclusion_csr(t.history[t.seg_user[imp[a:b]]], pad)
                 excl = torch.from_numpy(xr), torch.from_numpy(xo)
             lo, hi = offsets[a], offsets[b]
-            r, s = pool_ranks(queries, pool, torch.from_numpy(rows[lo:hi]), torch.from_numpy(offsets[a:b + 1] - lo), *excl)
+            r, s = pool_ranks(queries, pool, torch.from_numpy(rows[lo:hi]), torch.from_numpy(offsets[a:b + 1] - lo), *excl,
+                              dnn=dnn)
             if int(flag.item()):
                 raise IndexError("evaluate_pool: a history row is outside the news table")
             rank[lo:hi], score[lo:hi] = r.cpu().numpy(), s.cpu().numpy()
@@ -156,7 +157,9 @@ def parse_ks(text):
 
 def parse_args(argv=None):
     import argparse
-    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0],
+                                 epilog="Every family is served: NRMS, NAML, LSTUR, TANR and Exp1 by the dot product of user and "
+                                        "news vectors, Hi-Fi Ark and DKN by their DNN click predictor.")
     ap.add_argument("--directory", default="./data/val", help="labelled split: news_parsed.tsv (the pool) and behaviors.tsv")
     ap.add_argument("--ks", default=",".join(map(str, DEFAULT_KS)), help="comma-separated cut-offs of recall@K and nDCG@K")
     g = ap.add_mutually_exclusive_group()

@@ -12,7 +12,11 @@ news without the U x n score matrix ever reaching memory (``ops.top_k_scores``, 
              lines formatted on the host and appended to the file.  Device memory is bounded by the chunk and the pool,
              not by the file, and the bytes do not depend on the chunk.
 
-The click predictor must be a dot product of a user vector and a news vector: NRMS, NAML, LSTUR, TANR and Exp1.
+NRMS, NAML, LSTUR, TANR and Exp1 score a user vector against a news vector by a dot product.  Hi-Fi Ark and DKN score them
+with their DNN click predictor, over the user's archive (Hi-Fi Ark, similarity attention) or its one attention vector (DKN):
+their models' ``pool_user_vector`` gives that operand and ``ops.top_k_scores(..., dnn=click_predictor.weights())``
+(nr_topk_archive) the top k under the same scores ``evaluate`` computes, to within the bound of include/newsrec_b200.h.
+A model of those two families without ``pool_user_vector`` is refused.
 
 Diversified lists: with ``max_per_category=m`` no line holds more than m news of one category (``diversify_by="category"``)
 or of one subcategory (``"subcategory"``), the column of ``news_parsed.tsv`` in the matrix's row order, copied once to the
@@ -41,13 +45,14 @@ import sys
 import numpy as np
 
 from . import NewsrecError
-from .evaluate import distinct_histories, new_flag, news_matrix, read_behaviors, read_news, user_tables, user_vectors
+from .evaluate import _gather, distinct_histories, new_flag, news_matrix, read_behaviors, read_news, user_tables, user_vectors
 
 DEFAULT_CHUNK = 65536
 MAX_K = 128
 DIVERSIFY_FIELDS = ("category", "subcategory")
 # Families whose click score is not users . news: Hi-Fi Ark's depends on the candidate through the similarity attention over
-# the user's archive; DKN's DNN scorer is separable (w2 . relu(W1c c + W1u u + b1)) but is not a single dot product.
+# the user's archive; DKN's DNN scorer is separable (w2 . relu(W1c c + W1u u + b1)) but is not a single dot product.  They
+# are served through the DNN scorer kernels when the model exposes pool_user_vector, and refused otherwise.
 _REFUSED = {
     "HiFiArk": "Hi-Fi Ark's click score depends on the candidate through the similarity attention over the archive, so it is "
                "not a dot product of one user vector and one news vector",
@@ -67,9 +72,7 @@ def check_request(model, directory, k, max_per_category=None, diversify_by="cate
         raise NewsrecError(f"recommend: max_per_category={max_per_category!r} must be an integer >= 1")
     if diversify_by not in DIVERSIFY_FIELDS:
         raise NewsrecError(f"recommend: diversify_by={diversify_by!r} must be one of {DIVERSIFY_FIELDS}")
-    name = type(model).__name__
-    if name in _REFUSED:
-        raise NewsrecError(f"recommend: {name} is not supported: {_REFUSED[name]}")
+    refuse_family("recommend", model)
     from .ops import mmr_request
     try:
         mmr = mmr_request(int(k), mmr_lambda, mmr_depth)
@@ -85,6 +88,26 @@ def check_request(model, directory, k, max_per_category=None, diversify_by="cate
             header = f.readline().rstrip("\r\n").split("\t")
         if diversify_by not in header:
             raise NewsrecError(f"recommend: {os.path.join(directory, 'news_parsed.tsv')} has no {diversify_by} column")
+
+
+def refuse_family(who, model):
+    """Raises NewsrecError for a model whose click score is not a dot product and that has no pool_user_vector."""
+    name = type(model).__name__
+    if name in _REFUSED and not hasattr(model, "pool_user_vector"):
+        raise NewsrecError(f"{who}: {name} is not supported: {_REFUSED[name]}")
+
+
+def pool_operands(model, tables, matrix, flag):
+    """(users, dnn) for the whole-pool kernels: (user_vectors(...), None) for a dot-product family; for Hi-Fi Ark and DKN,
+    model.pool_user_vector over batches of batch_size * 16 histories ((U, P, F) or (U, F)) and click_predictor.weights()."""
+    import torch
+    if type(model).__name__ not in _REFUSED:
+        return user_vectors(model, tables, matrix, flag), None
+    bs, H, F = model.config.batch_size * 16, tables.history.shape[1], matrix.shape[1]
+    out = [model.pool_user_vector(_gather(tables.history[lo:lo + bs].reshape(-1), matrix, flag).view(-1, H, F))
+           for lo in range(0, len(tables.user), bs)]
+    users = torch.cat(out) if out else torch.zeros((0, F), dtype=torch.float32, device=matrix.device)
+    return users, model.click_predictor.weights()
 
 
 def exclusion_csr(history, pad):
@@ -147,12 +170,12 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
             with open(tmp, "wb") as f:
                 for a in range(0, U, chunk_users):
                     b = min(U, a + chunk_users)
-                    users = user_vectors(model, _Users(user[a:b], history[a:b], length[a:b]), matrix, flag)
+                    users, dnn = pool_operands(model, _Users(user[a:b], history[a:b], length[a:b]), matrix, flag)
                     excl = None, None
                     if exclude_clicked:
                         rows, offsets = exclusion_csr(history[a:b], pad)
                         excl = torch.from_numpy(rows), torch.from_numpy(offsets)
-                    idx, _ = top_k_scores(users, pool, int(k), *excl, **cap)  # reads its flags: synchronises
+                    idx, _ = top_k_scores(users, pool, int(k), *excl, dnn=dnn, **cap)  # reads its flags: synchronises
                     if int(flag.item()):
                         raise IndexError("recommend: a history row is outside the news table")
                     f.write(format_lines(user_ids[a:b], idx.cpu().numpy(), news_ids))
@@ -165,7 +188,9 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
 
 def parse_args(argv=None):
     import argparse
-    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0],
+                                 epilog="Every family is served: NRMS, NAML, LSTUR, TANR and Exp1 by the dot product of user and "
+                                        "news vectors, Hi-Fi Ark and DKN by their DNN click predictor.")
     ap.add_argument("--directory", default="./data/test", help="split: news_parsed.tsv (the pool) and behaviors.tsv (the users)")
     ap.add_argument("--out", default="recommendations.tsv", help="the file to write")
     ap.add_argument("--k", type=int, default=10, help=f"news per user, 1 .. {MAX_K}")

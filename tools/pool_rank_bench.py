@@ -4,6 +4,10 @@ nr_topk_dot at k = 10 on the same rows and exclusions and against chunked torch.
 greater scores of every target, the three timed alternately in the same run.
 
     python tools/pool_rank_bench.py [--rows 700000] [--news 120000] [--dim 300] [--reps 3] [--seed 0]
+                                    [--scorer {dot,hifiark,dkn} [--baseline-users 8192]]
+
+--scorer hifiark | dkn times nr_pool_ranks_archive under the DNN click score instead, with nr_topk_archive at k = 10 and a
+torch restatement (tools/archive_pool_bench.py).
 
 Time: CUDA events around the library call alone (operand planes, the rank or top-k kernel, the split merge when there is one)
 on device-resident CSR, after a warm-up, best and median over reps.  Check: on a sample of rows, the kernel's ranks and the
@@ -22,6 +26,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "news-recommendation_b200", "src"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+import archive_pool_bench  # noqa: E402
 from recommend_bench import card  # noqa: E402
 
 
@@ -34,7 +39,11 @@ def main(argv=None):
     ap.add_argument("--baseline-chunk", type=int, default=4096, help="rows per torch.matmul + count pass")
     ap.add_argument("--sample", type=int, default=300, help="rows checked against the fp64 band")
     ap.add_argument("--seed", type=int, default=0)
+    archive_pool_bench.add_args(ap)
     a = ap.parse_args(argv)
+    if a.scorer != "dot":
+        print(f"card: {card()}", flush=True)
+        return archive_pool_bench.rank_arms(a, card)
     import torch
     from newsrec_b200 import check, load_library, require_cuda
     lib = load_library()

@@ -16,9 +16,13 @@ mmr_lambda=, mmr_depth=): the shortlist plus the rerank.  Quality over a sample 
 mean cosine of the pairs within a list, and the mean relevance (the score scaled to [0, 1] over the user's shortlist).  The
 sampled MMR lists go through the fp64 path verifier of tests/mmr_ref.py.
 
+DNN click scores (--scorer hifiark | dkn): nr_topk_archive, with and without a category cap (--max-per-category, default 2),
+against a torch restatement and the per-user nr_archive_score_fwd path (tools/archive_pool_bench.py).
+
     python tools/recommend_bench.py [--users 700000] [--news 120000] [--dim 300] [--k 10 100] [--reps 3] [--seed 0]
                                     [--max-per-category M [--categories 17] [--zipf 0]]
                                     [--mmr-lambda X [--mmr-depth 40] [--stories 2000]]
+                                    [--scorer {dot,hifiark,dkn} [--baseline-users 8192] [--sample-users 256]]
 
 Time: CUDA events around the library's launches (operand planes, the top-k kernel, the split merge when there is one), after
 a warm-up, best and median over reps.  Rates: multiply-adds of the three bf16 products per score (3 n_users n_news
@@ -36,6 +40,9 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "news-recommendation_b200", "src"))
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+import archive_pool_bench  # noqa: E402
 
 
 def card():
@@ -63,7 +70,13 @@ def main(argv=None):
                     help="time nr_mmr_rerank at this lambda against nr_topk_dot and a torch restatement")
     ap.add_argument("--mmr-depth", type=int, default=40, metavar="L", help="shortlist length (with --mmr-lambda)")
     ap.add_argument("--stories", type=int, default=2000, help="story centroids of the clustered pool (with --mmr-lambda)")
+    archive_pool_bench.add_args(ap)
     a = ap.parse_args(argv)
+    if a.scorer != "dot":
+        if a.mmr_lambda is not None:
+            ap.error("--mmr-lambda is timed with --scorer dot")
+        print(f"card: {card()}", flush=True)
+        return archive_pool_bench.recommend_arms(a, card)
     if a.mmr_lambda is not None and (a.max_per_category is not None or not 0 <= a.mmr_lambda <= 1 or
                                      not max(a.k) <= a.mmr_depth <= 128):
         ap.error("--mmr-lambda takes a lambda in [0, 1], a --mmr-depth in [max(--k), 128] and no --max-per-category")
