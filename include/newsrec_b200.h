@@ -320,6 +320,27 @@ int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, cons
 int nr_mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* shortlist_idx, const float* shortlist_score,
                   long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag, void* stream);
 
+/* Statistics of recommendation lists (how similar and how varied each list is).  news fp32 [n_news][ld_news] (pitch >= D);
+ * idx int64 [n_rows][k], e.g. nr_topk_dot's, nr_topk_dot_capped's or nr_mmr_rerank's output; categories device int32
+ * [n_news] (any values) or null; ks a HOST array of n_ks cut-offs, strictly ascending, each in [1, k], n_ks <= 8.  For row r
+ * the live entries are those before the first -1 (entries after it are ignored), L_r of them; for cut-off K, K' = min(K, L_r):
+ *   pair_sum[r][c] = sum_{j < K'} ( sum_{i < j} sim(i, j) )     (fp64 [n_rows][n_ks]; each inner sum in fp64 with i
+ *                    ascending, the outer sum in fp64 with j ascending; 0 when K' < 2)
+ *   distinct[r][c] = the number of distinct categories values among the first K' entries   (int32 [n_rows][n_ks], exact)
+ * with K = ks[c].  sim is nr_mmr_rerank's cosine, computed the same way by the same device routines: the rows gathered into
+ * hi/lo bf16 planes 64 columns at a time, G = hi.lo + lo.hi + hi.hi on the tensor cores with fp32 accumulation,
+ * sim(i, j) = (G_ji rsqrt(G_jj)) rsqrt(G_ii) in correctly rounded fp32, 0 when either row is all zeros.  So each pair is
+ * within nr_mmr_rerank's
+ *     e_sim = c eps + 2^-21,    c = 2 / (1 - eps),    eps = 2^-15 + 3 round_up(D, 64) 2^-23
+ * of the exact cosine of the fp32 rows (rows whose squared norms are fp32 normal numbers), and with P = K'(K' - 1) / 2 pairs,
+ *     |pair_sum - sum of the exact cosines| <= P e_sim + P^2 2^-52     (the second term: the fp64 additions),
+ * so the mean over the pairs is within e_sim + P 2^-52 of the exact mean.  distinct is null iff categories is null.
+ * Limits: 1 <= D <= 4096; 1 <= k <= 128; ks as above; n_rows and n_news in [0, 2^31 - 64).  A live entry outside
+ * [0, n_news) sets *bad_row_flag (that row's outputs are then undefined).  Every limit is refused (-1) before the first
+ * launch; n_rows == 0 launches nothing.  The same inputs give the same bits on every run.  One block per row. */
+int nr_list_stats(const float* news, long long n_news, int ld_news, int D, const long long* idx, long long n_rows, int k,
+                  const int* categories, const int* ks, int n_ks, double* pair_sum, int* distinct, int* bad_row_flag, void* stream);
+
 /* Ranks over a whole news pool under nr_topk_dot's scores.  Query row q (queries fp32 [n_rows][ld_queries]) has the target
  * set T_q = tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) and the exclusion set X_q (excl_offsets / excl_rows as in
  * nr_topk_dot: both null, or both device int64; a set, any length, order or duplicates).  For every target t of q:

@@ -239,6 +239,12 @@ int nr_mmr_rerank(const float* news, long long n_news, int ld_news, int D, const
     return mmr_rerank(news, n_news, ld_news, D, shortlist_idx, shortlist_score, n_users, depth, k, lambda, idx, score, bad_row_flag,
                       as_stream(stream));
 }
+int nr_list_stats(const float* news, long long n_news, int ld_news, int D, const long long* idx, long long n_rows, int k,
+                  const int* categories, const int* ks, int n_ks, double* pair_sum, int* distinct, int* bad_row_flag, void* stream) {
+    NR_REQUIRE(news && idx && ks && pair_sum && bad_row_flag, "nr_list_stats: null operand");
+    return list_stats(news, n_news, ld_news, D, idx, n_rows, k, categories, ks, n_ks, pair_sum, distinct, bad_row_flag,
+                      as_stream(stream));
+}
 long long nr_pool_ranks_workspace(long long n_rows, long long n_news, int D) { return pool_ranks_workspace(n_rows, n_news, D); }
 int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
                   const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,

@@ -303,6 +303,10 @@ int pool_ranks_archive(const float* archive, long long n_rows, int P, const floa
 int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* sl_idx, const float* sl_score,
                long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag,
                cudaStream_t stream);
+// per-list pair similarity sums and distinct-category counts (topk.cu; include/newsrec_b200.h, nr_list_stats)
+int list_stats(const float* news, long long n_news, int ld_news, int D, const long long* idx, long long n_rows, int k,
+               const int* categories, const int* ks, int n_ks, double* pair_sum, int* distinct, int* bad_row_flag,
+               cudaStream_t stream);
 int num_sms();
 extern int g_launches;  // kernels launched by this library (nr_launch_count)
 

@@ -41,6 +41,10 @@
 // MMR re-ranking (nr_mmr_rerank): one block per user re-ranks nr_topk_dot's shortlist (<= 128 entries).  The live rows are
 // gathered and split into hi/lo planes in the swizzled layout the TMA boxes above have, their Gram runs on the same three
 // products, and the greedy reads the Gram from shared memory.  The bounds and their derivation are in the header and DESIGN §3.
+//
+// List statistics (nr_list_stats): one block per list, the same live-row load, gather and Gram routines (load_live_rows,
+// gram_hilo) and the same cosine (gram_sim), so a pair's similarity is the bits nr_mmr_rerank uses; the fp64 pair sums and
+// the distinct-category counts are then a few hundred operations per list.
 #include <algorithm>
 #include <cmath>
 
@@ -713,11 +717,17 @@ constexpr size_t kMmrGram = size_t(kMmrDepth) * kMmrGramLd * 4;  // aliases the 
 constexpr size_t kMmrSmem = 1024 + (kMmrBuf > kMmrGram ? kMmrBuf : kMmrGram) + 1024;
 static_assert(kMmrSmem <= 232448, "mmr_rerank_kernel: shared memory");
 
-struct MmrParams {
+// the rows whose Gram one block computes: fp32 [.][ld], D columns in k_chunks blocks of 64
+struct GramRows {
     const float* news;
-    long long n_news, n_users;
-    int ld, D, k_chunks, depth, k;
+    int ld, D, k_chunks;
     bool vec4;                // news and ld allow 16-byte loads
+};
+
+struct MmrParams {
+    GramRows src;
+    long long n_news, n_users;
+    int depth, k;
     float lam, one_minus_lam;
     const long long* sl_idx;  // [n_users][depth] nr_topk_dot's list
     const float* sl_score;
@@ -726,9 +736,29 @@ struct MmrParams {
     int* bad_row_flag;
 };
 
-// chunk c (columns [64c, 64c + 64)) of the shortlist's rows into hi / lo planes, rows at and past live zero: thread t
+// the live entries of one list of len <= 128 (those before the first -1) into rows, all threads: a row outside [0, n_news)
+// sets the flag and reads as zeros (-1).  Returns the number of live entries.
+__device__ __forceinline__ int load_live_rows(const long long* list, int len, long long n_news, int* rows, int* s_live,
+                                              int* bad_row_flag) {
+    const int tid = threadIdx.x;
+    if (tid == 0) *s_live = len;
+    __syncthreads();
+    const long long r = tid < len ? list[tid] : -1;
+    if (tid < len && r == -1) atomicMin(s_live, tid);
+    __syncthreads();
+    const int live = *s_live;
+    if (tid < live) {
+        const bool ok = r >= 0 && r < n_news;
+        if (!ok) atomicOr(bad_row_flag, 1);
+        rows[tid] = ok ? static_cast<int>(r) : -1;
+    }
+    __syncthreads();
+    return live;
+}
+
+// chunk c (columns [64c, 64c + 64)) of the list's rows into hi / lo planes, rows at and past live zero: thread t
 // converts the 16-byte pieces t, t + 256, ... (row q / 8, piece q % 8, which lands at piece (q % 8) ^ (row % 8))
-__device__ __forceinline__ void mmr_gather_chunk(const MmrParams& p, const int* rows, int live, int c, uint8_t* buf) {
+__device__ __forceinline__ void gram_gather_chunk(const GramRows& p, const int* rows, int live, int c, uint8_t* buf) {
     for (int q = threadIdx.x; q < kMmrDepth * 8; q += kMmrThreads) {
         const int r = q >> 3, j = q & 7, col0 = c * 64 + 8 * j;
         float x[8];
@@ -755,41 +785,16 @@ __device__ __forceinline__ void mmr_gather_chunk(const MmrParams& p, const int* 
     }
 }
 
-// one block per user.  Gram G[i][j] of the live rows (hi.lo + lo.hi + hi.hi on wgmma, m64n128 per warpgroup, the gather of
-// chunk c + 1 under the MMAs of chunk c), then the greedy on warpgroup 0, one thread per shortlist position
-__global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* G = reinterpret_cast<float*>(base);  // [kMmrDepth][kMmrGramLd], after the last chunk
-    __shared__ int rows[kMmrDepth];
-    __shared__ float rn[kMmrDepth];                    // 1 / |row| from the diagonal, 0 for a zero row
-    __shared__ float red_s[2][4];                      // per-warp (objective or score) and position of a step
-    __shared__ int red_i[2][4];
-    __shared__ int s_live;
+// all 256 threads: the Gram G[i][j] = hi_i.lo_j + lo_i.hi_j + hi_i.hi_j of the first live rows (rows past live are zeros)
+// on wgmma, m64n128 per warpgroup, the gather of chunk c + 1 under the MMAs of chunk c; G [kMmrDepth][kMmrGramLd] fp32
+// overwrites the chunk buffers at base and is complete for every thread on return
+__device__ __forceinline__ void gram_hilo(const GramRows& p, const int* rows, int live, uint8_t* base) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
-    const long long u = blockIdx.x;
-    const long long* sl_idx = p.sl_idx + u * p.depth;
-    const float* sl_score = p.sl_score + u * p.depth;
-
-    // ---- the live entries: those before the first -1; a row outside [0, n_news) is flagged and reads as zeros ----
-    if (tid == 0) s_live = p.depth;
-    __syncthreads();
-    const long long r = tid < p.depth ? sl_idx[tid] : -1;
-    if (tid < p.depth && r == -1) atomicMin(&s_live, tid);
-    __syncthreads();
-    const int live = s_live;
-    if (tid < live) {
-        const bool ok = r >= 0 && r < p.n_news;
-        if (!ok) atomicOr(p.bad_row_flag, 1);
-        rows[tid] = ok ? static_cast<int>(r) : -1;
-    }
-    __syncthreads();
-
-    // ---- Gram ----
+    float* G = reinterpret_cast<float*>(base);
     float acc[kMmrDepth / 2];
 #pragma unroll
     for (int i = 0; i < kMmrDepth / 2; ++i) acc[i] = 0.f;
-    mmr_gather_chunk(p, rows, live, 0, base);
+    gram_gather_chunk(p, rows, live, 0, base);
     fence_proxy_async();
     __syncthreads();
     // every warpgroup issues its MMAs on every chunk (rows past live are zeros): a warpgroup-divergent wgmma is serialised
@@ -808,7 +813,7 @@ __global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams
         }
         wgmma_commit();
         // the other buffer was last read by chunk c - 1's MMAs, which every warpgroup waited for before the barrier
-        if (c + 1 < p.k_chunks) mmr_gather_chunk(p, rows, live, c + 1, base + ((c + 1) & 1) * 2 * kMmrPlane);
+        if (c + 1 < p.k_chunks) gram_gather_chunk(p, rows, live, c + 1, base + ((c + 1) & 1) * 2 * kMmrPlane);
         wgmma_wait<0>();
 #pragma unroll
         for (int i = 0; i < kMmrDepth / 2; ++i) wgmma_reg_fence(acc[i]);
@@ -824,6 +829,31 @@ __global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams
             *reinterpret_cast<float2*>(G + row * kMmrGramLd + col) = make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]);
         }
     __syncthreads();
+}
+
+// 1 / |x_i| from the Gram's diagonal, 0 for a zero row
+__device__ __forceinline__ float gram_rnorm(float g_ii) { return g_ii > 0.f ? __frsqrt_rn(g_ii) : 0.f; }
+
+// sim(i, j) = (G_ji rsqrt(G_jj)) rsqrt(G_ii), each product rounded on its own (the cosine of nr_mmr_rerank and nr_list_stats)
+__device__ __forceinline__ float gram_sim(float g_ji, float rn_j, float rn_i) { return __fmul_rn(__fmul_rn(g_ji, rn_j), rn_i); }
+
+// one block per user: the Gram of the live rows (gram_hilo), then the greedy on warpgroup 0, one thread per shortlist position
+__global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const float* G = reinterpret_cast<const float*>(base);  // [kMmrDepth][kMmrGramLd], after gram_hilo
+    __shared__ int rows[kMmrDepth];
+    __shared__ float rn[kMmrDepth];                    // 1 / |row| from the diagonal, 0 for a zero row
+    __shared__ float red_s[2][4];                      // per-warp (objective or score) and position of a step
+    __shared__ int red_i[2][4];
+    __shared__ int s_live;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const long long u = blockIdx.x;
+    const long long* sl_idx = p.sl_idx + u * p.depth;
+    const float* sl_score = p.sl_score + u * p.depth;
+
+    const int live = load_live_rows(sl_idx, p.depth, p.n_news, rows, &s_live, p.bad_row_flag);
+    gram_hilo(p.src, rows, live, base);
     if (wg != 0) return;
 
     // ---- relevance: (s_i - s_min) / (s_max - s_min) over the live entries, 1 when they are all equal ----
@@ -841,8 +871,7 @@ __global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams
         red_s[1][warp] = smin;
     }
     if (is_live) {
-        const float g = G[i * kMmrGramLd + i];
-        rn[i] = g > 0.f ? __frsqrt_rn(g) : 0.f;
+        rn[i] = gram_rnorm(G[i * kMmrGramLd + i]);
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     smax = fmaxf(fmaxf(red_s[0][0], red_s[0][1]), fmaxf(red_s[0][2], red_s[0][3]));
@@ -896,12 +925,83 @@ __global__ void __launch_bounds__(kMmrThreads) mmr_rerank_kernel(const MmrParams
             out_score[t] = s;
         }
         // sim(i, best) = (G[best][i] / |best|) / |i|: row best of the Gram
-        const float sim = __fmul_rn(__fmul_rn(G[best * kMmrGramLd + i], rn[best]), rn_i);
+        const float sim = gram_sim(G[best * kMmrGramLd + i], rn[best], rn_i);
         msim = t == 0 ? sim : fmaxf(msim, sim);
     }
     for (int t = picks + i; t < p.k; t += 128) {
         out_idx[t] = -1;
         out_score[t] = -INFINITY;
+    }
+}
+
+// ---- per-list similarity and category statistics (nr_list_stats) ----
+constexpr int kListMaxKs = 8;  // cut-offs per call
+
+struct ListStatsParams {
+    GramRows src;
+    long long n_news;
+    const long long* idx;      // [n_rows][k]
+    const int* categories;     // [n_news] or null
+    int k, n_ks, k_max;        // k_max = ks[n_ks - 1]
+    int ks[kListMaxKs];        // ascending, in [1, k]
+    double* pair_sum;          // [n_rows][n_ks]
+    int* distinct;             // [n_rows][n_ks], null iff categories is
+    int* bad_row_flag;
+};
+
+// one block per list: the Gram of the entries the largest cut-off reads (gram_hilo, as nr_mmr_rerank), then thread j sums
+// sim(i, j) over i < j in fp64 (i ascending) and marks whether its category is new among entries 0 .. j; thread c of the
+// cut-offs adds those up over j < K' (j ascending)
+__global__ void __launch_bounds__(kMmrThreads) list_stats_kernel(const ListStatsParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const float* G = reinterpret_cast<const float*>(base);  // [kMmrDepth][kMmrGramLd], after gram_hilo
+    __shared__ int rows[kMmrDepth];
+    __shared__ float rn[kMmrDepth];
+    __shared__ double row_sum[kMmrDepth];              // sum_{i < j} sim(i, j)
+    __shared__ int cat[kMmrDepth];
+    __shared__ int is_new[kMmrDepth];                  // entry j's category is not among entries 0 .. j - 1
+    __shared__ int s_live;
+    const int tid = threadIdx.x;
+    const long long r = blockIdx.x;
+
+    const int live = load_live_rows(p.idx + r * p.k, p.k, p.n_news, rows, &s_live, p.bad_row_flag);
+    const int used = min(live, p.k_max);               // block-uniform
+    if (used >= 2) {
+        gram_hilo(p.src, rows, used, base);
+        if (tid < used) rn[tid] = gram_rnorm(G[tid * kMmrGramLd + tid]);
+    }
+    if (p.categories && tid < used) cat[tid] = rows[tid] >= 0 ? __ldg(p.categories + rows[tid]) : 0;
+    __syncthreads();
+    if (tid < used) {
+        const int j = tid;
+        double s = 0.0;
+        if (used >= 2) {
+            const float rn_j = rn[j];
+            for (int i = 0; i < j; ++i) s += static_cast<double>(gram_sim(G[j * kMmrGramLd + i], rn_j, rn[i]));
+        }
+        row_sum[j] = s;
+        if (p.categories) {
+            const int c = cat[j];
+            int fresh = 1;
+            for (int i = 0; i < j; ++i) fresh &= cat[i] != c;
+            is_new[j] = fresh;
+        }
+    }
+    __syncthreads();
+    if (tid < p.n_ks) {
+        int K = 0;
+#pragma unroll
+        for (int c = 0; c < kListMaxKs; ++c) K = c == tid ? p.ks[c] : K;  // no dynamic index into the parameters
+        const int kk = min(K, live);
+        double s = 0.0;
+        int d = 0;
+        for (int j = 0; j < kk; ++j) s += row_sum[j];
+        p.pair_sum[r * p.n_ks + tid] = s;
+        if (p.categories) {
+            for (int j = 0; j < kk; ++j) d += is_new[j];
+            p.distinct[r * p.n_ks + tid] = d;
+        }
     }
 }
 
@@ -1562,6 +1662,16 @@ int pool_ranks(const float* queries, long long n_rows, int ld_queries, const flo
     return 0;
 }
 
+static topk::GramRows gram_rows(const float* news, int ld_news, int D) {
+    topk::GramRows g;
+    g.news = news;
+    g.ld = ld_news;
+    g.D = D;
+    g.k_chunks = ceil_div(D, 64);
+    g.vec4 = ld_news % 4 == 0 && (reinterpret_cast<uintptr_t>(news) & 15) == 0;
+    return g;
+}
+
 int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* sl_idx, const float* sl_score,
                long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag,
                cudaStream_t stream) {
@@ -1580,15 +1690,11 @@ int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const lo
         attr_set = true;
     }
     MmrParams p;
-    p.news = news;
+    p.src = gram_rows(news, ld_news, D);
     p.n_news = n_news;
     p.n_users = n_users;
-    p.ld = ld_news;
-    p.D = D;
-    p.k_chunks = ceil_div(D, 64);
     p.depth = depth;
     p.k = k;
-    p.vec4 = ld_news % 4 == 0 && (reinterpret_cast<uintptr_t>(news) & 15) == 0;
     p.lam = lambda;
     p.one_minus_lam = 1.f - lambda;
     p.sl_idx = sl_idx;
@@ -1598,6 +1704,45 @@ int mmr_rerank(const float* news, long long n_news, int ld_news, int D, const lo
     p.bad_row_flag = bad_row_flag;
     ProfScope ps("mmr_rerank", static_cast<int>(n_users), depth, k, stream);
     mmr_rerank_kernel<<<static_cast<unsigned>(n_users), kMmrThreads, kMmrSmem, stream>>>(p);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int list_stats(const float* news, long long n_news, int ld_news, int D, const long long* idx, long long n_rows, int k,
+               const int* categories, const int* ks, int n_ks, double* pair_sum, int* distinct, int* bad_row_flag,
+               cudaStream_t stream) {
+    using namespace topk;
+    NR_REQUIRE(D >= 1 && D <= 4096, "nr_list_stats: D=%d outside [1, 4096]", D);
+    NR_REQUIRE(ld_news >= D, "nr_list_stats: pitch ld_news=%d below D=%d", ld_news, D);
+    NR_REQUIRE(k >= 1 && k <= kMmrDepth, "nr_list_stats: k=%d outside [1, %d]", k, kMmrDepth);
+    NR_REQUIRE(n_news >= 0 && n_news < (1ll << 31) - kNews, "nr_list_stats: n_news=%lld outside [0, 2^31 - 64)", n_news);
+    NR_REQUIRE(n_rows >= 0 && n_rows < (1ll << 31) - kUsers, "nr_list_stats: n_rows=%lld outside [0, 2^31 - 64)", n_rows);
+    NR_REQUIRE(n_ks >= 1 && n_ks <= kListMaxKs, "nr_list_stats: n_ks=%d outside [1, %d]", n_ks, kListMaxKs);
+    for (int c = 0; c < n_ks; ++c)
+        NR_REQUIRE(ks[c] >= 1 && ks[c] <= k && (c == 0 || ks[c] > ks[c - 1]),
+                   "nr_list_stats: ks[%d]=%d is not above the previous cut-off or outside [1, k=%d]", c, ks[c], k);
+    NR_REQUIRE((categories == nullptr) == (distinct == nullptr), "nr_list_stats: categories and distinct go together");
+    if (n_rows == 0) return 0;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NR_CHECK_CUDA(cudaFuncSetAttribute(list_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kMmrSmem)));
+        attr_set = true;
+    }
+    ListStatsParams p;
+    p.src = gram_rows(news, ld_news, D);
+    p.n_news = n_news;
+    p.idx = idx;
+    p.categories = categories;
+    p.k = k;
+    p.n_ks = n_ks;
+    p.k_max = ks[n_ks - 1];
+    for (int c = 0; c < kListMaxKs; ++c) p.ks[c] = c < n_ks ? ks[c] : k;
+    p.pair_sum = pair_sum;
+    p.distinct = distinct;
+    p.bad_row_flag = bad_row_flag;
+    ProfScope ps("list_stats", static_cast<int>(n_rows), k, n_ks, stream);
+    list_stats_kernel<<<static_cast<unsigned>(n_rows), kMmrThreads, kMmrSmem, stream>>>(p);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

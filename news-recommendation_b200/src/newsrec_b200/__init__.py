@@ -180,6 +180,7 @@ SIGNATURES = {
     "nr_topk_dot": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_topk_dot_capped": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_mmr_rerank": (_i, [_vp, _ll, _i, _i, _vp, _vp, _ll, _i, _i, _f, _vp, _vp, _vp, _vp]),
+    "nr_list_stats": (_i, [_vp, _ll, _i, _i, _vp, _ll, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "nr_pool_ranks_workspace": (_ll, [_ll, _ll, _i]),
     "nr_pool_ranks": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_topk_archive_workspace": (_ll, [_ll, _i, _ll, _i, _i, _i]),

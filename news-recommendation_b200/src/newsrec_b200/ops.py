@@ -751,6 +751,49 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     return idx, score
 
 
+LIST_STATS_MAX_KS = 8  # cut-offs per call (nr_list_stats)
+
+
+def list_stats(news, idx, ks, categories=None):
+    """Per-list similarity and category statistics in one launch (nr_list_stats): news (n, D) fp32, idx (R, k) int64 lists
+    of news rows (top_k_scores' output: the entries before the first -1 are the list), ks ascending distinct cut-offs in
+    [1, k] (at most 8).  For row r and cut-off K, with K' = min(K, the list's length):
+        pair_sum[r, c] = sum over the pairs i < j < K' of the cosine of news rows idx[r, i] and idx[r, j], in fp64
+        distinct[r, c] = the number of distinct categories[idx[r, j]], j < K'   (only with categories (n,) integer keys)
+    The cosine is nr_mmr_rerank's, within its e_sim of the exact one (include/newsrec_b200.h).  Returns (pair_sum (R, n_ks)
+    fp64, distinct (R, n_ks) int32 or None) on the device.  Raises NewsrecError on arguments the kernel refuses (before any
+    launch) and IndexError on a listed row outside [0, n) (reads the device flag: one synchronisation)."""
+    lib = load_library()
+    if news.dim() != 2 or idx.dim() != 2:
+        raise NewsrecError(f"list_stats: news {tuple(news.shape)} and idx {tuple(idx.shape)} must be (n, D) and (R, k)")
+    ks = list(ks)
+    if any(isinstance(x, bool) or not isinstance(x, numbers.Integral) or not -2 ** 31 <= x < 2 ** 31 for x in ks):
+        raise NewsrecError(f"list_stats: ks={ks!r} must be integers")
+    dev = require_cuda()
+    news = news.to(dev).float().contiguous()
+    idx = idx.to(dev).long().contiguous()
+    (n, D), (R, k) = news.shape, idx.shape
+    cat = None
+    if categories is not None:
+        categories = torch.as_tensor(categories)
+        if categories.dim() != 1 or categories.shape[0] != n or categories.dtype.is_floating_point or \
+                categories.dtype.is_complex or categories.dtype == torch.bool:
+            raise NewsrecError(f"list_stats: categories {tuple(categories.shape)} {categories.dtype} must be ({n},) integer keys")
+        if categories.dtype != torch.int32 and categories.numel() and \
+                (int(categories.min()) < -2 ** 31 or int(categories.max()) >= 2 ** 31):
+            raise NewsrecError("list_stats: a category key does not fit in int32")
+        cat = categories.to(device=dev, dtype=torch.int32).contiguous()
+    pair_sum = torch.empty((R, len(ks)), dtype=torch.float64, device=dev)
+    distinct = torch.empty((R, len(ks)), dtype=torch.int32, device=dev) if cat is not None else None
+    flag = torch.zeros(1, dtype=torch.int32, device=dev)
+    c_ks = (C.c_int * max(len(ks), 1))(*ks)
+    check(lib.nr_list_stats(_p(news), n, D, D, _p(idx), R, k, _p(cat), c_ks, len(ks), _p(pair_sum), _p(distinct), _p(flag),
+                            _stream()), "nr_list_stats")
+    if int(flag.item()):
+        raise IndexError("list_stats: a listed row is outside the news pool")
+    return pair_sum, distinct
+
+
 POOL_RANK_MAX_TARGETS = 32  # targets per kernel row (nr_pool_ranks)
 
 

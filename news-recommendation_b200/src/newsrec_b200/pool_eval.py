@@ -18,9 +18,16 @@ Exp1 are ranked under the dot product of user and news vectors; Hi-Fi Ark and DK
 their models' ``pool_user_vector`` and ``ops.pool_ranks(..., dnn=)`` (nr_pool_ranks_archive: the scores nr_topk_archive
 computes).  A model of those two families without ``pool_user_vector`` is refused.
 
+``evaluate_lists`` (``--lists``) evaluates the k-lists ``recommend`` writes instead, plain, capped (``max_per_category``) or
+MMR re-ranked (``mmr_lambda``), over the same impressions: where each click lands in its user's list (recall@K, nDCG@K,
+MRR) and how the lists look (intra-list similarity, distinct categories, catalog coverage, exposure Gini), the similarity
+statistics from one kernel (``ops.list_stats``, nr_list_stats).
+
     python -m newsrec_b200.pool_eval --directory data/val [--ks 5,10,20,50,100] [--keep-clicked]
                                      [--checkpoint PATH | --checkpoint-dir DIR] [--user2int data/train/user2int.tsv]
                                      [--chunk-impressions N] [--set KNOB=VALUE ...]
+                                     [--lists [--k 10] [--max-per-category M [--diversify-by {category,subcategory}]
+                                                        | --mmr-lambda X [--mmr-depth L]]]
 """
 from __future__ import annotations
 
@@ -31,8 +38,10 @@ import sys
 import numpy as np
 
 from . import NewsrecError
-from .evaluate import build_tables, new_flag, news_matrix, read_behaviors, _gather
-from .recommend import _Users, exclusion_csr, pool_operands, refuse_family
+from .evaluate import build_tables, new_flag, news_matrix, read_behaviors, read_news, _gather
+from .recommend import (DIVERSIFY_FIELDS, MAX_K, _Users, add_diversify_args, check_diversify_args, exclusion_csr, list_options,
+                        news_columns, pool_operands, refuse_family)
+from .recommend import check_request as check_list_request
 
 DEFAULT_KS = (5, 10, 20, 50, 100)
 DEFAULT_CHUNK = 65536
@@ -48,9 +57,14 @@ def check_request(model, directory, ks):
     for f in ("behaviors.tsv", "news_parsed.tsv"):
         if not os.path.isfile(os.path.join(directory, f)):
             raise FileNotFoundError(f"evaluate_pool: {os.path.join(directory, f)} not found")
+    require_labels("evaluate_pool", directory)
+
+
+def require_labels(who, directory):
+    """Raises NewsrecError when directory/behaviors.tsv has an impression without labels."""
     beh = read_behaviors(directory)
     if any("-" not in item for imp in beh["impressions"].tolist() for item in str(imp).split()):
-        raise NewsrecError(f"evaluate_pool: {directory}/behaviors.tsv has unlabelled impressions (a test split?): "
+        raise NewsrecError(f"{who}: {directory}/behaviors.tsv has unlabelled impressions (a test split?): "
                            "retrieval metrics need the clicks")
 
 
@@ -142,6 +156,149 @@ def evaluate_pool(model, directory, ks=DEFAULT_KS, *, exclude_clicked=True, max_
     return metrics(positions(rank, score, rows, offsets), offsets, tuple(int(k) for k in ks))
 
 
+# ---- the lists recommend writes ----
+LIST_MAX_KS = 8  # cut-offs of one evaluate_lists call (nr_list_stats)
+
+
+def list_ks(k, ks=None):
+    """The cut-offs of evaluate_lists, ascending and distinct: by default the DEFAULT_KS below k, then k.  Raises
+    NewsrecError on a K that is not an integer in [1, k] or on more than 8 distinct cut-offs."""
+    if ks is None:
+        return tuple(x for x in DEFAULT_KS if x < k) + (int(k),)
+    ks = tuple(ks)
+    if not ks or any(isinstance(x, bool) or not isinstance(x, (int, np.integer)) or not 1 <= x <= k for x in ks):
+        raise NewsrecError(f"evaluate_lists: ks={ks!r} must be integers in [1, k] = [1, {k}]")
+    ks = tuple(sorted(set(int(x) for x in ks)))
+    if len(ks) > LIST_MAX_KS:
+        raise NewsrecError(f"evaluate_lists: {len(ks)} distinct cut-offs; at most {LIST_MAX_KS}")
+    return ks
+
+
+def check_lists_request(model, directory, k, ks=None, max_per_category=None, diversify_by="category", mmr_lambda=None,
+                        mmr_depth=None):
+    """Everything evaluate_lists() refuses, before any device work: every refusal of recommend.check_request (k, the cap, the
+    field, the family, MMR, MMR together with a cap, missing files), a bad ks (list_ks) and an unlabelled split.  Returns the
+    cut-offs."""
+    check_list_request(model, directory, k, max_per_category, diversify_by, mmr_lambda, mmr_depth, who="evaluate_lists")
+    ks = list_ks(int(k), ks)
+    require_labels("evaluate_lists", directory)
+    return ks
+
+
+def list_lengths(lists):
+    """The number of entries before the first -1 of every row of lists (S, k)."""
+    dead = np.asarray(lists) < 0
+    return np.where(dead.any(1), dead.argmax(1), dead.shape[1]).astype(np.int64)
+
+
+def gini(x):
+    """Gini coefficient of the counts x (every item, zeros included): sum_i (2i - n - 1) x_(i) / (n sum x), x ascending, i
+    from 1; NaN when sum x = 0.  The numerator is an exact integer sum."""
+    x = np.sort(np.asarray(x, np.int64))
+    n, total = len(x), int(x.sum())
+    if total == 0:
+        return np.float64(np.nan)
+    w = 2 * np.arange(1, n + 1, dtype=np.int64) - n - 1
+    return np.float64(int(np.dot(w, x))) / (np.float64(n) * np.float64(total))
+
+
+def list_metrics(lists, rows, offsets, pair_sum, distinct, n_pool, ks, field=None):
+    """The dict evaluate_lists returns, from every counted impression's list and statistics at once:
+    lists (S, k) int64 news rows (the entries before the first -1 are the list), rows / offsets the positives (CSR over the
+    S impressions), pair_sum (S, len(ks)) fp64 and distinct (S, len(ks)) (or None) from ops.list_stats, n_pool the pool's
+    size, ks the ascending cut-offs, field the name of distinct's column."""
+    lists = np.asarray(lists, np.int64)
+    S, k = lists.shape
+    n_pos = np.diff(offsets)
+    seg = np.repeat(np.arange(S, dtype=np.int64), n_pos)
+    L = list_lengths(lists)
+    live = np.arange(k) < L[:, None]
+    match = (lists[seg] == np.asarray(rows, np.int64)[:, None]) & live[seg]
+    c = np.where(match.any(1), match.argmax(1), k)  # a positive outside the list sits at k: past every cut-off
+    out = metrics(c, offsets, ks)
+    del out["mrr"], out["impressions"]
+    first = np.full(S, k, np.int64)
+    np.minimum.at(first, seg, c)
+    out[f"mrr@{k}"] = np.float64(np.mean(np.where(first < k, 1.0 / (1.0 + first), 0.0))) if S else np.float64(np.nan)
+    for j, K in enumerate(ks):
+        Kp = np.minimum(L, K)
+        q = Kp >= 2
+        out[f"ils@{K}"] = np.float64(np.mean(pair_sum[q, j] / (Kp[q] * (Kp[q] - 1) / 2.0))) if q.any() else np.float64(np.nan)
+        if distinct is not None:
+            out[f"distinct_{field}@{K}"] = np.float64(np.mean(np.asarray(distinct, np.float64)[:, j])) if S else np.float64(np.nan)
+        exposure = np.bincount(lists[:, :K][live[:, :K]], minlength=n_pool)
+        out[f"coverage@{K}"] = np.float64(np.count_nonzero(exposure)) / np.float64(n_pool) if n_pool else np.float64(np.nan)
+        out[f"gini@{K}"] = gini(exposure)
+        out[f"list_length@{K}"] = np.float64(np.mean(Kp)) if S else np.float64(np.nan)
+    out["impressions"] = int(S)
+    return out
+
+
+def evaluate_lists(model, directory, k=10, ks=None, *, exclude_clicked=True, max_per_category=None, diversify_by="category",
+                   mmr_lambda=None, mmr_depth=None, max_count=sys.maxsize, user2int_path="data/train/user2int.tsv",
+                   chunk_impressions=DEFAULT_CHUNK) -> dict:
+    """Evaluate the k-lists recommend() writes, with the same k, exclusions and cap or MMR knobs, over the impressions
+    evaluate_pool counts (at least one click; the first max_count - 1 rows; a positive listed twice counted once; the user
+    of an impression is its distinct history).  Each distinct user of a chunk gets its list once (ops.top_k_scores through
+    recommend.pool_operands) and its statistics once (ops.list_stats on the model's news vectors); both are gathered per
+    impression.  With c_p the 0-based position of positive p in the list (absent: a miss), each an fp64 mean over the
+    impressions:
+        recall@K, ndcg@K     evaluate_pool's formulas with these c_p;   mrr@k  1 / (1 + min_p c_p), 0 when none is listed;
+        ils@K                pair_sum / (K'(K' - 1) / 2) over the lists with K' = min(K, list length) >= 2 (NaN if none);
+        distinct_<field>@K   distinct diversify_by values among the first K' (only when news_parsed.tsv has the column);
+        coverage@K, gini@K   the share of pool news in some first-K list; the Gini coefficient of the per-news counts of
+                             first-K lists holding them, over all pool news (NaN when nothing is listed);
+        list_length@K        K';   impressions  the number of counted impressions.
+    With exclude_clicked a positive that is in the user's history can never be listed, so it counts as a miss here, while
+    evaluate_pool still ranks it.  Every mean is taken once, at the end, from the per-impression values, so the result does
+    not depend on chunk_impressions, bit for bit.  Refusals (check_lists_request) come before any device work; a non-finite
+    score raises ValueError, a history row outside the news table IndexError.  Runs under torch.no_grad() on the model as
+    given (call .eval() first)."""
+    import torch
+    from .ops import list_stats, top_k_scores
+    ks = check_lists_request(model, directory, k, ks, max_per_category, diversify_by, mmr_lambda, mmr_depth)
+    k = int(k)
+    if chunk_impressions < 1:
+        raise ValueError(f"evaluate_lists: chunk_impressions={chunk_impressions}")
+    with torch.no_grad():
+        news_index, matrix = news_matrix(model, directory)
+        pad = news_index["PADDED_NEWS"]
+        t = build_tables(directory, news_index, model.config.num_clicked_news_a_user, max_count, user2int_path)
+        if (t.labels > 1).any():
+            raise ValueError("evaluate_lists: a label other than 0 or 1")
+        imp, rows, offsets = positives(t.cand, t.labels, t.seg_offsets)
+        pool = matrix[:pad]
+        opts = list_options("evaluate_lists", directory, matrix.device, max_per_category, diversify_by, mmr_lambda, mmr_depth)
+        field = diversify_by if diversify_by in news_columns(directory) else None
+        keys = None
+        if field is not None:  # distinct counts only need equal keys to stay equal: any key width fits
+            raw = read_news(directory, [field])[1][field]
+            keys = torch.from_numpy(np.unique(raw, return_inverse=True)[1].reshape(-1).astype(np.int32)).to(matrix.device)
+        flag = new_flag(matrix.device)
+        S = len(imp)
+        lists = np.full((S, k), -1, np.int64)
+        pair_sum = np.zeros((S, len(ks)), np.float64)
+        distinct = np.zeros((S, len(ks)), np.int64) if field is not None else None
+        for a in range(0, S, chunk_impressions):
+            b = min(S, a + chunk_impressions)
+            who, inv = np.unique(t.seg_user[imp[a:b]], return_inverse=True)
+            inv = inv.reshape(-1)
+            users, dnn = pool_operands(model, _Users(t.user[who], t.history[who], t.history_length[who]), matrix, flag)
+            excl = None, None
+            if exclude_clicked:
+                xr, xo = exclusion_csr(t.history[who], pad)
+                excl = torch.from_numpy(xr), torch.from_numpy(xo)
+            idx, _ = top_k_scores(users, pool, k, *excl, dnn=dnn, **opts)  # reads its flags: synchronises
+            ps, dc = list_stats(pool, idx, ks, categories=keys)
+            if int(flag.item()):
+                raise IndexError("evaluate_lists: a history row is outside the news table")
+            lists[a:b] = idx.cpu().numpy()[inv]
+            pair_sum[a:b] = ps.cpu().numpy()[inv]
+            if distinct is not None:
+                distinct[a:b] = dc.cpu().numpy()[inv]
+    return list_metrics(lists, rows, offsets, pair_sum, distinct, pad, ks, field)
+
+
 def parse_ks(text):
     ks = []
     for x in text.split(","):
@@ -161,7 +318,9 @@ def parse_args(argv=None):
                                  epilog="Every family is served: NRMS, NAML, LSTUR, TANR and Exp1 by the dot product of user and "
                                         "news vectors, Hi-Fi Ark and DKN by their DNN click predictor.")
     ap.add_argument("--directory", default="./data/val", help="labelled split: news_parsed.tsv (the pool) and behaviors.tsv")
-    ap.add_argument("--ks", default=",".join(map(str, DEFAULT_KS)), help="comma-separated cut-offs of recall@K and nDCG@K")
+    ap.add_argument("--ks", default=None,
+                    help="comma-separated cut-offs of recall@K and nDCG@K (default 5,10,20,50,100; with --lists those below "
+                         "--k, then --k)")
     g = ap.add_mutually_exclusive_group()
     g.add_argument("--checkpoint", help="a checkpoint file (a dict with model_state_dict, as the trainer saves)")
     g.add_argument("--checkpoint-dir", help="load its latest ckpt-<n>.pth (default: ./checkpoint/<MODEL_NAME>)")
@@ -170,13 +329,38 @@ def parse_args(argv=None):
     ap.add_argument("--chunk-impressions", type=int, default=DEFAULT_CHUNK, help="impressions ranked per device pass")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
                     help="override a knob of the selected <MODEL_NAME>Config (repeatable)")
+    ap.add_argument("--lists", action="store_true",
+                    help="evaluate the k-lists recommend writes (accuracy and diversity) instead of full-pool ranks")
+    ap.add_argument("--k", type=int, default=None, help=f"with --lists: news per list, 1 .. {MAX_K} (default 10)")
+    add_diversify_args(ap, None)
     args = ap.parse_args(argv)
+    if not args.lists:
+        for name in ("k", "max_per_category", "diversify_by", "mmr_lambda", "mmr_depth"):
+            if getattr(args, name) is not None:
+                ap.error(f"--{name.replace('_', '-')} needs --lists")
     try:
-        args.ks = parse_ks(args.ks)
+        if args.ks is not None:
+            args.ks = parse_ks(args.ks)
+        elif not args.lists:
+            args.ks = DEFAULT_KS
     except ValueError as e:
         ap.error(str(e))
     if args.chunk_impressions < 1:
         ap.error("--chunk-impressions must be at least 1")
+    if args.lists:
+        if args.k is None:
+            args.k = 10
+        if not 1 <= args.k <= MAX_K:
+            ap.error(f"--k must be in [1, {MAX_K}]")
+        check_diversify_args(ap, args)
+        if args.diversify_by is None:
+            args.diversify_by = DIVERSIFY_FIELDS[0]
+        if args.ks is not None and max(args.ks) > args.k:
+            ap.error(f"--ks: {max(args.ks)} is above --k {args.k}")
+        try:
+            args.ks = list_ks(args.k, args.ks)
+        except NewsrecError as e:
+            ap.error(str(e))
     return args
 
 
@@ -184,8 +368,14 @@ def main(argv=None):
     from .predict import load_model
     args = parse_args(argv)
     name, path, model = load_model(args.checkpoint, args.checkpoint_dir, args.set)
-    out = evaluate_pool(model, args.directory, args.ks, exclude_clicked=not args.keep_clicked, user2int_path=args.user2int,
-                        chunk_impressions=args.chunk_impressions)
+    if args.lists:
+        out = evaluate_lists(model, args.directory, args.k, args.ks, exclude_clicked=not args.keep_clicked,
+                             max_per_category=args.max_per_category, diversify_by=args.diversify_by,
+                             mmr_lambda=args.mmr_lambda, mmr_depth=args.mmr_depth, user2int_path=args.user2int,
+                             chunk_impressions=args.chunk_impressions)
+    else:
+        out = evaluate_pool(model, args.directory, args.ks, exclude_clicked=not args.keep_clicked, user2int_path=args.user2int,
+                            chunk_impressions=args.chunk_impressions)
     print(json.dumps({"model": name, "checkpoint": path, **out}))
     return 0
 

@@ -60,34 +60,50 @@ _REFUSED = {
 }
 
 
-def check_request(model, directory, k, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None):
+def check_request(model, directory, k, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None,
+                  who="recommend"):
     """Everything recommend() refuses, checked before any device work: k outside [1, 128], a cap that is not an integer >= 1,
     a diversify_by other than "category" / "subcategory", a family whose click predictor is not a dot product, an MMR
     request ops.mmr_request refuses or one together with a cap, a split without behaviors.tsv or news_parsed.tsv, and (with
-    a cap) a news_parsed.tsv without the diversify_by column."""
+    a cap) a news_parsed.tsv without the diversify_by column.  Messages start with who."""
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= MAX_K:
-        raise NewsrecError(f"recommend: k={k!r} must be an integer in [1, {MAX_K}]")
+        raise NewsrecError(f"{who}: k={k!r} must be an integer in [1, {MAX_K}]")
     if max_per_category is not None and (isinstance(max_per_category, bool) or
                                          not isinstance(max_per_category, (int, np.integer)) or max_per_category < 1):
-        raise NewsrecError(f"recommend: max_per_category={max_per_category!r} must be an integer >= 1")
+        raise NewsrecError(f"{who}: max_per_category={max_per_category!r} must be an integer >= 1")
     if diversify_by not in DIVERSIFY_FIELDS:
-        raise NewsrecError(f"recommend: diversify_by={diversify_by!r} must be one of {DIVERSIFY_FIELDS}")
-    refuse_family("recommend", model)
+        raise NewsrecError(f"{who}: diversify_by={diversify_by!r} must be one of {DIVERSIFY_FIELDS}")
+    refuse_family(who, model)
     from .ops import mmr_request
     try:
         mmr = mmr_request(int(k), mmr_lambda, mmr_depth)
     except NewsrecError as e:
-        raise NewsrecError(f"recommend: {e}") from None
+        raise NewsrecError(f"{who}: {e}") from None
     if mmr is not None and max_per_category is not None:
-        raise NewsrecError("recommend: mmr_lambda and max_per_category do not combine")
+        raise NewsrecError(f"{who}: mmr_lambda and max_per_category do not combine")
     for f in ("behaviors.tsv", "news_parsed.tsv"):
         if not os.path.isfile(os.path.join(directory, f)):
-            raise FileNotFoundError(f"recommend: {os.path.join(directory, f)} not found")
-    if max_per_category is not None:
-        with open(os.path.join(directory, "news_parsed.tsv")) as f:
-            header = f.readline().rstrip("\r\n").split("\t")
-        if diversify_by not in header:
-            raise NewsrecError(f"recommend: {os.path.join(directory, 'news_parsed.tsv')} has no {diversify_by} column")
+            raise FileNotFoundError(f"{who}: {os.path.join(directory, f)} not found")
+    if max_per_category is not None and diversify_by not in news_columns(directory):
+        raise NewsrecError(f"{who}: {os.path.join(directory, 'news_parsed.tsv')} has no {diversify_by} column")
+
+
+def news_columns(directory):
+    """The column names of directory/news_parsed.tsv."""
+    with open(os.path.join(directory, "news_parsed.tsv")) as f:
+        return f.readline().rstrip("\r\n").split("\t")
+
+
+def list_options(who, directory, device, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None):
+    """The keyword arguments of ops.top_k_scores that make recommend's lists: {} for the plain lists, the MMR knobs, or the
+    category cap with the diversify_by column of news_parsed.tsv (in the matrix's row order) as int32 keys on device."""
+    import torch
+    if max_per_category is None:
+        return {} if mmr_lambda is None else dict(mmr_lambda=mmr_lambda, mmr_depth=mmr_depth)
+    keys = read_news(directory, [diversify_by])[1][diversify_by]
+    if len(keys) and (keys.min() < -2 ** 31 or keys.max() >= 2 ** 31):
+        raise NewsrecError(f"{who}: a {diversify_by} id does not fit in int32")
+    return dict(categories=torch.from_numpy(keys.astype(np.int32)).to(device), max_per_category=int(max_per_category))
 
 
 def refuse_family(who, model):
@@ -156,13 +172,7 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
         user_ids = distinct_histories(beh)["user"].tolist()
         user, history, length, _ = user_tables(beh, news_index, model.config.num_clicked_news_a_user, user2int_path)
         pool = matrix[:pad]
-        cap = {} if mmr_lambda is None else dict(mmr_lambda=mmr_lambda, mmr_depth=mmr_depth)
-        if max_per_category is not None:
-            keys = read_news(directory, [diversify_by])[1][diversify_by]
-            if len(keys) and (keys.min() < -2 ** 31 or keys.max() >= 2 ** 31):
-                raise NewsrecError(f"recommend: a {diversify_by} id does not fit in int32")
-            cap = dict(categories=torch.from_numpy(keys.astype(np.int32)).to(matrix.device),
-                       max_per_category=int(max_per_category))
+        cap = list_options("recommend", directory, matrix.device, max_per_category, diversify_by, mmr_lambda, mmr_depth)
         U = len(user)
         flag = new_flag(matrix.device)
         tmp = f"{out_path}.partial"
@@ -198,16 +208,7 @@ def parse_args(argv=None):
     g.add_argument("--checkpoint", help="a checkpoint file (a dict with model_state_dict, as the trainer saves)")
     g.add_argument("--checkpoint-dir", help="load its latest ckpt-<n>.pth (default: ./checkpoint/<MODEL_NAME>)")
     ap.add_argument("--keep-clicked", action="store_true", help="let a user's clicked news be recommended back")
-    d = ap.add_mutually_exclusive_group()
-    d.add_argument("--max-per-category", type=int, default=None, metavar="M",
-                   help="at most M news of one category (see --diversify-by) per line")
-    d.add_argument("--mmr-lambda", type=float, default=None, metavar="X",
-                   help="re-rank each user's shortlist by maximal marginal relevance: X in [0, 1] weighs the click score "
-                        "against similarity to the news already listed (1: the plain lines)")
-    ap.add_argument("--diversify-by", choices=DIVERSIFY_FIELDS, default="category",
-                    help="the news_parsed.tsv column --max-per-category caps")
-    ap.add_argument("--mmr-depth", type=int, default=None, metavar="L",
-                    help=f"shortlist length --mmr-lambda re-ranks, k .. {MAX_K} (default min({MAX_K}, 4k))")
+    add_diversify_args(ap, "category")
     ap.add_argument("--user2int", default="./data/train/user2int.tsv")
     ap.add_argument("--chunk-users", type=int, default=DEFAULT_CHUNK, help="users scored per device pass")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
@@ -217,6 +218,27 @@ def parse_args(argv=None):
         ap.error(f"--k must be in [1, {MAX_K}]")
     if args.chunk_users < 1:
         ap.error("--chunk-users must be at least 1")
+    check_diversify_args(ap, args)
+    return args
+
+
+def add_diversify_args(ap, diversify_by_default):
+    """The list knobs of the command line, shared with pool_eval --lists: --max-per-category | --mmr-lambda, --diversify-by
+    and --mmr-depth."""
+    d = ap.add_mutually_exclusive_group()
+    d.add_argument("--max-per-category", type=int, default=None, metavar="M",
+                   help="at most M news of one category (see --diversify-by) per line")
+    d.add_argument("--mmr-lambda", type=float, default=None, metavar="X",
+                   help="re-rank each user's shortlist by maximal marginal relevance: X in [0, 1] weighs the click score "
+                        "against similarity to the news already listed (1: the plain lines)")
+    ap.add_argument("--diversify-by", choices=DIVERSIFY_FIELDS, default=diversify_by_default,
+                    help="the news_parsed.tsv column --max-per-category caps")
+    ap.add_argument("--mmr-depth", type=int, default=None, metavar="L",
+                    help=f"shortlist length --mmr-lambda re-ranks, k .. {MAX_K} (default min({MAX_K}, 4k))")
+
+
+def check_diversify_args(ap, args):
+    """argparse errors for the knobs of add_diversify_args, given args.k."""
     if args.max_per_category is not None and args.max_per_category < 1:
         ap.error("--max-per-category must be at least 1")
     if args.mmr_lambda is not None and not 0.0 <= args.mmr_lambda <= 1.0:
@@ -226,7 +248,6 @@ def parse_args(argv=None):
             ap.error("--mmr-depth needs --mmr-lambda")
         if not args.k <= args.mmr_depth <= MAX_K:
             ap.error(f"--mmr-depth must be in [--k, {MAX_K}]")
-    return args
 
 
 def main(argv=None):
