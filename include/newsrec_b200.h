@@ -287,6 +287,21 @@ int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, cons
                        long long* idx, float* score, int* bad_row_flag, int* bad_score_flag, void* workspace,
                        long long workspace_bytes, void* stream);
 
+/* nr_topk_dot (categories null) or nr_topk_dot_capped (categories non-null, max_per_category >= 1) over a news range per
+ * user (recommendation from the news live at each request's time).  row_lo / row_hi are device int64 [n_users], both
+ * non-null: news row n is a candidate of user u iff row_lo[u] <= n < row_hi[u].  The outputs equal, bit for bit, those of the
+ * unranged call with the rows outside [row_lo[u], row_hi[u]) added to u's exclusions (the same scores, order, caps,
+ * padding and determinism).  A range with row_lo[u] < 0, row_hi[u] > n_news or row_lo[u] > row_hi[u] sets *bad_row_flag
+ * and gives that user an empty list (-1 / -inf); the other users are unaffected.  A non-finite score of a pair inside its
+ * user's range sets *bad_score_flag.  Each block of 64 users streams only the 64-row news tiles its users' ranges touch, so
+ * the work follows the ranges' spans: sort users by their ranges to keep a block's ranges close.  Every limit of
+ * nr_topk_dot (nr_topk_dot_capped's with categories) and a null row_lo / row_hi are refused (-1) before the first launch.
+ * workspace: nr_topk_dot_workspace(...) bytes (the same layout). */
+int nr_topk_dot_ranged(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D,
+                       int k, const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+                       const long long* row_lo, const long long* row_hi, long long* idx, float* score, int* bad_row_flag,
+                       int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
+
 /* Maximal-marginal-relevance (MMR) re-ranking of nr_topk_dot's shortlists (content-diversified recommendation).  news fp32
  * [n_news][ld_news] (pitch >= D), the pool nr_topk_dot scored; shortlist_idx int64 / shortlist_score fp32 [n_users][depth],
  * nr_topk_dot's output at k = depth.  For user u:
@@ -362,6 +377,19 @@ int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const 
                   long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                   long long workspace_bytes, void* stream);
 
+/* nr_pool_ranks over a news range per query row: row_lo / row_hi device int64 [n_rows], both non-null, and row q counts only
+ * news rows n with row_lo[q] <= n < row_hi[q].  rank and score equal, bit for bit, those of nr_pool_ranks with the rows
+ * outside [row_lo[q], row_hi[q]) added to X_q.  A target outside its row's range is still ranked, against the row's eligible
+ * news (as a target in X_q is).  A range with row_lo[q] < 0, row_hi[q] > n_news or row_lo[q] > row_hi[q] sets
+ * *bad_row_flag and gives that row's targets rank -1 (score NaN); the other rows are unaffected.  Only the news tiles that
+ * hold a block's targets and that its rows' ranges touch are streamed.  Limits and workspace as nr_pool_ranks'; a null
+ * row_lo / row_hi is refused (-1) before the first launch. */
+int nr_pool_ranks_ranged(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news,
+                         int D, const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets,
+                         const long long* excl_rows, const long long* row_lo, const long long* row_hi, long long* rank, float* score,
+                         int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace, long long workspace_bytes,
+                         void* stream);
+
 /* Recommendation over a whole news pool under the archive DNN click score of Hi-Fi Ark and DKN (the scorer of
  * nr_archive_score_fwd).  archive fp32 [n_users][P][F] contiguous (DKN: P = 1, the user vector), news fp32 [n_news][F]
  * contiguous, W1 fp32 [hidden][2F] over [c; u], b1 [hidden], w2 [hidden], b2 [1], all device.  For user u and news c:
@@ -396,6 +424,15 @@ int nr_topk_archive(const float* archive, long long n_users, int P, const float*
                     const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
                     int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
 
+/* nr_topk_archive over a news range per user: row_lo / row_hi, the contract (the unranged outputs with the complement of
+ * each range added to the exclusions, bit for bit), bad ranges and flags as nr_topk_dot_ranged's.  Limits and workspace as
+ * nr_topk_archive's; a null row_lo / row_hi is refused (-1) before the first launch. */
+int nr_topk_archive_ranged(const float* archive, long long n_users, int P, const float* news, long long n_news, int F,
+                           const float* W1, const float* b1, int hidden, const float* w2, const float* b2, int k,
+                           const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+                           const long long* row_lo, const long long* row_hi, long long* idx, float* score, int* bad_row_flag,
+                           int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream);
+
 /* nr_pool_ranks under nr_topk_archive's scores (the same bits per pair): targets, exclusions, 32-target rows, flags and the
  * rank definition are nr_pool_ranks'; archive [n_rows][P][F] as nr_topk_archive's, one archive per query row.  The band
  * holds with nr_topk_archive's e(n).  Limits as nr_topk_archive's without k, with 1 <= n_news.  workspace:
@@ -406,6 +443,16 @@ int nr_pool_ranks_archive(const float* archive, long long n_rows, int P, const f
                           const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
                           float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                           long long workspace_bytes, void* stream);
+
+/* nr_pool_ranks_archive over a news range per query row: row_lo / row_hi, the contract, targets outside the range and bad
+ * ranges as nr_pool_ranks_ranged's.  Limits and workspace as nr_pool_ranks_archive's; a null row_lo / row_hi is refused
+ * (-1) before the first launch. */
+int nr_pool_ranks_archive_ranged(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F,
+                                 const float* W1, const float* b1, int hidden, const float* w2, const float* b2,
+                                 const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets,
+                                 const long long* excl_rows, const long long* row_lo, const long long* row_hi, long long* rank,
+                                 float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                                 long long workspace_bytes, void* stream);
 
 /* Host-side glue of the weight-gradient GEMMs (nr_gemm_tn with the ones column): ext is [rows][ld] fp32 whose columns
  * [0,D) hold dW and column D holds db.  Adds them into the parameters' own gradient storage (dW [rows][D] contiguous,

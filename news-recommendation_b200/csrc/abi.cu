@@ -221,8 +221,8 @@ int nr_topk_dot(const float* users, long long n_users, int ld_users, const float
                 const long long* excl_offsets, const long long* excl_rows, long long* idx, float* score, int* bad_row_flag,
                 int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream) {
     NR_REQUIRE(users && news && idx && score && bad_row_flag && bad_score_flag, "nr_topk_dot: null operand");
-    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, nullptr, 0, idx, score,
-                    bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, nullptr, 0, nullptr, nullptr,
+                    idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
 }
 int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D,
                        int k, const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
@@ -231,7 +231,16 @@ int nr_topk_dot_capped(const float* users, long long n_users, int ld_users, cons
     NR_REQUIRE(users && news && categories && idx && score && bad_row_flag && bad_score_flag, "nr_topk_dot_capped: null operand");
     NR_REQUIRE(max_per_category >= 1, "nr_topk_dot_capped: max_per_category=%d below 1", max_per_category);
     return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, categories, max_per_category,
-                    idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+                    nullptr, nullptr, idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+}
+int nr_topk_dot_ranged(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D,
+                       int k, const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+                       const long long* row_lo, const long long* row_hi, long long* idx, float* score, int* bad_row_flag,
+                       int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream) {
+    NR_REQUIRE(users && news && row_lo && row_hi && idx && score && bad_row_flag && bad_score_flag, "nr_topk_dot_ranged: null operand");
+    NR_REQUIRE(categories == nullptr || max_per_category >= 1, "nr_topk_dot_ranged: max_per_category=%d below 1", max_per_category);
+    return topk_dot(users, n_users, ld_users, news, n_news, ld_news, D, k, excl_offsets, excl_rows, categories, max_per_category,
+                    row_lo, row_hi, idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
 }
 int nr_mmr_rerank(const float* news, long long n_news, int ld_news, int D, const long long* shortlist_idx, const float* shortlist_score,
                   long long n_users, int depth, int k, float lambda, long long* idx, float* score, int* bad_row_flag, void* stream) {
@@ -252,8 +261,19 @@ int nr_pool_ranks(const float* queries, long long n_rows, int ld_queries, const 
                   long long workspace_bytes, void* stream) {
     NR_REQUIRE(queries && news && tgt_offsets && tgt_rows && rank && score && bad_row_flag && bad_score_flag && target_flag,
                "nr_pool_ranks: null operand");
-    return pool_ranks(queries, n_rows, ld_queries, news, n_news, ld_news, D, tgt_offsets, tgt_rows, excl_offsets, excl_rows, rank,
-                      score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes, as_stream(stream));
+    return pool_ranks(queries, n_rows, ld_queries, news, n_news, ld_news, D, tgt_offsets, tgt_rows, excl_offsets, excl_rows, nullptr,
+                      nullptr, rank, score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes, as_stream(stream));
+}
+int nr_pool_ranks_ranged(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news,
+                         int D, const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets,
+                         const long long* excl_rows, const long long* row_lo, const long long* row_hi, long long* rank, float* score,
+                         int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace, long long workspace_bytes,
+                         void* stream) {
+    NR_REQUIRE(queries && news && tgt_offsets && tgt_rows && row_lo && row_hi && rank && score && bad_row_flag && bad_score_flag &&
+                   target_flag,
+               "nr_pool_ranks_ranged: null operand");
+    return pool_ranks(queries, n_rows, ld_queries, news, n_news, ld_news, D, tgt_offsets, tgt_rows, excl_offsets, excl_rows, row_lo,
+                      row_hi, rank, score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes, as_stream(stream));
 }
 long long nr_topk_archive_workspace(long long n_users, int P, long long n_news, int F, int hidden, int k) {
     return topk_archive_workspace(n_users, P, n_news, F, hidden, k);
@@ -265,7 +285,19 @@ int nr_topk_archive(const float* archive, long long n_users, int P, const float*
     NR_REQUIRE(archive && news && W1 && b1 && w2 && b2 && idx && score && bad_row_flag && bad_score_flag,
                "nr_topk_archive: null operand");
     return topk_archive(archive, n_users, P, news, n_news, F, W1, b1, hidden, w2, b2, k, excl_offsets, excl_rows, categories,
-                        max_per_category, idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes, as_stream(stream));
+                        max_per_category, nullptr, nullptr, idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes,
+                        as_stream(stream));
+}
+int nr_topk_archive_ranged(const float* archive, long long n_users, int P, const float* news, long long n_news, int F,
+                           const float* W1, const float* b1, int hidden, const float* w2, const float* b2, int k,
+                           const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+                           const long long* row_lo, const long long* row_hi, long long* idx, float* score, int* bad_row_flag,
+                           int* bad_score_flag, void* workspace, long long workspace_bytes, void* stream) {
+    NR_REQUIRE(archive && news && W1 && b1 && w2 && b2 && row_lo && row_hi && idx && score && bad_row_flag && bad_score_flag,
+               "nr_topk_archive_ranged: null operand");
+    return topk_archive(archive, n_users, P, news, n_news, F, W1, b1, hidden, w2, b2, k, excl_offsets, excl_rows, categories,
+                        max_per_category, row_lo, row_hi, idx, score, bad_row_flag, bad_score_flag, workspace, workspace_bytes,
+                        as_stream(stream));
 }
 long long nr_pool_ranks_archive_workspace(long long n_rows, int P, long long n_news, int F, int hidden) {
     return pool_ranks_archive_workspace(n_rows, P, n_news, F, hidden);
@@ -279,8 +311,21 @@ int nr_pool_ranks_archive(const float* archive, long long n_rows, int P, const f
                    bad_score_flag && target_flag,
                "nr_pool_ranks_archive: null operand");
     return pool_ranks_archive(archive, n_rows, P, news, n_news, F, W1, b1, hidden, w2, b2, tgt_offsets, tgt_rows, excl_offsets,
-                              excl_rows, rank, score, bad_row_flag, bad_score_flag, target_flag, workspace, workspace_bytes,
-                              as_stream(stream));
+                              excl_rows, nullptr, nullptr, rank, score, bad_row_flag, bad_score_flag, target_flag, workspace,
+                              workspace_bytes, as_stream(stream));
+}
+int nr_pool_ranks_archive_ranged(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F,
+                                 const float* W1, const float* b1, int hidden, const float* w2, const float* b2,
+                                 const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets,
+                                 const long long* excl_rows, const long long* row_lo, const long long* row_hi, long long* rank,
+                                 float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+                                 long long workspace_bytes, void* stream) {
+    NR_REQUIRE(archive && news && W1 && b1 && w2 && b2 && tgt_offsets && tgt_rows && row_lo && row_hi && rank && score &&
+                   bad_row_flag && bad_score_flag && target_flag,
+               "nr_pool_ranks_archive_ranged: null operand");
+    return pool_ranks_archive(archive, n_rows, P, news, n_news, F, W1, b1, hidden, w2, b2, tgt_offsets, tgt_rows, excl_offsets,
+                              excl_rows, row_lo, row_hi, rank, score, bad_row_flag, bad_score_flag, target_flag, workspace,
+                              workspace_bytes, as_stream(stream));
 }
 long long nr_prediction_line_offsets_workspace(long long n_seg) {
     NR_REQUIRE(n_seg >= 0, "nr_prediction_line_offsets_workspace: n_seg=%lld", n_seg);

@@ -274,29 +274,33 @@ int feed_gather(const FeedField* fields, int n_fields, const int* behaviors, int
 // candidates (include/newsrec_b200.h, nr_sample_negatives)
 int sample_negatives(const int* cand_rows, const unsigned char* labels, const long long* imp_offsets, long long n_imp, const long long* row_offsets,
                      int K, unsigned long long seed, long long epoch, int* behaviors, int H, cudaStream_t stream);
-// top-k of users . news over a whole pool, categories null, or at most max_per_category news of one category key per list
-// (topk.cu; include/newsrec_b200.h, nr_topk_dot and nr_topk_dot_capped)
+// top-k of users . news over a whole pool, categories null, or at most max_per_category news of one category key per list;
+// row_lo / row_hi null, or each user's news range (topk.cu; include/newsrec_b200.h, nr_topk_dot, nr_topk_dot_capped and
+// nr_topk_dot_ranged)
 long long topk_dot_workspace(long long n_users, long long n_news, int D, int k);
 int topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
-             const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category, long long* idx,
-             float* score, int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
-// ranks of target news among a whole pool under the same scores (topk.cu; include/newsrec_b200.h, nr_pool_ranks)
+             const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+             const long long* row_lo, const long long* row_hi, long long* idx, float* score, int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
+// ranks of target news among a whole pool under the same scores, row_lo / row_hi as topk_dot's (topk.cu;
+// include/newsrec_b200.h, nr_pool_ranks and nr_pool_ranks_ranged)
 long long pool_ranks_workspace(long long n_rows, long long n_news, int D);
 int pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
                const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
-               long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
+               const long long* row_lo, const long long* row_hi, long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                long long workspace_bytes, cudaStream_t stream);
-// top-k and ranks over a whole pool under the archive DNN scorer (topk.cu; include/newsrec_b200.h, nr_topk_archive and
-// nr_pool_ranks_archive)
+// top-k and ranks over a whole pool under the archive DNN scorer, row_lo / row_hi as topk_dot's (topk.cu;
+// include/newsrec_b200.h, nr_topk_archive, nr_pool_ranks_archive and their _ranged variants)
 long long topk_archive_workspace(long long n_users, int P, long long n_news, int F, int hidden, int k);
 int topk_archive(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
                  const float* b1, int hidden, const float* w2, const float* b2, int k, const long long* excl_offsets,
-                 const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
+                 const long long* excl_rows, const int* categories, int max_per_category, const long long* row_lo,
+                 const long long* row_hi, long long* idx, float* score,
                  int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream);
 long long pool_ranks_archive_workspace(long long n_rows, int P, long long n_news, int F, int hidden);
 int pool_ranks_archive(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F, const float* W1,
                        const float* b1, int hidden, const float* w2, const float* b2, const long long* tgt_offsets,
-                       const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
+                       const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
+                       const long long* row_lo, const long long* row_hi, long long* rank,
                        float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
                        long long workspace_bytes, cudaStream_t stream);
 // maximal-marginal-relevance re-ranking of nr_topk_dot's shortlists (topk.cu; include/newsrec_b200.h, nr_mmr_rerank)

@@ -45,6 +45,13 @@
 // List statistics (nr_list_stats): one block per list, the same live-row load, gather and Gram routines (load_live_rows,
 // gram_hilo) and the same cosine (gram_sim), so a pair's similarity is the bits nr_mmr_rerank uses; the fp64 pair sums and
 // the distinct-category counts are then a few hundred operations per list.
+//
+// Row ranges (the *_ranged entry points): query row q only sees news rows [row_lo[q], row_hi[q]).  Each CTA takes the union
+// of the tiles its rows' ranges touch, [min lo / 64, ceil(max hi / 64)), and divides that interval among the splits instead
+// of the pool (tile_interval, split_tiles); the epilogues drop a news outside its row's own range with one compare, where the
+// unranged calls drop rows past n_news (their range is [0, n_news)).  Tile t still covers rows [64t, 64t + 64), so every
+// pair's score is the bits of the unranged kernels.  The ranks kernels still run their targets' tiles first, wherever
+// they are.  Without ranges the interval is [0, tiles): one code path.
 #include <algorithm>
 #include <cmath>
 
@@ -159,10 +166,56 @@ struct Params {
     int* bad_score_flag;
     const int* cat;                 // capped instantiation: [n_news] category keys, at most cap news of one key per list
     int cap;
+    const long long* row_lo;        // [n_users] or null: user u sees news rows [row_lo[u], row_hi[u]) only
+    const long long* row_hi;
 };
 
 // a before b in the output order: higher score, then lower row
 __device__ __forceinline__ bool before(float sa, int ra, float sb, int rb) { return sa > sb || (sa == sb && ra < rb); }
+
+// The news rows [lo, hi) query row q may see: [0, n_news) without ranges; a range with lo < 0, hi > n_news or lo > hi sets
+// the flag, is empty and returns false.
+__device__ __forceinline__ bool row_range(const long long* row_lo, const long long* row_hi, long long q, int n_news,
+                                          int* bad_row_flag, int& lo, int& hi) {
+    lo = 0;
+    hi = n_news;
+    if (row_lo == nullptr) return true;
+    const long long a = row_lo[q], b = row_hi[q];
+    if (a < 0 || b > n_news || a > b) {
+        atomicOr(bad_row_flag, 1);
+        lo = hi = 0;
+        return false;
+    }
+    lo = static_cast<int>(a);
+    hi = static_cast<int>(b);
+    return true;
+}
+
+// Threads 0..63 (two whole warps), one query row each: the union of the tiles that the non-empty ranges of the rows with
+// `in` touch, per warp into iv[2 warp], iv[2 warp + 1].  The caller syncs before split_tiles reads them.
+__device__ __forceinline__ void tile_interval(int lo, int hi, bool in, int* iv) {
+    const bool live = in && lo < hi;
+    const int a = __reduce_min_sync(~0u, live ? lo / kNews : 0x7fffffff);
+    const int b = __reduce_max_sync(~0u, live ? (hi + kNews - 1) / kNews : 0);
+    if ((threadIdx.x & 31) == 0) {
+        iv[2 * (threadIdx.x >> 5)] = a;
+        iv[2 * (threadIdx.x >> 5) + 1] = b;
+    }
+}
+
+// The tiles [t0, t1) of split `split`: its share of the CTA's interval (tile_interval; [0, tiles) without ranges).  An empty
+// interval gives every split no tile.
+__device__ __forceinline__ void split_tiles(const int* iv, bool ranged, int tiles, int split, int splits, int& t0, int& t1) {
+    int a = 0, b = tiles;
+    if (ranged) {
+        a = min(iv[0], iv[2]);
+        b = max(iv[1], iv[3]);
+        if (a >= b) a = b = 0;
+    }
+    const long long n = b - a;
+    t0 = a + static_cast<int>(n * split / splits);
+    t1 = a + static_cast<int>(n * (split + 1) / splits);
+}
 
 // one warp sorts n (a power of two, <= 1024) (score, row) pairs in shared memory into output order (bitonic)
 __device__ void warp_sort(float* s, int* r, int n) {
@@ -273,19 +326,26 @@ __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_cons
     uint64_t* empty = full + kStages;                                   // [kStages]
     int* cnt = reinterpret_cast<int*>(empty + kStages);                 // [kUsers]
     float* thr = reinterpret_cast<float*>(cnt + kUsers);                // [kUsers]
+    int* iv = reinterpret_cast<int*>(thr + kUsers);                     // [4] tile_interval
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long u0 = static_cast<long long>(blockIdx.x) * kUsers;
     const int split = blockIdx.y;
-    const int t0 = static_cast<int>(static_cast<long long>(p.tiles) * split / p.splits);
-    const int t1 = static_cast<int>(static_cast<long long>(p.tiles) * (split + 1) / p.splits);
 
     Ring ring{sStage, full, empty};
     if (warp == 4 && lane == 0) ring_init(ring, &tmUh, &tmUl, &tmNh, &tmNl);
     if (threadIdx.x < kUsers) {
         cnt[threadIdx.x] = 0;
         thr[threadIdx.x] = -INFINITY;
+        if (p.row_lo != nullptr) {
+            const long long ug = u0 + threadIdx.x;
+            int lo = 0, hi = 0;
+            if (ug < p.n_users) row_range(p.row_lo, p.row_hi, ug, p.n_news, p.bad_row_flag, lo, hi);
+            tile_interval(lo, hi, ug < p.n_users, iv);
+        }
     }
     __syncthreads();
+    int t0, t1;
+    split_tiles(iv, p.row_lo != nullptr, p.tiles, split, p.splits, t0, t1);
 
     if (warp == 4) {
         // ===================== TMA producer: users and news boxes of every (tile, k-chunk) =====================
@@ -306,13 +366,15 @@ __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_cons
         if (bad) atomicOr(p.bad_row_flag, 1);
     }
     // fragment rows of this thread (consume_tile)
-    int urow[2];
+    int urow[2], nlo[2], nhi[2];  // the row's news range (row_range)
     long long ex0[2], ex1[2];
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
         urow[e] = 16 * warp + (lane >> 2) + 8 * e;
         const long long ug = u0 + urow[e];
         ex0[e] = ex1[e] = 0;
+        nlo[e] = nhi[e] = 0;
+        if (ug < p.n_users) row_range(p.row_lo, p.row_hi, ug, p.n_news, p.bad_row_flag, nlo[e], nhi[e]);
         if (p.excl_offsets != nullptr && ug < p.n_users) {
             ex0[e] = p.excl_offsets[ug];
             ex1[e] = p.excl_offsets[ug + 1];
@@ -335,7 +397,7 @@ __global__ void __launch_bounds__(kThreads, 1) topk_dot_kernel(const __grid_cons
                 for (int i = 0; i < 2; ++i) {
                     const int n = nrow0 + 8 * j + 2 * (lane & 3) + i;
                     const float s = acc[4 * j + 2 * e + i];
-                    if (n >= p.n_news) continue;
+                    if (n < nlo[e] || n >= nhi[e]) continue;
                     bad_score |= !(fabsf(s) <= 3.402823466e38f);
                     if (!(s > th)) continue;
                     bool excluded = false;
@@ -429,6 +491,8 @@ struct RankParams {
     const long long* tgt_rows;
     const long long* excl_offsets;  // [n_rows + 1] or null
     const long long* excl_rows;
+    const long long* row_lo;        // [n_rows] or null: row q counts news rows [row_lo[q], row_hi[q]) only
+    const long long* row_hi;
     long long* rank;                // [n_targets]
     float* score;
     int* part;                      // splits > 1: [n_rows][splits][kMaxTargets] counts by target slot; slot 0 = -1: bad row
@@ -457,11 +521,12 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_kernel(const __grid_co
     int* tm = reinterpret_cast<int*>(empty + kStages);                  // [kUsers] targets of the row, -1: bad row
     int* n_pro = tm + kUsers;
     int* qc = n_pro + 1;                                                // [2] queue length, by tile parity
+    int* rlo = qc + 2;                                                  // [kUsers] the row's news range (row_range)
+    int* rhi = rlo + kUsers;
+    int* iv = rhi + kUsers;                                             // [4] tile_interval
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long q0 = static_cast<long long>(blockIdx.x) * kUsers;
     const int split = blockIdx.y;
-    const int t0 = static_cast<int>(static_cast<long long>(p.tiles) * split / p.splits);
-    const int t1 = static_cast<int>(static_cast<long long>(p.tiles) * (split + 1) / p.splits);
 
     Ring ring{sStage, full, empty};
     if (warp == 4 && lane == 0) ring_init(ring, &tmQh, &tmQl, &tmNh, &tmNl);
@@ -472,12 +537,15 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_kernel(const __grid_co
     if (threadIdx.x < kUsers) {
         const int r = threadIdx.x;
         const long long q = q0 + r;
-        int m = 0;
+        int m = 0, lo = 0, hi = 0;
         if (q < p.n_rows) {
+            const bool ok = row_range(p.row_lo, p.row_hi, q, p.n_news, p.bad_row_flag, lo, hi);
             const long long a = p.tgt_offsets[q], cnt = p.tgt_offsets[q + 1] - a;
             if (cnt > kMaxTargets) {
                 m = -1;
                 atomicOr(p.target_flag, 1);
+            } else if (!ok) {
+                m = -1;
             } else {
                 m = static_cast<int>(cnt);
                 for (int j = 0; j < m; ++j) {
@@ -494,6 +562,9 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_kernel(const __grid_co
             }
         }
         tm[r] = m;
+        rlo[r] = lo;
+        rhi[r] = hi;
+        if (p.row_lo != nullptr) tile_interval(lo, hi, m > 0, iv);
     }
     if (p.excl_offsets != nullptr) {
         bool bad = false;
@@ -531,6 +602,8 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_kernel(const __grid_co
     }
     __syncthreads();
     const int npro = *n_pro;
+    int t0, t1;
+    split_tiles(iv, p.row_lo != nullptr, p.tiles, split, p.splits, t0, t1);
 
     if (warp == 4) {
         // ===================== TMA producer: the target tiles, then the split's tiles =====================
@@ -593,10 +666,12 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_kernel(const __grid_co
     asm volatile("bar.sync 1, 128;" ::: "memory");
     // thresholds: a score counts when it comes before the row's last target; before its first, it beats all of them
     float hi_s[2], lo_s[2];
-    int hi_r[2], lo_r[2], cnt0[2] = {0, 0};
+    int hi_r[2], lo_r[2], cnt0[2] = {0, 0}, nlo[2], nhi[2];
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
         const int r = urow[e], m = tm[r];
+        nlo[e] = rlo[r];
+        nhi[e] = rhi[r];
         hi_s[e] = lo_s[e] = INFINITY;  // nothing comes before (+inf, -1)
         hi_r[e] = lo_r[e] = -1;
         if (m > 0) {
@@ -620,7 +695,7 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_kernel(const __grid_co
                 for (int i = 0; i < 2; ++i) {
                     const int col = 8 * j + 2 * (lane & 3) + i, n = nrow0 + col;
                     const float s = acc[4 * j + 2 * e + i];
-                    if (n >= p.n_news) continue;
+                    if (n < nlo[e] || n >= nhi[e]) continue;
                     bad_score |= !(fabsf(s) <= 3.402823466e38f);
                     if (!before(s, n, lo_s[e], lo_r[e])) continue;
                     if ((fw >> col) & 1ull) {  // maybe a target or an exclusion of the row: queued
@@ -1038,11 +1113,11 @@ struct ArchSmem {
         bytes = rest + rest_bytes;
     }
 };
-__host__ __device__ constexpr int topk_archive_rest(int G) { return G * kCap * 8 + 2 * kStages * 8 + 2 * kUsers * 4; }
+__host__ __device__ constexpr int topk_archive_rest(int G) { return G * kCap * 8 + 2 * kStages * 8 + 4 * kUsers * 4 + 16; }
 __host__ __device__ constexpr int ranks_archive_rest(int G) {
     // hist and tiles hold kUsers * kMaxTargets entries: the tile sort needs a power of two
     return G * kFiltWords * 8 + 3 * G * kMaxTargets * 4 + 2 * kUsers * kMaxTargets * 4 + 3 * G * kNews * 4 + 2 * kStages * 8 +
-           3 * G * 4 + 16;
+           5 * G * 4 + 32;
 }
 
 // X or Y: out[r][j] = (sum_f W[j][f] src[r][f]) (+ b[j]) for j < hid, in f order, 0 for hid <= j < hp; one warp per row
@@ -1166,21 +1241,32 @@ __global__ void __launch_bounds__(kThreads, 1) topk_archive_kernel(const __grid_
     uint64_t* empty = full + kStages;                               // [kStages]
     int* cnt = reinterpret_cast<int*>(empty + kStages);             // [G]
     float* thr = reinterpret_cast<float*>(cnt + kUsers);            // [G]
+    int* rlo = reinterpret_cast<int*>(thr + kUsers);                // [G] the user's news range (row_range)
+    int* rhi = rlo + kUsers;
+    int* iv = rhi + kUsers;                                         // [4] tile_interval
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long u0 = static_cast<long long>(blockIdx.x) * G;
     const int here = static_cast<int>(min(static_cast<long long>(G), p.n_users - u0));
     const int split = blockIdx.y;
-    const int t0 = static_cast<int>(static_cast<long long>(p.tiles) * split / p.splits);
-    const int t1 = static_cast<int>(static_cast<long long>(p.tiles) * (split + 1) / p.splits);
 
     Ring ring{base, full, empty};
     if (o.P > 1 && warp == 4 && lane == 0) ring_init(ring, &tmAh, &tmAl, &tmNh, &tmNl);
-    if (threadIdx.x < G) {
-        cnt[threadIdx.x] = 0;
-        thr[threadIdx.x] = -INFINITY;
+    if (threadIdx.x < kUsers) {
+        const int g = threadIdx.x;
+        int lo = 0, hi = 0;
+        if (g < here) row_range(p.row_lo, p.row_hi, u0 + g, p.n_news, p.bad_row_flag, lo, hi);
+        if (g < G) {
+            cnt[g] = 0;
+            thr[g] = -INFINITY;
+            rlo[g] = lo;
+            rhi[g] = hi;
+        }
+        if (p.row_lo != nullptr) tile_interval(lo, hi, g < here, iv);
     }
     arch_stage_users(o, u0, here, Ys, w2s);
     __syncthreads();
+    int t0, t1;
+    split_tiles(iv, p.row_lo != nullptr, p.tiles, split, p.splits, t0, t1);
 
     if (warp == 4) {
         // ===================== TMA producer (P > 1): archive rows [u0 P, u0 P + 64) and the news of every tile =====================
@@ -1205,7 +1291,7 @@ __global__ void __launch_bounds__(kThreads, 1) topk_archive_kernel(const __grid_
         // ---- survivors of the tile into the candidate buffers ----
         arch_tile_pairs(o, T, Xs, Ys, w2s, Ws, here, [&](int g, int c, float s) {
             const int n = t * kNews + c;
-            if (n >= p.n_news) return;
+            if (n < rlo[g] || n >= rhi[g]) return;
             bad_score |= !(fabsf(s) <= 3.402823466e38f);
             if (!(s > thr[g])) return;
             if (p.excl_offsets != nullptr) {
@@ -1275,12 +1361,13 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_archive_kernel(const _
     int* tm = lo_r + G;                                             // [G] targets of the row, -1: bad row
     int* n_pro = tm + G;
     int* qc = n_pro + 1;                                            // [2] queue length, by tile parity
+    int* rlo = qc + 2;                                              // [G] the row's news range (row_range)
+    int* rhi = rlo + G;
+    int* iv = rhi + G;                                              // [4] tile_interval
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long q0 = static_cast<long long>(blockIdx.x) * G;
     const int here = static_cast<int>(min(static_cast<long long>(G), p.n_rows - q0));
     const int split = blockIdx.y;
-    const int t0 = static_cast<int>(static_cast<long long>(p.tiles) * split / p.splits);
-    const int t1 = static_cast<int>(static_cast<long long>(p.tiles) * (split + 1) / p.splits);
 
     Ring ring{base, full, empty};
     if (o.P > 1 && warp == 4 && lane == 0) ring_init(ring, &tmAh, &tmAl, &tmNh, &tmNl);
@@ -1289,14 +1376,17 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_archive_kernel(const _
     arch_stage_users(o, q0, here, Ys, w2s);
     __syncthreads();
     // ---- the rows' targets and the membership filter of targets and exclusions ----
+    int m = 0, lo = 0, hi = 0;
     if (threadIdx.x < G) {
         const int r = threadIdx.x;
-        int m = 0;
         if (r < here) {
             const long long q = q0 + r, a = p.tgt_offsets[q], cnt = p.tgt_offsets[q + 1] - a;
+            const bool ok = row_range(p.row_lo, p.row_hi, q, p.n_news, p.bad_row_flag, lo, hi);
             if (cnt > kMaxTargets) {
                 m = -1;
                 atomicOr(p.target_flag, 1);
+            } else if (!ok) {
+                m = -1;
             } else {
                 m = static_cast<int>(cnt);
                 for (int j = 0; j < m; ++j) {
@@ -1313,7 +1403,10 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_archive_kernel(const _
             }
         }
         tm[r] = m;
+        rlo[r] = lo;
+        rhi[r] = hi;
     }
+    if (p.row_lo != nullptr && threadIdx.x < kUsers) tile_interval(lo, hi, m > 0, iv);
     if (p.excl_offsets != nullptr) {
         bool bad = false;
         for (int r = 0; r < here; ++r)
@@ -1350,6 +1443,8 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_archive_kernel(const _
     }
     __syncthreads();
     const int npro = *n_pro;
+    int t0, t1;
+    split_tiles(iv, p.row_lo != nullptr, p.tiles, split, p.splits, t0, t1);
 
     if (warp == 4) {
         // ===================== TMA producer (P > 1): the target tiles, then the split's tiles =====================
@@ -1410,7 +1505,7 @@ __global__ void __launch_bounds__(kThreads, 1) pool_ranks_archive_kernel(const _
         asm volatile("bar.sync 1, 128;" ::: "memory");
         arch_tile_pairs(o, T, Xs, Ys, w2s, Ws, here, [&](int g, int c, float s) {
             const int n = t * kNews + c;
-            if (lo_r[g] < 0 || n >= p.n_news) return;  // no target, or a bad row
+            if (lo_r[g] < 0 || n < rlo[g] || n >= rhi[g]) return;  // no target, a bad row, or outside the row's range
             bad_score |= !(fabsf(s) <= 3.402823466e38f);
             if (!before(s, n, lo_s[g], lo_r[g])) return;
             if ((filt[g * kFiltWords + (t & (kFiltWords - 1))] >> c) & 1ull) {  // maybe a target or an exclusion of the row: queued
@@ -1556,12 +1651,14 @@ static int topk_launch(const CUtensorMap (&tm)[4], const topk::Params& p, cudaSt
 }
 
 int topk_dot(const float* users, long long n_users, int ld_users, const float* news, long long n_news, int ld_news, int D, int k,
-             const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category, long long* idx,
-             float* score, int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+             const long long* excl_offsets, const long long* excl_rows, const int* categories, int max_per_category,
+             const long long* row_lo, const long long* row_hi, long long* idx, float* score, int* bad_row_flag,
+             int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
     using namespace topk;
     NR_PROPAGATE(topk_check(n_users, n_news, D, k));
     NR_REQUIRE(ld_users >= D && ld_news >= D, "nr_topk_dot: pitches ld_users=%d ld_news=%d below D=%d", ld_users, ld_news, D);
     NR_REQUIRE((excl_offsets == nullptr) == (excl_rows == nullptr), "nr_topk_dot: excl_offsets and excl_rows go together");
+    NR_REQUIRE((row_lo == nullptr) == (row_hi == nullptr), "nr_topk_dot: row_lo and row_hi go together");
     const int splits = topk_splits(n_users, n_news);
     TopkWorkspace ws(workspace, n_users, n_news, D, k, splits);
     NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
@@ -1586,6 +1683,8 @@ int topk_dot(const float* users, long long n_users, int ld_users, const float* n
     p.bad_score_flag = bad_score_flag;
     p.cat = categories;
     p.cap = max_per_category;
+    p.row_lo = row_lo;
+    p.row_hi = row_hi;
     return categories != nullptr ? topk_launch<true>(tm, p, stream) : topk_launch<false>(tm, p, stream);
 }
 
@@ -1612,12 +1711,13 @@ long long pool_ranks_workspace(long long n_rows, long long n_news, int D) {
 
 int pool_ranks(const float* queries, long long n_rows, int ld_queries, const float* news, long long n_news, int ld_news, int D,
                const long long* tgt_offsets, const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
-               long long* rank, float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
-               long long workspace_bytes, cudaStream_t stream) {
+               const long long* row_lo, const long long* row_hi, long long* rank, float* score, int* bad_row_flag,
+               int* bad_score_flag, int* target_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
     using namespace topk;
     NR_PROPAGATE(pool_ranks_check(n_rows, n_news, D));
     NR_REQUIRE(ld_queries >= D && ld_news >= D, "nr_pool_ranks: pitches ld_queries=%d ld_news=%d below D=%d", ld_queries, ld_news, D);
     NR_REQUIRE((excl_offsets == nullptr) == (excl_rows == nullptr), "nr_pool_ranks: excl_offsets and excl_rows go together");
+    NR_REQUIRE((row_lo == nullptr) == (row_hi == nullptr), "nr_pool_ranks: row_lo and row_hi go together");
     const int splits = topk_splits(n_rows, n_news);
     RankWorkspace ws(workspace, n_rows, n_news, D, splits);
     NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
@@ -1640,6 +1740,8 @@ int pool_ranks(const float* queries, long long n_rows, int ld_queries, const flo
     p.tgt_rows = tgt_rows;
     p.excl_offsets = excl_offsets;
     p.excl_rows = excl_rows;
+    p.row_lo = row_lo;
+    p.row_hi = row_hi;
     p.rank = rank;
     p.score = score;
     p.part = ws.part;
@@ -1851,12 +1953,14 @@ static int topk_archive_launch(const CUtensorMap (&tm)[4], const topk::Params& p
 
 int topk_archive(const float* archive, long long n_users, int P, const float* news, long long n_news, int F, const float* W1,
                  const float* b1, int hidden, const float* w2, const float* b2, int k, const long long* excl_offsets,
-                 const long long* excl_rows, const int* categories, int max_per_category, long long* idx, float* score,
-                 int* bad_row_flag, int* bad_score_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
+                 const long long* excl_rows, const int* categories, int max_per_category, const long long* row_lo,
+                 const long long* row_hi, long long* idx, float* score, int* bad_row_flag, int* bad_score_flag, void* workspace,
+                 long long workspace_bytes, cudaStream_t stream) {
     using namespace topk;
     NR_PROPAGATE(topk_archive_check(n_users, P, n_news, F, hidden, k));
     NR_REQUIRE((excl_offsets == nullptr) == (excl_rows == nullptr), "nr_topk_archive: excl_offsets and excl_rows go together");
     NR_REQUIRE(categories == nullptr || max_per_category >= 1, "nr_topk_archive: max_per_category=%d below 1", max_per_category);
+    NR_REQUIRE((row_lo == nullptr) == (row_hi == nullptr), "nr_topk_archive: row_lo and row_hi go together");
     const int splits = archive_splits(n_users, P, n_news);
     TopkArchiveWorkspace ws(workspace, n_users, P, n_news, F, hidden, k, splits);
     NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
@@ -1882,6 +1986,8 @@ int topk_archive(const float* archive, long long n_users, int P, const float* ne
     p.bad_score_flag = bad_score_flag;
     p.cat = categories;
     p.cap = max_per_category;
+    p.row_lo = row_lo;
+    p.row_hi = row_hi;
     return categories != nullptr ? topk_archive_launch<true>(tm, p, o, stream) : topk_archive_launch<false>(tm, p, o, stream);
 }
 
@@ -1901,12 +2007,13 @@ long long pool_ranks_archive_workspace(long long n_rows, int P, long long n_news
 
 int pool_ranks_archive(const float* archive, long long n_rows, int P, const float* news, long long n_news, int F, const float* W1,
                        const float* b1, int hidden, const float* w2, const float* b2, const long long* tgt_offsets,
-                       const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows, long long* rank,
-                       float* score, int* bad_row_flag, int* bad_score_flag, int* target_flag, void* workspace,
-                       long long workspace_bytes, cudaStream_t stream) {
+                       const long long* tgt_rows, const long long* excl_offsets, const long long* excl_rows,
+                       const long long* row_lo, const long long* row_hi, long long* rank, float* score, int* bad_row_flag,
+                       int* bad_score_flag, int* target_flag, void* workspace, long long workspace_bytes, cudaStream_t stream) {
     using namespace topk;
     NR_PROPAGATE(archive_check("nr_pool_ranks_archive", n_rows, P, n_news, 1, F, hidden));
     NR_REQUIRE((excl_offsets == nullptr) == (excl_rows == nullptr), "nr_pool_ranks_archive: excl_offsets and excl_rows go together");
+    NR_REQUIRE((row_lo == nullptr) == (row_hi == nullptr), "nr_pool_ranks_archive: row_lo and row_hi go together");
     const int splits = archive_splits(n_rows, P, n_news);
     RankArchiveWorkspace ws(workspace, n_rows, P, n_news, F, hidden, splits);
     NR_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0 && workspace_bytes >= ws.bytes(),
@@ -1930,6 +2037,8 @@ int pool_ranks_archive(const float* archive, long long n_rows, int P, const floa
     p.tgt_rows = tgt_rows;
     p.excl_offsets = excl_offsets;
     p.excl_rows = excl_rows;
+    p.row_lo = row_lo;
+    p.row_hi = row_hi;
     p.rank = rank;
     p.score = score;
     p.part = ws.part;

@@ -179,16 +179,24 @@ SIGNATURES = {
     "nr_topk_dot_workspace": (_ll, [_ll, _ll, _i, _i]),
     "nr_topk_dot": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_topk_dot_capped": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "nr_topk_dot_ranged": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll,
+                                _vp]),
     "nr_mmr_rerank": (_i, [_vp, _ll, _i, _i, _vp, _vp, _ll, _i, _i, _f, _vp, _vp, _vp, _vp]),
     "nr_list_stats": (_i, [_vp, _ll, _i, _i, _vp, _ll, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "nr_pool_ranks_workspace": (_ll, [_ll, _ll, _i]),
     "nr_pool_ranks": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "nr_pool_ranks_ranged": (_i, [_vp, _ll, _i, _vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                  _ll, _vp]),
     "nr_topk_archive_workspace": (_ll, [_ll, _i, _ll, _i, _i, _i]),
     "nr_topk_archive": (_i, [_vp, _ll, _i, _vp, _ll, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp,
                              _vp, _ll, _vp]),
+    "nr_topk_archive_ranged": (_i, [_vp, _ll, _i, _vp, _ll, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp,
+                                    _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_pool_ranks_archive_workspace": (_ll, [_ll, _i, _ll, _i, _i]),
     "nr_pool_ranks_archive": (_i, [_vp, _ll, _i, _vp, _ll, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                    _vp, _vp, _ll, _vp]),
+    "nr_pool_ranks_archive_ranged": (_i, [_vp, _ll, _i, _vp, _ll, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "nr_prediction_line_offsets_workspace": (_ll, [_ll]),
     "nr_prediction_line_offsets": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _ll, _vp]),
     "nr_prediction_text": (_i, [_vp, _vp, _vp, _ll, _vp, _vp, _vp]),

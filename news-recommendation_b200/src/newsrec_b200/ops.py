@@ -639,8 +639,22 @@ def _pool_dnn(who, users, news, dnn):
                                          for t, s in ((W1, (hidden, 2 * F)), (b1, (-1,)), (w2, (-1,)), (b2, (1,))))
 
 
+def _row_range(who, row_range, U, dev):
+    """(lo, hi) of a row_range argument as contiguous int64 device tensors of U entries each; raises NewsrecError on anything
+    else.  The values themselves are checked by the kernels (a bad range sets the bad-row flag)."""
+    if not isinstance(row_range, (tuple, list)) or len(row_range) != 2:
+        raise NewsrecError(f"{who}: row_range must be a (lo, hi) pair of tensors")
+    out = []
+    for t in row_range:
+        t = torch.as_tensor(t)
+        if t.dim() != 1 or t.shape[0] != U or t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise NewsrecError(f"{who}: row_range entries {tuple(t.shape)} {t.dtype} must be ({U},) integer tensors")
+        out.append(t.to(device=dev, dtype=torch.int64).contiguous())
+    return out
+
+
 def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categories=None, max_per_category=None,
-                 mmr_lambda=None, mmr_depth=None, dnn=None):
+                 mmr_lambda=None, mmr_depth=None, dnn=None, row_range=None):
     """The k best news of every user over the whole pool, one pass (nr_topk_dot): users (U, D) and news (n, D) fp32, scores
     users[u] . news[r] at fp32 level on the tensor cores (the bound is in include/newsrec_b200.h) without the U x n score
     matrix.  Optional exclusions in CSR form: user u never gets rows excl_rows[excl_offsets[u] .. excl_offsets[u + 1]).
@@ -662,7 +676,13 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     DNN click scores (nr_topk_archive): with dnn = the (W1, b1, w2, b2) of Hi-Fi Ark's or DKN's click predictor, users is
     (U, F) (one vector per user, P = 1) or (U, P, F) (an archive per user) and the score of user u and news c is
     b2 + w2 . relu(W1 [c; softmax_p(A_u c)^T A_u] + b1), fp32-accurate (the bound is in include/newsrec_b200.h).  The
-    exclusions, the category cap and MMR work as above."""
+    exclusions, the category cap and MMR work as above.
+
+    News ranges (nr_topk_dot_ranged, nr_topk_archive_ranged): with row_range = (lo, hi), two (U,) integer tensors, user u
+    only gets news rows lo[u] <= r < hi[u]: the answer is, bit for bit, the one with every row outside that range excluded,
+    and the kernels only stream the news tiles the ranges of a block of 64 users touch (sort users by their ranges to keep
+    them close).  Caps, MMR (on the ranged shortlist) and dnn= work as above.  A range outside [0, n] or with lo > hi raises
+    IndexError."""
     lib = load_library()
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 128:
         raise NewsrecError(f"top_k_scores: k={k!r} must be an integer in [1, 128]")
@@ -678,6 +698,9 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
         users, *dnn = _pool_dnn("top_k_scores", users, news, dnn)
     if (excl_rows is None) != (excl_offsets is None):
         raise NewsrecError("top_k_scores: excl_rows and excl_offsets go together")
+    lo = hi = None
+    if row_range is not None:
+        lo, hi = _row_range("top_k_scores", row_range, users.shape[0], require_cuda())
     capped = categories is not None or max_per_category is not None
     if capped:
         if categories is None or max_per_category is None:
@@ -722,15 +745,24 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
     score = torch.empty((U, kk), dtype=torch.float32, device=dev)
     flags = torch.zeros(2, dtype=torch.int32, device=dev)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    if dnn is not None:
-        cat = categories.to(device=dev, dtype=torch.int32).contiguous() if capped else None
+    cat = categories.to(device=dev, dtype=torch.int32).contiguous() if capped else None
+    if lo is not None and dnn is not None:
+        W1, b1, w2, b2 = dnn
+        check(lib.nr_topk_archive_ranged(_p(users), U, P, _p(news), n, D, _p(W1), _p(b1), hidden, _p(w2), _p(b2), kk,
+                                         _p(excl_offsets), _p(excl_rows), _p(cat), max_per_category if capped else 0, _p(lo),
+                                         _p(hi), _p(idx), _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes,
+                                         _stream()), "nr_topk_archive_ranged")
+    elif lo is not None:
+        check(lib.nr_topk_dot_ranged(_p(users), U, D, _p(news), n, D, D, kk, _p(excl_offsets), _p(excl_rows), _p(cat),
+                                     max_per_category if capped else 0, _p(lo), _p(hi), _p(idx), _p(score), _p(flags[0:1]),
+                                     _p(flags[1:2]), _p(workspace), ws_bytes, _stream()), "nr_topk_dot_ranged")
+    elif dnn is not None:
         W1, b1, w2, b2 = dnn
         check(lib.nr_topk_archive(_p(users), U, P, _p(news), n, D, _p(W1), _p(b1), hidden, _p(w2), _p(b2), kk,
                                   _p(excl_offsets), _p(excl_rows), _p(cat), max_per_category if capped else 0, _p(idx),
                                   _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace), ws_bytes, _stream()),
               "nr_topk_archive")
     elif capped:
-        cat = categories.to(device=dev, dtype=torch.int32).contiguous()
         check(lib.nr_topk_dot_capped(_p(users), U, D, _p(news), n, D, D, k, _p(excl_offsets), _p(excl_rows), _p(cat),
                                      max_per_category, _p(idx), _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(workspace),
                                      ws_bytes, _stream()), "nr_topk_dot_capped")
@@ -745,7 +777,8 @@ def top_k_scores(users, news, k, excl_rows=None, excl_offsets=None, *, categorie
                                 _p(score), _p(flags[0:1]), _stream()), "nr_mmr_rerank")
     bad_row, bad_score = (int(x) for x in flags.tolist())
     if bad_row:
-        raise IndexError("top_k_scores: an exclusion row is outside the news pool")
+        raise IndexError("top_k_scores: an exclusion row is outside the news pool" if lo is None else
+                         "top_k_scores: an exclusion row or a row range is outside the news pool")
     if bad_score:
         raise ValueError("top_k_scores: a score is not finite; the order is undefined")
     return idx, score
@@ -830,7 +863,7 @@ def target_parts(tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None, max_t
     return query, offsets, ex_rows, ex_off
 
 
-def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None, *, dnn=None):
+def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=None, *, dnn=None, row_range=None):
     """Ranks of target news among the whole pool under nr_topk_dot's scores (nr_pool_ranks): query q (users (Q, D) fp32)
     has targets tgt_rows[tgt_offsets[q] .. tgt_offsets[q + 1]) of news (n, D) fp32 and optional exclusions in CSR form.
     rank(q, t) is t's 0-based position in the order top_k_scores returns for q over the pool without q's exclusions and
@@ -839,7 +872,10 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
     kernel rows (target_parts).  Raises NewsrecError on bad arguments (before any launch), IndexError on a target or
     exclusion row outside [0, n) and ValueError on a non-finite score (the device flags are read once: one
     synchronisation).  With dnn = (W1, b1, w2, b2) the scores are top_k_scores(..., dnn=)'s (nr_pool_ranks_archive) and
-    users is (Q, F) or (Q, P, F)."""
+    users is (Q, F) or (Q, P, F).  With row_range = (lo, hi), two (Q,) integer tensors, query q only counts news rows
+    lo[q] <= r < hi[q] (nr_pool_ranks_ranged, nr_pool_ranks_archive_ranged): the ranks of the call with every row outside
+    that range excluded, bit for bit; a target outside its range is still ranked.  A range outside [0, n] or with lo > hi
+    raises IndexError."""
     import numpy as np
     lib = load_library()
     if dnn is None and (users.dim() != 2 or news.dim() != 2 or users.shape[1] != news.shape[1]):
@@ -850,6 +886,9 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
         raise NewsrecError("pool_ranks: excl_rows and excl_offsets go together")
     to = torch.as_tensor(tgt_offsets).cpu().long().numpy()
     Q, D = users.shape[0], users.shape[-1]
+    lo = hi = None
+    if row_range is not None:
+        lo, hi = _row_range("pool_ranks", row_range, Q, require_cuda())
     n = news.shape[0]
     if to.ndim != 1 or len(to) != Q + 1 or to[0] != 0 or (np.diff(to) < 0).any() or to[-1] != len(tgt_rows):
         raise NewsrecError("pool_ranks: tgt_offsets must be (Q + 1,), start at 0, not decrease and end at len(tgt_rows)")
@@ -883,6 +922,8 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
     users = users.to(dev).float()
     same = R == Q and bool((query == np.arange(Q)).all())
     rows = users.contiguous() if same else users.index_select(0, torch.from_numpy(query).to(dev)).contiguous()
+    if lo is not None and not same:
+        lo, hi = (t.index_select(0, torch.from_numpy(query).to(dev)).contiguous() for t in (lo, hi))
     news = news.to(dev).float().contiguous()
     ws_bytes = workspace_bytes(R)
     if ws_bytes < 0:
@@ -897,7 +938,17 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
     score = torch.empty(n_t, dtype=torch.float32, device=dev)
     flags = torch.zeros(3, dtype=torch.int32, device=dev)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    if dnn is None:
+    if lo is not None and dnn is None:
+        check(lib.nr_pool_ranks_ranged(_p(rows), R, D, _p(news), n, D, D, _p(d_to), _p(d_tr), _p(d_xo), _p(d_xr), _p(lo), _p(hi),
+                                       _p(rank), _p(score), _p(flags[0:1]), _p(flags[1:2]), _p(flags[2:3]), _p(workspace),
+                                       ws_bytes, _stream()), "nr_pool_ranks_ranged")
+    elif lo is not None:
+        W1, b1, w2, b2 = dnn
+        check(lib.nr_pool_ranks_archive_ranged(_p(rows), R, P, _p(news), n, D, _p(W1), _p(b1), hidden, _p(w2), _p(b2),
+                                               _p(d_to), _p(d_tr), _p(d_xo), _p(d_xr), _p(lo), _p(hi), _p(rank), _p(score),
+                                               _p(flags[0:1]), _p(flags[1:2]), _p(flags[2:3]), _p(workspace), ws_bytes,
+                                               _stream()), "nr_pool_ranks_archive_ranged")
+    elif dnn is None:
         check(lib.nr_pool_ranks(_p(rows), R, D, _p(news), n, D, D, _p(d_to), _p(d_tr), _p(d_xo), _p(d_xr), _p(rank), _p(score),
                                 _p(flags[0:1]), _p(flags[1:2]), _p(flags[2:3]), _p(workspace), ws_bytes, _stream()),
               "nr_pool_ranks")
@@ -908,7 +959,8 @@ def pool_ranks(users, news, tgt_rows, tgt_offsets, excl_rows=None, excl_offsets=
                                         _p(flags[2:3]), _p(workspace), ws_bytes, _stream()), "nr_pool_ranks_archive")
     bad_row, bad_score, too_many = (int(x) for x in flags.tolist())
     if bad_row:
-        raise IndexError("pool_ranks: a target or exclusion row is outside the news pool")
+        raise IndexError("pool_ranks: a target or exclusion row is outside the news pool" if lo is None else
+                         "pool_ranks: a target or exclusion row or a row range is outside the news pool")
     if bad_score:
         raise ValueError("pool_ranks: a score is not finite; the ranks are undefined")
     if too_many:

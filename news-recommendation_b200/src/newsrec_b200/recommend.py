@@ -31,9 +31,15 @@ cosine that of the model's news vectors (``ops.top_k_scores(..., mmr_lambda=, mm
 the plain lines byte for byte; lower lambda trades relevance for lines that do not repeat one story.  Not together with a
 category cap.
 
+Live news only: with ``max_age_hours=H`` a line only holds news first shown in ``behaviors.tsv`` within H hours before the
+line's request time, the time of the row ``evaluate.distinct_histories`` keeps for it (``window``: the definition, the
+time order the device work runs in, and ties).  Each chunk's users are sorted by request time, so a block of 64 users
+shares nearly one window and the kernels stream only its news tiles; the file does not depend on the chunk.  Caps, MMR and
+every family work as above.
+
     python -m newsrec_b200.recommend --directory data/test --out recommendations.tsv [--k 10] [--keep-clicked]
                                      [--max-per-category M [--diversify-by {category,subcategory}]
-                                      | --mmr-lambda X [--mmr-depth L]]
+                                      | --mmr-lambda X [--mmr-depth L]] [--max-age-hours H]
                                      [--checkpoint PATH | --checkpoint-dir DIR] [--user2int data/train/user2int.tsv]
                                      [--chunk-users N] [--set KNOB=VALUE ...]
 """
@@ -44,7 +50,7 @@ import sys
 
 import numpy as np
 
-from . import NewsrecError
+from . import NewsrecError, window
 from .evaluate import _gather, distinct_histories, new_flag, news_matrix, read_behaviors, read_news, user_tables, user_vectors
 
 DEFAULT_CHUNK = 65536
@@ -61,11 +67,13 @@ _REFUSED = {
 
 
 def check_request(model, directory, k, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None,
-                  who="recommend"):
+                  who="recommend", max_age_hours=None):
     """Everything recommend() refuses, checked before any device work: k outside [1, 128], a cap that is not an integer >= 1,
     a diversify_by other than "category" / "subcategory", a family whose click predictor is not a dot product, an MMR
-    request ops.mmr_request refuses or one together with a cap, a split without behaviors.tsv or news_parsed.tsv, and (with
-    a cap) a news_parsed.tsv without the diversify_by column.  Messages start with who."""
+    request ops.mmr_request refuses or one together with a cap, a split without behaviors.tsv or news_parsed.tsv, (with
+    a cap) a news_parsed.tsv without the diversify_by column, and (with max_age_hours) an age that is not a real number > 0
+    or a behaviors.tsv time that does not parse.  Messages start with who.  Returns window.load's (W, behaviors, times), or
+    None without max_age_hours."""
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= MAX_K:
         raise NewsrecError(f"{who}: k={k!r} must be an integer in [1, {MAX_K}]")
     if max_per_category is not None and (isinstance(max_per_category, bool) or
@@ -74,6 +82,8 @@ def check_request(model, directory, k, max_per_category=None, diversify_by="cate
     if diversify_by not in DIVERSIFY_FIELDS:
         raise NewsrecError(f"{who}: diversify_by={diversify_by!r} must be one of {DIVERSIFY_FIELDS}")
     refuse_family(who, model)
+    if max_age_hours is not None:
+        window.max_age_seconds(who, max_age_hours)
     from .ops import mmr_request
     try:
         mmr = mmr_request(int(k), mmr_lambda, mmr_depth)
@@ -86,6 +96,7 @@ def check_request(model, directory, k, max_per_category=None, diversify_by="cate
             raise FileNotFoundError(f"{who}: {os.path.join(directory, f)} not found")
     if max_per_category is not None and diversify_by not in news_columns(directory):
         raise NewsrecError(f"{who}: {os.path.join(directory, 'news_parsed.tsv')} has no {diversify_by} column")
+    return window.load(who, directory, max_age_hours)
 
 
 def news_columns(directory):
@@ -104,6 +115,17 @@ def list_options(who, directory, device, max_per_category=None, diversify_by="ca
     if len(keys) and (keys.min() < -2 ** 31 or keys.max() >= 2 ** 31):
         raise NewsrecError(f"{who}: a {diversify_by} id does not fit in int32")
     return dict(categories=torch.from_numpy(keys.astype(np.int32)).to(device), max_per_category=int(max_per_category))
+
+
+def time_ordered(pw, pool, opts):
+    """The pool matrix and the top_k_scores keyword arguments of list_options in pw's time order (window): the matrix
+    permuted by one gather, the category keys through pw.perm."""
+    import torch
+    perm = torch.from_numpy(pw.perm).to(pool.device)
+    opts = dict(opts)
+    if "categories" in opts:
+        opts["categories"] = opts["categories"].index_select(0, perm)
+    return pool.index_select(0, perm), opts
 
 
 def refuse_family(who, model):
@@ -153,15 +175,18 @@ class _Users:
 
 
 def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2int_path="data/train/user2int.tsv",
-              chunk_users=DEFAULT_CHUNK, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None) -> int:
+              chunk_users=DEFAULT_CHUNK, max_per_category=None, diversify_by="category", mmr_lambda=None, mmr_depth=None,
+              max_age_hours=None) -> int:
     """Write the k best news of the pool for every distinct history of directory/behaviors.tsv to out_path; returns the
     number of lines.  Runs under torch.no_grad() on the model as given (call .eval() first).  The file appears only when
     every line is written; a non-finite score raises ValueError, a history row outside the news table IndexError.  With
     max_per_category=m a line holds at most m news of one diversify_by value; with mmr_lambda the lines are the MMR
-    re-rankings of each user's top mmr_depth (module docstring)."""
+    re-rankings of each user's top mmr_depth; with max_age_hours=H only news first shown within H hours before the line's
+    request time are listed (module docstring)."""
     import torch
     from .ops import top_k_scores
-    check_request(model, directory, k, max_per_category, diversify_by, mmr_lambda, mmr_depth)
+    win = check_request(model, directory, k, max_per_category, diversify_by, mmr_lambda, mmr_depth,
+                        max_age_hours=max_age_hours)
     if chunk_users < 1:
         raise ValueError(f"recommend: chunk_users={chunk_users}")
     with torch.no_grad():
@@ -173,6 +198,11 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
         user, history, length, _ = user_tables(beh, news_index, model.config.num_clicked_news_a_user, user2int_path)
         pool = matrix[:pad]
         cap = list_options("recommend", directory, matrix.device, max_per_category, diversify_by, mmr_lambda, mmr_depth)
+        if win is not None:
+            W, wbeh, times = win
+            pw = window.pool_window(wbeh, times, news_ids)
+            t_user = times[distinct_histories(wbeh).index.to_numpy()]
+            pool, cap = time_ordered(pw, pool, cap)
         U = len(user)
         flag = new_flag(matrix.device)
         tmp = f"{out_path}.partial"
@@ -180,15 +210,24 @@ def recommend(model, directory, out_path, k=10, *, exclude_clicked=True, user2in
             with open(tmp, "wb") as f:
                 for a in range(0, U, chunk_users):
                     b = min(U, a + chunk_users)
-                    users, dnn = pool_operands(model, _Users(user[a:b], history[a:b], length[a:b]), matrix, flag)
+                    sel, row_range = slice(a, b), None
+                    if win is not None:  # by request time within the chunk: a block of 64 users shares nearly one window
+                        sel = a + np.argsort(t_user[a:b], kind="stable")
+                        row_range = tuple(torch.from_numpy(x) for x in pw.ranges(t_user[sel], W))
+                    users, dnn = pool_operands(model, _Users(user[sel], history[sel], length[sel]), matrix, flag)
                     excl = None, None
                     if exclude_clicked:
-                        rows, offsets = exclusion_csr(history[a:b], pad)
+                        rows, offsets = exclusion_csr(history[sel], pad)
+                        if win is not None:
+                            rows = pw.to_time_order(rows)
                         excl = torch.from_numpy(rows), torch.from_numpy(offsets)
-                    idx, _ = top_k_scores(users, pool, int(k), *excl, dnn=dnn, **cap)  # reads its flags: synchronises
+                    idx, _ = top_k_scores(users, pool, int(k), *excl, dnn=dnn, row_range=row_range, **cap)  # synchronises
                     if int(flag.item()):
                         raise IndexError("recommend: a history row is outside the news table")
-                    f.write(format_lines(user_ids[a:b], idx.cpu().numpy(), news_ids))
+                    idx = idx.cpu().numpy()
+                    if win is not None:  # back to pool rows and to the users' order
+                        idx[sel - a] = pw.to_rows(idx.copy())
+                    f.write(format_lines(user_ids[a:b], idx, news_ids))
             os.replace(tmp, out_path)
         finally:
             if os.path.exists(tmp):
@@ -209,6 +248,8 @@ def parse_args(argv=None):
     g.add_argument("--checkpoint-dir", help="load its latest ckpt-<n>.pth (default: ./checkpoint/<MODEL_NAME>)")
     ap.add_argument("--keep-clicked", action="store_true", help="let a user's clicked news be recommended back")
     add_diversify_args(ap, "category")
+    add_window_arg(ap, "list only news first shown in behaviors.tsv within H hours before the line's request time "
+                       "(inf: every news shown by then)")
     ap.add_argument("--user2int", default="./data/train/user2int.tsv")
     ap.add_argument("--chunk-users", type=int, default=DEFAULT_CHUNK, help="users scored per device pass")
     ap.add_argument("--set", action="append", default=[], metavar="KNOB=VALUE",
@@ -219,7 +260,18 @@ def parse_args(argv=None):
     if args.chunk_users < 1:
         ap.error("--chunk-users must be at least 1")
     check_diversify_args(ap, args)
+    check_window_arg(ap, args)
     return args
+
+
+def add_window_arg(ap, help_text):
+    """--max-age-hours H, shared with pool_eval; check_window_arg refuses what window.max_age_seconds refuses."""
+    ap.add_argument("--max-age-hours", type=float, default=None, metavar="H", help=help_text)
+
+
+def check_window_arg(ap, args):
+    if args.max_age_hours is not None and not args.max_age_hours > 0.0:
+        ap.error("--max-age-hours must be a number > 0 (inf: no age limit)")
 
 
 def add_diversify_args(ap, diversify_by_default):
@@ -256,10 +308,12 @@ def main(argv=None):
     name, path, model = load_model(args.checkpoint, args.checkpoint_dir, args.set)
     n = recommend(model, args.directory, args.out, args.k, exclude_clicked=not args.keep_clicked, user2int_path=args.user2int,
                   chunk_users=args.chunk_users, max_per_category=args.max_per_category, diversify_by=args.diversify_by,
-                  mmr_lambda=args.mmr_lambda, mmr_depth=args.mmr_depth)
+                  mmr_lambda=args.mmr_lambda, mmr_depth=args.mmr_depth, max_age_hours=args.max_age_hours)
     cap = "" if args.max_per_category is None else f" (at most {args.max_per_category} per {args.diversify_by})"
     if args.mmr_lambda is not None:
         cap = f" (MMR re-ranked, lambda {args.mmr_lambda})"
+    if args.max_age_hours is not None:
+        cap += f" (news at most {args.max_age_hours:g} h old)"
     print(f"{name} from {path}: top {args.k} news{cap} of {n} users written to {args.out}")
     return 0
 
