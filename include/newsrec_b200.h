@@ -508,8 +508,17 @@ typedef struct {
     /* dense variants only (NULL otherwise): fp32 [T][d] contiguous positional addend; the rows entering the projection are
      * X = dense + dense_pos[t], summed in fp32 before any rounding (Exp1's user encoder) */
     const float* dense_pos;
+    /* ids variant at the title-level attention kernel's shape (T = 20, d_k = 20, <= 15 heads), either precision: NULL, or a
+     * buffer of nr_mhsa_encoder_live_bytes(n_seq, T, d) bytes (16-byte aligned) that selects the forward over live tokens
+     * (id in [1, V), or every token when row 0 of the table is nonzero).  X_bf16, QKV_bf16 and V_lo_bf16 then hold the live
+     * tokens' rows only, in ascending token order, followed by zero X rows up to the next multiple of 64 (below n_seq*T);
+     * C_bf16 / C_lo_bf16, w and out are as without it.  The buffer, X_bf16 and QKV_bf16 go to the backward together
+     * (nr_mhsa_encoder_bwd_args.live).  Anywhere else a non-NULL live is refused (-1) before any launch. */
+    void* live;
+    long long live_bytes;
 } nr_mhsa_encoder_fwd_args;
 int nr_mhsa_accurate_supported(int T, int d, int heads); /* 1: the accurate news variant exists for this shape */
+long long nr_mhsa_encoder_live_bytes(long long n_seq, int T, int d); /* bytes of the live-token buffer of the two calls */
 int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream);
 
 typedef struct {
@@ -552,6 +561,10 @@ typedef struct {
      * for padding.  NULL: the same verdict from the gathered rows X instead (a token is live when its id is in [1, V) or its
      * row of X is nonzero below column d), which costs a read of the dead tokens' rows.  NULL for the dense variant. */
     const void* table_bf16;
+    /* the forward's live-token buffer (nr_mhsa_encoder_fwd_args.live), or NULL: X_bf16 / QKV_bf16 are the forward's compact
+     * rows, and the backward reuses its compaction instead of classifying the tokens again */
+    void* live;
+    long long live_bytes;
 } nr_mhsa_encoder_bwd_args;
 long long nr_mhsa_encoder_bwd_workspace(long long n_seq, int T, int d, int q);
 int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream);

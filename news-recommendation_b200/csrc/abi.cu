@@ -47,7 +47,7 @@ int nr_debug_live_tokens(const long long* ids, long long n_seq, int T, int d, co
                "nr_debug_live_tokens: null operand or n_seq=%lld d=%d", n_seq, d);
     const cudaStream_t st = as_stream(stream);
     const int sec = (d + 7) & ~7, ld3 = (3 * sec + 15) & ~15;
-    const long long bytes = live_tokens_bytes(n_seq, T, ld3);
+    const long long bytes = live_tokens_bytes(n_seq, T, sec, ld3);
     char* buf = nullptr;
     NR_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), bytes, st));
     LiveTokens lt;
@@ -410,6 +410,10 @@ static bool mhsa_accurate_shape(int T, int d, int heads, int ld3, int ldx) {
 int nr_mhsa_accurate_supported(int T, int d, int heads) {
     return mhsa_accurate_shape(T, d, heads, (3 * qkv_section(d) + 15) & ~15, (d + 8) & ~7) ? 1 : 0;
 }
+long long nr_mhsa_encoder_live_bytes(long long n_seq, int T, int d) {
+    NR_REQUIRE(n_seq >= 0 && T >= 1 && d >= 1, "nr_mhsa_encoder_live_bytes: n_seq=%lld T=%d d=%d", n_seq, T, d);
+    return live_tokens_bytes(n_seq, T, qkv_section(d), (3 * qkv_section(d) + 15) & ~15);
+}
 
 // the padding-title buffers of one encoder call, released (stream-ordered) on every way out of it
 struct PaddingScope {
@@ -434,11 +438,43 @@ int nr_mhsa_encoder_fwd(const nr_mhsa_encoder_fwd_args* a, void* stream) {
     NR_REQUIRE(precise_dense || (a->wqkv_bf16 && a->bqkv && a->X_bf16 && a->QKV_bf16), "nr_mhsa_encoder_fwd: null operand");
     NR_REQUIRE(a->p_drop >= 0.f && a->p_drop < 1.f, "nr_mhsa_encoder_fwd: dropout p=%f", a->p_drop);
     NR_REQUIRE(a->dense_pos == nullptr || a->dense != nullptr, "nr_mhsa_encoder_fwd: dense_pos needs the dense (user-level) variant");
+    const int sec = qkv_section(a->d);
+    if (a->live != nullptr) {
+        NR_REQUIRE(a->ids != nullptr && mhsa_title_fwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx) &&
+                       (a->V_lo_bf16 == nullptr || mhsa_accurate_shape(a->T, a->d, a->heads, a->ld3, a->ldx)),
+                   "nr_mhsa_encoder_fwd: live tokens need the ids variant at the title-level attention kernel's shape");
+        NR_REQUIRE(a->live_bytes >= live_tokens_bytes(a->n_seq, a->T, sec, a->ld3), "nr_mhsa_encoder_fwd: live buffer too small (%lld bytes)",
+                   a->live_bytes);
+    }
     if (a->n_seq == 0) return 0;
     const int M = static_cast<int>(a->n_seq * a->T);
     const cudaStream_t st = as_stream(stream);
-    const int sec = qkv_section(a->d);
     prof_context(a->ids != nullptr ? "news.fwd" : "user.fwd");
+    if (a->live != nullptr) {
+        // the news encoder over live tokens (LiveTokens, nr_ops.h; about a third of a batch of padded titles and left-padded
+        // histories): the gather and the projection write the live tokens' X and Q|K|V rows only, in compact order, and the title
+        // attention reads a dead token's Q|K|V from the bias rows.  The context stays in token order.  The backward reuses the
+        // compaction, the compact X and the compact Q|K|V.
+        NR_REQUIRE(a->table_bf16 && a->bad_id_flag && a->V >= 1 && (a->V_lo_bf16 == nullptr || a->C_lo_bf16 != nullptr),
+                   "nr_mhsa_encoder_fwd: table / bad_id_flag missing (or V_lo_bf16 without C_lo_bf16)");
+        LiveTokens live;
+        NR_PROPAGATE(live_tokens(a->ids, a->n_seq, a->T, a->d, a->table_bf16, a->ldx, a->V, a->bqkv, sec, a->ld3, nullptr, a->ldx, nullptr,
+                                 nullptr, a->live, a->live_bytes, &live, st, a->bad_id_flag));
+        NR_PROPAGATE(gather_rows(a->ids, M, a->T, a->table_bf16, a->V, a->d, a->ldx, a->X_bf16, a->ldx, 0, DropoutCfg{a->p_drop, a->seed},
+                                 a->bad_id_flag, st, &live));
+        const bool hilo = a->V_lo_bf16 != nullptr;
+        NR_PROPAGATE(gemm_store({.A = a->X_bf16, .M = M, .lda = a->ldx, .W = a->wqkv_bf16, .N = 3 * sec, .ldw = a->ldx, .K = a->d},
+                                {.out = a->QKV_bf16, .ld_out = a->ld3, .out_bf16 = 1, .bias = a->bqkv, .lo_out = a->V_lo_bf16,
+                                 .ld_lo = hilo ? sec : 0, .lo_col0 = hilo ? 2 * sec : 0, .tile_list = live.tiles}, st));
+        {
+            ProfScope ps(hilo ? "mhsa_core_fwd_hilo" : "mhsa_core_fwd", static_cast<int>(a->n_seq), a->T, a->d, st);
+            NR_PROPAGATE(mhsa_title_fwd(a->QKV_bf16, a->ld3, sec, a->n_seq, a->heads, a->C_bf16, a->ldx, context_dropout(a->p_drop, a->seed),
+                                        st, a->V_lo_bf16, hilo ? sec : 0, hilo ? a->C_lo_bf16 : nullptr, nullptr, &live));
+        }
+        NR_PROPAGATE(gemm_additive_pool(a->C_bf16, M, a->ldx, a->d, a->wa_bf16, a->q, a->ldx, a->ba, a->qv, a->T, a->out, a->d,
+                                        a->w, st, hilo ? a->C_lo_bf16 : nullptr));
+        return 0;
+    }
     if (a->dense != nullptr && a->C_lo_bf16 != nullptr) {
         // precise user encoder (user_encoder.py:15-26 at fp32 accuracy): the input enters as a hi/lo pair against the
         // K-concatenated weights [W | W], Q|K|V stays fp32, the attention runs in fp32, the context leaves as hi/lo planes
@@ -517,7 +553,7 @@ struct MhsaBwdWorkspace : WorkspaceLayout {
         : WorkspaceLayout{static_cast<char*>(base)}, dscore(take<float>(n_seq * T)), dpre(take<__nv_bfloat16>(n_seq * T * round_up(q, 16))),
           dC(take<__nv_bfloat16>(n_seq * T * round_up(d + 1, 8))), dQKV(take<__nv_bfloat16>(n_seq * T * round_up(3 * qkv_section(d), 16))),
           QKV(take<__nv_bfloat16>(n_seq * T * round_up(3 * qkv_section(d), 16))),
-          live_bytes(live_tokens_bytes(n_seq, T, round_up(3 * qkv_section(d), 16))) {
+          live_bytes(live_tokens_bytes(n_seq, T, qkv_section(d), round_up(3 * qkv_section(d), 16))) {
         live = take<char>(live_bytes);
     }
 };
@@ -541,10 +577,17 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     NR_REQUIRE(a->table_bf16 == nullptr || a->ids != nullptr, "nr_mhsa_encoder_bwd: table_bf16 needs the ids (news) variant");
     const MhsaBwdWorkspace ws(a->workspace, a->n_seq, a->T, a->d, a->q);
     NR_REQUIRE(a->workspace_bytes >= ws.bytes(), "nr_mhsa_encoder_bwd: workspace too small (%lld bytes)", a->workspace_bytes);
+    const int sec = qkv_section(a->d);
+    const bool title_shape = mhsa_title_bwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx, a->ld3);
+    if (a->live != nullptr) {
+        NR_REQUIRE(a->ids != nullptr && title_shape && a->QKV_bf16 != nullptr,
+                   "nr_mhsa_encoder_bwd: live tokens need the ids variant at the title-level attention kernel's shape");
+        NR_REQUIRE(a->live_bytes >= live_tokens_bytes(a->n_seq, a->T, sec, a->ld3), "nr_mhsa_encoder_bwd: live buffer too small (%lld bytes)",
+                   a->live_bytes);
+    }
     if (a->n_seq == 0) return 0;
     const int M = static_cast<int>(a->n_seq * a->T);
     const cudaStream_t st = as_stream(stream);
-    const int sec = qkv_section(a->d);
 
     prof_context(a->ids != nullptr ? "news.bwd" : "user.bwd");
     const void* QKV = a->QKV_bf16;
@@ -566,14 +609,20 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     // dQ|dK|dV rows in compact order and sums the dead tokens' rows into the bias column, the dead tokens' only weight-gradient
     // term (their X rows are [0 .. 0, 1]); padding titles read their Q|K|V from the shared bias tile (the accurate forward left
     // their rows unwritten)
+    // with the forward's live tokens (a->live) the compaction, the compact X and the compact Q|K|V are the forward's: only the
+    // tail rows of the compact dQ|dK|dV need their zeros
     LiveTokens live;
-    const bool compact = a->ids != nullptr && mhsa_title_bwd_supported(a->T, a->d / a->heads, a->heads, sec, a->ld3, a->ldx, a->ld3);
-    if (compact) {
+    const bool compact = a->ids != nullptr && title_shape;
+    const bool from_fwd = a->live != nullptr;
+    if (from_fwd) {
+        live = live_tokens_view(a->live, a->n_seq, a->T, sec, a->ld3);
+        NR_PROPAGATE(live_zero_tail(live, a->n_seq, a->T, ws.dQKV, a->ld3, st));
+    } else if (compact) {
         NR_REQUIRE(a->V >= 1, "nr_mhsa_encoder_bwd: V=%d", a->V);
         NR_PROPAGATE(live_tokens(a->ids, a->n_seq, a->T, a->d, a->table_bf16, a->ldx, a->V, a->bqkv, sec, a->ld3, a->X_bf16, a->ldx, ws.QKV,
                                  ws.dQKV, ws.live, ws.live_bytes, &live, st));
     }
-    const TitleBwdLive title_live{.tokens = &live, .dbias = a->dWqkv_ext + a->d, .ld_dbias = a->ldx};
+    const TitleBwdLive title_live{.tokens = &live, .dbias = a->dWqkv_ext + a->d, .ld_dbias = a->ldx, .compact_qkv = from_fwd ? 1 : 0};
     NR_PROPAGATE(mhsa_core_bwd(QKV, a->ld3, sec, ws.dC, a->ldx, a->n_seq, a->T, a->heads, a->d / a->heads, ws.dQKV, a->ld3, st,
                                compact ? &title_live : nullptr));
     // --- projection backward: the input first (the embedding gradient is 97 % of a data-parallel step's all-reduce: the
@@ -594,9 +643,10 @@ int nr_mhsa_encoder_bwd(const nr_mhsa_encoder_bwd_args* a, void* stream) {
     // both weight-gradient GEMMs run AFTER the embedding gradient is complete: together they are the window (~0.4 ms) under which
     // the caller's all-reduce of that gradient hides
     NR_PROPAGATE(gemm_weight_grad(ws.dpre, M, a->q, a->ldq, a->C_bf16, a->d, a->ldx, a->dWa_ext, st));
-    // compact: the live tokens' dQ|dK|dV against the compact copy of their X rows (+ bias through its ones column)
-    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, compact ? ws.QKV : a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st, 0,
-                                  live.tiles));
+    // compact: the live tokens' dQ|dK|dV against the compact copy of their X rows (+ bias through its ones column); the
+    // forward's X when it ran over live tokens
+    NR_PROPAGATE(gemm_weight_grad(ws.dQKV, M, 3 * sec, a->ld3, compact && !from_fwd ? ws.QKV : a->X_bf16, a->d, a->ldx, a->dWqkv_ext, st,
+                                  0, live.tiles));
     return 0;
 }
 

@@ -16,7 +16,9 @@
 //     even h:  [0,16) as one k16 step, [16,24) as a k8 step whose columns 20..23 belong to head h+1
 //     odd  h:  [-4,4) as a k8 step whose columns -4..-1 belong to head h-1, [4,20) as one k16 step
 // Foreign columns are zeroed in the fragment registers (select, so that NaN payloads cannot leak) when they are a
-// contraction index and simply not stored when they are an output column.  Rows 20..23 of a tile (k8 steps over the title
+// contraction index and simply not stored when they are an output column.  Every Q|K|V row address goes through a per-lane
+// row map (row_offsets): the identity, or over the live tokens' compact rows a title's rank map with the dead rows (and rows
+// 20..23) pointed at a bias row in shared memory.  Rows 20..23 of a tile in token order (k8 steps over the title
 // rows) are whatever follows the tile in shared memory: the matching fragment lanes are zeroed the same way.
 //
 // Shared-memory row pitches are (odd multiple of 16) bytes: eight consecutive rows start in eight distinct bank quads, so
@@ -52,6 +54,25 @@ constexpr int kScrPitch = 48;    // bytes per scratch row: 24 bf16 key columns
 constexpr int kScrTile = 24 * kScrPitch;
 constexpr int kScrWarp = 2 * kScrTile;  // A | dS of one head
 
+// Shared-memory offsets, from a stage's Q|K|V (or V low plane) tile, of the tile rows lane & 7, 8 + (lane & 7) and
+// 16 + (lane & 7): every ldmatrix row address of a lane is one of them.  Token order (mask null): the rows themselves.
+// Compact rows (LiveTokens; the tile holds the rows from the title's first compact row on): a live token's rank among the
+// title's live tokens, and for a dead token and the rows 20..23 the CTA's copy of the bias row, `to_bias` from the tile.
+__device__ __forceinline__ void row_offsets(const uint32_t* mask, int title, uint32_t pitch, uint32_t to_bias, int lane, uint32_t ro[3]) {
+    const uint32_t m = mask != nullptr ? __ldg(mask + title) : 0u;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        const uint32_t r = 8u * j + static_cast<uint32_t>(lane & 7);
+        const bool live = r < kT && ((m >> r) & 1u);
+        ro[j] = mask == nullptr ? r * pitch : live ? static_cast<uint32_t>(__popc(m & ((1u << r) - 1u))) * pitch : to_bias;
+    }
+}
+// the bias row (row_bytes) into shared memory, zeros up to pitch bytes; every thread of the block takes part
+__device__ __forceinline__ void copy_bias_row(uint8_t* dst, const void* src, uint32_t row_bytes, uint32_t pitch) {
+    for (uint32_t i = threadIdx.x; i < pitch / 16u; i += blockDim.x)
+        reinterpret_cast<uint4*>(dst)[i] = i < row_bytes / 16u ? __ldg(static_cast<const uint4*>(src) + i) : make_uint4(0, 0, 0, 0);
+}
+
 struct Params {
     int n_seq, heads;
     uint32_t sec2;        // section stride in bytes
@@ -70,6 +91,10 @@ struct Params {
     uint32_t ld_out, row_bytes;
     float* dbias;
     int ld_dbias;
+    // compact (the compact forward's Q|K|V): title s reads its rows from compact row offset[s] on through the row map of
+    // row_offsets, a dead token the bias row (LiveTokens::qkv), kept in shared memory behind the barriers
+    int compact;
+    const void* bias;
 };
 
 __device__ __forceinline__ uint32_t sel(bool keep, uint32_t v) { return keep ? v : 0u; }
@@ -91,6 +116,8 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
 
     // every byte a fragment load can touch is initialised: slack rows / padding columns read finite zeros before the first TMA
     for (uint32_t i = tid; i < bar_off / 16; i += blockDim.x) reinterpret_cast<uint4*>(base_ptr)[i] = make_uint4(0, 0, 0, 0);
+    const uint32_t bias_off = bar_off + 128u;
+    if (p.compact) copy_bias_row(base_ptr + bias_off, p.bias, 3u * p.sec2, p.pq);
     if (tid == 0) {
         for (int i = 0; i < kIn; ++i) {
             mbar_init(&full[i], 1);
@@ -118,8 +145,9 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                 const int s = it % kIn;
                 const int title = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x), row = title * kT;
                 const bool pad = p.pad != nullptr && p.pad[title] != 0;  // a padding title reads the shared bias tile
-                mbar_arrive_expect_tx(&full[s], p.tx);
-                tma_load_2d(base_ptr + s * p.in_stage, pad ? &tm_pad : &tm_qkv, &full[s], 0, pad ? 0 : row);
+                const bool none = pad && p.compact;                      // compact: its rows are all the bias row
+                mbar_arrive_expect_tx(&full[s], none ? p.tx - kT * p.pq : p.tx);
+                if (!none) tma_load_2d(base_ptr + s * p.in_stage, pad ? &tm_pad : &tm_qkv, &full[s], 0, pad ? 0 : p.compact ? p.offset[title] : row);
                 tma_load_2d(base_ptr + s * p.in_stage + p.qkv_tile, &tm_dc, &full[s], 0, row);
             };
             for (int it = 0; it < kIn && it < n_my; ++it) load(it);
@@ -163,7 +191,7 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
     const bool c2ok = odd || t4 < 2;
     const bool lo2 = t4 < 2;                        // key columns 16 + 2*t4 (+1) < 20; also: rows 16 + 2*t4 (+1) < 20
     const uint32_t pq = p.pq, pc = p.pc;
-    const uint32_t r15q = (lane & 15) * pq, r7q = (lane & 7) * pq, r15c = (lane & 15) * pc, r7c = (lane & 7) * pc;
+    const uint32_t r15c = (lane & 15) * pc, r7c = (lane & 7) * pc;
     const uint32_t hi = (lane >> 4) * 16u, mid = ((lane >> 3) & 1) * 16u;
     const uint32_t ps = scr_base + h * kScrWarp, dsb = ps + kScrTile;  // A | dS scratch of this head
     const uint32_t at0 = ((lane & 7) + (lane >> 4) * 8) * kScrPitch + mid;  // x4.trans, key rows 0..15 as m
@@ -183,38 +211,42 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
         const int s = it % kIn, o = it % kOut;
         const uint32_t Q = in_base + s * p.in_stage, K = Q + p.sec2, V = K + p.sec2, G = Q + p.qkv_tile;
         const uint32_t ob = out_base + o * p.out_stage;
-        const uint32_t dead = p.mask != nullptr ? ~__ldg(p.mask + static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x)) : 0u;
+        const int title = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
+        const uint32_t dead = p.mask != nullptr ? ~__ldg(p.mask + title) : 0u;
+        uint32_t ro[3];  // Q|K|V rows lane & 7 (+ 8, + 16) of the tile
+        row_offsets(p.compact ? p.mask : nullptr, title, pq, base + bias_off - Q, lane, ro);
+        const uint32_t r15 = (lane & 8) ? ro[1] : ro[0];
         f_wait(&full[s], (it / kIn) & 1, 72);
 
         // ---- phase A (query rows i): A, dS -> scratch; dQ -> result tile ----
         uint32_t kb16[3][2], kb8[3], vb16[3][2], vb8[3], kt16[3][2], kt8[3];
 #pragma unroll
         for (int nt = 0; nt < 3; ++nt) {
-            lds_x2(kb16[nt], K + k16b + nt * 8 * pq + r7q + mid);
-            lds_x2(vb16[nt], V + k16b + nt * 8 * pq + r7q + mid);
-            lds_x1(&kb8[nt], K + k8b + nt * 8 * pq + r7q);
-            lds_x1(&vb8[nt], V + k8b + nt * 8 * pq + r7q);
+            lds_x2(kb16[nt], K + k16b + ro[nt] + mid);
+            lds_x2(vb16[nt], V + k16b + ro[nt] + mid);
+            lds_x1(&kb8[nt], K + k8b + ro[nt]);
+            lds_x1(&vb8[nt], V + k8b + ro[nt]);
             kb8[nt] = sel(v8, kb8[nt]);
             vb8[nt] = sel(v8, vb8[nt]);
-            lds_x2_t(kt16[nt], K + gb + 16 * nt + r15q);
-            lds_x1_t(&kt8[nt], K + gb + 16 * nt + 16 * pq + r7q);
+            lds_x2_t(kt16[nt], K + gb + 16 * nt + r15);
+            lds_x1_t(&kt8[nt], K + gb + 16 * nt + ro[2]);
             kt8[nt] = sel(lo2, kt8[nt]);
         }
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
             uint32_t aq[4], ag[4], aq8[2], ag8[2];
             if (mt == 0) {
-                lds_x4(aq, Q + k16b + r15q + hi);
+                lds_x4(aq, Q + k16b + r15 + hi);
                 lds_x4(ag, G + k16b + r15c + hi);
-                lds_x2(aq8, Q + k8b + r15q);
+                lds_x2(aq8, Q + k8b + r15);
                 lds_x2(ag8, G + k8b + r15c);
             } else {  // rows 16..23 only: the second half of this row block is dead
                 uint32_t t[2];
-                lds_x2(t, Q + k16b + 16 * pq + r7q + mid);
+                lds_x2(t, Q + k16b + ro[2] + mid);
                 aq[0] = t[0], aq[1] = 0u, aq[2] = t[1], aq[3] = 0u;
                 lds_x2(t, G + k16b + 16 * pc + r7c + mid);
                 ag[0] = t[0], ag[1] = 0u, ag[2] = t[1], ag[3] = 0u;
-                lds_x1(&aq8[0], Q + k8b + 16 * pq + r7q);
+                lds_x1(&aq8[0], Q + k8b + ro[2]);
                 lds_x1(&ag8[0], G + k8b + 16 * pc + r7c);
                 aq8[1] = ag8[1] = 0u;
             }
@@ -328,9 +360,9 @@ mhsa_title_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
         uint32_t qt16[3][2], qt8[3], gt16[3][2], gt8[3];
 #pragma unroll
         for (int nd = 0; nd < 3; ++nd) {
-            lds_x2_t(qt16[nd], Q + gb + 16 * nd + r15q);
+            lds_x2_t(qt16[nd], Q + gb + 16 * nd + r15);
             lds_x2_t(gt16[nd], G + gb + 16 * nd + r15c);
-            lds_x1_t(&qt8[nd], Q + gb + 16 * nd + 16 * pq + r7q);
+            lds_x1_t(&qt8[nd], Q + gb + 16 * nd + ro[2]);
             lds_x1_t(&gt8[nd], G + gb + 16 * nd + 16 * pc + r7c);
             qt8[nd] = sel(lo2, qt8[nd]);
             gt8[nd] = sel(lo2, gt8[nd]);
@@ -421,6 +453,11 @@ struct FwdParams {
     float sc;
     Dropout drop;
     const unsigned char* pad;  // PaddingTitles::pad or null
+    // compact rows (LiveTokens) or null: title s reads its rows from compact row offset[s] on through the row map of
+    // row_offsets (mask[s] == 0: no load at all), a dead token the bias rows bias_q / bias_v, kept in shared memory
+    const uint32_t* mask;
+    const int* offset;
+    const void *bias_q, *bias_v;
 };
 
 template <bool HILO>
@@ -441,6 +478,11 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
     uint64_t* const ofull = bars + 2 * kIn;
     uint64_t* const oempty = bars + 2 * kIn + kOut;
     for (uint32_t i = tid; i < bar_off / 16; i += blockDim.x) reinterpret_cast<uint4*>(base_ptr)[i] = make_uint4(0, 0, 0, 0);
+    const uint32_t bias_q = bar_off + 128u, bias_v = bias_q + p.pq;  // the bias rows behind the barriers
+    if (p.mask != nullptr) {
+        copy_bias_row(base_ptr + bias_q, p.bias_q, 3u * p.sec2, p.pq);
+        if (HILO) copy_bias_row(base_ptr + bias_v, p.bias_v, p.sec2, p.pv);
+    }
     __syncthreads();
     if (tid < kOut * kT)  // the ones column of the context rows (bias trick of the pooling GEMM); hi plane only
         *reinterpret_cast<__nv_bfloat16*>(base_ptr + kIn * p.in_stage + (tid / kT) * p.out_stage + (tid % kT) * p.pc + p.heads * kDk * 2) =
@@ -476,7 +518,11 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
                 const int s = it % kIn;
                 const int title = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
                 const bool pad = p.pad != nullptr && p.pad[title] != 0;  // a padding title reads the shared bias tile
-                const int row = pad ? 0 : title * kT;
+                if (p.mask != nullptr && p.mask[title] == 0) {          // compact: its rows are all the bias rows
+                    mbar_arrive(&full[s]);
+                    return;
+                }
+                const int row = pad ? 0 : p.mask != nullptr ? p.offset[title] : title * kT;
                 mbar_arrive_expect_tx(&full[s], p.tx);
                 tma_load_2d(base_ptr + s * p.in_stage, pad ? &tm_pad : &tm_qkv, &full[s], 0, row);
                 if (HILO) tma_load_2d(base_ptr + s * p.in_stage + p.qkv_tile, pad ? &tm_padlo : &tm_vlo, &full[s], 0, row);
@@ -508,7 +554,6 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
     const bool v8 = odd ? (t4 >= 2) : (t4 < 2);
     const bool c0ok = !odd || t4 >= 2, c2ok = odd || t4 < 2, lo2 = t4 < 2;
     const uint32_t pq = p.pq, pc = p.pc, pv = p.pv;
-    const uint32_t r15q = (lane & 15) * pq, r7q = (lane & 7) * pq;
     const uint32_t hi = (lane >> 4) * 16u, mid = ((lane >> 3) & 1) * 16u;
     const float sc = p.sc;
 
@@ -516,20 +561,25 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
         const int s = it % kIn, o = it % kOut;
         const uint32_t Q = in_base + s * p.in_stage, K = Q + p.sec2, V = K + p.sec2, VL = Q + p.qkv_tile;
         const uint32_t ob = out_base + o * p.out_stage;
-        const long long row_base = static_cast<long long>(static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x)) * kT;
+        const int title = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
+        const long long row_base = static_cast<long long>(title) * kT;
+        uint32_t ro[3], rv[3];  // rows lane & 7 (+ 8, + 16) of the Q|K|V tile and of the V low-plane tile
+        row_offsets(p.mask, title, pq, base + bias_q - Q, lane, ro);
+        if (HILO) row_offsets(p.mask, title, pv, base + bias_v - VL, lane, rv);
+        const uint32_t r15 = (lane & 8) ? ro[1] : ro[0];
         f_wait(&full[s], (it / kIn) & 1, 82);
         uint32_t kb16[3][2], kb8[3], vt16[3][2], vt8[3], vl16[HILO ? 3 : 1][2], vl8[HILO ? 3 : 1];
 #pragma unroll
         for (int nt = 0; nt < 3; ++nt) {
-            lds_x2(kb16[nt], K + k16b + nt * 8 * pq + r7q + mid);
-            lds_x1(&kb8[nt], K + k8b + nt * 8 * pq + r7q);
+            lds_x2(kb16[nt], K + k16b + ro[nt] + mid);
+            lds_x1(&kb8[nt], K + k8b + ro[nt]);
             kb8[nt] = sel(v8, kb8[nt]);
-            lds_x2_t(vt16[nt], V + gb + 16 * nt + r15q);
-            lds_x1_t(&vt8[nt], V + gb + 16 * nt + 16 * pq + r7q);
+            lds_x2_t(vt16[nt], V + gb + 16 * nt + r15);
+            lds_x1_t(&vt8[nt], V + gb + 16 * nt + ro[2]);
             vt8[nt] = sel(lo2, vt8[nt]);
             if (HILO) {
-                lds_x2_t(vl16[nt], VL + gb + 16 * nt + (lane & 15) * pv);
-                lds_x1_t(&vl8[nt], VL + gb + 16 * nt + 16 * pv + (lane & 7) * pv);
+                lds_x2_t(vl16[nt], VL + gb + 16 * nt + ((lane & 8) ? rv[1] : rv[0]));
+                lds_x1_t(&vl8[nt], VL + gb + 16 * nt + rv[2]);
                 vl8[nt] = sel(lo2, vl8[nt]);
             }
         }
@@ -537,13 +587,13 @@ mhsa_title_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_c
         for (int mt = 0; mt < 2; ++mt) {
             uint32_t aq[4], aq8[2];
             if (mt == 0) {
-                lds_x4(aq, Q + k16b + r15q + hi);
-                lds_x2(aq8, Q + k8b + r15q);
+                lds_x4(aq, Q + k16b + r15 + hi);
+                lds_x2(aq8, Q + k8b + r15);
             } else {
                 uint32_t t[2];
-                lds_x2(t, Q + k16b + 16 * pq + r7q + mid);
+                lds_x2(t, Q + k16b + ro[2] + mid);
                 aq[0] = t[0], aq[1] = 0u, aq[2] = t[1], aq[3] = 0u;
-                lds_x1(&aq8[0], Q + k8b + 16 * pq + r7q);
+                lds_x1(&aq8[0], Q + k8b + ro[2]);
                 aq8[1] = 0u;
             }
             aq8[0] = sel(v8, aq8[0]), aq8[1] = sel(v8, aq8[1]);
@@ -726,8 +776,10 @@ int mhsa_title_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int l
     p.row_bytes = qkv_row;
     p.dbias = live != nullptr ? live->dbias : nullptr;
     p.ld_dbias = live != nullptr ? live->ld_dbias : 0;
+    p.compact = live != nullptr && live->compact_qkv ? 1 : 0;
+    p.bias = lt != nullptr ? lt->qkv : nullptr;
     const size_t smem = 128 + static_cast<size_t>(kIn) * p.in_stage + static_cast<size_t>(kOut) * p.out_stage +
-                       static_cast<size_t>(heads) * kScrWarp + (2 * kIn + 2 * kOut) * sizeof(uint64_t) + 64;
+                       static_cast<size_t>(heads) * kScrWarp + 128 + p.pq + 64;  // barriers | bias row
     NR_REQUIRE(smem <= 227 * 1024, "mhsa_title_bwd: %zu bytes of shared memory", smem);
     const long long rows = n_seq * kT;
     CUtensorMap tq, tc, to, tp;
@@ -760,7 +812,7 @@ bool mhsa_title_fwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int
 // v_lo / ctx_lo both non-null: the accurate (hi/lo) variant.  v_lo bf16 [rows][ld_vlo] = low plane of the V section (column 0
 // = first V column); ctx_lo bf16 [rows][ld_ctx] = low plane of the context (no ones column).
 int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int heads, void* ctx, int ld_ctx, DropoutCfg drop,
-                   cudaStream_t stream, const void* v_lo, int ld_vlo, void* ctx_lo, const PaddingTitles* pad) {
+                   cudaStream_t stream, const void* v_lo, int ld_vlo, void* ctx_lo, const PaddingTitles* pad, const LiveTokens* live) {
     using namespace title;
     NR_REQUIRE(mhsa_title_fwd_supported(kT, kDk, heads, sec, ld_qkv, ld_ctx), "mhsa_title_fwd: unsupported layout");
     NR_REQUIRE(n_seq * kT < (1ll << 31), "mhsa_title_fwd: too many rows");
@@ -786,12 +838,18 @@ int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int he
     p.drop = Dropout::make(drop.p, drop.seed);
     NR_REQUIRE(pad == nullptr || (pad->pad != nullptr && pad->qkv != nullptr && (!hilo || (pad->v_lo != nullptr && ld_vlo == sec))),
                "mhsa_title_fwd: padding titles without their Q|K|V tile (or its V low plane at pitch sec)");
+    NR_REQUIRE(live == nullptr || (pad == nullptr && live->pad && live->mask && live->offset && live->qkv && (!hilo || (live->v_lo && ld_vlo == sec))),
+               "mhsa_title_fwd: live tokens without their flags, offsets or bias rows (or with padding titles as well)");
     p.pad = pad != nullptr ? pad->pad : nullptr;
+    p.mask = live != nullptr ? live->mask : nullptr;
+    p.offset = live != nullptr ? live->offset : nullptr;
+    p.bias_q = live != nullptr ? live->qkv : nullptr;
+    p.bias_v = live != nullptr ? live->v_lo : nullptr;
     // fragment loads of rows 20..23 of a tile run into whatever follows it (the low-plane tile, the next stage, the result
     // tiles): always inside the allocation, always initialised
     const int n_in = hilo ? kInHilo : kIn;
     const size_t smem = 128 + static_cast<size_t>(n_in) * p.in_stage + static_cast<size_t>(kOut) * p.out_stage +
-                       (2 * n_in + 2 * kOut) * sizeof(uint64_t) + 64;
+                       128 + p.pq + p.pv + 64;  // barriers | bias rows
     const size_t cap = hilo ? 227 * 1024 : 113 * 1024;
     NR_REQUIRE(smem <= cap, "mhsa_title_fwd: %zu bytes of shared memory", smem);
     const long long rows = n_seq * kT;

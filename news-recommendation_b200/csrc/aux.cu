@@ -117,32 +117,44 @@ constexpr int kGatherThreads = 320;
 __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long long* __restrict__ ids, long long n_tok, int T,
                                                                    const uint4* __restrict__ table, int V, int D, int ld,
                                                                    uint4* __restrict__ X, int ld_x, int padded, Dropout drop,
-                                                                   int* bad_flag) {
+                                                                   int* bad_flag, const int* __restrict__ index,
+                                                                   const int* __restrict__ n_live) {
     const int chunks = ld >> 3;  // 16-byte chunks per table row
     const int x_chunks = ld_x >> 3;
     const int rows_per_it = kGatherThreads / chunks;
     const int rl = threadIdx.x / chunks, c = threadIdx.x - rl * chunks;
     if (rl >= rows_per_it) return;
     const long long stride = static_cast<long long>(gridDim.x) * rows_per_it;
-    long long tok = static_cast<long long>(blockIdx.x) * rows_per_it + rl;
+    // compact rows (index non-null): X row i < M' is token index[i]; the rows [M', round_up(M', 64)) below n_tok are zero rows
+    long long n_rows = n_tok;
+    if (index != nullptr) {
+        n_rows = __ldg(n_live);
+        const long long tail_end = min(n_tok, (n_rows + 63) / 64 * 64);
+        for (long long r = static_cast<long long>(blockIdx.x) * rows_per_it + rl + n_rows; r < tail_end; r += stride)
+            X[r * x_chunks + c] = make_uint4(0, 0, 0, 0);
+    }
+    const auto token = [&](long long i) -> long long { return index != nullptr ? __ldg(index + i) : i; };
+    long long i = static_cast<long long>(blockIdx.x) * rows_per_it + rl;
     // software pipeline: the (id -> table row) loads of the NEXT row are in flight while this one is stored
-    long long n_id = tok < n_tok ? __ldg(ids + tok) : 0;
-    if (tok < n_tok && (n_id < 0 || n_id >= V)) { atomicExch(bad_flag, 1); n_id = 0; }
-    uint4 n_u = tok < n_tok ? __ldg(table + n_id * chunks + c) : make_uint4(0, 0, 0, 0);
+    long long tok = i < n_rows ? token(i) : 0;
+    long long n_id = i < n_rows ? __ldg(ids + tok) : 0;
+    if (i < n_rows && (n_id < 0 || n_id >= V)) { atomicExch(bad_flag, 1); n_id = 0; }
+    uint4 n_u = i < n_rows ? __ldg(table + n_id * chunks + c) : make_uint4(0, 0, 0, 0);
     const int col = c * 8;
-    for (; tok < n_tok; tok += stride) {
+    for (; i < n_rows; i += stride) {
         uint4 u = n_u;
-        const long long tok2 = tok + stride;
-        if (tok2 < n_tok) {
-            n_id = __ldg(ids + tok2);
+        const long long cur = tok, i2 = i + stride;
+        if (i2 < n_rows) {
+            tok = token(i2);
+            n_id = __ldg(ids + tok);
             if (n_id < 0 || n_id >= V) { atomicExch(bad_flag, 1); n_id = 0; }
             n_u = __ldg(table + n_id * chunks + c);
         }
-        long long xr = tok;
+        long long xr = cur;  // the row of the token: it keys the dropout draw
         int t = 0;
         if (padded) {
-            const long long seg = tok / T;
-            t = static_cast<int>(tok - seg * T);
+            const long long seg = cur / T;
+            t = static_cast<int>(cur - seg * T);
             xr = seg * (T + 2) + 1 + t;
         }
         uint32_t w[4] = {u.x, u.y, u.z, u.w};
@@ -160,7 +172,7 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long 
             __nv_bfloat16* e = reinterpret_cast<__nv_bfloat16*>(w);
             for (int j = D - col; j < 8; ++j) e[j] = __float2bfloat16_rn(j == D - col ? 1.0f : 0.f);
         }
-        X[xr * x_chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
+        X[(index != nullptr ? i : xr) * x_chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
         if (padded) {
             if (t == 0) X[(xr - 1) * x_chunks + c] = make_uint4(0, 0, 0, 0);
             if (t == T - 1) X[(xr + 1) * x_chunks + c] = make_uint4(0, 0, 0, 0);
@@ -168,16 +180,19 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_kernel(const long 
     }
 }
 int gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld_table, void* X,
-                int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream) {
+                int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream, const LiveTokens* live) {
     if (n_tok == 0) return 0;
     NR_REQUIRE(ld_table % 8 == 0 && ld_x % 8 == 0 && ld_x >= ld_table && ld_table >= D + 1 && ld_table / 8 <= kGatherThreads,
                "gather_rows: pitch %d/%d for D=%d", ld_table, ld_x, D);
+    NR_REQUIRE(live == nullptr || (!padded && ld_x == ld_table && live->index && live->offset),
+               "gather_rows: compact rows need the unpadded layout, ld_x == ld_table and the live tokens' index");
     const int rows_per_it = kGatherThreads / (ld_table / 8);
     const int blocks = static_cast<int>(std::min<long long>((n_tok + rows_per_it - 1) / rows_per_it, 148 * 6));
     ProfScope ps("gather_rows", static_cast<int>(n_tok), D, ld_x, stream);
     gather_rows_kernel<<<blocks, kGatherThreads, 0, stream>>>(ids, n_tok, T, static_cast<const uint4*>(table), V, D, ld_table,
                                                    static_cast<uint4*>(X), ld_x, padded, Dropout::make(drop.p, drop.seed),
-                                                   bad_id_flag);
+                                                   bad_id_flag, live != nullptr ? live->index : nullptr,
+                                                   live != nullptr ? live->offset + n_tok / T : nullptr);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

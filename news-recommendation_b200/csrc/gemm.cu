@@ -958,13 +958,14 @@ struct LiveJob {
     int* counts;           // [n_seq] live tokens per title
     int* block_base;       // [n_blocks] live tokens of the titles before the block
     unsigned* ticket;
+    int* bad_id_flag;      // or null
     LiveTokens out;
 };
 
 __global__ void __launch_bounds__(kLiveTilesThreads) live_classify_kernel(const LiveJob j) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = kLiveTilesThreads / 32;
     const bool all_live = j.row0 != nullptr && block_row_nonzero(j.row0, j.d);
-    write_padding_qkv(j.bqkv, j.T, j.sec, j.ld3, j.out.qkv, nullptr);
+    write_padding_qkv(j.bqkv, j.T, j.sec, j.ld3, j.out.qkv, j.out.v_lo);
     const int gtid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
     for (int i = gtid; i < (j.M + kTileM - 1) / kTileM; i += nthreads) j.out.tiles[1 + i] = i;
     const int px = j.ldx / 8;  // 16-byte pieces per row of X
@@ -973,6 +974,7 @@ __global__ void __launch_bounds__(kLiveTilesThreads) live_classify_kernel(const 
     for (int s = s0 + warp; s < s1; s += warps) {
         const long long id = lane < j.T ? j.ids[static_cast<long long>(s) * j.T + lane] : 0;
         uint32_t mask = __ballot_sync(0xffffffffu, lane < j.T && (all_live || (id >= 1 && id < j.V)));
+        if (j.bad_id_flag != nullptr && __any_sync(0xffffffffu, lane < j.T && (id < 0 || id >= j.V)) && lane == 0) atomicExch(j.bad_id_flag, 1);
         if (j.row0 == nullptr) {  // no table: a token whose gathered row is nonzero below column d is live as well
             for (uint32_t cand = ((j.T == 32 ? 0u : 1u << j.T) - 1u) & ~mask; cand != 0; cand &= cand - 1) {
                 const int r = __ffs(cand) - 1;
@@ -1061,9 +1063,9 @@ __global__ void __launch_bounds__(kLiveTilesThreads) live_compact_kernel(const L
         const int m_live = j.out.offset[j.n_seq];
         const int tail_end = min(j.M, (m_live + kTileM - 1) / kTileM * kTileM);
         for (int r = m_live + threadIdx.x; r < tail_end; r += blockDim.x) j.out.index[r] = -1;
-        for (int i = threadIdx.x; i < (tail_end - m_live) * px; i += blockDim.x)
+        for (int i = threadIdx.x; j.Xc != nullptr && i < (tail_end - m_live) * px; i += blockDim.x)
             j.Xc[static_cast<long long>(m_live) * px + i] = make_uint4(0, 0, 0, 0);
-        for (int i = threadIdx.x; i < (tail_end - m_live) * p3; i += blockDim.x)
+        for (int i = threadIdx.x; j.dqkv_c != nullptr && i < (tail_end - m_live) * p3; i += blockDim.x)
             j.dqkv_c[static_cast<long long>(m_live) * p3 + i] = make_uint4(0, 0, 0, 0);
     }
     // a warp per title: the index entries, then every 16-byte piece of the title's live rows spread over the lanes
@@ -1077,6 +1079,7 @@ __global__ void __launch_bounds__(kLiveTilesThreads) live_compact_kernel(const L
             src_row[warp][rank] = s * j.T + lane;
         }
         __syncwarp();
+        if (j.Xc == nullptr) continue;
         const uint4* X = j.X;
         uint4* Xc = j.Xc + static_cast<long long>(dst) * px;
 #pragma unroll 4
@@ -1088,51 +1091,71 @@ __global__ void __launch_bounds__(kLiveTilesThreads) live_compact_kernel(const L
     }
 }
 
-// bytes of the LiveTokens buffers of a call (live_tokens carves them from `buf`)
-long long live_tokens_bytes(long long n_seq, int T, int ld3) {
-    const long long n = n_seq, M = n_seq * T, nb = (n + kLiveTitlesPerBlock - 1) / kLiveTitlesPerBlock;
-    WorkspaceLayout l{nullptr};
-    l.take<unsigned char>(n);           // pad
-    l.take<uint32_t>(n);                // mask
-    l.take<int>(n);                     // counts
-    l.take<int>(n + 1);                 // offset
-    l.take<int>(M);                     // index
-    l.take<int>(M / kTileM + 2);        // tiles
-    l.take<int>(nb + 1);                // block bases | ticket
-    l.take<__nv_bfloat16>(static_cast<long long>(T) * ld3);  // shared Q|K|V tile
-    return l.bytes();
-}
+// the LiveTokens buffers of a call, carved from `buf` (null: only measured) -- the one layout behind live_tokens_bytes,
+// live_tokens and live_tokens_view
+struct LiveLayout : WorkspaceLayout {
+    LiveTokens out;
+    int *counts, *block_base;
+    LiveLayout(void* buf, long long n_seq, int T, int sec, int ld3) : WorkspaceLayout{static_cast<char*>(buf)} {
+        const long long n = n_seq, M = n_seq * T, nb = (n + kLiveTitlesPerBlock - 1) / kLiveTitlesPerBlock;
+        out.pad = take<unsigned char>(n);
+        out.mask = take<uint32_t>(n);
+        counts = take<int>(n);
+        out.offset = take<int>(n + 1);
+        out.index = take<int>(M);
+        out.tiles = take<int>(M / kTileM + 2);
+        block_base = take<int>(nb + 1);  // block bases | ticket
+        out.qkv = take<__nv_bfloat16>(static_cast<long long>(T) * ld3);
+        out.v_lo = take<__nv_bfloat16>(static_cast<long long>(T) * sec);
+    }
+};
+
+long long live_tokens_bytes(long long n_seq, int T, int sec, int ld3) { return LiveLayout(nullptr, n_seq, T, sec, ld3).bytes(); }
+LiveTokens live_tokens_view(void* buf, long long n_seq, int T, int sec, int ld3) { return LiveLayout(buf, n_seq, T, sec, ld3).out; }
 
 int live_tokens(const long long* ids, long long n_seq, int T, int d, const void* table, int ld_table, int V, const float* bqkv,
                 int sec, int ld3, const void* X, int ldx, void* Xc, void* dqkv_c, void* buf, long long buf_bytes, LiveTokens* out,
-                cudaStream_t stream) {
-    NR_REQUIRE(ids && bqkv && X && Xc && dqkv_c && buf, "live_tokens: null operand");
+                cudaStream_t stream, int* bad_id_flag) {
+    NR_REQUIRE(ids && bqkv && buf && (table || X) && (!Xc || X), "live_tokens: null operand");
     NR_REQUIRE(T >= 1 && T <= 32 && d % 2 == 0 && ld_table % 8 == 0 && ldx % 8 == 0 && ld3 % 8 == 0 && V >= 1 && n_seq * T < (1ll << 31),
                "live_tokens: T=%d d=%d ld_table=%d ldx=%d ld3=%d V=%d", T, d, ld_table, ldx, ld3, V);
     const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
     NR_REQUIRE(a16(X) && a16(Xc) && a16(dqkv_c) && a16(buf), "live_tokens: rows not 16-byte aligned");
-    NR_REQUIRE(buf_bytes >= live_tokens_bytes(n_seq, T, ld3), "live_tokens: buffer too small (%lld bytes)", buf_bytes);
+    NR_REQUIRE(buf_bytes >= live_tokens_bytes(n_seq, T, sec, ld3), "live_tokens: buffer too small (%lld bytes)", buf_bytes);
     const int n = static_cast<int>(n_seq), M = n * T, nb = ceil_div(n, kLiveTitlesPerBlock);
-    WorkspaceLayout l{static_cast<char*>(buf)};
-    out->pad = l.take<unsigned char>(n);
-    out->mask = l.take<uint32_t>(n);
-    int* counts = l.take<int>(n);
-    out->offset = l.take<int>(n + 1);
-    out->index = l.take<int>(M);
-    out->tiles = l.take<int>(M / kTileM + 2);
-    int* block_base = l.take<int>(nb + 1);
-    out->qkv = l.take<__nv_bfloat16>(static_cast<long long>(T) * ld3);
+    const LiveLayout l(buf, n_seq, T, sec, ld3);
+    *out = l.out;
+    int* counts = l.counts;
+    int* block_base = l.block_base;
     if (n == 0) return 0;
     unsigned* ticket = reinterpret_cast<unsigned*>(block_base + nb);
     NR_CHECK_CUDA(cudaMemsetAsync(ticket, 0, sizeof(unsigned), stream));
     const LiveJob j{.ids = ids, .n_seq = n, .T = T, .d = d, .M = M, .V = V, .n_blocks = nb, .row0 = static_cast<const uint32_t*>(table),
                     .bqkv = bqkv, .sec = sec, .ld3 = ld3, .ldx = ldx, .X = static_cast<const uint4*>(X), .Xc = static_cast<uint4*>(Xc),
-                    .dqkv_c = static_cast<uint4*>(dqkv_c), .counts = counts, .block_base = block_base, .ticket = ticket, .out = *out};
+                    .dqkv_c = static_cast<uint4*>(dqkv_c), .counts = counts, .block_base = block_base, .ticket = ticket,
+                    .bad_id_flag = bad_id_flag, .out = *out};
     ProfScope ps("live_tokens", M, n, 0, stream);
     live_classify_kernel<<<nb, kLiveTilesThreads, 0, stream>>>(j);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     live_compact_kernel<<<nb, kLiveTilesThreads, 0, stream>>>(j);
+    ++g_launches;
+    NR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+__global__ void __launch_bounds__(kLiveTilesThreads) live_zero_tail_kernel(const int* m_live_p, int M, uint4* rows, int p16) {
+    const int m_live = *m_live_p, tail_end = min(M, (m_live + kTileM - 1) / kTileM * kTileM);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (tail_end - m_live) * p16; i += gridDim.x * blockDim.x)
+        rows[static_cast<long long>(m_live) * p16 + i] = make_uint4(0, 0, 0, 0);
+}
+
+int live_zero_tail(const LiveTokens& live, long long n_seq, int T, void* rows, int ld, cudaStream_t stream) {
+    NR_REQUIRE(live.offset && rows && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(rows) & 15) == 0, "live_zero_tail: bad operand");
+    if (n_seq == 0) return 0;
+    ProfScope ps("live_zero_tail", static_cast<int>(n_seq * T), ld, 0, stream);
+    live_zero_tail_kernel<<<8, kLiveTilesThreads, 0, stream>>>(live.offset + n_seq, static_cast<int>(n_seq * T), static_cast<uint4*>(rows),
+                                                               ld / 8);
     ++g_launches;
     NR_CHECK_CUDA(cudaGetLastError());
     return 0;

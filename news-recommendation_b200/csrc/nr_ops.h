@@ -124,11 +124,11 @@ int padding_titles(const long long* ids, long long n_seq, int T, int d, const vo
                    int ld3, PaddingTitles* out, cudaStream_t stream);
 void free_padding_titles(PaddingTitles& pt, cudaStream_t stream);
 
-// Live tokens of the news encoder's backward.  Token r is live when its id is in [1, V), or when row 0 of the bf16 table is
-// nonzero (then every token is).  A dead token's gathered row is [0 .. 0, 1] (gather_rows reads an out-of-range id as row 0),
-// so its dQ|dK|dV row adds nothing to the embedding gradient and reaches the weight gradient only through the bias column.
-// The compact order lists the live tokens in ascending token order.  A title without a live token is a padding title: the
-// same verdict as padding_titles, from the same ids and table row.  Nothing is read back to the host.
+// Live tokens of the news encoder.  Token r is live when its id is in [1, V), or when row 0 of the bf16 table is nonzero (then
+// every token is).  A dead token's gathered row is [0 .. 0, 1] (gather_rows reads an out-of-range id as row 0), so its Q|K|V
+// row is bf16(b_qkv), its dQ|dK|dV row adds nothing to the embedding gradient and reaches the weight gradient only through the
+// bias column.  The compact order lists the live tokens in ascending token order.  A title without a live token is a padding
+// title: the same verdict as padding_titles, from the same ids and table row.  Nothing is read back to the host.
 struct LiveTokens {
     unsigned char* pad = nullptr;  // [n_seq] 1 = padding title (mask 0)
     uint32_t* mask = nullptr;      // [n_seq] bit t: token t of the title is live
@@ -136,16 +136,23 @@ struct LiveTokens {
     int* index = nullptr;          // [n_seq * T] compact row -> token; -1 on the rows [M', round_up(M', 64)) below n_seq * T
     int* tiles = nullptr;          // the compact 64-row tiles 0 .. ceil(M' / 64) - 1 in GemmNTParams::tile_list layout
     void* qkv = nullptr;           // bf16 [T][ld3] Q|K|V of a padding title (every row bf16(b_qkv))
+    void* v_lo = nullptr;          // bf16 [T][sec] low plane of its V section, bf16(b - bf16(b))
 };
 // table null: a token is live when its id is in [1, V) or its row of X is nonzero below column d (the same tokens, found by
-// reading X; a dead token's row is [0 .. 0, 1] either way).  Also copies the live rows of X (bf16, pitch ldx) to Xc in
-// compact order and writes zeros to the rows [M', round_up(M', 64)) below n_seq * T of Xc and of dqkv_c (bf16, pitch ld3),
-// the rows a 64-row tile of the compact GEMMs reads past M'.  d even, T <= 32.  The buffers of `out` are carved from `buf`
-// (16-byte aligned, live_tokens_bytes(n_seq, T, ld3) bytes): nothing is allocated, nothing is read back to the host.
-long long live_tokens_bytes(long long n_seq, int T, int ld3);
+// reading X; a dead token's row is [0 .. 0, 1] either way).  Xc non-null: also copies the live rows of X (bf16, pitch ldx) to
+// Xc in compact order and writes zeros to its rows [M', round_up(M', 64)) below n_seq * T; dqkv_c non-null: zeros on the same
+// rows of dqkv_c (bf16, pitch ld3), the rows a 64-row tile of the compact GEMMs reads past M'.  bad_id_flag non-null: set to 1
+// when an id is outside [0, V) (the compact gather does not read the dead tokens' ids).  d even, T <= 32.  The buffers of
+// `out` are carved from `buf` (16-byte aligned, live_tokens_bytes(n_seq, T, sec, ld3) bytes): nothing is allocated, nothing is
+// read back to the host.
+long long live_tokens_bytes(long long n_seq, int T, int sec, int ld3);
 int live_tokens(const long long* ids, long long n_seq, int T, int d, const void* table, int ld_table, int V, const float* bqkv,
                 int sec, int ld3, const void* X, int ldx, void* Xc, void* dqkv_c, void* buf, long long buf_bytes, LiveTokens* out,
-                cudaStream_t stream);
+                cudaStream_t stream, int* bad_id_flag = nullptr);
+// the buffers of a LiveTokens that live_tokens filled in `buf` earlier (no launch)
+LiveTokens live_tokens_view(void* buf, long long n_seq, int T, int sec, int ld3);
+// zeros on the rows [M', round_up(M', 64)) below n_seq * T of rows (bf16, pitch ld), M' = live.offset[n_seq]
+int live_zero_tail(const LiveTokens& live, long long n_seq, int T, void* rows, int ld, cudaStream_t stream);
 
 // ---- memory-bound companions (aux.cu) --------------------------------------------------------------
 // fp32 rows -> zero-padded bf16 planes: every operand cast, dense-input conversion and hi/lo split in front of a GEMM.
@@ -183,13 +190,16 @@ inline int rows_to_bf16(const Bf16Rows& job, Bf16Op op, cudaStream_t stream) { r
 int sum_over_seq(const float* src, long long n_seq, long long L, float* dst, cudaStream_t stream);
 // X[row(seg,t)] = table_bf16[ids[seg*T+t]] (bit-exact copy), ones column at D, optional dropout, optional padded layout.
 // X may be wider than the table (ld_x >= ld_table): only its first ld_table columns are written.
+// live non-null (padded 0): compact rows -- X row i < M' = live->offset[n_tok / T] is token live->index[i], with that token's
+// dropout draw (the same bits as row index[i] of the full gather); rows [M', round_up(M', 64)) below n_tok are zero rows
 int gather_rows(const long long* ids, long long n_tok, int T, const void* table, int V, int D, int ld_table, void* X,
-                int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream);
+                int ld_x, int padded, DropoutCfg drop, int* bad_id_flag, cudaStream_t stream, const LiveTokens* live = nullptr);
 // the news encoder's backward over live tokens (LiveTokens above): what the title-level attention backward needs of it
 struct TitleBwdLive {
     const LiveTokens* tokens;
     float* dbias;  // the bias column of the Q|K|V weight gradient
     int ld_dbias;
+    int compact_qkv = 0;  // 1: Q|K|V holds the live tokens' rows only, in compact order (the compact forward's)
 };
 // multi-head self attention core on packed Q|K|V bf16 [n_seq*T x ld_qkv]: sections start at columns 0, sec, 2*sec
 // (sec >= d = heads*dk; dQKV uses the same sections)
@@ -201,9 +211,11 @@ int mhsa_core_bwd(const void* qkv, int ld_qkv, int sec, const void* dctx, int ld
 bool mhsa_title_fwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int ld_ctx);
 // pad (PaddingTitles, may be null): the padding titles take their Q|K|V rows (and V low plane) from pad->qkv / pad->v_lo, not
 // from qkv / v_lo, whose rows they may have left unwritten
+// live (LiveTokens, may be null; pad must then be null): qkv / v_lo hold the live tokens' rows only, in compact order; a dead
+// token reads its rows from live->qkv / live->v_lo, and a padding title loads nothing else.  The context stays in token order.
 int mhsa_title_fwd(const void* qkv, int ld_qkv, int sec, long long n_seq, int heads, void* ctx, int ld_ctx, DropoutCfg drop,
                    cudaStream_t stream, const void* v_lo = nullptr, int ld_vlo = 0, void* ctx_lo = nullptr,
-                   const PaddingTitles* pad = nullptr);
+                   const PaddingTitles* pad = nullptr, const LiveTokens* live = nullptr);
 bool mhsa_title_bwd_supported(int T, int dk, int heads, int sec, int ld_qkv, int ld_dctx, int ld_dqkv);
 // live (may be null): the padding titles take their Q|K|V rows from live->tokens->qkv; only the live tokens' dQ|dK|dV rows are
 // stored, in compact order (row live->tokens->offset[s] + rank of the token among its title's live tokens); the bf16-rounded

@@ -28,6 +28,7 @@ class MhsaEncoderFwdArgs(C.Structure):
         ("wqkv_kcat_bf16", _vp), ("X_kcat_bf16", _vp), ("QKV_f32", _vp),
         ("V_lo_bf16", _vp),
         ("dense_pos", _vp),
+        ("live", _vp), ("live_bytes", _ll),
     ]
 
 
@@ -43,6 +44,7 @@ class MhsaEncoderBwdArgs(C.Structure):
         ("workspace", _vp), ("workspace_bytes", _ll),
         ("wqkv_bf16", _vp), ("bqkv", _vp), ("emb_grad_ready_event", _vp),
         ("dpos", _vp), ("table_bf16", _vp),
+        ("live", _vp), ("live_bytes", _ll),
     ]
 
 
@@ -204,6 +206,7 @@ SIGNATURES = {
     "nr_dot_score_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "nr_mhsa_accurate_supported": (_i, [_i, _i, _i]),
     "nr_mhsa_encoder_fwd": (_i, [C.POINTER(MhsaEncoderFwdArgs), _vp]),
+    "nr_mhsa_encoder_live_bytes": (_ll, [_ll, _i, _i]),
     "nr_mhsa_encoder_bwd_workspace": (_ll, [_ll, _i, _i, _i]),
     "nr_mhsa_encoder_bwd": (_i, [C.POINTER(MhsaEncoderBwdArgs), _vp]),
     "nr_cnn_encoder_fwd": (_i, [C.POINTER(CnnEncoderFwdArgs), _vp]),

@@ -258,10 +258,19 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
             a.wqkv_kcat_bf16, a.X_kcat_bf16, a.QKV_f32, a.C_lo_bf16 = _p(kcat), _p(keep[0]), _p(keep[1]), _p(C_lo)
         a.X_bf16, a.QKV_bf16, a.C_bf16, a.w, a.out = _p(X), _p(QKV), _p(Cx), _p(w), _p(out)
         a.bad_id_flag = _p(bad_flag)
+        # the news encoder at the title-level kernels' shape runs over live tokens only: X, Q|K|V (and V_lo) then hold the live
+        # tokens' rows in compact order (their count is known on the device only, so the buffers keep their full size), and the
+        # backward reuses the compaction in `live`
+        live = None
+        if ids is not None and bool(lib.nr_mhsa_accurate_supported(T, d, heads)):
+            live_bytes = int(lib.nr_mhsa_encoder_live_bytes(n_seq, T, d))
+            live = torch.empty((live_bytes,), dtype=torch.uint8, device=dev)
+            a.live, a.live_bytes = _p(live), live_bytes
         check(lib.nr_mhsa_encoder_fwd(C.byref(a), _stream()), "nr_mhsa_encoder_fwd")
         if need_bwd:
             ctx.save_for_backward(X, QKV if QKV is not None else torch.empty(0, device=dev), Cx, w,
-                                  ids if ids is not None else torch.empty(0, device=dev))
+                                  ids if ids is not None else torch.empty(0, device=dev),
+                                  live if live is not None else torch.empty(0, dtype=torch.uint8, device=dev))
         ctx.meta = dict(n_seq=n_seq, T=T, d=d, q=q, heads=heads, p_drop=float(p_drop), seed=seed, ops=ops,
                         has_ids=ids is not None, V=emb_w.shape[0] if ids is not None else 0,
                         dense_shape=None if dense is None else tuple(dense.shape),
@@ -272,7 +281,7 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         lib = load_library()
-        X, QKV, Cx, w, ids = ctx.saved_tensors
+        X, QKV, Cx, w, ids, live = ctx.saved_tensors
         m = ctx.meta
         dev = X.device
         d, q, T, n_seq = m["d"], m["q"], m["T"], m["n_seq"]
@@ -329,6 +338,8 @@ class MhsaPoolEncoderFn(torch.autograd.Function):
         a.dWqkv_ext, a.dWa_ext, a.dqv = _p(dWqkv), _p(dWa), _p(dqv)
         a.demb, a.ddense, a.dpos = _p(demb), _p(ddense), _p(dpos)
         a.workspace, a.workspace_bytes = _p(ws), ws_bytes
+        if live.numel():
+            a.live, a.live_bytes = _p(live), live.numel()
         check(lib.nr_mhsa_encoder_bwd(C.byref(a), _stream()), "nr_mhsa_encoder_bwd")
         g_dense = ddense.view(m["dense_shape"]) if ddense is not None else None
         g_emb = None if emb_direct else demb
